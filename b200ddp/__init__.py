@@ -1,9 +1,9 @@
-"""b200ddp - a Blackwell-native (sm_100a) distributed-data-parallel training template.
+"""b200ddp - a Hopper-native (sm_90a) distributed-data-parallel training template.
 
 Same capabilities and launch shape as howardlau1999/pytorch-ddp-template (``ddp.py`` + ``model.py`` +
-``dataset.py``, torchrun-spawned) with the delegated native layers rebuilt for 8xB200: a DDP wrapper
+``dataset.py``, torchrun-spawned) with the delegated native layers rebuilt for 8xH100: a DDP wrapper
 whose C++ reducer launches fused allreduce kernels over NVSwitch peer memory, a peer-memory init
-broadcast, tcgen05/TMEM/TMA GEMMs, fused LayerNorm / loss / clip+SGD kernels, CUDA-graph steps.
+broadcast, wgmma/TMA GEMMs, fused LayerNorm / loss / clip+SGD kernels, CUDA-graph steps.
 """
 __version__ = "0.1.0"
 

@@ -1,5 +1,5 @@
 """Loader for the native extension.  ``get()`` imports the in-tree ``_C`` module, building it first if
-it is missing (CPU-only boxes can build: nvcc cross-compiles sm_100a without a GPU).  On a GPU box a
+it is missing (machines without a GPU can build: nvcc cross-compiles sm_90a).  On a GPU machine a
 missing extension is a hard error for every CUDA op - there is no silent PyTorch fallback."""
 from __future__ import annotations
 

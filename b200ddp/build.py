@@ -1,9 +1,10 @@
-"""In-tree build of the sm_100a extension ``b200ddp/_C*.so``.
+"""In-tree build of the sm_90a (H100) extension ``b200ddp/_C*.so``.
 
-Explicit nvcc / g++ invocations (no JIT cache under ~/.cache: the built ``.so`` must sit in the
-repo so it travels to the GPU box with the snapshot).  ``-gencode arch=compute_100a,code=sm_100a``
-is passed directly, which bypasses torch's own arch list; ``-lineinfo`` keeps ncu's source page
-usable.  Objects are rebuilt only when the content hash of (source + headers + flags) changes.
+Explicit nvcc / g++ invocations (no JIT cache under ~/.cache: the built ``.so`` sits in the package
+directory, where ``_ext`` imports it from).  ``-gencode arch=compute_90a,code=sm_90a`` is passed
+directly, which bypasses torch's own arch list (the wgmma / TMA kernels need the ``a`` target);
+``-lineinfo`` keeps profiler source views usable.  Objects are rebuilt only when the content hash of
+(source + headers + flags) changes.
 """
 from __future__ import annotations
 
@@ -22,10 +23,10 @@ BUILD = PKG / "_build"
 EXT_NAME = "_C"
 
 CUDA_SOURCES = ["allreduce.cu", "broadcast.cu", "optim.cu", "loss.cu", "layernorm.cu", "linear_small.cu", "input.cu",
-                "gemm_tcgen05.cu", "batchnorm.cu", "pool.cu", "conv_tcgen05.cu", "conv_wgrad_tcgen05.cu", "conv_stem.cu"]
+                "gemm_wgmma.cu", "batchnorm.cu", "pool.cu", "conv_wgmma.cu", "conv_wgrad_wgmma.cu", "conv_stem.cu"]
 CPP_SOURCES = ["peer_mem.cpp", "reducer.cpp", "bindings.cpp"]
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def ext_path() -> Path:

@@ -1,4 +1,4 @@
-// Fused gradient-bucket allreduce over NVSwitch peer memory (SURVEY K4/N5/N6 replacement).
+// Fused gradient-bucket allreduce over NVSwitch peer memory (replaces NCCL's allreduce on the DDP hot path).
 //
 // ONE launch per bucket does, tile by tile:
 //   gather (flatten scattered .grad tensors) -> x scale (1/world) -> cast to wire dtype -> local

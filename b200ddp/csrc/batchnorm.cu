@@ -2,8 +2,8 @@
 //
 // Why: in the ResNet-50 bf16 step the stock path (ATen batch_norm_collect_statistics / transform_input /
 // backward_reduce / backward_elemt + separate ReLU, residual-add and threshold_backward kernels + per-layer
-// num_batches_tracked / running-stat updates) is 58% of all kernel time (profiles/launches_graph.md) and runs
-// ~16x below the HBM roofline at batch 32.  A [N,C,H,W] channels_last tensor is a row-major [R = N*H*W, C]
+// num_batches_tracked / running-stat updates) is the largest share of the ResNet-50 step outside the convolutions and
+// runs far below the HBM roofline at batch 32.  A [N,C,H,W] channels_last tensor is a row-major [R = N*H*W, C]
 // matrix, so every per-channel quantity is a column reduction:
 //
 //   forward : bn_stats      column sum / sum-of-squares -> mean, rstd, scale = gamma*rstd, shift = beta - mean*scale,
@@ -565,8 +565,8 @@ dim3 apply_grid(const Tile& t, int R) {
 // Fused (single-launch) variants need every block of a channel tile resident at once: cap the grid at 2 blocks per SM.
 bool fused_tile(int R, int C, Tile* t) {
   static int enabled = -1;
-  // measured (profiles/README.md): one launch per direction is NOT faster than two at batch 32 (the co-residency cap
-  // on the grid costs what the saved launch gains), so the two-launch form stays the default; opt in with =1
+  // one launch per direction caps the grid at what can be co-resident, which costs what the saved launch gains, so the
+  // two-launch form stays the default; opt in with =1
   if (enabled < 0) { const char* e = getenv("B200DDP_BN_FUSED"); enabled = (e && atoi(e) == 1) ? 1 : 0; }
   *t = pick_tile(R, C);
   if (!enabled || t->grid_x > 2 * kNumSMs) return false;
@@ -579,8 +579,8 @@ bool fused_tile(int R, int C, Tile* t) {
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------
-// Statistics from the producing convolution's epilogue (csrc/conv_tcgen05.cu): partial = [2][G][C] per-CTA column sums and
-// sums of squares, G <= 148.  NO separate finishing launch: every block of the normalisation kernel first reduces the G
+// Statistics from the producing convolution's epilogue (csrc/conv_wgmma.cu): partial = [2][G][C] per-CTA column sums and
+// sums of squares, G <= 132.  NO separate finishing launch: every block of the normalisation kernel first reduces the G
 // rows of ITS <= 64 channels (a few tens of KB out of L2, fixed order -> deterministic), then normalises its rows; the
 // blocks of the first row split also publish mean / rstd (for the backward pass) and update the running statistics.
 template <typename T>

@@ -1,5 +1,5 @@
 // Python bindings.  The only translation unit that sees torch headers.  Which reference call site each op stands in for is
-// documented on the Python side (b200ddp/ops/functional.py, parallel/peer.py, optim/sgd.py) and in docs/INVENTORY.md.
+// documented on the Python side (b200ddp/ops/functional.py, parallel/peer.py, optim/sgd.py).
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -180,7 +180,7 @@ struct SgdPlan {
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "b200ddp native extension (sm_100a)";
+  m.doc() = "b200ddp native extension (sm_90a)";
   m.attr("MAX_BUCKET_TENSORS") = kMaxBucketTensors;
   m.attr("MAX_COMM_BLOCKS") = kMaxCommBlocks;
   m.attr("SIGNAL_BYTES") = (long long)kSignalBytes;
@@ -413,7 +413,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(dx, dw, db);
   });
 
-  // tcgen05 GEMM: D[M,N] = act(A[M,K] @ B[N,K]^T + bias) ; all bf16 row-major, fp32 accumulate in TMEM
+  // wgmma GEMM: D[M,N] = act(A[M,K] @ B[N,K]^T + bias) ; all bf16 row-major, fp32 accumulate in registers
   m.def("gemm_nt", [](at::Tensor a, at::Tensor b, c10::optional<at::Tensor> bias, int epilogue, c10::optional<at::Tensor> out) {
     check_cuda(a, "a"); check_cuda(b, "b");
     TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm_nt: bf16 operands");
@@ -480,7 +480,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return out;
   });
 
-  // ---- convolutions on tcgen05 (conv_tcgen05.cu / conv_wgrad_tcgen05.cu): channels_last bf16, stride 1, 1x1 or 3x3 ------
+  // ---- convolutions on wgmma (conv_wgmma.cu / conv_wgrad_wgmma.cu): channels_last bf16, stride 1, 1x1 or 3x3 ------
   m.def("conv_fprop", [](at::Tensor x, at::Tensor w, int stride, int pad, int mode, int block_n, int base_offset, bool stats,
                          c10::optional<at::Tensor> debug, int kc) {
     check_cuda(x, "x"); check_cuda(w, "w");
@@ -572,7 +572,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return dw;
   }, py::arg("dy"), py::arg("x"), py::arg("ksize"), py::arg("stride") = 1, py::arg("pad") = 0, py::arg("split") = 0,
      py::arg("tile_m") = 0, py::arg("tile_n") = 0);
-  // strided 7x7 stem (3 -> 64 channels, stride 2, padding 3) on the tcgen05 tap-GEMM through an overlapping-window tensor map
+  // strided 7x7 stem (3 -> 64 channels, stride 2, padding 3) on the wgmma tap-GEMM through an overlapping-window tensor map
   m.def("stem_conv_supported", [](int H, int W) { StemGeom g; return stem_geom(H, W, &g); });
   m.def("stem_pack_input", [](at::Tensor x) {
     check_cuda(x, "x");

@@ -1,5 +1,5 @@
-// Rank-`src` -> everyone broadcast of a list of tensors through peer memory (SURVEY K3/K7/N4:
-// replaces `_sync_module_states` -> ncclBroadcast + flatten/unflatten copies).
+// Rank-`src` -> everyone broadcast of a list of tensors through peer memory
+// (replaces `_sync_module_states` -> ncclBroadcast + flatten/unflatten copies).
 //
 // One launch moves one chunk (<= staging size, <= kMaxBucketTensors tensors):
 //   src rank : gather its tensors (bytes) into staging - its own arena, or, with NVLS, a

@@ -1,5 +1,5 @@
 // Host-callable entry points of the peer-memory collectives: what replaces the NCCL calls torch DDP issues for the
-// reference (init broadcast at wrap time, ddp.py:192-196; per-bucket allreduce during backward, ddp.py:230-232; SURVEY K3, K4, K7).
+// reference (init broadcast at wrap time, ddp.py:192-196; per-bucket allreduce during backward, ddp.py:230-232).
 #pragma once
 #include <cuda_runtime.h>
 #include "common.h"

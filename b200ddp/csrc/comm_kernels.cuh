@@ -1,6 +1,6 @@
 // Device-side building blocks for the peer-memory collectives: system-scope signal primitives,
 // the block-wise cross-GPU barrier, multimem (NVLS) accessors and the bucket tensor table.
-// (SURVEY N7 / section 5.8: the transport the reference gets from ProcessGroupNCCL, `init_process_group("nccl")` at ddp.py:103.)
+// (the transport the reference gets from ProcessGroupNCCL, `init_process_group("nccl")` at ddp.py:103.)
 #pragma once
 #include "common.h"
 #include "peer_mem.h"
@@ -11,7 +11,7 @@ constexpr int kMaxBucketTensors = 192;      // keeps the whole launch argument b
 // Comm CTAs are deliberately light (256 threads, <= 85 registers/thread -> a third of an SM's register
 // file): they must slot in beside the CTAs of the backward kernels they overlap with instead of
 // evicting them (a 512-thread / 118-register CTA monopolises an SM and turns persistent cuDNN kernels
-// into two waves - measured as "comm time fully exposed", profiles/ddp_overhead_diag_n2_v1.txt).
+// into two waves, which exposes the whole communication time).
 constexpr int kCommThreads = 256;
 constexpr int kCommMinCtasPerSm = 3;
 

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a extension.  Nothing here includes torch headers: kernels take raw
+// Shared helpers for the sm_90a extension.  Nothing here includes torch headers: kernels take raw
 // pointers + cudaStream_t so each .cu compiles in seconds; only bindings.cpp sees torch/extension.h.
 #pragma once
 #include <cuda_runtime.h>
@@ -40,7 +40,7 @@ inline void ensure_max_dynamic_smem(Kernel kernel, int bytes, std::atomic<unsign
   done.fetch_or(bit, std::memory_order_release);
 }
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74
+constexpr int kNumSMs = 132;  // H100 SXM
 constexpr int kWarp = 32;
 
 enum class DType : int { F32 = 0, BF16 = 1, U8 = 2, I64 = 3 };

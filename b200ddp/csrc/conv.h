@@ -1,5 +1,5 @@
-// tcgen05 convolution entry points (conv_tcgen05.cu, conv_wgrad_tcgen05.cu) for channels_last bf16 activations.
-// They replace the cuDNN calls behind the model's forward / backward (reference hot path: /root/reference/ddp.py:221,231).
+// wgmma convolution entry points (conv_wgmma.cu, conv_wgrad_wgmma.cu) for channels_last bf16 activations.
+// They replace the cuDNN calls behind the model's forward / backward (reference hot path: the reference ddp.py:221,231).
 #pragma once
 #include <cuda_runtime.h>
 #include "common.h"
@@ -26,10 +26,11 @@ bool conv_tile_plan(int N, int H, int W, int R, int S, int want_mode, ConvTilePl
 
 struct ConvLaunchCfg {
   int mode = -1;             // -1 auto
-  int block_n = 0;           // 0 auto; 64 / 128 / 256
+  int block_n = 0;           // 0 auto; 64 / 128; 256 runs as two 128-wide n-tiles (a wider accumulator does not fit in registers)
   int kc = 0;                // 0 auto; 64-deep k chunks per pipeline stage (flat / patch tilings)
   void* debug_counters = nullptr;   // device int64[16]: cycle breakdown of CTA 0's producer / issuer / epilogue (diagnostics)
-  int set_base_offset = 0;   // halo mode experiment knob: 1 = fill the descriptor base-offset field (measured WRONG on B200: the swizzle phase follows the absolute address)
+  int set_base_offset = 0;   // halo mode experiment knob: 1 = fill the A descriptors' base-offset field with the 128-byte row phase of
+                             // their start address (default 0: the swizzle phase is taken from the absolute address)
 };
 
 // Forward (dgrad = false):  y[N,H,W,Cout] = conv(x[N,H,W,Cin], w[Cout,R,S,Cin]),  stride 1, padding (R-1)/2.

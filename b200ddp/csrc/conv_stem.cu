@@ -1,6 +1,6 @@
 // Operand packing for the strided 7x7 stem convolution (conv.h: launch_stem_conv_fprop / launch_stem_conv_wgrad).
-// Reference hot path replaced: the first convolution of the model's forward / backward (/root/reference/ddp.py:221,231), which
-// the library runs as a padded-to-8-channels mma.sync kernel (211 us forward, 145 us weight gradient at batch 32, bench/stem_bench.py).
+// Reference hot path replaced: the first convolution of the model's forward / backward (the reference ddp.py:221,231), which
+// the library runs as a padded-to-8-channels kernel (bench/stem_bench.py times both).
 #include "conv.h"
 
 #include <cuda_bf16.h>
@@ -71,7 +71,7 @@ void launch_stem_pack_input(const void* x_nhwc3, void* xp, int N, int H, int W, 
   StemGeom g;
   if (!stem_geom(H, W, &g)) throw std::runtime_error("stem conv: unsupported image size");
   const long long total = (long long)N * g.Hp2 * g.Wp;
-  const int blocks = (int)std::min<long long>((total + 255) / 256, 148LL * 32);
+  const int blocks = (int)std::min<long long>((total + 255) / 256, (long long)kNumSMs * 32);
   stem_pack_input_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(x_nhwc3), reinterpret_cast<uint4*>(xp), N, H, W, g.Hp2, g.Wp);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA bf16 GEMM entry points (gemm_tcgen05.cu).
+// wgmma / TMA bf16 GEMM entry points (gemm_wgmma.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include "common.h"
@@ -21,13 +21,10 @@ void launch_gemm_bf16(const void* a, const void* b, void* d, const void* bias, i
 void launch_gemm_nt_bf16(const void* a, const void* b, void* d, const void* bias, int M, int N, int K, int epilogue,
                          DType out_dtype, cudaStream_t stream);
 bool gemm_shape_supported(int M, int N, int K, bool a_mn, bool b_mn);
-// 0 = auto (CTA pairs for large problems), 1 = always 1-CTA kernel, 2 = always the cta_group::2 kernel
-void set_gemm_cta_mode(int mode);
 
 // Persistent-tile rasterisation shared by the producer, issuer and epilogue roles (and mirrored on the host for
 // tests).  group_m <= 0: m-fastest over the whole problem (default).  group_m > 0: bands of `group_m` m-tiles
-// are swept n-major, so the ~148 tiles in flight form a near-square patch and both operands are reused out of L2
-// (ncu on 8192^3: 64.8 % L2 hit / 2.2 GB DRAM reads with the m-fastest order, 8x the compulsory traffic).
+// are swept n-major, so the ~132 tiles in flight form a near-square patch and both operands are reused out of L2.
 B200_HD inline void gemm_tile_coords(int tile, int num_m, int num_n, int group_m, int* m_blk, int* n_blk) {
   if (group_m <= 0) { *m_blk = tile % num_m; *n_blk = tile / num_m; return; }
   const int per_group = group_m * num_n;
@@ -38,6 +35,8 @@ B200_HD inline void gemm_tile_coords(int tile, int num_m, int num_n, int group_m
   *m_blk = first_m + r % rows;
   *n_blk = r / rows;
 }
+// 0 = auto, 1 = always single-CTA tiles, 2 = always cluster pairs (two CTAs share the B tile through TMA multicast)
+void set_gemm_cta_mode(int mode);
 // -1 = read B200DDP_GEMM_GROUP_M (default 0 = m-fastest)
 void set_gemm_group_m(int group_m);
 // -1 = read B200DDP_GEMM_TMA_STORE (default 0); 1 = bf16 outputs leave through shared memory + TMA stores

@@ -1,5 +1,5 @@
 // Input pipeline kernel (reference: the blocking `x, y = x.to(args.device), y.to(args.device)` at ddp.py:220 moves fp32
-// tensors as they are; SURVEY G10).  Here the host ships raw NCHW batches (uint8 pixels or fp32) from pinned memory;
+// tensors as they are).  Here the host ships raw NCHW batches (uint8 pixels or fp32) from pinned memory;
 // this kernel does scale/mean/std normalisation, the cast to the compute dtype and the NCHW ->
 // channels_last permutation in one pass (the stock path would be .float(), sub_, div_, .to(bf16),
 // .contiguous(channels_last) = 5 launches and 5 round trips through HBM).

@@ -1,4 +1,4 @@
-// LayerNorm forward / backward (named hot op in BASELINE.json's north-star; needed by the BERT
+// LayerNorm forward / backward (needed by the BERT
 // config).  One warp per row, 16-byte vector loads, fp32 statistics; backward produces dx in the same
 // pass as per-CTA partial dgamma/dbeta, finished by a small column-reduce kernel (no atomics, so the
 // result is deterministic).

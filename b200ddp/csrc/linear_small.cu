@@ -1,8 +1,8 @@
-// Linear layers whose dims are far below one tcgen05 tile (reference model.py:11-13: 10->10->5 at
+// Linear layers whose dims are far below one wgmma tile (reference model.py:11-13: 10->10->5 at
 // batch 32; the smallest MMA atom is 64x8x16 and TMA needs 16-byte row pitches, which a 10-wide
 // bf16 row does not have).  These are latency problems, not FLOP problems: one CTA, operands in
 // shared memory, fused bias + ReLU forward, and ONE backward launch producing dx, dw and db (with
-// the ReLU mask recomputed from the saved output).  Larger, aligned shapes go to gemm_tcgen05.cu.
+// the ReLU mask recomputed from the saved output).  Larger, aligned shapes go to gemm_wgmma.cu.
 #include "ops.h"
 
 namespace b200 {

@@ -1,4 +1,4 @@
-// Fused loss forward+backward kernels (SURVEY G4): the stock path runs sub / pow / mean-reduce and a
+// Fused loss forward+backward kernels: the stock path runs sub / pow / mean-reduce and a
 // separate mse_loss_backward; cross-entropy is log_softmax + nll_loss + their two backwards.
 // Each loss here is one launch that emits the scalar loss AND the gradient w.r.t. its input, so the
 // autograd Function's backward is just "return the saved tensor (x upstream scale)".

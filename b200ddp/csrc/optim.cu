@@ -1,4 +1,4 @@
-// Multi-tensor fused optimizer path (SURVEY G7/G8/G9, N11/N12): the stock stack runs
+// Multi-tensor fused optimizer path: the stock stack runs
 // `_foreach_norm` -> stack -> `vector_norm` -> clamp -> `_foreach_mul_` -> `_foreach_add_` (>= 6
 // launches + a fresh grad allocation per step).  Here: [sum of squares partials come from the
 // allreduce epilogue, or from multi_sqnorm on one GPU] -> clip_coef (1 tiny block) -> multi_sgd,

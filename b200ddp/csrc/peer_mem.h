@@ -1,4 +1,4 @@
-// NVSwitch peer-memory substrate (SURVEY N7 replacement for ProcessGroupNCCL on the hot path).
+// NVSwitch peer-memory substrate (replacement for ProcessGroupNCCL on the hot path).
 //
 // Every rank owns one VMM allocation (cuMemCreate, POSIX-FD shareable) - the "arena".  Arenas of all
 // ranks are mapped into ONE contiguous VA window per process, rank r at `base + r*stride`, so a
@@ -21,8 +21,8 @@ namespace b200 {
 
 constexpr size_t kSignalBytes = 4 << 20;   // 4 MiB of signal pads at the start of every arena
 constexpr size_t kPadSetBytes = 32 << 10;  // one PadSet (comm_kernels.cuh) per staging region -> 128 sets
-constexpr int kMaxRanks = 8;               // one NVSwitch domain (HGX B200)
-constexpr int kMaxCommBlocks = 296;             // 2 light CTAs per SM on 148 SMs
+constexpr int kMaxRanks = 8;               // one NVSwitch domain (HGX H100)
+constexpr int kMaxCommBlocks = 264;             // 2 light CTAs per SM on 132 SMs
 
 class PeerArena {
  public:

@@ -1,5 +1,5 @@
 // 3x3 / stride-2 / pad-1 max pooling for channels_last activations (the ResNet stem), forward + backward.
-// ATen's max_pool_backward_nhwc is 228 us at batch 32 (profiles/launches_graph.md) for ~64 MB of traffic; both
+// ATen's max_pool_backward_nhwc is far from the copy rate for its ~64 MB of traffic at batch 32; both
 // directions here are single-pass, 16-byte-vector kernels.  Forward stores the arg-max window slot (0..8) per
 // element in one byte, so backward is a pure gather: every input pixel looks at the <= 4 output windows that
 // cover it and sums the gradients whose recorded slot points back at it - no atomics, deterministic.

@@ -1,6 +1,6 @@
 // Host side of the gradient reducer (see reducer.h).  Reference behaviour being replaced: the c10d Reducer that
 // `DistributedDataParallel(model, ..., find_unused_parameters=True)` (reference ddp.py:192-196) builds at wrap time and
-// drives from autograd hooks on every `loss.backward()` (reference ddp.py:230-232); SURVEY N1, N2, K4, K5.
+// drives from autograd hooks on every `loss.backward()` (reference ddp.py:230-232).
 #include "reducer.h"
 
 #include <algorithm>

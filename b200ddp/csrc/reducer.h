@@ -1,4 +1,4 @@
-// Native gradient reducer (SURVEY N1/N2 replacement for c10d::Reducer).
+// Native gradient reducer (replacement for c10d::Reducer).
 //
 // Host-side state machine only - all data movement happens inside the fused kernel it launches:
 //   mark_ready(param, grad_ptr, compute_stream)  called from the parameter's post-accumulate hook;
@@ -51,11 +51,10 @@ struct ReducerOptions {
   // Where the bucket kernels run.  -1 (default): launches recorded into a CUDA graph fork onto the comm stream (they overlap the
   // rest of backward when the graph replays); launches issued eagerly follow set_eager_inline(): on the comm stream for an
   // eager training loop, IN LINE on the compute stream for the few eager warm-up steps of a graph-captured loop.  Reason,
-  // measured (profiles/ddp_timeline.md): once a THIRD stream of the process has executed work, every later graph replay pays
-  // ~0.4 us at each of its ~430 kernel boundaries (+0.17 ms per ResNet-50 step, more than the link time of the whole
-  // gradient exchange); default stream + capture stream are two.  0 / 1 force comm stream / in line everywhere.
+  // once a THIRD stream of the process has executed work, every later graph replay pays extra at each of its ~430 kernel
+  // boundaries; default stream + capture stream are two.  0 / 1 force comm stream / in line everywhere.
   int serial = -1;
-  int wide_blocks = 296;
+  int wide_blocks = 264;
 };
 
 class Reducer {

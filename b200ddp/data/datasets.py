@@ -1,6 +1,6 @@
 """Synthetic datasets.  ``FooDataset`` mirrors the reference (``dataset.py:6-17``: X ~ N(0,1)^(n,10),
 Y ~ N(0,1)^(n,5), held in host memory, drawn from the global torch RNG *after* seeding so every rank
-holds the same data).  The ImageNet- and token-shaped variants feed the BASELINE.json perf configs
+holds the same data).  The ImageNet- and token-shaped variants feed the benchmark configurations
 (there is no network for real data)."""
 from __future__ import annotations
 

@@ -1,7 +1,7 @@
 """Batch loading and host->device staging.
 
 Reference: ``DataLoader(dataset, batch_size, sampler, pin_memory=True)`` with no workers, followed by a
-*blocking* ``x.to(device)`` per step (``ddp.py:148-152,220``; SURVEY Q9/N16).
+*blocking* ``x.to(device)`` per step (``ddp.py:148-152,220``).
 
 Here:
 * ``BatchLoader`` walks a sampler and gathers a whole batch with one ``index_select`` per field straight

@@ -1,12 +1,12 @@
 """Command line + process lifecycle (reference ``ddp.py:80-121`` ``setup``/``cleanup`` and ``ddp.py:291-314`` ``main``).
 
-All 16 reference flags keep their names and defaults (SURVEY §5.6); ``--local-rank`` is accepted as an
-alias because ``torch.distributed.launch`` on torch >= 2 passes that spelling (SURVEY Q7).  New flags
+All 16 reference flags keep their names and defaults; ``--local-rank`` is accepted as an
+alias because ``torch.distributed.launch`` on torch >= 2 passes that spelling.  New flags
 select the model, the DDP transport and its knobs, resume, and the CUDA-graph step.
 
 Mode selection mirrors the reference: CPU (``--no_cuda`` / no GPU), single GPU, single-process multi-GPU
 ``DataParallel`` (no launcher, several GPUs), DDP (launcher present).  Unlike the reference, a launcher
-with ``--no_cuda`` (or no GPU) gives a working gloo DDP run instead of a crash (SURVEY Q6).
+with ``--no_cuda`` (or no GPU) gives a working gloo DDP run instead of a crash.
 """
 from __future__ import annotations
 
@@ -24,7 +24,7 @@ log = None
 
 
 def build_parser() -> argparse.ArgumentParser:
-    p = argparse.ArgumentParser(description="B200-native DDP training template")
+    p = argparse.ArgumentParser(description="H100-native DDP training template")
     # ---- reference flags (ddp.py:293-308), same names and defaults -----------------------------
     p.add_argument("--global-step", type=int, default=0, help="(reference flag; resume uses --resume_from)")
     p.add_argument("--no_cuda", action="store_true")

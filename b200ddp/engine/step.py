@@ -2,7 +2,7 @@
 
 Reference hot loop (``ddp.py:216-243``): forward, loss, backward, two ``loss.item()`` host syncs,
 ``clip_grad_norm_`` (>=4 launches), ``optimizer.step()``, ``scheduler.step()``, ``model.zero_grad()``.
-For the reference's own 165-parameter workload that loop is pure launch/sync latency (SURVEY §3.3).
+For the reference's own 165-parameter workload that loop is pure launch/sync latency.
 
 Here the whole step - forward, fused loss fwd+bwd, backward with the DDP reducer's comm kernels forked
 onto the comm stream, clip coefficient, fused SGD - is enqueued with no host synchronisation, and with
@@ -168,7 +168,7 @@ class TrainStep:
             self._apply_optimizer()
             self.optimizer.zero_grad(set_to_none=True)
             if not self._rebuilt:
-                # what stock DDP does once after the first iteration when find_unused_parameters=False (SURVEY K6): re-plan
+                # what stock DDP does once after the first iteration when find_unused_parameters=False: re-plan
                 # the buckets by the gradient-ready order just observed - before any graph is captured
                 self._rebuilt = True
                 if getattr(self.model, "world_size", 1) > 1 and hasattr(self.model, "rebuild_buckets") \

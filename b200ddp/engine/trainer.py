@@ -1,7 +1,7 @@
 """Training runtime: the reference's ``train(args, model)`` (``ddp.py:126-288``) rebuilt around
 ``TrainStep`` / ``BatchLoader`` / ``DevicePrefetcher`` / the native DDP wrapper.
 
-Kept from the reference (SURVEY §7.5): flag names/defaults, sampler choice and ``set_epoch``, total-step
+Kept from the reference: flag names/defaults, sampler choice and ``set_epoch``, total-step
 arithmetic (``ddp.py:155-161``), ``global_step`` starting at 1 and exiting when it exceeds ``max_steps``
 (``ddp.py:206,280``), TensorBoard scalars ``lr`` / ``loss`` on the main process, checkpoint layout, tqdm only
 on local rank -1/0, banner log lines.
@@ -84,7 +84,7 @@ class Trainer:
         self.compute_dtype = torch.float32
         if getattr(args, "fp16", False) and self.device.type == "cuda":
             # the reference's --fp16 asks apex for O2 (half model + fp32 master weights + dynamic loss
-            # scaling, ddp.py:174-180); on B200 that is bf16 weights + fp32 masters, no loss scaling needed
+            # scaling, ddp.py:174-180); here that is bf16 weights + fp32 masters, no loss scaling needed
             self.compute_dtype = torch.bfloat16
         model = model.to(self.device)
         if self.compute_dtype != torch.float32:
@@ -283,7 +283,7 @@ class Trainer:
     # ------------------------------------------------------------------------------------------
     def _make_tracer(self):
         """``--trace_dir``: torch.profiler timeline (CPU ops, CUDA kernels, the NVTX-style ranges of ``nvtx_range``) of a
-        few optimizer steps per rank.  The reference has no tracing at all (SURVEY 5.1); numbers are never taken from a
+        few optimizer steps per rank.  The reference has no tracing at all; numbers are never taken from a
         traced run (``StepTimer`` reports the untraced steps)."""
         trace_dir = getattr(self.args, "trace_dir", None)
         steps = int(getattr(self.args, "trace_steps", 0) or 0)
@@ -307,7 +307,7 @@ class Trainer:
     # ------------------------------------------------------------------------------------------
     def save(self, epoch: int, batches_in_epoch: int) -> Optional[str]:
         """Main process writes; a barrier keeps other ranks from racing ahead into a half-written dir
-        (the reference has no barrier, SURVEY Q14)."""
+        (the reference has no barrier)."""
         path = None
         if self.is_main:
             state = {"global_step": self.global_step, "epoch": epoch, "batches_in_epoch": batches_in_epoch,

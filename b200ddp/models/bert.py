@@ -1,7 +1,7 @@
-"""BERT-base encoder + MLM head for the "BERT-base DDP bf16, seq 512" config in BASELINE.json.
-Every linear is a ``b200ddp.ops.Linear`` (tcgen05 GEMM with bias / bias+GELU epilogues), every
+"""BERT-base encoder + MLM head for the "BERT-base DDP bf16, seq 512" config.
+Every linear is a ``b200ddp.ops.Linear`` (wgmma GEMM with bias / bias+GELU epilogues), every
 LayerNorm the hand-written kernel, the loss the fused cross-entropy; attention uses torch's SDPA
-(library flash attention - not a named hot op).  109.5 M encoder parameters as in SURVEY §2.4-K4
+(library flash attention - not a named hot op).  109.5 M encoder parameters as in the stock model
 (199 tensors in the stock naming; 151 here because Q / K / V are one stored parameter) when built with ``with_mlm_head=False``."""
 from __future__ import annotations
 
@@ -56,7 +56,7 @@ class BertLayer(nn.Module):
         super().__init__()
         self.heads = c.heads
         # Q, K and V projections are ONE stored [3*hidden, hidden] parameter (rows: query, key, value): forward, dgrad and
-        # wgrad are one tcgen05 launch each and nothing is concatenated per step.  ``load_hf_state_dict`` fuses the stock
+        # wgrad are one wgmma launch each and nothing is concatenated per step.  ``load_hf_state_dict`` fuses the stock
         # model's three tensors; ``split_qkv_state_dict`` gives them back.
         self.qkv = Linear(c.hidden, 3 * c.hidden)
         self.attn_out = Linear(c.hidden, c.hidden)

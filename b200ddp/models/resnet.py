@@ -1,7 +1,7 @@
-"""ResNet-50 / ResNet-152 (He et al.) for the BASELINE.json perf configs.  Own definition (not
+"""ResNet-50 / ResNet-152 (He et al.) for the benchmark configurations.  Own definition (not
 torchvision's module) so that the stride-1 1x1 / 3x3 convolutions, BatchNorm(+add+ReLU), the stem pool and the classifier
-run on this package's kernels; parameter order / shapes match torchvision's - bucket layouts quoted in SURVEY §2.4-K4
-therefore hold.  The 7x7 stem runs on the tcgen05 tap-GEMM (``ops.StemConv7x7``); the six stride-2 convolutions stay on the library."""
+run on this package's kernels; parameter order / shapes match torchvision's - bucket layouts of stock DDP
+therefore hold.  The 7x7 stem runs on the wgmma tap-GEMM (``ops.StemConv7x7``); the six stride-2 convolutions stay on the library."""
 from __future__ import annotations
 
 import os
@@ -19,7 +19,7 @@ class Bottleneck(nn.Module):
 
     def __init__(self, inplanes: int, planes: int, stride: int = 1, downsample: nn.Module | None = None):
         super().__init__()
-        # Convolutions: tcgen05 implicit GEMMs whose epilogue hands the following BatchNorm its statistics; BatchNorm + ReLU
+        # Convolutions: wgmma implicit GEMMs whose epilogue hands the following BatchNorm its statistics; BatchNorm + ReLU
         # (and, for bn3, the shortcut add) are single fused kernels on channels_last CUDA tensors.
         self.conv1 = PointwiseConv2d(inplanes, planes)
         self.bn1 = FusedBatchNormAct2d(planes, relu=True)

@@ -5,7 +5,7 @@ extra knobs: ``relu=True`` fuses the activation, and ``forward(x, residual=...)`
 CPU, in eval mode, or for layouts the kernel does not cover, it computes the same thing with stock torch ops.
 
 The reference's own model has no normalisation (``model.py:8-16``); this op exists for the ResNet-50 / ResNet-152 configs
-BASELINE.json names, where the stock ATen BatchNorm + add + ReLU kernels were 58 % of the step (``profiles/launches.md``)."""
+the benchmark runs, where the stock ATen BatchNorm + add + ReLU kernels are a large share of the step."""
 from __future__ import annotations
 
 from typing import Optional

@@ -1,5 +1,5 @@
 """ResNet Bottleneck block as ONE autograd node whose backward is written out by hand, so that work the autograd engine would
-schedule as separate kernels rides in the convolution epilogues instead (``csrc/conv_tcgen05.cu``):
+schedule as separate kernels rides in the convolution epilogues instead (``csrc/conv_wgmma.cu``):
 
 forward    conv (+ BatchNorm statistics from the epilogue) -> BatchNorm apply (+ReLU, +shortcut): the activations are read
            once for normalisation, never for statistics.
@@ -7,7 +7,7 @@ backward   the data gradient of conv2 / conv3 also emits the partial sums S1 = s
            backward that consumes it (bn1 / bn2: no reduction pass over dy and x), and the data gradient of conv1 adds the
            shortcut gradient in its epilogue (no separate add kernel).
 
-Reference hot path replaced: ``outputs = model(x)`` / ``loss.backward()`` (``/root/reference/ddp.py:221,231``) with a ResNet
+Reference hot path replaced: ``outputs = model(x)`` / ``loss.backward()`` (``the reference ddp.py:221,231``) with a ResNet
 handed to ``train()``.  Used by ``models.resnet.Bottleneck`` for blocks whose convolutions all run on the native kernels
 (stride 1, channels_last bf16 CUDA tensors); other blocks compose the per-layer ops."""
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Autograd bindings for the hand-written sm_100a kernels.
+"""Autograd bindings for the hand-written sm_90a kernels.
 
 Every op has two bodies: CUDA tensors go to the native extension (and raise if it is missing - no
 silent fallback on a GPU box); CPU tensors use plain PyTorch math so the CPU test-suite and the gloo
@@ -7,7 +7,7 @@ kernel dispatch.
 
 Reference call sites being replaced: ``nn.Linear``/``nn.ReLU`` in ``model.py:11-16`` (cuBLASLt +
 clamp kernels), ``nn.MSELoss`` in ``ddp.py:164,222``; LayerNorm / cross-entropy / GELU are needed by the
-BERT config named in BASELINE.json.
+BERT config.
 """
 from __future__ import annotations
 
@@ -32,12 +32,12 @@ def _C():
 # Linear
 # ------------------------------------------------------------------------------------------------
 def _tc_ok(M: int, N: int, K: int) -> bool:
-    """tcgen05 path needs 16-byte row pitches for TMA for all three GEMMs (fwd, dgrad, wgrad)."""
+    """wgmma path needs 16-byte row pitches for TMA for all three GEMMs (fwd, dgrad, wgrad)."""
     return K % 8 == 0 and N % 8 == 0 and M % 8 == 0
 
 
 class _LinearTC(torch.autograd.Function):
-    """bf16 linear on tcgen05: fwd y = act(x W^T + b); bwd dgrad/wgrad without transposes (MN-major
+    """bf16 linear on wgmma: fwd y = act(x W^T + b); bwd dgrad/wgrad without transposes (MN-major
     operand descriptors), ReLU/GELU backward applied to dy before the two GEMMs."""
 
     @staticmethod
@@ -131,11 +131,11 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
 
 
 # ------------------------------------------------------------------------------------------------
-# Convolutions on tcgen05 (csrc/conv_tcgen05.cu, csrc/conv_wgrad_tcgen05.cu)
+# Convolutions on wgmma (csrc/conv_wgmma.cu, csrc/conv_wgrad_wgmma.cu)
 # ------------------------------------------------------------------------------------------------
 def _conv_policy() -> str:
-    """B200DDP_CONV: ``auto`` (default) = the hand-written tcgen05 kernels for the layer shapes where they beat the library
-    per layer (``profiles/conv_layers.md``), the library elsewhere; ``native`` = the tcgen05 kernels wherever they apply
+    """B200DDP_CONV: ``auto`` (default) = the hand-written wgmma kernels for the layer shapes where they beat the library
+    per layer, the library elsewhere; ``native`` = the wgmma kernels wherever they apply
     (every stride-1 1x1 / 3x3 convolution: forward, data gradient, BatchNorm-statistics epilogue); ``lib`` = library only."""
     return os.environ.get("B200DDP_CONV", "auto")
 
@@ -146,13 +146,12 @@ def _fprop_native(cin: int, cout: int, k: int, pixels: int) -> bool:
         return True
     if mode == "lib":
         return False
-    # No layer shape wins inside the training step yet: the 64 -> 256 expansion of layer1 is faster in isolation (14.2 us vs
-    # 18.2 us, cold L2) but the step with it is 5.08 ms vs 4.95 ms (gpurun_out/step1_{auto,lib}.json), so `auto` == library.
+    # No layer shape is selected inside the training step: `auto` == library.
     return False
 
 
 def _dgrad_native(cin: int, cout: int, k: int, pixels: int) -> bool:
-    """Data gradient: the tcgen05 kernel under ``native``; under ``auto`` no layer shape beats the library yet."""
+    """Data gradient: the wgmma kernel under ``native``; under ``auto`` no layer shape beats the library yet."""
     return _conv_policy() == "native"
 
 
@@ -189,10 +188,10 @@ def _cl(t: torch.Tensor) -> torch.Tensor:
 
 
 class _ConvTC(torch.autograd.Function):
-    """y = conv(x, w) (stride 1, 'same' padding) as a tcgen05 implicit GEMM; optionally also returns the per-CTA partial
+    """y = conv(x, w) (stride 1, 'same' padding) as a wgmma implicit GEMM; optionally also returns the per-CTA partial
     column sums / sums of squares of y from the epilogue, so the BatchNorm that follows never re-reads y for its statistics.
     Backward: data gradient on the same kernel (mirrored taps, filter read MN-major - no transposed weights), weight
-    gradient on the split-pixel tcgen05 kernel or the library (``_wgrad_native``)."""
+    gradient on the split-pixel wgmma kernel or the library (``_wgrad_native``)."""
 
     @staticmethod
     def forward(ctx, x, w, want_stats):
@@ -240,10 +239,10 @@ def conv2d_tc(x: torch.Tensor, weight: torch.Tensor, want_stats: bool = False):
 
 
 # ------------------------------------------------------------------------------------------------
-# The strided 7x7 stem (reference hot path: the model's first convolution, /root/reference/ddp.py:221,231)
+# The strided 7x7 stem (reference hot path: the model's first convolution, the reference ddp.py:221,231)
 # ------------------------------------------------------------------------------------------------
 def _stem_policy() -> str:
-    """B200DDP_STEM: ``native`` (default) = the tcgen05 stem kernels where they apply, ``lib`` = library."""
+    """B200DDP_STEM: ``native`` (default) = the wgmma stem kernels where they apply, ``lib`` = library."""
     return os.environ.get("B200DDP_STEM", "native")
 
 
@@ -262,9 +261,9 @@ def stem_conv_supported(x: torch.Tensor, weight: torch.Tensor, stride, padding) 
 
 
 class _StemConv(torch.autograd.Function):
-    """y = conv7x7/s2(x, w) on the tcgen05 tap-GEMM: the input is repacked into a zero-bordered image of row pairs whose
+    """y = conv7x7/s2(x, w) on the wgmma tap-GEMM: the input is repacked into a zero-bordered image of row pairs whose
     overlapping 128-byte windows ARE the im2col rows (one TMA tensor map, nothing materialised; csrc/conv.h); optional
-    BatchNorm-statistics epilogue.  Backward: weight gradient over the same windows on the dedicated split-pixel tcgen05
+    BatchNorm-statistics epilogue.  Backward: weight gradient over the same windows on the dedicated split-pixel wgmma
     kernel (``B200DDP_STEM_WGRAD=generic`` selects the general kernel); the input gets no gradient."""
 
     @staticmethod

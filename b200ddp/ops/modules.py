@@ -40,7 +40,7 @@ class Linear(nn.Module):
 class Conv2dTC(nn.Conv2d):
     """Bias-free ``nn.Conv2d`` (same parameter name, shape and init, so checkpoints and DDP bucket layouts are unchanged)
     whose stride-1 1x1 / 3x3 instances run forward, data gradient and (where it wins) weight gradient on the hand-written
-    tcgen05 kernels for channels_last bf16 CUDA tensors; everything else (CPU, fp32, stride 2, odd channel counts) takes
+    wgmma kernels for channels_last bf16 CUDA tensors; everything else (CPU, fp32, stride 2, odd channel counts) takes
     the stock path.  ``forward_with_stats`` additionally hands the following BatchNorm its statistics from the epilogue."""
 
     def __init__(self, in_channels: int, out_channels: int, kernel_size: int = 1, stride: int = 1, **kw):
@@ -73,7 +73,7 @@ class Conv3x3(Conv2dTC):
 
 class StemConv7x7(nn.Conv2d):
     """The ResNet stem: bias-free ``nn.Conv2d(3, 64, 7, stride=2, padding=3)`` (same parameter name / shape / init) that runs
-    forward and weight gradient on the tcgen05 kernels for channels_last bf16 CUDA input, and hands the following BatchNorm
+    forward and weight gradient on the wgmma kernels for channels_last bf16 CUDA input, and hands the following BatchNorm
     its statistics from the epilogue; anything else takes the stock path."""
 
     def __init__(self, in_channels: int = 3, out_channels: int = 64, **kw):

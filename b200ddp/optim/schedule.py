@@ -2,7 +2,7 @@
 
 Parity: reference ``ddp.py:52-61`` (factor rises 0->1 over ``warmup`` optimizer
 steps, then falls linearly to 0 at ``total``).  The reference builds a
-``LambdaLR``; here the schedule is a small host-side object (SURVEY N13) whose
+``LambdaLR``; here the schedule is a small host-side object whose
 value is pushed into the optimizer's param groups *and*, for the fused CUDA
 optimizer, into a device scalar so a captured CUDA graph never bakes the lr.
 """

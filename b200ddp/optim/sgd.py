@@ -4,7 +4,7 @@ Reference behaviour: ``optim.SGD(model.parameters(), lr=1e-3)`` (``ddp.py:183``)
 ``clip_grad_norm_(model.parameters(), max_grad_norm)`` (``ddp.py:238-239``), with an (intended, broken)
 apex O2 mixed-precision variant (``ddp.py:165-181``: fp16 model, fp32 master weights, FusedSGD).
 
-Native design (SURVEY N11/N12/N17): on CUDA the whole "norm -> clip -> update" sequence is
+Native design: on CUDA the whole "norm -> clip -> update" sequence is
   [sum-of-squares partials]  (free: written by the fused allreduce epilogue under DDP, otherwise one
                               multi-tensor launch reading the gradients where autograd left them)
   -> clip_coef                (one tiny block: sqrt, clamp - result stays on the device)

@@ -3,12 +3,12 @@
 The reference hard-codes ``init_process_group(backend="nccl")`` (``ddp.py:103``) and lets torch's
 Reducer issue NCCL calls.  Here the wrapper talks to one of:
 
-* ``b200``  - the product: hand-written sm_100a kernels over NVSwitch peer memory
+* ``b200``  - the product: hand-written sm_90a kernels over NVSwitch peer memory
               (``csrc/peer_mem.cpp`` + ``csrc/allreduce.cu`` + ``csrc/broadcast.cu``); torch's
               process group is used only to bootstrap (handle exchange) and for host-side checks.
 * ``nccl``  - stock ``torch.distributed`` collectives on GPU: the *baseline* path, kept for
               comparison runs and as the multi-node fallback.
-* ``gloo``  - CPU plumbing (BASELINE config 1: world_size=2 on CPU, no GPU).
+* ``gloo``  - CPU plumbing (world_size=2 on CPU, no GPU).
 
 This is a transport choice for one hardware target, not a multi-vendor dispatch layer: the b200
 path is the only one with native kernels.

@@ -3,8 +3,8 @@
 What the reference runs (delegated): ``torch.distributed._compute_bucket_assignment_by_size``
 called from ``TORCH/nn/parallel/distributed.py:1237-1244`` with limits ``[1 MiB, 25 MiB]``
 (because ``ddp.py:195`` passes ``find_unused_parameters=True``), and the result reversed before it
-reaches the Reducer (SURVEY N2).  ``assign_by_size`` reproduces that greedy algorithm exactly so the
-layouts quoted in SURVEY §2.4-K4 can be asserted on CPU.
+reaches the Reducer.  ``assign_by_size`` reproduces that greedy algorithm exactly so the
+layouts stock DDP builds can be asserted on CPU.
 
 The native design differs in two ways: (1) ``plan_buckets`` walks the parameters in *reverse*
 registration order (the order gradients become ready in backward) so the small first bucket is the
@@ -144,7 +144,7 @@ def plan_buckets(numels: Sequence[int], elem_sizes: Sequence[int], keys: Optiona
         # is ready; with several dtypes in play (bf16 weights + fp32 BatchNorm) the per-dtype groups interleave,
         # and sorting by first member would park e.g. the all-BatchNorm bucket (finishes at the very end) in
         # front of buckets that finish early - the in-order launch rule would then hold those back until the
-        # end of backward and expose all of their communication (measured: profiles/ddp_overhead_diag_n2_v2.txt).
+        # end of backward and expose all of their communication.
         groups.sort(key=lambda grp: (max(grp), min(grp)))
     specs = []
     last_positions = set(range(max(0, n - tail_window), n))

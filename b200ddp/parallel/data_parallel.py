@@ -1,6 +1,6 @@
 """Single-process multi-GPU mode (reference ``ddp.py:189-191``: ``DataParallel(model)`` when launched
 without a launcher on a multi-GPU host).  Kept for CLI parity only - the reference README itself says
-DDP is the faster choice (``README.md:5``) and this is not a performance target (SURVEY N14).
+DDP is the faster choice (``README.md:5``) and this is not a performance target.
 
 Implementation: scatter the batch along dim 0, replicate the module onto every visible GPU, run the
 replicas on threads, gather outputs on the first device.  Gradients flow back through the differentiable

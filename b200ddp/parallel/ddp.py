@@ -1,8 +1,8 @@
-"""DistributedDataParallel - the B200-native replacement for ``torch.nn.parallel.DistributedDataParallel``
+"""DistributedDataParallel - the H100-native replacement for ``torch.nn.parallel.DistributedDataParallel``
 as the reference uses it (``ddp.py:194-195``: ``DistributedDataParallel(model, device_ids=[local_rank],
 output_device=local_rank, find_unused_parameters=True)``).
 
-Stock behaviour being replaced (SURVEY N1-N6): parameter verification + rank-0 broadcast at wrap
+Stock behaviour being replaced: parameter verification + rank-0 broadcast at wrap
 time, per-parameter autograd hooks that copy ``grad/world`` into flat buckets, one NCCL allreduce per
 bucket overlapped with the rest of backward, an extra allreduce of the unused-parameter bitmap,
 copy-back into ``.grad``.
@@ -18,7 +18,7 @@ Native design:
 * the "which parameters were used" bitmap rides in the bucket itself (``BucketSpec.flags_offset``):
   no second collective (stock K5).
 * ``no_sync()`` makes gradient accumulation skip communication on non-boundary micro-steps (the
-  reference allreduces every micro-step, SURVEY Q5).
+  reference allreduces every micro-step).
 * gloo / nccl backends run the same bucket plan through ``torch.distributed`` for CPU tests and for
   baseline comparison.
 """
@@ -246,7 +246,7 @@ class DistributedDataParallel(nn.Module):
     def _sync_buffers_after_forward(self) -> None:
         """Native backend: rank 0's buffers (BatchNorm running statistics) reach every rank on the COMM stream right after
         the forward pass, overlapped with backward, instead of on the compute stream before the forward pass (stock
-        ``_sync_buffers``, SURVEY K7).  Training-mode forward never reads the running statistics, so at every forward
+        ``_sync_buffers``).  Training-mode forward never reads the running statistics, so at every forward
         start each rank still holds "rank 0's buffers as of its previous forward" - the stock contract - but the
         cross-GPU rendezvous of the broadcast kernel is off the critical path.  It is the first kernel on the comm stream
         of this iteration on every rank (bucket launches follow in plan order), and ``Reducer::finalize`` joins that
@@ -334,7 +334,7 @@ class DistributedDataParallel(nn.Module):
 
     def rebuild_buckets(self) -> bool:
         """Re-plan buckets by the gradient-ready order observed in the first iteration (stock Reducer
-        does this once when ``find_unused_parameters=False``, SURVEY K6).  Deterministic across ranks
+        does this once when ``find_unused_parameters=False``).  Deterministic across ranks
         because every rank runs the same graph; verified over the store."""
         order = list(getattr(self.reducer, "ready_order", []))
         if len(order) != len(self._params):

@@ -5,7 +5,7 @@ Bootstrap (once per process group): rank 0 draws a job id, every rank creates it
 abstract unix socket, [store barrier], swaps POSIX FDs with every peer and maps all arenas into one
 VA window; if every GPU reports multicast support the arenas are also bound to one NVLS multicast
 object.  ``torch.distributed`` is used for those barriers / tiny object exchanges only - it is the
-rendezvous, not the data path (SURVEY N8).
+rendezvous, not the data path.
 """
 from __future__ import annotations
 
@@ -230,7 +230,7 @@ class NativeReducer:
         self._ctor = dict(wire_dtype=wire_dtype, algo=algo, max_blocks=max_blocks)
         one_shot_max = int(os.environ.get("B200DDP_ONE_SHOT_MAX_KB", "256")) * 1024
         serial = int(os.environ.get("B200DDP_DDP_SERIAL", "-1"))       # -1: in line under CUDA-graph capture, overlapped otherwise
-        wide = int(os.environ.get("B200DDP_WIDE_BLOCKS", "296"))
+        wide = int(os.environ.get("B200DDP_WIDE_BLOCKS", "264"))
         self._c = C.Reducer(comm.arena, plans, len(params), _ALGO[algo], blocks, comm.tail_blocks, one_shot_max, gradient_as_bucket_view,
                             find_unused, 1.0, comm.timeout_s, serial, wide,
                             int(float(os.environ.get("B200DDP_TAIL_ONE_SHOT_MAX_MB", "8")) * MiB))

@@ -3,7 +3,7 @@
 Save layout is the reference's (``ddp.py:64-77,255-277``): ``<output_dir>/checkpoint-<global_step>/`` with
 ``model.bin`` (state_dict of the *unwrapped* module - no ``module.`` prefix), ``training_args.bin`` (pickled
 Namespace), ``optimizer.pt``, ``scheduler.pt``; written by the main process only.  The reference has no
-load path (``--global-step`` is parsed and ignored, SURVEY Q2); ``load_checkpoint`` + ``trainer_state.pt``
+load path (``--global-step`` is parsed and ignored); ``load_checkpoint`` + ``trainer_state.pt``
 (global step, epoch, batches consumed in the epoch, RNG state, running loss) add resume.
 """
 from __future__ import annotations

@@ -15,7 +15,7 @@ def set_seed(seed: int, n_gpu: int = 0) -> None:
 
 
 def rng_state() -> dict:
-    """Snapshot for checkpoint/resume (the reference saves none, SURVEY §5.4)."""
+    """Snapshot for checkpoint/resume (the reference saves none)."""
     state = {"python": random.getstate(), "numpy": np.random.get_state(), "torch": torch.get_rng_state()}
     if torch.cuda.is_available():
         state["cuda"] = torch.cuda.get_rng_state_all()

@@ -1,4 +1,4 @@
-"""Device-side timing helpers (SURVEY §5.1: the reference has no timers beyond tqdm's it/s).
+"""Device-side timing helpers (the reference has no timers beyond tqdm's it/s).
 
 ``StepTimer`` brackets optimizer steps with CUDA events on the launching stream and reports milliseconds per step
 and samples/s as the MAX over ranks (a multi-GPU step is as slow as its slowest rank); nothing synchronises until

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Headline benchmark (BASELINE.json): samples/sec, whole box, device-timed, max over ranks, for
-ResNet-50 data-parallel training in bf16 at 1/2/4/8 B200.
+"""Headline benchmark: samples/sec, whole box, device-timed, max over ranks, for ResNet-50 data-parallel
+training in bf16 at 1/2/4/8 H100.
 
   python bench.py --gpus 1 --steps 30 --warmup 5                       # this framework
+  python bench.py --gpus 1 --steps 30 --warmup 5 --dump-outputs DIR    # + what the last timed step computed, as .npy
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
       --master-port P bench.py --gpus N --steps K --warmup W           # N > 1
   python bench.py --impl reference ...                                 # the UNMODIFIED reference from baseline/_ref
@@ -39,7 +40,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 # the image exports NCCL_DEBUG=VERSION, which makes NCCL print a banner on stdout; stdout carries the JSON line
 os.environ["NCCL_DEBUG"] = os.environ.get("B200DDP_NCCL_DEBUG", "WARN")
-BASELINE_PUBLISHED = None   # the reference publishes no number (BASELINE.md) -> vs_baseline = null
+BASELINE_PUBLISHED = None   # the reference publishes no number -> vs_baseline = null
 
 MODEL_CHOICES = ("resnet50", "resnet152", "foo", "bert-base")
 
@@ -50,7 +51,7 @@ def parse_args():
     p.add_argument("--steps", type=int, default=30)
     p.add_argument("--warmup", type=int, default=8)
     p.add_argument("--impl", type=str, default="ours", choices=["ours", "reference", "stock"],
-                   help="ours | reference (unmodified template from baseline/_ref) | stock (torch DDP + NCCL + cuBLAS/cuDNN loop for the non-headline BASELINE configs)")
+                   help="ours | reference (unmodified template from baseline/_ref) | stock (torch DDP + NCCL + cuBLAS/cuDNN loop for the non-headline configurations)")
     p.add_argument("--model", type=str, default="resnet50", choices=MODEL_CHOICES)
     p.add_argument("--per_gpu_batch", type=int, default=None, help="default: 32 (resnet/foo, the reference default), 16 (bert-base, seq 512)")
     p.add_argument("--image_size", type=int, default=224)
@@ -66,8 +67,10 @@ def parse_args():
     p.add_argument("--no_comm", action="store_true", help="diagnostic: N ranks, gradient communication disabled")
     p.add_argument("--profile_range", action="store_true", help="cudaProfilerStart/Stop around the device-timed loop (ncu --profile-from-start off)")
     p.add_argument("--trace_dir", type=str, default=None, help="after the timed loops: 4 more steps under the CUPTI profiler, one chrome trace per rank "
-                                                                  "(<dir>/rank<r>.json) for tools/trace_digest.py; never a timing source")
+                                                                  "(<dir>/rank<r>.json); never a timing source")
     p.add_argument("--no_broadcast_buffers", action="store_true", help="diagnostic: DDP without the per-step buffer broadcast")
+    p.add_argument("--dump-outputs", dest="dump_outputs", type=str, default=None,
+                   help="after the timed steps, write what the last one computed to DIR/<name>.npy (rank 0; --impl ours)")
     args = p.parse_args()
     if args.per_gpu_batch is None:
         args.per_gpu_batch = 16 if args.model.startswith("bert") else 32
@@ -75,7 +78,7 @@ def parse_args():
 
 
 # --------------------------------------------------------------------------------------------------
-# clocks / throttle sampling during the timed region (B200_PROFILING.md recipe)
+# clocks / throttle sampling during the timed region
 # --------------------------------------------------------------------------------------------------
 class ClockSampler:
     QUERY = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -176,7 +179,7 @@ def config_dict(args, world, extra=None):
            "seq_len": 512 if args.model.startswith("bert") else None,
            "parallelism": f"dp{world}", "loss": "mse(dense one-hot target)" if not args.model.startswith("bert") else "ce",
            "optimizer": "sgd lr1e-3 + clip_grad_norm 1000 + linear warmup/decay",
-           "l2": "per-step working set (bf16 activations + weights + grads, > 2 GB at batch 32) exceeds the 126 MB L2; "
+           "l2": "per-step working set (bf16 activations + weights + grads, > 2 GB at batch 32) exceeds the 50 MB L2; "
                  "input batches rotate over distinct pinned host batches"}
     if extra:
         cfg.update(extra)
@@ -259,7 +262,7 @@ def run_ours(args):
 
     dataset = make_dataset(args)
     sampler = ShardedSampler(dataset, num_replicas=world, rank=rank, shuffle=True, seed=0) if world > 1 else \
-        torch.utils.data.RandomSampler(dataset)
+        torch.utils.data.RandomSampler(dataset, generator=torch.Generator().manual_seed(0))     # same batches every run
     # an endless index stream: with a small synthetic dataset sharded over 8 ranks an epoch is only 4 batches, and
     # draining the prefetch pipeline at every epoch boundary would be an artefact of the benchmark, not of training
     loader = BatchLoader(dataset, batch_size=args.per_gpu_batch, sampler=EndlessSampler(sampler), drop_last=True, pin_memory=True)
@@ -300,7 +303,7 @@ def run_ours(args):
     ev0.record()
     for i in range(args.steps):
         x, y = resident[i % len(resident)]
-        step(x, y)
+        last_loss_t = step(x, y)
         sched.step()
     ev1.record()
     sync_all()
@@ -327,6 +330,7 @@ def run_ours(args):
             wait_s += time.perf_counter() - t_w
             h2d_bytes += x.numel() * x.element_size() + y.numel() * y.element_size()
             loss = step(x, y)
+            last_loss_t = loss
             sched.step()
             slot = loss_ring[i % len(loss_ring)]
             slot.copy_(loss.detach().float().reshape(()), non_blocking=True)     # D2H read of this step's loss
@@ -355,7 +359,7 @@ def run_ours(args):
     value = global_batch * args.steps / (ms_dev / 1e3)
     stats = model.ddp_stats() if hasattr(model, "ddp_stats") else {}
     if rank == 0:
-        out = {"metric": "samples/sec (whole box, device-timed, max over ranks) for ResNet-50 DDP at 1/2/4/8 B200"
+        out = {"metric": "samples/sec (whole box, device-timed, max over ranks) for ResNet-50 DDP at 1/2/4/8 H100"
                if args.model == "resnet50" else f"samples/sec {args.model}",
                "impl": "ours", "value": value, "unit": "samples/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                "ms_per_step": ms_dev / args.steps, "higher_is_better": True, "scaling": "weak",
@@ -372,6 +376,8 @@ def run_ours(args):
                           "d2h_bytes_per_step": e2e["d2h"], "last_loss": e2e["last_loss"],
                           "host_wait_for_batch_ms_per_step": e2e["loader_wait_ms"]}
         emit(out)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_loss_t, inner)
     if args.trace_dir:
         from torch.profiler import ProfilerActivity, profile
         os.makedirs(args.trace_dir, exist_ok=True)
@@ -391,6 +397,26 @@ def run_ours(args):
         except Exception:
             pass
         dist.destroy_process_group()
+
+
+DUMP_SAMPLE = 1 << 20      # parameter elements kept by --dump-outputs (4 MB as float32)
+
+
+def dump_outputs(out_dir, loss, model):
+    """What a caller of the timed step receives from its last call: the loss it returned and the parameters it left
+    behind.  ``loss.npy`` (float32), ``param_sums.npy`` (float64 sum of every parameter tensor, in ``named_parameters``
+    order) and ``params_sample.npy`` (float32, a fixed seeded sample of DUMP_SAMPLE elements of all parameters
+    flattened in that order), so that two builds can be compared output for output."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    params = [p.detach() for _, p in model.named_parameters()]
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    np.save(os.path.join(out_dir, "param_sums.npy"), torch.stack([p.double().sum() for p in params]).cpu().numpy())
+    flat = torch.cat([p.float().reshape(-1) for p in params])
+    n = min(DUMP_SAMPLE, flat.numel())
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:n].sort().values
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat[idx.to(flat.device)].cpu().numpy())
 
 
 # --------------------------------------------------------------------------------------------------
@@ -523,7 +549,7 @@ def run_reference(args):
     value = global_batch * K / (ms / 1e3)
     target_bytes = args.per_gpu_batch * (5 if args.model == "foo" else 1000) * 4
     if rank == 0:
-        emit({"metric": "samples/sec (whole box, device-timed, max over ranks) for ResNet-50 DDP at 1/2/4/8 B200",
+        emit({"metric": "samples/sec (whole box, device-timed, max over ranks) for ResNet-50 DDP at 1/2/4/8 H100",
               "impl": "reference", "model": args.model, "value": value, "unit": "samples/s", "n_gpus": world, "steps": K, "warmup": W,
               "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
               "data": "synthetic (random-init weights, random ImageNet-shaped batches via the reference DataLoader, pin_memory)",
@@ -537,7 +563,7 @@ def run_reference(args):
 
 
 # --------------------------------------------------------------------------------------------------
-# stock arm: plain torch DDP + NCCL + library kernels on the same workload (BASELINE configs 3 and 4)
+# stock arm: plain torch DDP + NCCL + library kernels on the same workload (the non-headline configurations)
 # --------------------------------------------------------------------------------------------------
 def run_stock(args):
     """Competent stock loop (the honest bar next to the host-bound reference loop): torch DDP + NCCL + cuDNN/cuBLAS on

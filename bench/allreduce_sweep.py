@@ -1,13 +1,12 @@
 #!/usr/bin/env python
-"""BASELINE config 5: allreduce bus-bandwidth sweep 1 KB - 1 GB at 2/4/8 GPUs, peer-memory kernels vs NCCL.
+"""Allreduce bus-bandwidth sweep 1 KB - 1 GB at 2/4/8 GPUs, peer-memory kernels vs NCCL.
 
-  torchrun --nproc-per-node N bench/allreduce_sweep.py [--max_mb 1024] [--out gpurun_out/sweep_N.json]
+  torchrun --nproc-per-node N bench/allreduce_sweep.py [--max_mb 1024] [--out sweep_N.json]
 
 busbw = (S / t) * 2 (P-1) / P with S the payload bytes per rank (what nccl-tests prints); device-timed with
 CUDA events, max over ranks, 5 warm-up + 20 timed launches per point, buffers rotated so each launch reads
 memory that is not L2-resident from the previous one when the payload is below L2 size.
-Roofline: bytes per direction per GPU = S (P-1)/P for two-shot / one-shot pull, ~S/P + S/P for NVLS; link peak
-770 GB/s measured per direction (B200_PROFILING.md).
+Roofline: bytes per direction per GPU = S (P-1)/P for two-shot / one-shot pull, ~S/P + S/P for NVLS.
 """
 import argparse
 import json
@@ -54,14 +53,17 @@ def main():
     ap.add_argument("--max_mb", type=int, default=1024)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--out", type=str, default=None)
-    ap.add_argument("--blocks", type=str, default="8,32,128,296")
+    ap.add_argument("--blocks", type=str, default=None, help="CTA counts to try (default: 8,32,128 and the largest the kernels accept)")
     args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
     dist.init_process_group("nccl", device_id=dev)
     os.environ.setdefault("B200DDP_SCRATCH_MB", str(args.max_mb + 8))
+    from b200ddp import _ext
     from b200ddp.parallel.peer import PeerCollectives
+    max_blocks = int(_ext.get().MAX_COMM_BLOCKS)
+    block_list = args.blocks or f"8,32,128,{max_blocks}"
     comm = PeerCollectives.get(None, dev, min_bytes=(args.max_mb + 16) << 20)
     sym_all = comm.symmetric_empty(args.max_mb * 1024 * 1024 // 4, torch.float32)
     results = {"world": world, "nvls": comm.nvls, "points": []}
@@ -83,7 +85,7 @@ def main():
                 (["nvls_one_shot"] if comm.nvls and size <= (4 << 20) else [])
         for wire in ("fp32", "bf16"):
             for algo in algos:
-                cand = sorted({int(b) for b in args.blocks.split(",")})
+                cand = sorted({int(b) for b in block_list.split(",") if 0 < int(b) <= max_blocks})
                 keep = [b for b in cand if not ((size < 65536 and b > 8) or (size >= (16 << 20) and b < 32))] or \
                        ([cand[0]] if size < 65536 else [cand[-1]])
                 for blocks in keep:
@@ -105,7 +107,7 @@ def main():
         sym.normal_()
         sbest = None
         for algo in ["two_shot"] + (["nvls"] if comm.nvls else []):
-            for blocks in (8, 32, 64, 128, 296):
+            for blocks in (8, 32, 64, 128, max_blocks):
                 if (size < 65536 and blocks > 8) or (size >= (16 << 20) and blocks < 64):
                     continue
                 ms = timed(lambda: comm.allreduce_symmetric_(sym, algo=algo, blocks=blocks), args.iters, world, dev)

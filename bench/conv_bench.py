@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Experimental tcgen05 3x3 convolution forward vs cuDNN on the ResNet-50 (batch 32) 3x3 shapes.
+"""Experimental wgmma 3x3 convolution forward vs cuDNN on the ResNet-50 (batch 32) 3x3 shapes.
 
   python bench/conv_bench.py [--iters 20]
 

@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Per-layer convolution table for ResNet-50 (batch 32, bf16, channels_last): cuDNN fprop / dgrad / wgrad time per
-distinct layer shape (the bar), next to this framework's tcgen05 kernels (``csrc/conv_tcgen05.cu``,
-``csrc/conv_wgrad_tcgen05.cu``), with an optional sweep over their tiling knobs.
+distinct layer shape (the bar), next to this framework's wgmma kernels (``csrc/conv_wgmma.cu``,
+``csrc/conv_wgrad_wgmma.cu``), with an optional sweep over their tiling knobs.
 
-  python bench/conv_layers.py [--reps 40] [--batch 32] [--sweep] [--only l3] [--out gpurun_out/conv_layers.json]
+  python bench/conv_layers.py [--reps 40] [--batch 32] [--sweep] [--only l3] [--out conv_layers.json]
 
 Timing: CUDA events around the replay of a CUDA graph holding `reps` back-to-back launches that rotate over enough
-distinct input sets to exceed the 126 MB L2 (>= 192 MB of operands in rotation), after warm-up rounds; best of 3 replays,
+distinct input sets to exceed the 50 MB L2 (>= 192 MB of operands in rotation), after warm-up rounds; best of 3 replays,
 reported per launch.  (Single eager launches are host-bound at ~10 us through the Python bindings and event timing is
 quantised at ~2 us, which hides kernels of 5-15 us.)
-The reference's hot path these replace: the model's forward / backward at /root/reference/ddp.py:221,231."""
+The reference's hot path these replace: the model's forward / backward at the reference ddp.py:221,231."""
 import argparse
 import json
 import os

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """The strided 7x7 stem of ResNet-50 (batch 32, 224x224, bf16, channels_last): library forward / weight gradient against
-this framework's tcgen05 path (csrc/conv_stem.cu packing + conv_tcgen05.cu / conv_wgrad_tcgen05.cu through the
+this framework's wgmma path (csrc/conv_stem.cu packing + conv_wgmma.cu / conv_wgrad_wgmma.cu through the
 overlapping-window tensor map).  Timing as in bench/conv_layers.py: CUDA events around the replay of a CUDA graph of
 `reps` launches rotating over > 192 MB of operands, best of 3.
-  python bench/stem_bench.py [--batch 32] [--reps 20] [--out gpurun_out/stem_bench.json]"""
+  python bench/stem_bench.py [--batch 32] [--reps 20] [--out stem_bench.json]"""
 import argparse
 import json
 import os

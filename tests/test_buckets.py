@@ -1,4 +1,4 @@
-"""Bucket planner vs torch's ``_compute_bucket_assignment_by_size`` and the layouts quoted in SURVEY §2.4-K4."""
+"""Bucket planner vs torch's ``_compute_bucket_assignment_by_size`` and the layouts stock DDP builds."""
 import pytest
 import torch
 import torch.distributed as dist
@@ -28,7 +28,7 @@ def test_torch_order_matches_stock_layout(name, expected):
 
 @pytest.mark.parametrize("cap,count", [(1, 76), (25, 14), (256, 3)])
 def test_bert_bucket_counts(cap, count):
-    """SURVEY 2.4-K4 layouts of the stock BERT-base tensor list (199 tensors: separate query / key / value), and the planner
+    """Layouts of the stock BERT-base tensor list (199 tensors: separate query / key / value), and the planner
     against torch's on this package's model, whose Q / K / V projection is one stored parameter (151 tensors)."""
     import torch
     model = build_model("bert-base", with_mlm_head=False)

@@ -1,4 +1,4 @@
-"""Host-side checks for the tcgen05 convolution kernels (csrc/conv_tcgen05.cu): the kernels need a GPU
+"""Host-side checks for the wgmma convolution kernels (csrc/conv_wgmma.cu): the kernels need a GPU
 (tests/test_gpu_conv.py); what can be pinned down here is their *index plan* - tile shapes, tap -> TMA coordinates, halo row
 offsets, mirrored taps of the data gradient, filter column order, accumulator row -> pixel.  ``emulate`` walks exactly the
 indices the kernel walks, with zero fill standing in for the TMA unit's out-of-bounds behaviour."""
@@ -131,7 +131,7 @@ def test_conv_module_falls_back_on_cpu_and_keeps_parameter_layout():
 
 
 def test_stem_window_algebra_and_geometry():
-    """The layout contract of the tcgen05 stem (csrc/conv.h): with the input repacked into a zero-bordered image of ROW PAIRS
+    """The layout contract of the wgmma stem (csrc/conv.h): with the input repacked into a zero-bordered image of ROW PAIRS
     (16-byte pixels: padded rows 2i and 2i+1, 4 channels each), the 64-element window starting every 16 elements (32 bytes)
     of pair row oh + t IS the im2col row of filter rows 2t, 2t+1 - for forward and weight gradient.  Checked here in plain
     PyTorch against F.conv2d; the host-side geometry predicate too."""

@@ -1,4 +1,4 @@
-"""Distributed plumbing on CPU (gloo, world_size 2): BASELINE config 1 and SURVEY §4 item 2."""
+"""Distributed plumbing on CPU (gloo, world_size 2)."""
 import copy
 import os
 import tempfile

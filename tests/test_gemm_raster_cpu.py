@@ -1,6 +1,6 @@
 """Host mirror of the persistent GEMM's tile rasterisation (csrc/gemm.h::gemm_tile_coords).
 
-The producer, issuer and epilogue roles of the tcgen05 kernels all map a linear tile id through this function, so a
+The producer, issuer and epilogue roles of the wgmma kernels all map a linear tile id through this function, so a
 bijection here is what guarantees every output tile is computed exactly once whatever the order.
 """
 import pytest
@@ -24,11 +24,11 @@ def test_default_order_is_m_fastest():
 
 
 def test_grouped_order_keeps_a_wave_in_a_compact_patch():
-    # 32x32 tiles, 74 tiles in flight (one wave of CTA pairs): the grouped order touches 8 m-blocks x ~10 n-blocks,
-    # the m-fastest order 32 m-blocks x 3 n-blocks -> operand tiles fetched per wave 18 vs 35.
+    # 32x32 tiles, 132 tiles in flight (one wave of single-CTA tiles, one per SM): the grouped order touches 8 m-blocks x 17
+    # n-blocks, the m-fastest order 32 m-blocks x 5 n-blocks -> operand tiles fetched per wave 25 vs 37.
     C = _ext.get()
-    for group_m, max_operand_tiles in ((0, 35), (8, 18)):
-        wave = C.gemm_tile_order(32, 32, group_m)[:74]
+    for group_m, max_operand_tiles in ((0, 37), (8, 25)):
+        wave = C.gemm_tile_order(32, 32, group_m)[:132]
         ms = {m for m, _ in wave}
         ns = {n for _, n in wave}
         assert len(ms) + len(ns) <= max_operand_tiles, (group_m, len(ms), len(ns))

@@ -106,7 +106,7 @@ def test_maxpool3x3s2_matches_torch(dtype, shape):
     assert torch.allclose(x.grad.float(), xr.grad.float(), atol=1e-2 if dtype == torch.bfloat16 else 1e-6)
 
 
-# ---- the two measured-and-kept experiment paths (default off; profiles/README.md timeline) ---------------------------
+# ---- the two kept experiment paths (default off) ---------------------------------------------------------------------
 def _bn_fwd_bwd(shape, relu, residual, seed=0):
     from b200ddp.ops import FusedBatchNormAct2d
     torch.manual_seed(seed)
@@ -143,7 +143,7 @@ def test_programmatic_dependent_launch_path_matches_default(shape, relu, residua
 
 
 def test_single_launch_batchnorm_path_matches_default():
-    """B200DDP_BN_FUSED=1 (one launch per direction with a tile barrier; measured not faster, kept selectable): same results as
+    """B200DDP_BN_FUSED=1 (one launch per direction with a tile barrier, kept selectable): same results as
     the default 2 + 2 launches.  The switch is read once per process, hence the subprocess."""
     import os
     import subprocess

@@ -1,4 +1,4 @@
-"""tcgen05 convolution kernels (csrc/conv_tcgen05.cu, csrc/conv_wgrad_tcgen05.cu) against a plain PyTorch fp32 reference of
+"""wgmma convolution kernels (csrc/conv_wgmma.cu, csrc/conv_wgrad_wgmma.cu) against a plain PyTorch fp32 reference of
 the same op: forward, data gradient, weight gradient, epilogue BatchNorm statistics, every tiling, ResNet's map sizes."""
 import pytest
 import torch
@@ -44,7 +44,7 @@ def test_forward_and_data_gradient_match_fp32_reference(n, ci, co, k, h, w):
     pad = (k - 1) // 2
     modes = [-1] if k == 1 else [1, 2]
     for mode in modes:
-        for bn in (0, 64, 128, 256):
+        for bn in (0, 64, 128, 256):                      # 256 runs as two 128-wide n-tiles (csrc/conv.h)
             if bn and (co % bn or ci % bn):
                 continue
             y = C.conv_fprop(x, wt, 1, pad, mode, bn, 0, False)[0]

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (fwd / dgrad / wgrad operand layouts, epilogues, ragged shapes) vs fp32 matmul."""
+"""wgmma GEMM (fwd / dgrad / wgrad operand layouts, epilogues, ragged shapes) vs fp32 matmul."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -73,7 +73,7 @@ def test_linear_module_fwd_bwd(C, act, tokens, fin, fout):
     y = lin(x)
     dy = torch.randn_like(y)
     y.backward(dy)
-    assert C.launch_count() - before >= 3                  # fwd + dgrad + wgrad on tcgen05
+    assert C.launch_count() - before >= 3                  # fwd + dgrad + wgrad on wgmma
     xr = x.detach().float().requires_grad_()
     wr, br = lin.weight.detach().float().requires_grad_(), lin.bias.detach().float().requires_grad_()
     yr = F.linear(xr, wr, br)

@@ -1,4 +1,5 @@
-"""cta_group::2 GEMM (CTA pairs, 256x256 tiles) vs fp32 matmul, every operand layout, ragged shapes."""
+"""Cluster-pair GEMM (two CTAs of a cluster, 256x128 pair tiles, B tile shared through TMA multicast) vs fp32 matmul and
+the single-CTA kernel, every operand layout, ragged shapes."""
 import pytest
 import torch
 

@@ -1,6 +1,6 @@
 """Grouped tile rasterisation (B200DDP_GEMM_GROUP_M / set_gemm_group_m): results must be bit-identical to the
-default m-fastest order, since only the order in which persistent CTAs pick tiles changes.  (Measured: not faster on any
-benchmarked shape - 8192^3 0.88 vs 0.72 ms - so the default stays m-fastest; the knob remains for larger-than-L2 problems.)"""
+default m-fastest order, since only the order in which persistent CTAs pick tiles changes.  The default stays m-fastest;
+the knob is for larger-than-L2 problems.  mode 1 = single-CTA tiles, mode 2 = cluster pairs."""
 
 import pytest
 import torch

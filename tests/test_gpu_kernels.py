@@ -1,4 +1,4 @@
-"""Numerics of every single-GPU sm_100a kernel against a plain PyTorch fp32 reference (SURVEY §4 item 3)."""
+"""Numerics of every single-GPU sm_90a kernel against a plain PyTorch fp32 reference."""
 import math
 
 import pytest
@@ -190,7 +190,7 @@ def test_gelu_fwd_bwd(C, dtype, n):
 
 
 def test_bert_tiny_gpu_matches_cpu_reference():
-    """bf16 BERT on the native kernels (fused-QKV tcgen05 GEMMs, LayerNorm, GELU, cross-entropy) vs the same weights in
+    """bf16 BERT on the native kernels (fused-QKV wgmma GEMMs, LayerNorm, GELU, cross-entropy) vs the same weights in
     fp32 on the CPU path: loss and every parameter gradient agree to bf16 accuracy."""
     from b200ddp.models.bert import BertConfig, BertForMaskedLM
     from b200ddp.ops import cross_entropy

@@ -1,4 +1,4 @@
-"""Multi-GPU checks of the NVSwitch peer-memory transport (run with >= 2 GPUs; SURVEY §4 items 3-4)."""
+"""Multi-GPU checks of the NVSwitch peer-memory transport (run with >= 2 GPUs)."""
 import os
 
 import pytest
@@ -356,7 +356,7 @@ def test_ddp_resnet50_matches_stock_ddp(free_port):
 # --------------------------------------------------------------------------------------------------
 def _check_timeout(rank, world):
     """A peer that never shows up must surface as an error after the timeout, not hang the kernel forever
-    (SURVEY §5.3: signal-pad waits need timeouts)."""
+    (signal-pad waits need timeouts)."""
     import time
     from b200ddp.parallel.peer import PeerCollectives, PeerCommError
     dev = torch.device("cuda", rank)

@@ -1,4 +1,4 @@
-"""Sampler / schedule / logger / CLI parity with the reference behaviour (SURVEY §4 item 1)."""
+"""Sampler / schedule / logger / CLI parity with the reference behaviour."""
 import logging
 import math
 import re

@@ -210,7 +210,7 @@ def test_resnet50_matches_torchvision_given_its_weights():
 
 
 def test_trace_dir_writes_a_chrome_trace(tmp_path):
-    """--trace_dir: a torch.profiler timeline of a few optimizer steps (SURVEY 5.1: the reference has no tracing)."""
+    """--trace_dir: a torch.profiler timeline of a few optimizer steps (the reference has no tracing)."""
     import json
     trace_dir = tmp_path / "traces"
     _run(tmp_path, "--max_steps", "12", "--save_steps", "0", "--trace_dir", str(trace_dir), "--trace_steps", "2", "--trace_skip", "3")
