@@ -9,5 +9,5 @@ __version__ = "0.1.0"
 
 from . import utils  # noqa: F401
 from .parallel import DistributedDataParallel, DataParallel, ShardedSampler  # noqa: F401
-from .optim import FusedSGD, get_linear_schedule_with_warmup  # noqa: F401
+from .optim import FusedAdamW, FusedSGD, get_linear_schedule_with_warmup  # noqa: F401
 from .models import FooModel, build_model  # noqa: F401

@@ -1,5 +1,5 @@
 // Python bindings.  The only translation unit that sees torch headers.  Which reference call site each op stands in for is
-// documented on the Python side (b200ddp/ops/functional.py, parallel/peer.py, optim/sgd.py).
+// documented on the Python side (b200ddp/ops/functional.py, parallel/peer.py, optim/).
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -117,12 +117,12 @@ int broadcast_tensors(PeerArena& arena, const std::vector<at::Tensor>& tensors, 
 }
 
 // ---- optimizer ---------------------------------------------------------------------------------
-struct SgdPlan {
+struct OptPlan {
   std::vector<uintptr_t> params;
   std::vector<long long> numels, flat_offs;
   DType p_dtype, g_dtype;
   int total_blocks = 0;
-  SgdPlan(std::vector<uintptr_t> p, std::vector<long long> n, std::vector<long long> fo, int pd, int gd)
+  OptPlan(std::vector<uintptr_t> p, std::vector<long long> n, std::vector<long long> fo, int pd, int gd)
       : params(std::move(p)), numels(std::move(n)), flat_offs(std::move(fo)), p_dtype((DType)pd), g_dtype((DType)gd) {
     for (auto v : numels) total_blocks += ceil_div(v, kOptChunk);
   }
@@ -149,7 +149,7 @@ struct SgdPlan {
     }
   }
   int sqnorm(const std::vector<uintptr_t>& grads, uintptr_t partials, uintptr_t stream) const {
-    TORCH_CHECK(grads.size() == params.size(), "SgdPlan: gradient list length mismatch");
+    TORCH_CHECK(grads.size() == params.size(), "OptPlan: gradient list length mismatch");
     for_each_table(grads, [&](const OptTable& tab, int base) {
       launch_multi_sqnorm(tab, g_dtype, reinterpret_cast<float*>(partials) + base, reinterpret_cast<cudaStream_t>(stream));
     });
@@ -158,7 +158,7 @@ struct SgdPlan {
   void step(const std::vector<uintptr_t>& grads, uintptr_t lr, uintptr_t clip_coef, uintptr_t master, uintptr_t mom,
             uintptr_t step_count, double momentum, double dampening, double weight_decay, double grad_scale, bool nesterov,
             bool zero_grad, uintptr_t stream) const {
-    TORCH_CHECK(grads.size() == params.size(), "SgdPlan: gradient list length mismatch");
+    TORCH_CHECK(grads.size() == params.size(), "OptPlan: gradient list length mismatch");
     SgdHyper h;
     h.lr = reinterpret_cast<const float*>(lr);
     h.clip_coef = reinterpret_cast<const float*>(clip_coef);
@@ -173,6 +173,28 @@ struct SgdPlan {
     h.zero_grad = zero_grad ? 1 : 0;
     for_each_table(grads, [&](const OptTable& tab, int) {
       launch_multi_sgd(tab, p_dtype, g_dtype, h, reinterpret_cast<cudaStream_t>(stream));
+    });
+  }
+  void adamw(const std::vector<uintptr_t>& grads, uintptr_t lr, uintptr_t clip_coef, uintptr_t master, uintptr_t exp_avg,
+             uintptr_t exp_avg_sq, uintptr_t step_count, double beta1, double beta2, double eps, double weight_decay,
+             double grad_scale, bool zero_grad, uintptr_t stream) const {
+    TORCH_CHECK(grads.size() == params.size(), "OptPlan: gradient list length mismatch");
+    TORCH_CHECK(lr && exp_avg && exp_avg_sq && step_count, "OptPlan.adamw: lr, moments and step count are required");
+    AdamHyper h;
+    h.lr = reinterpret_cast<const float*>(lr);
+    h.clip_coef = reinterpret_cast<const float*>(clip_coef);
+    h.master = reinterpret_cast<float*>(master);
+    h.exp_avg = reinterpret_cast<float*>(exp_avg);
+    h.exp_avg_sq = reinterpret_cast<float*>(exp_avg_sq);
+    h.step_count = reinterpret_cast<const int*>(step_count);
+    h.beta1 = (float)beta1;
+    h.beta2 = (float)beta2;
+    h.eps = (float)eps;
+    h.weight_decay = (float)weight_decay;
+    h.grad_scale = (float)grad_scale;
+    h.zero_grad = zero_grad ? 1 : 0;
+    for_each_table(grads, [&](const OptTable& tab, int) {
+      launch_multi_adamw(tab, p_dtype, g_dtype, h, reinterpret_cast<cudaStream_t>(stream));
     });
   }
 };
@@ -293,11 +315,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def_readonly("iterations", &Reducer::iterations)
       .def_readonly("ready_order", &Reducer::ready_order);
 
-  py::class_<SgdPlan>(m, "SgdPlan")
+  py::class_<OptPlan>(m, "OptPlan")
       .def(py::init<std::vector<uintptr_t>, std::vector<long long>, std::vector<long long>, int, int>())
-      .def_readonly("total_blocks", &SgdPlan::total_blocks)
-      .def("sqnorm", &SgdPlan::sqnorm)
-      .def("step", &SgdPlan::step);
+      .def_readonly("total_blocks", &OptPlan::total_blocks)
+      .def("sqnorm", &OptPlan::sqnorm)
+      .def("step", &OptPlan::step)
+      .def("adamw", &OptPlan::adamw);
   m.def("clip_coef", [](at::Tensor partials, int n, double max_norm, double grad_scale, at::Tensor coef, at::Tensor norm) {
     launch_clip_coef(partials.data_ptr<float>(), n, (float)max_norm, (float)grad_scale, coef.data_ptr<float>(),
                      norm.data_ptr<float>(), cur_stream());

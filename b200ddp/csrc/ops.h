@@ -32,11 +32,24 @@ struct SgdHyper {
   int nesterov;
   int zero_grad;            // write zeros back into g after use
 };
+// AdamW (decoupled weight decay).  One launch per (param group, dtype, table): the table fills the kernel-parameter space,
+// so per-group hyper-parameters travel here rather than per slot.
+struct AdamHyper {
+  const float* lr;          // device scalar of this param group
+  const float* clip_coef;   // device scalar from clip_coef kernel (nullptr = 1)
+  float* master;            // flat fp32 master weights (nullptr when params are fp32)
+  float* exp_avg;           // flat fp32 first moment
+  float* exp_avg_sq;        // flat fp32 second moment
+  const int* step_count;    // device scalar: steps already taken (bias correction uses *step_count + 1)
+  float beta1, beta2, eps, weight_decay, grad_scale;
+  int zero_grad;            // write zeros back into g after use
+};
 
 void launch_multi_sqnorm(const OptTable& tab, DType g_dtype, float* partials /*[total_blocks]*/, cudaStream_t s);
 void launch_clip_coef(const float* partials, int n, float max_norm, float grad_scale, float* coef_out,
                       float* norm_out, cudaStream_t s);
 void launch_multi_sgd(const OptTable& tab, DType p_dtype, DType g_dtype, const SgdHyper& h, cudaStream_t s);
+void launch_multi_adamw(const OptTable& tab, DType p_dtype, DType g_dtype, const AdamHyper& h, cudaStream_t s);
 void launch_scale_inplace(float* x, size_t n, const float* scalar, cudaStream_t s);
 
 // ---------------- losses (loss.cu) --------------------------------------------------------------

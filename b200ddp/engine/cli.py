@@ -48,6 +48,11 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--lr", type=float, default=1e-3)
     p.add_argument("--momentum", type=float, default=0.0)
     p.add_argument("--weight_decay", type=float, default=0.0)
+    p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adamw"],
+                   help="fused SGD, or fused AdamW with fp32 masters (weight decay on ndim >= 2 parameters only)")
+    p.add_argument("--adam_beta1", type=float, default=0.9)
+    p.add_argument("--adam_beta2", type=float, default=0.999)
+    p.add_argument("--adam_epsilon", type=float, default=1e-8)
     p.add_argument("--dataset_size", type=int, default=100000)
     p.add_argument("--seq_len", type=int, default=512)
     p.add_argument("--backend", type=str, default="auto", choices=["auto", "b200", "nccl", "gloo"])

@@ -24,7 +24,7 @@ from tqdm.auto import trange
 
 from ..data import BatchLoader, DevicePrefetcher, FooDataset, SyntheticImageNet, SyntheticTokens
 from ..ops import CrossEntropyLoss, MSELoss
-from ..optim import FusedSGD, get_linear_schedule_with_warmup
+from ..optim import FusedAdamW, FusedSGD, get_linear_schedule_with_warmup, weight_decay_groups
 from ..parallel import DataParallel, DistributedDataParallel, ShardedSampler
 from ..utils import StepTimer, is_main_process, nvtx_range, rng_state, restore_rng_state, to_mixed_bf16
 from ..utils.checkpoint import latest_checkpoint, load_checkpoint, save_checkpoint
@@ -133,8 +133,7 @@ class Trainer:
                 wire_dtype=getattr(args, "wire_dtype", None), broadcast_buffers=getattr(args, "broadcast_buffers", True))
 
         # ---- optimizer / schedule: built AFTER the broadcast so fp32 master weights start identical --
-        self.optimizer = FusedSGD(inner.parameters(), lr=getattr(args, "lr", 1e-3), momentum=getattr(args, "momentum", 0.0),
-                                  weight_decay=getattr(args, "weight_decay", 0.0), max_grad_norm=args.max_grad_norm)
+        self.optimizer = self._build_optimizer(inner)
         self.scheduler = get_linear_schedule_with_warmup(self.optimizer, num_warmup_steps=args.warmup_steps,
                                                          num_training_steps=self.t_total)
         if self.resume_dir:
@@ -153,6 +152,18 @@ class Trainer:
         self.last_throughput = None
 
     # ------------------------------------------------------------------------------------------
+    def _build_optimizer(self, inner: torch.nn.Module):
+        args = self.args
+        lr, wd = getattr(args, "lr", 1e-3), getattr(args, "weight_decay", 0.0)
+        if getattr(args, "optimizer", "sgd") == "adamw":
+            groups = weight_decay_groups(inner, wd)
+            self.log.info("AdamW parameter groups.", dict(decay=len(groups[0]["params"]), no_decay=len(groups[1]["params"]),
+                                                          weight_decay=wd))
+            return FusedAdamW(groups, lr=lr, betas=(getattr(args, "adam_beta1", 0.9), getattr(args, "adam_beta2", 0.999)),
+                              eps=getattr(args, "adam_epsilon", 1e-8), max_grad_norm=args.max_grad_norm)
+        return FusedSGD(inner.parameters(), lr=lr, momentum=getattr(args, "momentum", 0.0), weight_decay=wd,
+                        max_grad_norm=args.max_grad_norm)
+
     def _make_image_transform(self):
         """Raw NCHW batch (fp32 or uint8) -> compute dtype, channels_last when the model is, in ONE kernel
         (``csrc/input.cu``); writes into the CUDA graph's static input once that exists."""

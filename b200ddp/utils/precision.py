@@ -1,7 +1,7 @@
 """Mixed-precision placement: bf16 weights/activations with BatchNorm kept in fp32 (cuDNN's fast NHWC
 batch-norm kernels want bf16 activations with fp32 scale/bias/statistics).  This is the working version of
 what the reference's ``--fp16`` asks apex for (O2: half model + fp32 master weights, ``ddp.py:174-180``); the
-fp32 masters live in ``b200ddp.optim.FusedSGD``."""
+fp32 masters live in the fused optimizers (``b200ddp.optim.FusedSGD``, ``b200ddp.optim.FusedAdamW``)."""
 from __future__ import annotations
 
 import torch
