@@ -492,6 +492,78 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                      stats.data_ptr<float>());
     return std::make_tuple(d, stats);
   });
+  // ---- FP8 (fp8.cu, gemm_wgmma.cu): E4M3 activations / weights, E5M2 gradients, power-of-two per-tensor scales ------------
+  m.def("fp8_amax", [](at::Tensor t) {
+    check_cuda(t, "t");
+    TORCH_CHECK(t.scalar_type() == at::kBFloat16 && t.is_contiguous(), "fp8_amax: contiguous bf16 tensor");
+    c10::cuda::CUDAGuard guard(t.device());
+    if ((reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) != 0) t = t.clone();
+    at::Tensor amax = at::empty({1}, t.options().dtype(at::kFloat));
+    launch_fp8_amax(t.data_ptr(), (size_t)t.numel(), amax.data_ptr<float>(), cur_stream());
+    return amax;
+  });
+  // q (t's shape), q^T [cols, rows] or None, scale_inv [1] (= 1/s), fp32 column sums [cols] or None; s comes from `amax`
+  auto fp8_cast = [](at::Tensor t, at::Tensor amax, const std::string& fmt, bool want_transpose, bool want_colsum) {
+    TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "fp8: format must be 'e4m3' or 'e5m2', got '", fmt, "'");
+    TORCH_CHECK(amax.is_cuda() && amax.scalar_type() == at::kFloat && amax.numel() == 1, "fp8: amax must be a 1-element fp32 CUDA tensor");
+    const bool e5m2 = fmt == "e5m2";
+    const int cols = (int)t.size(-1);
+    const int rows = (int)(t.numel() / cols);
+    at::Tensor q = at::empty(t.sizes(), t.options().dtype(e5m2 ? at::kFloat8_e5m2 : at::kFloat8_e4m3fn));
+    at::Tensor qt = want_transpose ? at::empty({cols, rows}, q.options()) : at::Tensor();
+    at::Tensor scale_inv = at::empty({1}, t.options().dtype(at::kFloat));
+    at::Tensor colsum, partial;
+    if (want_colsum) {
+      colsum = at::empty({cols}, t.options().dtype(at::kFloat));
+      partial = at::empty({fp8_colsum_parts(rows), cols}, t.options().dtype(at::kFloat));
+    }
+    launch_fp8_cast_transpose(t.data_ptr(), rows, cols, amax.data_ptr<float>(), e5m2, q.data_ptr(),
+                              want_transpose ? qt.data_ptr() : nullptr, want_colsum ? partial.data_ptr<float>() : nullptr,
+                              want_colsum ? colsum.data_ptr<float>() : nullptr, scale_inv.data_ptr<float>(), cur_stream());
+    return py::make_tuple(q, want_transpose ? py::cast(qt) : py::none(), scale_inv, want_colsum ? py::cast(colsum) : py::none());
+  };
+  auto fp8_input = [](at::Tensor t) {
+    check_cuda(t, "t");
+    TORCH_CHECK(t.scalar_type() == at::kBFloat16 && t.is_contiguous() && t.dim() >= 1, "fp8: contiguous bf16 tensor");
+    return (reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) != 0 ? t.clone() : t;
+  };
+  m.def("fp8_cast_transpose", [fp8_cast, fp8_input](at::Tensor t, at::Tensor amax, const std::string& fmt, bool want_transpose, bool want_colsum) {
+    t = fp8_input(t);
+    c10::cuda::CUDAGuard guard(t.device());
+    return fp8_cast(t, amax, fmt, want_transpose, want_colsum);
+  }, py::arg("t"), py::arg("amax"), py::arg("fmt"), py::arg("want_transpose") = false, py::arg("want_colsum") = false);
+  m.def("fp8_quantize", [fp8_cast, fp8_input](at::Tensor t, const std::string& fmt, bool want_transpose, bool want_colsum) {
+    t = fp8_input(t);
+    c10::cuda::CUDAGuard guard(t.device());
+    at::Tensor amax = at::empty({1}, t.options().dtype(at::kFloat));
+    launch_fp8_amax(t.data_ptr(), (size_t)t.numel(), amax.data_ptr<float>(), cur_stream());
+    return fp8_cast(t, amax, fmt, want_transpose, want_colsum);
+  }, py::arg("t"), py::arg("fmt"), py::arg("want_transpose") = false, py::arg("want_colsum") = false);
+  // D[M,N] bf16 = epi(a_scale_inv * b_scale_inv * A[M,K] @ B[N,K]^T + bias): A e4m3 or e5m2, B e4m3, both K-major
+  m.def("gemm_fp8", [](at::Tensor a, at::Tensor b, at::Tensor a_scale_inv, at::Tensor b_scale_inv, c10::optional<at::Tensor> bias,
+                       int epilogue) {
+    check_cuda(a, "a"); check_cuda(b, "b");
+    TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn || a.scalar_type() == at::kFloat8_e5m2, "gemm_fp8: A must be float8_e4m3fn or float8_e5m2");
+    TORCH_CHECK(b.scalar_type() == at::kFloat8_e4m3fn, "gemm_fp8: B must be float8_e4m3fn");
+    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.is_contiguous() && b.is_contiguous() && a.size(1) == b.size(1),
+                "gemm_fp8: A [M,K], B [N,K], both K-major contiguous");
+    for (const at::Tensor* s : {&a_scale_inv, &b_scale_inv})
+      TORCH_CHECK(s->is_cuda() && s->scalar_type() == at::kFloat && s->numel() == 1, "gemm_fp8: scale factors are 1-element fp32 CUDA tensors");
+    c10::cuda::CUDAGuard guard(a.device());
+    const int M = (int)a.size(0), K = (int)a.size(1), N = (int)b.size(0);
+    TORCH_CHECK(K % 16 == 0, "gemm_fp8: K = ", K, " must be a multiple of 16 (row pitch of the 8-bit operands)");
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(a.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(b.data_ptr()) & 15) == 0,
+                "gemm_fp8: operands must be 16-byte aligned");
+    at::Tensor d = at::empty({M, N}, a.options().dtype(at::kBFloat16));
+    const void* bias_ptr = nullptr;
+    if (bias.has_value()) {
+      TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N && bias->is_contiguous(), "gemm_fp8: bias bf16 [N]");
+      bias_ptr = bias->data_ptr();
+    }
+    launch_gemm_fp8(a.data_ptr(), b.data_ptr(), d.data_ptr(), bias_ptr, a_scale_inv.data_ptr<float>(), b_scale_inv.data_ptr<float>(),
+                    M, N, K, a.scalar_type() == at::kFloat8_e5m2, epilogue, cur_stream());
+    return d;
+  }, py::arg("a"), py::arg("b"), py::arg("a_scale_inv"), py::arg("b_scale_inv"), py::arg("bias") = py::none(), py::arg("epilogue") = 0);
   m.def("gemm_supported", &gemm_shape_supported);
   m.def("set_gemm_cta_mode", &set_gemm_cta_mode);
   m.def("set_gemm_group_m", &set_gemm_group_m);

@@ -21,6 +21,11 @@ void launch_gemm_bf16(const void* a, const void* b, void* d, const void* bias, i
 void launch_gemm_nt_bf16(const void* a, const void* b, void* d, const void* bias, int M, int N, int K, int epilogue,
                          DType out_dtype, cudaStream_t stream);
 bool gemm_shape_supported(int M, int N, int K, bool a_mn, bool b_mn);
+// FP8: D[M,N] (bf16) = epi( a_scale_inv * b_scale_inv * sum_k A[m,k] * B[n,k] ), A stored [M,K] (e4m3, or e5m2 with
+// a_e5m2), B stored [N,K] e4m3 - both K-major, the only layout FP8 wgmma takes.  The scale factors are fp32 device scalars
+// (no host round trip).  K % 16 == 0 (16-byte row pitch).  Same epilogue codes as launch_gemm_bf16.
+void launch_gemm_fp8(const void* a, const void* b, void* d, const void* bias, const float* a_scale_inv, const float* b_scale_inv,
+                     int M, int N, int K, bool a_e5m2, int epilogue, cudaStream_t stream);
 
 // Persistent-tile rasterisation shared by the producer, issuer and epilogue roles (and mirrored on the host for
 // tests).  group_m <= 0: m-fastest over the whole problem (default).  group_m > 0: bands of `group_m` m-tiles

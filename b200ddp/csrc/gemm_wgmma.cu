@@ -14,6 +14,12 @@
 //   A "MN-major" : A stored [K, M] row-major   (wgrad: dy^T)
 //   B "K-major"  : B stored [N, K] row-major   (forward W)
 //   B "MN-major" : B stored [K, N] row-major   (dgrad W, wgrad x)
+//
+// FP8 variants (OP != 0): 8-bit operands, K-major only (the only layout FP8 wgmma accepts), 128-element k-blocks (still
+// 128 bytes per row, so the swizzle, the TMA boxes in bytes and the descriptor stepping are those of bf16) and k32
+// steps.  Each k-block's four k32 steps accumulate into a fresh register tile that is then added to an fp32 tile: FP8
+// wgmma keeps fewer accumulator bits than fp32, and promoting every 128 products bounds the loss at large K.  The
+// epilogue multiplies by the device-resident dequantisation factors 1/s_a * 1/s_b before bias / activation / store.
 #include "gemm.h"
 
 #include <cuda.h>
@@ -31,6 +37,7 @@ using namespace tc;
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;          // 64 bf16 = 128 bytes = one swizzle-128B row
 constexpr int UMMA_K = 16;
+constexpr int kOpBF16 = 0, kOpE4M3 = 1, kOpE5M2 = 2;   // operand types: bf16 x bf16, e4m3 x e4m3, e5m2 x e4m3
 constexpr int kNumEpilogueWarps = 4;
 constexpr int kNumThreads = 128 + kNumEpilogueWarps * 32;   // warp 0: TMA producer, warps 1..3 idle; warps 4..7: MMA + epilogue
 
@@ -46,6 +53,8 @@ struct GemmParams {
   float* col_stats;       // [2][stat_groups][N] per-32-row partial column sums / sums of squares of the stored output, or nullptr
   void* d;
   const __nv_bfloat16* bias;
+  const float* scale_a;   // FP8 only: device scalars 1/s_a, 1/s_b (dequantisation factors)
+  const float* scale_b;
 };
 
 // bias / activation on 32 consecutive accumulator columns starting at `col0`
@@ -207,12 +216,16 @@ struct SmemLayout {
 // pair tile).  Each CTA loads its own A tile and HALF of the B tile, multicast into both CTAs' shared memory, so every B
 // byte leaves L2 once per pair.  A stage may be refilled only when the consumers of BOTH CTAs are done with it: the empty
 // barriers count the arrivals of the local and the peer warpgroup.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS, bool PAIR>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS, bool PAIR, int OP = kOpBF16>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const __grid_constant__ CUtensorMap map_d, const GemmParams p) {
   using L = SmemLayout<BLOCK_N, A_MN, B_MN, TMA_ST>;
   constexpr int kStages = L::kStages;
+  constexpr bool kFP8 = OP != kOpBF16;
+  static_assert(!kFP8 || (!A_MN && !B_MN && !TMA_ST && !STATS && !PAIR && BLOCK_N == 64),
+                "FP8: K-major operands, direct epilogue, 128 x 64 tiles (partial + promoted accumulators fill the registers)");
+  constexpr int kBK = kFP8 ? 2 * BLOCK_K : BLOCK_K;            // elements per k-block: one 128-byte row either way
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* barrier_area = smem + kStages * L::kStageBytes;
@@ -229,7 +242,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   const int num_m_blocks = (p.M + kM - 1) / kM;
   const int num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
   const int num_tiles = num_m_blocks * num_n_blocks;
-  const int num_k_blocks = (p.K + BLOCK_K - 1) / BLOCK_K;
+  const int num_k_blocks = (p.K + kBK - 1) / kBK;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&map_a);
@@ -257,7 +270,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           uint8_t* sa = smem + stage * L::kStageBytes;
           uint8_t* sb = sa + L::kABytes;
           mbar_expect_tx(&full_bar[stage], L::kStageBytes);
-          const int k0 = kb * BLOCK_K;
+          const int k0 = kb * kBK;
           if constexpr (!A_MN) {
             tma_load_2d(&map_a, &full_bar[stage], sa, k0, m0);                    // box {64 k, 128 m}
           } else {
@@ -302,17 +315,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       const int m0 = mb * kM + (int)rank * BLOCK_M;
       const int n0 = nb * BLOCK_N;
       WgAcc<BLOCK_N> acc;
+      [[maybe_unused]] WgAcc<BLOCK_N> part;                    // FP8: this k-block's products before promotion
+      if constexpr (kFP8) {
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) { acc.h[0][i] = 0.f; acc.h[1][i] = 0.f; }
+      }
       for (int kb = 0; kb < num_k_blocks; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
         const uint32_t b_addr = a_addr + L::kABytes;
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
+        for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {            // 32 bytes of every row per step: k16 bf16 or k32 FP8
           const uint64_t da0 = make_smem_desc(a_addr + k * kStepA, kLboA, kSbo);
           const uint64_t da1 = make_smem_desc(a_addr + kHalfA + k * kStepA, kLboA, kSbo);
           const uint64_t db = make_smem_desc(b_addr + k * kStepB, kLboB, kSbo);
-          wgmma_tile<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da0, da1, db, (kb | k) != 0 ? 1u : 0u);
+          if constexpr (kFP8) wgmma_tile_fp8<BLOCK_N, OP == kOpE5M2 ? 1 : 0>(part, da0, da1, db, k != 0 ? 1u : 0u);
+          else wgmma_tile<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da0, da1, db, (kb | k) != 0 ? 1u : 0u);
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -322,6 +341,15 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           if constexpr (PAIR) mbar_arrive_cluster(&empty_bar[stage], rank ^ 1u);   // the peer multicasts into it too
         }
         if (++stage == kStages) { stage = 0; phase ^= 1; }
+        if constexpr (kFP8) {                                   // promote into the fp32 tile
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 2; ++i) { acc.h[0][i] += part.h[0][i]; acc.h[1][i] += part.h[1][i]; }
+        }
+      }
+      if constexpr (kFP8) {
+        const float deq = __ldg(p.scale_a) * __ldg(p.scale_b);  // both powers of two: exact
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) { acc.h[0][i] *= deq; acc.h[1][i] *= deq; }
       }
       wg_bar_sync();                                           // the previous tile's epilogue is done reading acc_smem
       acc_to_smem<BLOCK_N>(acc, acc_smem, L::kAccStride, threadIdx.x - 128);
@@ -358,22 +386,25 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 
 // ---------------- host side ------------------------------------------------------------------------
 struct MapKey {
-  const void* ptr; int rows, cols, box_rows, box_cols;
-  bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows && box_cols == o.box_cols; }
+  const void* ptr; int rows, cols, box_rows, box_cols, elem_bytes;
+  bool operator==(const MapKey& o) const {
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows && box_cols == o.box_cols && elem_bytes == o.elem_bytes;
+  }
 };
 struct MapKeyHash {
   size_t operator()(const MapKey& k) const {
     size_t h = std::hash<const void*>()(k.ptr);
-    for (int v : {k.rows, k.cols, k.box_rows, k.box_cols}) h = h * 1000003u ^ (size_t)v;
+    for (int v : {k.rows, k.cols, k.box_rows, k.box_cols, k.elem_bytes}) h = h * 1000003u ^ (size_t)v;
     return h;
   }
 };
 
-// 2-D row-major bf16 tensor [rows, cols]; box = [box_rows, box_cols] with box_cols * 2 == 128 bytes.
-CUtensorMap make_map(const void* ptr, int rows, int cols, int box_rows, int box_cols) {
+// 2-D row-major tensor [rows, cols] of bf16 (elem_bytes 2) or 8-bit (elem_bytes 1) elements; box = [box_rows, box_cols]
+// with box_cols * elem_bytes == 128 bytes.
+CUtensorMap make_map(const void* ptr, int rows, int cols, int box_rows, int box_cols, int elem_bytes = 2) {
   static std::mutex mu;
   static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
-  MapKey key{ptr, rows, cols, box_rows, box_cols};
+  MapKey key{ptr, rows, cols, box_rows, box_cols, elem_bytes};
   {
     std::lock_guard<std::mutex> g(mu);
     auto it = cache.find(key);
@@ -386,10 +417,11 @@ CUtensorMap make_map(const void* ptr, int rows, int cols, int box_rows, int box_
   if (!ctx_bound) { B200_CUDA_CHECK(cudaFree(nullptr)); ctx_bound = true; }
   CUtensorMap map;
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)cols * elem_bytes};
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t elem_strides[2] = {1, 1};
-  B200_DRV_CHECK(drv.TensorMapEncodeTiled(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box,
+  const CUtensorMapDataType dt = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  B200_DRV_CHECK(drv.TensorMapEncodeTiled(&map, dt, 2, const_cast<void*>(ptr), dims, strides, box,
                                           elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
   std::lock_guard<std::mutex> g(mu);
@@ -399,16 +431,19 @@ CUtensorMap make_map(const void* ptr, int rows, int cols, int box_rows, int box_
 }
 
 // TMA_ST: epilogue through shared memory + TMA store (bf16 output, N % 8 == 0); the D map's box is one warp slab.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS = false, bool PAIR = false>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS = false, bool PAIR = false, int OP = kOpBF16>
 void launch_variant(const void* a, const void* b, const GemmParams& p, cudaStream_t stream) {
   using L = SmemLayout<BLOCK_N, A_MN, B_MN, TMA_ST>;
   constexpr int kSmem = L::kTotal;
   static_assert(L::kStages >= 3 && kSmem <= 227 * 1024, "shared memory budget");
   // A: K-major stored [M,K] -> box {BLOCK_M rows, 64 cols};  MN-major stored [K,M] -> box {64 rows(k), 64 cols(m)}
-  CUtensorMap map_a = A_MN ? make_map(a, p.K, p.M, BLOCK_K, 64) : make_map(a, p.M, p.K, BLOCK_M, BLOCK_K);
-  CUtensorMap map_b = B_MN ? make_map(b, p.K, p.N, BLOCK_K, 64) : make_map(b, p.N, p.K, PAIR ? BLOCK_N / 2 : BLOCK_N, BLOCK_K);
+  // FP8: K-major boxes of 128 one-byte elements (the same 128 bytes per row)
+  constexpr int kEB = OP == kOpBF16 ? 2 : 1;
+  constexpr int kBK = 128 / kEB;
+  CUtensorMap map_a = A_MN ? make_map(a, p.K, p.M, BLOCK_K, 64) : make_map(a, p.M, p.K, BLOCK_M, kBK, kEB);
+  CUtensorMap map_b = B_MN ? make_map(b, p.K, p.N, BLOCK_K, 64) : make_map(b, p.N, p.K, PAIR ? BLOCK_N / 2 : BLOCK_N, kBK, kEB);
   CUtensorMap map_d = TMA_ST ? make_map(p.d, p.M, p.N, 32, 64) : map_a;       // unused by the direct epilogue
-  auto kernel = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, TMA_ST, STATS, PAIR>;
+  auto kernel = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, TMA_ST, STATS, PAIR, OP>;
   static std::atomic<unsigned long long> configured{0};
   ensure_max_dynamic_smem(kernel, kSmem, configured);
   if constexpr (PAIR) {
@@ -524,6 +559,29 @@ void launch_gemm_bf16(const void* a, const void* b, void* d, const void* bias, i
 void launch_gemm_nt_bf16(const void* a, const void* b, void* d, const void* bias, int M, int N, int K, int epilogue,
                          DType out_dtype, cudaStream_t stream) {
   launch_gemm_bf16(a, b, d, bias, M, N, K, false, false, epilogue, out_dtype, false, stream, nullptr);
+}
+
+void launch_gemm_fp8(const void* a, const void* b, void* d, const void* bias, const float* a_scale_inv, const float* b_scale_inv,
+                     int M, int N, int K, bool a_e5m2, int epilogue, cudaStream_t stream) {
+  if (M < 1 || N < 1 || K < 1) throw std::runtime_error("gemm_fp8: empty problem");
+  // TMA: the operands' row pitch (K one-byte elements) must be a multiple of 16 bytes
+  if (K % 16 != 0) throw std::runtime_error("gemm_fp8: K = " + std::to_string(K) + " is not a multiple of 16");
+  if (a_scale_inv == nullptr || b_scale_inv == nullptr) throw std::runtime_error("gemm_fp8: missing dequantisation factors");
+  if (epilogue < 0 || epilogue > 3) throw std::runtime_error("gemm_fp8: bad epilogue");
+  GemmParams p = {};
+  p.M = M; p.N = N; p.K = K;
+  p.epilogue = epilogue;
+  p.d = d;
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.scale_a = a_scale_inv;
+  p.scale_b = b_scale_inv;
+  if (g_gemm_group_m == -1) {
+    const char* e = getenv("B200DDP_GEMM_GROUP_M");
+    g_gemm_group_m = e ? atoi(e) : 0;
+  }
+  p.group_m = g_gemm_group_m > 0 ? g_gemm_group_m : 0;
+  if (a_e5m2) launch_variant<64, false, false, false, false, false, kOpE5M2>(a, b, p, stream);
+  else launch_variant<64, false, false, false, false, false, kOpE4M3>(a, b, p, stream);
 }
 
 }  // namespace b200

@@ -73,6 +73,16 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
                           int partial_rows, void* dgamma, void* dbeta, cudaStream_t s);
 int layernorm_partial_rows(int rows);
 
+// ---------------- FP8 quantisation, current per-tensor power-of-two scaling (fp8.cu) ------------------
+// amax[0] = max |x| over n bf16 elements (x 16-byte aligned); zeroes amax first, so the two launches are graph-capturable.
+void launch_fp8_amax(const void* x, size_t n, float* amax, cudaStream_t s);
+// x bf16 [rows, cols] (cols % 16 == 0) -> q [rows, cols] E4M3 (or E5M2), optionally qt = q^T [cols, rows] (rows % 16 == 0)
+// and colsum[cols] = fp32 column sums of x (colsum_partial: fp32 [fp8_colsum_parts(rows), cols] workspace).  The scale
+// s = 2^e comes from amax in device memory; *scale_inv = 1/s.
+void launch_fp8_cast_transpose(const void* x, int rows, int cols, const float* amax, bool e5m2, void* q, void* qt,
+                               float* colsum_partial, float* colsum, float* scale_inv, cudaStream_t s);
+int fp8_colsum_parts(int rows);
+
 // ---------------- small linears on CUDA cores (linear_small.cu) ------------------------------
 // y[M,N] = act(x[M,K] w[N,K]^T + b[N]) ; fp32, dims far below one tensor-core tile (FooModel).
 void launch_small_linear_fwd(const float* x, const float* w, const float* b, float* y, int M, int N, int K,

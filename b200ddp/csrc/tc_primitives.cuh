@@ -117,6 +117,59 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t desc_a, uint
       : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
+// D (+)= A * B, m64 x N x k32 with 8-bit operands -> fp32 in registers.  FP8 wgmma takes K-major operands only (no
+// transpose immediates).  A k32 step spans 32 bytes of a row, the same as a bf16 k16 step, so descriptors and their
+// stepping are those of the bf16 K-major case.  AType: 0 = e4m3, 1 = e5m2; B is always e4m3.
+#define B200_WGMMA_FP8_N64(NAME, ATYPE)                                                                                            \
+  __device__ __forceinline__ void NAME(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {                   \
+    asm volatile(                                                                                                                  \
+        "{\n\t.reg .pred p;\n\t"                                                                                                   \
+        "setp.ne.b32 p, %34, 0;\n\t"                                                                                               \
+        "wgmma.mma_async.sync.aligned.m64n64k32.f32." ATYPE ".e4m3 "                                                               \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, " \
+        "%26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"                                                                  \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),  \
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),     \
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),     \
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])                                                                      \
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));                                                                              \
+  }
+#define B200_WGMMA_FP8_N128(NAME, ATYPE)                                                                                           \
+  __device__ __forceinline__ void NAME(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {                   \
+    asm volatile(                                                                                                                  \
+        "{\n\t.reg .pred p;\n\t"                                                                                                   \
+        "setp.ne.b32 p, %66, 0;\n\t"                                                                                               \
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32." ATYPE ".e4m3 "                                                              \
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, " \
+        "%26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, "  \
+        "%50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"                          \
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),  \
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),     \
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),     \
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),     \
+          "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),     \
+          "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),     \
+          "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])      \
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));                                                                              \
+  }
+B200_WGMMA_FP8_N64(wgmma_n64_e4m3, "e4m3")
+B200_WGMMA_FP8_N64(wgmma_n64_e5m2, "e5m2")
+B200_WGMMA_FP8_N128(wgmma_n128_e4m3, "e4m3")
+B200_WGMMA_FP8_N128(wgmma_n128_e5m2, "e5m2")
+#undef B200_WGMMA_FP8_N64
+#undef B200_WGMMA_FP8_N128
+
+template <int AType>
+__device__ __forceinline__ void wgmma_fp8_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  if constexpr (AType == 0) wgmma_n64_e4m3(d, desc_a, desc_b, accumulate);
+  else wgmma_n64_e5m2(d, desc_a, desc_b, accumulate);
+}
+template <int AType>
+__device__ __forceinline__ void wgmma_fp8_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  if constexpr (AType == 0) wgmma_n128_e4m3(d, desc_a, desc_b, accumulate);
+  else wgmma_n128_e5m2(d, desc_a, desc_b, accumulate);
+}
+
 // A 128 x BN fp32 accumulator tile held by one warpgroup: rows [0, 64) in h[0], rows [64, 128) in h[1].  Thread t of the
 // warpgroup holds, per half, rows 16 * (t / 32) + (t % 32) / 4 (+ 8) and column pairs 8 j + 2 (t % 4) of every 8-column group.
 template <int BN>
@@ -134,6 +187,17 @@ __device__ __forceinline__ void wgmma_tile(WgAcc<BN>& acc, uint64_t da0, uint64_
   } else {
     wgmma_n128<TA, TB>(acc.h[0], da0, db, accumulate);
     wgmma_n128<TA, TB>(acc.h[1], da1, db, accumulate);
+  }
+}
+// acc (+)= A * B for one k32 step of 8-bit operands (both K-major)
+template <int BN, int AType>
+__device__ __forceinline__ void wgmma_tile_fp8(WgAcc<BN>& acc, uint64_t da0, uint64_t da1, uint64_t db, uint32_t accumulate) {
+  if constexpr (BN == 64) {
+    wgmma_fp8_n64<AType>(acc.h[0], da0, db, accumulate);
+    wgmma_fp8_n64<AType>(acc.h[1], da1, db, accumulate);
+  } else {
+    wgmma_fp8_n128<AType>(acc.h[0], da0, db, accumulate);
+    wgmma_fp8_n128<AType>(acc.h[1], da1, db, accumulate);
   }
 }
 

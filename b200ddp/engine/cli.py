@@ -63,6 +63,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--wire_dtype", type=str, default=None, choices=[None, "fp32", "bf16"])
     p.add_argument("--channels_last", action="store_true")
     p.add_argument("--cuda_graph", action="store_true", help="capture the whole optimizer step in a CUDA graph")
+    p.add_argument("--fp8", action="store_true",
+                   help="BERT encoder linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs --model bert-base, "
+                        "--fp16 and a GPU")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -118,10 +121,23 @@ def setup(args):
                                                                         transport=args.backend))
         args.n_gpu = 1 if have_cuda else 0
     args.device = device
+    check_fp8_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
     return log
+
+
+def check_fp8_args(args) -> None:
+    """``--fp8`` is a BERT feature on top of bf16 weights on a GPU: reject every other combination up front."""
+    if not getattr(args, "fp8", False):
+        return
+    if args.model != "bert-base":
+        raise ValueError(f"--fp8 covers the BERT encoder linears only; it needs --model bert-base (got --model {args.model})")
+    if not args.fp16:
+        raise ValueError("--fp8 needs --fp16: the FP8 GEMMs read bf16 activations and weights")
+    if getattr(args, "device", None) is None or args.device.type != "cuda":
+        raise ValueError("--fp8 needs a CUDA device (it runs on FP8 tensor cores); drop --no_cuda")
 
 
 def cleanup(args) -> None:
@@ -143,7 +159,7 @@ def main(argv=None) -> int:
     from .trainer import Trainer
     args = build_parser().parse_args(argv)
     setup(args)
-    model = build_model(args.model)
+    model = build_model(args.model, **({"fp8": True} if args.fp8 else {}))
     trainer = Trainer(args, model, log)
     trainer.train()
     if args.eval_at_end:

@@ -87,6 +87,9 @@ class Trainer:
             # scaling, ddp.py:174-180); here that is bf16 weights + fp32 masters, no loss scaling needed
             self.compute_dtype = torch.bfloat16
         model = model.to(self.device)
+        fp8_linears = sum(1 for m in model.modules() if getattr(m, "fp8", False) is True)
+        if fp8_linears:
+            log.info("FP8 linears on.", dict(linears=fp8_linears, formats="e4m3 x/W, e5m2 dy", scaling="per-tensor, power of two"))
         if self.compute_dtype != torch.float32:
             model = to_mixed_bf16(model)
         if getattr(args, "channels_last", False):

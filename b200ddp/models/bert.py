@@ -26,6 +26,7 @@ class BertConfig:
     eps: float = 1e-12
     dropout: float = 0.0
     pad_vocab_to: int = 1          # MLM head pads to 64 so logits rows keep the 16-byte pitch TMA needs
+    fp8: bool = False              # encoder linears (qkv, attn_out, ffn_in, ffn_out) on FP8 tensor cores; same parameters
 
     @property
     def padded_vocab(self) -> int:
@@ -58,11 +59,11 @@ class BertLayer(nn.Module):
         # Q, K and V projections are ONE stored [3*hidden, hidden] parameter (rows: query, key, value): forward, dgrad and
         # wgrad are one wgmma launch each and nothing is concatenated per step.  ``load_hf_state_dict`` fuses the stock
         # model's three tensors; ``split_qkv_state_dict`` gives them back.
-        self.qkv = Linear(c.hidden, 3 * c.hidden)
-        self.attn_out = Linear(c.hidden, c.hidden)
+        self.qkv = Linear(c.hidden, 3 * c.hidden, fp8=c.fp8)
+        self.attn_out = Linear(c.hidden, c.hidden, fp8=c.fp8)
         self.attn_norm = LayerNorm(c.hidden, eps=c.eps)
-        self.ffn_in = Linear(c.hidden, c.intermediate, activation="gelu")
-        self.ffn_out = Linear(c.intermediate, c.hidden)
+        self.ffn_in = Linear(c.hidden, c.intermediate, activation="gelu", fp8=c.fp8)
+        self.ffn_out = Linear(c.intermediate, c.hidden, fp8=c.fp8)
         self.ffn_norm = LayerNorm(c.hidden, eps=c.eps)
         self.dropout = nn.Dropout(c.dropout)
 
@@ -172,5 +173,9 @@ def split_qkv_state_dict(state: dict) -> dict:
     return out
 
 
-def bert_base(with_mlm_head: bool = True) -> nn.Module:
-    return BertForMaskedLM() if with_mlm_head else BertModel()
+def bert_base(with_mlm_head: bool = True, fp8: bool = False) -> nn.Module:
+    """BERT-base; ``fp8=True`` puts the 48 encoder linears on FP8 tensor cores (embeddings, MLM transform and the tied
+    decoder stay bf16).  The state dict is the same either way."""
+    if with_mlm_head:
+        return BertForMaskedLM(BertConfig(pad_vocab_to=64, fp8=fp8))
+    return BertModel(BertConfig(fp8=fp8))

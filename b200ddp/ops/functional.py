@@ -107,9 +107,147 @@ class _LinearSmall(torch.autograd.Function):
         return (dx if ctx.needs_input_grad[0] else None), dw, (db if ctx.has_bias else None), None
 
 
+# ------------------------------------------------------------------------------------------------
+# FP8 linear (csrc/fp8.cu, csrc/gemm_wgmma.cu): E4M3 x / W, E5M2 dy, current per-tensor power-of-two scales
+# ------------------------------------------------------------------------------------------------
+FP8_FORMATS = {"e4m3": (torch.float8_e4m3fn, 448.0), "e5m2": (torch.float8_e5m2, 57344.0)}
+
+
+def fp8_scale(amax: float, fmt: str) -> float:
+    """s = 2^e with e the largest integer such that amax * 2^e <= fmax, e clamped to [-126, 127]; amax = 0 gives 1.
+    The same rule as ``fp8_scale_exponent`` in csrc/fp8.cu, evaluated exactly on the mantissas."""
+    fmax = FP8_FORMATS[fmt][1]
+    if not (amax > 0.0) or not math.isfinite(amax):
+        return 1.0
+    ma, ea = math.frexp(amax)
+    mf, ef = math.frexp(fmax)
+    e = ef - ea - (1 if ma > mf else 0)
+    return math.ldexp(1.0, min(max(e, -126), 127))
+
+
+def fp8_quantize_reference(t: torch.Tensor, fmt: str):
+    """(q, s) on the CPU: q = (t.float() * s).to(float8) - bitwise what the CUDA quantiser writes."""
+    s = fp8_scale(float(t.detach().abs().max().float()) if t.numel() else 0.0, fmt)
+    return (t.detach().float() * s).to(FP8_FORMATS[fmt][0]), s
+
+
+def _fp8_round_trip(t: torch.Tensor, fmt: str) -> torch.Tensor:
+    """fp32 values of t after quantisation and exact dequantisation."""
+    q, s = fp8_quantize_reference(t, fmt)
+    return q.float() / s
+
+
+def _fp8_check(x2: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], need_transpose_x: bool) -> None:
+    M, K = x2.shape
+    N = weight.shape[0]
+    if x2.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16 or (bias is not None and bias.dtype != torch.bfloat16):
+        raise ValueError(f"fp8 linear on CUDA needs bf16 input, weight and bias, got {x2.dtype} x {weight.dtype} "
+                         f"(input {tuple(x2.shape)}, weight {tuple(weight.shape)})")
+    if K % 16 or N % 16:
+        raise ValueError(f"fp8 linear needs in_features and out_features divisible by 16, got weight {tuple(weight.shape)}")
+    if need_transpose_x and M % 16:
+        raise ValueError(f"fp8 linear backward needs the row count divisible by 16 (the weight gradient reduces over rows "
+                         f"of a transposed FP8 copy), got input {tuple(x2.shape)}")
+
+
+class _LinearFP8(torch.autograd.Function):
+    """FP8 linear: y = act(x W^T + b) with x, W quantised to E4M3 and dy to E5M2 (per-tensor power-of-two scales).
+    FP8 wgmma takes K-major operands only, so every quantisation writes the transposed copy the backward needs:
+    forward x8 [M,K] . W8 [N,K], dgrad dy8 [M,N] . W8^T [K,N], wgrad dy8^T [N,M] . x8^T [K,M].  The bias gradient comes
+    from the column sums of the dy quantisation pass.  Parameters and gradients stay bf16.
+    CPU body: the same recipe emulated exactly (same scales, a torch.float8 round trip, fp32 matmuls)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, activation, grad_enabled):
+        x2 = x.reshape(-1, x.shape[-1])
+        if not x2.is_contiguous():
+            x2 = x2.contiguous()
+        if bias is None and activation is not None:
+            raise ValueError("fused activation needs a bias (use bias=True)")
+        # transposed copies only where a backward will read them (no_grad inference needs none)
+        need_dx, need_dw = grad_enabled and ctx.needs_input_grad[0], grad_enabled and ctx.needs_input_grad[1]
+        ctx.activation = activation
+        ctx.has_bias = bias is not None
+        ctx.x_shape = x.shape
+        if x.is_cuda:
+            C = _C()
+            _fp8_check(x2, weight, bias, need_dw)
+            xq, xqt, xs, _ = C.fp8_quantize(x2, "e4m3", need_dw, False)
+            wq, wqt, ws, _ = C.fp8_quantize(weight.contiguous(), "e4m3", need_dx, False)
+            if activation == "gelu":
+                pre = C.gemm_fp8(xq, wq, xs, ws, bias, EPI_BIAS)
+                y = C.gelu_fwd(pre)
+            else:
+                pre = None
+                y = C.gemm_fp8(xq, wq, xs, ws, bias, _ACT_TO_EPI[activation] if bias is not None else EPI_NONE)
+                if activation == "relu":
+                    pre = y
+            ctx.save_for_backward(xqt, xs, wqt, ws, pre)
+        else:
+            xd = _fp8_round_trip(x2, "e4m3")
+            wd = _fp8_round_trip(weight, "e4m3")
+            acc = xd @ wd.t()
+            if bias is not None:
+                acc = acc + bias.float()
+            pre = acc.to(x.dtype)
+            if activation == "gelu":
+                y = F.gelu(pre.float()).to(x.dtype)
+            elif activation == "relu":
+                y = F.relu(pre)
+            else:
+                y = pre
+            ctx.save_for_backward(xd, wd, pre if activation is not None else None)
+            ctx.dtypes = (x.dtype, weight.dtype, bias.dtype if bias is not None else None)
+        return y.view(*x.shape[:-1], weight.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        dx = dw = db = None
+        if dy.is_cuda:
+            C = _C()
+            xqt, xs, wqt, ws, aux = ctx.saved_tensors
+            if ctx.activation == "relu":
+                dy2 = dy2 * (aux > 0).to(dy2.dtype)
+            elif ctx.activation == "gelu":
+                dy2 = C.gelu_bwd(dy2.contiguous(), aux)
+            if not dy2.is_contiguous():
+                dy2 = dy2.contiguous()
+            if dy2.shape[0] % 16:
+                raise ValueError(f"fp8 linear backward needs the row count divisible by 16, got gradient {tuple(dy2.shape)}")
+            need_db = ctx.has_bias and ctx.needs_input_grad[2]
+            dyq, dyqt, dys, colsum = C.fp8_quantize(dy2, "e5m2", ctx.needs_input_grad[1], need_db)
+            if ctx.needs_input_grad[0]:
+                dx = C.gemm_fp8(dyq, wqt, dys, ws, None, EPI_NONE).view(ctx.x_shape)       # [M,K], reduction over N
+            if ctx.needs_input_grad[1]:
+                dw = C.gemm_fp8(dyqt, xqt, dys, xs, None, EPI_NONE)                        # [N,K], reduction over M
+            if need_db:
+                db = colsum.to(dy.dtype)
+        else:
+            xd, wd, aux = ctx.saved_tensors
+            x_dtype, w_dtype, b_dtype = ctx.dtypes
+            if ctx.activation == "relu":
+                dy2 = dy2 * (aux > 0).to(dy2.dtype)
+            elif ctx.activation == "gelu":
+                p = aux.float()                                    # gelu'(p) = Phi(p) + p phi(p)
+                dgelu = 0.5 * (1.0 + torch.erf(p * math.sqrt(0.5))) + p * torch.exp(-0.5 * p * p) / math.sqrt(2.0 * math.pi)
+                dy2 = (dy2.float() * dgelu).to(dy.dtype)
+            dyd = _fp8_round_trip(dy2, "e5m2")
+            if ctx.needs_input_grad[0]:
+                dx = (dyd @ wd).to(x_dtype).view(ctx.x_shape)
+            if ctx.needs_input_grad[1]:
+                dw = (dyd.t() @ xd).to(w_dtype)
+            if ctx.has_bias and ctx.needs_input_grad[2]:
+                db = dy2.float().sum(0).to(b_dtype)
+        return dx, dw, db, None, None
+
+
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None,
-           activation: Optional[str] = None) -> torch.Tensor:
-    """y = act(x @ weight.T + bias), activation in {None, "relu", "gelu"}."""
+           activation: Optional[str] = None, fp8: bool = False) -> torch.Tensor:
+    """y = act(x @ weight.T + bias), activation in {None, "relu", "gelu"}.  ``fp8=True`` runs the three GEMMs on FP8
+    tensor cores (``_LinearFP8``); on CUDA it needs bf16 tensors and raises ``ValueError`` for anything else."""
+    if fp8:
+        return _LinearFP8.apply(x, weight, bias, activation, torch.is_grad_enabled())
     if x.is_cuda:
         N, K = weight.shape
         M = x.numel() // K

@@ -13,12 +13,17 @@ from . import functional as Fn
 
 
 class Linear(nn.Module):
-    """``nn.Linear`` replacement with an optional fused activation epilogue."""
+    """``nn.Linear`` replacement with an optional fused activation epilogue.  ``fp8=True`` runs forward, data gradient and
+    weight gradient on FP8 tensor cores (E4M3 activations / weights, E5M2 gradients, per-tensor power-of-two scales); the
+    parameters, their names and shapes are the same either way."""
 
     def __init__(self, in_features: int, out_features: int, bias: bool = True, activation: Optional[str] = None,
-                 device=None, dtype=None):
+                 device=None, dtype=None, fp8: bool = False):
         super().__init__()
+        if fp8 and (in_features % 16 or out_features % 16):
+            raise ValueError(f"fp8 Linear needs in_features and out_features divisible by 16, got {in_features} -> {out_features}")
         self.in_features, self.out_features, self.activation = in_features, out_features, activation
+        self.fp8 = bool(fp8)
         self.weight = nn.Parameter(torch.empty(out_features, in_features, device=device, dtype=dtype))
         self.bias = nn.Parameter(torch.empty(out_features, device=device, dtype=dtype)) if bias else None
         self.reset_parameters()
@@ -31,10 +36,11 @@ class Linear(nn.Module):
             nn.init.uniform_(self.bias, -bound, bound)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        return Fn.linear(x, self.weight, self.bias, self.activation)
+        return Fn.linear(x, self.weight, self.bias, self.activation, fp8=self.fp8)
 
     def extra_repr(self) -> str:
-        return f"in={self.in_features}, out={self.out_features}, bias={self.bias is not None}, act={self.activation}"
+        return (f"in={self.in_features}, out={self.out_features}, bias={self.bias is not None}, act={self.activation}"
+                + (", fp8=True" if self.fp8 else ""))
 
 
 class Conv2dTC(nn.Conv2d):
