@@ -1,0 +1,530 @@
+// Multi-head attention with a key-padding mask on the Hopper tensor cores (the BERT encoder's attention for right-padded
+// batches).  Head dim 64, softmax scale 1/8.
+//
+//   qkv  bf16 [B*S, 3*H*64]   the fused projection's output: column blocks query | key | value, head h at h*64 .. h*64+63
+//   o    bf16 [B*S, H*64]     written in the layout the output projection reads (no transpose)
+//   lse  fp32 [B, H, S]       natural-log row log-sum-exp of the scaled scores (-inf for a sequence of length 0)
+//
+// Key j of sequence b is visible iff j < seq_lens[b] (clamped to [0, S] here: the host cannot validate device lengths
+// without a synchronisation).  Every query row is computed, padded ones included, so every row equals softmax attention
+// over the visible keys; a sequence of length 0 gets zero output and zero gradients.
+//
+// Each kernel has one TMA producer warp (warp 0; warps 1-3 idle) and two consumer warpgroups (warps 4-7, 8-11) that own
+// 64 rows each.  All tiles are 64-row boxes of one 2-D tensor map over qkv (or dO), 128B-swizzled, so a head's 64
+// columns are exactly one swizzle row and the same shared-memory tile serves as a K-major operand (Q K^T) or an MN-major
+// one (P V).  P and dS never touch shared memory: the fp32 accumulator fragment packed to bf16x2 IS the register A
+// fragment of the next wgmma (tc::wgmma_n64_rs).
+//
+// Forward (flash attention): CTA = (query tile of 128, head, batch); K/V tiles of 128 keys stream through a 2-stage ring;
+// online softmax in fp32 registers; key tiles at or beyond the length are never loaded.
+// Backward, deterministic (no atomics; every output element has one writer):
+//   attn_bwd_dot  D = rowsum(dO * O)
+//   attn_bwd_dkdv CTA = (key tile of 128, head, batch), loops over all query tiles: S^T = K Q^T, P^T = exp(S^T - lse),
+//                 dV += P^T dO, dP^T = V dO^T, dS^T = P^T (dP^T - D), dK += dS^T Q.  Key tiles wholly beyond the length
+//                 only write zeros.
+//   attn_bwd_dq   CTA = (query tile of 128, head, batch), loops over the key tiles below the length: S, P, dP = dO V^T,
+//                 dS, dQ += dS K.
+// Recomputing P in both backward kernels costs two GEMMs more than accumulating dQ with atomics inside the dK/dV loop;
+// that is the price of bit-identical gradients on every run.
+#include <cuda.h>
+
+#include "common.h"
+#include "drv.h"
+#include "ops.h"
+#include "tc_primitives.cuh"
+
+namespace b200 {
+
+CUtensorMap conv_encode_map(const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box);   // conv_wgmma.cu
+
+namespace {
+using namespace tc;
+
+constexpr int kHd = 64;                        // head dim: 128 bytes, one swizzle row
+constexpr int kBoxRows = 64;
+constexpr int kBoxBytes = kBoxRows * kHd * 2;  // 8 KB
+constexpr int kThreads = 384;
+constexpr int kConsumerArrivals = 8;           // lane 0 of each consumer warp releases a ring stage
+constexpr float kScale = 0.125f;               // 1/sqrt(64)
+constexpr float kLog2e = 1.4426950408889634f;
+constexpr float kScaleLog2 = kScale * kLog2e;
+constexpr uint32_t kSbo = 1024;                // 8 rows x 128 B
+constexpr uint32_t kLboMN = kBoxRows * 128;    // MN-major: distance between 64-wide chunks (only one chunk is used)
+constexpr uint32_t kStepK = 32;                // K-major: 16 bf16 columns
+constexpr uint32_t kStepMN = 16 * 128;         // MN-major: 16 rows
+
+constexpr int kFwdStages = 2;
+constexpr int kFwdSmem = 1024 + 2 * kBoxBytes + kFwdStages * 4 * kBoxBytes + 256;   // Q 128 rows + ring of (K, V) 128 rows
+constexpr int kBwdStages = 4;
+constexpr int kBwdSmem = 1024 + 4 * kBoxBytes + kBwdStages * 2 * kBoxBytes + 256;   // fixed 2 x 128 rows + ring of 2 x 64 rows
+
+__device__ __forceinline__ int clamped_len(const int* lens, int b, int S) {
+  const int n = __ldg(lens + b);
+  return n < 0 ? 0 : (n > S ? S : n);
+}
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+__device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
+}
+__device__ __forceinline__ uint64_t desc_k(uint32_t addr) { return make_smem_desc(addr, 16, kSbo); }
+__device__ __forceinline__ uint64_t desc_mn(uint32_t addr) { return make_smem_desc(addr, kLboMN, kSbo); }
+
+// S (+)= A B^T over the 64-wide head dim (four k16 steps), both operands K-major 64-row tiles (B: 64 or 128 rows)
+__device__ __forceinline__ void mma_hd_n64(float (&acc)[32], uint32_t a, uint32_t b) {
+#pragma unroll
+  for (int k = 0; k < kHd / 16; ++k) wgmma_n64<0, 0>(acc, desc_k(a + k * kStepK), desc_k(b + k * kStepK), k != 0 ? 1u : 0u);
+}
+
+// Zero rows [row0, row0 + rows) of one head's 64 columns in a row-major bf16 matrix with `pitch` elements per row
+__device__ __forceinline__ void zero_rows(__nv_bfloat16* base, size_t pitch, size_t row0, int rows) {
+  for (int i = threadIdx.x; i < rows * 32; i += blockDim.x)
+    *reinterpret_cast<uint32_t*>(base + (row0 + (i >> 5)) * pitch + 2 * (i & 31)) = 0u;
+}
+
+// Stores one warpgroup's m64 x 64 fp32 fragment (times `scale`) as bf16: rows r0 / r0 + 8, column pairs 8 j + c0.
+__device__ __forceinline__ void store_frag(const float (&acc)[32], float scale0, float scale1, __nv_bfloat16* row0_ptr,
+                                           size_t pitch, int c0) {
+  __nv_bfloat16* row1_ptr = row0_ptr + 8 * pitch;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    *reinterpret_cast<uint32_t*>(row0_ptr + 8 * j + c0) = pack_bf16x2(acc[4 * j] * scale0, acc[4 * j + 1] * scale0);
+    *reinterpret_cast<uint32_t*>(row1_ptr + 8 * j + c0) = pack_bf16x2(acc[4 * j + 2] * scale1, acc[4 * j + 3] * scale1);
+  }
+}
+
+// ============================================== forward ==============================================================
+__global__ void __launch_bounds__(kThreads, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restrict__ seq_lens, int S, int H,
+                __nv_bfloat16* __restrict__ o, float* __restrict__ lse) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* sq = smem;                                           // 128 query rows
+  uint8_t* ring = sq + 2 * kBoxBytes;                           // stage: K 128 rows, V 128 rows
+  uint64_t* q_bar = reinterpret_cast<uint64_t*>(ring + kFwdStages * 4 * kBoxBytes);
+  uint64_t* full_bar = q_bar + 1;
+  uint64_t* empty_bar = full_bar + kFwdStages;
+
+  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int HD = H * kHd;
+  const int len = clamped_len(seq_lens, b, S);
+  const int n_kt = (len + 127) / 128;
+  const size_t seq_row = (size_t)b * S;
+  float* lse_bh = lse + ((size_t)b * H + h) * S;
+  if (n_kt == 0) {                                              // no visible key: zero output, empty log-sum-exp
+    zero_rows(o + h * kHd, HD, seq_row + qt * 128, 128);
+    if (threadIdx.x < 128) lse_bh[qt * 128 + threadIdx.x] = -INFINITY;
+    return;
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 1 && lane == 0) {
+    mbar_init(q_bar, 1);
+    for (int i = 0; i < kFwdStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerArrivals); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp == 0) {
+    if (lane == 0) {
+      tma_prefetch_desc(&map_qkv);
+      const int q_row = (int)seq_row + qt * 128;
+      mbar_expect_tx(q_bar, 2 * kBoxBytes);
+      tma_load_2d(&map_qkv, q_bar, sq, h * kHd, q_row);
+      tma_load_2d(&map_qkv, q_bar, sq + kBoxBytes, h * kHd, q_row + 64);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kt = 0; kt < n_kt; ++kt) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sk = ring + stage * 4 * kBoxBytes;
+        uint8_t* sv = sk + 2 * kBoxBytes;
+        const int k_row = (int)seq_row + kt * 128;
+        mbar_expect_tx(&full_bar[stage], 4 * kBoxBytes);
+        tma_load_2d(&map_qkv, &full_bar[stage], sk, HD + h * kHd, k_row);
+        tma_load_2d(&map_qkv, &full_bar[stage], sk + kBoxBytes, HD + h * kHd, k_row + 64);
+        tma_load_2d(&map_qkv, &full_bar[stage], sv, 2 * HD + h * kHd, k_row);
+        tma_load_2d(&map_qkv, &full_bar[stage], sv + kBoxBytes, 2 * HD + h * kHd, k_row + 64);
+        if (++stage == kFwdStages) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else if (warp >= 4) {
+    const int wg = (warp - 4) >> 2;                             // query rows [64 wg, 64 wg + 64) of the tile
+    const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);         // this thread's rows: r0 and r0 + 8 of the warpgroup's 64
+    const int c0 = 2 * (lane & 3);
+    const uint32_t q_addr = smem_u32(sq + wg * kBoxBytes);
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    mbar_wait(q_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int kt = 0; kt < n_kt; ++kt) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t k_addr = smem_u32(ring + stage * 4 * kBoxBytes);
+      const uint32_t v_addr = k_addr + 2 * kBoxBytes;
+      float s[64];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kHd / 16; ++k)
+        wgmma_n128<0, 0>(s, desc_k(q_addr + k * kStepK), desc_k(k_addr + k * kStepK), k != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      const int key0 = kt * 128;
+      if (key0 + 128 > len) {                                   // partial tile: hide keys at or beyond the length
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (key0 + 8 * j + c0 + e >= len) { s[4 * j + e] = -INFINITY; s[4 * j + 2 + e] = -INFINITY; }
+          }
+        }
+      }
+      // online softmax: the four threads of a quad share a row
+      float mx[2] = {m[0], m[1]};
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
+        mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
+      }
+      float alpha[2], mb[2], rs[2] = {0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+        mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+        alpha[i] = exp2f((m[i] - mx[i]) * kScaleLog2);          // key 0 is visible, so mx is finite; 0 on the first tile
+        m[i] = mx[i];
+        mb[i] = mx[i] * kScaleLog2;
+      }
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        s[4 * j] = exp2f(s[4 * j] * kScaleLog2 - mb[0]);
+        s[4 * j + 1] = exp2f(s[4 * j + 1] * kScaleLog2 - mb[0]);
+        s[4 * j + 2] = exp2f(s[4 * j + 2] * kScaleLog2 - mb[1]);
+        s[4 * j + 3] = exp2f(s[4 * j + 3] * kScaleLog2 - mb[1]);
+        rs[0] += s[4 * j] + s[4 * j + 1];
+        rs[1] += s[4 * j + 2] + s[4 * j + 3];
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) l[i] = l[i] * alpha[i] + rs[i];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        acc[4 * j] *= alpha[0]; acc[4 * j + 1] *= alpha[0];
+        acc[4 * j + 2] *= alpha[1]; acc[4 * j + 3] *= alpha[1];
+      }
+      // O += P V: P from registers (16 keys per k16 step), V MN-major
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint32_t a[4] = {pack_bf16x2(s[8 * kk], s[8 * kk + 1]), pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]),
+                               pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7])};
+        wgmma_n64_rs<1>(acc, a, desc_mn(v_addr + kk * kStepMN), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == kFwdStages) { stage = 0; phase ^= 1; }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+      l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+    }
+    const int row = qt * 128 + wg * 64 + r0;                    // position in the sequence
+    store_frag(acc, 1.f / l[0], 1.f / l[1], o + (seq_row + row) * HD + h * kHd, HD, c0);
+    if ((lane & 3) == 0) {
+      lse_bh[row] = m[0] * kScale + logf(l[0]);
+      lse_bh[row + 8] = m[1] * kScale + logf(l[1]);
+    }
+  }
+}
+
+// ============================================== backward =============================================================
+// D[b, h, s] = sum_d dO[b*S + s, h*64 + d] * O[b*S + s, h*64 + d]; eight threads per (row, head), 16 bytes each
+__global__ void attn_bwd_dot_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* __restrict__ out, int rows,
+                                    int S, int H, float* __restrict__ D) {
+  const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t item = gid >> 3;
+  const int part = (int)(gid & 7);
+  const bool live = item < (size_t)rows * H;
+  float acc = 0.f;
+  size_t row = 0;
+  int hh = 0;
+  if (live) {
+    row = item / H;
+    hh = (int)(item % H);
+    const size_t off = row * (size_t)H * kHd + hh * kHd + part * 8;
+    float a[8], c[8];
+    unpack8(*reinterpret_cast<const Bf16x8*>(dout + off), a);
+    unpack8(*reinterpret_cast<const Bf16x8*>(out + off), c);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc += a[i] * c[i];
+  }
+  acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+  if (live && part == 0) {
+    const size_t b = row / S, s = row % S;
+    D[(b * H + hh) * S + s] = acc;
+  }
+}
+
+// Shared layout of both backward kernels: two fixed 128-row tiles (loaded once), then a ring of two 64-row tiles.
+struct BwdSmem {
+  uint8_t* fixed0;      // 128 rows
+  uint8_t* fixed1;      // 128 rows
+  uint8_t* ring;        // stage: tile0 64 rows, tile1 64 rows
+  uint64_t* fixed_bar;
+  uint64_t* full_bar;
+  uint64_t* empty_bar;
+};
+__device__ __forceinline__ BwdSmem bwd_smem(uint8_t* raw) {
+  BwdSmem L;
+  L.fixed0 = align1024(raw);
+  L.fixed1 = L.fixed0 + 2 * kBoxBytes;
+  L.ring = L.fixed1 + 2 * kBoxBytes;
+  L.fixed_bar = reinterpret_cast<uint64_t*>(L.ring + kBwdStages * 2 * kBoxBytes);
+  L.full_bar = L.fixed_bar + 1;
+  L.empty_bar = L.full_bar + kBwdStages;
+  return L;
+}
+__device__ __forceinline__ void bwd_init_barriers(const BwdSmem& L) {
+  mbar_init(L.fixed_bar, 1);
+  for (int i = 0; i < kBwdStages; ++i) { mbar_init(&L.full_bar[i], 1); mbar_init(&L.empty_bar[i], kConsumerArrivals); }
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+// Producer: fixed tiles (map0 at column col0f, map1 at col1f, rows fixed_row .. + 127), then `n` ring stages of
+// (map0r at col0r, map1r at col1r, rows ring_row0 + 64 i .. + 63).
+__device__ __forceinline__ void bwd_produce(const BwdSmem& L, const CUtensorMap* map0, int col0f, const CUtensorMap* map1, int col1f,
+                                            int fixed_row, const CUtensorMap* map0r, int col0r, const CUtensorMap* map1r, int col1r,
+                                            int ring_row0, int n) {
+  mbar_expect_tx(L.fixed_bar, 4 * kBoxBytes);
+  tma_load_2d(map0, L.fixed_bar, L.fixed0, col0f, fixed_row);
+  tma_load_2d(map0, L.fixed_bar, L.fixed0 + kBoxBytes, col0f, fixed_row + 64);
+  tma_load_2d(map1, L.fixed_bar, L.fixed1, col1f, fixed_row);
+  tma_load_2d(map1, L.fixed_bar, L.fixed1 + kBoxBytes, col1f, fixed_row + 64);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int i = 0; i < n; ++i) {
+    mbar_wait(&L.empty_bar[stage], phase ^ 1);
+    uint8_t* t0 = L.ring + stage * 2 * kBoxBytes;
+    mbar_expect_tx(&L.full_bar[stage], 2 * kBoxBytes);
+    tma_load_2d(map0r, &L.full_bar[stage], t0, col0r, ring_row0 + 64 * i);
+    tma_load_2d(map1r, &L.full_bar[stage], t0 + kBoxBytes, col1r, ring_row0 + 64 * i);
+    if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+  }
+}
+
+// dK, dV for one tile of 128 keys.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries, all S / 64 of them.
+__global__ void __launch_bounds__(kThreads, 1)
+attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
+                     const int* __restrict__ seq_lens, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
+                     __nv_bfloat16* __restrict__ dqkv) {
+  extern __shared__ uint8_t smem_raw[];
+  const BwdSmem L = bwd_smem(smem_raw);
+  const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int HD = H * kHd;
+  const size_t pitch = (size_t)3 * HD;
+  const int len = clamped_len(seq_lens, b, S);
+  const size_t seq_row = (size_t)b * S;
+  if (kt * 128 >= len) {                                        // every key of the tile is hidden: no gradient
+    zero_rows(dqkv + HD + h * kHd, pitch, seq_row + kt * 128, 128);
+    zero_rows(dqkv + 2 * HD + h * kHd, pitch, seq_row + kt * 128, 128);
+    return;
+  }
+  const int n_qt = S / 64;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 1 && lane == 0) bwd_init_barriers(L);
+  __syncthreads();
+
+  if (warp == 0) {
+    if (lane == 0) {
+      tma_prefetch_desc(&map_qkv);
+      tma_prefetch_desc(&map_do);
+      bwd_produce(L, &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row + kt * 128,
+                  &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row, n_qt);
+    }
+  } else if (warp >= 4) {
+    const int wg = (warp - 4) >> 2;                             // keys [64 wg, 64 wg + 64) of the tile
+    const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+    const int key = kt * 128 + wg * 64 + r0;
+    const bool vis0 = key < len, vis1 = key + 8 < len;
+    const uint32_t k_addr = smem_u32(L.fixed0 + wg * kBoxBytes), v_addr = smem_u32(L.fixed1 + wg * kBoxBytes);
+    const float* lse_bh = lse + ((size_t)b * H + h) * S;
+    const float* D_bh = Dsum + ((size_t)b * H + h) * S;
+    float dv[32], dk[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+    mbar_wait(L.fixed_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int qt = 0; qt < n_qt; ++qt) {
+      mbar_wait(&L.full_bar[stage], phase);
+      const uint32_t q_addr = smem_u32(L.ring + stage * 2 * kBoxBytes), do_addr = q_addr + kBoxBytes;
+      float st[32], dpt[32];
+      wgmma_fence();
+      mma_hd_n64(st, k_addr, q_addr);                           // S^T = K Q^T     [keys, queries]
+      mma_hd_n64(dpt, v_addr, do_addr);                         // dP^T = V dO^T
+      wgmma_commit();
+      wgmma_wait<0>();
+      uint32_t pa[16], dsa[16];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {                             // query columns 8 j + c0, + 1
+        const int q = qt * 64 + 8 * j + c0;
+        const float2 lq = *reinterpret_cast<const float2*>(lse_bh + q);
+        const float2 dq = *reinterpret_cast<const float2*>(D_bh + q);
+        const float l0 = lq.x * kLog2e, l1 = lq.y * kLog2e;
+        const float p00 = vis0 ? exp2f(st[4 * j] * kScaleLog2 - l0) : 0.f;
+        const float p01 = vis0 ? exp2f(st[4 * j + 1] * kScaleLog2 - l1) : 0.f;
+        const float p10 = vis1 ? exp2f(st[4 * j + 2] * kScaleLog2 - l0) : 0.f;
+        const float p11 = vis1 ? exp2f(st[4 * j + 3] * kScaleLog2 - l1) : 0.f;
+        pa[2 * j] = pack_bf16x2(p00, p01);
+        pa[2 * j + 1] = pack_bf16x2(p10, p11);
+        dsa[2 * j] = pack_bf16x2(p00 * (dpt[4 * j] - dq.x), p01 * (dpt[4 * j + 1] - dq.y));
+        dsa[2 * j + 1] = pack_bf16x2(p10 * (dpt[4 * j + 2] - dq.x), p11 * (dpt[4 * j + 3] - dq.y));
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_n64_rs<1>(dv, pa + 4 * kk, desc_mn(do_addr + kk * kStepMN), 1u);   // dV += P^T dO
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_n64_rs<1>(dk, dsa + 4 * kk, desc_mn(q_addr + kk * kStepMN), 1u);  // dK += dS^T Q
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&L.empty_bar[stage]);
+      if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+    }
+    __nv_bfloat16* krow = dqkv + (seq_row + key) * pitch + h * kHd;
+    store_frag(dk, kScale, kScale, krow + HD, pitch, c0);
+    store_frag(dv, 1.f, 1.f, krow + 2 * HD, pitch, c0);
+  }
+}
+
+// dQ for one tile of 128 queries.  Fixed: Q, dO.  Ring: (K, V) tiles of 64 keys below the length.
+__global__ void __launch_bounds__(kThreads, 1)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
+                   const int* __restrict__ seq_lens, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
+                   __nv_bfloat16* __restrict__ dqkv) {
+  extern __shared__ uint8_t smem_raw[];
+  const BwdSmem L = bwd_smem(smem_raw);
+  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int HD = H * kHd;
+  const size_t pitch = (size_t)3 * HD;
+  const int len = clamped_len(seq_lens, b, S);
+  const size_t seq_row = (size_t)b * S;
+  if (len == 0) {
+    zero_rows(dqkv + h * kHd, pitch, seq_row + qt * 128, 128);
+    return;
+  }
+  const int n_kt = (len + 63) / 64;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 1 && lane == 0) bwd_init_barriers(L);
+  __syncthreads();
+
+  if (warp == 0) {
+    if (lane == 0) {
+      tma_prefetch_desc(&map_qkv);
+      tma_prefetch_desc(&map_do);
+      bwd_produce(L, &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + qt * 128,
+                  &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row, n_kt);
+    }
+  } else if (warp >= 4) {
+    const int wg = (warp - 4) >> 2;
+    const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+    const int row = qt * 128 + wg * 64 + r0;
+    const uint32_t q_addr = smem_u32(L.fixed0 + wg * kBoxBytes), do_addr = smem_u32(L.fixed1 + wg * kBoxBytes);
+    const size_t bh = ((size_t)b * H + h) * S;
+    const float l0 = lse[bh + row] * kLog2e, l1 = lse[bh + row + 8] * kLog2e;
+    const float d0 = Dsum[bh + row], d1 = Dsum[bh + row + 8];
+    float dq[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+    mbar_wait(L.fixed_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int kt = 0; kt < n_kt; ++kt) {
+      mbar_wait(&L.full_bar[stage], phase);
+      const uint32_t k_addr = smem_u32(L.ring + stage * 2 * kBoxBytes), v_addr = k_addr + kBoxBytes;
+      float s[32], dp[32];
+      wgmma_fence();
+      mma_hd_n64(s, q_addr, k_addr);                            // S = Q K^T
+      mma_hd_n64(dp, do_addr, v_addr);                          // dP = dO V^T
+      wgmma_commit();
+      wgmma_wait<0>();
+      uint32_t dsa[16];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int k0 = kt * 64 + 8 * j + c0;
+        const bool v0 = k0 < len, v1 = k0 + 1 < len;
+        const float p00 = v0 ? exp2f(s[4 * j] * kScaleLog2 - l0) : 0.f;
+        const float p01 = v1 ? exp2f(s[4 * j + 1] * kScaleLog2 - l0) : 0.f;
+        const float p10 = v0 ? exp2f(s[4 * j + 2] * kScaleLog2 - l1) : 0.f;
+        const float p11 = v1 ? exp2f(s[4 * j + 3] * kScaleLog2 - l1) : 0.f;
+        dsa[2 * j] = pack_bf16x2(p00 * (dp[4 * j] - d0), p01 * (dp[4 * j + 1] - d0));
+        dsa[2 * j + 1] = pack_bf16x2(p10 * (dp[4 * j + 2] - d1), p11 * (dp[4 * j + 3] - d1));
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_n64_rs<1>(dq, dsa + 4 * kk, desc_mn(k_addr + kk * kStepMN), 1u);  // dQ += dS K
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&L.empty_bar[stage]);
+      if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+    }
+    store_frag(dq, kScale, kScale, dqkv + (seq_row + row) * pitch + h * kHd, pitch, c0);
+  }
+}
+
+CUtensorMap rows_map(const void* ptr, int rows, int cols) {
+  const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows};
+  const uint64_t strides[1] = {(uint64_t)cols * 2};
+  const uint32_t box[2] = {(uint32_t)kHd, (uint32_t)kBoxRows};
+  return conv_encode_map(ptr, 2, dims, strides, box);
+}
+
+void check_shape(const char* who, int B, int S, int heads) {
+  if (B < 1 || heads < 1 || S < 128 || S % 128 != 0)
+    throw std::runtime_error(std::string(who) + ": needs B >= 1, heads >= 1 and S a positive multiple of 128 (got B=" +
+                             std::to_string(B) + ", S=" + std::to_string(S) + ", heads=" + std::to_string(heads) + ")");
+  if (B > 65535 || (long long)B * S * 3 * heads * kHd >= (1ll << 31))
+    throw std::runtime_error(std::string(who) + ": problem too large");
+}
+
+}  // namespace
+
+void launch_attention_fwd(const void* qkv, const int* seq_lens, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
+  check_shape("attention_fwd", B, S, heads);
+  const CUtensorMap map_qkv = rows_map(qkv, B * S, 3 * heads * kHd);
+  static std::atomic<unsigned long long> configured{0};
+  ensure_max_dynamic_smem(attn_fwd_kernel, kFwdSmem, configured);
+  attn_fwd_kernel<<<dim3(S / 128, heads, B), kThreads, kFwdSmem, s>>>(map_qkv, seq_lens, S, heads,
+                                                                      reinterpret_cast<__nv_bfloat16*>(o), lse);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void launch_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* seq_lens, int B, int S,
+                          int heads, float* dsum, void* dqkv, cudaStream_t s) {
+  check_shape("attention_bwd", B, S, heads);
+  const int rows = B * S;
+  const long long items = (long long)rows * heads * 8;
+  attn_bwd_dot_kernel<<<ceil_div(items, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dout),
+                                                           reinterpret_cast<const __nv_bfloat16*>(o), rows, S, heads, dsum);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  const CUtensorMap map_qkv = rows_map(qkv, rows, 3 * heads * kHd);
+  const CUtensorMap map_do = rows_map(dout, rows, heads * kHd);
+  auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
+  static std::atomic<unsigned long long> configured_dkdv{0}, configured_dq{0};
+  ensure_max_dynamic_smem(attn_bwd_dkdv_kernel, kBwdSmem, configured_dkdv);
+  ensure_max_dynamic_smem(attn_bwd_dq_kernel, kBwdSmem, configured_dq);
+  attn_bwd_dkdv_kernel<<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, seq_lens, S, heads, lse, dsum, dq);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  attn_bwd_dq_kernel<<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, seq_lens, S, heads, lse, dsum, dq);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+}  // namespace b200

@@ -83,6 +83,15 @@ void launch_fp8_cast_transpose(const void* x, int rows, int cols, const float* a
                                float* colsum_partial, float* colsum, float* scale_inv, cudaStream_t s);
 int fp8_colsum_parts(int rows);
 
+// ---------------- key-padding attention on wgmma, head dim 64 (attention.cu) ------------------------
+// qkv bf16 [B*S, 3*heads*64] (16-byte aligned), seq_lens int32 [B] on the device (clamped to [0, S]), S % 128 == 0.
+// o bf16 [B*S, heads*64]; lse fp32 [B, heads, S], natural log (-inf where the length is 0).
+void launch_attention_fwd(const void* qkv, const int* seq_lens, int B, int S, int heads, void* o, float* lse, cudaStream_t s);
+// dout, o bf16 [B*S, heads*64] (16-byte aligned); dsum fp32 [B, heads, S] workspace; dqkv bf16 [B*S, 3*heads*64], every
+// element written.  Three launches: rowsum(dO * O), dK / dV, dQ.  Deterministic.
+void launch_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* seq_lens, int B, int S,
+                          int heads, float* dsum, void* dqkv, cudaStream_t s);
+
 // ---------------- small linears on CUDA cores (linear_small.cu) ------------------------------
 // y[M,N] = act(x[M,K] w[N,K]^T + b[N]) ; fp32, dims far below one tensor-core tile (FooModel).
 void launch_small_linear_fwd(const float* x, const float* w, const float* b, float* y, int M, int N, int K,

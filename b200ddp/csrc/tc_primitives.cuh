@@ -117,6 +117,22 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t desc_a, uint
       : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
+// D (+)= A[registers] * B[smem desc], m64 x 64 x k16, bf16 x bf16 -> fp32.  A is four .b32 registers of bf16x2 per thread:
+// rows 16 * warp + lane / 4 (a0, a2) and + 8 (a1, a3), columns 2 * (lane % 4) (a0, a1) and + 8 (a2, a3).  That is the fp32
+// accumulator fragment of an m64nN tile, 16 columns of it packed pairwise, so the output of one wgmma feeds the next
+// without leaving registers.  TB: 1 = B is MN-major.
+template <int TB>
+__device__ __forceinline__ void wgmma_n64_rs(float (&d)[32], const uint32_t* a, uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate), "n"(TB));
+}
+
 // D (+)= A * B, m64 x N x k32 with 8-bit operands -> fp32 in registers.  FP8 wgmma takes K-major operands only (no
 // transpose immediates).  A k32 step spans 32 bytes of a row, the same as a bf16 k16 step, so descriptors and their
 // stepping are those of the bf16 K-major case.  AType: 0 = e4m3, 1 = e5m2; B is always e4m3.

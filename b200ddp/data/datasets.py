@@ -69,15 +69,35 @@ class SyntheticImageNet(Dataset):
 
 
 class SyntheticTokens(Dataset):
-    """Token ids [seq] + MLM labels [seq] (-100 = not predicted) for the BERT config."""
+    """Token ids [seq] + MLM labels [seq] (-100 = not predicted) for the BERT config.
 
-    def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 30522, mask_prob: float = 0.15, seed: int = 1234):
+    ``min_len < seq_len`` gives right-padded rows: each row's length is uniform in [min_len, seq_len] (seeded), its
+    prefix holds tokens from [1, vocab) and the tail is ``PAD_ID`` labelled -100.  ``lengths`` then holds the lengths and
+    ``pad_token_id`` is ``PAD_ID``; without padding both are None and the tensors are those of fixed-length rows."""
+
+    PAD_ID = 0
+
+    def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 30522, mask_prob: float = 0.15, seed: int = 1234,
+                 min_len: int | None = None):
+        if min_len is not None and not 1 <= min_len <= seq_len:
+            raise ValueError(f"SyntheticTokens: min_len must lie in [1, seq_len = {seq_len}], got {min_len}")
         g = torch.Generator().manual_seed(seed)
         self.samples = int(samples)
-        self.X = torch.randint(0, vocab, (self.samples, seq_len), generator=g)
+        self.lengths = None
+        self.pad_token_id = None
+        if min_len is None or min_len == seq_len:
+            self.X = torch.randint(0, vocab, (self.samples, seq_len), generator=g)
+        else:
+            self.lengths = torch.randint(min_len, seq_len + 1, (self.samples,), generator=g)
+            self.pad_token_id = self.PAD_ID
+            self.X = torch.randint(1, vocab, (self.samples, seq_len), generator=g)
         labels = torch.randint(0, vocab, (self.samples, seq_len), generator=g)
         masked = torch.rand(self.samples, seq_len, generator=g) < mask_prob
         self.Y = torch.where(masked, labels, torch.full_like(labels, -100))
+        if self.lengths is not None:
+            pad = torch.arange(seq_len)[None, :] >= self.lengths[:, None]
+            self.X.masked_fill_(pad, self.PAD_ID)
+            self.Y.masked_fill_(pad, -100)
 
     def __len__(self) -> int:
         return self.samples

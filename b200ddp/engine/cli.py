@@ -66,6 +66,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--fp8", action="store_true",
                    help="BERT encoder linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs --model bert-base, "
                         "--fp16 and a GPU")
+    p.add_argument("--min_seq_len", type=int, default=None,
+                   help="BERT on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded keys are "
+                        "hidden from attention (native key-padding kernel on the GPU; needs --fp16 and --seq_len %% 128 == 0 "
+                        "there).  Default: fixed-length rows")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -122,6 +126,7 @@ def setup(args):
         args.n_gpu = 1 if have_cuda else 0
     args.device = device
     check_fp8_args(args)
+    check_min_seq_len_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -138,6 +143,29 @@ def check_fp8_args(args) -> None:
         raise ValueError("--fp8 needs --fp16: the FP8 GEMMs read bf16 activations and weights")
     if getattr(args, "device", None) is None or args.device.type != "cuda":
         raise ValueError("--fp8 needs a CUDA device (it runs on FP8 tensor cores); drop --no_cuda")
+
+
+def check_min_seq_len_args(args) -> None:
+    """``--min_seq_len`` pads BERT rows; on the GPU their attention runs on the bf16 key-padding kernel (head dim 64,
+    sequence length a multiple of 128): reject every other combination up front."""
+    n = getattr(args, "min_seq_len", None)
+    if n is None:
+        return
+    if args.model != "bert-base":
+        raise ValueError(f"--min_seq_len pads BERT token rows; it needs --model bert-base (got --model {args.model})")
+    if not 1 <= n <= args.seq_len:
+        raise ValueError(f"--min_seq_len must lie in [1, --seq_len = {args.seq_len}], got {n}")
+    if getattr(args, "device", None) is not None and args.device.type == "cuda":
+        if not args.fp16:
+            raise ValueError("--min_seq_len on a GPU needs --fp16: the key-padding attention kernel reads bf16 activations")
+        if args.seq_len % 128:
+            raise ValueError(f"--min_seq_len on a GPU needs --seq_len to be a multiple of 128 (got {args.seq_len})")
+
+
+def padding_on(args) -> bool:
+    """Rows are padded (and the model must hide padded keys) when some row can be shorter than --seq_len."""
+    n = getattr(args, "min_seq_len", None)
+    return n is not None and n < args.seq_len
 
 
 def cleanup(args) -> None:
@@ -159,7 +187,11 @@ def main(argv=None) -> int:
     from .trainer import Trainer
     args = build_parser().parse_args(argv)
     setup(args)
-    model = build_model(args.model, **({"fp8": True} if args.fp8 else {}))
+    kwargs = {"fp8": True} if args.fp8 else {}
+    if padding_on(args):
+        from ..data import SyntheticTokens
+        kwargs["pad_token_id"] = SyntheticTokens.PAD_ID
+    model = build_model(args.model, **kwargs)
     trainer = Trainer(args, model, log)
     trainer.train()
     if args.eval_at_end:

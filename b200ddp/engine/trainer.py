@@ -52,7 +52,8 @@ def build_dataset(args):
         dense = loss_kind(args) == "mse"
         return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
     if name.startswith("bert"):
-        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)))
+        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)),
+                               min_len=getattr(args, "min_seq_len", None))
     raise ValueError(f"no default dataset for model {name!r}")
 
 
@@ -103,6 +104,7 @@ class Trainer:
 
         # ---- data ---------------------------------------------------------------------------------
         self.dataset = dataset if dataset is not None else build_dataset(args)
+        self._check_padding(model)
         # one seedable, skippable sampler in every mode (single process = 1 replica), so mid-epoch resume replays nothing
         if self.distributed:
             self.sampler = ShardedSampler(self.dataset, seed=getattr(args, "sampler_seed", 0))
@@ -155,6 +157,22 @@ class Trainer:
         self.last_throughput = None
 
     # ------------------------------------------------------------------------------------------
+    def _check_padding(self, model: torch.nn.Module) -> None:
+        """A right-padded dataset needs a model that derives the lengths from the pad id (``BertConfig.pad_token_id``);
+        otherwise padded keys would be attended to without any error."""
+        pad_id = getattr(self.dataset, "pad_token_id", None)
+        lengths = getattr(self.dataset, "lengths", None)
+        if pad_id is None or lengths is None:
+            return
+        model_pads = {getattr(m.config, "pad_token_id", None) for m in model.modules() if hasattr(m, "config")}
+        if pad_id not in model_pads:
+            raise ValueError(f"the dataset pads its rows with token {pad_id}, but the model derives no sequence lengths from "
+                             f"it (model pad_token_id: {sorted(model_pads - {None}) or None}); build it with pad_token_id={pad_id}")
+        seq_len = self.dataset.X.shape[1]
+        self.log.info("Padded sequences.", dict(min_len=int(lengths.min()), max_len=int(lengths.max()),
+                                                mean_len=round(float(lengths.float().mean()), 1),
+                                                padding_fraction=round(1.0 - float(lengths.float().mean()) / seq_len, 4)))
+
     def _build_optimizer(self, inner: torch.nn.Module):
         args = self.args
         lr, wd = getattr(args, "lr", 1e-3), getattr(args, "weight_decay", 0.0)

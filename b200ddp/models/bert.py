@@ -1,7 +1,8 @@
 """BERT-base encoder + MLM head for the "BERT-base DDP bf16, seq 512" config.
 Every linear is a ``b200ddp.ops.Linear`` (wgmma GEMM with bias / bias+GELU epilogues), every
-LayerNorm the hand-written kernel, the loss the fused cross-entropy; attention uses torch's SDPA
-(library flash attention - not a named hot op).  109.5 M encoder parameters as in the stock model
+LayerNorm the hand-written kernel, the loss the fused cross-entropy.  Attention on fixed-length rows uses torch's SDPA
+(library flash attention); with ``BertConfig.pad_token_id`` set, right-padded rows run on the native key-padding
+attention kernel (``ops.attention``), which reads Q / K / V straight out of the fused projection.  109.5 M encoder parameters as in the stock model
 (199 tensors in the stock naming; 151 here because Q / K / V are one stored parameter) when built with ``with_mlm_head=False``."""
 from __future__ import annotations
 
@@ -11,7 +12,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops import LayerNorm, Linear
+from ..ops import LayerNorm, Linear, attention
 
 
 @dataclass
@@ -27,6 +28,7 @@ class BertConfig:
     dropout: float = 0.0
     pad_vocab_to: int = 1          # MLM head pads to 64 so logits rows keep the 16-byte pitch TMA needs
     fp8: bool = False              # encoder linears (qkv, attn_out, ffn_in, ffn_out) on FP8 tensor cores; same parameters
+    pad_token_id: int | None = None  # right-padded input: lengths = non-pad count per row, padded keys hidden (ops.attention)
 
     @property
     def padded_vocab(self) -> int:
@@ -67,7 +69,7 @@ class BertLayer(nn.Module):
         self.ffn_norm = LayerNorm(c.hidden, eps=c.eps)
         self.dropout = nn.Dropout(c.dropout)
 
-    def forward(self, x, attn_mask=None):
+    def forward(self, x, attn_mask=None, seq_lens=None):
         B, S, H = x.shape
         hd = H // self.heads
 
@@ -75,9 +77,12 @@ class BertLayer(nn.Module):
             return t.view(B, S, self.heads, hd).transpose(1, 2)
 
         qkv = self.qkv(x)
-        q, k, v = (split(t) for t in qkv.split(H, dim=-1))
-        a = F.scaled_dot_product_attention(q, k, v, attn_mask=attn_mask)
-        a = a.transpose(1, 2).reshape(B, S, H)
+        if seq_lens is not None:
+            a = attention(qkv, seq_lens, self.heads)       # [B, S, H], the layout attn_out reads
+        else:
+            q, k, v = (split(t) for t in qkv.split(H, dim=-1))
+            a = F.scaled_dot_product_attention(q, k, v, attn_mask=attn_mask)
+            a = a.transpose(1, 2).reshape(B, S, H)
         x = self.attn_norm(x + self.dropout(self.attn_out(a)))
         return self.ffn_norm(x + self.dropout(self.ffn_out(self.ffn_in(x))))
 
@@ -99,9 +104,17 @@ class BertModel(nn.Module):
                 nn.init.zeros_(m.bias)
 
     def forward(self, input_ids, token_type_ids=None, attn_mask=None):
+        seq_lens = None
+        pad = self.config.pad_token_id
+        if pad is not None:
+            if attn_mask is not None:
+                raise ValueError("BertModel: pass either attn_mask or a config with pad_token_id, not both "
+                                 "(with pad_token_id the padding mask comes from input_ids)")
+            # right padding: the length is the non-pad count; computed on the device, so no host synchronisation
+            seq_lens = (input_ids != pad).sum(1, dtype=torch.int32)
         x = self.embeddings(input_ids, token_type_ids)
         for layer in self.encoder:
-            x = layer(x, attn_mask)
+            x = layer(x, attn_mask, seq_lens)
         return x
 
 
@@ -173,9 +186,10 @@ def split_qkv_state_dict(state: dict) -> dict:
     return out
 
 
-def bert_base(with_mlm_head: bool = True, fp8: bool = False) -> nn.Module:
+def bert_base(with_mlm_head: bool = True, fp8: bool = False, pad_token_id: int | None = None) -> nn.Module:
     """BERT-base; ``fp8=True`` puts the 48 encoder linears on FP8 tensor cores (embeddings, MLM transform and the tied
-    decoder stay bf16).  The state dict is the same either way."""
+    decoder stay bf16).  ``pad_token_id`` takes right-padded input (padded keys are hidden from attention).  The state
+    dict is the same either way."""
     if with_mlm_head:
-        return BertForMaskedLM(BertConfig(pad_vocab_to=64, fp8=fp8))
-    return BertModel(BertConfig(fp8=fp8))
+        return BertForMaskedLM(BertConfig(pad_vocab_to=64, fp8=fp8, pad_token_id=pad_token_id))
+    return BertModel(BertConfig(fp8=fp8, pad_token_id=pad_token_id))

@@ -269,6 +269,94 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
 
 
 # ------------------------------------------------------------------------------------------------
+# Key-padding attention (csrc/attention.cu): Q / K / V read straight out of the fused projection
+# ------------------------------------------------------------------------------------------------
+ATTENTION_HEAD_DIM = 64
+ATTENTION_SEQ_MULTIPLE = 128
+
+
+def _key_mask(seq_lens: torch.Tensor, S: int, device) -> torch.Tensor:
+    """[B, S] bool: key j of sequence b is visible iff j < seq_lens[b] (lengths clamped to [0, S], like the kernel)."""
+    lens = seq_lens.to(device=device, dtype=torch.long).clamp(0, S)
+    return torch.arange(S, device=device)[None, :] < lens[:, None]
+
+
+def attention_reference(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> torch.Tensor:
+    """softmax(Q K^T / sqrt(d)) V with the key-padding mask, in fp32 (fp64 stays fp64); a sequence of length 0 gives zeros.
+    qkv [B, S, 3 * hidden] (query | key | value column blocks), returns [B, S, hidden] in qkv's dtype.  Differentiable."""
+    B, S, W = qkv.shape
+    hidden = W // 3
+    hd = hidden // heads
+    ct = torch.promote_types(qkv.dtype, torch.float32)
+    q, k, v = (t.to(ct).reshape(B, S, heads, hd).transpose(1, 2) for t in qkv.split(hidden, dim=-1))
+    keep = _key_mask(seq_lens, S, qkv.device)[:, None, None, :]
+    scores = (q @ k.transpose(-1, -2)) * (1.0 / math.sqrt(hd))
+    # a finite fill keeps an all-hidden row free of NaN; multiplying by the mask then zeroes it (and its gradients)
+    p = torch.softmax(scores.masked_fill(~keep, torch.finfo(ct).min), dim=-1) * keep
+    return (p @ v).transpose(1, 2).reshape(B, S, hidden).to(qkv.dtype)
+
+
+def _attention_check(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> None:
+    if qkv.dim() != 3 or qkv.shape[-1] % 3:
+        raise ValueError(f"attention needs qkv [B, S, 3 * hidden], got {tuple(qkv.shape)}")
+    B, S, W = qkv.shape
+    if heads < 1 or (W // 3) % heads or (W // 3) // heads != ATTENTION_HEAD_DIM:
+        raise ValueError(f"attention on CUDA supports head dim {ATTENTION_HEAD_DIM} only, got hidden {W // 3} over {heads} heads")
+    if qkv.dtype != torch.bfloat16:
+        raise ValueError(f"attention on CUDA needs bf16 qkv, got {qkv.dtype}")
+    if S % ATTENTION_SEQ_MULTIPLE or S == 0:
+        raise ValueError(f"attention on CUDA needs the sequence length to be a multiple of {ATTENTION_SEQ_MULTIPLE}, got {S}")
+    if not qkv.is_contiguous():
+        raise ValueError("attention on CUDA needs a contiguous qkv (the fused projection's output)")
+    if seq_lens.dim() != 1 or seq_lens.shape[0] != B or seq_lens.is_floating_point() or seq_lens.is_complex():
+        raise ValueError(f"attention needs integer seq_lens [B] = [{B}], got {seq_lens.dtype} {tuple(seq_lens.shape)}")
+
+
+class _Attention(torch.autograd.Function):
+    """Key-padding attention.  CUDA body: the sm_90a kernels (forward keeps the row log-sum-exp; backward is three
+    deterministic launches writing one dqkv tensor, the exact gradient the qkv linear consumes).  CPU body:
+    ``attention_reference`` (backward by recomputation through autograd)."""
+
+    @staticmethod
+    def forward(ctx, qkv, seq_lens, heads):
+        ctx.heads = heads
+        if qkv.is_cuda:
+            B, S, W = qkv.shape
+            lens = seq_lens.to(device=qkv.device, dtype=torch.int32).contiguous()
+            o, lse = _C().attention_fwd(qkv.view(B * S, W), lens, heads)
+            ctx.save_for_backward(qkv, o, lse, lens)
+            return o.view(B, S, W // 3)
+        ctx.save_for_backward(qkv, seq_lens)
+        return attention_reference(qkv, seq_lens, heads)
+
+    @staticmethod
+    def backward(ctx, dy):
+        if dy.is_cuda:
+            qkv, o, lse, lens = ctx.saved_tensors
+            B, S, W = qkv.shape
+            do = dy.reshape(B * S, W // 3).to(torch.bfloat16).contiguous()
+            if do.data_ptr() % 16:                                # the kernels read dO in 16-byte vectors / TMA boxes
+                do = do.clone()
+            dqkv = _C().attention_bwd(do, qkv.view(B * S, W), o, lse, lens, ctx.heads)
+            return dqkv.view(B, S, W), None, None
+        qkv, seq_lens = ctx.saved_tensors
+        with torch.enable_grad():
+            x = qkv.detach().requires_grad_(True)
+            (g,) = torch.autograd.grad(attention_reference(x, seq_lens, ctx.heads), x, dy)
+        return g, None, None
+
+
+def attention(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> torch.Tensor:
+    """Multi-head attention over right-padded sequences: qkv [B, S, 3 * hidden] (the fused projection's output, column
+    blocks query | key | value), seq_lens [B] integer lengths (key j of sequence b is visible iff j < seq_lens[b]; every
+    query row is computed).  Returns [B, S, hidden].  On CUDA: bf16, head dim 64, S % 128 == 0 and contiguous qkv, else
+    ``ValueError``; lengths stay on the device (no host synchronisation, CUDA-graph safe)."""
+    if qkv.is_cuda:
+        _attention_check(qkv, seq_lens, heads)
+    return _Attention.apply(qkv, seq_lens, heads)
+
+
+# ------------------------------------------------------------------------------------------------
 # Convolutions on wgmma (csrc/conv_wgmma.cu, csrc/conv_wgrad_wgmma.cu)
 # ------------------------------------------------------------------------------------------------
 def _conv_policy() -> str:
