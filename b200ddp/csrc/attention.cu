@@ -5,9 +5,16 @@
 //   o    bf16 [B*S, H*64]     written in the layout the output projection reads (no transpose)
 //   lse  fp32 [B, H, S]       natural-log row log-sum-exp of the scaled scores (-inf for a sequence of length 0)
 //
-// Key j of sequence b is visible iff j < seq_lens[b] (clamped to [0, S] here: the host cannot validate device lengths
-// without a synchronisation).  Every query row is computed, padded ones included, so every row equals softmax attention
-// over the visible keys; a sequence of length 0 gets zero output and zero gradients.
+// Two mask modes, chosen at compile time (template parameter kMode):
+//   kKeyPadding  seq_lens int32 [B]: key j of sequence b is visible iff j < seq_lens[b] (clamped to [0, S] here: the host
+//                cannot validate device lengths without a synchronisation).  Every query row is computed, padded ones
+//                included, so every row equals softmax attention over the visible keys; a sequence of length 0 gets zero
+//                output and zero gradients.
+//   kSegment     bounds int32 [B*S, 2] (packed documents): query i of a sequence sees key j of the same sequence iff
+//                start[i] <= j < end[i] (start clamped to [0, S], end to [start, S]).  A row with start == end (padding)
+//                gets zero output, lse = -inf and zero gradients.  Each CTA visits only the tiles inside the union of its
+//                128 rows' intervals; dK / dV mask with the key rows' own bounds, which is the same test as the query's for
+//                a block-diagonal mask.
 //
 // Each kernel has one TMA producer warp (warp 0; warps 1-3 idle) and two consumer warpgroups (warps 4-7, 8-11) that own
 // 64 rows each.  All tiles are 64-row boxes of one 2-D tensor map over qkv (or dO), 128B-swizzled, so a head's 64
@@ -58,9 +65,43 @@ constexpr int kFwdSmem = 1024 + 2 * kBoxBytes + kFwdStages * 4 * kBoxBytes + 256
 constexpr int kBwdStages = 4;
 constexpr int kBwdSmem = 1024 + 4 * kBoxBytes + kBwdStages * 2 * kBoxBytes + 256;   // fixed 2 x 128 rows + ring of 2 x 64 rows
 
+constexpr int kKeyPadding = 0;
+constexpr int kSegment = 1;
+
 __device__ __forceinline__ int clamped_len(const int* lens, int b, int S) {
   const int n = __ldg(lens + b);
   return n < 0 ? 0 : (n > S ? S : n);
+}
+// (start, end) of global row `row` of bounds [B*S, 2], clamped to 0 <= start <= end <= S
+__device__ __forceinline__ int2 row_bounds(const int* bounds, size_t row, int S) {
+  const int2 v = __ldg(reinterpret_cast<const int2*>(bounds) + row);
+  const int s = min(max(v.x, 0), S);
+  return make_int2(s, min(max(v.y, s), S));
+}
+__device__ __forceinline__ bool inside(int j, int2 r) { return (unsigned)(j - r.x) < (unsigned)(r.y - r.x); }
+// A fragment thread owns columns 8 j + e (j < 8, e < 2) of a 64-wide tile, counted from its first column.  Bit 2 j + e
+// is set where that column lies in [lo, hi).  The columns are increasing in the bit index, so the set bits are the range
+// [#columns below lo, #columns below hi).
+__device__ __forceinline__ uint32_t frag_mask16(int lo, int hi) {
+  lo = min(max(lo, 0), 64);
+  hi = min(max(hi, lo), 64);
+  const int nlo = 2 * (lo >> 3) + min(lo & 7, 2), nhi = 2 * (hi >> 3) + min(hi & 7, 2);
+  return ((1u << nhi) - 1u) & ~((1u << nlo) - 1u);
+}
+// [lo, hi): the union of the intervals of rows row0 .. row0 + 127 (lo >= hi when all are empty).  Every thread of the
+// block calls it (it holds a __syncthreads); scratch is 8 ints of shared memory.
+__device__ __forceinline__ int2 cta_range(const int* bounds, size_t row0, int S, int* scratch) {
+  const int t = threadIdx.x;
+  if (t < 128) {
+    const int2 r = row_bounds(bounds, row0 + t, S);
+    const bool empty = r.x >= r.y;
+    const int lo = __reduce_min_sync(0xffffffffu, empty ? S : r.x);
+    const int hi = __reduce_max_sync(0xffffffffu, empty ? 0 : r.y);
+    if ((t & 31) == 0) { scratch[t >> 5] = lo; scratch[4 + (t >> 5)] = hi; }
+  }
+  __syncthreads();
+  return make_int2(min(min(scratch[0], scratch[1]), min(scratch[2], scratch[3])),
+                   max(max(scratch[4], scratch[5]), max(scratch[6], scratch[7])));
 }
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
@@ -96,8 +137,10 @@ __device__ __forceinline__ void store_frag(const float (&acc)[32], float scale0,
 }
 
 // ============================================== forward ==============================================================
+// mask: seq_lens [B] (kKeyPadding) or bounds [B*S, 2] (kSegment)
+template <int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restrict__ seq_lens, int S, int H,
+attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restrict__ mask, int S, int H,
                 __nv_bfloat16* __restrict__ o, float* __restrict__ lse) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
@@ -109,9 +152,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
 
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int HD = H * kHd;
-  const int len = clamped_len(seq_lens, b, S);
-  const int n_kt = (len + 127) / 128;
   const size_t seq_row = (size_t)b * S;
+  int len = 0, kt0 = 0, n_kt;                                   // key tiles kt0 .. kt0 + n_kt - 1
+  if constexpr (kMode == kKeyPadding) {
+    len = clamped_len(mask, b, S);
+    n_kt = (len + 127) / 128;
+  } else {
+    const int2 r = cta_range(mask, seq_row + qt * 128, S, reinterpret_cast<int*>(empty_bar + kFwdStages));
+    kt0 = r.x / 128;
+    n_kt = r.x < r.y ? (r.y + 127) / 128 - kt0 : 0;
+  }
   float* lse_bh = lse + ((size_t)b * H + h) * S;
   if (n_kt == 0) {                                              // no visible key: zero output, empty log-sum-exp
     zero_rows(o + h * kHd, HD, seq_row + qt * 128, 128);
@@ -135,7 +185,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
       tma_load_2d(&map_qkv, q_bar, sq + kBoxBytes, h * kHd, q_row + 64);
       int stage = 0;
       uint32_t phase = 0;
-      for (int kt = 0; kt < n_kt; ++kt) {
+      for (int kt = kt0; kt < kt0 + n_kt; ++kt) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* sk = ring + stage * 4 * kBoxBytes;
         uint8_t* sv = sk + 2 * kBoxBytes;
@@ -153,6 +203,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
     const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);         // this thread's rows: r0 and r0 + 8 of the warpgroup's 64
     const int c0 = 2 * (lane & 3);
     const uint32_t q_addr = smem_u32(sq + wg * kBoxBytes);
+    int2 rb0, rb1;                                              // kSegment: the intervals of this thread's two rows
+    if constexpr (kMode == kSegment) {
+      rb0 = row_bounds(mask, seq_row + qt * 128 + wg * 64 + r0, S);
+      rb1 = row_bounds(mask, seq_row + qt * 128 + wg * 64 + r0 + 8, S);
+    }
     float acc[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[i] = 0.f;
@@ -160,7 +215,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
     mbar_wait(q_bar, 0);
     int stage = 0;
     uint32_t phase = 0;
-    for (int kt = 0; kt < n_kt; ++kt) {
+    for (int kt = kt0; kt < kt0 + n_kt; ++kt) {
       mbar_wait(&full_bar[stage], phase);
       const uint32_t k_addr = smem_u32(ring + stage * 4 * kBoxBytes);
       const uint32_t v_addr = k_addr + 2 * kBoxBytes;
@@ -172,12 +227,26 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
       wgmma_commit();
       wgmma_wait<0>();
       const int key0 = kt * 128;
-      if (key0 + 128 > len) {                                   // partial tile: hide keys at or beyond the length
+      if constexpr (kMode == kKeyPadding) {
+        if (key0 + 128 > len) {                                 // partial tile: hide keys at or beyond the length
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+          for (int j = 0; j < 16; ++j) {
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            if (key0 + 8 * j + c0 + e >= len) { s[4 * j + e] = -INFINITY; s[4 * j + 2 + e] = -INFINITY; }
+            for (int e = 0; e < 2; ++e) {
+              if (key0 + 8 * j + c0 + e >= len) { s[4 * j + e] = -INFINITY; s[4 * j + 2 + e] = -INFINITY; }
+            }
+          }
+        }
+      } else {
+        if (key0 < max(rb0.x, rb1.x) || key0 + 128 > min(rb0.y, rb1.y)) {   // tile not wholly inside both intervals
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int key = key0 + 8 * j + c0 + e;
+              if (!inside(key, rb0)) s[4 * j + e] = -INFINITY;
+              if (!inside(key, rb1)) s[4 * j + 2 + e] = -INFINITY;
+            }
           }
         }
       }
@@ -193,9 +262,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
       for (int i = 0; i < 2; ++i) {
         mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
         mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-        alpha[i] = exp2f((m[i] - mx[i]) * kScaleLog2);          // key 0 is visible, so mx is finite; 0 on the first tile
-        m[i] = mx[i];
-        mb[i] = mx[i] * kScaleLog2;
+        if constexpr (kMode == kKeyPadding) {
+          alpha[i] = exp2f((m[i] - mx[i]) * kScaleLog2);        // key 0 is visible, so mx is finite; 0 on the first tile
+          m[i] = mx[i];
+          mb[i] = mx[i] * kScaleLog2;
+        } else {
+          // a row may have seen no visible key yet (mx = -inf): subtract 0 instead, so exp2 gives 0 rather than NaN
+          const float base = mx[i] == -INFINITY ? 0.f : mx[i];
+          alpha[i] = exp2f((m[i] - base) * kScaleLog2);
+          m[i] = mx[i];
+          mb[i] = base * kScaleLog2;
+        }
       }
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
@@ -233,10 +310,18 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
       l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
     }
     const int row = qt * 128 + wg * 64 + r0;                    // position in the sequence
-    store_frag(acc, 1.f / l[0], 1.f / l[1], o + (seq_row + row) * HD + h * kHd, HD, c0);
-    if ((lane & 3) == 0) {
-      lse_bh[row] = m[0] * kScale + logf(l[0]);
-      lse_bh[row + 8] = m[1] * kScale + logf(l[1]);
+    if constexpr (kMode == kKeyPadding) {
+      store_frag(acc, 1.f / l[0], 1.f / l[1], o + (seq_row + row) * HD + h * kHd, HD, c0);
+      if ((lane & 3) == 0) {
+        lse_bh[row] = m[0] * kScale + logf(l[0]);
+        lse_bh[row + 8] = m[1] * kScale + logf(l[1]);
+      }
+    } else {                                                    // a row that saw no key: zeros and -inf
+      store_frag(acc, l[0] > 0.f ? 1.f / l[0] : 0.f, l[1] > 0.f ? 1.f / l[1] : 0.f, o + (seq_row + row) * HD + h * kHd, HD, c0);
+      if ((lane & 3) == 0) {
+        lse_bh[row] = l[0] > 0.f ? m[0] * kScale + logf(l[0]) : -INFINITY;
+        lse_bh[row + 8] = l[1] > 0.f ? m[1] * kScale + logf(l[1]) : -INFINITY;
+      }
     }
   }
 }
@@ -317,24 +402,35 @@ __device__ __forceinline__ void bwd_produce(const BwdSmem& L, const CUtensorMap*
   }
 }
 
-// dK, dV for one tile of 128 keys.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries, all S / 64 of them.
+// dK, dV for one tile of 128 keys.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries: all S / 64 of them (kKeyPadding),
+// or those inside the union of the key rows' intervals (kSegment).
+template <int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
-                     const int* __restrict__ seq_lens, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
+                     const int* __restrict__ mask, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
                      __nv_bfloat16* __restrict__ dqkv) {
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
   const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int HD = H * kHd;
   const size_t pitch = (size_t)3 * HD;
-  const int len = clamped_len(seq_lens, b, S);
   const size_t seq_row = (size_t)b * S;
-  if (kt * 128 >= len) {                                        // every key of the tile is hidden: no gradient
+  int len = 0, qt0 = 0, n_qt = S / 64;                          // query tiles qt0 .. qt0 + n_qt - 1
+  bool hidden;
+  if constexpr (kMode == kKeyPadding) {
+    len = clamped_len(mask, b, S);
+    hidden = kt * 128 >= len;
+  } else {
+    const int2 r = cta_range(mask, seq_row + kt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
+    hidden = r.x >= r.y;
+    qt0 = r.x / 64;
+    n_qt = (r.y + 63) / 64 - qt0;
+  }
+  if (hidden) {                                                 // every key of the tile is hidden: no gradient
     zero_rows(dqkv + HD + h * kHd, pitch, seq_row + kt * 128, 128);
     zero_rows(dqkv + 2 * HD + h * kHd, pitch, seq_row + kt * 128, 128);
     return;
   }
-  const int n_qt = S / 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 1 && lane == 0) bwd_init_barriers(L);
   __syncthreads();
@@ -344,14 +440,14 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
       tma_prefetch_desc(&map_qkv);
       tma_prefetch_desc(&map_do);
       bwd_produce(L, &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row + kt * 128,
-                  &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row, n_qt);
+                  &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + 64 * qt0, n_qt);
     }
   } else if (warp >= 4) {
     const int wg = (warp - 4) >> 2;                             // keys [64 wg, 64 wg + 64) of the tile
     const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
     const int c0 = 2 * (lane & 3);
     const int key = kt * 128 + wg * 64 + r0;
-    const bool vis0 = key < len, vis1 = key + 8 < len;
+    const bool vis0 = key < len, vis1 = key + 8 < len;          // kKeyPadding
     const uint32_t k_addr = smem_u32(L.fixed0 + wg * kBoxBytes), v_addr = smem_u32(L.fixed1 + wg * kBoxBytes);
     const float* lse_bh = lse + ((size_t)b * H + h) * S;
     const float* D_bh = Dsum + ((size_t)b * H + h) * S;
@@ -361,7 +457,15 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
     mbar_wait(L.fixed_bar, 0);
     int stage = 0;
     uint32_t phase = 0;
-    for (int qt = 0; qt < n_qt; ++qt) {
+    for (int qt = qt0; qt < qt0 + n_qt; ++qt) {
+      // kSegment: the key rows' intervals as one bit mask over this thread's 16 query columns (bits 0-15: row key,
+      // 16-31: row key + 8), so the mask costs one register while the accumulators are live
+      uint32_t vis = 0;
+      if constexpr (kMode == kSegment) {
+        const int2 kb0 = row_bounds(mask, seq_row + key, S), kb1 = row_bounds(mask, seq_row + key + 8, S);
+        const int q0 = qt * 64 + c0;
+        vis = frag_mask16(kb0.x - q0, kb0.y - q0) | (frag_mask16(kb1.x - q0, kb1.y - q0) << 16);
+      }
       mbar_wait(&L.full_bar[stage], phase);
       const uint32_t q_addr = smem_u32(L.ring + stage * 2 * kBoxBytes), do_addr = q_addr + kBoxBytes;
       float st[32], dpt[32];
@@ -376,11 +480,23 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
         const int q = qt * 64 + 8 * j + c0;
         const float2 lq = *reinterpret_cast<const float2*>(lse_bh + q);
         const float2 dq = *reinterpret_cast<const float2*>(D_bh + q);
-        const float l0 = lq.x * kLog2e, l1 = lq.y * kLog2e;
-        const float p00 = vis0 ? exp2f(st[4 * j] * kScaleLog2 - l0) : 0.f;
-        const float p01 = vis0 ? exp2f(st[4 * j + 1] * kScaleLog2 - l1) : 0.f;
-        const float p10 = vis1 ? exp2f(st[4 * j + 2] * kScaleLog2 - l0) : 0.f;
-        const float p11 = vis1 ? exp2f(st[4 * j + 3] * kScaleLog2 - l1) : 0.f;
+        float l0 = lq.x * kLog2e, l1 = lq.y * kLog2e;
+        if constexpr (kMode == kSegment) {                      // a query that saw no key (lse = -inf) gets P = 0, even
+          l0 = lq.x == -INFINITY ? INFINITY : l0;               // where malformed bounds put it inside a key's interval
+          l1 = lq.y == -INFINITY ? INFINITY : l1;
+        }
+        bool v00, v01, v10, v11;                                // (key row, query column)
+        if constexpr (kMode == kKeyPadding) {
+          v00 = v01 = vis0;
+          v10 = v11 = vis1;
+        } else {
+          v00 = (vis >> (2 * j)) & 1u; v01 = (vis >> (2 * j + 1)) & 1u;
+          v10 = (vis >> (16 + 2 * j)) & 1u; v11 = (vis >> (17 + 2 * j)) & 1u;
+        }
+        const float p00 = v00 ? exp2f(st[4 * j] * kScaleLog2 - l0) : 0.f;
+        const float p01 = v01 ? exp2f(st[4 * j + 1] * kScaleLog2 - l1) : 0.f;
+        const float p10 = v10 ? exp2f(st[4 * j + 2] * kScaleLog2 - l0) : 0.f;
+        const float p11 = v11 ? exp2f(st[4 * j + 3] * kScaleLog2 - l1) : 0.f;
         pa[2 * j] = pack_bf16x2(p00, p01);
         pa[2 * j + 1] = pack_bf16x2(p10, p11);
         dsa[2 * j] = pack_bf16x2(p00 * (dpt[4 * j] - dq.x), p01 * (dpt[4 * j + 1] - dq.y));
@@ -403,23 +519,35 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
   }
 }
 
-// dQ for one tile of 128 queries.  Fixed: Q, dO.  Ring: (K, V) tiles of 64 keys below the length.
+// dQ for one tile of 128 queries.  Fixed: Q, dO.  Ring: (K, V) tiles of 64 keys below the length (kKeyPadding), or
+// inside the union of the query rows' intervals (kSegment).
+template <int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
-                   const int* __restrict__ seq_lens, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
+                   const int* __restrict__ mask, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
                    __nv_bfloat16* __restrict__ dqkv) {
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int HD = H * kHd;
   const size_t pitch = (size_t)3 * HD;
-  const int len = clamped_len(seq_lens, b, S);
   const size_t seq_row = (size_t)b * S;
-  if (len == 0) {
+  int len = 0, kt0 = 0, kt_end = 0;
+  bool hidden;
+  if constexpr (kMode == kKeyPadding) {
+    len = clamped_len(mask, b, S);
+    hidden = len == 0;
+  } else {
+    const int2 r = cta_range(mask, seq_row + qt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
+    hidden = r.x >= r.y;
+    kt0 = r.x / 64;
+    kt_end = (r.y + 63) / 64;
+  }
+  if (hidden) {
     zero_rows(dqkv + h * kHd, pitch, seq_row + qt * 128, 128);
     return;
   }
-  const int n_kt = (len + 63) / 64;
+  const int n_kt = kMode == kKeyPadding ? (len + 63) / 64 : kt_end - kt0;   // key tiles kt0 .. kt0 + n_kt - 1
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 1 && lane == 0) bwd_init_barriers(L);
   __syncthreads();
@@ -429,13 +557,18 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
       tma_prefetch_desc(&map_qkv);
       tma_prefetch_desc(&map_do);
       bwd_produce(L, &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + qt * 128,
-                  &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row, n_kt);
+                  &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row + 64 * kt0, n_kt);
     }
   } else if (warp >= 4) {
     const int wg = (warp - 4) >> 2;
     const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
     const int c0 = 2 * (lane & 3);
     const int row = qt * 128 + wg * 64 + r0;
+    int2 qb0, qb1;                                              // kSegment: the intervals of query rows row, row + 8
+    if constexpr (kMode == kSegment) {
+      qb0 = row_bounds(mask, seq_row + row, S);
+      qb1 = row_bounds(mask, seq_row + row + 8, S);
+    }
     const uint32_t q_addr = smem_u32(L.fixed0 + wg * kBoxBytes), do_addr = smem_u32(L.fixed1 + wg * kBoxBytes);
     const size_t bh = ((size_t)b * H + h) * S;
     const float l0 = lse[bh + row] * kLog2e, l1 = lse[bh + row + 8] * kLog2e;
@@ -446,7 +579,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
     mbar_wait(L.fixed_bar, 0);
     int stage = 0;
     uint32_t phase = 0;
-    for (int kt = 0; kt < n_kt; ++kt) {
+    for (int kt = kt0; kt < kt0 + n_kt; ++kt) {
       mbar_wait(&L.full_bar[stage], phase);
       const uint32_t k_addr = smem_u32(L.ring + stage * 2 * kBoxBytes), v_addr = k_addr + kBoxBytes;
       float s[32], dp[32];
@@ -459,11 +592,18 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int k0 = kt * 64 + 8 * j + c0;
-        const bool v0 = k0 < len, v1 = k0 + 1 < len;
-        const float p00 = v0 ? exp2f(s[4 * j] * kScaleLog2 - l0) : 0.f;
-        const float p01 = v1 ? exp2f(s[4 * j + 1] * kScaleLog2 - l0) : 0.f;
-        const float p10 = v0 ? exp2f(s[4 * j + 2] * kScaleLog2 - l1) : 0.f;
-        const float p11 = v1 ? exp2f(s[4 * j + 3] * kScaleLog2 - l1) : 0.f;
+        bool v00, v01, v10, v11;                                // (query row, key column)
+        if constexpr (kMode == kKeyPadding) {
+          v00 = v10 = k0 < len;
+          v01 = v11 = k0 + 1 < len;
+        } else {
+          v00 = inside(k0, qb0); v01 = inside(k0 + 1, qb0);
+          v10 = inside(k0, qb1); v11 = inside(k0 + 1, qb1);
+        }
+        const float p00 = v00 ? exp2f(s[4 * j] * kScaleLog2 - l0) : 0.f;
+        const float p01 = v01 ? exp2f(s[4 * j + 1] * kScaleLog2 - l0) : 0.f;
+        const float p10 = v10 ? exp2f(s[4 * j + 2] * kScaleLog2 - l1) : 0.f;
+        const float p11 = v11 ? exp2f(s[4 * j + 3] * kScaleLog2 - l1) : 0.f;
         dsa[2 * j] = pack_bf16x2(p00 * (dp[4 * j] - d0), p01 * (dp[4 * j + 1] - d0));
         dsa[2 * j + 1] = pack_bf16x2(p10 * (dp[4 * j + 2] - d1), p11 * (dp[4 * j + 3] - d1));
       }
@@ -495,21 +635,21 @@ void check_shape(const char* who, int B, int S, int heads) {
     throw std::runtime_error(std::string(who) + ": problem too large");
 }
 
-}  // namespace
-
-void launch_attention_fwd(const void* qkv, const int* seq_lens, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
-  check_shape("attention_fwd", B, S, heads);
+template <int kMode>
+void attention_fwd(const char* who, const void* qkv, const int* mask, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
+  check_shape(who, B, S, heads);
   const CUtensorMap map_qkv = rows_map(qkv, B * S, 3 * heads * kHd);
   static std::atomic<unsigned long long> configured{0};
-  ensure_max_dynamic_smem(attn_fwd_kernel, kFwdSmem, configured);
-  attn_fwd_kernel<<<dim3(S / 128, heads, B), kThreads, kFwdSmem, s>>>(map_qkv, seq_lens, S, heads,
-                                                                      reinterpret_cast<__nv_bfloat16*>(o), lse);
+  ensure_max_dynamic_smem(attn_fwd_kernel<kMode>, kFwdSmem, configured);
+  attn_fwd_kernel<kMode><<<dim3(S / 128, heads, B), kThreads, kFwdSmem, s>>>(map_qkv, mask, S, heads,
+                                                                             reinterpret_cast<__nv_bfloat16*>(o), lse);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 
-void launch_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* seq_lens, int B, int S,
-                          int heads, float* dsum, void* dqkv, cudaStream_t s) {
-  check_shape("attention_bwd", B, S, heads);
+template <int kMode>
+void attention_bwd(const char* who, const void* dout, const void* qkv, const void* o, const float* lse, const int* mask, int B,
+                   int S, int heads, float* dsum, void* dqkv, cudaStream_t s) {
+  check_shape(who, B, S, heads);
   const int rows = B * S;
   const long long items = (long long)rows * heads * 8;
   attn_bwd_dot_kernel<<<ceil_div(items, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dout),
@@ -519,12 +659,32 @@ void launch_attention_bwd(const void* dout, const void* qkv, const void* o, cons
   const CUtensorMap map_do = rows_map(dout, rows, heads * kHd);
   auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
   static std::atomic<unsigned long long> configured_dkdv{0}, configured_dq{0};
-  ensure_max_dynamic_smem(attn_bwd_dkdv_kernel, kBwdSmem, configured_dkdv);
-  ensure_max_dynamic_smem(attn_bwd_dq_kernel, kBwdSmem, configured_dq);
-  attn_bwd_dkdv_kernel<<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, seq_lens, S, heads, lse, dsum, dq);
+  ensure_max_dynamic_smem(attn_bwd_dkdv_kernel<kMode>, kBwdSmem, configured_dkdv);
+  ensure_max_dynamic_smem(attn_bwd_dq_kernel<kMode>, kBwdSmem, configured_dq);
+  attn_bwd_dkdv_kernel<kMode><<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, mask, S, heads, lse, dsum, dq);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
-  attn_bwd_dq_kernel<<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, seq_lens, S, heads, lse, dsum, dq);
+  attn_bwd_dq_kernel<kMode><<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, mask, S, heads, lse, dsum, dq);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+}  // namespace
+
+void launch_attention_fwd(const void* qkv, const int* seq_lens, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
+  attention_fwd<kKeyPadding>("attention_fwd", qkv, seq_lens, B, S, heads, o, lse, s);
+}
+
+void launch_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* seq_lens, int B, int S,
+                          int heads, float* dsum, void* dqkv, cudaStream_t s) {
+  attention_bwd<kKeyPadding>("attention_bwd", dout, qkv, o, lse, seq_lens, B, S, heads, dsum, dqkv, s);
+}
+
+void launch_packed_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
+  attention_fwd<kSegment>("packed_attention_fwd", qkv, bounds, B, S, heads, o, lse, s);
+}
+
+void launch_packed_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                 int S, int heads, float* dsum, void* dqkv, cudaStream_t s) {
+  attention_bwd<kSegment>("packed_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s);
 }
 
 }  // namespace b200

@@ -564,52 +564,91 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                     M, N, K, a.scalar_type() == at::kFloat8_e5m2, epilogue, cur_stream());
     return d;
   }, py::arg("a"), py::arg("b"), py::arg("a_scale_inv"), py::arg("b_scale_inv"), py::arg("bias") = py::none(), py::arg("epilogue") = 0);
-  // ---- key-padding attention (attention.cu): head dim 64, S % 128 == 0, lengths on the device ---------------------------
-  auto attn_check = [](const at::Tensor& qkv, const at::Tensor& seq_lens, int heads, const char* who) {
-    check_cuda(qkv, "qkv"); check_cuda(seq_lens, "seq_lens");
+  // ---- attention (attention.cu): head dim 64, S % 128 == 0, masks on the device ----------------------------------------
+  auto attn_qkv_check = [](const at::Tensor& qkv, int heads, const char* who) {
+    check_cuda(qkv, "qkv");
     TORCH_CHECK(qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 2 && qkv.is_contiguous(), who, ": qkv must be contiguous bf16 [B*S, 3*heads*64]");
     TORCH_CHECK(heads >= 1 && qkv.size(1) == 3LL * heads * 64, who, ": qkv has ", qkv.size(1), " columns, expected 3 * heads * 64 with heads = ", heads);
+  };
+  // key padding: seq_lens int32 [B]; returns B
+  auto attn_check = [attn_qkv_check](const at::Tensor& qkv, const at::Tensor& seq_lens, int heads, const char* who) {
+    attn_qkv_check(qkv, heads, who);
+    check_cuda(seq_lens, "seq_lens");
     TORCH_CHECK(seq_lens.scalar_type() == at::kInt && seq_lens.dim() == 1 && seq_lens.is_contiguous() && seq_lens.numel() >= 1, who, ": seq_lens must be int32 [B]");
     TORCH_CHECK(qkv.size(0) % seq_lens.numel() == 0, who, ": qkv rows (", qkv.size(0), ") are not B * S for B = ", seq_lens.numel());
     TORCH_CHECK(seq_lens.device() == qkv.device(), who, ": seq_lens must be on qkv's device");
     TORCH_CHECK((reinterpret_cast<uintptr_t>(qkv.data_ptr()) & 15) == 0, who, ": qkv must be 16-byte aligned");
+    return (int)seq_lens.numel();
   };
+  // packed documents: bounds int32 [B, S, 2] (contiguous, so [B*S, 2] rows of (start, end)); returns B
+  auto packed_check = [attn_qkv_check](const at::Tensor& qkv, const at::Tensor& bounds, int heads, const char* who) {
+    attn_qkv_check(qkv, heads, who);
+    check_cuda(bounds, "bounds");
+    TORCH_CHECK(bounds.scalar_type() == at::kInt && bounds.dim() == 3 && bounds.size(2) == 2 && bounds.is_contiguous() && bounds.numel() >= 2,
+                who, ": bounds must be contiguous int32 [B, S, 2]");
+    TORCH_CHECK(qkv.size(0) == bounds.size(0) * bounds.size(1), who, ": qkv rows (", qkv.size(0), ") are not B * S for bounds [",
+                bounds.size(0), ", ", bounds.size(1), ", 2]");
+    TORCH_CHECK(bounds.device() == qkv.device(), who, ": bounds must be on qkv's device");
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(qkv.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(bounds.data_ptr()) & 7) == 0,
+                who, ": qkv must be 16-byte and bounds 8-byte aligned");
+    return (int)bounds.size(0);
+  };
+  using AttnFwd = void (*)(const void*, const int*, int, int, int, void*, float*, cudaStream_t);
+  using AttnBwd = void (*)(const void*, const void*, const void*, const float*, const int*, int, int, int, float*, void*, cudaStream_t);
   // (o [B*S, heads*64] bf16, lse [B, heads, S] fp32); optional caller-owned outputs
-  m.def("attention_fwd", [attn_check](at::Tensor qkv, at::Tensor seq_lens, int heads, c10::optional<at::Tensor> o_out,
-                                      c10::optional<at::Tensor> lse_out) {
-    attn_check(qkv, seq_lens, heads, "attention_fwd");
+  auto attn_fwd = [](AttnFwd launch, const char* who, const at::Tensor& qkv, const at::Tensor& mask, int B, int heads,
+                     c10::optional<at::Tensor> o_out, c10::optional<at::Tensor> lse_out) {
     c10::cuda::CUDAGuard guard(qkv.device());
-    const int B = (int)seq_lens.numel(), S = (int)(qkv.size(0) / B);
+    const int S = (int)(qkv.size(0) / B);
     at::Tensor o = o_out.has_value() ? *o_out : at::empty({qkv.size(0), (int64_t)heads * 64}, qkv.options());
     at::Tensor lse = lse_out.has_value() ? *lse_out : at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-    TORCH_CHECK(o.is_cuda() && o.scalar_type() == at::kBFloat16 && o.is_contiguous() && o.numel() == qkv.numel() / 3, "attention_fwd: bad o");
-    TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S, "attention_fwd: bad lse");
+    TORCH_CHECK(o.is_cuda() && o.scalar_type() == at::kBFloat16 && o.is_contiguous() && o.numel() == qkv.numel() / 3, who, ": bad o");
+    TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S, who, ": bad lse");
     TORCH_CHECK((reinterpret_cast<uintptr_t>(o.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0,
-                "attention_fwd: o must be 16-byte and lse 8-byte aligned");
-    launch_attention_fwd(qkv.data_ptr(), seq_lens.data_ptr<int>(), B, S, heads, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
+                who, ": o must be 16-byte and lse 8-byte aligned");
+    launch(qkv.data_ptr(), mask.data_ptr<int>(), B, S, heads, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
     return std::make_tuple(o, lse);
-  }, py::arg("qkv"), py::arg("seq_lens"), py::arg("heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
+  };
   // dqkv [B*S, 3*heads*64] bf16: the query / key / value column blocks hold dQ / dK / dV
-  m.def("attention_bwd", [attn_check](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor seq_lens, int heads,
-                                      c10::optional<at::Tensor> dqkv_out) {
-    attn_check(qkv, seq_lens, heads, "attention_bwd");
+  auto attn_bwd = [](AttnBwd launch, const char* who, const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o,
+                     const at::Tensor& lse, const at::Tensor& mask, int B, int heads, c10::optional<at::Tensor> dqkv_out) {
     c10::cuda::CUDAGuard guard(qkv.device());
-    const int B = (int)seq_lens.numel(), S = (int)(qkv.size(0) / B);
+    const int S = (int)(qkv.size(0) / B);
     for (const at::Tensor* t : {&dout, &o}) {
       check_cuda(*t, "dout / o");
       TORCH_CHECK(t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->numel() == qkv.numel() / 3 &&
-                  (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, "attention_bwd: dout and o must be 16-byte aligned contiguous bf16 [B*S, heads*64]");
+                  (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, who, ": dout and o must be 16-byte aligned contiguous bf16 [B*S, heads*64]");
     }
     TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S &&
-                (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0, "attention_bwd: lse must be 8-byte aligned contiguous fp32 [B, heads, S]");
+                (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0, who, ": lse must be 8-byte aligned contiguous fp32 [B, heads, S]");
     at::Tensor dqkv = dqkv_out.has_value() ? *dqkv_out : at::empty_like(qkv);
     TORCH_CHECK(dqkv.is_cuda() && dqkv.scalar_type() == at::kBFloat16 && dqkv.is_contiguous() && dqkv.numel() == qkv.numel() &&
-                (reinterpret_cast<uintptr_t>(dqkv.data_ptr()) & 3) == 0, "attention_bwd: bad dqkv");
+                (reinterpret_cast<uintptr_t>(dqkv.data_ptr()) & 3) == 0, who, ": bad dqkv");
     at::Tensor dsum = at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-    launch_attention_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), seq_lens.data_ptr<int>(), B, S, heads,
-                         dsum.data_ptr<float>(), dqkv.data_ptr(), cur_stream());
+    launch(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), mask.data_ptr<int>(), B, S, heads,
+           dsum.data_ptr<float>(), dqkv.data_ptr(), cur_stream());
     return dqkv;
+  };
+  m.def("attention_fwd", [attn_check, attn_fwd](at::Tensor qkv, at::Tensor seq_lens, int heads, c10::optional<at::Tensor> o_out,
+                                                c10::optional<at::Tensor> lse_out) {
+    const int B = attn_check(qkv, seq_lens, heads, "attention_fwd");
+    return attn_fwd(&launch_attention_fwd, "attention_fwd", qkv, seq_lens, B, heads, o_out, lse_out);
+  }, py::arg("qkv"), py::arg("seq_lens"), py::arg("heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
+  m.def("attention_bwd", [attn_check, attn_bwd](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor seq_lens,
+                                                int heads, c10::optional<at::Tensor> dqkv_out) {
+    const int B = attn_check(qkv, seq_lens, heads, "attention_bwd");
+    return attn_bwd(&launch_attention_bwd, "attention_bwd", dout, qkv, o, lse, seq_lens, B, heads, dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("seq_lens"), py::arg("heads"), py::arg("dqkv") = py::none());
+  m.def("packed_attention_fwd", [packed_check, attn_fwd](at::Tensor qkv, at::Tensor bounds, int heads, c10::optional<at::Tensor> o_out,
+                                                         c10::optional<at::Tensor> lse_out) {
+    const int B = packed_check(qkv, bounds, heads, "packed_attention_fwd");
+    return attn_fwd(&launch_packed_attention_fwd, "packed_attention_fwd", qkv, bounds, B, heads, o_out, lse_out);
+  }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
+  m.def("packed_attention_bwd", [packed_check, attn_bwd](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds,
+                                                         int heads, c10::optional<at::Tensor> dqkv_out) {
+    const int B = packed_check(qkv, bounds, heads, "packed_attention_bwd");
+    return attn_bwd(&launch_packed_attention_bwd, "packed_attention_bwd", dout, qkv, o, lse, bounds, B, heads, dqkv_out);
+  }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("dqkv") = py::none());
   m.def("gemm_supported", &gemm_shape_supported);
   m.def("set_gemm_cta_mode", &set_gemm_cta_mode);
   m.def("set_gemm_group_m", &set_gemm_group_m);

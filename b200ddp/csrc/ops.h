@@ -91,6 +91,12 @@ void launch_attention_fwd(const void* qkv, const int* seq_lens, int B, int S, in
 // element written.  Three launches: rowsum(dO * O), dK / dV, dQ.  Deterministic.
 void launch_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* seq_lens, int B, int S,
                           int heads, float* dsum, void* dqkv, cudaStream_t s);
+// Packed documents: bounds int32 [B*S, 2] on the device (8-byte aligned), (start, end) per row in its sequence's
+// coordinates; query i sees key j of its sequence iff start[i] <= j < end[i] (clamped on the device).  A row with
+// start == end gets zero output, lse = -inf and zero gradients.  Same shapes, outputs and workspace as above.
+void launch_packed_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s);
+void launch_packed_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                 int S, int heads, float* dsum, void* dqkv, cudaStream_t s);
 
 // ---------------- small linears on CUDA cores (linear_small.cu) ------------------------------
 // y[M,N] = act(x[M,K] w[N,K]^T + b[N]) ; fp32, dims far below one tensor-core tile (FooModel).

@@ -73,18 +73,30 @@ class SyntheticTokens(Dataset):
 
     ``min_len < seq_len`` gives right-padded rows: each row's length is uniform in [min_len, seq_len] (seeded), its
     prefix holds tokens from [1, vocab) and the tail is ``PAD_ID`` labelled -100.  ``lengths`` then holds the lengths and
-    ``pad_token_id`` is ``PAD_ID``; without padding both are None and the tensors are those of fixed-length rows."""
+    ``pad_token_id`` is ``PAD_ID``; without padding both are None and the tensors are those of fixed-length rows.
+
+    ``pack=True`` packs documents instead: ``samples`` documents with lengths uniform in [min_len, seq_len] (``min_len``
+    defaults to ``seq_len``), each starting with ``CLS_ID`` and holding tokens from [1, vocab) other than ``CLS_ID``,
+    are placed into rows of ``seq_len`` by first-fit decreasing (longest first, ties in document order).  Row tails are
+    ``PAD_ID`` labelled -100, the ``CLS_ID`` tokens are labelled -100 too.  ``lengths`` then holds each row's filled
+    length, ``cls_token_id`` is ``CLS_ID``, and ``doc_ids`` / ``doc_lengths`` list each row's documents (in row order)."""
 
     PAD_ID = 0
+    CLS_ID = 101                   # [CLS] in the BERT vocabulary
 
     def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 30522, mask_prob: float = 0.15, seed: int = 1234,
-                 min_len: int | None = None):
+                 min_len: int | None = None, pack: bool = False):
         if min_len is not None and not 1 <= min_len <= seq_len:
             raise ValueError(f"SyntheticTokens: min_len must lie in [1, seq_len = {seq_len}], got {min_len}")
         g = torch.Generator().manual_seed(seed)
         self.samples = int(samples)
         self.lengths = None
         self.pad_token_id = None
+        self.cls_token_id = None
+        self.doc_ids = self.doc_lengths = None
+        if pack:
+            self._pack(g, seq_len, vocab, mask_prob, seq_len if min_len is None else min_len)
+            return
         if min_len is None or min_len == seq_len:
             self.X = torch.randint(0, vocab, (self.samples, seq_len), generator=g)
         else:
@@ -98,6 +110,44 @@ class SyntheticTokens(Dataset):
             pad = torch.arange(seq_len)[None, :] >= self.lengths[:, None]
             self.X.masked_fill_(pad, self.PAD_ID)
             self.Y.masked_fill_(pad, -100)
+
+    def _pack(self, g: torch.Generator, seq_len: int, vocab: int, mask_prob: float, min_len: int) -> None:
+        if vocab <= self.CLS_ID + 1:
+            raise ValueError(f"SyntheticTokens: packing needs vocab > {self.CLS_ID + 1} (token {self.CLS_ID} starts a document)")
+        lens = torch.randint(min_len, seq_len + 1, (self.samples,), generator=g)
+        total = int(lens.sum())
+        tokens = torch.randint(1, vocab - 1, (total,), generator=g)
+        tokens += tokens >= self.CLS_ID                            # [1, vocab) without CLS_ID
+        labels = torch.randint(0, vocab, (total,), generator=g)
+        masked = torch.rand(total, generator=g) < mask_prob
+        labels = torch.where(masked, labels, torch.full_like(labels, -100))
+        offsets = torch.cumsum(lens, 0) - lens
+        tokens[offsets] = self.CLS_ID
+        labels[offsets] = -100
+        lens_l, offsets_l = lens.tolist(), offsets.tolist()
+        rows, free = [], []
+        for i in sorted(range(self.samples), key=lambda i: (-lens_l[i], i)):   # first-fit decreasing
+            r = next((r for r, f in enumerate(free) if f >= lens_l[i]), len(rows))
+            if r == len(rows):
+                rows.append([])
+                free.append(seq_len)
+            rows[r].append(i)
+            free[r] -= lens_l[i]
+        self.X = torch.full((len(rows), seq_len), self.PAD_ID, dtype=torch.long)
+        self.Y = torch.full((len(rows), seq_len), -100, dtype=torch.long)
+        for r, docs in enumerate(rows):
+            at = 0
+            for i in docs:
+                n, o = lens_l[i], offsets_l[i]
+                self.X[r, at:at + n] = tokens[o:o + n]
+                self.Y[r, at:at + n] = labels[o:o + n]
+                at += n
+        self.samples = len(rows)
+        self.doc_ids = rows
+        self.doc_lengths = [[lens_l[i] for i in docs] for docs in rows]
+        self.lengths = torch.tensor([seq_len - f for f in free])
+        self.pad_token_id = self.PAD_ID
+        self.cls_token_id = self.CLS_ID
 
     def __len__(self) -> int:
         return self.samples

@@ -222,13 +222,20 @@ class DevicePrefetcher:
 
     def _stage(self, host: Tuple[torch.Tensor, ...], slot: int):
         cur = self._dev[slot]
-        if cur is None or any(c.shape != h.shape or c.dtype != h.dtype for c, h in zip(cur, host)):
+        consumer = torch.cuda.current_stream(self.device)
+        fresh = cur is None or any(c.shape != h.shape or c.dtype != h.dtype for c, h in zip(cur, host))
+        if fresh:
             cur = tuple(torch.empty(h.shape, dtype=h.dtype, device=self.device) for h in host)
             self._dev[slot] = cur
         with torch.cuda.stream(self.copy_stream):
+            if fresh:
+                # The allocator hands out memory freed on the consumer stream at once, though kernels queued there may
+                # still use it (an eager step's activations, say): the copy must not write it before they ran.
+                self.copy_stream.wait_stream(consumer)
             self.copy_stream.wait_event(self._consumed[slot])      # previous user of this slot is done
             for d, h in zip(cur, host):
                 d.copy_(h, non_blocking=True)
+                d.record_stream(self.copy_stream)                  # freed with the copy in flight: not reused before it ends
                 self.h2d_bytes += h.numel() * h.element_size()
             self._ready[slot].record(self.copy_stream)
         events = getattr(self.loader, "slot_events", None)

@@ -70,6 +70,10 @@ def build_parser() -> argparse.ArgumentParser:
                    help="BERT on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded keys are "
                         "hidden from attention (native key-padding kernel on the GPU; needs --fp16 and --seq_len %% 128 == 0 "
                         "there).  Default: fixed-length rows")
+    p.add_argument("--pack", action="store_true",
+                   help="BERT on packed documents: documents with lengths uniform in [--min_seq_len, --seq_len], each "
+                        "starting with [CLS], packed first-fit decreasing into rows; attention stays inside a document "
+                        "(native document-boundary kernel on the GPU).  Needs --model bert-base and --min_seq_len < --seq_len")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -127,6 +131,7 @@ def setup(args):
     args.device = device
     check_fp8_args(args)
     check_min_seq_len_args(args)
+    check_pack_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -162,6 +167,18 @@ def check_min_seq_len_args(args) -> None:
             raise ValueError(f"--min_seq_len on a GPU needs --seq_len to be a multiple of 128 (got {args.seq_len})")
 
 
+def check_pack_args(args) -> None:
+    """``--pack`` packs documents into padded BERT rows, so it needs everything ``--min_seq_len`` needs (on the GPU:
+    ``--fp16``, ``--seq_len`` % 128 == 0) and a ``--min_seq_len`` below ``--seq_len``."""
+    if not getattr(args, "pack", False):
+        return
+    if args.model != "bert-base":
+        raise ValueError(f"--pack packs BERT documents; it needs --model bert-base (got --model {args.model})")
+    if not padding_on(args):
+        raise ValueError("--pack needs --min_seq_len below --seq_len (documents have lengths in [--min_seq_len, --seq_len])")
+    check_min_seq_len_args(args)
+
+
 def padding_on(args) -> bool:
     """Rows are padded (and the model must hide padded keys) when some row can be shorter than --seq_len."""
     n = getattr(args, "min_seq_len", None)
@@ -191,6 +208,8 @@ def main(argv=None) -> int:
     if padding_on(args):
         from ..data import SyntheticTokens
         kwargs["pad_token_id"] = SyntheticTokens.PAD_ID
+        if args.pack:
+            kwargs["cls_token_id"] = SyntheticTokens.CLS_ID
     model = build_model(args.model, **kwargs)
     trainer = Trainer(args, model, log)
     trainer.train()

@@ -53,7 +53,7 @@ def build_dataset(args):
         return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
     if name.startswith("bert"):
         return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)),
-                               min_len=getattr(args, "min_seq_len", None))
+                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)))
     raise ValueError(f"no default dataset for model {name!r}")
 
 
@@ -158,17 +158,34 @@ class Trainer:
 
     # ------------------------------------------------------------------------------------------
     def _check_padding(self, model: torch.nn.Module) -> None:
-        """A right-padded dataset needs a model that derives the lengths from the pad id (``BertConfig.pad_token_id``);
-        otherwise padded keys would be attended to without any error."""
+        """A right-padded dataset needs a model that derives the lengths from the pad id (``BertConfig.pad_token_id``),
+        and a packed one also a model that derives the documents from the same CLS id (``BertConfig.cls_token_id``);
+        otherwise padded keys, or other documents, would be attended to without any error."""
+        self.count_pad_id = None
         pad_id = getattr(self.dataset, "pad_token_id", None)
         lengths = getattr(self.dataset, "lengths", None)
         if pad_id is None or lengths is None:
             return
-        model_pads = {getattr(m.config, "pad_token_id", None) for m in model.modules() if hasattr(m, "config")}
+        self.count_pad_id = pad_id                 # rows hold padding: samples/s counts rows, so also count real tokens
+        configs = [m.config for m in model.modules() if hasattr(m, "config")]
+        model_pads = {getattr(c, "pad_token_id", None) for c in configs}
         if pad_id not in model_pads:
             raise ValueError(f"the dataset pads its rows with token {pad_id}, but the model derives no sequence lengths from "
                              f"it (model pad_token_id: {sorted(model_pads - {None}) or None}); build it with pad_token_id={pad_id}")
         seq_len = self.dataset.X.shape[1]
+        cls_id = getattr(self.dataset, "cls_token_id", None)
+        if cls_id is not None:
+            model_cls = {getattr(c, "cls_token_id", None) for c in configs}
+            if cls_id not in model_cls:
+                raise ValueError(f"the dataset packs documents that start with token {cls_id}, but the model derives no "
+                                 f"documents from it (model cls_token_id: {sorted(model_cls - {None}) or None}); build it "
+                                 f"with cls_token_id={cls_id}, or documents attend to each other")
+            docs = [n for row in self.dataset.doc_lengths for n in row]
+            self.log.info("Packed sequences.", dict(documents=len(docs), rows=len(self.dataset),
+                                                    docs_per_row=round(len(docs) / len(self.dataset), 2),
+                                                    mean_doc_len=round(sum(docs) / len(docs), 1),
+                                                    padding_fraction=round(1.0 - float(lengths.float().mean()) / seq_len, 4)))
+            return
         self.log.info("Padded sequences.", dict(min_len=int(lengths.min()), max_len=int(lengths.max()),
                                                 mean_len=round(float(lengths.float().mean()), 1),
                                                 padding_fraction=round(1.0 - float(lengths.float().mean()) / seq_len, 4)))
@@ -242,6 +259,9 @@ class Trainer:
                 restore_rng_state(self._resume_state["rng"])
         self.optimizer.zero_grad(set_to_none=True)
         t_start = time.time()
+        # non-pad tokens of the rows trained, summed on the device (no host synchronisation until the end)
+        tokens = torch.zeros((), dtype=torch.long, device=self.device) if self.count_pad_id is not None else None
+        rows = 0
         done = False
         tracer = self._make_tracer()
         if self.device.type == "cuda":
@@ -258,6 +278,9 @@ class Trainer:
                     if x.device != self.device:
                         x, y = x.to(self.device, non_blocking=True), y.to(self.device, non_blocking=True)
                     x, y = self._to_compute(x), self._to_compute(y)
+                    if tokens is not None:
+                        tokens += (x != self.count_pad_id).sum()
+                        rows += x.shape[0]
                     boundary = (step + 1) % accum == 0
                     with nvtx_range("train_step"):
                         self.step_fn(x, y, boundary=boundary)
@@ -303,6 +326,8 @@ class Trainer:
         if self.last_throughput:
             extra.update({"ms_per_step": round(self.last_throughput["ms_per_step"], 4),
                           "samples_per_s": round(self.last_throughput.get("samples_per_s", 0.0), 1)})
+            if tokens is not None and rows:          # samples/s times the mean non-pad tokens of the rows trained
+                extra["tokens_per_s"] = round(self.last_throughput.get("samples_per_s", 0.0) * float(tokens) / rows, 1)
         if hasattr(self.model, "ddp_stats"):
             extra["ddp"] = self.model.ddp_stats()
         log.info("Finished training.", dict(global_step=self.global_step, average_loss=total_loss / self.global_step,

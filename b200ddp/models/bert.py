@@ -2,7 +2,9 @@
 Every linear is a ``b200ddp.ops.Linear`` (wgmma GEMM with bias / bias+GELU epilogues), every
 LayerNorm the hand-written kernel, the loss the fused cross-entropy.  Attention on fixed-length rows uses torch's SDPA
 (library flash attention); with ``BertConfig.pad_token_id`` set, right-padded rows run on the native key-padding
-attention kernel (``ops.attention``), which reads Q / K / V straight out of the fused projection.  109.5 M encoder parameters as in the stock model
+attention kernel (``ops.attention``), which reads Q / K / V straight out of the fused projection; with
+``BertConfig.cls_token_id`` set as well, rows hold packed documents (each starting with that id) and run on the
+document-boundary kernel (``ops.packed_attention``), with position ids restarting per document.  109.5 M encoder parameters as in the stock model
 (199 tensors in the stock naming; 151 here because Q / K / V are one stored parameter) when built with ``with_mlm_head=False``."""
 from __future__ import annotations
 
@@ -12,7 +14,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops import LayerNorm, Linear, attention
+from ..ops import LayerNorm, Linear, attention, document_bounds, packed_attention
 
 
 @dataclass
@@ -29,6 +31,7 @@ class BertConfig:
     pad_vocab_to: int = 1          # MLM head pads to 64 so logits rows keep the 16-byte pitch TMA needs
     fp8: bool = False              # encoder linears (qkv, attn_out, ffn_in, ffn_out) on FP8 tensor cores; same parameters
     pad_token_id: int | None = None  # right-padded input: lengths = non-pad count per row, padded keys hidden (ops.attention)
+    cls_token_id: int | None = None  # packed input: a document starts at each such id (and at 0), attention stays inside it
 
     @property
     def padded_vocab(self) -> int:
@@ -45,12 +48,13 @@ class BertEmbeddings(nn.Module):
         self.LayerNorm = LayerNorm(c.hidden, eps=c.eps)
         self.dropout = nn.Dropout(c.dropout)
 
-    def forward(self, input_ids, token_type_ids=None):
+    def forward(self, input_ids, token_type_ids=None, position_ids=None):
         B, S = input_ids.shape
-        pos = torch.arange(S, device=input_ids.device)
+        pos = self.position_embeddings(torch.arange(S, device=input_ids.device))[None] if position_ids is None \
+            else self.position_embeddings(position_ids)
         if token_type_ids is None:
             token_type_ids = torch.zeros_like(input_ids)
-        x = self.word_embeddings(input_ids) + self.position_embeddings(pos)[None] + self.token_type_embeddings(token_type_ids)
+        x = self.word_embeddings(input_ids) + pos + self.token_type_embeddings(token_type_ids)
         return self.dropout(self.LayerNorm(x))
 
 
@@ -69,7 +73,7 @@ class BertLayer(nn.Module):
         self.ffn_norm = LayerNorm(c.hidden, eps=c.eps)
         self.dropout = nn.Dropout(c.dropout)
 
-    def forward(self, x, attn_mask=None, seq_lens=None):
+    def forward(self, x, attn_mask=None, seq_lens=None, bounds=None):
         B, S, H = x.shape
         hd = H // self.heads
 
@@ -77,8 +81,10 @@ class BertLayer(nn.Module):
             return t.view(B, S, self.heads, hd).transpose(1, 2)
 
         qkv = self.qkv(x)
-        if seq_lens is not None:
-            a = attention(qkv, seq_lens, self.heads)       # [B, S, H], the layout attn_out reads
+        if bounds is not None:
+            a = packed_attention(qkv, bounds, self.heads)  # [B, S, H], the layout attn_out reads
+        elif seq_lens is not None:
+            a = attention(qkv, seq_lens, self.heads)
         else:
             q, k, v = (split(t) for t in qkv.split(H, dim=-1))
             a = F.scaled_dot_product_attention(q, k, v, attn_mask=attn_mask)
@@ -104,17 +110,20 @@ class BertModel(nn.Module):
                 nn.init.zeros_(m.bias)
 
     def forward(self, input_ids, token_type_ids=None, attn_mask=None):
-        seq_lens = None
-        pad = self.config.pad_token_id
-        if pad is not None:
-            if attn_mask is not None:
-                raise ValueError("BertModel: pass either attn_mask or a config with pad_token_id, not both "
-                                 "(with pad_token_id the padding mask comes from input_ids)")
+        seq_lens = bounds = position_ids = None
+        pad, cls = self.config.pad_token_id, self.config.cls_token_id
+        if attn_mask is not None and (pad is not None or cls is not None):
+            raise ValueError("BertModel: pass either attn_mask or a config with pad_token_id / cls_token_id, not both "
+                             "(with those ids the mask comes from input_ids)")
+        if cls is not None:
+            # packed documents: boundaries and per-document positions, computed on the device (no host synchronisation)
+            bounds, position_ids = document_bounds(input_ids, cls, pad)
+        elif pad is not None:
             # right padding: the length is the non-pad count; computed on the device, so no host synchronisation
             seq_lens = (input_ids != pad).sum(1, dtype=torch.int32)
-        x = self.embeddings(input_ids, token_type_ids)
+        x = self.embeddings(input_ids, token_type_ids, position_ids)
         for layer in self.encoder:
-            x = layer(x, attn_mask, seq_lens)
+            x = layer(x, attn_mask, seq_lens, bounds)
         return x
 
 
@@ -186,10 +195,12 @@ def split_qkv_state_dict(state: dict) -> dict:
     return out
 
 
-def bert_base(with_mlm_head: bool = True, fp8: bool = False, pad_token_id: int | None = None) -> nn.Module:
+def bert_base(with_mlm_head: bool = True, fp8: bool = False, pad_token_id: int | None = None,
+              cls_token_id: int | None = None) -> nn.Module:
     """BERT-base; ``fp8=True`` puts the 48 encoder linears on FP8 tensor cores (embeddings, MLM transform and the tied
-    decoder stay bf16).  ``pad_token_id`` takes right-padded input (padded keys are hidden from attention).  The state
-    dict is the same either way."""
+    decoder stay bf16).  ``pad_token_id`` takes right-padded input (padded keys are hidden from attention);
+    ``cls_token_id`` takes packed documents, each starting with that id (attention stays inside a document and position
+    ids restart in each).  The state dict is the same either way."""
     if with_mlm_head:
-        return BertForMaskedLM(BertConfig(pad_vocab_to=64, fp8=fp8, pad_token_id=pad_token_id))
-    return BertModel(BertConfig(fp8=fp8, pad_token_id=pad_token_id))
+        return BertForMaskedLM(BertConfig(pad_vocab_to=64, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id))
+    return BertModel(BertConfig(fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id))

@@ -284,12 +284,16 @@ def _key_mask(seq_lens: torch.Tensor, S: int, device) -> torch.Tensor:
 def attention_reference(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> torch.Tensor:
     """softmax(Q K^T / sqrt(d)) V with the key-padding mask, in fp32 (fp64 stays fp64); a sequence of length 0 gives zeros.
     qkv [B, S, 3 * hidden] (query | key | value column blocks), returns [B, S, hidden] in qkv's dtype.  Differentiable."""
+    return _masked_attention_reference(qkv, _key_mask(seq_lens, qkv.shape[1], qkv.device)[:, None, None, :], heads)
+
+
+def _masked_attention_reference(qkv: torch.Tensor, keep: torch.Tensor, heads: int) -> torch.Tensor:
+    """Body of the references: ``keep`` is a bool mask broadcastable to [B, heads, S (query), S (key)]."""
     B, S, W = qkv.shape
     hidden = W // 3
     hd = hidden // heads
     ct = torch.promote_types(qkv.dtype, torch.float32)
     q, k, v = (t.to(ct).reshape(B, S, heads, hd).transpose(1, 2) for t in qkv.split(hidden, dim=-1))
-    keep = _key_mask(seq_lens, S, qkv.device)[:, None, None, :]
     scores = (q @ k.transpose(-1, -2)) * (1.0 / math.sqrt(hd))
     # a finite fill keeps an all-hidden row free of NaN; multiplying by the mask then zeroes it (and its gradients)
     p = torch.softmax(scores.masked_fill(~keep, torch.finfo(ct).min), dim=-1) * keep
@@ -297,6 +301,13 @@ def attention_reference(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -
 
 
 def _attention_check(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> None:
+    _qkv_check(qkv, heads)
+    B = qkv.shape[0]
+    if seq_lens.dim() != 1 or seq_lens.shape[0] != B or seq_lens.is_floating_point() or seq_lens.is_complex():
+        raise ValueError(f"attention needs integer seq_lens [B] = [{B}], got {seq_lens.dtype} {tuple(seq_lens.shape)}")
+
+
+def _qkv_check(qkv: torch.Tensor, heads: int) -> None:
     if qkv.dim() != 3 or qkv.shape[-1] % 3:
         raise ValueError(f"attention needs qkv [B, S, 3 * hidden], got {tuple(qkv.shape)}")
     B, S, W = qkv.shape
@@ -308,42 +319,44 @@ def _attention_check(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> N
         raise ValueError(f"attention on CUDA needs the sequence length to be a multiple of {ATTENTION_SEQ_MULTIPLE}, got {S}")
     if not qkv.is_contiguous():
         raise ValueError("attention on CUDA needs a contiguous qkv (the fused projection's output)")
-    if seq_lens.dim() != 1 or seq_lens.shape[0] != B or seq_lens.is_floating_point() or seq_lens.is_complex():
-        raise ValueError(f"attention needs integer seq_lens [B] = [{B}], got {seq_lens.dtype} {tuple(seq_lens.shape)}")
 
 
 class _Attention(torch.autograd.Function):
-    """Key-padding attention.  CUDA body: the sm_90a kernels (forward keeps the row log-sum-exp; backward is three
-    deterministic launches writing one dqkv tensor, the exact gradient the qkv linear consumes).  CPU body:
-    ``attention_reference`` (backward by recomputation through autograd)."""
+    """Key-padding (``packed=False``, mask = seq_lens [B]) or packed-document (``packed=True``, mask = bounds [B, S, 2])
+    attention.  CUDA body: the sm_90a kernels (forward keeps the row log-sum-exp; backward is three deterministic
+    launches writing one dqkv tensor, the exact gradient the qkv linear consumes).  CPU body: the matching reference
+    (backward by recomputation through autograd)."""
 
     @staticmethod
-    def forward(ctx, qkv, seq_lens, heads):
-        ctx.heads = heads
+    def forward(ctx, qkv, mask, heads, packed):
+        ctx.heads, ctx.packed = heads, packed
         if qkv.is_cuda:
             B, S, W = qkv.shape
-            lens = seq_lens.to(device=qkv.device, dtype=torch.int32).contiguous()
-            o, lse = _C().attention_fwd(qkv.view(B * S, W), lens, heads)
-            ctx.save_for_backward(qkv, o, lse, lens)
+            m = mask.to(device=qkv.device, dtype=torch.int32).contiguous()
+            fwd = _C().packed_attention_fwd if packed else _C().attention_fwd
+            o, lse = fwd(qkv.view(B * S, W), m, heads)
+            ctx.save_for_backward(qkv, o, lse, m)
             return o.view(B, S, W // 3)
-        ctx.save_for_backward(qkv, seq_lens)
-        return attention_reference(qkv, seq_lens, heads)
+        ctx.save_for_backward(qkv, mask)
+        return (packed_attention_reference if packed else attention_reference)(qkv, mask, heads)
 
     @staticmethod
     def backward(ctx, dy):
         if dy.is_cuda:
-            qkv, o, lse, lens = ctx.saved_tensors
+            qkv, o, lse, m = ctx.saved_tensors
             B, S, W = qkv.shape
             do = dy.reshape(B * S, W // 3).to(torch.bfloat16).contiguous()
             if do.data_ptr() % 16:                                # the kernels read dO in 16-byte vectors / TMA boxes
                 do = do.clone()
-            dqkv = _C().attention_bwd(do, qkv.view(B * S, W), o, lse, lens, ctx.heads)
-            return dqkv.view(B, S, W), None, None
-        qkv, seq_lens = ctx.saved_tensors
+            bwd = _C().packed_attention_bwd if ctx.packed else _C().attention_bwd
+            dqkv = bwd(do, qkv.view(B * S, W), o, lse, m, ctx.heads)
+            return dqkv.view(B, S, W), None, None, None
+        qkv, mask = ctx.saved_tensors
+        ref = packed_attention_reference if ctx.packed else attention_reference
         with torch.enable_grad():
             x = qkv.detach().requires_grad_(True)
-            (g,) = torch.autograd.grad(attention_reference(x, seq_lens, ctx.heads), x, dy)
-        return g, None, None
+            (g,) = torch.autograd.grad(ref(x, mask, ctx.heads), x, dy)
+        return g, None, None, None
 
 
 def attention(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> torch.Tensor:
@@ -353,7 +366,65 @@ def attention(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> torch.Te
     ``ValueError``; lengths stay on the device (no host synchronisation, CUDA-graph safe)."""
     if qkv.is_cuda:
         _attention_check(qkv, seq_lens, heads)
-    return _Attention.apply(qkv, seq_lens, heads)
+    return _Attention.apply(qkv, seq_lens, heads, False)
+
+
+# ------------------------------------------------------------------------------------------------
+# Packed-document attention (csrc/attention.cu, segment mode): several documents per row, block-diagonal mask
+# ------------------------------------------------------------------------------------------------
+def document_bounds(input_ids: torch.Tensor, cls_token_id: int, pad_token_id: Optional[int]):
+    """Documents of packed rows, on the device with no host synchronisation (CUDA-graph safe).
+
+    input_ids [B, S].  A row's length is its non-pad count (S when ``pad_token_id`` is None); positions at or beyond it
+    are padding, whatever their id.  A document starts at position 0 and at every ``cls_token_id`` below the length, and
+    runs to the next start or the length.  Returns ``(bounds, position_ids)``: bounds int32 [B, S, 2] holds each
+    position's document as (start, end), (0, 0) for padding; position_ids long [B, S] restart at 0 in each document and
+    are 0 for padding."""
+    B, S = input_ids.shape
+    pos = torch.arange(S, device=input_ids.device).expand(B, S)
+    if pad_token_id is None:
+        lens = torch.full((B, 1), S, device=input_ids.device, dtype=torch.long)
+    else:
+        lens = (input_ids != pad_token_id).sum(1, keepdim=True)
+    valid = pos < lens
+    is_start = ((input_ids == cls_token_id) | (pos == 0)) & valid
+    start = torch.where(is_start, pos, 0).cummax(1).values                   # the last start at or before each position
+    nxt = torch.where(is_start, pos, S)[:, 1:]                                  # the first start after each position
+    nxt = torch.cat([nxt, torch.full((B, 1), S, device=pos.device, dtype=pos.dtype)], 1).flip(1).cummin(1).values.flip(1)
+    end = torch.minimum(nxt, lens)
+    bounds = torch.stack([torch.where(valid, start, 0), torch.where(valid, end, 0)], -1).to(torch.int32)
+    return bounds, torch.where(valid, pos - start, 0)
+
+
+def _bounds_mask(bounds: torch.Tensor, S: int, device) -> torch.Tensor:
+    """[B, S, S] bool: query i sees key j iff start[i] <= j < end[i] (start clamped to [0, S], end to [start, S], like
+    the kernel)."""
+    b = bounds.to(device=device, dtype=torch.long).reshape(-1, S, 2)
+    start = b[..., 0].clamp(0, S)
+    end = torch.maximum(b[..., 1].clamp(max=S), start)
+    j = torch.arange(S, device=device)
+    return (j >= start[..., None]) & (j < end[..., None])
+
+
+def packed_attention_reference(qkv: torch.Tensor, bounds: torch.Tensor, heads: int) -> torch.Tensor:
+    """softmax(Q K^T / sqrt(d)) V where query i sees key j of its row iff bounds[b, i, 0] <= j < bounds[b, i, 1], in
+    fp32 (fp64 stays fp64); a row that sees no key gives zeros.  qkv [B, S, 3 * hidden], bounds integer [B, S, 2];
+    returns [B, S, hidden] in qkv's dtype.  Differentiable."""
+    return _masked_attention_reference(qkv, _bounds_mask(bounds, qkv.shape[1], qkv.device)[:, None], heads)
+
+
+def packed_attention(qkv: torch.Tensor, bounds: torch.Tensor, heads: int) -> torch.Tensor:
+    """Multi-head attention over packed documents: qkv [B, S, 3 * hidden] (the fused projection's output), bounds
+    integer [B, S, 2] (``document_bounds``): query i of a row sees key j of the same row iff start[i] <= j < end[i].
+    Rows with start == end (padding) give zeros and get zero gradients.  Returns [B, S, hidden].  On CUDA: bf16, head
+    dim 64, S % 128 == 0 and contiguous qkv, else ``ValueError``; bounds stay on the device (CUDA-graph safe)."""
+    if qkv.is_cuda:
+        _qkv_check(qkv, heads)
+        B, S = qkv.shape[:2]
+        if tuple(bounds.shape) != (B, S, 2) or bounds.is_floating_point() or bounds.is_complex():
+            raise ValueError(f"packed attention needs integer bounds [B, S, 2] = [{B}, {S}, 2], got {bounds.dtype} "
+                             f"{tuple(bounds.shape)}")
+    return _Attention.apply(qkv, bounds, heads, True)
 
 
 # ------------------------------------------------------------------------------------------------

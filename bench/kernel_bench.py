@@ -205,6 +205,37 @@ def main():
             record(f"attention bwd {label} B{B} S{S} H{H}", timeit(lambda: C.attention_bwd(dout, qkv, o, lse, lt, H), args.iters),
                    flops=2.5 * fwd_flops, lib_ms=lib, note=f"lib = {lib_name} backward into qkv")
             del x, q, k, v, y
+        # Packed documents: B evenly spaced rows of the training set's packing (documents U[128, 512], first-fit
+        # decreasing, which fills its first rows with the longest documents alone), native segment-mode kernels against
+        # SDPA with the dense block-diagonal boolean mask [B, 1, S, S].  FLOPs count only the block-diagonal: forward
+        # 4 sum_docs len^2 d H, backward 2.5x that.
+        from b200ddp.data import SyntheticTokens
+        from b200ddp.ops import document_bounds
+        packed = SyntheticTokens(seq_len=S, min_len=128, pack=True)
+        rows = torch.linspace(0, len(packed) - 1, B).long().tolist()
+        bounds, _ = document_bounds(packed.X[rows].to(dev), packed.cls_token_id, packed.pad_token_id)
+        docs = [n for r in rows for n in packed.doc_lengths[r]]
+        fwd_flops = 4.0 * sum(n * n for n in docs) * d * H
+        label = f"packed {len(docs)} docs U[128,512]"
+        x = qkv.view(B, S, 3 * H * d).detach().clone().requires_grad_(True)
+        q, k, v = (t.reshape(B, S, H, d).transpose(1, 2) for t in x.split(H * d, dim=-1))
+        j = torch.arange(S, device=dev)
+        mask = ((j >= bounds[..., :1]) & (j < bounds[..., 1:]))[:, None]
+        mask |= torch.eye(S, dtype=torch.bool, device=dev)          # tail padding rows: their own key, not a NaN row
+
+        def sdpa():
+            return F.scaled_dot_product_attention(q, k, v, attn_mask=mask).transpose(1, 2).reshape(B, S, H * d)
+        lib = timeit(lambda: sdpa().detach(), args.iters)
+        record(f"attention fwd {label} B{B} S{S} H{H}", timeit(lambda: C.packed_attention_fwd(qkv, bounds, H), args.iters),
+               flops=fwd_flops, lib_ms=lib, note="lib = SDPA block-diagonal bool mask + output transpose")
+        o, lse = C.packed_attention_fwd(qkv, bounds, H)
+        y = sdpa()
+        dy = dout.view(B, S, H * d)
+        lib = timeit(lambda: torch.autograd.grad(y, x, dy, retain_graph=True), args.iters)
+        record(f"attention bwd {label} B{B} S{S} H{H}",
+               timeit(lambda: C.packed_attention_bwd(dout, qkv, o, lse, bounds, H), args.iters),
+               flops=2.5 * fwd_flops, lib_ms=lib, note="lib = SDPA block-diagonal bool mask backward into qkv")
+        del x, q, k, v, y
 
     if "conv" in want:
         import torch.nn.functional as F
