@@ -5,7 +5,7 @@
 //   o    bf16 [B*S, H*64]     written in the layout the output projection reads (no transpose)
 //   lse  fp32 [B, H, S]       natural-log row log-sum-exp of the scaled scores (-inf for a sequence of length 0)
 //
-// Two mask modes, chosen at compile time (template parameter kMode):
+// Three mask modes, chosen at compile time (template parameter kMode):
 //   kKeyPadding  seq_lens int32 [B]: key j of sequence b is visible iff j < seq_lens[b] (clamped to [0, S] here: the host
 //                cannot validate device lengths without a synchronisation).  Every query row is computed, padded ones
 //                included, so every row equals softmax attention over the visible keys; a sequence of length 0 gets zero
@@ -15,6 +15,12 @@
 //                gets zero output, lse = -inf and zero gradients.  Each CTA visits only the tiles inside the union of its
 //                128 rows' intervals; dK / dV mask with the key rows' own bounds, which is the same test as the query's for
 //                a block-diagonal mask.
+//   kCausal      the same bounds, causal inside each document: query i sees key j iff start[i] <= j <= i and j < end[i].
+//                Both sides are still intervals: query i sees keys [start_i, min(end_i, i + 1)), key k is seen by
+//                queries [max(start_k, k), end_k), so the forward and dQ stop at the diagonal tile and dK / dV start at
+//                it.  Padding rows behave as in kSegment; a row inside its document always sees itself.  Tile work
+//                grows with the query tile (forward, dQ) and shrinks with the key tile (dK / dV), so the grid is walked
+//                heaviest tiles first.
 //
 // Each kernel has one TMA producer warp (warp 0; warps 1-3 idle) and two consumer warpgroups (warps 4-7, 8-11) that own
 // 64 rows each.  All tiles are 64-row boxes of one 2-D tensor map over qkv (or dO), 128B-swizzled, so a head's 64
@@ -67,6 +73,7 @@ constexpr int kBwdSmem = 1024 + 4 * kBoxBytes + kBwdStages * 2 * kBoxBytes + 256
 
 constexpr int kKeyPadding = 0;
 constexpr int kSegment = 1;
+constexpr int kCausal = 2;
 
 __device__ __forceinline__ int clamped_len(const int* lens, int b, int S) {
   const int n = __ldg(lens + b);
@@ -78,6 +85,18 @@ __device__ __forceinline__ int2 row_bounds(const int* bounds, size_t row, int S)
   const int s = min(max(v.x, 0), S);
   return make_int2(s, min(max(v.y, s), S));
 }
+// The interval of global row `row` (position `pos` in its sequence) as a query (the keys it sees, kKeySide = false) or as
+// a key (the queries that see it, kKeySide = true).  kSegment: the row's bounds either way.  kCausal: the query side
+// stops after `pos`, the key side starts at `pos`; both stay non-empty-or-(x == y) so `inside` and the masks hold.
+template <int kMode, bool kKeySide>
+__device__ __forceinline__ int2 mask_interval(const int* bounds, size_t row, int pos, int S) {
+  int2 r = row_bounds(bounds, row, S);
+  if constexpr (kMode == kCausal) {
+    if constexpr (kKeySide) r.x = min(max(r.x, pos), r.y);
+    else r.y = max(min(r.y, pos + 1), r.x);
+  }
+  return r;
+}
 __device__ __forceinline__ bool inside(int j, int2 r) { return (unsigned)(j - r.x) < (unsigned)(r.y - r.x); }
 // A fragment thread owns columns 8 j + e (j < 8, e < 2) of a 64-wide tile, counted from its first column.  Bit 2 j + e
 // is set where that column lies in [lo, hi).  The columns are increasing in the bit index, so the set bits are the range
@@ -88,12 +107,13 @@ __device__ __forceinline__ uint32_t frag_mask16(int lo, int hi) {
   const int nlo = 2 * (lo >> 3) + min(lo & 7, 2), nhi = 2 * (hi >> 3) + min(hi & 7, 2);
   return ((1u << nhi) - 1u) & ~((1u << nlo) - 1u);
 }
-// [lo, hi): the union of the intervals of rows row0 .. row0 + 127 (lo >= hi when all are empty).  Every thread of the
-// block calls it (it holds a __syncthreads); scratch is 8 ints of shared memory.
-__device__ __forceinline__ int2 cta_range(const int* bounds, size_t row0, int S, int* scratch) {
+// [lo, hi): the union of the intervals (mask_interval) of rows row0 .. row0 + 127, at positions pos0 .. pos0 + 127 (lo >= hi
+// when all are empty).  Every thread of the block calls it (it holds a __syncthreads); scratch is 8 ints of shared memory.
+template <int kMode, bool kKeySide>
+__device__ __forceinline__ int2 cta_range(const int* bounds, size_t row0, int pos0, int S, int* scratch) {
   const int t = threadIdx.x;
   if (t < 128) {
-    const int2 r = row_bounds(bounds, row0 + t, S);
+    const int2 r = mask_interval<kMode, kKeySide>(bounds, row0 + t, pos0 + t, S);
     const bool empty = r.x >= r.y;
     const int lo = __reduce_min_sync(0xffffffffu, empty ? S : r.x);
     const int hi = __reduce_max_sync(0xffffffffu, empty ? 0 : r.y);
@@ -109,6 +129,20 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 }
 __device__ __forceinline__ uint8_t* align1024(uint8_t* p) {
   return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~uintptr_t(1023));
+}
+// (tile, head, batch) of this CTA.  kCausal walks the grid heaviest tiles first: every (head, batch) pair's last query
+// tile (kKeySide = false: the forward and dQ, whose work grows with the tile) or first key tile (dK / dV) before any
+// pair's next one, so the light tiles fill the tail of the launch.
+template <int kMode, bool kKeySide>
+__device__ __forceinline__ int3 tile_coords() {
+  if constexpr (kMode == kCausal) {
+    const int pairs = gridDim.y * gridDim.z;
+    const int id = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
+    const int step = id / pairs, pair = id - step * pairs;
+    return make_int3(kKeySide ? step : (int)gridDim.x - 1 - step, pair % (int)gridDim.y, pair / (int)gridDim.y);
+  } else {
+    return make_int3(blockIdx.x, blockIdx.y, blockIdx.z);
+  }
 }
 __device__ __forceinline__ uint64_t desc_k(uint32_t addr) { return make_smem_desc(addr, 16, kSbo); }
 __device__ __forceinline__ uint64_t desc_mn(uint32_t addr) { return make_smem_desc(addr, kLboMN, kSbo); }
@@ -137,7 +171,7 @@ __device__ __forceinline__ void store_frag(const float (&acc)[32], float scale0,
 }
 
 // ============================================== forward ==============================================================
-// mask: seq_lens [B] (kKeyPadding) or bounds [B*S, 2] (kSegment)
+// mask: seq_lens [B] (kKeyPadding) or bounds [B*S, 2] (kSegment, kCausal)
 template <int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restrict__ mask, int S, int H,
@@ -150,7 +184,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
   uint64_t* full_bar = q_bar + 1;
   uint64_t* empty_bar = full_bar + kFwdStages;
 
-  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int3 tc = tile_coords<kMode, false>();
+  const int qt = tc.x, h = tc.y, b = tc.z;
   const int HD = H * kHd;
   const size_t seq_row = (size_t)b * S;
   int len = 0, kt0 = 0, n_kt;                                   // key tiles kt0 .. kt0 + n_kt - 1
@@ -158,7 +193,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
     len = clamped_len(mask, b, S);
     n_kt = (len + 127) / 128;
   } else {
-    const int2 r = cta_range(mask, seq_row + qt * 128, S, reinterpret_cast<int*>(empty_bar + kFwdStages));
+    const int2 r = cta_range<kMode, false>(mask, seq_row + qt * 128, qt * 128, S, reinterpret_cast<int*>(empty_bar + kFwdStages));
     kt0 = r.x / 128;
     n_kt = r.x < r.y ? (r.y + 127) / 128 - kt0 : 0;
   }
@@ -203,10 +238,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
     const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);         // this thread's rows: r0 and r0 + 8 of the warpgroup's 64
     const int c0 = 2 * (lane & 3);
     const uint32_t q_addr = smem_u32(sq + wg * kBoxBytes);
-    int2 rb0, rb1;                                              // kSegment: the intervals of this thread's two rows
-    if constexpr (kMode == kSegment) {
-      rb0 = row_bounds(mask, seq_row + qt * 128 + wg * 64 + r0, S);
-      rb1 = row_bounds(mask, seq_row + qt * 128 + wg * 64 + r0 + 8, S);
+    int2 rb0, rb1;                                              // kSegment / kCausal: the intervals of this thread's two rows
+    if constexpr (kMode != kKeyPadding) {
+      rb0 = mask_interval<kMode, false>(mask, seq_row + qt * 128 + wg * 64 + r0, qt * 128 + wg * 64 + r0, S);
+      rb1 = mask_interval<kMode, false>(mask, seq_row + qt * 128 + wg * 64 + r0 + 8, qt * 128 + wg * 64 + r0 + 8, S);
     }
     float acc[32];
 #pragma unroll
@@ -403,7 +438,7 @@ __device__ __forceinline__ void bwd_produce(const BwdSmem& L, const CUtensorMap*
 }
 
 // dK, dV for one tile of 128 keys.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries: all S / 64 of them (kKeyPadding),
-// or those inside the union of the key rows' intervals (kSegment).
+// or those inside the union of the key rows' intervals (kSegment, kCausal).
 template <int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
@@ -411,7 +446,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
                      __nv_bfloat16* __restrict__ dqkv) {
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
-  const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int3 tc = tile_coords<kMode, true>();
+  const int kt = tc.x, h = tc.y, b = tc.z;
   const int HD = H * kHd;
   const size_t pitch = (size_t)3 * HD;
   const size_t seq_row = (size_t)b * S;
@@ -421,7 +457,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
     len = clamped_len(mask, b, S);
     hidden = kt * 128 >= len;
   } else {
-    const int2 r = cta_range(mask, seq_row + kt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
+    const int2 r = cta_range<kMode, true>(mask, seq_row + kt * 128, kt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
     hidden = r.x >= r.y;
     qt0 = r.x / 64;
     n_qt = (r.y + 63) / 64 - qt0;
@@ -458,11 +494,12 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
     int stage = 0;
     uint32_t phase = 0;
     for (int qt = qt0; qt < qt0 + n_qt; ++qt) {
-      // kSegment: the key rows' intervals as one bit mask over this thread's 16 query columns (bits 0-15: row key,
-      // 16-31: row key + 8), so the mask costs one register while the accumulators are live
+      // kSegment / kCausal: the key rows' intervals as one bit mask over this thread's 16 query columns (bits 0-15: row
+      // key, 16-31: row key + 8), so the mask costs one register while the accumulators are live
       uint32_t vis = 0;
-      if constexpr (kMode == kSegment) {
-        const int2 kb0 = row_bounds(mask, seq_row + key, S), kb1 = row_bounds(mask, seq_row + key + 8, S);
+      if constexpr (kMode != kKeyPadding) {
+        const int2 kb0 = mask_interval<kMode, true>(mask, seq_row + key, key, S);
+        const int2 kb1 = mask_interval<kMode, true>(mask, seq_row + key + 8, key + 8, S);
         const int q0 = qt * 64 + c0;
         vis = frag_mask16(kb0.x - q0, kb0.y - q0) | (frag_mask16(kb1.x - q0, kb1.y - q0) << 16);
       }
@@ -481,7 +518,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
         const float2 lq = *reinterpret_cast<const float2*>(lse_bh + q);
         const float2 dq = *reinterpret_cast<const float2*>(D_bh + q);
         float l0 = lq.x * kLog2e, l1 = lq.y * kLog2e;
-        if constexpr (kMode == kSegment) {                      // a query that saw no key (lse = -inf) gets P = 0, even
+        if constexpr (kMode != kKeyPadding) {                   // a query that saw no key (lse = -inf) gets P = 0, even
           l0 = lq.x == -INFINITY ? INFINITY : l0;               // where malformed bounds put it inside a key's interval
           l1 = lq.y == -INFINITY ? INFINITY : l1;
         }
@@ -520,7 +557,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
 }
 
 // dQ for one tile of 128 queries.  Fixed: Q, dO.  Ring: (K, V) tiles of 64 keys below the length (kKeyPadding), or
-// inside the union of the query rows' intervals (kSegment).
+// inside the union of the query rows' intervals (kSegment, kCausal).
 template <int kMode>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
@@ -528,7 +565,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
                    __nv_bfloat16* __restrict__ dqkv) {
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
-  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int3 tc = tile_coords<kMode, false>();
+  const int qt = tc.x, h = tc.y, b = tc.z;
   const int HD = H * kHd;
   const size_t pitch = (size_t)3 * HD;
   const size_t seq_row = (size_t)b * S;
@@ -538,7 +576,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
     len = clamped_len(mask, b, S);
     hidden = len == 0;
   } else {
-    const int2 r = cta_range(mask, seq_row + qt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
+    const int2 r = cta_range<kMode, false>(mask, seq_row + qt * 128, qt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
     hidden = r.x >= r.y;
     kt0 = r.x / 64;
     kt_end = (r.y + 63) / 64;
@@ -564,10 +602,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
     const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
     const int c0 = 2 * (lane & 3);
     const int row = qt * 128 + wg * 64 + r0;
-    int2 qb0, qb1;                                              // kSegment: the intervals of query rows row, row + 8
-    if constexpr (kMode == kSegment) {
-      qb0 = row_bounds(mask, seq_row + row, S);
-      qb1 = row_bounds(mask, seq_row + row + 8, S);
+    int2 qb0, qb1;                                              // kSegment / kCausal: the intervals of query rows row, row + 8
+    if constexpr (kMode != kKeyPadding) {
+      qb0 = mask_interval<kMode, false>(mask, seq_row + row, row, S);
+      qb1 = mask_interval<kMode, false>(mask, seq_row + row + 8, row + 8, S);
     }
     const uint32_t q_addr = smem_u32(L.fixed0 + wg * kBoxBytes), do_addr = smem_u32(L.fixed1 + wg * kBoxBytes);
     const size_t bh = ((size_t)b * H + h) * S;
@@ -685,6 +723,15 @@ void launch_packed_attention_fwd(const void* qkv, const int* bounds, int B, int 
 void launch_packed_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
                                  int S, int heads, float* dsum, void* dqkv, cudaStream_t s) {
   attention_bwd<kSegment>("packed_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s);
+}
+
+void launch_causal_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
+  attention_fwd<kCausal>("causal_attention_fwd", qkv, bounds, B, S, heads, o, lse, s);
+}
+
+void launch_causal_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                 int S, int heads, float* dsum, void* dqkv, cudaStream_t s) {
+  attention_bwd<kCausal>("causal_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s);
 }
 
 }  // namespace b200

@@ -356,22 +356,23 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(loss, dlogits);
   });
 
-  m.def("gelu_fwd", [](at::Tensor pre) {
+  // tanh = false: the erf form; true: the tanh approximation
+  m.def("gelu_fwd", [](at::Tensor pre, bool tanh) {
     check_cuda(pre, "pre");
     TORCH_CHECK(pre.is_contiguous(), "gelu_fwd: contiguous input");
     c10::cuda::CUDAGuard guard(pre.device());
     at::Tensor out = at::empty_like(pre);
-    launch_gelu(pre.data_ptr(), nullptr, out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), false, cur_stream());
+    launch_gelu(pre.data_ptr(), nullptr, out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), false, cur_stream(), tanh);
     return out;
-  });
-  m.def("gelu_bwd", [](at::Tensor dy, at::Tensor pre) {
+  }, py::arg("pre"), py::arg("tanh") = false);
+  m.def("gelu_bwd", [](at::Tensor dy, at::Tensor pre, bool tanh) {
     check_cuda(pre, "pre");
     TORCH_CHECK(pre.is_contiguous() && dy.is_contiguous() && dy.dtype() == pre.dtype() && dy.numel() == pre.numel(), "gelu_bwd: matching contiguous tensors");
     c10::cuda::CUDAGuard guard(pre.device());
     at::Tensor out = at::empty_like(pre);
-    launch_gelu(pre.data_ptr(), dy.data_ptr(), out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), true, cur_stream());
+    launch_gelu(pre.data_ptr(), dy.data_ptr(), out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), true, cur_stream(), tanh);
     return out;
-  });
+  }, py::arg("dy"), py::arg("pre"), py::arg("tanh") = false);
 
   // ---- layer norm -------------------------------------------------------------------------------
   m.def("layernorm_fwd", [](at::Tensor x, at::Tensor gamma, at::Tensor beta, double eps) {
@@ -648,6 +649,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                                          int heads, c10::optional<at::Tensor> dqkv_out) {
     const int B = packed_check(qkv, bounds, heads, "packed_attention_bwd");
     return attn_bwd(&launch_packed_attention_bwd, "packed_attention_bwd", dout, qkv, o, lse, bounds, B, heads, dqkv_out);
+  }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("dqkv") = py::none());
+  // causal documents: the same bounds and checks as the packed pair
+  m.def("causal_attention_fwd", [packed_check, attn_fwd](at::Tensor qkv, at::Tensor bounds, int heads, c10::optional<at::Tensor> o_out,
+                                                         c10::optional<at::Tensor> lse_out) {
+    const int B = packed_check(qkv, bounds, heads, "causal_attention_fwd");
+    return attn_fwd(&launch_causal_attention_fwd, "causal_attention_fwd", qkv, bounds, B, heads, o_out, lse_out);
+  }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
+  m.def("causal_attention_bwd", [packed_check, attn_bwd](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds,
+                                                         int heads, c10::optional<at::Tensor> dqkv_out) {
+    const int B = packed_check(qkv, bounds, heads, "causal_attention_bwd");
+    return attn_bwd(&launch_causal_attention_bwd, "causal_attention_bwd", dout, qkv, o, lse, bounds, B, heads, dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("dqkv") = py::none());
   m.def("gemm_supported", &gemm_shape_supported);
   m.def("set_gemm_cta_mode", &set_gemm_cta_mode);

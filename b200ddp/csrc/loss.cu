@@ -256,8 +256,9 @@ void launch_xent_fwd_bwd(const void* logits, const long long* targets, DType dt,
 }  // namespace b200
 
 // ---------------------------------------------------------------------------------------------------------
-// GELU (erf form) forward and backward as single vectorised passes.  The stock autograd formula for the backward
-// (cast to fp32, erf, exp, three multiplies, cast back) is ~8 launches over a [tokens, 3072] tensor per BERT layer.
+// GELU forward and backward as single vectorised passes, erf form (BERT) or tanh approximation (GPT-2).  The stock
+// autograd formula for the backward (cast to fp32, erf, exp, three multiplies, cast back) is ~8 launches over a
+// [tokens, 3072] tensor per BERT layer.
 namespace b200 {
 namespace {
 
@@ -267,8 +268,24 @@ __device__ __forceinline__ float gelu_grad_f(float x) {
   const float pdf = 0.3989422804014327f * __expf(-0.5f * x * x);
   return cdf + x * pdf;
 }
+// tanh approximation: gelu(x) = 0.5 x (1 + t), t = tanh(u), u = sqrt(2 / pi) (x + 0.044715 x^3);
+// gelu'(x) = 0.5 (1 + t) + 0.5 x (1 - t^2) sqrt(2 / pi) (1 + 3 * 0.044715 x^2)
+constexpr float kSqrt2OverPi = 0.7978845608028654f;
+constexpr float kGeluTanhC = 0.044715f;
+__device__ __forceinline__ float gelu_tanh_f(float x) {
+  return 0.5f * x * (1.f + tanhf(kSqrt2OverPi * (x + kGeluTanhC * x * x * x)));
+}
+__device__ __forceinline__ float gelu_tanh_grad_f(float x) {
+  const float t = tanhf(kSqrt2OverPi * (x + kGeluTanhC * x * x * x));
+  return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * kSqrt2OverPi * (1.f + 3.f * kGeluTanhC * x * x);
+}
+template <bool BWD, bool TANH>
+__device__ __forceinline__ float gelu_op(float x, float g) {
+  if constexpr (TANH) return BWD ? g * gelu_tanh_grad_f(x) : gelu_tanh_f(x);
+  else return BWD ? g * gelu_grad_f(x) : gelu_f(x);
+}
 
-template <typename T, bool BWD>
+template <typename T, bool BWD, bool TANH>
 __global__ void __launch_bounds__(kLossThreads) gelu_kernel(const T* __restrict__ pre, const T* __restrict__ dy, T* __restrict__ out, size_t n) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -281,31 +298,37 @@ __global__ void __launch_bounds__(kLossThreads) gelu_kernel(const T* __restrict_
       loss_load8<T>(pre + v * 8, a);
       if (BWD) loss_load8<T>(dy + v * 8, g);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) a[i] = BWD ? g[i] * gelu_grad_f(a[i]) : gelu_f(a[i]);
+      for (int i = 0; i < 8; ++i) a[i] = gelu_op<BWD, TANH>(a[i], g[i]);
       loss_store8<T>(out + v * 8, a);
     }
     done = nvec * 8;
   }
   for (size_t i = done + tid; i < n; i += stride) {
     const float x = to_f32<T>(pre[i]);
-    out[i] = from_f32<T>(BWD ? to_f32<T>(dy[i]) * gelu_grad_f(x) : gelu_f(x));
+    out[i] = from_f32<T>(gelu_op<BWD, TANH>(x, BWD ? to_f32<T>(dy[i]) : 0.f));
   }
 }
 
 }  // namespace
 
-void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s) {
+template <bool TANH>
+void gelu_dispatch(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, int blocks, cudaStream_t s) {
+  if (dt == DType::BF16) {
+    if (backward) gelu_kernel<__nv_bfloat16, true, TANH><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, (const __nv_bfloat16*)dy, (__nv_bfloat16*)out, n);
+    else gelu_kernel<__nv_bfloat16, false, TANH><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, nullptr, (__nv_bfloat16*)out, n);
+  } else {
+    if (backward) gelu_kernel<float, true, TANH><<<blocks, kLossThreads, 0, s>>>((const float*)pre, (const float*)dy, (float*)out, n);
+    else gelu_kernel<float, false, TANH><<<blocks, kLossThreads, 0, s>>>((const float*)pre, nullptr, (float*)out, n);
+  }
+}
+
+void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s, bool tanh) {
   size_t b = (n / 8 + kLossThreads - 1) / kLossThreads;
   if (b < 1) b = 1;
   if (b > (size_t)16 * kNumSMs) b = (size_t)16 * kNumSMs;
   const int blocks = (int)b;
-  if (dt == DType::BF16) {
-    if (backward) gelu_kernel<__nv_bfloat16, true><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, (const __nv_bfloat16*)dy, (__nv_bfloat16*)out, n);
-    else gelu_kernel<__nv_bfloat16, false><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, nullptr, (__nv_bfloat16*)out, n);
-  } else {
-    if (backward) gelu_kernel<float, true><<<blocks, kLossThreads, 0, s>>>((const float*)pre, (const float*)dy, (float*)out, n);
-    else gelu_kernel<float, false><<<blocks, kLossThreads, 0, s>>>((const float*)pre, nullptr, (float*)out, n);
-  }
+  if (tanh) gelu_dispatch<true>(pre, dy, out, dt, n, backward, blocks, s);
+  else gelu_dispatch<false>(pre, dy, out, dt, n, backward, blocks, s);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 

@@ -62,8 +62,9 @@ void launch_xent_fwd_bwd(const void* logits, const long long* targets, DType dt,
                          long long ignore_index, float gscale, float* row_loss /*[rows+1]*/, float* loss /*1*/,
                          void* dlogits, cudaStream_t s);
 
-// GELU (erf) forward: out = gelu(pre); backward: out = dy * gelu'(pre).  One vectorised pass each (loss.cu).
-void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s);
+// GELU forward: out = gelu(pre); backward: out = dy * gelu'(pre).  One vectorised pass each (loss.cu).  The erf form, or
+// with `tanh` the tanh approximation 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3))) (GPT-2's MLP).
+void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s, bool tanh = false);
 
 // ---------------- layer norm (layernorm.cu) -----------------------------------------------------
 void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, DType dt, int rows, int cols,
@@ -96,6 +97,11 @@ void launch_attention_bwd(const void* dout, const void* qkv, const void* o, cons
 // start == end gets zero output, lse = -inf and zero gradients.  Same shapes, outputs and workspace as above.
 void launch_packed_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s);
 void launch_packed_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                 int S, int heads, float* dsum, void* dqkv, cudaStream_t s);
+// Causal documents: the same bounds, and query i also sees no key after itself: key j iff start[i] <= j <= i and
+// j < end[i].  Padding rows as above; same shapes, outputs and workspace.
+void launch_causal_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s);
+void launch_causal_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
                                  int S, int heads, float* dsum, void* dqkv, cudaStream_t s);
 
 // ---------------- small linears on CUDA cores (linear_small.cu) ------------------------------

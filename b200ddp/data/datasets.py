@@ -79,13 +79,19 @@ class SyntheticTokens(Dataset):
     defaults to ``seq_len``), each starting with ``CLS_ID`` and holding tokens from [1, vocab) other than ``CLS_ID``,
     are placed into rows of ``seq_len`` by first-fit decreasing (longest first, ties in document order).  Row tails are
     ``PAD_ID`` labelled -100, the ``CLS_ID`` tokens are labelled -100 too.  ``lengths`` then holds each row's filled
-    length, ``cls_token_id`` is ``CLS_ID``, and ``doc_ids`` / ``doc_lengths`` list each row's documents (in row order)."""
+    length, ``cls_token_id`` is ``CLS_ID``, and ``doc_ids`` / ``doc_lengths`` list each row's documents (in row order).
+
+    ``causal=True`` gives causal-LM rows (GPT) in the same three layouts: within a document ``labels[t] = ids[t + 1]``,
+    and each document's last token and the padding are labelled -100.  Tokens come from [1, vocab); packed documents
+    start with ``BOS_ID`` instead of ``CLS_ID`` (and hold no other ``BOS_ID``), and ``bos_token_id`` is set instead of
+    ``cls_token_id``."""
 
     PAD_ID = 0
     CLS_ID = 101                   # [CLS] in the BERT vocabulary
+    BOS_ID = 50256                 # <|endoftext|> in the GPT-2 vocabulary, which starts each GPT-2 document
 
     def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 30522, mask_prob: float = 0.15, seed: int = 1234,
-                 min_len: int | None = None, pack: bool = False):
+                 min_len: int | None = None, pack: bool = False, causal: bool = False):
         if min_len is not None and not 1 <= min_len <= seq_len:
             raise ValueError(f"SyntheticTokens: min_len must lie in [1, seq_len = {seq_len}], got {min_len}")
         g = torch.Generator().manual_seed(seed)
@@ -93,9 +99,13 @@ class SyntheticTokens(Dataset):
         self.lengths = None
         self.pad_token_id = None
         self.cls_token_id = None
+        self.bos_token_id = None
         self.doc_ids = self.doc_lengths = None
         if pack:
-            self._pack(g, seq_len, vocab, mask_prob, seq_len if min_len is None else min_len)
+            self._pack(g, seq_len, vocab, mask_prob, seq_len if min_len is None else min_len, causal)
+            return
+        if causal:
+            self._causal_rows(g, seq_len, vocab, min_len)
             return
         if min_len is None or min_len == seq_len:
             self.X = torch.randint(0, vocab, (self.samples, seq_len), generator=g)
@@ -111,19 +121,37 @@ class SyntheticTokens(Dataset):
             self.X.masked_fill_(pad, self.PAD_ID)
             self.Y.masked_fill_(pad, -100)
 
-    def _pack(self, g: torch.Generator, seq_len: int, vocab: int, mask_prob: float, min_len: int) -> None:
-        if vocab <= self.CLS_ID + 1:
-            raise ValueError(f"SyntheticTokens: packing needs vocab > {self.CLS_ID + 1} (token {self.CLS_ID} starts a document)")
+    def _causal_rows(self, g: torch.Generator, seq_len: int, vocab: int, min_len: int | None) -> None:
+        """Fixed-length or right-padded causal-LM rows: next-token labels, -100 at each row's last token and padding."""
+        self.X = torch.randint(1, vocab, (self.samples, seq_len), generator=g)
+        length = torch.full((self.samples,), seq_len)
+        if min_len is not None and min_len < seq_len:
+            self.lengths = length = torch.randint(min_len, seq_len + 1, (self.samples,), generator=g)
+            self.pad_token_id = self.PAD_ID
+            self.X.masked_fill_(torch.arange(seq_len)[None, :] >= length[:, None], self.PAD_ID)
+        self.Y = torch.cat([self.X[:, 1:], torch.full((self.samples, 1), -100)], 1)
+        self.Y.masked_fill_(torch.arange(seq_len)[None, :] >= (length - 1)[:, None], -100)
+
+    def _pack(self, g: torch.Generator, seq_len: int, vocab: int, mask_prob: float, min_len: int, causal: bool = False) -> None:
+        start_id = self.BOS_ID if causal else self.CLS_ID
+        need = start_id if causal else start_id + 1
+        if vocab <= need:
+            raise ValueError(f"SyntheticTokens: packing needs vocab > {need} (token {start_id} starts a document)")
         lens = torch.randint(min_len, seq_len + 1, (self.samples,), generator=g)
         total = int(lens.sum())
         tokens = torch.randint(1, vocab - 1, (total,), generator=g)
-        tokens += tokens >= self.CLS_ID                            # [1, vocab) without CLS_ID
-        labels = torch.randint(0, vocab, (total,), generator=g)
-        masked = torch.rand(total, generator=g) < mask_prob
-        labels = torch.where(masked, labels, torch.full_like(labels, -100))
+        tokens += tokens >= start_id                               # [1, vocab) without start_id
         offsets = torch.cumsum(lens, 0) - lens
-        tokens[offsets] = self.CLS_ID
-        labels[offsets] = -100
+        if causal:                                                 # next token inside the document, -100 at its last
+            tokens[offsets] = start_id
+            labels = torch.cat([tokens[1:], torch.full((1,), -100)])
+            labels[offsets + lens - 1] = -100
+        else:
+            labels = torch.randint(0, vocab, (total,), generator=g)
+            masked = torch.rand(total, generator=g) < mask_prob
+            labels = torch.where(masked, labels, torch.full_like(labels, -100))
+            tokens[offsets] = start_id
+            labels[offsets] = -100
         lens_l, offsets_l = lens.tolist(), offsets.tolist()
         rows, free = [], []
         for i in sorted(range(self.samples), key=lambda i: (-lens_l[i], i)):   # first-fit decreasing
@@ -147,7 +175,10 @@ class SyntheticTokens(Dataset):
         self.doc_lengths = [[lens_l[i] for i in docs] for docs in rows]
         self.lengths = torch.tensor([seq_len - f for f in free])
         self.pad_token_id = self.PAD_ID
-        self.cls_token_id = self.CLS_ID
+        if causal:
+            self.bos_token_id = start_id
+        else:
+            self.cls_token_id = start_id
 
     def __len__(self) -> int:
         return self.samples

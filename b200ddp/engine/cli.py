@@ -64,16 +64,17 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--channels_last", action="store_true")
     p.add_argument("--cuda_graph", action="store_true", help="capture the whole optimizer step in a CUDA graph")
     p.add_argument("--fp8", action="store_true",
-                   help="BERT encoder linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs --model bert-base, "
-                        "--fp16 and a GPU")
+                   help="BERT encoder / GPT-2 block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs --model "
+                        "bert-base or gpt2, --fp16 and a GPU")
     p.add_argument("--min_seq_len", type=int, default=None,
-                   help="BERT on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded keys are "
-                        "hidden from attention (native key-padding kernel on the GPU; needs --fp16 and --seq_len %% 128 == 0 "
-                        "there).  Default: fixed-length rows")
+                   help="BERT / GPT-2 on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
+                        "keys are hidden from attention (native key-padding or causal kernel on the GPU; needs --fp16 and "
+                        "--seq_len %% 128 == 0 there).  Default: fixed-length rows")
     p.add_argument("--pack", action="store_true",
-                   help="BERT on packed documents: documents with lengths uniform in [--min_seq_len, --seq_len], each "
-                        "starting with [CLS], packed first-fit decreasing into rows; attention stays inside a document "
-                        "(native document-boundary kernel on the GPU).  Needs --model bert-base and --min_seq_len < --seq_len")
+                   help="BERT / GPT-2 on packed documents: documents with lengths uniform in [--min_seq_len, --seq_len], "
+                        "each starting with [CLS] (BERT) or <|endoftext|> (GPT-2), packed first-fit decreasing into rows; "
+                        "attention stays inside a document (native document-boundary or causal kernel on the GPU).  Needs "
+                        "--model bert-base or gpt2 and --min_seq_len < --seq_len")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -129,6 +130,7 @@ def setup(args):
                                                                         transport=args.backend))
         args.n_gpu = 1 if have_cuda else 0
     args.device = device
+    check_gpt_args(args)
     check_fp8_args(args)
     check_min_seq_len_args(args)
     check_pack_args(args)
@@ -138,12 +140,25 @@ def setup(args):
     return log
 
 
+# models whose token rows can be right-padded or packed, and whose block linears can run on FP8
+TOKEN_MODELS = ("bert-base", "gpt2")
+GPT2_MAX_SEQ_LEN = 1024
+
+
+def check_gpt_args(args) -> None:
+    """GPT-2 has 1024 learned positions: reject a longer ``--seq_len`` up front."""
+    if args.model == "gpt2" and args.seq_len > GPT2_MAX_SEQ_LEN:
+        raise ValueError(f"--model gpt2 has {GPT2_MAX_SEQ_LEN} positions; --seq_len must be at most {GPT2_MAX_SEQ_LEN} "
+                         f"(got {args.seq_len})")
+
+
 def check_fp8_args(args) -> None:
-    """``--fp8`` is a BERT feature on top of bf16 weights on a GPU: reject every other combination up front."""
+    """``--fp8`` is a BERT / GPT-2 feature on top of bf16 weights on a GPU: reject every other combination up front."""
     if not getattr(args, "fp8", False):
         return
-    if args.model != "bert-base":
-        raise ValueError(f"--fp8 covers the BERT encoder linears only; it needs --model bert-base (got --model {args.model})")
+    if args.model not in TOKEN_MODELS:
+        raise ValueError(f"--fp8 covers the BERT encoder and GPT-2 block linears only; it needs --model bert-base or gpt2 "
+                         f"(got --model {args.model})")
     if not args.fp16:
         raise ValueError("--fp8 needs --fp16: the FP8 GEMMs read bf16 activations and weights")
     if getattr(args, "device", None) is None or args.device.type != "cuda":
@@ -151,13 +166,13 @@ def check_fp8_args(args) -> None:
 
 
 def check_min_seq_len_args(args) -> None:
-    """``--min_seq_len`` pads BERT rows; on the GPU their attention runs on the bf16 key-padding kernel (head dim 64,
-    sequence length a multiple of 128): reject every other combination up front."""
+    """``--min_seq_len`` pads BERT / GPT-2 rows; on the GPU their attention runs on the bf16 key-padding or causal
+    kernel (head dim 64, sequence length a multiple of 128): reject every other combination up front."""
     n = getattr(args, "min_seq_len", None)
     if n is None:
         return
-    if args.model != "bert-base":
-        raise ValueError(f"--min_seq_len pads BERT token rows; it needs --model bert-base (got --model {args.model})")
+    if args.model not in TOKEN_MODELS:
+        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (got --model {args.model})")
     if not 1 <= n <= args.seq_len:
         raise ValueError(f"--min_seq_len must lie in [1, --seq_len = {args.seq_len}], got {n}")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -168,12 +183,12 @@ def check_min_seq_len_args(args) -> None:
 
 
 def check_pack_args(args) -> None:
-    """``--pack`` packs documents into padded BERT rows, so it needs everything ``--min_seq_len`` needs (on the GPU:
-    ``--fp16``, ``--seq_len`` % 128 == 0) and a ``--min_seq_len`` below ``--seq_len``."""
+    """``--pack`` packs documents into padded BERT / GPT-2 rows, so it needs everything ``--min_seq_len`` needs (on the
+    GPU: ``--fp16``, ``--seq_len`` % 128 == 0) and a ``--min_seq_len`` below ``--seq_len``."""
     if not getattr(args, "pack", False):
         return
-    if args.model != "bert-base":
-        raise ValueError(f"--pack packs BERT documents; it needs --model bert-base (got --model {args.model})")
+    if args.model not in TOKEN_MODELS:
+        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (got --model {args.model})")
     if not padding_on(args):
         raise ValueError("--pack needs --min_seq_len below --seq_len (documents have lengths in [--min_seq_len, --seq_len])")
     check_min_seq_len_args(args)
@@ -208,7 +223,9 @@ def main(argv=None) -> int:
     if padding_on(args):
         from ..data import SyntheticTokens
         kwargs["pad_token_id"] = SyntheticTokens.PAD_ID
-        if args.pack:
+        if args.pack and args.model == "gpt2":
+            kwargs["bos_token_id"] = SyntheticTokens.BOS_ID
+        elif args.pack:
             kwargs["cls_token_id"] = SyntheticTokens.CLS_ID
     model = build_model(args.model, **kwargs)
     trainer = Trainer(args, model, log)

@@ -54,6 +54,10 @@ def build_dataset(args):
     if name.startswith("bert"):
         return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)),
                                min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)))
+    if name == "gpt2":                                        # causal-LM rows over GPT-2's vocabulary
+        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=50257,
+                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
+                               causal=True)
     raise ValueError(f"no default dataset for model {name!r}")
 
 
@@ -158,8 +162,9 @@ class Trainer:
 
     # ------------------------------------------------------------------------------------------
     def _check_padding(self, model: torch.nn.Module) -> None:
-        """A right-padded dataset needs a model that derives the lengths from the pad id (``BertConfig.pad_token_id``),
-        and a packed one also a model that derives the documents from the same CLS id (``BertConfig.cls_token_id``);
+        """A right-padded dataset needs a model that derives the lengths from the pad id (``BertConfig.pad_token_id``,
+        ``GPTConfig.pad_token_id``), and a packed one also a model that derives the documents from the same document id
+        (``BertConfig.cls_token_id`` for CLS-started documents, ``GPTConfig.bos_token_id`` for BOS-started ones);
         otherwise padded keys, or other documents, would be attended to without any error."""
         self.count_pad_id = None
         pad_id = getattr(self.dataset, "pad_token_id", None)
@@ -173,13 +178,14 @@ class Trainer:
             raise ValueError(f"the dataset pads its rows with token {pad_id}, but the model derives no sequence lengths from "
                              f"it (model pad_token_id: {sorted(model_pads - {None}) or None}); build it with pad_token_id={pad_id}")
         seq_len = self.dataset.X.shape[1]
-        cls_id = getattr(self.dataset, "cls_token_id", None)
-        if cls_id is not None:
-            model_cls = {getattr(c, "cls_token_id", None) for c in configs}
-            if cls_id not in model_cls:
-                raise ValueError(f"the dataset packs documents that start with token {cls_id}, but the model derives no "
-                                 f"documents from it (model cls_token_id: {sorted(model_cls - {None}) or None}); build it "
-                                 f"with cls_token_id={cls_id}, or documents attend to each other")
+        doc_attr = next((a for a in ("cls_token_id", "bos_token_id") if getattr(self.dataset, a, None) is not None), None)
+        if doc_attr is not None:
+            doc_id = getattr(self.dataset, doc_attr)
+            model_docs = {getattr(c, doc_attr, None) for c in configs}
+            if doc_id not in model_docs:
+                raise ValueError(f"the dataset packs documents that start with token {doc_id}, but the model derives no "
+                                 f"documents from it (model {doc_attr}: {sorted(model_docs - {None}) or None}); build it "
+                                 f"with {doc_attr}={doc_id}, or documents attend to each other")
             docs = [n for row in self.dataset.doc_lengths for n in row]
             self.log.info("Packed sequences.", dict(documents=len(docs), rows=len(self.dataset),
                                                     docs_per_row=round(len(docs) / len(self.dataset), 2),

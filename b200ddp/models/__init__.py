@@ -2,12 +2,14 @@
 from .foo import FooModel, BranchyFooModel
 from .resnet import ResNet, resnet50, resnet152
 from .bert import BertConfig, BertModel, BertForMaskedLM, bert_base
+from .gpt import GPTConfig, GPTModel, GPTLMHeadModel, gpt2
 
 MODEL_REGISTRY = {
     "foo": FooModel,
     "resnet50": resnet50,
     "resnet152": resnet152,
     "bert-base": bert_base,
+    "gpt2": gpt2,
 }
 
 
@@ -19,4 +21,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "MODEL_REGISTRY", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "MODEL_REGISTRY", "build_model"]

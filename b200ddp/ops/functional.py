@@ -22,6 +22,16 @@ from .. import _ext
 
 EPI_NONE, EPI_BIAS, EPI_BIAS_RELU, EPI_BIAS_GELU = 0, 1, 2, 3
 _ACT_TO_EPI = {None: EPI_BIAS, "relu": EPI_BIAS_RELU, "gelu": EPI_BIAS_GELU}
+# GELU variants: the erf form ("gelu", BERT) and the tanh approximation ("gelu_tanh", GPT-2's ``gelu_new``).  Both run as
+# a bias epilogue plus one elementwise pass (csrc/loss.cu) that keeps the pre-activation for the backward.
+_GELU_TANH = {"gelu": False, "gelu_tanh": True}
+
+
+def _gelu_tanh_grad(p: torch.Tensor) -> torch.Tensor:
+    """d/dp of 0.5 p (1 + tanh(sqrt(2 / pi) (p + 0.044715 p^3))), in p's dtype."""
+    k = math.sqrt(2.0 / math.pi)
+    t = torch.tanh(k * (p + 0.044715 * p * p * p))
+    return 0.5 * (1.0 + t) + 0.5 * p * (1.0 - t * t) * k * (1.0 + 3.0 * 0.044715 * p * p)
 
 
 def _C():
@@ -46,16 +56,15 @@ class _LinearTC(torch.autograd.Function):
         x2 = x.reshape(-1, x.shape[-1])
         if not x2.is_contiguous():
             x2 = x2.contiguous()
-        epi = _ACT_TO_EPI[activation] if bias is not None else EPI_NONE
         if bias is None and activation is not None:
             raise ValueError("fused activation needs a bias (use bias=True)")
-        if activation == "gelu":
+        if activation in _GELU_TANH:
             # keep the pre-activation for the backward (GELU' needs it): two launches, one extra tensor
             pre = C.gemm_nt(x2, weight, bias, EPI_BIAS, None)
-            y = C.gelu_fwd(pre)
+            y = C.gelu_fwd(pre, _GELU_TANH[activation])
             ctx.save_for_backward(x2, weight, pre)
         else:
-            y = C.gemm_nt(x2, weight, bias, epi, None)
+            y = C.gemm_nt(x2, weight, bias, _ACT_TO_EPI[activation] if bias is not None else EPI_NONE, None)
             ctx.save_for_backward(x2, weight, y if activation == "relu" else None)
         ctx.activation = activation
         ctx.has_bias = bias is not None
@@ -69,8 +78,8 @@ class _LinearTC(torch.autograd.Function):
         dy2 = dy.reshape(-1, dy.shape[-1])
         if ctx.activation == "relu":
             dy2 = dy2 * (aux > 0).to(dy2.dtype)
-        elif ctx.activation == "gelu":
-            dy2 = C.gelu_bwd(dy2.contiguous(), aux)          # dy * gelu'(pre) in one pass
+        elif ctx.activation in _GELU_TANH:
+            dy2 = C.gelu_bwd(dy2.contiguous(), aux, _GELU_TANH[ctx.activation])   # dy * gelu'(pre) in one pass
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
         dx = dw = db = None
@@ -174,9 +183,9 @@ class _LinearFP8(torch.autograd.Function):
             _fp8_check(x2, weight, bias, need_dw)
             xq, xqt, xs, _ = C.fp8_quantize(x2, "e4m3", need_dw, False)
             wq, wqt, ws, _ = C.fp8_quantize(weight.contiguous(), "e4m3", need_dx, False)
-            if activation == "gelu":
+            if activation in _GELU_TANH:
                 pre = C.gemm_fp8(xq, wq, xs, ws, bias, EPI_BIAS)
-                y = C.gelu_fwd(pre)
+                y = C.gelu_fwd(pre, _GELU_TANH[activation])
             else:
                 pre = None
                 y = C.gemm_fp8(xq, wq, xs, ws, bias, _ACT_TO_EPI[activation] if bias is not None else EPI_NONE)
@@ -192,6 +201,8 @@ class _LinearFP8(torch.autograd.Function):
             pre = acc.to(x.dtype)
             if activation == "gelu":
                 y = F.gelu(pre.float()).to(x.dtype)
+            elif activation == "gelu_tanh":
+                y = F.gelu(pre.float(), approximate="tanh").to(x.dtype)
             elif activation == "relu":
                 y = F.relu(pre)
             else:
@@ -209,8 +220,8 @@ class _LinearFP8(torch.autograd.Function):
             xqt, xs, wqt, ws, aux = ctx.saved_tensors
             if ctx.activation == "relu":
                 dy2 = dy2 * (aux > 0).to(dy2.dtype)
-            elif ctx.activation == "gelu":
-                dy2 = C.gelu_bwd(dy2.contiguous(), aux)
+            elif ctx.activation in _GELU_TANH:
+                dy2 = C.gelu_bwd(dy2.contiguous(), aux, _GELU_TANH[ctx.activation])
             if not dy2.is_contiguous():
                 dy2 = dy2.contiguous()
             if dy2.shape[0] % 16:
@@ -232,6 +243,8 @@ class _LinearFP8(torch.autograd.Function):
                 p = aux.float()                                    # gelu'(p) = Phi(p) + p phi(p)
                 dgelu = 0.5 * (1.0 + torch.erf(p * math.sqrt(0.5))) + p * torch.exp(-0.5 * p * p) / math.sqrt(2.0 * math.pi)
                 dy2 = (dy2.float() * dgelu).to(dy.dtype)
+            elif ctx.activation == "gelu_tanh":
+                dy2 = (dy2.float() * _gelu_tanh_grad(aux.float())).to(dy.dtype)
             dyd = _fp8_round_trip(dy2, "e5m2")
             if ctx.needs_input_grad[0]:
                 dx = (dyd @ wd).to(x_dtype).view(ctx.x_shape)
@@ -244,8 +257,9 @@ class _LinearFP8(torch.autograd.Function):
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None,
            activation: Optional[str] = None, fp8: bool = False) -> torch.Tensor:
-    """y = act(x @ weight.T + bias), activation in {None, "relu", "gelu"}.  ``fp8=True`` runs the three GEMMs on FP8
-    tensor cores (``_LinearFP8``); on CUDA it needs bf16 tensors and raises ``ValueError`` for anything else."""
+    """y = act(x @ weight.T + bias), activation in {None, "relu", "gelu", "gelu_tanh"} ("gelu" is the erf form,
+    "gelu_tanh" the tanh approximation).  ``fp8=True`` runs the three GEMMs on FP8 tensor cores (``_LinearFP8``); on CUDA
+    it needs bf16 tensors and raises ``ValueError`` for anything else."""
     if fp8:
         return _LinearFP8.apply(x, weight, bias, activation, torch.is_grad_enabled())
     if x.is_cuda:
@@ -265,6 +279,8 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
         y = F.relu(y)
     elif activation == "gelu":
         y = F.gelu(y)
+    elif activation == "gelu_tanh":
+        y = F.gelu(y, approximate="tanh")
     return y
 
 
@@ -321,24 +337,31 @@ def _qkv_check(qkv: torch.Tensor, heads: int) -> None:
         raise ValueError("attention on CUDA needs a contiguous qkv (the fused projection's output)")
 
 
+# mask modes of _Attention: name -> (native forward, native backward, CPU reference)
+_ATTENTION_MODES = {
+    "key_padding": ("attention_fwd", "attention_bwd", lambda: attention_reference),
+    "packed": ("packed_attention_fwd", "packed_attention_bwd", lambda: packed_attention_reference),
+    "causal": ("causal_attention_fwd", "causal_attention_bwd", lambda: causal_attention_reference),
+}
+
+
 class _Attention(torch.autograd.Function):
-    """Key-padding (``packed=False``, mask = seq_lens [B]) or packed-document (``packed=True``, mask = bounds [B, S, 2])
-    attention.  CUDA body: the sm_90a kernels (forward keeps the row log-sum-exp; backward is three deterministic
-    launches writing one dqkv tensor, the exact gradient the qkv linear consumes).  CPU body: the matching reference
-    (backward by recomputation through autograd)."""
+    """Key-padding (``mode="key_padding"``, mask = seq_lens [B]), packed-document (``"packed"``, mask = bounds [B, S, 2])
+    or causal-document (``"causal"``, the same bounds) attention.  CUDA body: the sm_90a kernels (forward keeps the row
+    log-sum-exp; backward is three deterministic launches writing one dqkv tensor, the exact gradient the qkv linear
+    consumes).  CPU body: the matching reference (backward by recomputation through autograd)."""
 
     @staticmethod
-    def forward(ctx, qkv, mask, heads, packed):
-        ctx.heads, ctx.packed = heads, packed
+    def forward(ctx, qkv, mask, heads, mode):
+        ctx.heads, ctx.mode = heads, mode
         if qkv.is_cuda:
             B, S, W = qkv.shape
             m = mask.to(device=qkv.device, dtype=torch.int32).contiguous()
-            fwd = _C().packed_attention_fwd if packed else _C().attention_fwd
-            o, lse = fwd(qkv.view(B * S, W), m, heads)
+            o, lse = getattr(_C(), _ATTENTION_MODES[mode][0])(qkv.view(B * S, W), m, heads)
             ctx.save_for_backward(qkv, o, lse, m)
             return o.view(B, S, W // 3)
         ctx.save_for_backward(qkv, mask)
-        return (packed_attention_reference if packed else attention_reference)(qkv, mask, heads)
+        return _ATTENTION_MODES[mode][2]()(qkv, mask, heads)
 
     @staticmethod
     def backward(ctx, dy):
@@ -348,11 +371,10 @@ class _Attention(torch.autograd.Function):
             do = dy.reshape(B * S, W // 3).to(torch.bfloat16).contiguous()
             if do.data_ptr() % 16:                                # the kernels read dO in 16-byte vectors / TMA boxes
                 do = do.clone()
-            bwd = _C().packed_attention_bwd if ctx.packed else _C().attention_bwd
-            dqkv = bwd(do, qkv.view(B * S, W), o, lse, m, ctx.heads)
+            dqkv = getattr(_C(), _ATTENTION_MODES[ctx.mode][1])(do, qkv.view(B * S, W), o, lse, m, ctx.heads)
             return dqkv.view(B, S, W), None, None, None
         qkv, mask = ctx.saved_tensors
-        ref = packed_attention_reference if ctx.packed else attention_reference
+        ref = _ATTENTION_MODES[ctx.mode][2]()
         with torch.enable_grad():
             x = qkv.detach().requires_grad_(True)
             (g,) = torch.autograd.grad(ref(x, mask, ctx.heads), x, dy)
@@ -366,18 +388,18 @@ def attention(qkv: torch.Tensor, seq_lens: torch.Tensor, heads: int) -> torch.Te
     ``ValueError``; lengths stay on the device (no host synchronisation, CUDA-graph safe)."""
     if qkv.is_cuda:
         _attention_check(qkv, seq_lens, heads)
-    return _Attention.apply(qkv, seq_lens, heads, False)
+    return _Attention.apply(qkv, seq_lens, heads, "key_padding")
 
 
 # ------------------------------------------------------------------------------------------------
 # Packed-document attention (csrc/attention.cu, segment mode): several documents per row, block-diagonal mask
 # ------------------------------------------------------------------------------------------------
-def document_bounds(input_ids: torch.Tensor, cls_token_id: int, pad_token_id: Optional[int]):
+def document_bounds(input_ids: torch.Tensor, cls_token_id: Optional[int], pad_token_id: Optional[int]):
     """Documents of packed rows, on the device with no host synchronisation (CUDA-graph safe).
 
     input_ids [B, S].  A row's length is its non-pad count (S when ``pad_token_id`` is None); positions at or beyond it
     are padding, whatever their id.  A document starts at position 0 and at every ``cls_token_id`` below the length, and
-    runs to the next start or the length.  Returns ``(bounds, position_ids)``: bounds int32 [B, S, 2] holds each
+    runs to the next start or the length; with ``cls_token_id=None`` each row is one document ``(0, length)``.  Returns ``(bounds, position_ids)``: bounds int32 [B, S, 2] holds each
     position's document as (start, end), (0, 0) for padding; position_ids long [B, S] restart at 0 in each document and
     are 0 for padding."""
     B, S = input_ids.shape
@@ -387,7 +409,8 @@ def document_bounds(input_ids: torch.Tensor, cls_token_id: int, pad_token_id: Op
     else:
         lens = (input_ids != pad_token_id).sum(1, keepdim=True)
     valid = pos < lens
-    is_start = ((input_ids == cls_token_id) | (pos == 0)) & valid
+    is_start = (pos == 0) if cls_token_id is None else (input_ids == cls_token_id) | (pos == 0)
+    is_start = is_start & valid
     start = torch.where(is_start, pos, 0).cummax(1).values                   # the last start at or before each position
     nxt = torch.where(is_start, pos, S)[:, 1:]                                  # the first start after each position
     nxt = torch.cat([nxt, torch.full((B, 1), S, device=pos.device, dtype=pos.dtype)], 1).flip(1).cummin(1).values.flip(1)
@@ -420,11 +443,42 @@ def packed_attention(qkv: torch.Tensor, bounds: torch.Tensor, heads: int) -> tor
     dim 64, S % 128 == 0 and contiguous qkv, else ``ValueError``; bounds stay on the device (CUDA-graph safe)."""
     if qkv.is_cuda:
         _qkv_check(qkv, heads)
-        B, S = qkv.shape[:2]
-        if tuple(bounds.shape) != (B, S, 2) or bounds.is_floating_point() or bounds.is_complex():
-            raise ValueError(f"packed attention needs integer bounds [B, S, 2] = [{B}, {S}, 2], got {bounds.dtype} "
-                             f"{tuple(bounds.shape)}")
-    return _Attention.apply(qkv, bounds, heads, True)
+        _bounds_check(qkv, bounds, "packed attention")
+    return _Attention.apply(qkv, bounds, heads, "packed")
+
+
+def _bounds_check(qkv: torch.Tensor, bounds: torch.Tensor, who: str) -> None:
+    B, S = qkv.shape[:2]
+    if tuple(bounds.shape) != (B, S, 2) or bounds.is_floating_point() or bounds.is_complex():
+        raise ValueError(f"{who} needs integer bounds [B, S, 2] = [{B}, {S}, 2], got {bounds.dtype} {tuple(bounds.shape)}")
+
+
+# ------------------------------------------------------------------------------------------------
+# Causal document attention (csrc/attention.cu, causal mode): packed documents, each causal (decoder LMs)
+# ------------------------------------------------------------------------------------------------
+def _causal_mask(bounds: torch.Tensor, S: int, device) -> torch.Tensor:
+    """[B, S, S] bool: query i sees key j iff start[i] <= j <= i and j < end[i] (bounds clamped like the kernel)."""
+    i = torch.arange(S, device=device)
+    return _bounds_mask(bounds, S, device) & (i[None, :] <= i[:, None])
+
+
+def causal_attention_reference(qkv: torch.Tensor, bounds: torch.Tensor, heads: int) -> torch.Tensor:
+    """softmax(Q K^T / sqrt(d)) V where query i sees key j of its row iff bounds[b, i, 0] <= j <= i and
+    j < bounds[b, i, 1], in fp32 (fp64 stays fp64), as a dense mask; a row that sees no key gives zeros.  qkv
+    [B, S, 3 * hidden], bounds integer [B, S, 2]; returns [B, S, hidden] in qkv's dtype.  Differentiable."""
+    return _masked_attention_reference(qkv, _causal_mask(bounds, qkv.shape[1], qkv.device)[:, None], heads)
+
+
+def causal_attention(qkv: torch.Tensor, bounds: torch.Tensor, heads: int) -> torch.Tensor:
+    """Causal multi-head attention inside documents: qkv [B, S, 3 * hidden] (the fused projection's output), bounds
+    integer [B, S, 2] (``document_bounds``; with ``cls_token_id=None`` it gives right-padded rows one document each):
+    query i of a row sees key j iff start[i] <= j <= i and j < end[i].  Rows with start == end (padding) give zeros and
+    get zero gradients.  Returns [B, S, hidden].  On CUDA: bf16, head dim 64, S % 128 == 0 and contiguous qkv, else
+    ``ValueError``; bounds stay on the device (CUDA-graph safe).  Tiles above the diagonal are never visited."""
+    if qkv.is_cuda:
+        _qkv_check(qkv, heads)
+        _bounds_check(qkv, bounds, "causal attention")
+    return _Attention.apply(qkv, bounds, heads, "causal")
 
 
 # ------------------------------------------------------------------------------------------------

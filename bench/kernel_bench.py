@@ -236,6 +236,53 @@ def main():
                timeit(lambda: C.packed_attention_bwd(dout, qkv, o, lse, bounds, H), args.iters),
                flops=2.5 * fwd_flops, lib_ms=lib, note="lib = SDPA block-diagonal bool mask backward into qkv")
         del x, q, k, v, y
+        # Causal documents (GPT-2 at batch 8 x seq 1024, 12 heads): the native causal kernels against SDPA with
+        # is_causal (flash) on full and right-padded rows, and against SDPA with the dense causal block-diagonal mask on
+        # packed rows.  FLOPs count only the causal part of each document: forward 2 d H sum_docs len (len + 1),
+        # backward 2.5x that.
+        from b200ddp.data import SyntheticTokens as _Tok
+        B, S = 8, 1024
+        qkv = torch.randn(B * S, 3 * H * d, device=dev, generator=g).to(torch.bfloat16)
+        dout = torch.randn(B * S, H * d, device=dev, generator=g).to(torch.bfloat16)
+        j = torch.arange(S, device=dev)
+        lens_random = torch.randint(128, S + 1, (B,), generator=torch.Generator().manual_seed(0))
+        packed = _Tok(seq_len=S, min_len=128, vocab=50257, pack=True, causal=True)
+        rows = torch.linspace(0, len(packed) - 1, B).long().tolist()
+        cases = [("full length", [[S]] * B, None), ("lengths U[128,1024]", [[int(n)] for n in lens_random], None),
+                 (None, [packed.doc_lengths[r] for r in rows], packed.X[rows])]
+        for label, docs, ids in cases:
+            if ids is None:
+                lt = torch.tensor([sum(r) for r in docs], device=dev)
+                bounds, _ = document_bounds(torch.where(j[None, :] < lt[:, None], 1, 0), None, 0)
+            else:
+                bounds, _ = document_bounds(ids.to(dev), packed.bos_token_id, packed.pad_token_id)
+                label = f"packed {sum(len(r) for r in docs)} docs U[128,1024]"
+            flat = [n for r in docs for n in r]
+            fwd_flops = 2.0 * sum(n * (n + 1) for n in flat) * d * H
+            x = qkv.view(B, S, 3 * H * d).detach().clone().requires_grad_(True)
+            q, k, v = (t.reshape(B, S, H, d).transpose(1, 2) for t in x.split(H * d, dim=-1))
+            if ids is None:
+                mask, lib_name = None, "SDPA is_causal (flash)"
+            else:
+                mask = ((j >= bounds[..., :1]) & (j < bounds[..., 1:]) & (j[None, :] <= j[:, None]))[:, None]
+                mask |= torch.eye(S, dtype=torch.bool, device=dev)   # tail padding rows: their own key, not a NaN row
+                lib_name = "SDPA causal block-diagonal bool mask"
+
+            def sdpa():
+                return F.scaled_dot_product_attention(q, k, v, attn_mask=mask, is_causal=mask is None) \
+                    .transpose(1, 2).reshape(B, S, H * d)
+            lib = timeit(lambda: sdpa().detach(), args.iters)
+            record(f"causal attention fwd {label} B{B} S{S} H{H}",
+                   timeit(lambda: C.causal_attention_fwd(qkv, bounds, H), args.iters),
+                   flops=fwd_flops, lib_ms=lib, note=f"lib = {lib_name} + output transpose")
+            o, lse = C.causal_attention_fwd(qkv, bounds, H)
+            y = sdpa()
+            dy = dout.view(B, S, H * d)
+            lib = timeit(lambda: torch.autograd.grad(y, x, dy, retain_graph=True), args.iters)
+            record(f"causal attention bwd {label} B{B} S{S} H{H}",
+                   timeit(lambda: C.causal_attention_bwd(dout, qkv, o, lse, bounds, H), args.iters),
+                   flops=2.5 * fwd_flops, lib_ms=lib, note=f"lib = {lib_name} backward into qkv")
+            del x, q, k, v, y
 
     if "conv" in want:
         import torch.nn.functional as F
