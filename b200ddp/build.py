@@ -24,7 +24,7 @@ EXT_NAME = "_C"
 
 CUDA_SOURCES = ["allreduce.cu", "broadcast.cu", "optim.cu", "loss.cu", "layernorm.cu", "linear_small.cu", "input.cu",
                 "gemm_wgmma.cu", "batchnorm.cu", "pool.cu", "conv_wgmma.cu", "conv_wgrad_wgmma.cu", "conv_stem.cu", "fp8.cu",
-                "attention.cu"]
+                "attention.cu", "rotary.cu"]
 CPP_SOURCES = ["peer_mem.cpp", "reducer.cpp", "bindings.cpp"]
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]

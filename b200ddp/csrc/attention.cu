@@ -39,6 +39,12 @@
 //                 dS, dQ += dS K.
 // Recomputing P in both backward kernels costs two GEMMs more than accumulating dQ with atomics inside the dK/dV loop;
 // that is the price of bit-identical gradients on every run.
+//
+// Grouped-query attention (kCausal only, compile-time kGqa): qkv is [B*S, (H + 2*Hkv)*64] with column blocks query (H
+// heads) | key (Hkv heads) | value (Hkv heads); query head h reads K/V head h / (H / Hkv) (Hugging Face's repeat_kv
+// order).  The forward and dQ keep their grid (S/128, H, B) and only read K/V at other columns.  dK/dV runs on
+// (S/128, Hkv, B): its ring walks every (query head of the group, query tile) pair and accumulates the whole group's
+// contribution in registers, so each dK/dV element still has one writer.
 #include <cuda.h>
 
 #include "common.h"
@@ -170,12 +176,23 @@ __device__ __forceinline__ void store_frag(const float (&acc)[32], float scale0,
   }
 }
 
+// Columns of query head h's key and value heads in qkv (H query heads, HD = H * 64; Hkv K/V heads when kGqa)
+template <bool kGqa>
+__device__ __forceinline__ int2 kv_cols(int h, int H, int HD, int Hkv) {
+  if constexpr (kGqa) {
+    const int hk = h / (H / Hkv);
+    return make_int2(HD + hk * kHd, HD + (Hkv + hk) * kHd);
+  } else {
+    return make_int2(HD + h * kHd, 2 * HD + h * kHd);
+  }
+}
+
 // ============================================== forward ==============================================================
-// mask: seq_lens [B] (kKeyPadding) or bounds [B*S, 2] (kSegment, kCausal)
-template <int kMode>
+// mask: seq_lens [B] (kKeyPadding) or bounds [B*S, 2] (kSegment, kCausal); Hkv: K/V heads (read only when kGqa)
+template <int kMode, bool kGqa = false>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restrict__ mask, int S, int H,
-                __nv_bfloat16* __restrict__ o, float* __restrict__ lse) {
+                __nv_bfloat16* __restrict__ o, float* __restrict__ lse, int Hkv) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sq = smem;                                           // 128 query rows
@@ -218,6 +235,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
       mbar_expect_tx(q_bar, 2 * kBoxBytes);
       tma_load_2d(&map_qkv, q_bar, sq, h * kHd, q_row);
       tma_load_2d(&map_qkv, q_bar, sq + kBoxBytes, h * kHd, q_row + 64);
+      const int2 kv = kv_cols<kGqa>(h, H, HD, Hkv);
       int stage = 0;
       uint32_t phase = 0;
       for (int kt = kt0; kt < kt0 + n_kt; ++kt) {
@@ -226,10 +244,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
         uint8_t* sv = sk + 2 * kBoxBytes;
         const int k_row = (int)seq_row + kt * 128;
         mbar_expect_tx(&full_bar[stage], 4 * kBoxBytes);
-        tma_load_2d(&map_qkv, &full_bar[stage], sk, HD + h * kHd, k_row);
-        tma_load_2d(&map_qkv, &full_bar[stage], sk + kBoxBytes, HD + h * kHd, k_row + 64);
-        tma_load_2d(&map_qkv, &full_bar[stage], sv, 2 * HD + h * kHd, k_row);
-        tma_load_2d(&map_qkv, &full_bar[stage], sv + kBoxBytes, 2 * HD + h * kHd, k_row + 64);
+        tma_load_2d(&map_qkv, &full_bar[stage], sk, kv.x, k_row);
+        tma_load_2d(&map_qkv, &full_bar[stage], sk + kBoxBytes, kv.x, k_row + 64);
+        tma_load_2d(&map_qkv, &full_bar[stage], sv, kv.y, k_row);
+        tma_load_2d(&map_qkv, &full_bar[stage], sv + kBoxBytes, kv.y, k_row + 64);
         if (++stage == kFwdStages) { stage = 0; phase ^= 1; }
       }
     }
@@ -437,19 +455,117 @@ __device__ __forceinline__ void bwd_produce(const BwdSmem& L, const CUtensorMap*
   }
 }
 
-// dK, dV for one tile of 128 keys.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries: all S / 64 of them (kKeyPadding),
-// or those inside the union of the key rows' intervals (kSegment, kCausal).
+// The ring of the GQA dK/dV kernel: for each of the `groups` query heads h0 + g, `n` stages of (Q, dO) tiles of 64 rows
+// from ring_row0, at columns (h0 + g) * 64 of qkv and dO.
+__device__ __forceinline__ void bwd_produce_groups(const BwdSmem& L, const CUtensorMap* map_qkv, const CUtensorMap* map_do,
+                                                   int h0, int groups, int ring_row0, int n) {
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int g = 0; g < groups; ++g) {
+    for (int i = 0; i < n; ++i) {
+      mbar_wait(&L.empty_bar[stage], phase ^ 1);
+      uint8_t* t0 = L.ring + stage * 2 * kBoxBytes;
+      mbar_expect_tx(&L.full_bar[stage], 2 * kBoxBytes);
+      tma_load_2d(map_qkv, &L.full_bar[stage], t0, (h0 + g) * kHd, ring_row0 + 64 * i);
+      tma_load_2d(map_do, &L.full_bar[stage], t0 + kBoxBytes, (h0 + g) * kHd, ring_row0 + 64 * i);
+      if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+    }
+  }
+}
+
+// The consumer warpgroups of the GQA dK/dV kernel: the loop of attn_bwd_dkdv_kernel (kSegment / kCausal masks), run
+// once per query head h * groups + g of K/V head h, all into the same dK / dV accumulators.  It is a copy of that loop
+// rather than a shared function because factoring the loop out changes the code the multi-head instantiations compile
+// to; keep the two in step.  lse and D are indexed with a 32-bit offset (B * H * S < 2^31) from the kernel parameters,
+// and the output columns are computed after the loop, so the kernel fits its 168 registers without spilling.
 template <int kMode>
+__device__ __forceinline__ void dkdv_consume_group(const BwdSmem& L, const int* __restrict__ mask, int S, int H, int Hkv, int b,
+                                                   int h, int kt, int qt0, int n_qt, const float* __restrict__ lse,
+                                                   const float* __restrict__ Dsum, __nv_bfloat16* __restrict__ dqkv) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = (warp - 4) >> 2;                               // keys [64 wg, 64 wg + 64) of the tile
+  const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+  const int key = kt * 128 + wg * 64 + r0;
+  const size_t seq_row = (size_t)b * S;
+  const uint32_t k_addr = smem_u32(L.fixed0 + wg * kBoxBytes), v_addr = smem_u32(L.fixed1 + wg * kBoxBytes);
+  float dv[32], dk[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  mbar_wait(L.fixed_bar, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  const int groups = H / Hkv;
+  const int bh_end = (b * H + (h + 1) * groups) * S;
+#pragma unroll 1
+  for (int bh = (b * H + h * groups) * S; bh < bh_end; bh += S) {   // lse / D rows of query heads h * groups + g
+    for (int qt = qt0; qt < qt0 + n_qt; ++qt) {
+      const int2 kb0 = mask_interval<kMode, true>(mask, seq_row + key, key, S);
+      const int2 kb1 = mask_interval<kMode, true>(mask, seq_row + key + 8, key + 8, S);
+      const int q0 = qt * 64 + c0;
+      const uint32_t vis = frag_mask16(kb0.x - q0, kb0.y - q0) | (frag_mask16(kb1.x - q0, kb1.y - q0) << 16);
+      mbar_wait(&L.full_bar[stage], phase);
+      const uint32_t q_addr = smem_u32(L.ring + stage * 2 * kBoxBytes), do_addr = q_addr + kBoxBytes;
+      float st[32], dpt[32];
+      wgmma_fence();
+      mma_hd_n64(st, k_addr, q_addr);                           // S^T = K Q^T     [keys, queries]
+      mma_hd_n64(dpt, v_addr, do_addr);                         // dP^T = V dO^T
+      wgmma_commit();
+      wgmma_wait<0>();
+      uint32_t pa[16], dsa[16];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {                             // query columns 8 j + c0, + 1
+        const int q = qt * 64 + 8 * j + c0;
+        const float2 lq = *reinterpret_cast<const float2*>(lse + (bh + q));
+        const float2 dq = *reinterpret_cast<const float2*>(Dsum + (bh + q));
+        const float l0 = lq.x == -INFINITY ? INFINITY : lq.x * kLog2e;   // a query that saw no key gets P = 0
+        const float l1 = lq.y == -INFINITY ? INFINITY : lq.y * kLog2e;
+        const bool v00 = (vis >> (2 * j)) & 1u, v01 = (vis >> (2 * j + 1)) & 1u;
+        const bool v10 = (vis >> (16 + 2 * j)) & 1u, v11 = (vis >> (17 + 2 * j)) & 1u;
+        const float p00 = v00 ? exp2f(st[4 * j] * kScaleLog2 - l0) : 0.f;
+        const float p01 = v01 ? exp2f(st[4 * j + 1] * kScaleLog2 - l1) : 0.f;
+        const float p10 = v10 ? exp2f(st[4 * j + 2] * kScaleLog2 - l0) : 0.f;
+        const float p11 = v11 ? exp2f(st[4 * j + 3] * kScaleLog2 - l1) : 0.f;
+        pa[2 * j] = pack_bf16x2(p00, p01);
+        pa[2 * j + 1] = pack_bf16x2(p10, p11);
+        dsa[2 * j] = pack_bf16x2(p00 * (dpt[4 * j] - dq.x), p01 * (dpt[4 * j + 1] - dq.y));
+        dsa[2 * j + 1] = pack_bf16x2(p10 * (dpt[4 * j + 2] - dq.x), p11 * (dpt[4 * j + 3] - dq.y));
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_n64_rs<1>(dv, pa + 4 * kk, desc_mn(do_addr + kk * kStepMN), 1u);   // dV += P^T dO
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_n64_rs<1>(dk, dsa + 4 * kk, desc_mn(q_addr + kk * kStepMN), 1u);  // dK += dS^T Q
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&L.empty_bar[stage]);
+      if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+    }
+  }
+  const size_t pitch = (size_t)(H + 2 * Hkv) * kHd;
+  __nv_bfloat16* krow = dqkv + (seq_row + key) * pitch + (H + h) * kHd;
+  store_frag(dk, kScale, kScale, krow, pitch, c0);
+  store_frag(dv, 1.f, 1.f, krow + Hkv * kHd, pitch, c0);
+}
+
+// dK, dV for one tile of 128 keys.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries: all S / 64 of them (kKeyPadding),
+// or those inside the union of the key rows' intervals (kSegment, kCausal); with kGqa, those tiles of every query head
+// of the K/V head's group in turn (h is then the K/V head).
+template <int kMode, bool kGqa = false>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
                      const int* __restrict__ mask, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
-                     __nv_bfloat16* __restrict__ dqkv) {
+                     __nv_bfloat16* __restrict__ dqkv, int Hkv) {
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
   const int3 tc = tile_coords<kMode, true>();
   const int kt = tc.x, h = tc.y, b = tc.z;
   const int HD = H * kHd;
-  const size_t pitch = (size_t)3 * HD;
+  const size_t pitch = kGqa ? (size_t)(H + 2 * Hkv) * kHd : (size_t)3 * HD;
+  const int groups = kGqa ? H / Hkv : 1;                        // query heads h * groups + g read this K/V head
+  const int kcol = HD + h * kHd;                                // this K/V head's key and value columns
+  const int vcol = kGqa ? HD + (Hkv + h) * kHd : 2 * HD + h * kHd;
   const size_t seq_row = (size_t)b * S;
   int len = 0, qt0 = 0, n_qt = S / 64;                          // query tiles qt0 .. qt0 + n_qt - 1
   bool hidden;
@@ -463,8 +579,13 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
     n_qt = (r.y + 63) / 64 - qt0;
   }
   if (hidden) {                                                 // every key of the tile is hidden: no gradient
-    zero_rows(dqkv + HD + h * kHd, pitch, seq_row + kt * 128, 128);
-    zero_rows(dqkv + 2 * HD + h * kHd, pitch, seq_row + kt * 128, 128);
+    if constexpr (kGqa) {
+      zero_rows(dqkv + kcol, pitch, seq_row + kt * 128, 128);
+      zero_rows(dqkv + vcol, pitch, seq_row + kt * 128, 128);
+    } else {
+      zero_rows(dqkv + HD + h * kHd, pitch, seq_row + kt * 128, 128);
+      zero_rows(dqkv + 2 * HD + h * kHd, pitch, seq_row + kt * 128, 128);
+    }
     return;
   }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -475,10 +596,23 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
     if (lane == 0) {
       tma_prefetch_desc(&map_qkv);
       tma_prefetch_desc(&map_do);
-      bwd_produce(L, &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row + kt * 128,
-                  &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + 64 * qt0, n_qt);
+      if constexpr (kGqa) {
+        mbar_expect_tx(L.fixed_bar, 4 * kBoxBytes);
+        tma_load_2d(&map_qkv, L.fixed_bar, L.fixed0, kcol, (int)seq_row + kt * 128);
+        tma_load_2d(&map_qkv, L.fixed_bar, L.fixed0 + kBoxBytes, kcol, (int)seq_row + kt * 128 + 64);
+        tma_load_2d(&map_qkv, L.fixed_bar, L.fixed1, vcol, (int)seq_row + kt * 128);
+        tma_load_2d(&map_qkv, L.fixed_bar, L.fixed1 + kBoxBytes, vcol, (int)seq_row + kt * 128 + 64);
+        bwd_produce_groups(L, &map_qkv, &map_do, h * groups, groups, (int)seq_row + 64 * qt0, n_qt);
+      } else {
+        bwd_produce(L, &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row + kt * 128,
+                    &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + 64 * qt0, n_qt);
+      }
     }
   } else if (warp >= 4) {
+    if constexpr (kGqa) {
+      dkdv_consume_group<kMode>(L, mask, S, H, Hkv, b, h, kt, qt0, n_qt, lse, Dsum, dqkv);
+      return;
+    }
     const int wg = (warp - 4) >> 2;                             // keys [64 wg, 64 wg + 64) of the tile
     const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
     const int c0 = 2 * (lane & 3);
@@ -557,18 +691,18 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
 }
 
 // dQ for one tile of 128 queries.  Fixed: Q, dO.  Ring: (K, V) tiles of 64 keys below the length (kKeyPadding), or
-// inside the union of the query rows' intervals (kSegment, kCausal).
-template <int kMode>
+// inside the union of the query rows' intervals (kSegment, kCausal).  kGqa: K / V from the query head's K/V head.
+template <int kMode, bool kGqa = false>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
                    const int* __restrict__ mask, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
-                   __nv_bfloat16* __restrict__ dqkv) {
+                   __nv_bfloat16* __restrict__ dqkv, int Hkv) {
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
   const int3 tc = tile_coords<kMode, false>();
   const int qt = tc.x, h = tc.y, b = tc.z;
   const int HD = H * kHd;
-  const size_t pitch = (size_t)3 * HD;
+  const size_t pitch = kGqa ? (size_t)(H + 2 * Hkv) * kHd : (size_t)3 * HD;
   const size_t seq_row = (size_t)b * S;
   int len = 0, kt0 = 0, kt_end = 0;
   bool hidden;
@@ -594,8 +728,14 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
     if (lane == 0) {
       tma_prefetch_desc(&map_qkv);
       tma_prefetch_desc(&map_do);
-      bwd_produce(L, &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + qt * 128,
-                  &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row + 64 * kt0, n_kt);
+      if constexpr (kGqa) {
+        const int2 kv = kv_cols<kGqa>(h, H, HD, Hkv);
+        bwd_produce(L, &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + qt * 128,
+                    &map_qkv, kv.x, &map_qkv, kv.y, (int)seq_row + 64 * kt0, n_kt);
+      } else {
+        bwd_produce(L, &map_qkv, h * kHd, &map_do, h * kHd, (int)seq_row + qt * 128,
+                    &map_qkv, HD + h * kHd, &map_qkv, 2 * HD + h * kHd, (int)seq_row + 64 * kt0, n_kt);
+      }
     }
   } else if (warp >= 4) {
     const int wg = (warp - 4) >> 2;
@@ -665,73 +805,91 @@ CUtensorMap rows_map(const void* ptr, int rows, int cols) {
   return conv_encode_map(ptr, 2, dims, strides, box);
 }
 
-void check_shape(const char* who, int B, int S, int heads) {
+// heads query heads and kv_heads K/V heads (equal for multi-head attention; a divisor of heads for GQA)
+void check_shape(const char* who, int B, int S, int heads, int kv_heads) {
   if (B < 1 || heads < 1 || S < 128 || S % 128 != 0)
     throw std::runtime_error(std::string(who) + ": needs B >= 1, heads >= 1 and S a positive multiple of 128 (got B=" +
                              std::to_string(B) + ", S=" + std::to_string(S) + ", heads=" + std::to_string(heads) + ")");
-  if (B > 65535 || (long long)B * S * 3 * heads * kHd >= (1ll << 31))
+  if (kv_heads < 1 || heads % kv_heads != 0)
+    throw std::runtime_error(std::string(who) + ": kv_heads must divide heads (got heads=" + std::to_string(heads) +
+                             ", kv_heads=" + std::to_string(kv_heads) + ")");
+  if (B > 65535 || (long long)B * S * (heads + 2 * kv_heads) * kHd >= (1ll << 31))
     throw std::runtime_error(std::string(who) + ": problem too large");
 }
 
-template <int kMode>
-void attention_fwd(const char* who, const void* qkv, const int* mask, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
-  check_shape(who, B, S, heads);
-  const CUtensorMap map_qkv = rows_map(qkv, B * S, 3 * heads * kHd);
+template <int kMode, bool kGqa = false>
+void attention_fwd(const char* who, const void* qkv, const int* mask, int B, int S, int heads, void* o, float* lse, cudaStream_t s,
+                   int kv_heads) {
+  check_shape(who, B, S, heads, kv_heads);
+  const CUtensorMap map_qkv = rows_map(qkv, B * S, (heads + 2 * kv_heads) * kHd);
   static std::atomic<unsigned long long> configured{0};
-  ensure_max_dynamic_smem(attn_fwd_kernel<kMode>, kFwdSmem, configured);
-  attn_fwd_kernel<kMode><<<dim3(S / 128, heads, B), kThreads, kFwdSmem, s>>>(map_qkv, mask, S, heads,
-                                                                             reinterpret_cast<__nv_bfloat16*>(o), lse);
+  ensure_max_dynamic_smem(attn_fwd_kernel<kMode, kGqa>, kFwdSmem, configured);
+  attn_fwd_kernel<kMode, kGqa><<<dim3(S / 128, heads, B), kThreads, kFwdSmem, s>>>(
+      map_qkv, mask, S, heads, reinterpret_cast<__nv_bfloat16*>(o), lse, kv_heads);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 
-template <int kMode>
+template <int kMode, bool kGqa = false>
 void attention_bwd(const char* who, const void* dout, const void* qkv, const void* o, const float* lse, const int* mask, int B,
-                   int S, int heads, float* dsum, void* dqkv, cudaStream_t s) {
-  check_shape(who, B, S, heads);
+                   int S, int heads, float* dsum, void* dqkv, cudaStream_t s, int kv_heads) {
+  check_shape(who, B, S, heads, kv_heads);
   const int rows = B * S;
   const long long items = (long long)rows * heads * 8;
   attn_bwd_dot_kernel<<<ceil_div(items, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dout),
                                                            reinterpret_cast<const __nv_bfloat16*>(o), rows, S, heads, dsum);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
-  const CUtensorMap map_qkv = rows_map(qkv, rows, 3 * heads * kHd);
+  const CUtensorMap map_qkv = rows_map(qkv, rows, (heads + 2 * kv_heads) * kHd);
   const CUtensorMap map_do = rows_map(dout, rows, heads * kHd);
   auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
   static std::atomic<unsigned long long> configured_dkdv{0}, configured_dq{0};
-  ensure_max_dynamic_smem(attn_bwd_dkdv_kernel<kMode>, kBwdSmem, configured_dkdv);
-  ensure_max_dynamic_smem(attn_bwd_dq_kernel<kMode>, kBwdSmem, configured_dq);
-  attn_bwd_dkdv_kernel<kMode><<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, mask, S, heads, lse, dsum, dq);
+  ensure_max_dynamic_smem(attn_bwd_dkdv_kernel<kMode, kGqa>, kBwdSmem, configured_dkdv);
+  ensure_max_dynamic_smem(attn_bwd_dq_kernel<kMode, kGqa>, kBwdSmem, configured_dq);
+  // dK / dV: one CTA per (key tile, K/V head, batch)
+  attn_bwd_dkdv_kernel<kMode, kGqa><<<dim3(S / 128, kGqa ? kv_heads : heads, B), kThreads, kBwdSmem, s>>>(
+      map_qkv, map_do, mask, S, heads, lse, dsum, dq, kv_heads);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
-  attn_bwd_dq_kernel<kMode><<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(map_qkv, map_do, mask, S, heads, lse, dsum, dq);
+  attn_bwd_dq_kernel<kMode, kGqa><<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(
+      map_qkv, map_do, mask, S, heads, lse, dsum, dq, kv_heads);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 
 }  // namespace
 
 void launch_attention_fwd(const void* qkv, const int* seq_lens, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
-  attention_fwd<kKeyPadding>("attention_fwd", qkv, seq_lens, B, S, heads, o, lse, s);
+  attention_fwd<kKeyPadding>("attention_fwd", qkv, seq_lens, B, S, heads, o, lse, s, heads);
 }
 
 void launch_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* seq_lens, int B, int S,
                           int heads, float* dsum, void* dqkv, cudaStream_t s) {
-  attention_bwd<kKeyPadding>("attention_bwd", dout, qkv, o, lse, seq_lens, B, S, heads, dsum, dqkv, s);
+  attention_bwd<kKeyPadding>("attention_bwd", dout, qkv, o, lse, seq_lens, B, S, heads, dsum, dqkv, s, heads);
 }
 
 void launch_packed_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
-  attention_fwd<kSegment>("packed_attention_fwd", qkv, bounds, B, S, heads, o, lse, s);
+  attention_fwd<kSegment>("packed_attention_fwd", qkv, bounds, B, S, heads, o, lse, s, heads);
 }
 
 void launch_packed_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
                                  int S, int heads, float* dsum, void* dqkv, cudaStream_t s) {
-  attention_bwd<kSegment>("packed_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s);
+  attention_bwd<kSegment>("packed_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s, heads);
 }
 
 void launch_causal_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
-  attention_fwd<kCausal>("causal_attention_fwd", qkv, bounds, B, S, heads, o, lse, s);
+  attention_fwd<kCausal>("causal_attention_fwd", qkv, bounds, B, S, heads, o, lse, s, heads);
 }
 
 void launch_causal_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
                                  int S, int heads, float* dsum, void* dqkv, cudaStream_t s) {
-  attention_bwd<kCausal>("causal_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s);
+  attention_bwd<kCausal>("causal_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s, heads);
+}
+
+void launch_causal_gqa_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, int kv_heads, void* o, float* lse,
+                                     cudaStream_t s) {
+  attention_fwd<kCausal, true>("causal_gqa_attention_fwd", qkv, bounds, B, S, heads, o, lse, s, kv_heads);
+}
+
+void launch_causal_gqa_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                     int S, int heads, int kv_heads, float* dsum, void* dqkv, cudaStream_t s) {
+  attention_bwd<kCausal, true>("causal_gqa_attention_bwd", dout, qkv, o, lse, bounds, B, S, heads, dsum, dqkv, s, kv_heads);
 }
 
 }  // namespace b200

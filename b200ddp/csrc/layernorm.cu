@@ -84,6 +84,8 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_bwd_kernel(const T* __re
 // ---- fast path: cols % 8 == 0 and cols <= 1024 (BERT hidden 768/1024) ----------------------------------
 // A lane owns up to 4 chunks of 8 consecutive columns (chunk c covers columns [8*(lane+32c), +8)): one
 // 16-byte load per chunk, the row lives in registers, statistics need no second pass over memory.
+// kRms (RMSNorm, y = x * rsqrt(mean(x^2) + eps) * gamma): no mean (mu = 0, `mean` is not written or read), no beta;
+// dx = rs * (dy*gamma - xn * mean(dy*gamma*xn)) and dgamma = sum dy * xn from the same column reduction.
 constexpr int kLnChunks = 4;
 
 template <typename T> __device__ __forceinline__ void ln_load8(const T* p, float* f);
@@ -103,7 +105,7 @@ template <> __device__ __forceinline__ void ln_store8<__nv_bfloat16>(__nv_bfloat
   *reinterpret_cast<Bf16x8*>(p) = pack8(f);
 }
 
-template <typename T>
+template <typename T, bool kRms = false>
 __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T* __restrict__ x, const T* __restrict__ gamma,
                                                                         const T* __restrict__ beta, int rows, int cols, float eps,
                                                                         T* __restrict__ y, float* __restrict__ mean, float* __restrict__ rstd) {
@@ -113,7 +115,15 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T*
 #pragma unroll
   for (int c = 0; c < kLnChunks; ++c) {
     const int ch = lane + 32 * c;
-    if (ch < nchunk) { ln_load8<T>(gamma + 8 * ch, g[c]); ln_load8<T>(beta + 8 * ch, b[c]); }
+    if (ch < nchunk) {
+      ln_load8<T>(gamma + 8 * ch, g[c]);
+      if constexpr (kRms) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) b[c][j] = 0.f;
+      } else {
+        ln_load8<T>(beta + 8 * ch, b[c]);
+      }
+    }
   }
   const float inv = 1.f / (float)cols;
   for (int row = blockIdx.x * warps + (threadIdx.x >> 5); row < rows; row += gridDim.x * warps) {
@@ -129,7 +139,7 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T*
         for (int j = 0; j < 8; ++j) s += v[c][j];
       }
     }
-    const float mu = warp_sum(s) * inv;
+    const float mu = kRms ? 0.f : warp_sum(s) * inv;
     float q = 0.f;
 #pragma unroll
     for (int c = 0; c < kLnChunks; ++c) {
@@ -146,16 +156,19 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T*
       if (ch < nchunk) {
         float o[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mu) * rs * g[c][j] + b[c][j];
+        for (int j = 0; j < 8; ++j) o[j] = kRms ? v[c][j] * rs * g[c][j] : (v[c][j] - mu) * rs * g[c][j] + b[c][j];
         ln_store8<T>(yr + 8 * ch, o);
       }
     }
-    if (lane == 0) { mean[row] = mu; rstd[row] = rs; }
+    if (lane == 0) {
+      if constexpr (!kRms) mean[row] = mu;
+      rstd[row] = rs;
+    }
   }
 }
 
 // dx only: rows live in registers, no cross-row state -> light enough for 2 CTAs per SM.
-template <typename T>
+template <typename T, bool kRms = false>
 __global__ void __launch_bounds__(kLnThreads, 2) layernorm_bwd_dx_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ gamma,
                                                                          const float* __restrict__ mean, const float* __restrict__ rstd, int rows,
                                                                          int cols, T* __restrict__ dx) {
@@ -171,7 +184,7 @@ __global__ void __launch_bounds__(kLnThreads, 2) layernorm_bwd_dx_kernel(const T
   for (int row = blockIdx.x * warps + (threadIdx.x >> 5); row < rows; row += gridDim.x * warps) {
     const T* xr = x + (size_t)row * cols;
     const T* dyr = dy + (size_t)row * cols;
-    const float mu = mean[row], rs = rstd[row];
+    const float mu = kRms ? 0.f : mean[row], rs = rstd[row];
     float xn[kLnChunks][8], d[kLnChunks][8];
     float s1 = 0.f, s2 = 0.f;
 #pragma unroll
@@ -189,7 +202,7 @@ __global__ void __launch_bounds__(kLnThreads, 2) layernorm_bwd_dx_kernel(const T
         }
       }
     }
-    s1 = warp_sum(s1) * inv;
+    s1 = kRms ? 0.f : warp_sum(s1) * inv;
     s2 = warp_sum(s2) * inv;
     T* dxr = dx + (size_t)row * cols;
 #pragma unroll
@@ -208,7 +221,7 @@ __global__ void __launch_bounds__(kLnThreads, 2) layernorm_bwd_dx_kernel(const T
 // dgamma / dbeta: column reduction over rows (same scheme as the BatchNorm reductions): threads own 8 columns,
 // rows are strided over the block and over gridDim.y splits, the last block of a column tile sums the partials
 // in a fixed order.  Re-reads dy and x, which are L2-resident right after the dx kernel.
-template <typename T>
+template <typename T, bool kRms = false>
 __global__ void __launch_bounds__(kLnThreads) layernorm_param_grad_kernel(const T* __restrict__ dy, const T* __restrict__ x,
                                                                           const float* __restrict__ mean, const float* __restrict__ rstd, int rows,
                                                                           int cols, int cvb, int ty, float* __restrict__ partial,
@@ -233,7 +246,7 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_param_grad_kernel(const 
       ln_load8<T>(x + (size_t)r * cols + col, x0);
       ln_load8<T>(dy + (size_t)(r + ty) * cols + col, d1);
       ln_load8<T>(x + (size_t)(r + ty) * cols + col, x1);
-      const float m0 = mean[r], s0 = rstd[r], m1 = mean[r + ty], s1 = rstd[r + ty];
+      const float m0 = kRms ? 0.f : mean[r], s0 = rstd[r], m1 = kRms ? 0.f : mean[r + ty], s1 = rstd[r + ty];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         ab[i] += d0[i] + d1[i];
@@ -245,7 +258,7 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_param_grad_kernel(const 
       float d0[8], x0[8];
       ln_load8<T>(dy + (size_t)r * cols + col, d0);
       ln_load8<T>(x + (size_t)r * cols + col, x0);
-      const float m0 = mean[r], s0 = rstd[r];
+      const float m0 = kRms ? 0.f : mean[r], s0 = rstd[r];
 #pragma unroll
       for (int i = 0; i < 8; ++i) { ab[i] += d0[i]; ag[i] = fmaf(d0[i], (x0[i] - m0) * s0, ag[i]); }
     }
@@ -276,7 +289,7 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_param_grad_kernel(const 
     float sg = 0.f, sb = 0.f;
     for (int k = 0; k < S; ++k) { sg += __ldcg(&partial[(size_t)(0 * S + k) * cols + ch]); sb += __ldcg(&partial[(size_t)(1 * S + k) * cols + ch]); }
     dgamma[ch] = from_f32<T>(sg);
-    dbeta[ch] = from_f32<T>(sb);
+    if constexpr (!kRms) dbeta[ch] = from_f32<T>(sb);
   }
   if (threadIdx.x == 0) counters[blockIdx.x] = 0u;
 }
@@ -293,6 +306,29 @@ __global__ void layernorm_bwd_finish_kernel(const float* __restrict__ dgamma_par
 }
 
 }  // namespace
+
+// Launch geometry of the fast path's backward (dx kernel + column-reduce kernel), shared by LayerNorm and RMSNorm:
+// cvb 8-column vectors x ty rows per reduce block, a gx x gy reduce grid (gy <= max_gy row splits), dx_blocks dx CTAs.
+struct LnBwdGeometry {
+  int cvb, ty, gx, gy, dx_blocks;
+  size_t psmem;
+};
+LnBwdGeometry ln_bwd_geometry(int rows, int cols, int max_gy) {
+  LnBwdGeometry g;
+  const int cv = cols / 8;
+  g.cvb = cv < 32 ? cv : 32;
+  while (kLnThreads % g.cvb != 0) --g.cvb;
+  g.ty = kLnThreads / g.cvb;
+  g.gx = (cv + g.cvb - 1) / g.cvb;
+  g.gy = (4 * kNumSMs + g.gx - 1) / g.gx;
+  const int by_rows = rows / (g.ty * 4) < 1 ? 1 : rows / (g.ty * 4);
+  if (g.gy > by_rows) g.gy = by_rows;
+  if (g.gy > max_gy) g.gy = max_gy < 1 ? 1 : max_gy;               // capacity of the partial buffer
+  g.dx_blocks = (rows + 7) / 8;
+  if (g.dx_blocks > 16 * kNumSMs) g.dx_blocks = 16 * kNumSMs;
+  g.psmem = (size_t)2 * kLnThreads * 8 * sizeof(float);
+  return g;
+}
 
 int layernorm_partial_rows(int rows) {
   int p = (rows + 63) / 64;
@@ -333,18 +369,9 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
                       reinterpret_cast<uintptr_t>(gamma)) & 31u) == 0;
   if (fast) {
     // workspace carved from the caller's partial buffers: dgamma_partial = [2][S][cols] partial sums, dbeta_partial = counters
-    const int cv = cols / 8;
-    int cvb = cv < 32 ? cv : 32;
-    while (kLnThreads % cvb != 0) --cvb;
-    const int ty = kLnThreads / cvb;
-    const int gx = (cv + cvb - 1) / cvb;
-    int gy = (4 * kNumSMs + gx - 1) / gx;
-    const int by_rows = rows / (ty * 4) < 1 ? 1 : rows / (ty * 4);
-    if (gy > by_rows) gy = by_rows;
-    if (gy > partial_rows / 2) gy = partial_rows / 2 < 1 ? 1 : partial_rows / 2;     // capacity of the partial buffer
-    int blocks = (rows + 7) / 8;
-    if (blocks > 16 * kNumSMs) blocks = 16 * kNumSMs;
-    const size_t psmem = (size_t)2 * kLnThreads * 8 * sizeof(float);
+    const LnBwdGeometry geo = ln_bwd_geometry(rows, cols, partial_rows / 2);
+    const int cvb = geo.cvb, ty = geo.ty, gx = geo.gx, gy = geo.gy, blocks = geo.dx_blocks;
+    const size_t psmem = geo.psmem;
     unsigned int* counters = reinterpret_cast<unsigned int*>(dbeta_partial);
     B200_CUDA_CHECK(cudaMemsetAsync(counters, 0, sizeof(unsigned int) * gx, s));   // fresh scratch from the caller
     if (dt == DType::BF16) {
@@ -370,6 +397,56 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
                                                                      rows, cols, (float*)dx, dgamma_partial, dbeta_partial);
     layernorm_bwd_finish_kernel<float><<<(cols + 255) / 256, 256, 0, s>>>(dgamma_partial, dbeta_partial, partial_rows, cols,
                                                                         (float*)dgamma, (float*)dbeta);
+  }
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+bool rmsnorm_supported(int cols) { return cols % 8 == 0 && cols >= 8 && cols <= 8 * 32 * kLnChunks; }
+
+// RMSNorm on the LayerNorm fast path (the only path it has): x, y, gamma 32-byte aligned, rstd [rows]
+void launch_rmsnorm_fwd(const void* x, const void* gamma, DType dt, int rows, int cols, float eps, void* y, float* rstd,
+                        cudaStream_t s) {
+  if (!rmsnorm_supported(cols) ||
+      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(gamma)) & 31u) != 0)
+    throw std::runtime_error("rmsnorm_fwd: needs cols % 8 == 0, cols <= 1024 and 32-byte aligned tensors (cols=" +
+                             std::to_string(cols) + ")");
+  int blocks = (rows + 7) / 8;
+  if (blocks > 8 * kNumSMs) blocks = 8 * kNumSMs;
+  if (blocks < 1) blocks = 1;
+  if (dt == DType::BF16)
+    layernorm_fwd_fast_kernel<__nv_bfloat16, true><<<blocks, kLnThreads, 0, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)gamma,
+                                                                               nullptr, rows, cols, eps, (__nv_bfloat16*)y, nullptr, rstd);
+  else
+    layernorm_fwd_fast_kernel<float, true><<<blocks, kLnThreads, 0, s>>>((const float*)x, (const float*)gamma, nullptr, rows, cols, eps,
+                                                                       (float*)y, nullptr, rstd);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+// partial: fp32 [2 * partial_rows, cols] workspace, counters: uint32 [>= cols / 8] workspace (zeroed here)
+void launch_rmsnorm_bwd(const void* dy, const void* x, const void* gamma, const float* rstd, DType dt, int rows, int cols, void* dx,
+                        float* partial, unsigned int* counters, int partial_rows, void* dgamma, cudaStream_t s) {
+  if (!rmsnorm_supported(cols) ||
+      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx) |
+        reinterpret_cast<uintptr_t>(gamma)) & 31u) != 0)
+    throw std::runtime_error("rmsnorm_bwd: needs cols % 8 == 0, cols <= 1024 and 32-byte aligned tensors (cols=" +
+                             std::to_string(cols) + ")");
+  const LnBwdGeometry geo = ln_bwd_geometry(rows, cols, partial_rows);
+  const int cvb = geo.cvb, ty = geo.ty, gx = geo.gx, gy = geo.gy, blocks = geo.dx_blocks < 1 ? 1 : geo.dx_blocks;
+  const size_t psmem = geo.psmem;
+  B200_CUDA_CHECK(cudaMemsetAsync(counters, 0, sizeof(unsigned int) * gx, s));
+  if (dt == DType::BF16) {
+    layernorm_bwd_dx_kernel<__nv_bfloat16, true><<<blocks, kLnThreads, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
+                                                                             (const __nv_bfloat16*)gamma, nullptr, rstd, rows, cols,
+                                                                             (__nv_bfloat16*)dx);
+    layernorm_param_grad_kernel<__nv_bfloat16, true><<<dim3(gx, gy), kLnThreads, psmem, s>>>(
+        (const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, nullptr, rstd, rows, cols, cvb, ty, partial, counters,
+        (__nv_bfloat16*)dgamma, nullptr);
+  } else {
+    layernorm_bwd_dx_kernel<float, true><<<blocks, kLnThreads, 0, s>>>((const float*)dy, (const float*)x, (const float*)gamma, nullptr,
+                                                                     rstd, rows, cols, (float*)dx);
+    layernorm_param_grad_kernel<float, true><<<dim3(gx, gy), kLnThreads, psmem, s>>>((const float*)dy, (const float*)x, nullptr, rstd,
+                                                                                   rows, cols, cvb, ty, partial, counters,
+                                                                                   (float*)dgamma, nullptr);
   }
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }

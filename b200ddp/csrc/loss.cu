@@ -333,3 +333,63 @@ void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n,
 }
 
 }  // namespace b200
+
+// ---------------------------------------------------------------------------------------------------------
+// SwiGLU (Llama MLP): in = [M, 2I] bf16 with column blocks gate | up, out = silu(gate) * up [M, I].  The backward writes
+// d[gate | up] [M, 2I] in one pass: dgate = dy * up * silu'(gate), dup = dy * silu(gate), silu'(g) = s (1 + g (1 - s)),
+// s = sigmoid(g).  One thread per 8 consecutive columns (I % 8 == 0), 16-byte loads and stores.
+namespace b200 {
+namespace {
+
+template <bool BWD>
+__global__ void __launch_bounds__(kLossThreads) swiglu_kernel(const __nv_bfloat16* __restrict__ in, const __nv_bfloat16* __restrict__ dy,
+                                                              __nv_bfloat16* __restrict__ out, size_t rows, int inter) {
+  const int vpr = inter / 8;                                    // 8-column vectors per row
+  const size_t n = rows * (size_t)vpr;
+  for (size_t v = (size_t)blockIdx.x * blockDim.x + threadIdx.x; v < n; v += (size_t)gridDim.x * blockDim.x) {
+    const size_t r = v / vpr;
+    const int c = (int)(v - r * vpr) * 8;
+    const __nv_bfloat16* gp = in + r * 2 * inter + c;
+    float g[8], u[8];
+    unpack8(*reinterpret_cast<const Bf16x8*>(gp), g);
+    unpack8(*reinterpret_cast<const Bf16x8*>(gp + inter), u);
+    if constexpr (BWD) {
+      float d[8], dg[8], du[8];
+      unpack8(*reinterpret_cast<const Bf16x8*>(dy + r * inter + c), d);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float sg = 1.f / (1.f + expf(-g[i]));
+        du[i] = d[i] * g[i] * sg;
+        dg[i] = d[i] * u[i] * sg * (1.f + g[i] * (1.f - sg));
+      }
+      __nv_bfloat16* op = out + r * 2 * inter + c;
+      *reinterpret_cast<Bf16x8*>(op) = pack8(dg);
+      *reinterpret_cast<Bf16x8*>(op + inter) = pack8(du);
+    } else {
+      float o[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) o[i] = g[i] / (1.f + expf(-g[i])) * u[i];
+      *reinterpret_cast<Bf16x8*>(out + r * inter + c) = pack8(o);
+    }
+  }
+}
+
+}  // namespace
+
+void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s) {
+  if (inter % 8 != 0 || ((reinterpret_cast<uintptr_t>(gate_up) | reinterpret_cast<uintptr_t>(out) |
+                          reinterpret_cast<uintptr_t>(dy)) & 15u) != 0)
+    throw std::runtime_error("swiglu: needs the intermediate size a multiple of 8 and 16-byte aligned tensors (inter=" +
+                             std::to_string(inter) + ")");
+  size_t b = (rows * (inter / 8) + kLossThreads - 1) / kLossThreads;
+  if (b < 1) b = 1;
+  if (b > (size_t)16 * kNumSMs) b = (size_t)16 * kNumSMs;
+  const auto* in = reinterpret_cast<const __nv_bfloat16*>(gate_up);
+  if (backward)
+    swiglu_kernel<true><<<(int)b, kLossThreads, 0, s>>>(in, reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<__nv_bfloat16*>(out), rows, inter);
+  else
+    swiglu_kernel<false><<<(int)b, kLossThreads, 0, s>>>(in, nullptr, reinterpret_cast<__nv_bfloat16*>(out), rows, inter);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+}  // namespace b200

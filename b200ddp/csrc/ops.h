@@ -66,6 +66,16 @@ void launch_xent_fwd_bwd(const void* logits, const long long* targets, DType dt,
 // with `tanh` the tanh approximation 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3))) (GPT-2's MLP).
 void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s, bool tanh = false);
 
+// SwiGLU: forward out[M, I] = silu(gate) * up from gate_up bf16 [M, 2I] (gate | up); backward out[M, 2I] = d[gate | up]
+// from dy [M, I].  I % 8 == 0, 16-byte aligned tensors (loss.cu).
+void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s);
+
+// ---------------- rotary position embedding (rotary.cu) ----------------------------------------------
+// qkv bf16 [rows, (heads + 2*kv_heads)*64] -> y (same shape): query and key heads rotated by position pos[r] (int32,
+// clamped to [0, max_pos)), value heads copied; table fp32 [max_pos, 2, 32] (cos | sin).  backward: the transpose rotation.
+void launch_rotary(const void* x, const int* pos, const float* table, int max_pos, size_t rows, int heads, int kv_heads, void* y,
+                   bool backward, cudaStream_t s);
+
 // ---------------- layer norm (layernorm.cu) -----------------------------------------------------
 void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, DType dt, int rows, int cols,
                           float eps, void* y, float* mean, float* rstd, cudaStream_t s);
@@ -73,6 +83,12 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
                           DType dt, int rows, int cols, void* dx, float* dgamma_partial, float* dbeta_partial,
                           int partial_rows, void* dgamma, void* dbeta, cudaStream_t s);
 int layernorm_partial_rows(int rows);
+// RMSNorm, y = x * rsqrt(mean(x^2) + eps) * gamma, on the LayerNorm fast path: cols % 8 == 0, cols <= 1024, 32-byte
+// aligned tensors.  rstd fp32 [rows]; backward workspace partial fp32 [2 * partial_rows, cols], counters uint32 [cols / 8].
+bool rmsnorm_supported(int cols);
+void launch_rmsnorm_fwd(const void* x, const void* gamma, DType dt, int rows, int cols, float eps, void* y, float* rstd, cudaStream_t s);
+void launch_rmsnorm_bwd(const void* dy, const void* x, const void* gamma, const float* rstd, DType dt, int rows, int cols, void* dx,
+                        float* partial, unsigned int* counters, int partial_rows, void* dgamma, cudaStream_t s);
 
 // ---------------- FP8 quantisation, current per-tensor power-of-two scaling (fp8.cu) ------------------
 // amax[0] = max |x| over n bf16 elements (x 16-byte aligned); zeroes amax first, so the two launches are graph-capturable.
@@ -103,6 +119,12 @@ void launch_packed_attention_bwd(const void* dout, const void* qkv, const void* 
 void launch_causal_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, void* o, float* lse, cudaStream_t s);
 void launch_causal_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
                                  int S, int heads, float* dsum, void* dqkv, cudaStream_t s);
+// Grouped-query causal documents: qkv (and dqkv) bf16 [B*S, (heads + 2*kv_heads)*64], query | key | value column blocks;
+// query head h reads K/V head h / (heads / kv_heads).  o, lse, dout and dsum as above (heads query heads).
+void launch_causal_gqa_attention_fwd(const void* qkv, const int* bounds, int B, int S, int heads, int kv_heads, void* o, float* lse,
+                                     cudaStream_t s);
+void launch_causal_gqa_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                     int S, int heads, int kv_heads, float* dsum, void* dqkv, cudaStream_t s);
 
 // ---------------- small linears on CUDA cores (linear_small.cu) ------------------------------
 // y[M,N] = act(x[M,K] w[N,K]^T + b[N]) ; fp32, dims far below one tensor-core tile (FooModel).

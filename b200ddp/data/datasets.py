@@ -84,14 +84,16 @@ class SyntheticTokens(Dataset):
     ``causal=True`` gives causal-LM rows (GPT) in the same three layouts: within a document ``labels[t] = ids[t + 1]``,
     and each document's last token and the padding are labelled -100.  Tokens come from [1, vocab); packed documents
     start with ``BOS_ID`` instead of ``CLS_ID`` (and hold no other ``BOS_ID``), and ``bos_token_id`` is set instead of
-    ``cls_token_id``."""
+    ``cls_token_id``.  ``bos_token_id`` picks another start id for causal packed documents (1, Llama's ``<s>``, for
+    SmolLM); GPT-2's 50256 stays the default."""
 
     PAD_ID = 0
     CLS_ID = 101                   # [CLS] in the BERT vocabulary
     BOS_ID = 50256                 # <|endoftext|> in the GPT-2 vocabulary, which starts each GPT-2 document
+    LLAMA_BOS_ID = 1               # <s> in the Llama / SmolLM vocabularies
 
     def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 30522, mask_prob: float = 0.15, seed: int = 1234,
-                 min_len: int | None = None, pack: bool = False, causal: bool = False):
+                 min_len: int | None = None, pack: bool = False, causal: bool = False, bos_token_id: int | None = None):
         if min_len is not None and not 1 <= min_len <= seq_len:
             raise ValueError(f"SyntheticTokens: min_len must lie in [1, seq_len = {seq_len}], got {min_len}")
         g = torch.Generator().manual_seed(seed)
@@ -102,7 +104,7 @@ class SyntheticTokens(Dataset):
         self.bos_token_id = None
         self.doc_ids = self.doc_lengths = None
         if pack:
-            self._pack(g, seq_len, vocab, mask_prob, seq_len if min_len is None else min_len, causal)
+            self._pack(g, seq_len, vocab, mask_prob, seq_len if min_len is None else min_len, causal, bos_token_id)
             return
         if causal:
             self._causal_rows(g, seq_len, vocab, min_len)
@@ -132,8 +134,11 @@ class SyntheticTokens(Dataset):
         self.Y = torch.cat([self.X[:, 1:], torch.full((self.samples, 1), -100)], 1)
         self.Y.masked_fill_(torch.arange(seq_len)[None, :] >= (length - 1)[:, None], -100)
 
-    def _pack(self, g: torch.Generator, seq_len: int, vocab: int, mask_prob: float, min_len: int, causal: bool = False) -> None:
-        start_id = self.BOS_ID if causal else self.CLS_ID
+    def _pack(self, g: torch.Generator, seq_len: int, vocab: int, mask_prob: float, min_len: int, causal: bool = False,
+              bos_token_id: int | None = None) -> None:
+        start_id = (self.BOS_ID if bos_token_id is None else bos_token_id) if causal else self.CLS_ID
+        if causal and (start_id == self.PAD_ID or not 0 < start_id < vocab):
+            raise ValueError(f"SyntheticTokens: the start id must lie in [1, vocab = {vocab}) and differ from PAD_ID, got {start_id}")
         need = start_id if causal else start_id + 1
         if vocab <= need:
             raise ValueError(f"SyntheticTokens: packing needs vocab > {need} (token {start_id} starts a document)")

@@ -64,17 +64,17 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--channels_last", action="store_true")
     p.add_argument("--cuda_graph", action="store_true", help="capture the whole optimizer step in a CUDA graph")
     p.add_argument("--fp8", action="store_true",
-                   help="BERT encoder / GPT-2 block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs --model "
-                        "bert-base or gpt2, --fp16 and a GPU")
+                   help="BERT encoder / GPT-2 / SmolLM block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs "
+                        "--model bert-base, gpt2 or smollm-135m, --fp16 and a GPU")
     p.add_argument("--min_seq_len", type=int, default=None,
-                   help="BERT / GPT-2 on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
+                   help="BERT / GPT-2 / SmolLM on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
                         "keys are hidden from attention (native key-padding or causal kernel on the GPU; needs --fp16 and "
                         "--seq_len %% 128 == 0 there).  Default: fixed-length rows")
     p.add_argument("--pack", action="store_true",
-                   help="BERT / GPT-2 on packed documents: documents with lengths uniform in [--min_seq_len, --seq_len], "
-                        "each starting with [CLS] (BERT) or <|endoftext|> (GPT-2), packed first-fit decreasing into rows; "
+                   help="BERT / GPT-2 / SmolLM on packed documents: documents with lengths uniform in [--min_seq_len, "
+                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2) or <s> (SmolLM), packed first-fit decreasing into rows; "
                         "attention stays inside a document (native document-boundary or causal kernel on the GPU).  Needs "
-                        "--model bert-base or gpt2 and --min_seq_len < --seq_len")
+                        "--model bert-base, gpt2 or smollm-135m and --min_seq_len < --seq_len")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -141,8 +141,11 @@ def setup(args):
 
 
 # models whose token rows can be right-padded or packed, and whose block linears can run on FP8
-TOKEN_MODELS = ("bert-base", "gpt2")
+TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m")
+# causal LMs: their packed documents start with a BOS id
+CAUSAL_MODELS = ("gpt2", "smollm-135m")
 GPT2_MAX_SEQ_LEN = 1024
+SMOLLM_MAX_SEQ_LEN = 2048
 
 
 def check_gpt_args(args) -> None:
@@ -150,6 +153,9 @@ def check_gpt_args(args) -> None:
     if args.model == "gpt2" and args.seq_len > GPT2_MAX_SEQ_LEN:
         raise ValueError(f"--model gpt2 has {GPT2_MAX_SEQ_LEN} positions; --seq_len must be at most {GPT2_MAX_SEQ_LEN} "
                          f"(got {args.seq_len})")
+    if args.model == "smollm-135m" and args.seq_len > SMOLLM_MAX_SEQ_LEN:
+        raise ValueError(f"--model smollm-135m has {SMOLLM_MAX_SEQ_LEN} positions; --seq_len must be at most "
+                         f"{SMOLLM_MAX_SEQ_LEN} (got {args.seq_len})")
 
 
 def check_fp8_args(args) -> None:
@@ -157,8 +163,8 @@ def check_fp8_args(args) -> None:
     if not getattr(args, "fp8", False):
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--fp8 covers the BERT encoder and GPT-2 block linears only; it needs --model bert-base or gpt2 "
-                         f"(got --model {args.model})")
+        raise ValueError(f"--fp8 covers the block linears of the token models; it needs --model bert-base, gpt2 or "
+                         f"smollm-135m (got --model {args.model})")
     if not args.fp16:
         raise ValueError("--fp8 needs --fp16: the FP8 GEMMs read bf16 activations and weights")
     if getattr(args, "device", None) is None or args.device.type != "cuda":
@@ -172,7 +178,8 @@ def check_min_seq_len_args(args) -> None:
     if n is None:
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (got --model {args.model})")
+        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (or smollm-135m; got --model "
+                         f"{args.model})")
     if not 1 <= n <= args.seq_len:
         raise ValueError(f"--min_seq_len must lie in [1, --seq_len = {args.seq_len}], got {n}")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -188,7 +195,8 @@ def check_pack_args(args) -> None:
     if not getattr(args, "pack", False):
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (got --model {args.model})")
+        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (or smollm-135m; got --model "
+                         f"{args.model})")
     if not padding_on(args):
         raise ValueError("--pack needs --min_seq_len below --seq_len (documents have lengths in [--min_seq_len, --seq_len])")
     check_min_seq_len_args(args)
@@ -225,6 +233,8 @@ def main(argv=None) -> int:
         kwargs["pad_token_id"] = SyntheticTokens.PAD_ID
         if args.pack and args.model == "gpt2":
             kwargs["bos_token_id"] = SyntheticTokens.BOS_ID
+        elif args.pack and args.model == "smollm-135m":
+            kwargs["bos_token_id"] = SyntheticTokens.LLAMA_BOS_ID
         elif args.pack:
             kwargs["cls_token_id"] = SyntheticTokens.CLS_ID
     model = build_model(args.model, **kwargs)

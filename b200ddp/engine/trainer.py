@@ -58,6 +58,10 @@ def build_dataset(args):
         return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=50257,
                                min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
                                causal=True)
+    if name == "smollm-135m":                                 # causal-LM rows over SmolLM's vocabulary, <s> starts a document
+        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=49152,
+                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
+                               causal=True, bos_token_id=SyntheticTokens.LLAMA_BOS_ID)
     raise ValueError(f"no default dataset for model {name!r}")
 
 

@@ -3,6 +3,7 @@ from .foo import FooModel, BranchyFooModel
 from .resnet import ResNet, resnet50, resnet152
 from .bert import BertConfig, BertModel, BertForMaskedLM, bert_base
 from .gpt import GPTConfig, GPTModel, GPTLMHeadModel, gpt2
+from .llama import LlamaConfig, LlamaModel, LlamaForCausalLM, smollm_135m
 
 MODEL_REGISTRY = {
     "foo": FooModel,
@@ -10,6 +11,7 @@ MODEL_REGISTRY = {
     "resnet152": resnet152,
     "bert-base": bert_base,
     "gpt2": gpt2,
+    "smollm-135m": smollm_135m,
 }
 
 
@@ -21,4 +23,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "MODEL_REGISTRY", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "MODEL_REGISTRY", "build_model"]

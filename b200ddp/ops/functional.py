@@ -462,23 +462,234 @@ def _causal_mask(bounds: torch.Tensor, S: int, device) -> torch.Tensor:
     return _bounds_mask(bounds, S, device) & (i[None, :] <= i[:, None])
 
 
-def causal_attention_reference(qkv: torch.Tensor, bounds: torch.Tensor, heads: int) -> torch.Tensor:
+def causal_attention_reference(qkv: torch.Tensor, bounds: torch.Tensor, heads: int, kv_heads: Optional[int] = None) -> torch.Tensor:
     """softmax(Q K^T / sqrt(d)) V where query i sees key j of its row iff bounds[b, i, 0] <= j <= i and
     j < bounds[b, i, 1], in fp32 (fp64 stays fp64), as a dense mask; a row that sees no key gives zeros.  qkv
-    [B, S, 3 * hidden], bounds integer [B, S, 2]; returns [B, S, hidden] in qkv's dtype.  Differentiable."""
+    [B, S, 3 * hidden], bounds integer [B, S, 2]; returns [B, S, hidden] in qkv's dtype.  Differentiable.
+    ``kv_heads`` (grouped-query attention): qkv is [B, S, (heads + 2 * kv_heads) * d], query head h reads K/V head
+    h // (heads // kv_heads); K and V are repeated per group (Hugging Face's ``repeat_kv``)."""
+    if kv_heads is not None and kv_heads != heads:
+        qkv = _repeat_kv(qkv, heads, kv_heads)
     return _masked_attention_reference(qkv, _causal_mask(bounds, qkv.shape[1], qkv.device)[:, None], heads)
 
 
-def causal_attention(qkv: torch.Tensor, bounds: torch.Tensor, heads: int) -> torch.Tensor:
+def _repeat_kv(qkv: torch.Tensor, heads: int, kv_heads: int) -> torch.Tensor:
+    """[B, S, (heads + 2 * kv_heads) * d] -> [B, S, 3 * heads * d]: each K/V head repeated heads // kv_heads times."""
+    B, S, Wd = qkv.shape
+    d = Wd // (heads + 2 * kv_heads)
+    q, k, v = qkv.split([heads * d, kv_heads * d, kv_heads * d], dim=-1)
+    rep = heads // kv_heads
+    k, v = (t.reshape(B, S, kv_heads, 1, d).expand(B, S, kv_heads, rep, d).reshape(B, S, heads * d) for t in (k, v))
+    return torch.cat([q, k, v], -1)
+
+
+def _gqa_check(qkv: torch.Tensor, heads: int, kv_heads: int) -> None:
+    if heads < 1 or kv_heads < 1 or heads % kv_heads:
+        raise ValueError(f"grouped-query attention needs kv_heads dividing heads, got heads={heads}, kv_heads={kv_heads}")
+    if qkv.dim() != 3 or qkv.shape[-1] != (heads + 2 * kv_heads) * ATTENTION_HEAD_DIM:
+        raise ValueError(f"grouped-query attention on CUDA needs qkv [B, S, (heads + 2 * kv_heads) * {ATTENTION_HEAD_DIM}] = "
+                         f"[B, S, {(heads + 2 * kv_heads) * ATTENTION_HEAD_DIM}], got {tuple(qkv.shape)}")
+    if qkv.dtype != torch.bfloat16:
+        raise ValueError(f"attention on CUDA needs bf16 qkv, got {qkv.dtype}")
+    S = qkv.shape[1]
+    if S % ATTENTION_SEQ_MULTIPLE or S == 0:
+        raise ValueError(f"attention on CUDA needs the sequence length to be a multiple of {ATTENTION_SEQ_MULTIPLE}, got {S}")
+    if not qkv.is_contiguous():
+        raise ValueError("attention on CUDA needs a contiguous qkv (the fused projection's output)")
+
+
+class _GqaAttention(torch.autograd.Function):
+    """Grouped-query causal-document attention.  CUDA body: the sm_90a GQA kernels (dK / dV accumulate across each group
+    in registers: one writer per element, deterministic).  CPU body: ``causal_attention_reference`` with K / V repeated."""
+
+    @staticmethod
+    def forward(ctx, qkv, bounds, heads, kv_heads):
+        ctx.heads, ctx.kv_heads = heads, kv_heads
+        if qkv.is_cuda:
+            B, S, Wd = qkv.shape
+            m = bounds.to(device=qkv.device, dtype=torch.int32).contiguous()
+            o, lse = _C().causal_gqa_attention_fwd(qkv.view(B * S, Wd), m, heads, kv_heads)
+            ctx.save_for_backward(qkv, o, lse, m)
+            return o.view(B, S, heads * ATTENTION_HEAD_DIM)
+        ctx.save_for_backward(qkv, bounds)
+        return causal_attention_reference(qkv, bounds, heads, kv_heads)
+
+    @staticmethod
+    def backward(ctx, dy):
+        if dy.is_cuda:
+            qkv, o, lse, m = ctx.saved_tensors
+            B, S, Wd = qkv.shape
+            do = dy.reshape(B * S, -1).to(torch.bfloat16).contiguous()
+            if do.data_ptr() % 16:
+                do = do.clone()
+            dqkv = _C().causal_gqa_attention_bwd(do, qkv.view(B * S, Wd), o, lse, m, ctx.heads, ctx.kv_heads)
+            return dqkv.view(B, S, Wd), None, None, None
+        qkv, bounds = ctx.saved_tensors
+        with torch.enable_grad():
+            x = qkv.detach().requires_grad_(True)
+            (g,) = torch.autograd.grad(causal_attention_reference(x, bounds, ctx.heads, ctx.kv_heads), x, dy)
+        return g, None, None, None
+
+
+def causal_attention(qkv: torch.Tensor, bounds: torch.Tensor, heads: int, kv_heads: Optional[int] = None) -> torch.Tensor:
     """Causal multi-head attention inside documents: qkv [B, S, 3 * hidden] (the fused projection's output), bounds
     integer [B, S, 2] (``document_bounds``; with ``cls_token_id=None`` it gives right-padded rows one document each):
     query i of a row sees key j iff start[i] <= j <= i and j < end[i].  Rows with start == end (padding) give zeros and
     get zero gradients.  Returns [B, S, hidden].  On CUDA: bf16, head dim 64, S % 128 == 0 and contiguous qkv, else
-    ``ValueError``; bounds stay on the device (CUDA-graph safe).  Tiles above the diagonal are never visited."""
+    ``ValueError``; bounds stay on the device (CUDA-graph safe).  Tiles above the diagonal are never visited.
+
+    ``kv_heads`` other than None or ``heads`` selects grouped-query attention: qkv is [B, S, (heads + 2 * kv_heads) * 64]
+    (query | key | value column blocks) and query head h reads K/V head h // (heads // kv_heads); the output stays
+    [B, S, heads * 64]."""
+    if kv_heads is not None and kv_heads != heads:
+        if qkv.is_cuda:
+            _gqa_check(qkv, heads, kv_heads)
+            _bounds_check(qkv, bounds, "causal attention")
+        elif heads < 1 or kv_heads < 1 or heads % kv_heads or qkv.dim() != 3 or qkv.shape[-1] % (heads + 2 * kv_heads):
+            raise ValueError(f"grouped-query attention needs kv_heads dividing heads and qkv [B, S, (heads + 2 * kv_heads) * d], "
+                             f"got heads={heads}, kv_heads={kv_heads}, qkv {tuple(qkv.shape)}")
+        return _GqaAttention.apply(qkv, bounds, heads, kv_heads)
     if qkv.is_cuda:
         _qkv_check(qkv, heads)
         _bounds_check(qkv, bounds, "causal attention")
     return _Attention.apply(qkv, bounds, heads, "causal")
+
+
+# ------------------------------------------------------------------------------------------------
+# Llama building blocks: rotary position embedding (csrc/rotary.cu), RMSNorm (csrc/layernorm.cu), SwiGLU (csrc/loss.cu)
+# ------------------------------------------------------------------------------------------------
+def rotary_cos_sin(max_position: int, head_dim: int = ATTENTION_HEAD_DIM, theta: float = 10000.0) -> torch.Tensor:
+    """fp32 [max_position, 2, head_dim // 2]: cos and sin of p * theta^(-2i / head_dim), computed in fp64 on the host."""
+    inv = theta ** (-torch.arange(0, head_dim, 2, dtype=torch.float64) / head_dim)
+    ang = torch.arange(max_position, dtype=torch.float64)[:, None] * inv[None, :]
+    return torch.stack([ang.cos(), ang.sin()], 1).float()
+
+
+def _rotary_reference(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor, heads: int, kv_heads: int,
+                      inverse: bool = False) -> torch.Tensor:
+    B, S, Wd = qkv.shape
+    d = Wd // (heads + 2 * kv_heads)
+    half = d // 2
+    ct = torch.promote_types(qkv.dtype, torch.float32)
+    pos = position_ids.to(device=qkv.device, dtype=torch.long).reshape(B, S).clamp(0, cos_sin.shape[0] - 1)
+    cs = cos_sin.to(device=qkv.device, dtype=ct)[pos]                        # [B, S, 2, half]
+    cos, sin = cs[:, :, None, 0], cs[:, :, None, 1]
+    if inverse:
+        sin = -sin
+    qk, v = qkv.to(ct).split([(heads + kv_heads) * d, kv_heads * d], dim=-1)
+    x = qk.reshape(B, S, heads + kv_heads, d)
+    lo, hi = x[..., :half], x[..., half:]
+    out = torch.cat([lo * cos - hi * sin, hi * cos + lo * sin], -1).reshape(B, S, -1)
+    return torch.cat([out, v], -1).to(qkv.dtype)
+
+
+class _Rotary(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, qkv, position_ids, cos_sin, heads, kv_heads):
+        ctx.heads, ctx.kv_heads = heads, kv_heads
+        if qkv.is_cuda:
+            B, S, Wd = qkv.shape
+            pos = position_ids.to(device=qkv.device, dtype=torch.int32).reshape(-1).contiguous()
+            table = cos_sin.to(device=qkv.device, dtype=torch.float32).contiguous()
+            ctx.save_for_backward(pos, table)
+            return _C().rotary(qkv.reshape(B * S, Wd).contiguous(), pos, table, heads, kv_heads, False).view(B, S, Wd)
+        ctx.save_for_backward(position_ids, cos_sin)
+        return _rotary_reference(qkv, position_ids, cos_sin, heads, kv_heads)
+
+    @staticmethod
+    def backward(ctx, dy):
+        pos, table = ctx.saved_tensors
+        if dy.is_cuda:
+            B, S, Wd = dy.shape
+            dx = _C().rotary(dy.reshape(B * S, Wd).to(torch.bfloat16).contiguous(), pos, table, ctx.heads, ctx.kv_heads, True)
+            return dx.view(B, S, Wd), None, None, None, None
+        return _rotary_reference(dy, pos, table, ctx.heads, ctx.kv_heads, inverse=True), None, None, None, None
+
+
+def rotary(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor, heads: int, kv_heads: int) -> torch.Tensor:
+    """Rotary position embedding (Hugging Face's ``rotate_half`` convention: element i of a head pairs with i + d/2) of
+    the query and key heads of qkv [B, S, (heads + 2 * kv_heads) * d]; the value heads pass through.  position_ids
+    integer [B, S] (clamped to the table), cos_sin fp32 [max_position, 2, d / 2] (``rotary_cos_sin``).  Out of place.  On
+    CUDA: bf16 and d = 64, else ``ValueError``; positions stay on the device (CUDA-graph safe)."""
+    if qkv.dim() != 3 or heads < 1 or kv_heads < 1 or qkv.shape[-1] % (heads + 2 * kv_heads) or \
+            (qkv.shape[-1] // (heads + 2 * kv_heads)) % 2:
+        raise ValueError(f"rotary needs qkv [B, S, (heads + 2 * kv_heads) * d] with an even d, got {tuple(qkv.shape)} for "
+                         f"heads={heads}, kv_heads={kv_heads}")
+    d = qkv.shape[-1] // (heads + 2 * kv_heads)
+    if tuple(position_ids.shape) != tuple(qkv.shape[:2]) or position_ids.is_floating_point() or position_ids.is_complex():
+        raise ValueError(f"rotary needs integer position_ids {tuple(qkv.shape[:2])}, got {position_ids.dtype} {tuple(position_ids.shape)}")
+    if cos_sin.dim() != 3 or tuple(cos_sin.shape[1:]) != (2, d // 2) or cos_sin.shape[0] < 1:
+        raise ValueError(f"rotary needs cos_sin [max_position, 2, {d // 2}], got {tuple(cos_sin.shape)}")
+    if qkv.is_cuda and (qkv.dtype != torch.bfloat16 or d != ATTENTION_HEAD_DIM):
+        raise ValueError(f"rotary on CUDA needs bf16 qkv and head dim {ATTENTION_HEAD_DIM}, got {qkv.dtype}, head dim {d}")
+    return _Rotary.apply(qkv, position_ids, cos_sin, heads, kv_heads)
+
+
+def _rms_norm_reference(x: torch.Tensor, weight: torch.Tensor, eps: float) -> torch.Tensor:
+    xf = x.float()
+    return (xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps) * weight.float()).to(x.dtype)
+
+
+class _RMSNormFused(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, eps):
+        xc = x.contiguous()
+        y, rstd = _C().rmsnorm_fwd(xc, weight.contiguous(), float(eps))
+        ctx.save_for_backward(xc, weight, rstd)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight, rstd = ctx.saved_tensors
+        dx, dw = _C().rmsnorm_bwd(dy.contiguous().to(x.dtype), x, weight.contiguous(), rstd)
+        return dx, dw, None
+
+
+def rms_norm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
+    """y = x * rsqrt(mean(x^2) + eps) * weight over the last dimension (statistics in fp32).  On CUDA: the LayerNorm
+    fast-path kernels (hidden % 8 == 0, hidden <= 1024, bf16 or fp32 with weight of the same dtype), else ``ValueError``;
+    the weight gradient is a deterministic column reduction."""
+    if x.dim() < 1 or weight.dim() != 1 or weight.shape[0] != x.shape[-1]:
+        raise ValueError(f"rms_norm needs x [..., hidden] and weight [hidden], got {tuple(x.shape)} and {tuple(weight.shape)}")
+    if x.is_cuda:
+        n = x.shape[-1]
+        if x.dtype not in (torch.float32, torch.bfloat16) or weight.dtype != x.dtype or n % 8 or n > 1024:
+            raise ValueError(f"rms_norm on CUDA needs bf16 or fp32 x and weight of one dtype and hidden % 8 == 0, <= 1024; got "
+                             f"{x.dtype} x {weight.dtype}, hidden {n}")
+        if weight.device != x.device:
+            raise ValueError(f"rms_norm needs the weight on x's device ({x.device}), got {weight.device}")
+        return _RMSNormFused.apply(x, weight, eps)
+    return _rms_norm_reference(x, weight, eps)
+
+
+class _SwiGLU(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, gate_up):
+        gu = gate_up.contiguous()
+        ctx.save_for_backward(gu)
+        return _C().swiglu_fwd(gu)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (gu,) = ctx.saved_tensors
+        return _C().swiglu_bwd(dy.to(gu.dtype).contiguous(), gu)
+
+
+def _swiglu_reference(gate_up: torch.Tensor) -> torch.Tensor:
+    g, u = gate_up.float().chunk(2, dim=-1)
+    return (F.silu(g) * u).to(gate_up.dtype)
+
+
+def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
+    """silu(gate) * up from one projection [..., 2 * I] with column blocks gate | up; returns [..., I].  On CUDA: one
+    vectorised pass each way (the backward writes d[gate | up] together); bf16 and I % 8 == 0, else ``ValueError``."""
+    if gate_up.dim() < 1 or gate_up.shape[-1] % 2:
+        raise ValueError(f"swiglu needs [..., 2 * I] (gate | up), got {tuple(gate_up.shape)}")
+    if gate_up.is_cuda:
+        if gate_up.dtype != torch.bfloat16 or (gate_up.shape[-1] // 2) % 8:
+            raise ValueError(f"swiglu on CUDA needs bf16 and I % 8 == 0, got {gate_up.dtype} {tuple(gate_up.shape)}")
+        return _SwiGLU.apply(gate_up)
+    return _swiglu_reference(gate_up)
 
 
 # ------------------------------------------------------------------------------------------------

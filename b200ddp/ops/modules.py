@@ -110,6 +110,18 @@ class LayerNorm(nn.Module):
         return Fn.layer_norm(x, self.weight, self.bias, self.eps)
 
 
+class RMSNorm(nn.Module):
+    """Llama's RMSNorm: y = x * rsqrt(mean(x^2) + eps) * weight (no mean, no bias)."""
+
+    def __init__(self, hidden: int, eps: float = 1e-5, device=None, dtype=None):
+        super().__init__()
+        self.eps = eps
+        self.weight = nn.Parameter(torch.ones(hidden, device=device, dtype=dtype))
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        return Fn.rms_norm(x, self.weight, self.eps)
+
+
 class MSELoss(nn.Module):
     def forward(self, out: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         return Fn.mse_loss(out, target)
