@@ -16,9 +16,21 @@
 // Threads own 8 consecutive channels (one 16-byte vector of bf16); rows are strided across the block and
 // across gridDim.y "row splits"; partial sums land in a [splits, C] workspace and the last block of each
 // channel tile finishes the reduction in a fixed order (no float atomics -> bitwise reproducible).
+//
+// Resident kernels (bf16, the default wherever the shape fits): one cooperative launch per direction that reads every
+// activation from HBM ONCE.  The persistent grid (<= one CTA per SM, ~200 KB of shared memory each) cuts [R, C] into
+// 64-channel tiles and row slabs; a wave of tiles is TMA-loaded into shared memory (x, or dy and x), reduced to per-CTA
+// partials, a grid barrier makes the partials visible, every CTA reduces its tile's partials in a fixed order and then
+// normalises / applies the gradient straight from shared memory, writing the result back in place and TMA-storing it.
 #include "ops.h"
+#include "drv.h"
+#include "tc_primitives.cuh"
 
+#include <algorithm>
 #include <cstdlib>
+#include <map>
+#include <mutex>
+#include <utility>
 
 namespace b200 {
 namespace {
@@ -576,6 +588,507 @@ bool fused_tile(int R, int C, Tile* t) {
   return true;
 }
 
+// ---- resident (single-read) kernels ---------------------------------------------------------------------------------
+constexpr int kResThreads = 256;     // 8 channel vectors x 32 row lanes
+constexpr int kResTile = 64;         // channels per tile: a 128-byte bf16 row segment, one TMA box row
+constexpr int kResMaxBox = 256;      // TMA box height limit
+constexpr int kResMaxBoxes = 16;     // boxes (and mbarriers) per CTA and stream
+constexpr int kResWarps = kResThreads / 32;
+// Each wave serialises load -> grid barrier -> apply, so HBM idles between waves.  Measured on an H100 SXM (700 W), the
+// 4-wave backward of [100352, 256] is slower than the two-pass kernels, while every 1- and 2-wave ResNet-50 shape is faster.
+constexpr int kResMaxWaves = 2;
+// shared memory behind the slabs: mbarriers, [warps][2][64] reduction scratch, [2][64] totals, [3][64] coefficients
+constexpr int kResFixedSmem = kResMaxBoxes * 8 + (kResWarps * 2 + 2 + 3) * kResTile * 4;
+
+// set when a grid barrier wait times out (a co-residency failure): read by bn_resident_error(), never cleared by a kernel
+__device__ unsigned int g_bn_resident_error = 0;
+
+struct ResGeom {
+  int R, C;
+  int T;          // channel tiles per wave
+  int P;          // CTAs per tile (row slabs); grid = T * P
+  int box_rows;   // rows per TMA box
+  int nbox;       // boxes per CTA: a CTA's slab is nbox * box_rows rows
+  int waves;
+};
+
+// Grid-wide barrier on two workspace words {arrivals, generation}; co-residency is guaranteed by the cooperative launch,
+// and the wait is still bounded (2 s) so that a failure surfaces as an error word instead of a hung GPU.
+__device__ __forceinline__ void res_grid_sync(unsigned int* bar, unsigned int nblocks) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned int* gen = bar + 1;
+    const unsigned int g0 = bn_ld_acquire(gen);
+    __threadfence();
+    if (atomicAdd(bar, 1u) == nblocks - 1) {
+      atomicExch(bar, 0u);                     // ready for the next barrier / launch (graph replay safe)
+      __threadfence();
+      bn_st_release(gen, g0 + 1u);
+    } else {
+      unsigned long long t0;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+      while (bn_ld_acquire(gen) == g0) {
+        unsigned long long t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+        if (t - t0 > 2000000000ull) { atomicExch(&g_bn_resident_error, 1u); break; }
+      }
+    }
+    __threadfence();
+  }
+  __syncthreads();
+}
+
+// Sum the 8 channels' two accumulators over the 4 row lanes of a warp, then over the warps in a fixed order, and write this
+// CTA's [2][64] partial row to partial[(a * P + p) * C + c0 + c].
+__device__ __forceinline__ void res_write_partials(float (&acc)[2][kVec], float* red, float* __restrict__ partial, int P, int p, int C,
+                                                   int c0) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, cv = threadIdx.x & 7;
+#pragma unroll
+  for (int a = 0; a < 2; ++a)
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) {
+      float v = acc[a][i];
+      v += __shfl_xor_sync(0xffffffffu, v, 8);
+      v += __shfl_xor_sync(0xffffffffu, v, 16);
+      if (lane < 8) red[(warp * 2 + a) * kResTile + cv * kVec + i] = v;
+    }
+  __syncthreads();
+  if (threadIdx.x < 2 * kResTile) {
+    const int a = threadIdx.x / kResTile, c = threadIdx.x % kResTile;
+    float s = 0.f;
+    for (int w = 0; w < kResWarps; ++w) s += red[(w * 2 + a) * kResTile + c];
+    if (c0 + c < C) partial[((size_t)a * P + p) * C + c0 + c] = s;
+  }
+}
+
+// After the grid barrier: the tile's P partial rows, summed in a fixed order (identical in every CTA of the tile).
+// On return red[a * 64 + c] (a = 0: sum, 1: second moment) holds the totals of channel c0 + c.
+__device__ __forceinline__ void res_reduce_partials(float* red, const float* __restrict__ partial, int P, int C, int c0) {
+  const int q = threadIdx.x & 31, l = threadIdx.x >> 5;       // 2 x 16 float4 columns x 8 lanes
+  const int a = q >> 4, c4 = (q & 15) * 4;
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (c0 + c4 < C) {
+    const float* base = partial + (size_t)a * P * C + c0 + c4;
+#pragma unroll 4
+    for (int k = l; k < P; k += kResWarps) {
+      const float4 v = __ldcg(reinterpret_cast<const float4*>(base + (size_t)k * C));
+      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+    }
+  }
+  __syncthreads();                                           // red may still be read by res_write_partials' tail
+  *reinterpret_cast<float4*>(red + (l * 2 + a) * kResTile + c4) = s;
+  __syncthreads();
+  if (threadIdx.x < 2 * kResTile) {
+    const int aa = threadIdx.x / kResTile, c = threadIdx.x % kResTile;
+    float t = 0.f;
+    for (int w = 0; w < kResWarps; ++w) t += red[(w * 2 + aa) * kResTile + c];
+    red[kResWarps * 2 * kResTile + aa * kResTile + c] = t;    // staged behind the scratch: other threads may still read it
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ void res_ld8(const unsigned char* s, float* f) { unpack8(*reinterpret_cast<const Bf16x8*>(s), f); }
+__device__ __forceinline__ void res_st8(unsigned char* s, const float* f) { *reinterpret_cast<Bf16x8*>(s) = pack8(f); }
+
+// Forward: statistics, running statistics, y = relu(x*scale + shift (+ residual)) and the ReLU bitmask, x read once.
+__global__ void __launch_bounds__(kResThreads, 2)
+bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y,
+                       const __grid_constant__ CUtensorMap map_res, const __nv_bfloat16* __restrict__ residual, unsigned char* __restrict__ mask, const float* __restrict__ gamma,
+                       const float* __restrict__ beta, float* __restrict__ running_mean, float* __restrict__ running_var,
+                       long long* __restrict__ num_batches, float* __restrict__ save_mean, float* __restrict__ save_rstd,
+                       float* __restrict__ scale, float* __restrict__ shift, float* __restrict__ partial, unsigned int* __restrict__ bar,
+                       float eps, float momentum, int relu, const ResGeom g) {
+  extern __shared__ __align__(128) unsigned char res_smem[];
+  const int slab_rows = g.nbox * g.box_rows;
+  const uint32_t box_bytes = (uint32_t)g.box_rows * kResTile * 2;
+  unsigned char* data = res_smem;
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(res_smem + (size_t)slab_rows * kResTile * 2);
+  float* red = reinterpret_cast<float*>(mbar + kResMaxBoxes);       // [warps][2][64], then [2][64] totals
+  float* coef = red + kResWarps * 2 * kResTile + 2 * kResTile;        // [2][64] scale, shift
+  const int cv = threadIdx.x & 7, rl = threadIdx.x >> 3;
+  const int ntiles = (g.C + kResTile - 1) / kResTile, cvs = g.C / kVec;
+  const int slot = blockIdx.x / g.P, p = blockIdx.x % g.P;
+  const int r0 = p * slab_rows;
+  const int nlive = r0 >= g.R ? 0 : min(g.nbox, (g.R - r0 + g.box_rows - 1) / g.box_rows);
+  if (threadIdx.x == 0) {
+    for (int b = 0; b < g.nbox; ++b) tc::mbar_init(&mbar[b], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    tc::tma_prefetch_desc(&map_x);
+    tc::tma_prefetch_desc(&map_y);
+    if (blockIdx.x == 0 && num_batches != nullptr) *num_batches += 1;
+  }
+  __syncthreads();
+  for (int w = 0; w < g.waves; ++w) {
+    const int t = w * g.T + slot;
+    const bool active = t < ntiles;
+    const int c0 = t * kResTile;
+    const int cvg = t * (kResTile / kVec) + cv;                       // global channel vector of this thread
+    if (active && threadIdx.x == 0) {
+      for (int b = 0; b < nlive; ++b) {
+        tc::mbar_expect_tx(&mbar[b], box_bytes);
+        tc::tma_load_2d(&map_x, &mbar[b], data + (size_t)b * box_bytes, c0, r0 + b * g.box_rows);
+      }
+    }
+    float acc[2][kVec];
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    if (active) {
+      for (int b = 0; b < nlive; ++b) {
+        tc::mbar_wait(&mbar[b], (uint32_t)(w & 1));
+        const unsigned char* box = data + (size_t)b * box_bytes + cv * 16;
+        for (int rr = rl; rr < g.box_rows; rr += 4 * 32) {            // rows past R and channels past C are zero-filled
+          float f[4][kVec];
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            if (rr + u * 32 < g.box_rows) res_ld8(box + (size_t)(rr + u * 32) * (kResTile * 2), f[u]);
+            else
+#pragma unroll
+              for (int i = 0; i < kVec; ++i) f[u][i] = 0.f;
+          }
+#pragma unroll
+          for (int u = 0; u < 4; ++u)
+#pragma unroll
+            for (int i = 0; i < kVec; ++i) { acc[0][i] += f[u][i]; acc[1][i] = fmaf(f[u][i], f[u][i], acc[1][i]); }
+        }
+      }
+      if (residual != nullptr && threadIdx.x == 0) {
+        // the residual slab is read right after the barrier: stage it in L2 while the grid synchronises
+        for (int b = 0; b < nlive; ++b)
+          asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];"
+                       ::"l"(reinterpret_cast<uint64_t>(&map_res)), "r"(c0), "r"(r0 + b * g.box_rows) : "memory");
+      }
+      res_write_partials(acc, red, partial, g.P, p, g.C, c0);
+    }
+    res_grid_sync(bar, gridDim.x);
+    if (!active) continue;
+    res_reduce_partials(red, partial, g.P, g.C, c0);
+    if (threadIdx.x < kResTile) {
+      const float* tot = red + kResWarps * 2 * kResTile;
+      const int c = threadIdx.x, ch = c0 + c;
+      if (ch < g.C) {
+        const float inv_r = 1.f / (float)g.R;
+        const float mean = tot[c] * inv_r;
+        const float var = fmaxf(tot[kResTile + c] * inv_r - mean * mean, 0.f);     // biased variance (normalisation)
+        const float rstd = rsqrtf(var + eps);
+        const float sc = gamma[ch] * rstd;
+        const float sh = beta[ch] - mean * sc;
+        coef[c] = sc;
+        coef[kResTile + c] = sh;
+        if (p == 0) {
+          save_mean[ch] = mean;
+          save_rstd[ch] = rstd;
+          scale[ch] = sc;
+          shift[ch] = sh;
+          if (running_mean != nullptr) {
+            const float unbiased = g.R > 1 ? var * ((float)g.R / (float)(g.R - 1)) : var;
+            running_mean[ch] = (1.f - momentum) * running_mean[ch] + momentum * mean;
+            running_var[ch] = (1.f - momentum) * running_var[ch] + momentum * unbiased;
+          }
+        }
+      } else {
+        coef[c] = 0.f;
+        coef[kResTile + c] = 0.f;
+      }
+    }
+    __syncthreads();
+    float sc[kVec], sh[kVec];
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) { sc[i] = coef[cv * kVec + i]; sh[i] = coef[kResTile + cv * kVec + i]; }
+    const bool live_cv = cvg < cvs;
+    for (int b = 0; b < nlive; ++b) {
+      unsigned char* box = data + (size_t)b * box_bytes + cv * 16;
+      const int rb = r0 + b * g.box_rows;
+      for (int rr = rl; rr < g.box_rows; rr += 8 * 32) {             // 8 residual loads in flight (raw 16-byte vectors)
+        Bf16x8 rv[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const int r = rb + rr + u * 32;
+          if (residual != nullptr && rr + u * 32 < g.box_rows && r < g.R && live_cv)
+            rv[u] = *reinterpret_cast<const Bf16x8*>(residual + (size_t)r * g.C + (size_t)cvg * kVec);
+        }
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+          const int r = rb + rr + u * 32;
+          if (!(rr + u * 32 < g.box_rows && r < g.R && live_cv)) continue;
+          float f[kVec], rs[kVec];
+          res_ld8(box + (size_t)(rr + u * 32) * (kResTile * 2), f);
+          if (residual != nullptr) unpack8(rv[u], rs);
+          unsigned int bits = 0;
+#pragma unroll
+          for (int i = 0; i < kVec; ++i) {
+            float v = fmaf(f[i], sc[i], sh[i]);
+            if (residual != nullptr) v += rs[i];
+            bits |= (v > 0.f ? 1u : 0u) << i;
+            f[i] = relu ? fmaxf(v, 0.f) : v;
+          }
+          res_st8(box + (size_t)(rr + u * 32) * (kResTile * 2), f);
+          if (mask != nullptr) mask[(size_t)r * cvs + cvg] = (unsigned char)bits;
+        }
+      }
+      tc::fence_async_smem();
+      __syncthreads();
+      if (threadIdx.x == 0) { tc::tma_store_2d(&map_y, data + (size_t)b * box_bytes, c0, rb); tc::bulk_commit(); }
+    }
+    if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // slabs are reloaded next wave
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) tc::bulk_wait_all();
+}
+
+// Backward: S1 = sum dy*, S2 = sum dy* xhat (dy* = dy masked by the forward ReLU), dgamma / dbeta, then
+// dx = a*dy* + b*x + c and the residual branch's gradient dy*, with dy and x read once.
+__global__ void __launch_bounds__(kResThreads, 2)
+bn_resident_bwd_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x,
+                       const __grid_constant__ CUtensorMap map_dx, const __grid_constant__ CUtensorMap map_dres,
+                       const unsigned char* __restrict__ mask, const float* __restrict__ save_mean, const float* __restrict__ save_rstd,
+                       const float* __restrict__ gamma, float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ coef_out,
+                       float* __restrict__ partial, unsigned int* __restrict__ bar, int relu, int want_dres, const ResGeom g) {
+  extern __shared__ __align__(128) unsigned char res_smem[];
+  const int slab_rows = g.nbox * g.box_rows;
+  const uint32_t box_bytes = (uint32_t)g.box_rows * kResTile * 2;
+  unsigned char* dyd = res_smem;                                      // dy slab, then dy* (the residual gradient)
+  unsigned char* xd = res_smem + (size_t)slab_rows * kResTile * 2;    // x slab, then dx
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(res_smem + (size_t)2 * slab_rows * kResTile * 2);
+  float* red = reinterpret_cast<float*>(mbar + kResMaxBoxes);
+  float* coef = red + kResWarps * 2 * kResTile + 2 * kResTile;        // [3][64] a, b, c
+  unsigned char* smask = reinterpret_cast<unsigned char*>(coef + 3 * kResTile);   // [slab rows][8] ReLU mask bytes of the tile
+  const int cv = threadIdx.x & 7, rl = threadIdx.x >> 3;
+  const int ntiles = (g.C + kResTile - 1) / kResTile, cvs = g.C / kVec;
+  const int slot = blockIdx.x / g.P, p = blockIdx.x % g.P;
+  const int r0 = p * slab_rows;
+  const int nlive = r0 >= g.R ? 0 : min(g.nbox, (g.R - r0 + g.box_rows - 1) / g.box_rows);
+  if (threadIdx.x == 0) {
+    for (int b = 0; b < g.nbox; ++b) tc::mbar_init(&mbar[b], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    tc::tma_prefetch_desc(&map_dy);
+    tc::tma_prefetch_desc(&map_x);
+  }
+  __syncthreads();
+  for (int w = 0; w < g.waves; ++w) {
+    const int t = w * g.T + slot;
+    const bool active = t < ntiles;
+    const int c0 = t * kResTile;
+    const int cvg = t * (kResTile / kVec) + cv;
+    const bool live_cv = cvg < cvs;
+    if (active && threadIdx.x == 0) {
+      for (int b = 0; b < nlive; ++b) {
+        tc::mbar_expect_tx(&mbar[b], 2 * box_bytes);
+        tc::tma_load_2d(&map_dy, &mbar[b], dyd + (size_t)b * box_bytes, c0, r0 + b * g.box_rows);
+        tc::tma_load_2d(&map_x, &mbar[b], xd + (size_t)b * box_bytes, c0, r0 + b * g.box_rows);
+      }
+    }
+    if (active && relu) {
+      // the slab's mask bytes (1/16 of its dy bytes), used by both passes: independent loads, overlapped with the TMA loads
+      const int n = min(slab_rows, g.R - r0) * 8;
+#pragma unroll 8
+      for (int i = threadIdx.x; i < n; i += kResThreads) {
+        const int cg = t * (kResTile / kVec) + (i & 7);
+        smask[i] = cg < cvs ? mask[(size_t)(r0 + (i >> 3)) * cvs + cg] : 0u;
+      }
+      __syncthreads();
+    }
+    float acc[2][kVec];
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    if (active) {
+      float mean[kVec], rstd[kVec];
+#pragma unroll
+      for (int i = 0; i < kVec; ++i) { mean[i] = 0.f; rstd[i] = 0.f; }
+      if (live_cv) { bn_load8<float>(save_mean + cvg * kVec, mean); bn_load8<float>(save_rstd + cvg * kVec, rstd); }
+      for (int b = 0; b < nlive; ++b) {
+        tc::mbar_wait(&mbar[b], (uint32_t)(w & 1));
+        // rows past R and channels past C hold zero dy (TMA zero fill): they add nothing whatever their mask byte says
+        for (int rr = rl; rr < g.box_rows; rr += 2 * 32) {
+          float gv[2][kVec], xv[2][kVec];
+          unsigned int mk[2];
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const int q = min(rr + u * 32, g.box_rows - 1);           // a clamped duplicate row is masked out below
+            res_ld8(dyd + (size_t)b * box_bytes + (size_t)q * (kResTile * 2) + cv * 16, gv[u]);
+            res_ld8(xd + (size_t)b * box_bytes + (size_t)q * (kResTile * 2) + cv * 16, xv[u]);
+            mk[u] = rr + u * 32 < g.box_rows ? (relu ? smask[(b * g.box_rows + q) * 8 + cv] : 0xffu) : 0u;
+          }
+#pragma unroll
+          for (int u = 0; u < 2; ++u)
+#pragma unroll
+            for (int i = 0; i < kVec; ++i) {
+              const float gm = ((mk[u] >> i) & 1u) ? gv[u][i] : 0.f;
+              acc[0][i] += gm;
+              acc[1][i] = fmaf(gm, (xv[u][i] - mean[i]) * rstd[i], acc[1][i]);
+            }
+        }
+      }
+      res_write_partials(acc, red, partial, g.P, p, g.C, c0);
+    }
+    res_grid_sync(bar, gridDim.x);
+    if (!active) continue;
+    res_reduce_partials(red, partial, g.P, g.C, c0);
+    if (threadIdx.x < kResTile) {
+      const float* tot = red + kResWarps * 2 * kResTile;
+      const int c = threadIdx.x, ch = c0 + c;
+      float ka = 0.f, kb = 0.f, kc = 0.f;
+      if (ch < g.C) {
+        const float inv_r = 1.f / (float)g.R;
+        const float s1 = tot[c], s2 = tot[kResTile + c];
+        const float c1 = s1 * inv_r, c2 = s2 * inv_r;                 // mean(dy*), mean(dy* xhat)
+        const float mean = save_mean[ch], rstd = save_rstd[ch];
+        ka = gamma[ch] * rstd;
+        kb = -ka * rstd * c2;
+        kc = -ka * (c1 - mean * rstd * c2);
+        if (p == 0) {
+          dbeta[ch] = s1;
+          dgamma[ch] = s2;
+          coef_out[ch] = c1;
+          coef_out[g.C + ch] = c2;
+        }
+      }
+      coef[c] = ka;
+      coef[kResTile + c] = kb;
+      coef[2 * kResTile + c] = kc;
+    }
+    __syncthreads();
+    float ka[kVec], kb[kVec], kc[kVec];
+#pragma unroll
+    for (int i = 0; i < kVec; ++i) {
+      ka[i] = coef[cv * kVec + i];
+      kb[i] = coef[kResTile + cv * kVec + i];
+      kc[i] = coef[2 * kResTile + cv * kVec + i];
+    }
+    for (int b = 0; b < nlive; ++b) {
+      const int rb = r0 + b * g.box_rows;
+      unsigned char* gbox = dyd + (size_t)b * box_bytes + cv * 16;
+      unsigned char* xbox = xd + (size_t)b * box_bytes + cv * 16;
+      for (int rr = rl; rr < g.box_rows; rr += 2 * 32) {
+        float gv[2][kVec], xv[2][kVec];
+        unsigned int mk[2];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int q = min(rr + u * 32, g.box_rows - 1);
+          res_ld8(gbox + (size_t)q * (kResTile * 2), gv[u]);
+          res_ld8(xbox + (size_t)q * (kResTile * 2), xv[u]);
+          mk[u] = relu ? smask[(b * g.box_rows + q) * 8 + cv] : 0xffu;
+        }
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          if (rr + u * 32 >= g.box_rows) continue;
+          const size_t off = (size_t)(rr + u * 32) * (kResTile * 2);
+          float o[kVec];
+#pragma unroll
+          for (int i = 0; i < kVec; ++i) {
+            if (!((mk[u] >> i) & 1u)) gv[u][i] = 0.f;
+            o[i] = fmaf(ka[i], gv[u][i], fmaf(kb[i], xv[u][i], kc[i]));
+          }
+          if (want_dres) res_st8(gbox + off, gv[u]);
+          res_st8(xbox + off, o);
+        }
+      }
+      tc::fence_async_smem();
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        tc::tma_store_2d(&map_dx, xd + (size_t)b * box_bytes, c0, rb);
+        if (want_dres) tc::tma_store_2d(&map_dres, dyd + (size_t)b * box_bytes, c0, rb);
+        tc::bulk_commit();
+      }
+    }
+    if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) tc::bulk_wait_all();
+}
+
+int g_bn_two_pass = 0;     // 1: the resident kernels are never selected (comparisons, benchmarks)
+
+bool resident_allowed() {
+  static int fused_env = -1;
+  if (fused_env < 0) { const char* e = getenv("B200DDP_BN_FUSED"); fused_env = (e && atoi(e) == 1) ? 1 : 0; }
+  return !g_bn_two_pass && !fused_env && !bn_pdl_enabled();
+}
+
+struct ResPlan {
+  bool ok = false;
+  ResGeom g{};
+  int grid = 0;
+  int smem = 0;
+};
+
+// Largest wave (channel tiles per wave) whose slabs fit in the co-resident CTAs' shared memory.  streams = 1 (forward: x) or
+// 2 (backward: dy and x).  Computed once per (device, R, C, streams).
+ResPlan resident_plan(int R, int C, int streams) {
+  static std::mutex mu;
+  static std::map<std::pair<int, std::pair<long long, int>>, ResPlan> cache;
+  int dev = 0;
+  B200_CUDA_CHECK(cudaGetDevice(&dev));
+  const auto key = std::make_pair(dev, std::make_pair(((long long)R << 20) | (long long)C, streams));
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = cache.find(key);
+  if (it != cache.end()) return it->second;
+  ResPlan plan;
+  int sms = 0, optin = 0;
+  B200_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  B200_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const long long budget = (long long)optin - kResFixedSmem - 1024;     // slabs; 1 KB for the runtime's static reservation
+  const int ntiles = (C + kResTile - 1) / kResTile;
+  const long long row_bytes = (long long)kResTile * 2 * streams + (streams == 2 ? 8 : 0);   // backward: + the mask bytes
+  for (int T = ntiles; T >= 1 && R > 0; --T) {
+    int P = sms / T;
+    if (P < 1) continue;
+    P = std::min(P, std::max(1, (R + 31) / 32));                        // >= 32 rows per CTA
+    const int need = (R + P - 1) / P;
+    const int nbox = (need + kResMaxBox - 1) / kResMaxBox;
+    if (nbox > kResMaxBoxes) continue;
+    const int box_rows = (need + nbox - 1) / nbox;
+    const long long slab = (long long)nbox * box_rows * row_bytes;
+    if (slab > budget) continue;
+    if ((ntiles + T - 1) / T > kResMaxWaves) break;                     // fewer tiles per wave only adds waves
+    plan.g = ResGeom{R, C, T, (R + nbox * box_rows - 1) / (nbox * box_rows), box_rows, nbox, (ntiles + T - 1) / T};
+    plan.grid = plan.g.T * plan.g.P;
+    plan.smem = (int)slab + kResFixedSmem;
+    plan.ok = true;
+    break;
+  }
+  cache.emplace(key, plan);
+  return plan;
+}
+
+// [R, C] bf16, row-major, 64-channel x box_rows boxes, no swizzle; out-of-range rows / channels read as zero, stores clip.
+CUtensorMap res_map(const void* ptr, int R, int C, int box_rows) {
+  auto& drv = Driver::get();
+  if (!drv.TensorMapEncodeTiled) throw std::runtime_error("batch norm: cuTensorMapEncodeTiled unavailable");
+  CUtensorMap map;
+  cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)R};
+  cuuint64_t strides[1] = {(cuuint64_t)C * 2};
+  cuuint32_t box[2] = {(cuuint32_t)kResTile, (cuuint32_t)box_rows};
+  cuuint32_t es[2] = {1, 1};
+  B200_DRV_CHECK(drv.TensorMapEncodeTiled(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, es,
+                                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
+  return map;
+}
+
+int res_smem_limit() {
+  int dev = 0, optin = 0;
+  B200_CUDA_CHECK(cudaGetDevice(&dev));
+  B200_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  return optin;
+}
+
+bool res_aligned(const void* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+template <typename... KArgs, typename... Args>
+void launch_cooperative(void (*kernel)(KArgs...), const ResPlan& plan, cudaStream_t s, Args... args) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(plan.grid);
+  cfg.blockDim = dim3(kResThreads);
+  cfg.dynamicSmemBytes = plan.smem;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------
@@ -697,10 +1210,21 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_apply_partials_kernel(const
 
 void set_bn_pdl(int on) { g_bn_pdl = on; }
 
+void set_bn_two_pass(int on) { g_bn_two_pass = on ? 1 : 0; }
+
+unsigned int bn_resident_error() {
+  unsigned int v = 0;
+  B200_CUDA_CHECK(cudaMemcpyFromSymbol(&v, g_bn_resident_error, sizeof(v)));
+  return v;
+}
+
+// Sizes the workspace of both paths and plans the resident kernels of this shape (cached for the launches).
 void bn_workspace_sizes(int R, int C, size_t* partial_floats, size_t* counters) {
   const Tile t = pick_tile(R, C);
-  *partial_floats = (size_t)2 * t.grid_y * C;
-  *counters = (size_t)2 * t.grid_x;          // tickets + generation words
+  const ResPlan fwd = resident_plan(R, C, 1), bwd = resident_plan(R, C, 2);
+  const int p = std::max(fwd.ok ? fwd.g.P : 0, bwd.ok ? bwd.g.P : 0);
+  *partial_floats = (size_t)2 * std::max(t.grid_y, p) * C;
+  *counters = (size_t)2 * t.grid_x + 2;      // tickets + generation words, then the resident kernels' grid barrier
 }
 
 void launch_bn_forward(const void* x, const void* residual, void* y, unsigned char* mask, DType dt, int R, int C, const float* gamma, const float* beta,
@@ -708,11 +1232,25 @@ void launch_bn_forward(const void* x, const void* residual, void* y, unsigned ch
                        float* scale, float* shift, float* partial, unsigned int* counters, float eps, float momentum, bool relu,
                        cudaStream_t s) {
   if (C % kVec != 0) throw std::runtime_error("fused batch norm: channel count must be a multiple of 8");
+  const int r = relu ? 1 : 0;
+  if (dt == DType::BF16 && resident_allowed() && res_aligned(x) && res_aligned(residual) && res_aligned(y)) {
+    const ResPlan plan = resident_plan(R, C, 1);
+    if (plan.ok) {
+      static std::atomic<unsigned long long> smem_done{0};
+      ensure_max_dynamic_smem(bn_resident_fwd_kernel, res_smem_limit(), smem_done);    // raised once: every plan fits below it
+      const CUtensorMap mx = res_map(x, R, C, plan.g.box_rows), my = res_map(y, R, C, plan.g.box_rows);
+      const CUtensorMap mres = residual != nullptr ? res_map(residual, R, C, plan.g.box_rows) : mx;
+      launch_cooperative(bn_resident_fwd_kernel, plan, s, mx, my, mres, (const __nv_bfloat16*)residual, mask, gamma, beta, running_mean, running_var,
+                         num_batches, save_mean, save_rstd, scale, shift, partial, counters + 2 * pick_tile(R, C).grid_x, eps, momentum, r,
+                         plan.g);
+      B200_COUNT_LAUNCH(1);
+      return;
+    }
+  }
   Tile t;
   const bool fused = fused_tile(R, C, &t);
   const size_t smem = (size_t)2 * t.ty * t.cvb * kVec * sizeof(float);
   const dim3 grid(t.grid_x, t.grid_y);
-  const int r = relu ? 1 : 0;
   if (!fused && bn_pdl_enabled()) {
     // opt-in: producer with an early launch_dependents, apply kernel as its programmatic dependent
 #define B200_BN_FWD_PDL(T)                                                                                                                  \
@@ -789,13 +1327,27 @@ void launch_bn_backward(const void* dy, const void* x, const void* y, void* dx, 
                         const float* save_mean, const float* save_rstd, float* dgamma, float* dbeta, float* coef, float* partial,
                         unsigned int* counters, bool relu, cudaStream_t s) {
   if (C % kVec != 0) throw std::runtime_error("fused batch norm: channel count must be a multiple of 8");
+  const int r = relu ? 1 : 0;
+  if (dt == DType::BF16 && resident_allowed() && res_aligned(dy) && res_aligned(x) && res_aligned(dx) && res_aligned(dres)) {
+    const ResPlan plan = resident_plan(R, C, 2);
+    if (plan.ok) {
+      static std::atomic<unsigned long long> smem_done{0};
+      ensure_max_dynamic_smem(bn_resident_bwd_kernel, res_smem_limit(), smem_done);    // raised once: every plan fits below it
+      const int br = plan.g.box_rows;
+      const CUtensorMap mdy = res_map(dy, R, C, br), mx = res_map(x, R, C, br), mdx = res_map(dx, R, C, br);
+      const CUtensorMap mdres = dres != nullptr ? res_map(dres, R, C, br) : mdx;
+      launch_cooperative(bn_resident_bwd_kernel, plan, s, mdy, mx, mdx, mdres, (const unsigned char*)y, save_mean, save_rstd, gamma, dgamma,
+                         dbeta, coef, partial, counters + 2 * pick_tile(R, C).grid_x, r, dres != nullptr ? 1 : 0, plan.g);
+      B200_COUNT_LAUNCH(1);
+      return;
+    }
+  }
   Tile t;
   const bool fused = fused_tile(R, C, &t);
   const size_t smem = (size_t)2 * t.ty * t.cvb * kVec * sizeof(float);
   const dim3 grid(t.grid_x, t.grid_y);
-  const int r = relu ? 1 : 0;
   if (!fused && bn_pdl_enabled()) {
-#define B200_BN_BWD_PDL(T)                                                                                                                    \
+#define B200_BN_BWD_PDL(T)                                                                                                                   \
     bn_bwd_reduce_kernel<T, false, true><<<grid, kBnThreads, smem, s>>>((const T*)dy, (const T*)x, (const unsigned char*)y, R, C, t.cvb, t.ty, r,  \
                                                                         save_mean, save_rstd, partial, counters, dgamma, dbeta, coef, gamma,      \
                                                                         (T*)dx, (T*)dres);                                                        \

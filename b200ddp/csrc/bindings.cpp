@@ -991,6 +991,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ---- fused BatchNorm ---------------------------------------------------------------------------
   m.def("set_bn_pdl", &set_bn_pdl);
+  m.def("set_bn_two_pass", &set_bn_two_pass);
+  m.def("bn_resident_error", &bn_resident_error);
   m.def("bn_workspace", [](int R, int C) {
     size_t pf = 0, cn = 0;
     bn_workspace_sizes(R, C, &pf, &cn);

@@ -138,6 +138,10 @@ void launch_small_linear_bwd(const float* dy, const float* x, const float* w, co
 void bn_workspace_sizes(int R, int C, size_t* partial_floats, size_t* counters);
 // -1 = read B200DDP_PDL (default 0); 1 = statistics -> apply and bwd-reduce -> bwd-apply as programmatic dependent launches
 void set_bn_pdl(int on);
+// 1 = never select the single-read resident kernels (compare against / benchmark the two-pass kernels); 0 = default
+void set_bn_two_pass(int on);
+// nonzero once a resident BatchNorm kernel's grid barrier wait has timed out (co-residency failure)
+unsigned int bn_resident_error();
 void launch_bn_forward(const void* x, const void* residual, void* y, unsigned char* relu_mask /*[R, C/8] or null*/, DType dt, int R, int C, const float* gamma, const float* beta,
                        float* running_mean, float* running_var, long long* num_batches, float* save_mean, float* save_rstd,
                        float* scale, float* shift, float* partial, unsigned int* counters, float eps, float momentum, bool relu,

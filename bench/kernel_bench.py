@@ -419,25 +419,57 @@ def main():
 
     if "bn" in want:
         from b200ddp.ops import FusedBatchNormAct2d
-        for shape in [(32, 64, 112, 112), (32, 256, 56, 56), (32, 64, 56, 56), (32, 512, 28, 28), (32, 1024, 14, 14), (32, 2048, 7, 7)]:
+        # Each shape runs the default kernels (resident: one launch per direction, activations read once, where the shape fits
+        # the CTAs' shared memory) and the two-pass kernels (set_bn_two_pass).  Algorithmic bytes per path, bf16 [R, C] with
+        # the 1-bit ReLU mask (R*C/8 bytes): forward resident x + res + y + mask, two-pass 2x + res + y + mask; backward
+        # resident dy + x + mask + dx + dres, two-pass 2 (dy + x + mask) + dx + dres.
+        # (32, 512, 28, 28) is also run without ReLU / residual (the downsample BatchNorm): x + y only.
+        for shape in [(32, 64, 112, 112), (32, 256, 56, 56), (32, 64, 56, 56), (32, 512, 28, 28), (32, 1024, 14, 14), (32, 2048, 7, 7),
+                      (32, 128, 56, 56), (32, 512, 28, 28, "plain")]:
+            relu = len(shape) == 4
+            shape = shape[:4]
             x = torch.randn(*shape, device=dev).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
-            res = torch.randn_like(x)
+            res = torch.randn_like(x) if relu else None
             nbytes = x.numel() * 2
-            bn = FusedBatchNormAct2d(shape[1], relu=True).to(dev)
+            mbytes = x.numel() // 8 if relu else 0
+            bn = FusedBatchNormAct2d(shape[1], relu=relu).to(dev)
             ref = torch.nn.BatchNorm2d(shape[1]).to(dev)
             ws = bn._workspace(x)
-            fwd = lambda: C.bn_forward(x, res, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.num_batches_tracked, 1e-5, 0.1, True, ws[0], ws[1])
-            ms = timeit(fwd, args.iters)
-            lib = timeit(lambda: torch.relu(ref(x) + res), args.iters)
-            record(f"bn+add+relu fwd {shape}", ms, bytes_=nbytes * 4, lib_ms=lib, note="min traffic: x read twice (2nd from L2), res, y")
-            y, stats, mask = fwd()
+            fwd = lambda: C.bn_forward(x, res, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.num_batches_tracked, 1e-5, 0.1, relu, ws[0], ws[1])
             dy = torch.randn_like(x)
-            ms = timeit(lambda: C.bn_backward(dy, x, mask, bn.weight, stats, True, True, ws[2], ws[3]), args.iters)
+            tag = "bn+add+relu" if relu else "bn"
+            lib_f = timeit((lambda: torch.relu(ref(x) + res)) if relu else (lambda: ref(x)), args.iters)
             xr = x.clone().requires_grad_()
-            rr = res.clone().requires_grad_()
-            yl = torch.relu(ref(xr) + rr)
-            lib = timeit(lambda: torch.autograd.grad(yl, (xr, rr), dy, retain_graph=True), args.iters)
-            record(f"bn+add+relu bwd {shape}", ms, bytes_=nbytes * 8, lib_ms=lib, note="reads dy,x,y twice; writes dx,dres")
+            rr = res.clone().requires_grad_() if relu else None
+            yl = torch.relu(ref(xr) + rr) if relu else ref(xr)
+            lib_b = timeit(lambda: torch.autograd.grad(yl, (xr, rr) if relu else (xr,), dy, retain_graph=True), args.iters)
+            streams_f = 2 if relu else 1               # x + res (read once) ... + y
+            streams_b = 4 if relu else 3               # dy, x, dx (+ dres)
+            for two_pass in (0, 1):
+                C.set_bn_two_pass(two_pass)
+                n0 = C.launch_count()
+                y, stats, mask = fwd()
+                path = "two-pass" if two_pass or C.launch_count() - n0 > 1 else "resident"
+                if two_pass == 0 and path == "two-pass":
+                    path = "default=two-pass"
+                ms = timeit(fwd, args.iters)
+                fb = nbytes * (streams_f + 1 + (1 if "two-pass" in path else 0)) + mbytes
+                record(f"{tag} fwd {shape} [{path}]", ms, bytes_=fb, lib_ms=lib_f,
+                       note=("x, res, y, mask" if relu else "x, y") + (" + 2nd x read" if "two-pass" in path else ""))
+                bwd = lambda: C.bn_backward(dy, x, mask if relu else None, bn.weight, stats, relu, relu, ws[2], ws[3])
+                n0 = C.launch_count()
+                bwd()
+                bpath = "two-pass" if two_pass or C.launch_count() - n0 > 1 else "resident"
+                if two_pass == 0 and bpath == "two-pass":
+                    bpath = "default=two-pass"
+                ms = timeit(bwd, args.iters)
+                reads = 2 * nbytes * (2 if "two-pass" in bpath else 1)
+                bb = reads + nbytes * (streams_b - 2) + mbytes * (2 if "two-pass" in bpath else 1)
+                record(f"{tag} bwd {shape} [{bpath}]", ms, bytes_=bb, lib_ms=lib_b,
+                       note="dy, x, dx" + (", dres" if relu else "") + (" + 2nd dy, x read" if "two-pass" in bpath else ""))
+            C.set_bn_two_pass(0)
+        if C.bn_resident_error():
+            raise RuntimeError("resident BatchNorm grid barrier timed out")
 
     if "sgd" in want:
         for dtype, label in ((torch.float32, "fp32"), (torch.bfloat16, "bf16+master")):
