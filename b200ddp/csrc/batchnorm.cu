@@ -594,13 +594,16 @@ constexpr int kResTile = 64;         // channels per tile: a 128-byte bf16 row s
 constexpr int kResMaxBox = 256;      // TMA box height limit
 constexpr int kResMaxBoxes = 16;     // boxes (and mbarriers) per CTA and stream
 constexpr int kResWarps = kResThreads / 32;
-// Each wave serialises load -> grid barrier -> apply, so HBM idles between waves.  Measured on an H100 SXM (700 W), the
-// 4-wave backward of [100352, 256] is slower than the two-pass kernels, while every 1- and 2-wave ResNet-50 shape is faster.
+static_assert(kResMaxBox <= 8 * (kResThreads / 8), "the forward apply gives each of the 32 row lanes 8 rows of a box");
+// Waves per launch.  A shape needing up to kResMaxLaunches * kResMaxWaves waves runs as that many launches over disjoint
+// ranges of channel tiles (the backward of [100352, 256]: 4 waves, two launches).
 constexpr int kResMaxWaves = 2;
+constexpr int kResMaxLaunches = 2;
+constexpr int kResMaxPartialLoads = 17;   // ceil(132 SMs / 8 warps): partial rows each thread of a tile reduction loads
 // shared memory behind the slabs: mbarriers, [warps][2][64] reduction scratch, [2][64] totals, [3][64] coefficients
 constexpr int kResFixedSmem = kResMaxBoxes * 8 + (kResWarps * 2 + 2 + 3) * kResTile * 4;
 
-// set when a grid barrier wait times out (a co-residency failure): read by bn_resident_error(), never cleared by a kernel
+// set when a tile barrier wait times out (a co-residency failure): read by bn_resident_error(), never cleared by a kernel
 __device__ unsigned int g_bn_resident_error = 0;
 
 struct ResGeom {
@@ -609,20 +612,24 @@ struct ResGeom {
   int P;          // CTAs per tile (row slabs); grid = T * P
   int box_rows;   // rows per TMA box
   int nbox;       // boxes per CTA: a CTA's slab is nbox * box_rows rows
-  int waves;
+  int waves;      // waves of this launch
+  int tile0;      // first channel tile of this launch: wave w, slot s runs tile tile0 + w * T + s
+  int tile_end;   // one past the last channel tile of this launch
 };
 
-// Grid-wide barrier on two workspace words {arrivals, generation}; co-residency is guaranteed by the cooperative launch,
-// and the wait is still bounded (2 s) so that a failure surfaces as an error word instead of a hung GPU.
-__device__ __forceinline__ void res_grid_sync(unsigned int* bar, unsigned int nblocks) {
+// Barrier of the P CTAs of one channel tile on that tile slot's two workspace words {arrivals, generation}: a tile
+// depends only on its own partials, so tiles of a wave proceed independently.  Co-residency is guaranteed by the
+// cooperative launch, and the wait is still bounded (2 s) so that a failure surfaces as an error word instead of a hung GPU.
+__device__ __forceinline__ void res_tile_sync(unsigned int* bar, unsigned int nblocks) {
   __syncthreads();
   if (threadIdx.x == 0) {
     unsigned int* gen = bar + 1;
     const unsigned int g0 = bn_ld_acquire(gen);
-    __threadfence();
-    if (atomicAdd(bar, 1u) == nblocks - 1) {
-      atomicExch(bar, 0u);                     // ready for the next barrier / launch (graph replay safe)
-      __threadfence();
+    // acq_rel: releases this CTA's partial row (ordered before it by the bar.sync above), acquires the earlier arrivals'
+    unsigned int old;
+    asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], 1;" : "=r"(old) : "l"(bar) : "memory");
+    if (old == nblocks - 1) {
+      asm volatile("st.relaxed.gpu.global.u32 [%0], 0;" ::"l"(bar) : "memory");   // ready for the next wave / launch
       bn_st_release(gen, g0 + 1u);
     } else {
       unsigned long long t0;
@@ -633,7 +640,6 @@ __device__ __forceinline__ void res_grid_sync(unsigned int* bar, unsigned int nb
         if (t - t0 > 2000000000ull) { atomicExch(&g_bn_resident_error, 1u); break; }
       }
     }
-    __threadfence();
   }
   __syncthreads();
 }
@@ -661,19 +667,22 @@ __device__ __forceinline__ void res_write_partials(float (&acc)[2][kVec], float*
   }
 }
 
-// After the grid barrier: the tile's P partial rows, summed in a fixed order (identical in every CTA of the tile).
+// After the tile barrier: the tile's P partial rows, summed in a fixed order (identical in every CTA of the tile).
 // On return red[a * 64 + c] (a = 0: sum, 1: second moment) holds the totals of channel c0 + c.
 __device__ __forceinline__ void res_reduce_partials(float* red, const float* __restrict__ partial, int P, int C, int c0) {
   const int q = threadIdx.x & 31, l = threadIdx.x >> 5;       // 2 x 16 float4 columns x 8 lanes
   const int a = q >> 4, c4 = (q & 15) * 4;
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
   if (c0 + c4 < C) {
+    // every load of the thread is issued before the first add: one L2 round trip on the critical path instead of P / 32
     const float* base = partial + (size_t)a * P * C + c0 + c4;
-#pragma unroll 4
-    for (int k = l; k < P; k += kResWarps) {
-      const float4 v = __ldcg(reinterpret_cast<const float4*>(base + (size_t)k * C));
-      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-    }
+    float4 v[kResMaxPartialLoads];
+#pragma unroll
+    for (int j = 0; j < kResMaxPartialLoads; ++j)
+      if (l + j * kResWarps < P) v[j] = __ldcg(reinterpret_cast<const float4*>(base + (size_t)(l + j * kResWarps) * C));
+#pragma unroll
+    for (int j = 0; j < kResMaxPartialLoads; ++j)
+      if (l + j * kResWarps < P) { s.x += v[j].x; s.y += v[j].y; s.z += v[j].z; s.w += v[j].w; }
   }
   __syncthreads();                                           // red may still be read by res_write_partials' tail
   *reinterpret_cast<float4*>(red + (l * 2 + a) * kResTile + c4) = s;
@@ -691,7 +700,7 @@ __device__ __forceinline__ void res_ld8(const unsigned char* s, float* f) { unpa
 __device__ __forceinline__ void res_st8(unsigned char* s, const float* f) { *reinterpret_cast<Bf16x8*>(s) = pack8(f); }
 
 // Forward: statistics, running statistics, y = relu(x*scale + shift (+ residual)) and the ReLU bitmask, x read once.
-__global__ void __launch_bounds__(kResThreads, 2)
+__global__ void __launch_bounds__(kResThreads, 1)
 bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y,
                        const __grid_constant__ CUtensorMap map_res, const __nv_bfloat16* __restrict__ residual, unsigned char* __restrict__ mask, const float* __restrict__ gamma,
                        const float* __restrict__ beta, float* __restrict__ running_mean, float* __restrict__ running_var,
@@ -706,33 +715,45 @@ bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
   float* red = reinterpret_cast<float*>(mbar + kResMaxBoxes);       // [warps][2][64], then [2][64] totals
   float* coef = red + kResWarps * 2 * kResTile + 2 * kResTile;        // [2][64] scale, shift
   const int cv = threadIdx.x & 7, rl = threadIdx.x >> 3;
-  const int ntiles = (g.C + kResTile - 1) / kResTile, cvs = g.C / kVec;
+  const int cvs = g.C / kVec;
   const int slot = blockIdx.x / g.P, p = blockIdx.x % g.P;
   const int r0 = p * slab_rows;
   const int nlive = r0 >= g.R ? 0 : min(g.nbox, (g.R - r0 + g.box_rows - 1) / g.box_rows);
+  bar += 2 * slot;
+  // box b of the slab of tile t (the first wave's loads here; later waves' loads are issued box by box during the
+  // previous wave's apply, as soon as the box's store has read it)
+  auto load_box = [&](int b, int t) {
+    tc::mbar_expect_tx(&mbar[b], box_bytes);
+    tc::tma_load_2d(&map_x, &mbar[b], data + (size_t)b * box_bytes, t * kResTile, r0 + b * g.box_rows);
+  };
   if (threadIdx.x == 0) {
     for (int b = 0; b < g.nbox; ++b) tc::mbar_init(&mbar[b], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tc::tma_prefetch_desc(&map_x);
     tc::tma_prefetch_desc(&map_y);
-    if (blockIdx.x == 0 && num_batches != nullptr) *num_batches += 1;
+    if (blockIdx.x == 0 && g.tile0 == 0 && num_batches != nullptr) *num_batches += 1;
+    if (g.tile0 + slot < g.tile_end)
+      for (int b = 0; b < nlive; ++b) load_box(b, g.tile0 + slot);
   }
   __syncthreads();
   for (int w = 0; w < g.waves; ++w) {
-    const int t = w * g.T + slot;
-    const bool active = t < ntiles;
+    const int t = g.tile0 + w * g.T + slot;
+    if (t >= g.tile_end) break;                                       // the whole tile slot is done: no later wave either
+    const bool next = t + g.T < g.tile_end;
     const int c0 = t * kResTile;
     const int cvg = t * (kResTile / kVec) + cv;                       // global channel vector of this thread
-    if (active && threadIdx.x == 0) {
-      for (int b = 0; b < nlive; ++b) {
-        tc::mbar_expect_tx(&mbar[b], box_bytes);
-        tc::tma_load_2d(&map_x, &mbar[b], data + (size_t)b * box_bytes, c0, r0 + b * g.box_rows);
-      }
+    // per-channel inputs of the coefficients, read before the barrier so that their latency is off the critical path
+    float gm = 0.f, bt = 0.f, rmean = 0.f, rvar = 0.f;
+    if (threadIdx.x < kResTile && c0 + (int)threadIdx.x < g.C) {
+      const int ch = c0 + threadIdx.x;
+      gm = gamma[ch];
+      bt = beta[ch];
+      if (p == 0 && running_mean != nullptr) { rmean = running_mean[ch]; rvar = running_var[ch]; }
     }
     float acc[2][kVec];
 #pragma unroll
     for (int i = 0; i < kVec; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
-    if (active) {
+    {
       for (int b = 0; b < nlive; ++b) {
         tc::mbar_wait(&mbar[b], (uint32_t)(w & 1));
         const unsigned char* box = data + (size_t)b * box_bytes + cv * 16;
@@ -759,8 +780,19 @@ bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
       }
       res_write_partials(acc, red, partial, g.P, p, g.C, c0);
     }
-    res_grid_sync(bar, gridDim.x);
-    if (!active) continue;
+    // the residual rows of box b this thread adds: a box has at most 8 * 32 rows, row lane rl owns rows rl + 32 u
+    const bool live_cv = cvg < cvs;
+    auto load_res = [&](int b, Bf16x8 (&d)[8]) {
+#pragma unroll
+      for (int u = 0; u < 8; ++u) {
+        const int q = rl + u * 32, r = r0 + b * g.box_rows + q;
+        if (residual != nullptr && q < g.box_rows && r < g.R && live_cv)
+          d[u] = *reinterpret_cast<const Bf16x8*>(residual + (size_t)r * g.C + (size_t)cvg * kVec);
+      }
+    };
+    Bf16x8 rv[8];
+    if (nlive > 0) load_res(0, rv);                                   // box 0's residual: in flight across the barrier
+    res_tile_sync(bar, g.P);
     res_reduce_partials(red, partial, g.P, g.C, c0);
     if (threadIdx.x < kResTile) {
       const float* tot = red + kResWarps * 2 * kResTile;
@@ -770,8 +802,8 @@ bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
         const float mean = tot[c] * inv_r;
         const float var = fmaxf(tot[kResTile + c] * inv_r - mean * mean, 0.f);     // biased variance (normalisation)
         const float rstd = rsqrtf(var + eps);
-        const float sc = gamma[ch] * rstd;
-        const float sh = beta[ch] - mean * sc;
+        const float sc = gm * rstd;
+        const float sh = bt - mean * sc;
         coef[c] = sc;
         coef[kResTile + c] = sh;
         if (p == 0) {
@@ -781,8 +813,8 @@ bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
           shift[ch] = sh;
           if (running_mean != nullptr) {
             const float unbiased = g.R > 1 ? var * ((float)g.R / (float)(g.R - 1)) : var;
-            running_mean[ch] = (1.f - momentum) * running_mean[ch] + momentum * mean;
-            running_var[ch] = (1.f - momentum) * running_var[ch] + momentum * unbiased;
+            running_mean[ch] = (1.f - momentum) * rmean + momentum * mean;
+            running_var[ch] = (1.f - momentum) * rvar + momentum * unbiased;
           }
         }
       } else {
@@ -794,42 +826,45 @@ bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
     float sc[kVec], sh[kVec];
 #pragma unroll
     for (int i = 0; i < kVec; ++i) { sc[i] = coef[cv * kVec + i]; sh[i] = coef[kResTile + cv * kVec + i]; }
-    const bool live_cv = cvg < cvs;
     for (int b = 0; b < nlive; ++b) {
       unsigned char* box = data + (size_t)b * box_bytes + cv * 16;
       const int rb = r0 + b * g.box_rows;
-      for (int rr = rl; rr < g.box_rows; rr += 8 * 32) {             // 8 residual loads in flight (raw 16-byte vectors)
-        Bf16x8 rv[8];
+      Bf16x8 rn[8];
+      if (b + 1 < nlive) load_res(b + 1, rn);                         // in flight while this box is normalised
 #pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int r = rb + rr + u * 32;
-          if (residual != nullptr && rr + u * 32 < g.box_rows && r < g.R && live_cv)
-            rv[u] = *reinterpret_cast<const Bf16x8*>(residual + (size_t)r * g.C + (size_t)cvg * kVec);
+      for (int u = 0; u < 8; ++u) {
+        const int q = rl + u * 32, r = rb + q;
+        if (!(q < g.box_rows && r < g.R && live_cv)) continue;
+        float f[kVec], rs[kVec];
+        res_ld8(box + (size_t)q * (kResTile * 2), f);
+        if (residual != nullptr) unpack8(rv[u], rs);
+        unsigned int bits = 0;
+#pragma unroll
+        for (int i = 0; i < kVec; ++i) {
+          float v = fmaf(f[i], sc[i], sh[i]);
+          if (residual != nullptr) v += rs[i];
+          bits |= (v > 0.f ? 1u : 0u) << i;
+          f[i] = relu ? fmaxf(v, 0.f) : v;
         }
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int r = rb + rr + u * 32;
-          if (!(rr + u * 32 < g.box_rows && r < g.R && live_cv)) continue;
-          float f[kVec], rs[kVec];
-          res_ld8(box + (size_t)(rr + u * 32) * (kResTile * 2), f);
-          if (residual != nullptr) unpack8(rv[u], rs);
-          unsigned int bits = 0;
-#pragma unroll
-          for (int i = 0; i < kVec; ++i) {
-            float v = fmaf(f[i], sc[i], sh[i]);
-            if (residual != nullptr) v += rs[i];
-            bits |= (v > 0.f ? 1u : 0u) << i;
-            f[i] = relu ? fmaxf(v, 0.f) : v;
-          }
-          res_st8(box + (size_t)(rr + u * 32) * (kResTile * 2), f);
-          if (mask != nullptr) mask[(size_t)r * cvs + cvg] = (unsigned char)bits;
-        }
+        res_st8(box + (size_t)q * (kResTile * 2), f);
+        if (mask != nullptr) mask[(size_t)r * cvs + cvg] = (unsigned char)bits;
       }
+#pragma unroll
+      for (int u = 0; u < 8; ++u) rv[u] = rn[u];
       tc::fence_async_smem();
       __syncthreads();
-      if (threadIdx.x == 0) { tc::tma_store_2d(&map_y, data + (size_t)b * box_bytes, c0, rb); tc::bulk_commit(); }
+      if (threadIdx.x == 0) {
+        tc::tma_store_2d(&map_y, data + (size_t)b * box_bytes, c0, rb);
+        tc::bulk_commit();
+        // the next wave's load into the previous box, once that box's store has read it: HBM streams the next wave's
+        // x while this wave's y drains
+        if (next && b > 0) { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); load_box(b - 1, t + g.T); }
+      }
     }
-    if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // slabs are reloaded next wave
+    if (threadIdx.x == 0) {
+      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+      if (next && nlive > 0) load_box(nlive - 1, t + g.T);
+    }
     __syncthreads();
   }
   if (threadIdx.x == 0) tc::bulk_wait_all();
@@ -837,7 +872,7 @@ bn_resident_fwd_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_c
 
 // Backward: S1 = sum dy*, S2 = sum dy* xhat (dy* = dy masked by the forward ReLU), dgamma / dbeta, then
 // dx = a*dy* + b*x + c and the residual branch's gradient dy*, with dy and x read once.
-__global__ void __launch_bounds__(kResThreads, 2)
+__global__ void __launch_bounds__(kResThreads, 1)
 bn_resident_bwd_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x,
                        const __grid_constant__ CUtensorMap map_dx, const __grid_constant__ CUtensorMap map_dres,
                        const unsigned char* __restrict__ mask, const float* __restrict__ save_mean, const float* __restrict__ save_rstd,
@@ -853,44 +888,65 @@ bn_resident_bwd_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_
   float* coef = red + kResWarps * 2 * kResTile + 2 * kResTile;        // [3][64] a, b, c
   unsigned char* smask = reinterpret_cast<unsigned char*>(coef + 3 * kResTile);   // [slab rows][8] ReLU mask bytes of the tile
   const int cv = threadIdx.x & 7, rl = threadIdx.x >> 3;
-  const int ntiles = (g.C + kResTile - 1) / kResTile, cvs = g.C / kVec;
+  const int cvs = g.C / kVec;
   const int slot = blockIdx.x / g.P, p = blockIdx.x % g.P;
   const int r0 = p * slab_rows;
   const int nlive = r0 >= g.R ? 0 : min(g.nbox, (g.R - r0 + g.box_rows - 1) / g.box_rows);
+  // whole tiles of channels and an 8-byte aligned mask: a row's 8 mask bytes of a tile are one aligned 8-byte word
+  const bool mask_words = g.C % kResTile == 0 && (reinterpret_cast<uintptr_t>(mask) & 7u) == 0;
+  bar += 2 * slot;
+  // box b of the dy and x slabs of tile t (the first wave's loads here; later waves' loads are issued box by box during
+  // the previous wave's apply, as soon as the box's stores have read it)
+  auto load_box = [&](int b, int t) {
+    tc::mbar_expect_tx(&mbar[b], 2 * box_bytes);
+    tc::tma_load_2d(&map_dy, &mbar[b], dyd + (size_t)b * box_bytes, t * kResTile, r0 + b * g.box_rows);
+    tc::tma_load_2d(&map_x, &mbar[b], xd + (size_t)b * box_bytes, t * kResTile, r0 + b * g.box_rows);
+  };
   if (threadIdx.x == 0) {
     for (int b = 0; b < g.nbox; ++b) tc::mbar_init(&mbar[b], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tc::tma_prefetch_desc(&map_dy);
     tc::tma_prefetch_desc(&map_x);
+    if (g.tile0 + slot < g.tile_end)
+      for (int b = 0; b < nlive; ++b) load_box(b, g.tile0 + slot);
   }
   __syncthreads();
   for (int w = 0; w < g.waves; ++w) {
-    const int t = w * g.T + slot;
-    const bool active = t < ntiles;
+    const int t = g.tile0 + w * g.T + slot;
+    if (t >= g.tile_end) break;                                       // the whole tile slot is done: no later wave either
+    const bool next = t + g.T < g.tile_end;
     const int c0 = t * kResTile;
     const int cvg = t * (kResTile / kVec) + cv;
     const bool live_cv = cvg < cvs;
-    if (active && threadIdx.x == 0) {
-      for (int b = 0; b < nlive; ++b) {
-        tc::mbar_expect_tx(&mbar[b], 2 * box_bytes);
-        tc::tma_load_2d(&map_dy, &mbar[b], dyd + (size_t)b * box_bytes, c0, r0 + b * g.box_rows);
-        tc::tma_load_2d(&map_x, &mbar[b], xd + (size_t)b * box_bytes, c0, r0 + b * g.box_rows);
-      }
+    // per-channel inputs of the coefficients, read before the barrier so that their latency is off the critical path
+    float gam = 0.f, smean = 0.f, srstd = 0.f;
+    if (threadIdx.x < kResTile && c0 + (int)threadIdx.x < g.C) {
+      const int ch = c0 + threadIdx.x;
+      gam = gamma[ch];
+      smean = save_mean[ch];
+      srstd = save_rstd[ch];
     }
-    if (active && relu) {
+    if (relu) {
       // the slab's mask bytes (1/16 of its dy bytes), used by both passes: independent loads, overlapped with the TMA loads
-      const int n = min(slab_rows, g.R - r0) * 8;
+      const int rows = min(slab_rows, g.R - r0);
+      if (mask_words) {
+#pragma unroll 4
+        for (int i = threadIdx.x; i < rows; i += kResThreads)
+          reinterpret_cast<unsigned long long*>(smask)[i] =
+              *reinterpret_cast<const unsigned long long*>(mask + (size_t)(r0 + i) * cvs + t * (kResTile / kVec));
+      } else {
 #pragma unroll 8
-      for (int i = threadIdx.x; i < n; i += kResThreads) {
-        const int cg = t * (kResTile / kVec) + (i & 7);
-        smask[i] = cg < cvs ? mask[(size_t)(r0 + (i >> 3)) * cvs + cg] : 0u;
+        for (int i = threadIdx.x; i < rows * 8; i += kResThreads) {
+          const int cg = t * (kResTile / kVec) + (i & 7);
+          smask[i] = cg < cvs ? mask[(size_t)(r0 + (i >> 3)) * cvs + cg] : 0u;
+        }
       }
       __syncthreads();
     }
     float acc[2][kVec];
 #pragma unroll
     for (int i = 0; i < kVec; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
-    if (active) {
+    {
       float mean[kVec], rstd[kVec];
 #pragma unroll
       for (int i = 0; i < kVec; ++i) { mean[i] = 0.f; rstd[i] = 0.f; }
@@ -920,8 +976,7 @@ bn_resident_bwd_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_
       }
       res_write_partials(acc, red, partial, g.P, p, g.C, c0);
     }
-    res_grid_sync(bar, gridDim.x);
-    if (!active) continue;
+    res_tile_sync(bar, g.P);
     res_reduce_partials(red, partial, g.P, g.C, c0);
     if (threadIdx.x < kResTile) {
       const float* tot = red + kResWarps * 2 * kResTile;
@@ -931,8 +986,8 @@ bn_resident_bwd_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_
         const float inv_r = 1.f / (float)g.R;
         const float s1 = tot[c], s2 = tot[kResTile + c];
         const float c1 = s1 * inv_r, c2 = s2 * inv_r;                 // mean(dy*), mean(dy* xhat)
-        const float mean = save_mean[ch], rstd = save_rstd[ch];
-        ka = gamma[ch] * rstd;
+        const float mean = smean, rstd = srstd;
+        ka = gam * rstd;
         kb = -ka * rstd * c2;
         kc = -ka * (c1 - mean * rstd * c2);
         if (p == 0) {
@@ -988,9 +1043,15 @@ bn_resident_bwd_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_
         tc::tma_store_2d(&map_dx, xd + (size_t)b * box_bytes, c0, rb);
         if (want_dres) tc::tma_store_2d(&map_dres, dyd + (size_t)b * box_bytes, c0, rb);
         tc::bulk_commit();
+        // the next wave's loads into the previous box, once that box's stores have read it: HBM streams the next wave's
+        // dy and x while this wave's dx (and dres) drain
+        if (next && b > 0) { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); load_box(b - 1, t + g.T); }
       }
     }
-    if (threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    if (threadIdx.x == 0) {
+      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+      if (next && nlive > 0) load_box(nlive - 1, t + g.T);
+    }
     __syncthreads();
   }
   if (threadIdx.x == 0) tc::bulk_wait_all();
@@ -1006,7 +1067,8 @@ bool resident_allowed() {
 
 struct ResPlan {
   bool ok = false;
-  ResGeom g{};
+  ResGeom g{};        // geometry of the first launch; launch k runs tiles [k * T * waves, (k + 1) * T * waves)
+  int launches = 0;
   int grid = 0;
   int smem = 0;
 };
@@ -1030,7 +1092,7 @@ ResPlan resident_plan(int R, int C, int streams) {
   const int ntiles = (C + kResTile - 1) / kResTile;
   const long long row_bytes = (long long)kResTile * 2 * streams + (streams == 2 ? 8 : 0);   // backward: + the mask bytes
   for (int T = ntiles; T >= 1 && R > 0; --T) {
-    int P = sms / T;
+    int P = std::min(sms / T, kResMaxPartialLoads * kResWarps);
     if (P < 1) continue;
     P = std::min(P, std::max(1, (R + 31) / 32));                        // >= 32 rows per CTA
     const int need = (R + P - 1) / P;
@@ -1039,8 +1101,11 @@ ResPlan resident_plan(int R, int C, int streams) {
     const int box_rows = (need + nbox - 1) / nbox;
     const long long slab = (long long)nbox * box_rows * row_bytes;
     if (slab > budget) continue;
-    if ((ntiles + T - 1) / T > kResMaxWaves) break;                     // fewer tiles per wave only adds waves
-    plan.g = ResGeom{R, C, T, (R + nbox * box_rows - 1) / (nbox * box_rows), box_rows, nbox, (ntiles + T - 1) / T};
+    const int waves = (ntiles + T - 1) / T;
+    if (waves > kResMaxLaunches * kResMaxWaves) break;                  // fewer tiles per wave only adds waves
+    plan.launches = (waves + kResMaxWaves - 1) / kResMaxWaves;
+    const int per_launch = (waves + plan.launches - 1) / plan.launches;
+    plan.g = ResGeom{R, C, T, (R + nbox * box_rows - 1) / (nbox * box_rows), box_rows, nbox, per_launch, 0, std::min(ntiles, T * per_launch)};
     plan.grid = plan.g.T * plan.g.P;
     plan.smem = (int)slab + kResFixedSmem;
     plan.ok = true;
@@ -1048,6 +1113,14 @@ ResPlan resident_plan(int R, int C, int streams) {
   }
   cache.emplace(key, plan);
   return plan;
+}
+
+// Geometry of launch k of a plan: the k-th contiguous range of T * waves channel tiles.
+ResGeom res_launch(const ResPlan& plan, int k) {
+  ResGeom g = plan.g;
+  g.tile0 = k * g.T * g.waves;
+  g.tile_end = std::min((g.C + kResTile - 1) / kResTile, g.tile0 + g.T * g.waves);
+  return g;
 }
 
 // [R, C] bf16, row-major, 64-channel x box_rows boxes, no swizzle; out-of-range rows / channels read as zero, stores clip.
@@ -1224,7 +1297,8 @@ void bn_workspace_sizes(int R, int C, size_t* partial_floats, size_t* counters) 
   const ResPlan fwd = resident_plan(R, C, 1), bwd = resident_plan(R, C, 2);
   const int p = std::max(fwd.ok ? fwd.g.P : 0, bwd.ok ? bwd.g.P : 0);
   *partial_floats = (size_t)2 * std::max(t.grid_y, p) * C;
-  *counters = (size_t)2 * t.grid_x + 2;      // tickets + generation words, then the resident kernels' grid barrier
+  // tickets + generation words of the two-pass kernels, then one {arrivals, generation} pair per resident tile slot
+  *counters = (size_t)2 * t.grid_x + 2 * (size_t)((C + kResTile - 1) / kResTile);
 }
 
 void launch_bn_forward(const void* x, const void* residual, void* y, unsigned char* mask, DType dt, int R, int C, const float* gamma, const float* beta,
@@ -1240,10 +1314,11 @@ void launch_bn_forward(const void* x, const void* residual, void* y, unsigned ch
       ensure_max_dynamic_smem(bn_resident_fwd_kernel, res_smem_limit(), smem_done);    // raised once: every plan fits below it
       const CUtensorMap mx = res_map(x, R, C, plan.g.box_rows), my = res_map(y, R, C, plan.g.box_rows);
       const CUtensorMap mres = residual != nullptr ? res_map(residual, R, C, plan.g.box_rows) : mx;
-      launch_cooperative(bn_resident_fwd_kernel, plan, s, mx, my, mres, (const __nv_bfloat16*)residual, mask, gamma, beta, running_mean, running_var,
-                         num_batches, save_mean, save_rstd, scale, shift, partial, counters + 2 * pick_tile(R, C).grid_x, eps, momentum, r,
-                         plan.g);
-      B200_COUNT_LAUNCH(1);
+      for (int k = 0; k < plan.launches; ++k)
+        launch_cooperative(bn_resident_fwd_kernel, plan, s, mx, my, mres, (const __nv_bfloat16*)residual, mask, gamma, beta, running_mean,
+                           running_var, num_batches, save_mean, save_rstd, scale, shift, partial, counters + 2 * pick_tile(R, C).grid_x, eps,
+                           momentum, r, res_launch(plan, k));
+      B200_COUNT_LAUNCH(plan.launches);
       return;
     }
   }
@@ -1336,9 +1411,10 @@ void launch_bn_backward(const void* dy, const void* x, const void* y, void* dx, 
       const int br = plan.g.box_rows;
       const CUtensorMap mdy = res_map(dy, R, C, br), mx = res_map(x, R, C, br), mdx = res_map(dx, R, C, br);
       const CUtensorMap mdres = dres != nullptr ? res_map(dres, R, C, br) : mdx;
-      launch_cooperative(bn_resident_bwd_kernel, plan, s, mdy, mx, mdx, mdres, (const unsigned char*)y, save_mean, save_rstd, gamma, dgamma,
-                         dbeta, coef, partial, counters + 2 * pick_tile(R, C).grid_x, r, dres != nullptr ? 1 : 0, plan.g);
-      B200_COUNT_LAUNCH(1);
+      for (int k = 0; k < plan.launches; ++k)
+        launch_cooperative(bn_resident_bwd_kernel, plan, s, mdy, mx, mdx, mdres, (const unsigned char*)y, save_mean, save_rstd, gamma, dgamma,
+                           dbeta, coef, partial, counters + 2 * pick_tile(R, C).grid_x, r, dres != nullptr ? 1 : 0, res_launch(plan, k));
+      B200_COUNT_LAUNCH(plan.launches);
       return;
     }
   }
