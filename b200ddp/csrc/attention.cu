@@ -1,5 +1,5 @@
 // Multi-head attention with a key-padding mask on the Hopper tensor cores (the BERT encoder's attention for right-padded
-// batches).  Head dim 64, softmax scale 1/8.
+// batches).  Head dim 64, softmax scale 1/8; the causal mode also runs at head dim 128 (last section of this file).
 //
 //   qkv  bf16 [B*S, 3*H*64]   the fused projection's output: column blocks query | key | value, head h at h*64 .. h*64+63
 //   o    bf16 [B*S, H*64]     written in the layout the output projection reads (no transpose)
@@ -798,6 +798,467 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
   }
 }
 
+// ============================================== head dim 128 (kCausal, grouped-query) ================================
+// The same causal-document contract, grid walk and determinism as the kernels above, at d = 128 for
+// qkv [B*S, (H + 2*Hkv)*128] (Hkv == H is multi-head attention).  A TMA box row is at most one 128-byte swizzle row, so a
+// tile of R rows x 128 columns is two R x 64 chunks side by side in shared memory, chunk 1 at R * 128 bytes: Q K^T walks
+// eight k16 steps, four per chunk, and an N = 128 product (P V, dS K, P^T dO, dS^T Q) is one wgmma n64 per chunk into two
+// 32-register accumulator halves.  The tiles are those of d = 64; the accumulators double (forward O: 64 registers,
+// dQ: 64, dK + dV: 128), which does not fit the 168 registers a thread gets at 384 threads and one CTA per SM.  So the
+// producer warpgroup, which needs few, gives registers back (setmaxnreg: 40) and the two consumer warpgroups take them
+// (232 each: 40 * 128 + 232 * 256 = 168 * 384).
+constexpr int kHd128 = 128;
+constexpr float kScale128 = 0.08838834764831845f;              // 1/sqrt(128)
+constexpr float kScale128Log2 = kScale128 * kLog2e;
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+constexpr int kFwd128Smem = 1024 + 4 * kBoxBytes + kFwdStages * 8 * kBoxBytes + 256;   // Q 128 x 128 + ring of (K, V) 128 x 128
+constexpr int kBwd128Smem = 1024 + 8 * kBoxBytes + kBwdStages * 4 * kBoxBytes + 256;   // fixed 2 x (128 x 128) + ring of 2 x (64 x 128)
+
+// S (+)= A B^T over d = 128: A and B K-major tiles of 64 rows, chunk 1 at a + a_chunk and b + b_chunk bytes
+__device__ __forceinline__ void mma_hd128_n64(float (&acc)[32], uint32_t a, uint32_t a_chunk, uint32_t b, uint32_t b_chunk) {
+#pragma unroll
+  for (int k = 0; k < kHd128 / 16; ++k)
+    wgmma_n64<0, 0>(acc, desc_k(a + (k >> 2) * a_chunk + (k & 3) * kStepK), desc_k(b + (k >> 2) * b_chunk + (k & 3) * kStepK),
+                    k != 0 ? 1u : 0u);
+}
+// D += A B over 16 kSteps k rows, N = 128: A the register fragments a[4 kSteps], B MN-major with chunk 1 at b + b_chunk
+template <int kSteps>
+__device__ __forceinline__ void mma_rs_n128(float (&d0)[32], float (&d1)[32], const uint32_t* a, uint32_t b, uint32_t b_chunk) {
+#pragma unroll
+  for (int kk = 0; kk < kSteps; ++kk) {
+    wgmma_n64_rs<1>(d0, a + 4 * kk, desc_mn(b + kk * kStepMN), 1u);
+    wgmma_n64_rs<1>(d1, a + 4 * kk, desc_mn(b + b_chunk + kk * kStepMN), 1u);
+  }
+}
+// TMA-loads `rows` (a multiple of 64) rows x 128 columns from column col, row row into two chunks at dst, dst + rows * 128
+__device__ __forceinline__ void tma_load_tile128(const CUtensorMap* map, uint64_t* bar, uint8_t* dst, int col, int row, int rows) {
+  for (int c = 0; c < 2; ++c)
+    for (int r = 0; r < rows; r += kBoxRows) tma_load_2d(map, bar, dst + (c * rows + r) * 128, col + c * kHd, row + r);
+}
+__device__ __forceinline__ void zero_rows128(__nv_bfloat16* base, size_t pitch, size_t row0, int rows) {
+  zero_rows(base, pitch, row0, rows);
+  zero_rows(base + kHd, pitch, row0, rows);
+}
+
+__global__ void __launch_bounds__(kThreads, 1)
+attn_fwd_d128_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restrict__ bounds, int S, int H,
+                     __nv_bfloat16* __restrict__ o, float* __restrict__ lse, int Hkv) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = align1024(smem_raw);
+  uint8_t* sq = smem;                                           // 128 query rows x 128
+  uint8_t* ring = sq + 4 * kBoxBytes;                           // stage: K 128 x 128, V 128 x 128
+  uint64_t* q_bar = reinterpret_cast<uint64_t*>(ring + kFwdStages * 8 * kBoxBytes);
+  uint64_t* full_bar = q_bar + 1;
+  uint64_t* empty_bar = full_bar + kFwdStages;
+
+  const int3 tc = tile_coords<kCausal, false>();
+  const int qt = tc.x, h = tc.y, b = tc.z;
+  const int HD = H * kHd128;
+  const size_t seq_row = (size_t)b * S;
+  const int2 r = cta_range<kCausal, false>(bounds, seq_row + qt * 128, qt * 128, S, reinterpret_cast<int*>(empty_bar + kFwdStages));
+  const int kt0 = r.x / 128;
+  const int n_kt = r.x < r.y ? (r.y + 127) / 128 - kt0 : 0;   // key tiles kt0 .. kt0 + n_kt - 1
+  float* lse_bh = lse + ((size_t)b * H + h) * S;
+  if (n_kt == 0) {
+    zero_rows128(o + h * kHd128, HD, seq_row + qt * 128, 128);
+    if (threadIdx.x < 128) lse_bh[qt * 128 + threadIdx.x] = -INFINITY;
+    return;
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 1 && lane == 0) {
+    mbar_init(q_bar, 1);
+    for (int i = 0; i < kFwdStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerArrivals); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    warpgroup_reg_dealloc<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
+      tma_prefetch_desc(&map_qkv);
+      const int q_row = (int)seq_row + qt * 128;
+      mbar_expect_tx(q_bar, 4 * kBoxBytes);
+      tma_load_tile128(&map_qkv, q_bar, sq, h * kHd128, q_row, 128);
+      const int hk = h / (H / Hkv);
+      const int kcol = HD + hk * kHd128, vcol = HD + (Hkv + hk) * kHd128;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int kt = kt0; kt < kt0 + n_kt; ++kt) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sk = ring + stage * 8 * kBoxBytes;
+        mbar_expect_tx(&full_bar[stage], 8 * kBoxBytes);
+        tma_load_tile128(&map_qkv, &full_bar[stage], sk, kcol, (int)seq_row + kt * 128, 128);
+        tma_load_tile128(&map_qkv, &full_bar[stage], sk + 4 * kBoxBytes, vcol, (int)seq_row + kt * 128, 128);
+        if (++stage == kFwdStages) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    warpgroup_reg_alloc<kConsumerRegs>();
+    const int wg = (warp - 4) >> 2;                             // query rows [64 wg, 64 wg + 64) of the tile
+    const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+    const uint32_t q_addr = smem_u32(sq + wg * kBoxBytes);      // chunk 1 at + 2 * kBoxBytes
+    const int row = qt * 128 + wg * 64 + r0;                    // position in the sequence
+    const int2 rb0 = mask_interval<kCausal, false>(bounds, seq_row + row, row, S);
+    const int2 rb1 = mask_interval<kCausal, false>(bounds, seq_row + row + 8, row + 8, S);
+    float acc0[32], acc1[32];                                   // O columns 0-63, 64-127
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    mbar_wait(q_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int kt = kt0; kt < kt0 + n_kt; ++kt) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t k_addr = smem_u32(ring + stage * 8 * kBoxBytes);   // K and V: chunk 1 at + 2 * kBoxBytes
+      const uint32_t v_addr = k_addr + 4 * kBoxBytes;
+      float s[64];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kHd128 / 16; ++k)
+        wgmma_n128<0, 0>(s, desc_k(q_addr + (k >> 2) * 2 * kBoxBytes + (k & 3) * kStepK),
+                         desc_k(k_addr + (k >> 2) * 2 * kBoxBytes + (k & 3) * kStepK), k != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      const int key0 = kt * 128;
+      if (key0 < max(rb0.x, rb1.x) || key0 + 128 > min(rb0.y, rb1.y)) {   // tile not wholly inside both intervals
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int key = key0 + 8 * j + c0 + e;
+            if (!inside(key, rb0)) s[4 * j + e] = -INFINITY;
+            if (!inside(key, rb1)) s[4 * j + 2 + e] = -INFINITY;
+          }
+        }
+      }
+      float mx[2] = {m[0], m[1]};
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
+        mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
+      }
+      float alpha[2], mb[2], rs[2] = {0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+        mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+        const float base = mx[i] == -INFINITY ? 0.f : mx[i];   // no visible key yet: exp2 gives 0 rather than NaN
+        alpha[i] = exp2f((m[i] - base) * kScale128Log2);
+        m[i] = mx[i];
+        mb[i] = base * kScale128Log2;
+      }
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        s[4 * j] = exp2f(s[4 * j] * kScale128Log2 - mb[0]);
+        s[4 * j + 1] = exp2f(s[4 * j + 1] * kScale128Log2 - mb[0]);
+        s[4 * j + 2] = exp2f(s[4 * j + 2] * kScale128Log2 - mb[1]);
+        s[4 * j + 3] = exp2f(s[4 * j + 3] * kScale128Log2 - mb[1]);
+        rs[0] += s[4 * j] + s[4 * j + 1];
+        rs[1] += s[4 * j + 2] + s[4 * j + 3];
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) l[i] = l[i] * alpha[i] + rs[i];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        acc0[4 * j] *= alpha[0]; acc0[4 * j + 1] *= alpha[0]; acc0[4 * j + 2] *= alpha[1]; acc0[4 * j + 3] *= alpha[1];
+        acc1[4 * j] *= alpha[0]; acc1[4 * j + 1] *= alpha[0]; acc1[4 * j + 2] *= alpha[1]; acc1[4 * j + 3] *= alpha[1];
+      }
+      // O += P V: P from registers (16 keys per k16 step), V MN-major, one n64 per 64-column chunk
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint32_t a[4] = {pack_bf16x2(s[8 * kk], s[8 * kk + 1]), pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]),
+                               pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7])};
+        wgmma_n64_rs<1>(acc0, a, desc_mn(v_addr + kk * kStepMN), 1u);
+        wgmma_n64_rs<1>(acc1, a, desc_mn(v_addr + 2 * kBoxBytes + kk * kStepMN), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == kFwdStages) { stage = 0; phase ^= 1; }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+      l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+    }
+    const float sc0 = l[0] > 0.f ? 1.f / l[0] : 0.f, sc1 = l[1] > 0.f ? 1.f / l[1] : 0.f;   // no key seen: zeros, -inf
+    __nv_bfloat16* orow = o + (seq_row + row) * HD + h * kHd128;
+    store_frag(acc0, sc0, sc1, orow, HD, c0);
+    store_frag(acc1, sc0, sc1, orow + kHd, HD, c0);
+    if ((lane & 3) == 0) {
+      lse_bh[row] = l[0] > 0.f ? m[0] * kScale128 + logf(l[0]) : -INFINITY;
+      lse_bh[row + 8] = l[1] > 0.f ? m[1] * kScale128 + logf(l[1]) : -INFINITY;
+    }
+  }
+}
+
+// D[b, h, s] = sum_d dO[b*S + s, h*128 + d] * O[b*S + s, h*128 + d]; sixteen threads per (row, head), 16 bytes each
+__global__ void attn_bwd_dot_d128_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* __restrict__ out, int rows,
+                                         int S, int H, float* __restrict__ D) {
+  const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t item = gid >> 4;
+  const int part = (int)(gid & 15);
+  const bool live = item < (size_t)rows * H;
+  float acc = 0.f;
+  if (live) {
+    const size_t off = item * kHd128 + part * 8;              // [rows, H * 128] row-major: item = row * H + head
+    float a[8], c[8];
+    unpack8(*reinterpret_cast<const Bf16x8*>(dout + off), a);
+    unpack8(*reinterpret_cast<const Bf16x8*>(out + off), c);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc += a[i] * c[i];
+  }
+  acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 8);
+  if (live && part == 0) {
+    const size_t row = item / H, hh = item % H;
+    const size_t b = row / S, s = row % S;
+    D[(b * H + hh) * S + s] = acc;
+  }
+}
+
+// Shared layout of both d = 128 backward kernels: fixed0, fixed1 of 128 x 128 (4 boxes each), then a ring of two 64 x 128
+// tiles (2 boxes each) per stage.
+__device__ __forceinline__ BwdSmem bwd128_smem(uint8_t* raw) {
+  BwdSmem L;
+  L.fixed0 = align1024(raw);
+  L.fixed1 = L.fixed0 + 4 * kBoxBytes;
+  L.ring = L.fixed1 + 4 * kBoxBytes;
+  L.fixed_bar = reinterpret_cast<uint64_t*>(L.ring + kBwdStages * 4 * kBoxBytes);
+  L.full_bar = L.fixed_bar + 1;
+  L.empty_bar = L.full_bar + kBwdStages;
+  return L;
+}
+
+// dK, dV for one tile of 128 keys of K/V head hk.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries inside the union of the
+// key rows' intervals, for every query head of the group in turn; the whole group accumulates in registers, so each
+// dK / dV element has one writer.
+__global__ void __launch_bounds__(kThreads, 1)
+attn_bwd_dkdv_d128_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
+                          const int* __restrict__ bounds, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
+                          __nv_bfloat16* __restrict__ dqkv, int Hkv) {
+  extern __shared__ uint8_t smem_raw[];
+  const BwdSmem L = bwd128_smem(smem_raw);
+  const int3 tc = tile_coords<kCausal, true>();
+  const int kt = tc.x, hk = tc.y, b = tc.z;
+  const int HD = H * kHd128;
+  const size_t pitch = (size_t)(H + 2 * Hkv) * kHd128;
+  const int groups = H / Hkv;                                   // query heads hk * groups + g read this K/V head
+  const int kcol = HD + hk * kHd128, vcol = HD + (Hkv + hk) * kHd128;
+  const size_t seq_row = (size_t)b * S;
+  const int2 r = cta_range<kCausal, true>(bounds, seq_row + kt * 128, kt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
+  if (r.x >= r.y) {                                             // every key of the tile is hidden: no gradient
+    zero_rows128(dqkv + kcol, pitch, seq_row + kt * 128, 128);
+    zero_rows128(dqkv + vcol, pitch, seq_row + kt * 128, 128);
+    return;
+  }
+  const int qt0 = r.x / 64, n_qt = (r.y + 63) / 64 - qt0;      // query tiles qt0 .. qt0 + n_qt - 1
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 1 && lane == 0) bwd_init_barriers(L);
+  __syncthreads();
+
+  if (warp < 4) {
+    warpgroup_reg_dealloc<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
+      tma_prefetch_desc(&map_qkv);
+      tma_prefetch_desc(&map_do);
+      mbar_expect_tx(L.fixed_bar, 8 * kBoxBytes);
+      tma_load_tile128(&map_qkv, L.fixed_bar, L.fixed0, kcol, (int)seq_row + kt * 128, 128);
+      tma_load_tile128(&map_qkv, L.fixed_bar, L.fixed1, vcol, (int)seq_row + kt * 128, 128);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int g = 0; g < groups; ++g) {
+        const int col = (hk * groups + g) * kHd128;
+        for (int i = 0; i < n_qt; ++i) {
+          mbar_wait(&L.empty_bar[stage], phase ^ 1);
+          uint8_t* t0 = L.ring + stage * 4 * kBoxBytes;
+          mbar_expect_tx(&L.full_bar[stage], 4 * kBoxBytes);
+          tma_load_tile128(&map_qkv, &L.full_bar[stage], t0, col, (int)seq_row + 64 * (qt0 + i), 64);
+          tma_load_tile128(&map_do, &L.full_bar[stage], t0 + 2 * kBoxBytes, col, (int)seq_row + 64 * (qt0 + i), 64);
+          if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    warpgroup_reg_alloc<kConsumerRegs>();
+    const int wg = (warp - 4) >> 2;                             // keys [64 wg, 64 wg + 64) of the tile
+    const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+    const int key = kt * 128 + wg * 64 + r0;
+    const uint32_t k_addr = smem_u32(L.fixed0 + wg * kBoxBytes), v_addr = smem_u32(L.fixed1 + wg * kBoxBytes);   // chunk 1: + 2 boxes
+    float dv0[32], dv1[32], dk0[32], dk1[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { dv0[i] = 0.f; dv1[i] = 0.f; dk0[i] = 0.f; dk1[i] = 0.f; }
+    mbar_wait(L.fixed_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    // lse / D rows of query heads hk * groups + g, with a 32-bit offset (B * H * S < 2^31)
+    const int bh_end = (b * H + (hk + 1) * groups) * S;
+#pragma unroll 1
+    for (int bh = (b * H + hk * groups) * S; bh < bh_end; bh += S) {
+      for (int qt = qt0; qt < qt0 + n_qt; ++qt) {
+        const int2 kb0 = mask_interval<kCausal, true>(bounds, seq_row + key, key, S);
+        const int2 kb1 = mask_interval<kCausal, true>(bounds, seq_row + key + 8, key + 8, S);
+        const int q0 = qt * 64 + c0;
+        const uint32_t vis = frag_mask16(kb0.x - q0, kb0.y - q0) | (frag_mask16(kb1.x - q0, kb1.y - q0) << 16);
+        mbar_wait(&L.full_bar[stage], phase);
+        const uint32_t q_addr = smem_u32(L.ring + stage * 4 * kBoxBytes), do_addr = q_addr + 2 * kBoxBytes;   // chunk 1: + 1 box
+        // two halves of 32 queries: S^T and dP^T of a whole 64-query tile (64 registers) beside the 128 of dK and dV
+        // would not fit the consumers' 232
+#pragma unroll 1
+        for (int half = 0; half < 2; ++half) {
+          const uint32_t qh = q_addr + half * 32 * 128, doh = do_addr + half * 32 * 128;
+          float st[16], dpt[16];
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < kHd128 / 16; ++k) {               // S^T = K Q^T, dP^T = V dO^T   [keys, 32 queries]
+            const uint32_t ko = (k >> 2) * 2 * kBoxBytes + (k & 3) * kStepK, qo = (k >> 2) * kBoxBytes + (k & 3) * kStepK;
+            wgmma_n32<0, 0>(st, desc_k(k_addr + ko), desc_k(qh + qo), k != 0 ? 1u : 0u);
+            wgmma_n32<0, 0>(dpt, desc_k(v_addr + ko), desc_k(doh + qo), k != 0 ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          uint32_t pa[8], dsa[8];
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {                      // query columns 32 half + 8 jj + c0, + 1
+            const int j = 4 * half + jj;                        // of the tile: bits 2 j, 2 j + 1 of vis
+            const int q = qt * 64 + 8 * j + c0;
+            const float2 lq = *reinterpret_cast<const float2*>(lse + (bh + q));
+            const float2 dq = *reinterpret_cast<const float2*>(Dsum + (bh + q));
+            const float l0 = lq.x == -INFINITY ? INFINITY : lq.x * kLog2e;   // a query that saw no key gets P = 0
+            const float l1 = lq.y == -INFINITY ? INFINITY : lq.y * kLog2e;
+            const bool v00 = (vis >> (2 * j)) & 1u, v01 = (vis >> (2 * j + 1)) & 1u;
+            const bool v10 = (vis >> (16 + 2 * j)) & 1u, v11 = (vis >> (17 + 2 * j)) & 1u;
+            const float p00 = v00 ? exp2f(st[4 * jj] * kScale128Log2 - l0) : 0.f;
+            const float p01 = v01 ? exp2f(st[4 * jj + 1] * kScale128Log2 - l1) : 0.f;
+            const float p10 = v10 ? exp2f(st[4 * jj + 2] * kScale128Log2 - l0) : 0.f;
+            const float p11 = v11 ? exp2f(st[4 * jj + 3] * kScale128Log2 - l1) : 0.f;
+            pa[2 * jj] = pack_bf16x2(p00, p01);
+            pa[2 * jj + 1] = pack_bf16x2(p10, p11);
+            dsa[2 * jj] = pack_bf16x2(p00 * (dpt[4 * jj] - dq.x), p01 * (dpt[4 * jj + 1] - dq.y));
+            dsa[2 * jj + 1] = pack_bf16x2(p10 * (dpt[4 * jj + 2] - dq.x), p11 * (dpt[4 * jj + 3] - dq.y));
+          }
+          wgmma_fence();
+          mma_rs_n128<2>(dv0, dv1, pa, doh, kBoxBytes);        // dV += P^T dO
+          mma_rs_n128<2>(dk0, dk1, dsa, qh, kBoxBytes);        // dK += dS^T Q
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&L.empty_bar[stage]);
+        if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+      }
+    }
+    __nv_bfloat16* krow = dqkv + (seq_row + key) * pitch + kcol;
+    store_frag(dk0, kScale128, kScale128, krow, pitch, c0);
+    store_frag(dk1, kScale128, kScale128, krow + kHd, pitch, c0);
+    store_frag(dv0, 1.f, 1.f, krow + (vcol - kcol), pitch, c0);
+    store_frag(dv1, 1.f, 1.f, krow + (vcol - kcol) + kHd, pitch, c0);
+  }
+}
+
+// dQ for one tile of 128 queries.  Fixed: Q, dO.  Ring: (K, V) tiles of 64 keys of the query head's K/V head inside the
+// union of the query rows' intervals.
+__global__ void __launch_bounds__(kThreads, 1)
+attn_bwd_dq_d128_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
+                        const int* __restrict__ bounds, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
+                        __nv_bfloat16* __restrict__ dqkv, int Hkv) {
+  extern __shared__ uint8_t smem_raw[];
+  const BwdSmem L = bwd128_smem(smem_raw);
+  const int3 tc = tile_coords<kCausal, false>();
+  const int qt = tc.x, h = tc.y, b = tc.z;
+  const int HD = H * kHd128;
+  const size_t pitch = (size_t)(H + 2 * Hkv) * kHd128;
+  const size_t seq_row = (size_t)b * S;
+  const int2 r = cta_range<kCausal, false>(bounds, seq_row + qt * 128, qt * 128, S, reinterpret_cast<int*>(L.empty_bar + kBwdStages));
+  if (r.x >= r.y) {
+    zero_rows128(dqkv + h * kHd128, pitch, seq_row + qt * 128, 128);
+    return;
+  }
+  const int kt0 = r.x / 64, n_kt = (r.y + 63) / 64 - kt0;      // key tiles kt0 .. kt0 + n_kt - 1
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (warp == 1 && lane == 0) bwd_init_barriers(L);
+  __syncthreads();
+
+  if (warp < 4) {
+    warpgroup_reg_dealloc<kProducerRegs>();
+    if (warp == 0 && lane == 0) {
+      tma_prefetch_desc(&map_qkv);
+      tma_prefetch_desc(&map_do);
+      mbar_expect_tx(L.fixed_bar, 8 * kBoxBytes);
+      tma_load_tile128(&map_qkv, L.fixed_bar, L.fixed0, h * kHd128, (int)seq_row + qt * 128, 128);
+      tma_load_tile128(&map_do, L.fixed_bar, L.fixed1, h * kHd128, (int)seq_row + qt * 128, 128);
+      const int hk = h / (H / Hkv);
+      const int kcol = HD + hk * kHd128, vcol = HD + (Hkv + hk) * kHd128;
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int i = 0; i < n_kt; ++i) {
+        mbar_wait(&L.empty_bar[stage], phase ^ 1);
+        uint8_t* t0 = L.ring + stage * 4 * kBoxBytes;
+        mbar_expect_tx(&L.full_bar[stage], 4 * kBoxBytes);
+        tma_load_tile128(&map_qkv, &L.full_bar[stage], t0, kcol, (int)seq_row + 64 * (kt0 + i), 64);
+        tma_load_tile128(&map_qkv, &L.full_bar[stage], t0 + 2 * kBoxBytes, vcol, (int)seq_row + 64 * (kt0 + i), 64);
+        if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else {
+    warpgroup_reg_alloc<kConsumerRegs>();
+    const int wg = (warp - 4) >> 2;
+    const int r0 = 16 * ((warp - 4) & 3) + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+    const int row = qt * 128 + wg * 64 + r0;
+    const int2 qb0 = mask_interval<kCausal, false>(bounds, seq_row + row, row, S);
+    const int2 qb1 = mask_interval<kCausal, false>(bounds, seq_row + row + 8, row + 8, S);
+    const uint32_t q_addr = smem_u32(L.fixed0 + wg * kBoxBytes), do_addr = smem_u32(L.fixed1 + wg * kBoxBytes);   // chunk 1: + 2 boxes
+    const size_t bh = ((size_t)b * H + h) * S;
+    const float l0 = lse[bh + row] * kLog2e, l1 = lse[bh + row + 8] * kLog2e;
+    const float d0 = Dsum[bh + row], d1 = Dsum[bh + row + 8];
+    float dq0[32], dq1[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { dq0[i] = 0.f; dq1[i] = 0.f; }
+    mbar_wait(L.fixed_bar, 0);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int kt = kt0; kt < kt0 + n_kt; ++kt) {
+      mbar_wait(&L.full_bar[stage], phase);
+      const uint32_t k_addr = smem_u32(L.ring + stage * 4 * kBoxBytes), v_addr = k_addr + 2 * kBoxBytes;   // chunk 1: + 1 box
+      float s[32], dp[32];
+      wgmma_fence();
+      mma_hd128_n64(s, q_addr, 2 * kBoxBytes, k_addr, kBoxBytes);      // S = Q K^T
+      mma_hd128_n64(dp, do_addr, 2 * kBoxBytes, v_addr, kBoxBytes);    // dP = dO V^T
+      wgmma_commit();
+      wgmma_wait<0>();
+      uint32_t dsa[16];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int k0 = kt * 64 + 8 * j + c0;
+        const float p00 = inside(k0, qb0) ? exp2f(s[4 * j] * kScale128Log2 - l0) : 0.f;
+        const float p01 = inside(k0 + 1, qb0) ? exp2f(s[4 * j + 1] * kScale128Log2 - l0) : 0.f;
+        const float p10 = inside(k0, qb1) ? exp2f(s[4 * j + 2] * kScale128Log2 - l1) : 0.f;
+        const float p11 = inside(k0 + 1, qb1) ? exp2f(s[4 * j + 3] * kScale128Log2 - l1) : 0.f;
+        dsa[2 * j] = pack_bf16x2(p00 * (dp[4 * j] - d0), p01 * (dp[4 * j + 1] - d0));
+        dsa[2 * j + 1] = pack_bf16x2(p10 * (dp[4 * j + 2] - d1), p11 * (dp[4 * j + 3] - d1));
+      }
+      wgmma_fence();
+      mma_rs_n128<4>(dq0, dq1, dsa, k_addr, kBoxBytes);        // dQ += dS K
+      wgmma_commit();
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&L.empty_bar[stage]);
+      if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
+    }
+    __nv_bfloat16* qrow = dqkv + (seq_row + row) * pitch + h * kHd128;
+    store_frag(dq0, kScale128, kScale128, qrow, pitch, c0);
+    store_frag(dq1, kScale128, kScale128, qrow + kHd, pitch, c0);
+  }
+}
+
 CUtensorMap rows_map(const void* ptr, int rows, int cols) {
   const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows};
   const uint64_t strides[1] = {(uint64_t)cols * 2};
@@ -805,15 +1266,15 @@ CUtensorMap rows_map(const void* ptr, int rows, int cols) {
   return conv_encode_map(ptr, 2, dims, strides, box);
 }
 
-// heads query heads and kv_heads K/V heads (equal for multi-head attention; a divisor of heads for GQA)
-void check_shape(const char* who, int B, int S, int heads, int kv_heads) {
+// heads query heads and kv_heads K/V heads (equal for multi-head attention; a divisor of heads for GQA) of width hd
+void check_shape(const char* who, int B, int S, int heads, int kv_heads, int hd = kHd) {
   if (B < 1 || heads < 1 || S < 128 || S % 128 != 0)
     throw std::runtime_error(std::string(who) + ": needs B >= 1, heads >= 1 and S a positive multiple of 128 (got B=" +
                              std::to_string(B) + ", S=" + std::to_string(S) + ", heads=" + std::to_string(heads) + ")");
   if (kv_heads < 1 || heads % kv_heads != 0)
     throw std::runtime_error(std::string(who) + ": kv_heads must divide heads (got heads=" + std::to_string(heads) +
                              ", kv_heads=" + std::to_string(kv_heads) + ")");
-  if (B > 65535 || (long long)B * S * (heads + 2 * kv_heads) * kHd >= (1ll << 31))
+  if (B > 65535 || (long long)B * S * (heads + 2 * kv_heads) * hd >= (1ll << 31))
     throw std::runtime_error(std::string(who) + ": problem too large");
 }
 
@@ -854,6 +1315,38 @@ void attention_bwd(const char* who, const void* dout, const void* qkv, const voi
 }
 
 }  // namespace
+
+void launch_causal_attention_d128_fwd(const void* qkv, const int* bounds, int B, int S, int heads, int kv_heads, void* o, float* lse, cudaStream_t s) {
+  check_shape("causal_attention_d128_fwd", B, S, heads, kv_heads, kHd128);
+  const CUtensorMap map_qkv = rows_map(qkv, B * S, (heads + 2 * kv_heads) * kHd128);
+  static std::atomic<unsigned long long> configured{0};
+  ensure_max_dynamic_smem(attn_fwd_d128_kernel, kFwd128Smem, configured);
+  attn_fwd_d128_kernel<<<dim3(S / 128, heads, B), kThreads, kFwd128Smem, s>>>(map_qkv, bounds, S, heads,
+                                                                              reinterpret_cast<__nv_bfloat16*>(o), lse, kv_heads);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void launch_causal_attention_d128_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                      int S, int heads, int kv_heads, float* dsum, void* dqkv, cudaStream_t s) {
+  check_shape("causal_attention_d128_bwd", B, S, heads, kv_heads, kHd128);
+  const int rows = B * S;
+  const long long items = (long long)rows * heads * 16;
+  attn_bwd_dot_d128_kernel<<<ceil_div(items, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dout),
+                                                                reinterpret_cast<const __nv_bfloat16*>(o), rows, S, heads, dsum);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  const CUtensorMap map_qkv = rows_map(qkv, rows, (heads + 2 * kv_heads) * kHd128);
+  const CUtensorMap map_do = rows_map(dout, rows, heads * kHd128);
+  auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
+  static std::atomic<unsigned long long> configured_dkdv{0}, configured_dq{0};
+  ensure_max_dynamic_smem(attn_bwd_dkdv_d128_kernel, kBwd128Smem, configured_dkdv);
+  ensure_max_dynamic_smem(attn_bwd_dq_d128_kernel, kBwd128Smem, configured_dq);
+  attn_bwd_dkdv_d128_kernel<<<dim3(S / 128, kv_heads, B), kThreads, kBwd128Smem, s>>>(map_qkv, map_do, bounds, S, heads, lse, dsum,
+                                                                                       dq, kv_heads);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  attn_bwd_dq_d128_kernel<<<dim3(S / 128, heads, B), kThreads, kBwd128Smem, s>>>(map_qkv, map_do, bounds, S, heads, lse, dsum, dq,
+                                                                                  kv_heads);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
 
 void launch_attention_fwd(const void* qkv, const int* seq_lens, int B, int S, int heads, void* o, float* lse, cudaStream_t s) {
   attention_fwd<kKeyPadding>("attention_fwd", qkv, seq_lens, B, S, heads, o, lse, s, heads);

@@ -199,6 +199,66 @@ struct OptPlan {
   }
 };
 
+// grouped-query causal documents: qkv [B*S, (heads + 2*kv_heads)*hd] with head dim hd = 64 (causal_gqa_attention_*) or
+// 128 (causal_attention_d128_*, kv_heads == heads included); the same bounds as the packed pair
+int gqa_check(const at::Tensor& qkv, const at::Tensor& bounds, int heads, int kv_heads, int hd, const char* who) {
+  check_cuda(qkv, "qkv");
+  TORCH_CHECK(qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 2 && qkv.is_contiguous(), who,
+              ": qkv must be contiguous bf16 [B*S, (heads + 2*kv_heads)*", hd, "]");
+  TORCH_CHECK(heads >= 1 && kv_heads >= 1 && heads % kv_heads == 0, who, ": kv_heads (", kv_heads, ") must divide heads (", heads, ")");
+  TORCH_CHECK(qkv.size(1) == (int64_t)(heads + 2 * kv_heads) * hd, who, ": qkv has ", qkv.size(1),
+              " columns, expected (heads + 2 * kv_heads) * ", hd, " with heads = ", heads, ", kv_heads = ", kv_heads);
+  check_cuda(bounds, "bounds");
+  TORCH_CHECK(bounds.scalar_type() == at::kInt && bounds.dim() == 3 && bounds.size(2) == 2 && bounds.is_contiguous() && bounds.numel() >= 2,
+              who, ": bounds must be contiguous int32 [B, S, 2]");
+  TORCH_CHECK(qkv.size(0) == bounds.size(0) * bounds.size(1), who, ": qkv rows (", qkv.size(0), ") are not B * S for bounds [",
+              bounds.size(0), ", ", bounds.size(1), ", 2]");
+  TORCH_CHECK(bounds.device() == qkv.device(), who, ": bounds must be on qkv's device");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(qkv.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(bounds.data_ptr()) & 7) == 0,
+              who, ": qkv must be 16-byte and bounds 8-byte aligned");
+  return (int)bounds.size(0);
+}
+
+using GqaFwd = void (*)(const void*, const int*, int, int, int, int, void*, float*, cudaStream_t);
+using GqaBwd = void (*)(const void*, const void*, const void*, const float*, const int*, int, int, int, int, float*, void*, cudaStream_t);
+
+std::tuple<at::Tensor, at::Tensor> gqa_fwd(GqaFwd launch, int hd, const char* who, const at::Tensor& qkv, const at::Tensor& bounds,
+                                           int heads, int kv_heads, c10::optional<at::Tensor> o_out, c10::optional<at::Tensor> lse_out) {
+  const int B = gqa_check(qkv, bounds, heads, kv_heads, hd, who);
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int S = (int)(qkv.size(0) / B);
+  at::Tensor o = o_out.has_value() ? *o_out : at::empty({qkv.size(0), (int64_t)heads * hd}, qkv.options());
+  at::Tensor lse = lse_out.has_value() ? *lse_out : at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
+  TORCH_CHECK(o.is_cuda() && o.scalar_type() == at::kBFloat16 && o.is_contiguous() && o.numel() == qkv.size(0) * heads * hd, who, ": bad o");
+  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S, who, ": bad lse");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(o.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0,
+              who, ": o must be 16-byte and lse 8-byte aligned");
+  launch(qkv.data_ptr(), bounds.data_ptr<int>(), B, S, heads, kv_heads, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
+  return std::make_tuple(o, lse);
+}
+
+at::Tensor gqa_bwd(GqaBwd launch, int hd, const char* who, const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o,
+                   const at::Tensor& lse, const at::Tensor& bounds, int heads, int kv_heads, c10::optional<at::Tensor> dqkv_out) {
+  const int B = gqa_check(qkv, bounds, heads, kv_heads, hd, who);
+  c10::cuda::CUDAGuard guard(qkv.device());
+  const int S = (int)(qkv.size(0) / B);
+  for (const at::Tensor* t : {&dout, &o}) {
+    check_cuda(*t, "dout / o");
+    TORCH_CHECK(t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->numel() == qkv.size(0) * heads * hd &&
+                (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, who, ": dout and o must be 16-byte aligned contiguous bf16 [B*S, heads*",
+                hd, "]");
+  }
+  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S &&
+              (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0, who, ": lse must be 8-byte aligned contiguous fp32 [B, heads, S]");
+  at::Tensor dqkv = dqkv_out.has_value() ? *dqkv_out : at::empty_like(qkv);
+  TORCH_CHECK(dqkv.is_cuda() && dqkv.scalar_type() == at::kBFloat16 && dqkv.is_contiguous() && dqkv.numel() == qkv.numel() &&
+              (reinterpret_cast<uintptr_t>(dqkv.data_ptr()) & 3) == 0, who, ": bad dqkv");
+  at::Tensor dsum = at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
+  launch(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), bounds.data_ptr<int>(), B, S, heads, kv_heads,
+         dsum.data_ptr<float>(), dqkv.data_ptr(), cur_stream());
+  return dqkv;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -661,77 +721,42 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     const int B = packed_check(qkv, bounds, heads, "causal_attention_bwd");
     return attn_bwd(&launch_causal_attention_bwd, "causal_attention_bwd", dout, qkv, o, lse, bounds, B, heads, dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("dqkv") = py::none());
-  // grouped-query causal documents: qkv [B*S, (heads + 2*kv_heads)*64]; the same bounds as the packed pair
-  auto gqa_check = [](const at::Tensor& qkv, const at::Tensor& bounds, int heads, int kv_heads, const char* who) {
-    check_cuda(qkv, "qkv");
-    TORCH_CHECK(qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 2 && qkv.is_contiguous(), who,
-                ": qkv must be contiguous bf16 [B*S, (heads + 2*kv_heads)*64]");
-    TORCH_CHECK(heads >= 1 && kv_heads >= 1 && heads % kv_heads == 0, who, ": kv_heads (", kv_heads, ") must divide heads (", heads, ")");
-    TORCH_CHECK(qkv.size(1) == (int64_t)(heads + 2 * kv_heads) * 64, who, ": qkv has ", qkv.size(1),
-                " columns, expected (heads + 2 * kv_heads) * 64 with heads = ", heads, ", kv_heads = ", kv_heads);
-    check_cuda(bounds, "bounds");
-    TORCH_CHECK(bounds.scalar_type() == at::kInt && bounds.dim() == 3 && bounds.size(2) == 2 && bounds.is_contiguous() && bounds.numel() >= 2,
-                who, ": bounds must be contiguous int32 [B, S, 2]");
-    TORCH_CHECK(qkv.size(0) == bounds.size(0) * bounds.size(1), who, ": qkv rows (", qkv.size(0), ") are not B * S for bounds [",
-                bounds.size(0), ", ", bounds.size(1), ", 2]");
-    TORCH_CHECK(bounds.device() == qkv.device(), who, ": bounds must be on qkv's device");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(qkv.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(bounds.data_ptr()) & 7) == 0,
-                who, ": qkv must be 16-byte and bounds 8-byte aligned");
-    return (int)bounds.size(0);
-  };
-  m.def("causal_gqa_attention_fwd", [gqa_check](at::Tensor qkv, at::Tensor bounds, int heads, int kv_heads, c10::optional<at::Tensor> o_out,
-                                                c10::optional<at::Tensor> lse_out) {
-    const char* who = "causal_gqa_attention_fwd";
-    const int B = gqa_check(qkv, bounds, heads, kv_heads, who);
-    c10::cuda::CUDAGuard guard(qkv.device());
-    const int S = (int)(qkv.size(0) / B);
-    at::Tensor o = o_out.has_value() ? *o_out : at::empty({qkv.size(0), (int64_t)heads * 64}, qkv.options());
-    at::Tensor lse = lse_out.has_value() ? *lse_out : at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-    TORCH_CHECK(o.is_cuda() && o.scalar_type() == at::kBFloat16 && o.is_contiguous() && o.numel() == qkv.size(0) * heads * 64, who, ": bad o");
-    TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S, who, ": bad lse");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(o.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0,
-                who, ": o must be 16-byte and lse 8-byte aligned");
-    launch_causal_gqa_attention_fwd(qkv.data_ptr(), bounds.data_ptr<int>(), B, S, heads, kv_heads, o.data_ptr(), lse.data_ptr<float>(),
-                                    cur_stream());
-    return std::make_tuple(o, lse);
+  m.def("causal_gqa_attention_fwd", [](at::Tensor qkv, at::Tensor bounds, int heads, int kv_heads, c10::optional<at::Tensor> o_out,
+                                              c10::optional<at::Tensor> lse_out) {
+    return gqa_fwd(&launch_causal_gqa_attention_fwd, 64, "causal_gqa_attention_fwd", qkv, bounds, heads, kv_heads, o_out, lse_out);
   }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
-  m.def("causal_gqa_attention_bwd", [gqa_check](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds, int heads,
-                                                int kv_heads, c10::optional<at::Tensor> dqkv_out) {
-    const char* who = "causal_gqa_attention_bwd";
-    const int B = gqa_check(qkv, bounds, heads, kv_heads, who);
-    c10::cuda::CUDAGuard guard(qkv.device());
-    const int S = (int)(qkv.size(0) / B);
-    for (const at::Tensor* t : {&dout, &o}) {
-      check_cuda(*t, "dout / o");
-      TORCH_CHECK(t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->numel() == qkv.size(0) * heads * 64 &&
-                  (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, who, ": dout and o must be 16-byte aligned contiguous bf16 [B*S, heads*64]");
-    }
-    TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S &&
-                (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0, who, ": lse must be 8-byte aligned contiguous fp32 [B, heads, S]");
-    at::Tensor dqkv = dqkv_out.has_value() ? *dqkv_out : at::empty_like(qkv);
-    TORCH_CHECK(dqkv.is_cuda() && dqkv.scalar_type() == at::kBFloat16 && dqkv.is_contiguous() && dqkv.numel() == qkv.numel() &&
-                (reinterpret_cast<uintptr_t>(dqkv.data_ptr()) & 3) == 0, who, ": bad dqkv");
-    at::Tensor dsum = at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-    launch_causal_gqa_attention_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), bounds.data_ptr<int>(), B, S,
-                                    heads, kv_heads, dsum.data_ptr<float>(), dqkv.data_ptr(), cur_stream());
-    return dqkv;
+  m.def("causal_gqa_attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds, int heads,
+                                              int kv_heads, c10::optional<at::Tensor> dqkv_out) {
+    return gqa_bwd(&launch_causal_gqa_attention_bwd, 64, "causal_gqa_attention_bwd", dout, qkv, o, lse, bounds, heads, kv_heads, dqkv_out);
+  }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"),
+     py::arg("dqkv") = py::none());
+  m.def("causal_attention_d128_fwd", [](at::Tensor qkv, at::Tensor bounds, int heads, int kv_heads, c10::optional<at::Tensor> o_out,
+                                               c10::optional<at::Tensor> lse_out) {
+    return gqa_fwd(&launch_causal_attention_d128_fwd, 128, "causal_attention_d128_fwd", qkv, bounds, heads, kv_heads, o_out, lse_out);
+  }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
+  m.def("causal_attention_d128_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds, int heads,
+                                               int kv_heads, c10::optional<at::Tensor> dqkv_out) {
+    return gqa_bwd(&launch_causal_attention_d128_bwd, 128, "causal_attention_d128_bwd", dout, qkv, o, lse, bounds, heads, kv_heads,
+                   dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"),
      py::arg("dqkv") = py::none());
 
   // ---- Llama building blocks: rotary embedding (rotary.cu), RMSNorm (layernorm.cu), SwiGLU (loss.cu) --------------------
-  // y = rope(qkv) (backward: the transpose rotation); qkv bf16 [rows, (heads + 2*kv_heads)*64], positions int32 [rows],
-  // table fp32 [max_pos, 2, 32]
+  // y = rope(qkv) (backward: the transpose rotation); qkv bf16 [rows, (heads + 2*kv_heads)*d] with d = 64 or 128, positions
+  // int32 [rows], table fp32 [max_pos, 2, d/2]
   m.def("rotary", [](at::Tensor x, at::Tensor pos, at::Tensor table, int heads, int kv_heads, bool backward) {
     check_cuda(x, "x"); check_cuda(pos, "position_ids"); check_cuda(table, "cos_sin");
+    TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == 2 &&
+                (table.size(2) == 32 || table.size(2) == 64), "rotary: cos_sin must be contiguous fp32 [max_position, 2, d/2], d = 64 or 128");
+    const int d = (int)table.size(2) * 2;
     TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous() && heads >= 1 && kv_heads >= 1 &&
-                x.size(1) == (int64_t)(heads + 2 * kv_heads) * 64, "rotary: x must be contiguous bf16 [rows, (heads + 2*kv_heads)*64]");
+                x.size(1) == (int64_t)(heads + 2 * kv_heads) * d, "rotary: x must be contiguous bf16 [rows, (heads + 2*kv_heads)*d] for the "
+                "table's head dim d = ", d);
     TORCH_CHECK(pos.scalar_type() == at::kInt && pos.is_contiguous() && pos.numel() == x.size(0), "rotary: position_ids must be int32 [rows]");
-    TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == 2 && table.size(2) == 32,
-                "rotary: cos_sin must be contiguous fp32 [max_position, 2, 32]");
     c10::cuda::CUDAGuard guard(x.device());
     if ((reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) != 0) x = x.clone();
     at::Tensor y = at::empty_like(x);
-    launch_rotary(x.data_ptr(), pos.data_ptr<int>(), table.data_ptr<float>(), (int)table.size(0), (size_t)x.size(0), heads, kv_heads,
+    launch_rotary(x.data_ptr(), pos.data_ptr<int>(), table.data_ptr<float>(), (int)table.size(0), (size_t)x.size(0), heads, kv_heads, d,
                   y.data_ptr(), backward, cur_stream());
     return y;
   }, py::arg("x"), py::arg("position_ids"), py::arg("cos_sin"), py::arg("heads"), py::arg("kv_heads"), py::arg("backward") = false);

@@ -294,6 +294,115 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_param_grad_kernel(const 
   if (threadIdx.x == 0) counters[blockIdx.x] = 0u;
 }
 
+// ---- wide RMSNorm: cols % 8 == 0 and 1024 < cols <= 4096 (1B-class Llama hidden sizes 1536 - 4096) -------------------
+// One 128-thread CTA per row (grid-stride over rows): thread t owns chunks t + 128 c (c < 4) of 8 columns, so the row stays
+// in registers as on the fast path, and the row sums go through shared memory.  dgamma comes from the fast path's column
+// reduction (layernorm_param_grad_kernel), which does not depend on the width.
+constexpr int kRmsWideThreads = 128;
+constexpr int kRmsWideChunks = 4;
+
+// Sum over the CTA of v; red: kRmsWideThreads / 32 floats of shared memory, free again when this returns
+__device__ __forceinline__ float rms_wide_block_sum(float v, float* red) {
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  const float r = (red[0] + red[1]) + (red[2] + red[3]);
+  __syncthreads();
+  return r;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const T* __restrict__ x, const T* __restrict__ gamma, int rows,
+                                                                          int cols, float eps, T* __restrict__ y, float* __restrict__ rstd) {
+  __shared__ float red[kRmsWideThreads / 32];
+  const int nchunk = cols >> 3;
+  float g[kRmsWideChunks][8];
+#pragma unroll
+  for (int c = 0; c < kRmsWideChunks; ++c) {
+    const int ch = threadIdx.x + kRmsWideThreads * c;
+    if (ch < nchunk) ln_load8<T>(gamma + 8 * ch, g[c]);
+  }
+  const float inv = 1.f / (float)cols;
+  for (int row = blockIdx.x; row < rows; row += gridDim.x) {
+    const T* xr = x + (size_t)row * cols;
+    float v[kRmsWideChunks][8];
+    float q = 0.f;
+#pragma unroll
+    for (int c = 0; c < kRmsWideChunks; ++c) {
+      const int ch = threadIdx.x + kRmsWideThreads * c;
+      if (ch < nchunk) {
+        ln_load8<T>(xr + 8 * ch, v[c]);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) q += v[c][j] * v[c][j];
+      }
+    }
+    const float rs = rsqrtf(rms_wide_block_sum(q, red) * inv + eps);
+    T* yr = y + (size_t)row * cols;
+#pragma unroll
+    for (int c = 0; c < kRmsWideChunks; ++c) {
+      const int ch = threadIdx.x + kRmsWideThreads * c;
+      if (ch < nchunk) {
+        float o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = v[c][j] * rs * g[c][j];
+        ln_store8<T>(yr + 8 * ch, o);
+      }
+    }
+    if (threadIdx.x == 0) rstd[row] = rs;
+  }
+}
+
+// dx = rs * (dy*gamma - xn * mean(dy*gamma*xn)), xn = x * rs
+template <typename T>
+__global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(const T* __restrict__ dy, const T* __restrict__ x,
+                                                                             const T* __restrict__ gamma, const float* __restrict__ rstd,
+                                                                             int rows, int cols, T* __restrict__ dx) {
+  __shared__ float red[kRmsWideThreads / 32];
+  const int nchunk = cols >> 3;
+  float g[kRmsWideChunks][8];
+#pragma unroll
+  for (int c = 0; c < kRmsWideChunks; ++c) {
+    const int ch = threadIdx.x + kRmsWideThreads * c;
+    if (ch < nchunk) ln_load8<T>(gamma + 8 * ch, g[c]);
+  }
+  const float inv = 1.f / (float)cols;
+  for (int row = blockIdx.x; row < rows; row += gridDim.x) {
+    const T* xr = x + (size_t)row * cols;
+    const T* dyr = dy + (size_t)row * cols;
+    const float rs = rstd[row];
+    float xn[kRmsWideChunks][8], d[kRmsWideChunks][8];
+    float s2 = 0.f;
+#pragma unroll
+    for (int c = 0; c < kRmsWideChunks; ++c) {
+      const int ch = threadIdx.x + kRmsWideThreads * c;
+      if (ch < nchunk) {
+        ln_load8<T>(xr + 8 * ch, xn[c]);
+        ln_load8<T>(dyr + 8 * ch, d[c]);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          xn[c][j] *= rs;
+          d[c][j] *= g[c][j];
+          s2 = fmaf(d[c][j], xn[c][j], s2);
+        }
+      }
+    }
+    s2 = rms_wide_block_sum(s2, red) * inv;
+    T* dxr = dx + (size_t)row * cols;
+#pragma unroll
+    for (int c = 0; c < kRmsWideChunks; ++c) {
+      const int ch = threadIdx.x + kRmsWideThreads * c;
+      if (ch < nchunk) {
+        float o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = rs * (d[c][j] - xn[c][j] * s2);
+        ln_store8<T>(dxr + 8 * ch, o);
+      }
+    }
+  }
+}
+
+int rmsnorm_wide_blocks(int rows) { return rows < 16 * kNumSMs ? (rows < 1 ? 1 : rows) : 16 * kNumSMs; }
+
 template <typename T>
 __global__ void layernorm_bwd_finish_kernel(const float* __restrict__ dgamma_partial, const float* __restrict__ dbeta_partial, int parts,
                                             int cols, T* __restrict__ dgamma, T* __restrict__ dbeta) {
@@ -401,15 +510,27 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 
-bool rmsnorm_supported(int cols) { return cols % 8 == 0 && cols >= 8 && cols <= 8 * 32 * kLnChunks; }
+bool rmsnorm_supported(int cols) { return cols % 8 == 0 && cols >= 8 && cols <= 8 * kRmsWideThreads * kRmsWideChunks; }
+static bool rmsnorm_wide(int cols) { return cols > 8 * 32 * kLnChunks; }
 
-// RMSNorm on the LayerNorm fast path (the only path it has): x, y, gamma 32-byte aligned, rstd [rows]
+// RMSNorm on the LayerNorm fast path up to 1024 columns, on the wide kernels above that: x, y, gamma 32-byte aligned,
+// rstd [rows]
 void launch_rmsnorm_fwd(const void* x, const void* gamma, DType dt, int rows, int cols, float eps, void* y, float* rstd,
                         cudaStream_t s) {
   if (!rmsnorm_supported(cols) ||
       ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(gamma)) & 31u) != 0)
-    throw std::runtime_error("rmsnorm_fwd: needs cols % 8 == 0, cols <= 1024 and 32-byte aligned tensors (cols=" +
+    throw std::runtime_error("rmsnorm_fwd: needs cols % 8 == 0, cols <= 4096 and 32-byte aligned tensors (cols=" +
                              std::to_string(cols) + ")");
+  if (rmsnorm_wide(cols)) {
+    if (dt == DType::BF16)
+      rmsnorm_wide_fwd_kernel<__nv_bfloat16><<<rmsnorm_wide_blocks(rows), kRmsWideThreads, 0, s>>>(
+          (const __nv_bfloat16*)x, (const __nv_bfloat16*)gamma, rows, cols, eps, (__nv_bfloat16*)y, rstd);
+    else
+      rmsnorm_wide_fwd_kernel<float><<<rmsnorm_wide_blocks(rows), kRmsWideThreads, 0, s>>>((const float*)x, (const float*)gamma, rows,
+                                                                                          cols, eps, (float*)y, rstd);
+    B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+    return;
+  }
   int blocks = (rows + 7) / 8;
   if (blocks > 8 * kNumSMs) blocks = 8 * kNumSMs;
   if (blocks < 1) blocks = 1;
@@ -428,22 +549,31 @@ void launch_rmsnorm_bwd(const void* dy, const void* x, const void* gamma, const 
   if (!rmsnorm_supported(cols) ||
       ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx) |
         reinterpret_cast<uintptr_t>(gamma)) & 31u) != 0)
-    throw std::runtime_error("rmsnorm_bwd: needs cols % 8 == 0, cols <= 1024 and 32-byte aligned tensors (cols=" +
+    throw std::runtime_error("rmsnorm_bwd: needs cols % 8 == 0, cols <= 4096 and 32-byte aligned tensors (cols=" +
                              std::to_string(cols) + ")");
   const LnBwdGeometry geo = ln_bwd_geometry(rows, cols, partial_rows);
   const int cvb = geo.cvb, ty = geo.ty, gx = geo.gx, gy = geo.gy, blocks = geo.dx_blocks < 1 ? 1 : geo.dx_blocks;
   const size_t psmem = geo.psmem;
   B200_CUDA_CHECK(cudaMemsetAsync(counters, 0, sizeof(unsigned int) * gx, s));
   if (dt == DType::BF16) {
-    layernorm_bwd_dx_kernel<__nv_bfloat16, true><<<blocks, kLnThreads, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
-                                                                             (const __nv_bfloat16*)gamma, nullptr, rstd, rows, cols,
-                                                                             (__nv_bfloat16*)dx);
+    if (rmsnorm_wide(cols))
+      rmsnorm_wide_bwd_dx_kernel<__nv_bfloat16><<<rmsnorm_wide_blocks(rows), kRmsWideThreads, 0, s>>>(
+          (const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, (const __nv_bfloat16*)gamma, rstd, rows, cols, (__nv_bfloat16*)dx);
+    else
+      layernorm_bwd_dx_kernel<__nv_bfloat16, true><<<blocks, kLnThreads, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
+                                                                               (const __nv_bfloat16*)gamma, nullptr, rstd, rows, cols,
+                                                                               (__nv_bfloat16*)dx);
     layernorm_param_grad_kernel<__nv_bfloat16, true><<<dim3(gx, gy), kLnThreads, psmem, s>>>(
         (const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, nullptr, rstd, rows, cols, cvb, ty, partial, counters,
         (__nv_bfloat16*)dgamma, nullptr);
   } else {
-    layernorm_bwd_dx_kernel<float, true><<<blocks, kLnThreads, 0, s>>>((const float*)dy, (const float*)x, (const float*)gamma, nullptr,
-                                                                     rstd, rows, cols, (float*)dx);
+    if (rmsnorm_wide(cols))
+      rmsnorm_wide_bwd_dx_kernel<float><<<rmsnorm_wide_blocks(rows), kRmsWideThreads, 0, s>>>((const float*)dy, (const float*)x,
+                                                                                             (const float*)gamma, rstd, rows, cols,
+                                                                                             (float*)dx);
+    else
+      layernorm_bwd_dx_kernel<float, true><<<blocks, kLnThreads, 0, s>>>((const float*)dy, (const float*)x, (const float*)gamma, nullptr,
+                                                                       rstd, rows, cols, (float*)dx);
     layernorm_param_grad_kernel<float, true><<<dim3(gx, gy), kLnThreads, psmem, s>>>((const float*)dy, (const float*)x, nullptr, rstd,
                                                                                    rows, cols, cvb, ty, partial, counters,
                                                                                    (float*)dgamma, nullptr);

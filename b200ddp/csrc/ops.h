@@ -71,10 +71,11 @@ void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n,
 void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s);
 
 // ---------------- rotary position embedding (rotary.cu) ----------------------------------------------
-// qkv bf16 [rows, (heads + 2*kv_heads)*64] -> y (same shape): query and key heads rotated by position pos[r] (int32,
-// clamped to [0, max_pos)), value heads copied; table fp32 [max_pos, 2, 32] (cos | sin).  backward: the transpose rotation.
-void launch_rotary(const void* x, const int* pos, const float* table, int max_pos, size_t rows, int heads, int kv_heads, void* y,
-                   bool backward, cudaStream_t s);
+// qkv bf16 [rows, (heads + 2*kv_heads)*head_dim] -> y (same shape), head_dim 64 or 128: query and key heads rotated by
+// position pos[r] (int32, clamped to [0, max_pos)), value heads copied; table fp32 [max_pos, 2, head_dim / 2] (cos | sin).
+// backward: the transpose rotation.
+void launch_rotary(const void* x, const int* pos, const float* table, int max_pos, size_t rows, int heads, int kv_heads, int head_dim,
+                   void* y, bool backward, cudaStream_t s);
 
 // ---------------- layer norm (layernorm.cu) -----------------------------------------------------
 void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, DType dt, int rows, int cols,
@@ -83,8 +84,9 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
                           DType dt, int rows, int cols, void* dx, float* dgamma_partial, float* dbeta_partial,
                           int partial_rows, void* dgamma, void* dbeta, cudaStream_t s);
 int layernorm_partial_rows(int rows);
-// RMSNorm, y = x * rsqrt(mean(x^2) + eps) * gamma, on the LayerNorm fast path: cols % 8 == 0, cols <= 1024, 32-byte
-// aligned tensors.  rstd fp32 [rows]; backward workspace partial fp32 [2 * partial_rows, cols], counters uint32 [cols / 8].
+// RMSNorm, y = x * rsqrt(mean(x^2) + eps) * gamma, on the LayerNorm fast path up to 1024 columns and on one CTA per row
+// above that: cols % 8 == 0, cols <= 4096, 32-byte aligned tensors.  rstd fp32 [rows]; backward workspace partial fp32
+// [2 * partial_rows, cols], counters uint32 [cols / 8].
 bool rmsnorm_supported(int cols);
 void launch_rmsnorm_fwd(const void* x, const void* gamma, DType dt, int rows, int cols, float eps, void* y, float* rstd, cudaStream_t s);
 void launch_rmsnorm_bwd(const void* dy, const void* x, const void* gamma, const float* rstd, DType dt, int rows, int cols, void* dx,
@@ -125,6 +127,12 @@ void launch_causal_gqa_attention_fwd(const void* qkv, const int* bounds, int B, 
                                      cudaStream_t s);
 void launch_causal_gqa_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
                                      int S, int heads, int kv_heads, float* dsum, void* dqkv, cudaStream_t s);
+// The same causal documents at head dim 128: qkv (and dqkv) bf16 [B*S, (heads + 2*kv_heads)*128], o and dout
+// [B*S, heads*128]; kv_heads divides heads (kv_heads == heads is multi-head attention).
+void launch_causal_attention_d128_fwd(const void* qkv, const int* bounds, int B, int S, int heads, int kv_heads, void* o, float* lse,
+                                      cudaStream_t s);
+void launch_causal_attention_d128_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds, int B,
+                                      int S, int heads, int kv_heads, float* dsum, void* dqkv, cudaStream_t s);
 
 // ---------------- small linears on CUDA cores (linear_small.cu) ------------------------------
 // y[M,N] = act(x[M,K] w[N,K]^T + b[N]) ; fp32, dims far below one tensor-core tile (FooModel).

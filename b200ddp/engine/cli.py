@@ -65,16 +65,17 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--cuda_graph", action="store_true", help="capture the whole optimizer step in a CUDA graph")
     p.add_argument("--fp8", action="store_true",
                    help="BERT encoder / GPT-2 / SmolLM block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs "
-                        "--model bert-base, gpt2 or smollm-135m, --fp16 and a GPU")
+                        "--model bert-base, gpt2, smollm-135m or qwen2.5-1.5b, --fp16 and a GPU")
     p.add_argument("--min_seq_len", type=int, default=None,
-                   help="BERT / GPT-2 / SmolLM on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
+                   help="BERT / GPT-2 / SmolLM / Qwen2.5 on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
                         "keys are hidden from attention (native key-padding or causal kernel on the GPU; needs --fp16 and "
                         "--seq_len %% 128 == 0 there).  Default: fixed-length rows")
     p.add_argument("--pack", action="store_true",
-                   help="BERT / GPT-2 / SmolLM on packed documents: documents with lengths uniform in [--min_seq_len, "
-                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2) or <s> (SmolLM), packed first-fit decreasing into rows; "
+                   help="BERT / GPT-2 / SmolLM / Qwen2.5 on packed documents: documents with lengths uniform in [--min_seq_len, "
+                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2, Qwen2.5) or <s> (SmolLM), packed "
+                        "first-fit decreasing into rows; "
                         "attention stays inside a document (native document-boundary or causal kernel on the GPU).  Needs "
-                        "--model bert-base, gpt2 or smollm-135m and --min_seq_len < --seq_len")
+                        "--model bert-base, gpt2, smollm-135m or qwen2.5-1.5b and --min_seq_len < --seq_len")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -141,11 +142,12 @@ def setup(args):
 
 
 # models whose token rows can be right-padded or packed, and whose block linears can run on FP8
-TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m")
+TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m", "qwen2.5-1.5b")
 # causal LMs: their packed documents start with a BOS id
-CAUSAL_MODELS = ("gpt2", "smollm-135m")
+CAUSAL_MODELS = ("gpt2", "smollm-135m", "qwen2.5-1.5b")
 GPT2_MAX_SEQ_LEN = 1024
 SMOLLM_MAX_SEQ_LEN = 2048
+QWEN_MAX_SEQ_LEN = 32768
 
 
 def check_gpt_args(args) -> None:
@@ -156,6 +158,9 @@ def check_gpt_args(args) -> None:
     if args.model == "smollm-135m" and args.seq_len > SMOLLM_MAX_SEQ_LEN:
         raise ValueError(f"--model smollm-135m has {SMOLLM_MAX_SEQ_LEN} positions; --seq_len must be at most "
                          f"{SMOLLM_MAX_SEQ_LEN} (got {args.seq_len})")
+    if args.model == "qwen2.5-1.5b" and args.seq_len > QWEN_MAX_SEQ_LEN:
+        raise ValueError(f"--model qwen2.5-1.5b has {QWEN_MAX_SEQ_LEN} positions; --seq_len must be at most "
+                         f"{QWEN_MAX_SEQ_LEN} (got {args.seq_len})")
 
 
 def check_fp8_args(args) -> None:
@@ -163,8 +168,8 @@ def check_fp8_args(args) -> None:
     if not getattr(args, "fp8", False):
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--fp8 covers the block linears of the token models; it needs --model bert-base, gpt2 or "
-                         f"smollm-135m (got --model {args.model})")
+        raise ValueError(f"--fp8 covers the block linears of the token models; it needs --model bert-base, gpt2, "
+                         f"smollm-135m or qwen2.5-1.5b (got --model {args.model})")
     if not args.fp16:
         raise ValueError("--fp8 needs --fp16: the FP8 GEMMs read bf16 activations and weights")
     if getattr(args, "device", None) is None or args.device.type != "cuda":
@@ -235,6 +240,8 @@ def main(argv=None) -> int:
             kwargs["bos_token_id"] = SyntheticTokens.BOS_ID
         elif args.pack and args.model == "smollm-135m":
             kwargs["bos_token_id"] = SyntheticTokens.LLAMA_BOS_ID
+        elif args.pack and args.model == "qwen2.5-1.5b":
+            kwargs["bos_token_id"] = SyntheticTokens.QWEN_BOS_ID
         elif args.pack:
             kwargs["cls_token_id"] = SyntheticTokens.CLS_ID
     model = build_model(args.model, **kwargs)

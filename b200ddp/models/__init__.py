@@ -3,7 +3,7 @@ from .foo import FooModel, BranchyFooModel
 from .resnet import ResNet, resnet50, resnet152
 from .bert import BertConfig, BertModel, BertForMaskedLM, bert_base
 from .gpt import GPTConfig, GPTModel, GPTLMHeadModel, gpt2
-from .llama import LlamaConfig, LlamaModel, LlamaForCausalLM, smollm_135m
+from .llama import LlamaConfig, LlamaModel, LlamaForCausalLM, smollm_135m, qwen2_5_1_5b
 
 MODEL_REGISTRY = {
     "foo": FooModel,
@@ -12,6 +12,7 @@ MODEL_REGISTRY = {
     "bert-base": bert_base,
     "gpt2": gpt2,
     "smollm-135m": smollm_135m,
+    "qwen2.5-1.5b": qwen2_5_1_5b,
 }
 
 
@@ -23,4 +24,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "MODEL_REGISTRY", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "MODEL_REGISTRY", "build_model"]

@@ -289,6 +289,7 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
 # ------------------------------------------------------------------------------------------------
 ATTENTION_HEAD_DIM = 64
 ATTENTION_SEQ_MULTIPLE = 128
+CAUSAL_WIDE_HEAD_DIM = 128      # the causal kernels also run at this head dim (grouped-query or multi-head)
 
 
 def _key_mask(seq_lens: torch.Tensor, S: int, device) -> torch.Tensor:
@@ -483,12 +484,12 @@ def _repeat_kv(qkv: torch.Tensor, heads: int, kv_heads: int) -> torch.Tensor:
     return torch.cat([q, k, v], -1)
 
 
-def _gqa_check(qkv: torch.Tensor, heads: int, kv_heads: int) -> None:
+def _gqa_check(qkv: torch.Tensor, heads: int, kv_heads: int, head_dim: int = ATTENTION_HEAD_DIM) -> None:
     if heads < 1 or kv_heads < 1 or heads % kv_heads:
         raise ValueError(f"grouped-query attention needs kv_heads dividing heads, got heads={heads}, kv_heads={kv_heads}")
-    if qkv.dim() != 3 or qkv.shape[-1] != (heads + 2 * kv_heads) * ATTENTION_HEAD_DIM:
-        raise ValueError(f"grouped-query attention on CUDA needs qkv [B, S, (heads + 2 * kv_heads) * {ATTENTION_HEAD_DIM}] = "
-                         f"[B, S, {(heads + 2 * kv_heads) * ATTENTION_HEAD_DIM}], got {tuple(qkv.shape)}")
+    if qkv.dim() != 3 or qkv.shape[-1] != (heads + 2 * kv_heads) * head_dim:
+        raise ValueError(f"grouped-query attention on CUDA needs qkv [B, S, (heads + 2 * kv_heads) * {head_dim}] = "
+                         f"[B, S, {(heads + 2 * kv_heads) * head_dim}], got {tuple(qkv.shape)}")
     if qkv.dtype != torch.bfloat16:
         raise ValueError(f"attention on CUDA needs bf16 qkv, got {qkv.dtype}")
     S = qkv.shape[1]
@@ -499,18 +500,21 @@ def _gqa_check(qkv: torch.Tensor, heads: int, kv_heads: int) -> None:
 
 
 class _GqaAttention(torch.autograd.Function):
-    """Grouped-query causal-document attention.  CUDA body: the sm_90a GQA kernels (dK / dV accumulate across each group
-    in registers: one writer per element, deterministic).  CPU body: ``causal_attention_reference`` with K / V repeated."""
+    """Grouped-query causal-document attention.  CUDA body: the sm_90a GQA kernels of the head dim, 64 or 128 (dK / dV
+    accumulate across each group in registers: one writer per element, deterministic).  CPU body:
+    ``causal_attention_reference`` with K / V repeated."""
 
     @staticmethod
     def forward(ctx, qkv, bounds, heads, kv_heads):
         ctx.heads, ctx.kv_heads = heads, kv_heads
         if qkv.is_cuda:
             B, S, Wd = qkv.shape
+            d = Wd // (heads + 2 * kv_heads)
             m = bounds.to(device=qkv.device, dtype=torch.int32).contiguous()
-            o, lse = _C().causal_gqa_attention_fwd(qkv.view(B * S, Wd), m, heads, kv_heads)
+            fwd = _C().causal_attention_d128_fwd if d == CAUSAL_WIDE_HEAD_DIM else _C().causal_gqa_attention_fwd
+            o, lse = fwd(qkv.view(B * S, Wd), m, heads, kv_heads)
             ctx.save_for_backward(qkv, o, lse, m)
-            return o.view(B, S, heads * ATTENTION_HEAD_DIM)
+            return o.view(B, S, heads * d)
         ctx.save_for_backward(qkv, bounds)
         return causal_attention_reference(qkv, bounds, heads, kv_heads)
 
@@ -522,7 +526,9 @@ class _GqaAttention(torch.autograd.Function):
             do = dy.reshape(B * S, -1).to(torch.bfloat16).contiguous()
             if do.data_ptr() % 16:
                 do = do.clone()
-            dqkv = _C().causal_gqa_attention_bwd(do, qkv.view(B * S, Wd), o, lse, m, ctx.heads, ctx.kv_heads)
+            wide = o.shape[-1] == ctx.heads * CAUSAL_WIDE_HEAD_DIM
+            bwd = _C().causal_attention_d128_bwd if wide else _C().causal_gqa_attention_bwd
+            dqkv = bwd(do, qkv.view(B * S, Wd), o, lse, m, ctx.heads, ctx.kv_heads)
             return dqkv.view(B, S, Wd), None, None, None
         qkv, bounds = ctx.saved_tensors
         with torch.enable_grad():
@@ -540,7 +546,15 @@ def causal_attention(qkv: torch.Tensor, bounds: torch.Tensor, heads: int, kv_hea
 
     ``kv_heads`` other than None or ``heads`` selects grouped-query attention: qkv is [B, S, (heads + 2 * kv_heads) * 64]
     (query | key | value column blocks) and query head h reads K/V head h // (heads // kv_heads); the output stays
-    [B, S, heads * 64]."""
+    [B, S, heads * 64].
+
+    Head dim 128 (qkv [B, S, (heads + 2 * kv_heads) * 128], kv_heads None meaning ``heads``) runs on CUDA on the head-dim-128
+    kernels, with the same layouts, masks and checks; the output is [B, S, heads * 128]."""
+    kv = heads if kv_heads is None else kv_heads
+    if qkv.is_cuda and heads >= 1 and kv >= 1 and qkv.dim() == 3 and qkv.shape[-1] == (heads + 2 * kv) * CAUSAL_WIDE_HEAD_DIM:
+        _gqa_check(qkv, heads, kv, CAUSAL_WIDE_HEAD_DIM)
+        _bounds_check(qkv, bounds, "causal attention")
+        return _GqaAttention.apply(qkv, bounds, heads, kv)
     if kv_heads is not None and kv_heads != heads:
         if qkv.is_cuda:
             _gqa_check(qkv, heads, kv_heads)
@@ -610,7 +624,7 @@ def rotary(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor,
     """Rotary position embedding (Hugging Face's ``rotate_half`` convention: element i of a head pairs with i + d/2) of
     the query and key heads of qkv [B, S, (heads + 2 * kv_heads) * d]; the value heads pass through.  position_ids
     integer [B, S] (clamped to the table), cos_sin fp32 [max_position, 2, d / 2] (``rotary_cos_sin``).  Out of place.  On
-    CUDA: bf16 and d = 64, else ``ValueError``; positions stay on the device (CUDA-graph safe)."""
+    CUDA: bf16 and d = 64 or 128, else ``ValueError``; positions stay on the device (CUDA-graph safe)."""
     if qkv.dim() != 3 or heads < 1 or kv_heads < 1 or qkv.shape[-1] % (heads + 2 * kv_heads) or \
             (qkv.shape[-1] // (heads + 2 * kv_heads)) % 2:
         raise ValueError(f"rotary needs qkv [B, S, (heads + 2 * kv_heads) * d] with an even d, got {tuple(qkv.shape)} for "
@@ -620,8 +634,9 @@ def rotary(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor,
         raise ValueError(f"rotary needs integer position_ids {tuple(qkv.shape[:2])}, got {position_ids.dtype} {tuple(position_ids.shape)}")
     if cos_sin.dim() != 3 or tuple(cos_sin.shape[1:]) != (2, d // 2) or cos_sin.shape[0] < 1:
         raise ValueError(f"rotary needs cos_sin [max_position, 2, {d // 2}], got {tuple(cos_sin.shape)}")
-    if qkv.is_cuda and (qkv.dtype != torch.bfloat16 or d != ATTENTION_HEAD_DIM):
-        raise ValueError(f"rotary on CUDA needs bf16 qkv and head dim {ATTENTION_HEAD_DIM}, got {qkv.dtype}, head dim {d}")
+    if qkv.is_cuda and (qkv.dtype != torch.bfloat16 or d not in (ATTENTION_HEAD_DIM, CAUSAL_WIDE_HEAD_DIM)):
+        raise ValueError(f"rotary on CUDA needs bf16 qkv and head dim {ATTENTION_HEAD_DIM} or {CAUSAL_WIDE_HEAD_DIM}, got {qkv.dtype}, "
+                         f"head dim {d}")
     return _Rotary.apply(qkv, position_ids, cos_sin, heads, kv_heads)
 
 
@@ -647,14 +662,14 @@ class _RMSNormFused(torch.autograd.Function):
 
 def rms_norm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
     """y = x * rsqrt(mean(x^2) + eps) * weight over the last dimension (statistics in fp32).  On CUDA: the LayerNorm
-    fast-path kernels (hidden % 8 == 0, hidden <= 1024, bf16 or fp32 with weight of the same dtype), else ``ValueError``;
-    the weight gradient is a deterministic column reduction."""
+    fast-path kernels up to hidden 1024 and the wide RMSNorm kernels up to 4096 (hidden % 8 == 0, bf16 or fp32 with weight
+    of the same dtype), else ``ValueError``; the weight gradient is a deterministic column reduction."""
     if x.dim() < 1 or weight.dim() != 1 or weight.shape[0] != x.shape[-1]:
         raise ValueError(f"rms_norm needs x [..., hidden] and weight [hidden], got {tuple(x.shape)} and {tuple(weight.shape)}")
     if x.is_cuda:
         n = x.shape[-1]
-        if x.dtype not in (torch.float32, torch.bfloat16) or weight.dtype != x.dtype or n % 8 or n > 1024:
-            raise ValueError(f"rms_norm on CUDA needs bf16 or fp32 x and weight of one dtype and hidden % 8 == 0, <= 1024; got "
+        if x.dtype not in (torch.float32, torch.bfloat16) or weight.dtype != x.dtype or n % 8 or n > 4096:
+            raise ValueError(f"rms_norm on CUDA needs bf16 or fp32 x and weight of one dtype and hidden % 8 == 0, <= 4096; got "
                              f"{x.dtype} x {weight.dtype}, hidden {n}")
         if weight.device != x.device:
             raise ValueError(f"rms_norm needs the weight on x's device ({x.device}), got {weight.device}")
