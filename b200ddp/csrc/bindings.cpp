@@ -415,6 +415,92 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                         dlogits.data_ptr(), cur_stream());
     return std::make_tuple(loss, dlogits);
   });
+  // Fused LM-head cross-entropy: mean over non-ignored rows of cross_entropy(hidden [N,H] . weight [V,H]^T + bias [V]) without
+  // the [N, V] logits.  Forward -> (loss fp32 [], lse fp32 [N], row_loss fp32 [N+1], row_loss[N] = non-ignored rows).
+  auto lm_check = [](const at::Tensor& hidden, const at::Tensor& weight, const at::Tensor& targets, const c10::optional<at::Tensor>& bias) {
+    check_cuda(hidden, "hidden"); check_cuda(weight, "weight"); check_cuda(targets, "targets");
+    TORCH_CHECK(hidden.scalar_type() == at::kBFloat16 && weight.scalar_type() == at::kBFloat16 && hidden.dim() == 2 && weight.dim() == 2 &&
+                hidden.is_contiguous() && weight.is_contiguous() && hidden.size(1) == weight.size(1),
+                "lm_loss: hidden [N,H] and weight [V,H], bf16 contiguous");
+    TORCH_CHECK(hidden.size(1) % 8 == 0 && weight.size(0) % 8 == 0, "lm_loss: H and V must be multiples of 8 (16-byte rows), got H=",
+                hidden.size(1), ", V=", weight.size(0));
+    TORCH_CHECK(hidden.size(0) >= 1, "lm_loss: no rows");
+    TORCH_CHECK(targets.scalar_type() == at::kLong && targets.is_contiguous() && targets.numel() == hidden.size(0), "lm_loss: targets int64 [N]");
+    if (bias.has_value())
+      TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->is_contiguous() && bias->numel() == weight.size(0), "lm_loss: bias bf16 [V]");
+  };
+  auto lm_out = [](const c10::optional<at::Tensor>& given, at::IntArrayRef sizes, const at::TensorOptions& opt, const char* name) {
+    if (!given.has_value()) return at::empty(sizes, opt);
+    TORCH_CHECK(given->is_contiguous() && given->sizes() == sizes && given->scalar_type() == opt.dtype().toScalarType(),
+                "lm_loss: bad ", name, " output");
+    return *given;
+  };
+  m.def("lm_loss_fwd", [lm_check, lm_out](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
+                                          long long ignore_index, c10::optional<at::Tensor> lse_out, c10::optional<at::Tensor> row_loss_out) {
+    lm_check(hidden, weight, targets, bias);
+    c10::cuda::CUDAGuard guard(hidden.device());
+    const int N = (int)hidden.size(0), H = (int)hidden.size(1), V = (int)weight.size(0), tiles = (V + 127) / 128;
+    const auto f32 = hidden.options().dtype(at::kFloat);
+    at::Tensor loss = at::empty({}, f32);
+    at::Tensor lse = lm_out(lse_out, {N}, f32, "lse");
+    at::Tensor row_loss = lm_out(row_loss_out, {N + 1}, f32, "row_loss");
+    at::Tensor partial = at::empty({tiles, N, 2}, f32);
+    at::Tensor target_logit = at::empty({N}, f32);
+    const auto* t = (const long long*)targets.data_ptr<int64_t>();
+    launch_gemm_lm_lse(hidden.data_ptr(), weight.data_ptr(), bias.has_value() ? bias->data_ptr() : nullptr, N, V, H, t,
+                       partial.data_ptr<float>(), target_logit.data_ptr<float>(), cur_stream());
+    launch_lm_loss_combine(partial.data_ptr<float>(), target_logit.data_ptr<float>(), t, N, tiles, V, ignore_index, lse.data_ptr<float>(),
+                           row_loss.data_ptr<float>(), loss.data_ptr<float>(), cur_stream());
+    return std::make_tuple(loss, lse, row_loss);
+  }, py::arg("hidden"), py::arg("weight"), py::arg("targets"), py::arg("bias") = py::none(), py::arg("ignore_index") = -100,
+     py::arg("lse_out") = py::none(), py::arg("row_loss_out") = py::none());
+  // Backward, `slice` vocabulary columns at a time: recompute the slice's logits into its bf16 gradient (one GEMM), then
+  // dh += dlogits . weight[slice] (fp32, cast to bf16 once at the end) and dweight[slice] = dlogits^T . hidden.  gscale:
+  // fp32 device scalar (the upstream gradient).  Returns (dh bf16 [N,H] or None, dweight bf16 [V,H] or None).
+  m.def("lm_loss_bwd", [lm_check, lm_out](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
+                                          at::Tensor lse, at::Tensor row_loss, at::Tensor gscale, long long ignore_index, int slice,
+                                          bool need_dh, bool need_dweight, c10::optional<at::Tensor> dh_out,
+                                          c10::optional<at::Tensor> dweight_out) {
+    lm_check(hidden, weight, targets, bias);
+    const int N = (int)hidden.size(0), H = (int)hidden.size(1), V = (int)weight.size(0);
+    TORCH_CHECK(slice >= 128 && slice % 128 == 0, "lm_loss_bwd: slice must be a positive multiple of 128, got ", slice);
+    for (const at::Tensor* t : {&lse, &row_loss, &gscale}) {
+      check_cuda(*t, "lse / row_loss / gscale");
+      TORCH_CHECK(t->scalar_type() == at::kFloat && t->is_contiguous(), "lm_loss_bwd: lse, row_loss and gscale are contiguous fp32");
+    }
+    TORCH_CHECK(lse.numel() == N && row_loss.numel() == N + 1 && gscale.numel() == 1, "lm_loss_bwd: lse [N], row_loss [N+1], gscale [1]");
+    c10::cuda::CUDAGuard guard(hidden.device());
+    const auto bf16 = hidden.options();
+    at::Tensor dh, dweight, dh32;
+    if (need_dh) {
+      dh = lm_out(dh_out, {N, H}, bf16, "dh");
+      dh32 = at::empty({N, H}, bf16.dtype(at::kFloat));
+    }
+    if (need_dweight) dweight = lm_out(dweight_out, {V, H}, bf16, "dweight");
+    if (!need_dh && !need_dweight) return std::make_tuple(dh, dweight);
+    const int width = slice < V ? slice : V;
+    at::Tensor dlogits = at::empty({(int64_t)N * width}, bf16);
+    const auto* t = (const long long*)targets.data_ptr<int64_t>();
+    const auto* w = reinterpret_cast<const __nv_bfloat16*>(weight.data_ptr());
+    const auto* b = bias.has_value() ? reinterpret_cast<const __nv_bfloat16*>(bias->data_ptr()) : nullptr;
+    for (int v0 = 0; v0 < V; v0 += width) {
+      const int vs = V - v0 < width ? V - v0 : width;
+      launch_gemm_lm_dlogits(hidden.data_ptr(), w + (size_t)v0 * H, b ? b + v0 : nullptr, N, vs, H, v0, V, t, ignore_index,
+                             lse.data_ptr<float>(), gscale.data_ptr<float>(), row_loss.data_ptr<float>() + N, dlogits.data_ptr(), cur_stream());
+      // dh [N,H] (+)= dlogits [N,vs] . weight[v0:v0+vs] (stored [vs,H]: MN-major B)
+      if (need_dh)
+        launch_gemm_bf16(dlogits.data_ptr(), w + (size_t)v0 * H, dh32.data_ptr(), nullptr, N, H, vs, false, true, 0, DType::F32, v0 > 0,
+                         cur_stream());
+      // dweight[v0:v0+vs] [vs,H] = dlogits^T (stored [N,vs]: MN-major A) . hidden (stored [N,H]: MN-major B)
+      if (need_dweight)
+        launch_gemm_bf16(dlogits.data_ptr(), hidden.data_ptr(), reinterpret_cast<__nv_bfloat16*>(dweight.data_ptr()) + (size_t)v0 * H,
+                         nullptr, vs, H, N, true, true, 0, DType::BF16, false, cur_stream());
+    }
+    if (need_dh) dh.copy_(dh32);
+    return std::make_tuple(dh, dweight);
+  }, py::arg("hidden"), py::arg("weight"), py::arg("targets"), py::arg("bias"), py::arg("lse"), py::arg("row_loss"), py::arg("gscale"),
+     py::arg("ignore_index"), py::arg("slice"), py::arg("need_dh") = true, py::arg("need_dweight") = true, py::arg("dh_out") = py::none(),
+     py::arg("dweight_out") = py::none());
 
   // tanh = false: the erf form; true: the tanh approximation
   m.def("gelu_fwd", [](at::Tensor pre, bool tanh) {

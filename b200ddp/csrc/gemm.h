@@ -27,6 +27,18 @@ bool gemm_shape_supported(int M, int N, int K, bool a_mn, bool b_mn);
 void launch_gemm_fp8(const void* a, const void* b, void* d, const void* bias, const float* a_scale_inv, const float* b_scale_inv,
                      int M, int N, int K, bool a_e5m2, int epilogue, cudaStream_t stream);
 
+// Fused LM-head cross-entropy GEMMs: logits x = bf16(hidden[M,K] . weight[V,K]^T + bias) on 128 x 128 tiles, never stored.
+// LSE: partial fp32 [ceil(V/128)][M][2] gets each row's (max, sum exp(x - max)) per 128-column tile; target_logit [M] gets
+// x[row, targets[row]] for targets in [0, V) (other rows are not written).  K % 8 == 0.
+void launch_gemm_lm_lse(const void* hidden, const void* weight, const void* bias, int M, int V, int K, const long long* targets,
+                        float* partial, float* target_logit, cudaStream_t stream);
+// Logit gradient of vocabulary columns [col_offset, col_offset + N): weight and bias point at that slice's first row.
+// dlogits bf16 [M, N] = (exp(x - lse[row]) - [col == target]) * gscale / valid, zero for rows whose target is ignore_index
+// or outside [0, vocab); gscale and valid are fp32 device scalars (valid <= 0 gives zeros).
+void launch_gemm_lm_dlogits(const void* hidden, const void* weight, const void* bias, int M, int N, int K, int col_offset, int vocab,
+                            const long long* targets, long long ignore_index, const float* lse, const float* gscale,
+                            const float* valid, void* dlogits, cudaStream_t stream);
+
 // Persistent-tile rasterisation shared by the producer, issuer and epilogue roles (and mirrored on the host for
 // tests).  group_m <= 0: m-fastest over the whole problem (default).  group_m > 0: bands of `group_m` m-tiles
 // are swept n-major, so the ~132 tiles in flight form a near-square patch and both operands are reused out of L2.

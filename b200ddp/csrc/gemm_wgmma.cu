@@ -55,7 +55,20 @@ struct GemmParams {
   const __nv_bfloat16* bias;
   const float* scale_a;   // FP8 only: device scalars 1/s_a, 1/s_b (dequantisation factors)
   const float* scale_b;
+  // fused LM-head cross-entropy (LM != kLmNone).  Appended after the fields above so that their offsets stay as they
+  // were, and kept to 56 bytes: at 128 bytes or less the struct's parameter loads, and the code of every other variant,
+  // compile as before.  kLmLse writes its (max, sum exp) partials to `d` (it stores no output tile).
+  const long long* lm_targets;   // [M] target column of each row (global vocabulary index)
+  float* lm_target_logit;        // kLmLse: [M] the row's target logit, written by the one tile that holds it
+  const float* lm_lse;           // kLmDlogits: [M] row log-sum-exp
+  const float* lm_gscale;        // kLmDlogits: device scalars, upstream gradient and number of non-ignored rows
+  const float* lm_valid;
+  int lm_ignore_index;           // kLmDlogits: ignore_index if it lies in [0, lm_vocab), else -1 (already ignored as out of range)
+  int lm_col_offset;             // kLmDlogits: global vocabulary index of this GEMM's column 0
+  int lm_vocab;                  // full vocabulary: targets outside [0, lm_vocab) are ignored
 };
+
+constexpr int kLmNone = 0, kLmLse = 1, kLmDlogits = 2;
 
 // bias / activation on 32 consecutive accumulator columns starting at `col0`
 __device__ __forceinline__ void epilogue_math(const GemmParams& p, int col0, const uint32_t* r, float* v) {
@@ -150,6 +163,86 @@ __device__ __forceinline__ void store_row_chunk(const GemmParams& p, int row, in
   }
 }
 
+// ---- fused LM-head cross-entropy epilogues (128-column tiles, one thread per row) -----------------------------
+// The logits are never stored.  Each value is biased and rounded to bf16 first, exactly as the unfused head GEMM
+// stores it, so both paths see the same logits.  The target column is found by comparing every column index with it
+// (a select per column: no dynamic register indexing).
+//   kLmLse     : (max, sum exp(x - max)) of the row over the tile -> d as float2 [ceil(N / 128)][M], the target logit ->
+//                lm_target_logit.
+//   kLmDlogits : d = (exp(x - lse) - [col == target]) * g / valid in bf16 -> D; ignored rows get zeros.
+template <int LM>
+__device__ __forceinline__ void lm_epilogue_tile(const GemmParams& p, const float* arow, int row, int n0) {
+  const bool live = row < p.M;
+  const long long t = live ? __ldg(p.lm_targets + row) : -1;
+  if constexpr (LM == kLmLse) {
+    const int tcol = (t >= n0 && t < n0 + 128 && t < p.N) ? (int)(t - n0) : -1;
+    float m = -INFINITY, s = 0.f, tl = 0.f;
+#pragma unroll 1
+    for (int c = 0; c < 128; c += 32) {
+      if (n0 + c >= p.N) break;                          // warp-uniform
+      uint32_t r[32];
+      float v[32];
+      acc_row_ld32(arow, 0, 0, c, r);
+      epilogue_math(p, n0 + c, r, v);
+      float cm = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const float x = n0 + c + i < p.N ? __bfloat162float(__float2bfloat16_rn(v[i])) : -INFINITY;
+        if (tcol == c + i) tl = x;
+        v[i] = x;
+        cm = fmaxf(cm, x);
+      }
+      const float nm = fmaxf(m, cm);
+      float cs = 0.f;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) cs += __expf(v[i] - nm);
+      s = s * __expf(m - nm) + cs;                       // first chunk: m = -inf, s = 0
+      m = nm;
+    }
+    if (live) {
+      reinterpret_cast<float2*>(p.d)[(size_t)(n0 / 128) * p.M + row] = make_float2(m, s);
+      if (tcol >= 0) p.lm_target_logit[row] = tl;
+    }
+  } else {
+    const bool ignored = t == p.lm_ignore_index || t < 0 || t >= p.lm_vocab;
+    const long long base = (long long)p.lm_col_offset + n0;
+    const int tcol = (!ignored && t >= base && t < base + 128) ? (int)(t - base) : -1;
+    const float valid = __ldg(p.lm_valid);
+    const float coef = (ignored || valid <= 0.f) ? 0.f : __ldg(p.lm_gscale) / valid;
+    const float lse = live ? p.lm_lse[row] : 0.f;
+#pragma unroll 1
+    for (int c = 0; c < 128; c += 32) {
+      if (n0 + c >= p.N) break;                          // warp-uniform
+      uint32_t r[32];
+      float v[32];
+      acc_row_ld32(arow, 0, 0, c, r);
+      epilogue_math(p, n0 + c, r, v);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        float d = __expf(__bfloat162float(__float2bfloat16_rn(v[i])) - lse);
+        if (tcol == c + i) d -= 1.f;
+        v[i] = d * coef;
+      }
+      if (!live) continue;
+      const int col0 = n0 + c;
+      __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(p.d) + (size_t)row * p.N + col0;
+      if (col0 + 32 <= p.N && ((reinterpret_cast<uintptr_t>(out) & 15) == 0)) {
+#pragma unroll
+        for (int i = 0; i < 32; i += 8) {
+          __nv_bfloat162 h[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) h[q] = __floats2bfloat162_rn(v[i + 2 * q], v[i + 2 * q + 1]);
+          *reinterpret_cast<uint4*>(out + i) = *reinterpret_cast<uint4*>(h);
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if (col0 + i < p.N) out[i] = __float2bfloat16_rn(v[i]);
+      }
+    }
+  }
+}
+
 // ---- opt-in epilogue through shared memory + TMA store (bf16 outputs) ---------------------------------------
 // Each epilogue warp owns two 4 KB staging buffers (32 rows x 64 bf16 columns, 128B-swizzled exactly like the
 // operand tiles).  A lane converts its accumulator row, writes eight 16-byte chunks at (chunk ^ (row & 7)) - bank
@@ -216,7 +309,7 @@ struct SmemLayout {
 // pair tile).  Each CTA loads its own A tile and HALF of the B tile, multicast into both CTAs' shared memory, so every B
 // byte leaves L2 once per pair.  A stage may be refilled only when the consumers of BOTH CTAs are done with it: the empty
 // barriers count the arrivals of the local and the peer warpgroup.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS, bool PAIR, int OP = kOpBF16>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS, bool PAIR, int OP = kOpBF16, int LM = kLmNone>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const __grid_constant__ CUtensorMap map_d, const GemmParams p) {
@@ -225,6 +318,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   constexpr bool kFP8 = OP != kOpBF16;
   static_assert(!kFP8 || (!A_MN && !B_MN && !TMA_ST && !STATS && !PAIR && BLOCK_N == 64),
                 "FP8: K-major operands, direct epilogue, 128 x 64 tiles (partial + promoted accumulators fill the registers)");
+  static_assert(sizeof(GemmParams) <= 128, "GemmParams: see the note on the LM-head fields");
+  static_assert(LM == kLmNone || (!kFP8 && !A_MN && !B_MN && !TMA_ST && !STATS && !PAIR && BLOCK_N == 128),
+                "LM-head epilogues: bf16 K-major operands, direct epilogue, single-CTA 128 x 128 tiles");
   constexpr int kBK = kFP8 ? 2 * BLOCK_K : BLOCK_K;            // elements per k-block: one 128-byte row either way
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -356,7 +452,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       wg_bar_sync();
       const int row = m0 + ew * 32 + lane;
       const float* arow = acc_smem + (size_t)(ew * 32 + lane) * L::kAccStride;
-      if constexpr (TMA_ST) {
+      if constexpr (LM != kLmNone) {
+        lm_epilogue_tile<LM>(p, arow, row, n0);
+      } else if constexpr (TMA_ST) {
         epilogue_tile_tma<BLOCK_N, STATS>(p, &map_d, store_stage + ew * 2 * kStoreSlabBytes, arow, m0 + ew * 32, n0, lane, slab);
       } else {
 #pragma unroll 1
@@ -431,7 +529,7 @@ CUtensorMap make_map(const void* ptr, int rows, int cols, int box_rows, int box_
 }
 
 // TMA_ST: epilogue through shared memory + TMA store (bf16 output, N % 8 == 0); the D map's box is one warp slab.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS = false, bool PAIR = false, int OP = kOpBF16>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS = false, bool PAIR = false, int OP = kOpBF16, int LM = kLmNone>
 void launch_variant(const void* a, const void* b, const GemmParams& p, cudaStream_t stream) {
   using L = SmemLayout<BLOCK_N, A_MN, B_MN, TMA_ST>;
   constexpr int kSmem = L::kTotal;
@@ -443,7 +541,7 @@ void launch_variant(const void* a, const void* b, const GemmParams& p, cudaStrea
   CUtensorMap map_a = A_MN ? make_map(a, p.K, p.M, BLOCK_K, 64) : make_map(a, p.M, p.K, BLOCK_M, kBK, kEB);
   CUtensorMap map_b = B_MN ? make_map(b, p.K, p.N, BLOCK_K, 64) : make_map(b, p.N, p.K, PAIR ? BLOCK_N / 2 : BLOCK_N, kBK, kEB);
   CUtensorMap map_d = TMA_ST ? make_map(p.d, p.M, p.N, 32, 64) : map_a;       // unused by the direct epilogue
-  auto kernel = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, TMA_ST, STATS, PAIR, OP>;
+  auto kernel = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, TMA_ST, STATS, PAIR, OP, LM>;
   static std::atomic<unsigned long long> configured{0};
   ensure_max_dynamic_smem(kernel, kSmem, configured);
   if constexpr (PAIR) {
@@ -582,6 +680,40 @@ void launch_gemm_fp8(const void* a, const void* b, void* d, const void* bias, co
   p.group_m = g_gemm_group_m > 0 ? g_gemm_group_m : 0;
   if (a_e5m2) launch_variant<64, false, false, false, false, false, kOpE5M2>(a, b, p, stream);
   else launch_variant<64, false, false, false, false, false, kOpE4M3>(a, b, p, stream);
+}
+
+namespace {
+GemmParams lm_params(int M, int N, int K, const void* bias, const long long* targets) {
+  if (!gemm_shape_supported(M, N, K, false, false)) throw std::runtime_error("gemm_lm: hidden size must be a multiple of 8");
+  GemmParams p = {};
+  p.M = M; p.N = N; p.K = K;
+  p.epilogue = bias != nullptr ? 1 : 0;
+  p.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
+  p.lm_targets = targets;
+  return p;
+}
+}  // namespace
+
+void launch_gemm_lm_lse(const void* hidden, const void* weight, const void* bias, int M, int V, int K, const long long* targets,
+                        float* partial, float* target_logit, cudaStream_t stream) {
+  GemmParams p = lm_params(M, V, K, bias, targets);
+  p.d = partial;
+  p.lm_target_logit = target_logit;
+  launch_variant<128, false, false, false, false, false, kOpBF16, kLmLse>(hidden, weight, p, stream);
+}
+
+void launch_gemm_lm_dlogits(const void* hidden, const void* weight, const void* bias, int M, int N, int K, int col_offset, int vocab,
+                            const long long* targets, long long ignore_index, const float* lse, const float* gscale,
+                            const float* valid, void* dlogits, cudaStream_t stream) {
+  GemmParams p = lm_params(M, N, K, bias, targets);
+  p.d = dlogits;
+  p.lm_lse = lse;
+  p.lm_gscale = gscale;
+  p.lm_valid = valid;
+  p.lm_ignore_index = ignore_index >= 0 && ignore_index < vocab ? (int)ignore_index : -1;
+  p.lm_col_offset = col_offset;
+  p.lm_vocab = vocab;
+  launch_variant<128, false, false, false, false, false, kOpBF16, kLmDlogits>(hidden, weight, p, stream);
 }
 
 }  // namespace b200

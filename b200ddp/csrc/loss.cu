@@ -202,6 +202,38 @@ __global__ void __launch_bounds__(1024) count_valid_kernel(const long long* __re
   if (threadIdx.x == 0) *out = cnt;
 }
 
+// (max, sum exp(x - max)) pairs; an empty pair (-inf, 0) is the identity
+__device__ __forceinline__ float2 lse_merge(float2 a, float2 b) {
+  if (b.x == -INFINITY) return a;
+  if (a.x == -INFINITY) return b;
+  const float m = fmaxf(a.x, b.x);
+  return make_float2(m, a.y * __expf(a.x - m) + b.y * __expf(b.x - m));
+}
+
+// Block = 32 rows x 8 tile groups: thread (x, y) merges tiles y, y + 8, ... of row x in order (a warp reads 32 consecutive
+// rows of one tile: coalesced), then the 8 group results are merged in order.  Deterministic: a fixed order per row.
+constexpr int kCombineGroups = 8;
+__global__ void __launch_bounds__(32 * kCombineGroups) lm_lse_combine_kernel(const float2* __restrict__ partial, const float* __restrict__ target_logit,
+                                                                             const long long* __restrict__ targets, int rows, int tiles, int cols,
+                                                                             long long ignore_index, float* __restrict__ lse,
+                                                                             float* __restrict__ row_loss) {
+  __shared__ float2 part[kCombineGroups][32];
+  const int row = blockIdx.x * 32 + threadIdx.x;
+  float2 acc = make_float2(-INFINITY, 0.f);
+  if (row < rows)
+    for (int i = threadIdx.y; i < tiles; i += kCombineGroups) acc = lse_merge(acc, partial[(size_t)i * rows + row]);
+  part[threadIdx.y][threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.y != 0 || row >= rows) return;
+#pragma unroll
+  for (int g = 1; g < kCombineGroups; ++g) acc = lse_merge(acc, part[g][threadIdx.x]);
+  const float l = acc.x + __logf(acc.y);
+  lse[row] = l;
+  const long long t = targets[row];
+  const bool ignored = (t == ignore_index) || t < 0 || t >= cols;
+  row_loss[row] = ignored ? 0.f : l - target_logit[row];
+}
+
 }  // namespace
 
 int mse_blocks(size_t n) {
@@ -248,6 +280,17 @@ void launch_xent_fwd_bwd(const void* logits, const long long* targets, DType dt,
   else
     xent_fwd_bwd_kernel<float><<<rows, kLossThreads, 0, s>>>((const float*)logits, targets, rows, cols, ignore_index, g, row_loss,
                                                            (float*)dlogits);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  xent_finish_kernel<<<1, 1024, 0, s>>>(row_loss, targets, rows, cols, ignore_index, loss);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void launch_lm_loss_combine(const float* partial, const float* target_logit, const long long* targets, int rows, int tiles, int cols,
+                            long long ignore_index, float* lse, float* row_loss, float* loss, cudaStream_t s) {
+  count_valid_kernel<<<1, 1024, 0, s>>>(targets, rows, cols, ignore_index, row_loss + rows);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  lm_lse_combine_kernel<<<(rows + 31) / 32, dim3(32, kCombineGroups), 0, s>>>(reinterpret_cast<const float2*>(partial), target_logit, targets,
+                                                                             rows, tiles, cols, ignore_index, lse, row_loss);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
   xent_finish_kernel<<<1, 1024, 0, s>>>(row_loss, targets, rows, cols, ignore_index, loss);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);

@@ -61,6 +61,11 @@ int mse_blocks(size_t n);
 void launch_xent_fwd_bwd(const void* logits, const long long* targets, DType dt, int rows, int cols,
                          long long ignore_index, float gscale, float* row_loss /*[rows+1]*/, float* loss /*1*/,
                          void* dlogits, cudaStream_t s);
+// Fused LM-head cross-entropy, after launch_gemm_lm_lse (gemm.h): lse[row] from the per-tile partials fp32
+// [tiles][rows][2] (a fixed-order merge), row_loss [rows+1] (lse - target logit, 0 for ignored rows; row_loss[rows] = the
+// number of non-ignored rows) and loss = their mean (0 when every row is ignored).
+void launch_lm_loss_combine(const float* partial, const float* target_logit, const long long* targets, int rows, int tiles, int cols,
+                            long long ignore_index, float* lse, float* row_loss, float* loss, cudaStream_t s);
 
 // GELU forward: out = gelu(pre); backward: out = dy * gelu'(pre).  One vectorised pass each (loss.cu).  The erf form, or
 // with `tanh` the tanh approximation 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3))) (GPT-2's MLP).

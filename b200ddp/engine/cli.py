@@ -76,6 +76,9 @@ def build_parser() -> argparse.ArgumentParser:
                         "first-fit decreasing into rows; "
                         "attention stays inside a document (native document-boundary or causal kernel on the GPU).  Needs "
                         "--model bert-base, gpt2, smollm-135m or qwen2.5-1.5b and --min_seq_len < --seq_len")
+    p.add_argument("--fused_lm_loss", action="store_true",
+                   help="GPT-2 / SmolLM / Qwen2.5: LM head and cross-entropy in one op that never builds the [tokens, vocab] "
+                        "logits (the head GEMM runs once more in the backward); needs --loss ce, and --fp16 on a GPU")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -135,6 +138,7 @@ def setup(args):
     check_fp8_args(args)
     check_min_seq_len_args(args)
     check_pack_args(args)
+    check_fused_lm_loss_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -207,6 +211,25 @@ def check_pack_args(args) -> None:
     check_min_seq_len_args(args)
 
 
+def check_fused_lm_loss_args(args) -> None:
+    """``--fused_lm_loss`` moves a causal LM's head into a cross-entropy criterion: it needs such a model and ``--loss ce``,
+    bf16 weights on a GPU (the native op is bf16), and a process per GPU (``DataParallel`` would split the hidden states
+    across GPUs and gather them back to one)."""
+    if not getattr(args, "fused_lm_loss", False):
+        return
+    if args.model not in CAUSAL_MODELS:
+        raise ValueError(f"--fused_lm_loss fuses a causal LM's head into its loss; it needs --model gpt2, smollm-135m or "
+                         f"qwen2.5-1.5b (got --model {args.model})")
+    if getattr(args, "loss", None) not in (None, "ce"):
+        raise ValueError(f"--fused_lm_loss computes cross-entropy; it needs --loss ce (got --loss {args.loss})")
+    if getattr(args, "device", None) is not None and args.device.type == "cuda":
+        if not args.fp16:
+            raise ValueError("--fused_lm_loss on a GPU needs --fp16: the fused head reads bf16 hidden states and weights")
+        if args.local_rank == -1 and getattr(args, "n_gpu", 1) > 1:
+            raise ValueError("--fused_lm_loss does not run under single-process multi-GPU DataParallel; launch one process "
+                             "per GPU (torchrun) or make one GPU visible")
+
+
 def padding_on(args) -> bool:
     """Rows are padded (and the model must hide padded keys) when some row can be shorter than --seq_len."""
     n = getattr(args, "min_seq_len", None)
@@ -233,6 +256,8 @@ def main(argv=None) -> int:
     args = build_parser().parse_args(argv)
     setup(args)
     kwargs = {"fp8": True} if args.fp8 else {}
+    if args.fused_lm_loss:
+        kwargs["fused_lm_loss"] = True
     if padding_on(args):
         from ..data import SyntheticTokens
         kwargs["pad_token_id"] = SyntheticTokens.PAD_ID

@@ -74,7 +74,12 @@ def loss_kind(args) -> str:
     return getattr(args, "loss", None) or ("mse" if getattr(args, "model", "foo") == "foo" else "ce")
 
 
-def build_criterion(args):
+def build_criterion(args, model: Optional[torch.nn.Module] = None):
+    """``--loss``'s criterion; with ``--fused_lm_loss`` the model's own head-plus-cross-entropy (``lm_head_loss``)."""
+    if getattr(args, "fused_lm_loss", False):
+        if model is None or not getattr(getattr(model, "config", None), "fused_lm_loss", False):
+            raise ValueError("--fused_lm_loss needs a causal LM built with fused_lm_loss=True (it has lm_head_loss)")
+        return model.lm_head_loss()
     return CrossEntropyLoss() if loss_kind(args) == "ce" else MSELoss()
 
 
@@ -132,7 +137,7 @@ class Trainer:
             self.t_total = steps_per_epoch * args.num_train_epochs
 
         # ---- resume (weights first: rank 0's reach every rank through the wrap-time broadcast) -----
-        self.criterion = criterion if criterion is not None else build_criterion(args)
+        self.criterion = criterion if criterion is not None else build_criterion(args, model)
         if self.resume_dir:
             load_checkpoint(self.resume_dir, model)
 

@@ -14,7 +14,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops import LayerNorm, Linear, causal_attention, document_bounds, linear
+from ..ops import LayerNorm, Linear, LinearCrossEntropyLoss, causal_attention, document_bounds, linear
 
 
 @dataclass
@@ -30,6 +30,7 @@ class GPTConfig:
     fp8: bool = False              # block linears (qkv, attn_out, ffn_in, ffn_out) on FP8 tensor cores; same parameters
     pad_token_id: int | None = None  # right-padded input: length = non-pad count per row, attention on the native kernel
     bos_token_id: int | None = None  # packed input: a document starts at each such id (and at 0), attention stays inside it
+    fused_lm_loss: bool = False    # forward returns the final hidden states; ``lm_head_loss`` applies the head inside the loss
 
     @property
     def padded_vocab(self) -> int:
@@ -99,7 +100,8 @@ class GPTModel(nn.Module):
 class GPTLMHeadModel(nn.Module):
     """Decoder + LM head tied to the token embedding (no bias); forward returns logits [B, S, padded vocab].  The padded
     vocabulary rows get a large negative logit bias (a non-persistent buffer, through the GEMM epilogue), so they take
-    no probability and leave the loss unchanged."""
+    no probability and leave the loss unchanged.  With ``GPTConfig.fused_lm_loss`` forward returns the final hidden states
+    [B, S, hidden] instead and ``lm_head_loss()`` is the criterion that applies the head (``ops.linear_cross_entropy``)."""
 
     def __init__(self, config: GPTConfig | None = None):
         super().__init__()
@@ -115,7 +117,14 @@ class GPTLMHeadModel(nn.Module):
 
     def forward(self, input_ids):
         h = self.transformer(input_ids)
+        if self.config.fused_lm_loss:
+            return h
         return linear(h, self.transformer.wte.weight, self.vocab_bias.to(h.dtype))
+
+    def lm_head_loss(self, ignore_index: int = -100) -> LinearCrossEntropyLoss:
+        """Criterion over ``forward``'s hidden states with ``fused_lm_loss``: the tied head and the padded-vocabulary bias,
+        read from this model at every call."""
+        return LinearCrossEntropyLoss(lambda: (self.transformer.wte.weight, self.vocab_bias), ignore_index)
 
     def load_hf_state_dict(self, hf: dict) -> None:
         """Load a ``transformers.GPT2LMHeadModel`` state dict.  Its ``Conv1D`` weights are stored [in, out] and are
@@ -146,8 +155,10 @@ class GPTLMHeadModel(nn.Module):
         self.load_state_dict(out, strict=True)
 
 
-def gpt2(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None) -> nn.Module:
+def gpt2(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
+         fused_lm_loss: bool = False) -> nn.Module:
     """GPT-2 small (124 M) with its LM head; ``fp8=True`` puts the 48 block linears on FP8 tensor cores (embeddings and
     the tied LM head stay bf16).  ``pad_token_id`` takes right-padded input; ``bos_token_id`` takes packed documents,
-    each starting with that id (causal attention stays inside a document and position ids restart in each)."""
-    return GPTLMHeadModel(GPTConfig(fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id))
+    each starting with that id (causal attention stays inside a document and position ids restart in each).
+    ``fused_lm_loss=True``: forward returns hidden states and ``lm_head_loss()`` computes the loss without the logits."""
+    return GPTLMHeadModel(GPTConfig(fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))

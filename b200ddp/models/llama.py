@@ -19,7 +19,7 @@ from dataclasses import dataclass
 import torch
 import torch.nn as nn
 
-from ..ops import Linear, RMSNorm, causal_attention, document_bounds, linear, rotary, rotary_cos_sin, swiglu
+from ..ops import Linear, LinearCrossEntropyLoss, RMSNorm, causal_attention, document_bounds, linear, rotary, rotary_cos_sin, swiglu
 
 
 @dataclass
@@ -37,6 +37,7 @@ class LlamaConfig:
     fp8: bool = False              # block linears (qkv, o_proj, gate_up, down_proj) on FP8 tensor cores; same parameters
     pad_token_id: int | None = None  # right-padded input: length = non-pad count per row
     bos_token_id: int | None = None  # packed input: a document starts at each such id (and at 0), attention stays inside it
+    fused_lm_loss: bool = False    # forward returns the final hidden states; ``lm_head_loss`` applies the head inside the loss
 
     @property
     def head_dim(self) -> int:
@@ -105,7 +106,8 @@ class LlamaModel(nn.Module):
 
 
 class LlamaForCausalLM(nn.Module):
-    """Decoder + LM head tied to the token embedding (no bias); forward returns logits [B, S, vocab]."""
+    """Decoder + LM head tied to the token embedding (no bias); forward returns logits [B, S, vocab], or with
+    ``LlamaConfig.fused_lm_loss`` the final hidden states [B, S, hidden], to be scored by ``lm_head_loss()``."""
 
     def __init__(self, config: LlamaConfig | None = None):
         super().__init__()
@@ -116,7 +118,12 @@ class LlamaForCausalLM(nn.Module):
         return self.model.config
 
     def forward(self, input_ids):
-        return linear(self.model(input_ids), self.model.embed_tokens.weight)
+        h = self.model(input_ids)
+        return h if self.config.fused_lm_loss else linear(h, self.model.embed_tokens.weight)
+
+    def lm_head_loss(self, ignore_index: int = -100) -> LinearCrossEntropyLoss:
+        """Criterion over ``forward``'s hidden states with ``fused_lm_loss``: the tied head, read from this model at every call."""
+        return LinearCrossEntropyLoss(lambda: (self.model.embed_tokens.weight, None), ignore_index)
 
     def load_hf_state_dict(self, hf: dict) -> None:
         """Load a ``transformers.LlamaForCausalLM`` or ``transformers.Qwen2ForCausalLM`` state dict: q / k / v (weights, and
@@ -137,16 +144,19 @@ class LlamaForCausalLM(nn.Module):
         self.load_state_dict({k: v.to(own[k].dtype).contiguous() for k, v in out.items()}, strict=True)
 
 
-def smollm_135m(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None) -> nn.Module:
+def smollm_135m(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
+                fused_lm_loss: bool = False) -> nn.Module:
     """SmolLM-135M with its tied LM head; ``fp8=True`` puts the 120 block linears on FP8 tensor cores (embedding and LM
     head stay bf16).  ``pad_token_id`` takes right-padded input; ``bos_token_id`` takes packed documents, each starting
-    with that id (attention stays inside a document and position ids restart in each)."""
-    return LlamaForCausalLM(LlamaConfig(fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id))
+    with that id (attention stays inside a document and position ids restart in each).  ``fused_lm_loss=True``: forward
+    returns hidden states and ``lm_head_loss()`` computes the loss without the logits."""
+    return LlamaForCausalLM(LlamaConfig(fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))
 
 
-def qwen2_5_1_5b(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None) -> nn.Module:
+def qwen2_5_1_5b(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
+                 fused_lm_loss: bool = False) -> nn.Module:
     """Qwen2.5-1.5B with its tied LM head (32768 positions); ``fp8=True`` puts the 112 block linears on FP8 tensor cores.
-    ``pad_token_id`` and ``bos_token_id`` as for ``smollm_135m``."""
+    ``pad_token_id``, ``bos_token_id`` and ``fused_lm_loss`` as for ``smollm_135m``."""
     return LlamaForCausalLM(LlamaConfig(vocab_size=151936, max_position=32768, hidden=1536, layers=28, heads=12, kv_heads=2,
                                         intermediate=8960, eps=1e-6, rope_theta=1e6, attention_bias=True, fp8=fp8,
-                                        pad_token_id=pad_token_id, bos_token_id=bos_token_id))
+                                        pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))

@@ -917,6 +917,81 @@ def cross_entropy(logits: torch.Tensor, targets: torch.Tensor, ignore_index: int
 
 
 # ------------------------------------------------------------------------------------------------
+# LM head + cross-entropy without the logits (csrc/gemm_wgmma.cu LM epilogues, csrc/loss.cu combine)
+# ------------------------------------------------------------------------------------------------
+# Vocabulary columns per backward slice: the bf16 logit gradient of one slice, [tokens, LM_LOSS_SLICE], is the largest
+# buffer the backward allocates (67 MB at 8192 tokens).  On an H100 (700 W) the Qwen2.5 head backward (8192 x 151936 x 1536)
+# took 27.0 - 28.3 ms at 4096, 8192, 16384 and 32768 columns in two runs of `bench/kernel_bench.py --only lmloss`, with no
+# width fastest in both, so the narrowest, with the smallest buffer, is used.
+LM_LOSS_SLICE = 4096
+
+
+class _LinearCrossEntropy(torch.autograd.Function):
+    """Forward: one GEMM whose epilogue reduces each row's logits per 128-column tile to (max, sum exp), then a fixed-order
+    merge to the row log-sum-exp and the mean loss.  Backward, per vocabulary slice: the GEMM again, its epilogue writing
+    the bf16 logit gradient, then dh += dlogits . weight[slice] (fp32) and dweight[slice] = dlogits^T . hidden.  The upstream
+    gradient and the valid-row count stay on the device (CUDA-graph safe).  Nothing of size [tokens, vocab] is allocated."""
+
+    @staticmethod
+    def forward(ctx, hidden, weight, targets, bias, ignore_index):
+        h2 = hidden.reshape(-1, hidden.shape[-1]).contiguous()
+        t = targets.reshape(-1).to(torch.long).contiguous()
+        w = weight.contiguous()
+        loss, lse, row_loss = _C().lm_loss_fwd(h2, w, t, bias, int(ignore_index))
+        ctx.save_for_backward(h2, w, t, bias, lse, row_loss)
+        ctx.ignore_index = int(ignore_index)
+        ctx.h_shape = hidden.shape
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        h2, w, t, bias, lse, row_loss = ctx.saved_tensors
+        gs = g.detach().float().reshape(1).contiguous()
+        dh, dw = _C().lm_loss_bwd(h2, w, t, bias, lse, row_loss, gs, ctx.ignore_index, LM_LOSS_SLICE,
+                                  ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        return (dh.view(ctx.h_shape) if dh is not None else None), dw, None, None, None
+
+
+def _linear_cross_entropy_reference(hidden, weight, targets, bias, ignore_index):
+    """CPU body: ``cross_entropy(linear(hidden, weight, bias), targets)`` with the same ignore rule (targets equal to
+    ``ignore_index``, negative or >= V are ignored; all ignored gives 0).  Differentiable through autograd."""
+    logits = F.linear(hidden.reshape(-1, hidden.shape[-1]), weight, bias).float()
+    t = targets.reshape(-1)
+    valid = (t != ignore_index) & (t >= 0) & (t < logits.shape[-1])
+    picked = logits.gather(1, torch.where(valid, t, 0)[:, None])[:, 0]
+    rows = torch.where(valid, torch.logsumexp(logits, -1) - picked, 0.0)
+    return rows.sum() / valid.sum().clamp(min=1)
+
+
+def linear_cross_entropy(hidden: torch.Tensor, weight: torch.Tensor, targets: torch.Tensor, bias: Optional[torch.Tensor] = None,
+                         ignore_index: int = -100) -> torch.Tensor:
+    """Mean over non-ignored rows of ``cross_entropy(linear(hidden, weight, bias), targets)``: hidden [..., H], weight [V, H],
+    bias [V] or None, targets [...] integer.  Targets equal to ``ignore_index``, negative or >= V are ignored; when every row
+    is ignored the loss and the gradients are 0.  On CUDA the [tokens, V] logits are never allocated (``_LinearCrossEntropy``):
+    bf16 hidden / weight / bias, H and V multiples of 8, else ``ValueError``.  The bias is a constant (GPT-2's
+    padded-vocabulary mask): it gets no gradient on CUDA."""
+    if hidden.dim() < 1 or weight.dim() != 2 or weight.shape[1] != hidden.shape[-1] or \
+            tuple(targets.shape) != tuple(hidden.shape[:-1]) or (bias is not None and tuple(bias.shape) != (weight.shape[0],)):
+        raise ValueError(f"linear_cross_entropy needs hidden [..., H], weight [V, H], targets [...] and bias [V], got hidden "
+                         f"{tuple(hidden.shape)}, weight {tuple(weight.shape)}, targets {tuple(targets.shape)}, bias "
+                         f"{None if bias is None else tuple(bias.shape)}")
+    if targets.is_floating_point() or targets.is_complex():
+        raise ValueError(f"linear_cross_entropy needs integer targets, got {targets.dtype}")
+    if not hidden.is_cuda:
+        return _linear_cross_entropy_reference(hidden, weight, targets, bias, ignore_index)
+    V, H = weight.shape
+    if hidden.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16 or (bias is not None and bias.dtype != torch.bfloat16):
+        raise ValueError(f"linear_cross_entropy on CUDA needs bf16 hidden, weight and bias, got {hidden.dtype}, {weight.dtype}, "
+                         f"{None if bias is None else bias.dtype}")
+    if H % 8 or V % 8 or hidden.numel() == 0:
+        raise ValueError(f"linear_cross_entropy on CUDA needs H and V multiples of 8 and at least one row, got weight "
+                         f"{tuple(weight.shape)}, hidden {tuple(hidden.shape)}")
+    if bias is not None:
+        bias = bias.detach().contiguous()
+    return _LinearCrossEntropy.apply(hidden, weight, targets, bias, ignore_index)
+
+
+# ------------------------------------------------------------------------------------------------
 # LayerNorm
 # ------------------------------------------------------------------------------------------------
 class _LayerNormFused(torch.autograd.Function):

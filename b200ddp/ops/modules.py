@@ -134,3 +134,20 @@ class CrossEntropyLoss(nn.Module):
 
     def forward(self, logits: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         return Fn.cross_entropy(logits, target, self.ignore_index)
+
+
+class LinearCrossEntropyLoss(nn.Module):
+    """Criterion over final hidden states: ``linear_cross_entropy(hidden, weight, target, bias)``, where ``head()`` returns
+    the model's current ``(weight, bias or None)`` at every call, so casts and moves of the model (``.to()``,
+    ``to_mixed_bf16``) are followed.  Holds no parameters; the bias is cast to the hidden states' dtype."""
+
+    def __init__(self, head, ignore_index: int = -100):
+        super().__init__()
+        self.head = head
+        self.ignore_index = ignore_index
+
+    def forward(self, hidden: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        weight, bias = self.head()
+        if bias is not None:
+            bias = bias.to(hidden.dtype)
+        return Fn.linear_cross_entropy(hidden, weight, target, bias, self.ignore_index)

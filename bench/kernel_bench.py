@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,conv,bn,sgd,adamw,ln,xent,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,conv,bn,sgd,adamw,ln,xent,lmloss,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -578,6 +578,50 @@ def main():
             torch.autograd.grad(loss, xr)
         lib = timeit(lib_xent, args.iters)
         record(f"xent fwd+bwd {rows_}x{cols} bf16", ms, bytes_=rows_ * cols * 2 * 2, lib_ms=lib, note="min traffic = read logits + write dlogits")
+
+    if "lmloss" in want:
+        # Fused LM-head cross-entropy (forward + backward, no logits) against cross_entropy(linear(h, E, b)) at the head
+        # shapes of the README's GPT-2 (8 x 1024, padded vocabulary with its bias), SmolLM (8 x 2048) and Qwen2.5 (4 x 2048)
+        # runs.  FLOPs: 4 head GEMMs fused (the forward is recomputed), 3 unfused.  Memory: rise of the peak over fwd+bwd.
+        print(f"lm-head loss on {card()}", flush=True)
+        for label, N, V, H, with_bias in (("gpt2", 8192, 50304, 768, True), ("smollm", 16384, 49152, 576, False),
+                                          ("qwen", 8192, 151936, 1536, False)):
+            h = torch.randn(N, H, device=dev).to(torch.bfloat16).requires_grad_(True)
+            w = (torch.randn(V, H, device=dev) * 0.02).to(torch.bfloat16).requires_grad_(True)
+            t = torch.randint(0, V, (N,), device=dev)
+            b = None
+            if with_bias:
+                b = torch.zeros(V, device=dev, dtype=torch.bfloat16)
+                b[50257:] = -1e4
+
+            def fused():
+                torch.autograd.grad(Fn.linear_cross_entropy(h, w, t, b), (h, w))
+
+            def unfused():
+                torch.autograd.grad(Fn.cross_entropy(Fn.linear(h, w, b), t), (h, w))
+
+            def peak_rise(fn):
+                torch.cuda.synchronize()
+                base = torch.cuda.memory_allocated()
+                torch.cuda.reset_peak_memory_stats()
+                fn()
+                torch.cuda.synchronize()
+                return (torch.cuda.max_memory_allocated() - base) / 1e9
+            gemm = 2.0 * N * V * H
+            mf, mu = peak_rise(fused), peak_rise(unfused)
+            lib = timeit(unfused, args.iters)
+            record(f"lm-loss {label} fwd+bwd {N}x{V}x{H}", timeit(fused, args.iters), flops=4 * gemm, lib_ms=lib,
+                   note=f"lib = unfused native linear + cross_entropy ({3 * gemm / lib / 1e9:.0f} TFLOP/s); peak rise "
+                        f"fused {mf:.2f} GB, unfused {mu:.2f} GB")
+            if label == "qwen":                                        # backward slice width
+                C_ = _ext.get()
+                tt = t.clone()
+                loss, lse, rl = C_.lm_loss_fwd(h.detach(), w.detach(), tt, None, -100)
+                g1 = torch.ones(1, device=dev)
+                for sl in (4096, 8192, 16384, 32768):
+                    ms = timeit(lambda: C_.lm_loss_bwd(h.detach(), w.detach(), tt, None, lse, rl, g1, -100, sl), args.iters)
+                    record(f"lm-loss qwen bwd slice {sl}", ms, flops=3 * gemm, note=f"dlogits buffer {N * sl * 2 / 1e6:.0f} MB")
+            del h, w
 
     if "mse" in want:
         n = 64 * 1024 * 1024
