@@ -830,7 +830,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // ---- Llama building blocks: rotary embedding (rotary.cu), RMSNorm (layernorm.cu), SwiGLU (loss.cu) --------------------
   // y = rope(qkv) (backward: the transpose rotation); qkv bf16 [rows, (heads + 2*kv_heads)*d] with d = 64 or 128, positions
   // int32 [rows], table fp32 [max_pos, 2, d/2]
-  m.def("rotary", [](at::Tensor x, at::Tensor pos, at::Tensor table, int heads, int kv_heads, bool backward) {
+  m.def("rotary", [](at::Tensor x, at::Tensor pos, at::Tensor table, int heads, int kv_heads, bool backward, double q_scale) {
     check_cuda(x, "x"); check_cuda(pos, "position_ids"); check_cuda(table, "cos_sin");
     TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == 2 &&
                 (table.size(2) == 32 || table.size(2) == 64), "rotary: cos_sin must be contiguous fp32 [max_position, 2, d/2], d = 64 or 128");
@@ -843,9 +843,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     if ((reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) != 0) x = x.clone();
     at::Tensor y = at::empty_like(x);
     launch_rotary(x.data_ptr(), pos.data_ptr<int>(), table.data_ptr<float>(), (int)table.size(0), (size_t)x.size(0), heads, kv_heads, d,
-                  y.data_ptr(), backward, cur_stream());
+                  y.data_ptr(), backward, cur_stream(), (float)q_scale);
     return y;
-  }, py::arg("x"), py::arg("position_ids"), py::arg("cos_sin"), py::arg("heads"), py::arg("kv_heads"), py::arg("backward") = false);
+  }, py::arg("x"), py::arg("position_ids"), py::arg("cos_sin"), py::arg("heads"), py::arg("kv_heads"), py::arg("backward") = false,
+     py::arg("q_scale") = 1.0);
   auto aligned32 = [](at::Tensor t) { return (reinterpret_cast<uintptr_t>(t.data_ptr()) & 31) != 0 ? t.clone() : t; };
   m.def("rmsnorm_fwd", [aligned32](at::Tensor x, at::Tensor gamma, double eps) {
     check_cuda(x, "x"); check_cuda(gamma, "gamma");
@@ -907,6 +908,130 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     at::Tensor out = at::empty_like(gate_up);
     launch_swiglu(gate_up.data_ptr(), dy.data_ptr(), out.data_ptr(), (size_t)(dy.numel() / inter), inter, true, cur_stream());
     return out;
+  });
+
+  // ---- mixture of experts (moe.cu, grouped GEMMs in gemm_wgmma.cu) -------------------------------------------------
+  auto moe_tensor = [](const at::Tensor& t, at::ScalarType st, int64_t numel, const char* what) {
+    check_cuda(t, what);
+    TORCH_CHECK(t.scalar_type() == st && t.is_contiguous() && t.numel() == numel, "moe: ", what, " must be a contiguous ",
+                c10::toString(st), " tensor of ", numel, " elements, got ", c10::toString(t.scalar_type()), " ", t.sizes());
+  };
+  // logits bf16 [T, E] -> (ids int32 [T, k], gates bf16 [T, k], probsum fp32 [E] (aux) or None)
+  m.def("moe_route", [moe_tensor](at::Tensor logits, int k, bool aux) {
+    TORCH_CHECK(logits.dim() == 2, "moe_route: logits [T, E]");
+    const int T = (int)logits.size(0), E = (int)logits.size(1);
+    moe_tensor(logits, at::kBFloat16, (int64_t)T * E, "logits");
+    c10::cuda::CUDAGuard guard(logits.device());
+    at::Tensor ids = at::empty({T, k}, logits.options().dtype(at::kInt));
+    at::Tensor gates = at::empty({T, k}, logits.options());
+    c10::optional<at::Tensor> probsum;
+    at::Tensor partial;
+    if (aux) {
+      probsum = at::empty({E}, logits.options().dtype(at::kFloat));
+      partial = at::empty({(T + 63) / 64, E}, logits.options().dtype(at::kFloat));
+    }
+    launch_moe_router_fwd(logits.data_ptr(), T, E, k, ids.data_ptr<int>(), gates.data_ptr(), aux ? partial.data_ptr<float>() : nullptr,
+                          aux ? probsum->data_ptr<float>() : nullptr, cur_stream());
+    return std::make_tuple(ids, gates, probsum);
+  });
+  // dlogits bf16 [T, E] from d(gates) fp32 [T, k] and d(probsum) fp32 [E] (or None)
+  m.def("moe_router_bwd", [moe_tensor](at::Tensor logits, at::Tensor ids, at::Tensor dgates, c10::optional<at::Tensor> dprobsum) {
+    TORCH_CHECK(logits.dim() == 2 && ids.dim() == 2 && ids.size(0) == logits.size(0), "moe_router_bwd: logits [T, E], ids [T, k]");
+    const int T = (int)logits.size(0), E = (int)logits.size(1), k = (int)ids.size(1);
+    moe_tensor(logits, at::kBFloat16, (int64_t)T * E, "logits");
+    moe_tensor(ids, at::kInt, (int64_t)T * k, "ids");
+    moe_tensor(dgates, at::kFloat, (int64_t)T * k, "dgates");
+    if (dprobsum.has_value()) moe_tensor(*dprobsum, at::kFloat, E, "dprobsum");
+    c10::cuda::CUDAGuard guard(logits.device());
+    at::Tensor dlogits = at::empty_like(logits);
+    launch_moe_router_bwd(logits.data_ptr(), T, E, k, ids.data_ptr<int>(), dgates.data_ptr<float>(),
+                          dprobsum.has_value() ? dprobsum->data_ptr<float>() : nullptr, dlogits.data_ptr(), cur_stream());
+    return dlogits;
+  });
+  // ids int32 [T, k] -> (counts [E], offsets [E + 1], fwd_map [capacity], inv_map [T, k], tile_expert [capacity / 128]), int32
+  m.def("moe_permute", [moe_tensor](at::Tensor ids, int E) {
+    TORCH_CHECK(ids.dim() == 2, "moe_permute: ids [T, k]");
+    const int T = (int)ids.size(0), k = (int)ids.size(1);
+    moe_tensor(ids, at::kInt, (int64_t)T * k, "ids");
+    TORCH_CHECK(T >= 1 && E >= 1 && E <= kMoeMaxExperts && k >= 1 && k <= kMoeMaxTopK && k <= E,
+                "moe_permute: needs T >= 1, 1 <= E <= 64, 1 <= k <= min(E, 8), got T=", T, " E=", E, " k=", k);
+    c10::cuda::CUDAGuard guard(ids.device());
+    const int cap = moe_capacity(T, E, k), chunks = moe_chunks(T, k);
+    auto opt = ids.options();
+    at::Tensor work = at::empty({2, chunks, E}, opt), counts = at::empty({E}, opt), offsets = at::empty({E + 1}, opt);
+    at::Tensor fwd = at::empty({cap}, opt), inv = at::empty({T, k}, opt), tiles = at::empty({cap / kMoeAlign}, opt);
+    launch_moe_permute(ids.data_ptr<int>(), T, E, k, work.data_ptr<int>(), counts.data_ptr<int>(), offsets.data_ptr<int>(),
+                       fwd.data_ptr<int>(), inv.data_ptr<int>(), tiles.data_ptr<int>(), cur_stream());
+    return std::make_tuple(counts, offsets, fwd, inv, tiles);
+  });
+  m.def("moe_capacity", [](int T, int E, int k) { return moe_capacity(T, E, k); });
+  // x bf16 [T, H] -> x_perm [capacity, H]
+  m.def("moe_gather", [moe_tensor](at::Tensor x, at::Tensor fwd_map, int k) {
+    TORCH_CHECK(x.dim() == 2 && fwd_map.dim() == 1, "moe_gather: x [T, H], fwd_map [capacity]");
+    moe_tensor(x, at::kBFloat16, x.numel(), "x");
+    moe_tensor(fwd_map, at::kInt, fwd_map.numel(), "fwd_map");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int H = (int)x.size(1), cap = (int)fwd_map.numel();
+    at::Tensor out = at::empty({cap, H}, x.options());
+    launch_moe_gather(x.data_ptr(), fwd_map.data_ptr<int>(), cap, H, k, out.data_ptr(), cur_stream());
+    return out;
+  });
+  // forward: a [capacity, K] . w_e^T with w [E, N, K] -> [capacity, N]; dgrad: a [capacity, K] . w_e with w [E, K, N] -> [capacity, N]
+  m.def("moe_gemm", [moe_tensor](at::Tensor a, at::Tensor w, at::Tensor tile_expert, bool dgrad, c10::optional<at::Tensor> out) {
+    TORCH_CHECK(a.dim() == 2 && w.dim() == 3, "moe_gemm: a [rows, K], w [E, *, *]");
+    const int rows = (int)a.size(0), E = (int)w.size(0);
+    const int K = (int)(dgrad ? w.size(1) : w.size(2)), N = (int)(dgrad ? w.size(2) : w.size(1));
+    TORCH_CHECK(a.size(1) == K, "moe_gemm: a has ", a.size(1), " columns, the weight's reduction dim is ", K);
+    moe_tensor(a, at::kBFloat16, a.numel(), "a");
+    moe_tensor(w, at::kBFloat16, w.numel(), "w");
+    moe_tensor(tile_expert, at::kInt, rows / kMoeAlign, "tile_expert");
+    c10::cuda::CUDAGuard guard(a.device());
+    at::Tensor d = out.has_value() ? *out : at::empty({rows, N}, a.options());
+    if (out.has_value()) moe_tensor(d, at::kBFloat16, (int64_t)rows * N, "out");
+    launch_gemm_grouped(a.data_ptr(), w.data_ptr(), d.data_ptr(), rows, N, K, E, dgrad, tile_expert.data_ptr<int>(), cur_stream());
+    return d;
+  }, py::arg("a"), py::arg("w"), py::arg("tile_expert"), py::arg("dgrad"), py::arg("out") = py::none());
+  // weight gradient: dw [E, M, N] (bf16), dw_e = a[s_e]^T . b[s_e] over expert e's segment of a [capacity, M] and b [capacity, N]
+  m.def("moe_gemm_wgrad", [moe_tensor](at::Tensor a, at::Tensor b, at::Tensor offsets, c10::optional<at::Tensor> out) {
+    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.size(0) == b.size(0) && offsets.dim() == 1, "moe_gemm_wgrad: a [rows, M], b [rows, N], offsets [E + 1]");
+    moe_tensor(a, at::kBFloat16, a.numel(), "a");
+    moe_tensor(b, at::kBFloat16, b.numel(), "b");
+    moe_tensor(offsets, at::kInt, offsets.numel(), "offsets");
+    c10::cuda::CUDAGuard guard(a.device());
+    const int rows = (int)a.size(0), M = (int)a.size(1), N = (int)b.size(1), E = (int)offsets.numel() - 1;
+    at::Tensor d = out.has_value() ? *out : at::empty({E, M, N}, a.options());
+    if (out.has_value()) moe_tensor(d, at::kBFloat16, (int64_t)E * M * N, "out");
+    launch_gemm_grouped_wgrad(a.data_ptr(), b.data_ptr(), d.data_ptr(), rows, M, N, E, offsets.data_ptr<int>(), cur_stream());
+    return d;
+  }, py::arg("a"), py::arg("b"), py::arg("offsets"), py::arg("out") = py::none());
+  // out [T, H] = sum_j gate[t, j] * y_perm[inv[t, j]] (gates None: weight 1)
+  m.def("moe_combine", [moe_tensor](at::Tensor y_perm, at::Tensor inv_map, c10::optional<at::Tensor> gates) {
+    TORCH_CHECK(y_perm.dim() == 2 && inv_map.dim() == 2, "moe_combine: y_perm [capacity, H], inv_map [T, k]");
+    const int T = (int)inv_map.size(0), k = (int)inv_map.size(1), H = (int)y_perm.size(1);
+    moe_tensor(y_perm, at::kBFloat16, y_perm.numel(), "y_perm");
+    moe_tensor(inv_map, at::kInt, (int64_t)T * k, "inv_map");
+    if (gates.has_value()) moe_tensor(*gates, at::kBFloat16, (int64_t)T * k, "gates");
+    c10::cuda::CUDAGuard guard(y_perm.device());
+    at::Tensor out = at::empty({T, H}, y_perm.options());
+    launch_moe_combine(y_perm.data_ptr(), inv_map.data_ptr<int>(), gates.has_value() ? gates->data_ptr() : nullptr, T, H, k, out.data_ptr(),
+                       cur_stream());
+    return out;
+  });
+  // (dy_perm bf16 [capacity, H], dgates fp32 [T, k]) from dout bf16 [T, H]
+  m.def("moe_combine_bwd", [moe_tensor](at::Tensor dout, at::Tensor y_perm, at::Tensor fwd_map, at::Tensor gates) {
+    TORCH_CHECK(dout.dim() == 2 && y_perm.dim() == 2 && gates.dim() == 2 && dout.size(1) == y_perm.size(1) && gates.size(0) == dout.size(0),
+                "moe_combine_bwd: dout [T, H], y_perm [capacity, H], gates [T, k]");
+    const int T = (int)dout.size(0), H = (int)dout.size(1), k = (int)gates.size(1), cap = (int)y_perm.size(0);
+    moe_tensor(dout, at::kBFloat16, dout.numel(), "dout");
+    moe_tensor(y_perm, at::kBFloat16, y_perm.numel(), "y_perm");
+    moe_tensor(fwd_map, at::kInt, cap, "fwd_map");
+    moe_tensor(gates, at::kBFloat16, (int64_t)T * k, "gates");
+    c10::cuda::CUDAGuard guard(dout.device());
+    at::Tensor dy = at::empty_like(y_perm);
+    at::Tensor dgates = at::empty({T, k}, dout.options().dtype(at::kFloat));
+    launch_moe_combine_bwd(dout.data_ptr(), y_perm.data_ptr(), fwd_map.data_ptr<int>(), gates.data_ptr(), cap, H, k, dy.data_ptr(),
+                           dgates.data_ptr<float>(), cur_stream());
+    return std::make_tuple(dy, dgates);
   });
   m.def("gemm_supported", &gemm_shape_supported);
   m.def("set_gemm_cta_mode", &set_gemm_cta_mode);

@@ -39,6 +39,19 @@ void launch_gemm_lm_dlogits(const void* hidden, const void* weight, const void* 
                             const long long* targets, long long ignore_index, const float* lse, const float* gscale,
                             const float* valid, void* dlogits, cudaStream_t stream);
 
+// Grouped (mixture-of-experts) GEMMs on 128 x 128 tiles, bf16 in and out.  A's rows are sorted by expert into segments that
+// start at multiples of 128, so each 128-row tile belongs to one expert; rows % 128 == 0, N and K multiples of 64.
+// launch_gemm_grouped: D [rows, N] = A [rows, K] . B_e^T per tile, B_e the tile's expert's [N, K] block of B stored
+// [E * N, K] (b_mn=false, forward), or D = A . B_e with B_e the [K, N] block of B stored [E * K, N] (b_mn=true, data
+// gradient).  tile_expert int32 [rows / 128] on the device: the tile's expert, -1 for unused tiles, whose D rows are not
+// written.
+void launch_gemm_grouped(const void* a, const void* b, void* d, int rows, int N, int K, int experts, bool b_mn, const int* tile_expert,
+                         cudaStream_t stream);
+// Weight gradient: D [E, M, N] with D_e = A[s_e]^T . B[s_e] over expert e's rows s_e = [offsets[e], offsets[e+1]) of
+// A [rows, M] and B [rows, N]; offsets int32 [E + 1] on the device, multiples of 64.  An expert without rows gets zeros.
+void launch_gemm_grouped_wgrad(const void* a, const void* b, void* d, int rows, int M, int N, int experts, const int* offsets,
+                               cudaStream_t stream);
+
 // Persistent-tile rasterisation shared by the producer, issuer and epilogue roles (and mirrored on the host for
 // tests).  group_m <= 0: m-fastest over the whole problem (default).  group_m > 0: bands of `group_m` m-tiles
 // are swept n-major, so the ~132 tiles in flight form a near-square patch and both operands are reused out of L2.

@@ -58,17 +58,27 @@ struct GemmParams {
   // fused LM-head cross-entropy (LM != kLmNone).  Appended after the fields above so that their offsets stay as they
   // were, and kept to 56 bytes: at 128 bytes or less the struct's parameter loads, and the code of every other variant,
   // compile as before.  kLmLse writes its (max, sum exp) partials to `d` (it stores no output tile).
-  const long long* lm_targets;   // [M] target column of each row (global vocabulary index)
+  // The grouped expert GEMMs (GRP != kGrpNone) never run an LM-head epilogue, so their four fields (grp_*) share these bytes:
+  //   grp_tile_expert  kGrpRows: [M / 128] expert of each 128-row tile of A and D, -1 = unused (skipped)
+  //   grp_offsets      kGrpWgrad: [E + 1] start row of each expert's 128-aligned segment of A and B
+  //   grp_rows         kGrpRows: B rows per expert (expert e's B starts at row e * grp_rows of its 2-D view);
+  //                    kGrpWgrad: output rows per expert (D is [E * grp_rows, N])
+  //   grp_experts      kGrpWgrad: E
+  union { const long long* lm_targets; const int* grp_tile_expert; };   // [M] target column of each row (global vocabulary index)
   float* lm_target_logit;        // kLmLse: [M] the row's target logit, written by the one tile that holds it
-  const float* lm_lse;           // kLmDlogits: [M] row log-sum-exp
+  union { const float* lm_lse; const int* grp_offsets; };              // kLmDlogits: [M] row log-sum-exp
   const float* lm_gscale;        // kLmDlogits: device scalars, upstream gradient and number of non-ignored rows
   const float* lm_valid;
   int lm_ignore_index;           // kLmDlogits: ignore_index if it lies in [0, lm_vocab), else -1 (already ignored as out of range)
-  int lm_col_offset;             // kLmDlogits: global vocabulary index of this GEMM's column 0
-  int lm_vocab;                  // full vocabulary: targets outside [0, lm_vocab) are ignored
+  union { int lm_col_offset; int grp_rows; };                          // kLmDlogits: global vocabulary index of this GEMM's column 0
+  union { int lm_vocab; int grp_experts; };                            // full vocabulary: targets outside [0, lm_vocab) are ignored
 };
 
 constexpr int kLmNone = 0, kLmLse = 1, kLmDlogits = 2;
+// Grouped (mixture-of-experts) modes.  kGrpRows: forward / data gradient, A's rows are sorted by expert in 128-aligned
+// segments, so every 128-row tile multiplies one expert's B.  kGrpWgrad: D_e = A_e^T B_e per expert e, both operands
+// MN-major, the k-loop running over expert e's segment only.
+constexpr int kGrpNone = 0, kGrpRows = 1, kGrpWgrad = 2;
 
 // bias / activation on 32 consecutive accumulator columns starting at `col0`
 __device__ __forceinline__ void epilogue_math(const GemmParams& p, int col0, const uint32_t* r, float* v) {
@@ -292,6 +302,29 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmParams& p, const CUt
   }
 }
 
+// The scheduled tile's coordinates.  Grouped modes also give its expert `e`, its k-block range [kb0, kb1) and B's row
+// offset; false = an unused tile of kGrpRows, which the producer and the MMA warpgroup both skip.
+template <int GRP>
+__device__ __forceinline__ bool grouped_tile(const GemmParams& p, int tile, int num_m, int num_n, int* mb,
+                                             int* nb, int* e, int* kb0, int* kb1, int* b_off) {
+  if constexpr (GRP == kGrpNone) {
+    gemm_tile_coords(tile, num_m, num_n, p.group_m, mb, nb);
+    return true;
+  } else if constexpr (GRP == kGrpRows) {
+    gemm_tile_coords(tile, num_m, num_n, 0, mb, nb);
+    *e = __ldg(p.grp_tile_expert + *mb);
+    *b_off = *e * p.grp_rows;
+    return *e >= 0;
+  } else {                                                     // expert-major: all tiles of expert 0, then expert 1, ...
+    const int per_expert = num_m * num_n;
+    *e = tile / per_expert;
+    gemm_tile_coords(tile - *e * per_expert, num_m, num_n, 0, mb, nb);
+    *kb0 = __ldg(p.grp_offsets + *e) / BLOCK_K;
+    *kb1 = __ldg(p.grp_offsets + *e + 1) / BLOCK_K;
+    return true;
+  }
+}
+
 template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
@@ -309,7 +342,8 @@ struct SmemLayout {
 // pair tile).  Each CTA loads its own A tile and HALF of the B tile, multicast into both CTAs' shared memory, so every B
 // byte leaves L2 once per pair.  A stage may be refilled only when the consumers of BOTH CTAs are done with it: the empty
 // barriers count the arrivals of the local and the peer warpgroup.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS, bool PAIR, int OP = kOpBF16, int LM = kLmNone>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS, bool PAIR, int OP = kOpBF16, int LM = kLmNone,
+          int GRP = kGrpNone>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const __grid_constant__ CUtensorMap map_d, const GemmParams p) {
@@ -321,6 +355,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   static_assert(sizeof(GemmParams) <= 128, "GemmParams: see the note on the LM-head fields");
   static_assert(LM == kLmNone || (!kFP8 && !A_MN && !B_MN && !TMA_ST && !STATS && !PAIR && BLOCK_N == 128),
                 "LM-head epilogues: bf16 K-major operands, direct epilogue, single-CTA 128 x 128 tiles");
+  static_assert(GRP == kGrpNone || (!kFP8 && LM == kLmNone && !TMA_ST && !STATS && !PAIR && BLOCK_N == 128 &&
+                                    (GRP == kGrpRows ? !A_MN : (A_MN && B_MN))),
+                "grouped GEMMs: bf16, direct epilogue, single-CTA 128 x 128 tiles; A K-major (rows) or A and B MN-major (wgrad)");
   constexpr int kBK = kFP8 ? 2 * BLOCK_K : BLOCK_K;            // elements per k-block: one 128-byte row either way
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -335,9 +372,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
   const int first = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
   const int stride = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int num_m_blocks = (p.M + kM - 1) / kM;
+  const int num_m_blocks = ((GRP == kGrpWgrad ? p.grp_rows : p.M) + kM - 1) / kM;
   const int num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int num_tiles = num_m_blocks * num_n_blocks;
+  const int num_tiles = num_m_blocks * num_n_blocks * (GRP == kGrpWgrad ? p.grp_experts : 1);
   const int num_k_blocks = (p.K + kBK - 1) / kBK;
 
   if (warp == 0 && lane == 0) {
@@ -357,11 +394,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = first; tile < num_tiles; tile += stride) {
-        int mb, nb;
-        gemm_tile_coords(tile, num_m_blocks, num_n_blocks, p.group_m, &mb, &nb);
+        int mb, nb, e, kb0 = 0, kb1 = num_k_blocks, b_off = 0;
+        if (!grouped_tile<GRP>(p, tile, num_m_blocks, num_n_blocks, &mb, &nb, &e, &kb0, &kb1, &b_off)) continue;
         const int m0 = mb * kM + (int)rank * BLOCK_M;            // rows past M arrive as zeros and are never stored
         const int n0 = nb * BLOCK_N;
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
+        for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * L::kStageBytes;
           uint8_t* sb = sa + L::kABytes;
@@ -380,11 +417,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             if constexpr (!B_MN) tma_load_2d_multicast(&map_b, &full_bar[stage], sb + rank * kHalfB, k0, n0 + 64 * (int)rank, 0x3);
             else tma_load_2d_multicast(&map_b, &full_bar[stage], sb + rank * kHalfB, n0 + 64 * (int)rank, k0, 0x3);
           } else if constexpr (!B_MN) {
-            tma_load_2d(&map_b, &full_bar[stage], sb, k0, n0);                    // box {64 k, BLOCK_N n}
+            tma_load_2d(&map_b, &full_bar[stage], sb, k0, n0 + b_off);            // box {64 k, BLOCK_N n}
           } else {
 #pragma unroll
             for (int c = 0; c < BLOCK_N / 64; ++c)
-              tma_load_2d(&map_b, &full_bar[stage], sb + c * (64 * BLOCK_K * 2), n0 + 64 * c, k0);
+              tma_load_2d(&map_b, &full_bar[stage], sb + c * (64 * BLOCK_K * 2), n0 + 64 * c, k0 + b_off);
           }
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
@@ -406,17 +443,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     uint32_t phase = 0;
     [[maybe_unused]] uint32_t slab = 0;
     for (int tile = first; tile < num_tiles; tile += stride) {
-      int mb, nb;
-      gemm_tile_coords(tile, num_m_blocks, num_n_blocks, p.group_m, &mb, &nb);
+      int mb, nb, e, kb0 = 0, kb1 = num_k_blocks, b_off = 0;
+      if (!grouped_tile<GRP>(p, tile, num_m_blocks, num_n_blocks, &mb, &nb, &e, &kb0, &kb1, &b_off)) continue;
       const int m0 = mb * kM + (int)rank * BLOCK_M;
       const int n0 = nb * BLOCK_N;
       WgAcc<BLOCK_N> acc;
       [[maybe_unused]] WgAcc<BLOCK_N> part;                    // FP8: this k-block's products before promotion
-      if constexpr (kFP8) {
+      if constexpr (kFP8 || GRP == kGrpWgrad) {                // wgrad: an expert without rows runs no wgmma and stores zeros
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 2; ++i) { acc.h[0][i] = 0.f; acc.h[1][i] = 0.f; }
       }
-      for (int kb = 0; kb < num_k_blocks; ++kb) {
+      for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t a_addr = smem_u32(smem + stage * L::kStageBytes);
         const uint32_t b_addr = a_addr + L::kABytes;
@@ -450,7 +487,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       wg_bar_sync();                                           // the previous tile's epilogue is done reading acc_smem
       acc_to_smem<BLOCK_N>(acc, acc_smem, L::kAccStride, threadIdx.x - 128);
       wg_bar_sync();
-      const int row = m0 + ew * 32 + lane;
+      int row = m0 + ew * 32 + lane;
+      if constexpr (GRP == kGrpWgrad) row = row < p.grp_rows ? e * p.grp_rows + row : p.M;   // expert e's rows of D; the rest unstored
       const float* arow = acc_smem + (size_t)(ew * 32 + lane) * L::kAccStride;
       if constexpr (LM != kLmNone) {
         lm_epilogue_tile<LM>(p, arow, row, n0);
@@ -714,6 +752,53 @@ void launch_gemm_lm_dlogits(const void* hidden, const void* weight, const void* 
   p.lm_col_offset = col_offset;
   p.lm_vocab = vocab;
   launch_variant<128, false, false, false, false, false, kOpBF16, kLmDlogits>(hidden, weight, p, stream);
+}
+
+namespace {
+template <bool A_MN, bool B_MN, int GRP>
+void launch_grouped(const CUtensorMap& map_a, const CUtensorMap& map_b, const GemmParams& p, int tiles, cudaStream_t stream) {
+  using L = SmemLayout<128, A_MN, B_MN, false>;
+  static_assert(L::kStages >= 3 && L::kTotal <= 227 * 1024, "shared memory budget");
+  auto kernel = gemm_bf16_kernel<128, A_MN, B_MN, false, false, false, kOpBF16, kLmNone, GRP>;
+  static std::atomic<unsigned long long> configured{0};
+  ensure_max_dynamic_smem(kernel, L::kTotal, configured);
+  const int grid = tiles < kNumSMs ? tiles : kNumSMs;
+  kernel<<<grid, kNumThreads, L::kTotal, stream>>>(map_a, map_b, map_a, p);     // D map unused by the direct epilogue
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void grouped_check(int rows, int N, int K, int experts) {
+  if (rows < 128 || rows % 128 != 0 || N < 64 || N % 64 != 0 || K < 64 || K % 64 != 0 || experts < 1)
+    throw std::runtime_error("gemm_grouped: needs rows a positive multiple of 128, N and K positive multiples of 64 and >= 1 expert, got rows=" +
+                             std::to_string(rows) + " N=" + std::to_string(N) + " K=" + std::to_string(K) + " experts=" + std::to_string(experts));
+}
+}  // namespace
+
+void launch_gemm_grouped(const void* a, const void* b, void* d, int rows, int N, int K, int experts, bool b_mn, const int* tile_expert,
+                         cudaStream_t stream) {
+  grouped_check(rows, N, K, experts);
+  GemmParams p = {};
+  p.M = rows; p.N = N; p.K = K;
+  p.d = d;
+  p.grp_tile_expert = tile_expert;
+  p.grp_rows = b_mn ? K : N;
+  const CUtensorMap map_a = make_map(a, rows, K, BLOCK_M, 64);
+  const int tiles = (rows / BLOCK_M) * ceil_div(N, 128);
+  if (b_mn) launch_grouped<false, true, kGrpRows>(map_a, make_map(b, experts * K, N, BLOCK_K, 64), p, tiles, stream);
+  else launch_grouped<false, false, kGrpRows>(map_a, make_map(b, experts * N, K, 128, 64), p, tiles, stream);
+}
+
+void launch_gemm_grouped_wgrad(const void* a, const void* b, void* d, int rows, int M, int N, int experts, const int* offsets,
+                               cudaStream_t stream) {
+  grouped_check(rows, N, M, experts);
+  GemmParams p = {};
+  p.M = experts * M; p.N = N; p.K = rows;
+  p.d = d;
+  p.grp_offsets = offsets;
+  p.grp_rows = M;
+  p.grp_experts = experts;
+  const int tiles = experts * ceil_div(M, BLOCK_M) * ceil_div(N, 128);
+  launch_grouped<true, true, kGrpWgrad>(make_map(a, rows, M, BLOCK_K, 64), make_map(b, rows, N, BLOCK_K, 64), p, tiles, stream);
 }
 
 }  // namespace b200

@@ -78,9 +78,37 @@ void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, 
 // ---------------- rotary position embedding (rotary.cu) ----------------------------------------------
 // qkv bf16 [rows, (heads + 2*kv_heads)*head_dim] -> y (same shape), head_dim 64 or 128: query and key heads rotated by
 // position pos[r] (int32, clamped to [0, max_pos)), value heads copied; table fp32 [max_pos, 2, head_dim / 2] (cos | sin).
-// backward: the transpose rotation.
+// backward: the transpose rotation.  q_scale (a positive power of two) also multiplies the query heads, in both directions
+// (Granite's attention multiplier folded into q).
 void launch_rotary(const void* x, const int* pos, const float* table, int max_pos, size_t rows, int heads, int kv_heads, int head_dim,
-                   void* y, bool backward, cudaStream_t s);
+                   void* y, bool backward, cudaStream_t s, float q_scale = 1.f);
+
+// ---------------- mixture-of-experts routing, permutation and combine (moe.cu) -----------------------------
+// T tokens, E <= 64 experts, k <= min(E, 8) experts per token, hidden H % 64 == 0.  Deterministic, no atomics, no host
+// synchronisation: every buffer size follows from (T, E, k) alone.
+constexpr int kMoeMaxExperts = 64, kMoeMaxTopK = 8, kMoeAlign = 128;
+inline int moe_capacity(int T, int E, int k) { return (int)(((long long)T * k + (long long)E * (kMoeAlign - 1) + kMoeAlign - 1) / kMoeAlign * kMoeAlign); }
+inline int moe_chunks(int T, int k) { return (int)(((long long)T * k + 1023) / 1024); }
+// Router: logits bf16 [T, E] -> ids int32 [T, k] (top-k, ties to the lower expert), gates bf16 [T, k] (softmax of the k
+// logits in fp32, rounded once); with probsum != nullptr also probsum fp32 [E] = sum over tokens of softmax(logits)
+// (partial: fp32 [ceil(T / 64), E] workspace, reduced in a fixed order).
+void launch_moe_router_fwd(const void* logits, int T, int E, int k, int* ids, void* gates, float* partial, float* probsum, cudaStream_t s);
+// dlogits bf16 [T, E] = top-k softmax Jacobian . dgates (fp32 [T, k]) + (dprobsum != nullptr) full-softmax Jacobian . dprobsum [E].
+void launch_moe_router_bwd(const void* logits, int T, int E, int k, const int* ids, const float* dgates, const float* dprobsum,
+                           void* dlogits, cudaStream_t s);
+// Stable counting sort of the T*k assignments a = t*k + j by expert: counts int32 [E], offsets int32 [E + 1] (segment
+// starts, multiples of 128), fwd_map int32 [capacity] (permuted row -> a, -1 in padding), inv_map int32 [T*k] (a -> row),
+// tile_expert int32 [capacity / 128] (-1 for unused tiles).  chunk_counts: int32 [2, moe_chunks(T, k), E] workspace.
+void launch_moe_permute(const int* ids, int T, int E, int k, int* chunk_counts, int* counts, int* offsets, int* fwd_map, int* inv_map,
+                        int* tile_expert, cudaStream_t s);
+// x_perm bf16 [capacity, H]: row r = x[fwd_map[r] / k], zeros where fwd_map[r] < 0.
+void launch_moe_gather(const void* x, const int* fwd_map, int capacity, int H, int k, void* x_perm, cudaStream_t s);
+// out bf16 [T, H]: out[t] = sum_j gate[t, j] * y_perm[inv_map[t*k + j]] in fp32, slot order (gates == nullptr: weight 1).
+void launch_moe_combine(const void* y_perm, const int* inv_map, const void* gates, int T, int H, int k, void* out, cudaStream_t s);
+// Combine backward, one writer per row: dy_perm bf16 [capacity, H] = gate * dout[token] (zeros in padding rows) and
+// dgates fp32 [T, k] = <dout[token], y_perm[row]>.
+void launch_moe_combine_bwd(const void* dout, const void* y_perm, const int* fwd_map, const void* gates, int capacity, int H, int k,
+                            void* dy_perm, float* dgates, cudaStream_t s);
 
 // ---------------- layer norm (layernorm.cu) -----------------------------------------------------
 void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, DType dt, int rows, int cols,

@@ -9,6 +9,8 @@
 // in fp64: the kernel evaluates no trigonometric function, so its error does not grow with the position.
 #include "ops.h"
 
+#include <cmath>
+
 namespace b200 {
 namespace {
 
@@ -16,10 +18,13 @@ constexpr int kRopeThreads = 256;
 
 // One thread per (row, head, 8 pairs): columns [8 c, 8 c + 8) and [8 c + kHalf, 8 c + kHalf + 8) of the head, c < kHalf / 8
 // (head dim 2 kHalf).
-template <bool kBwd, int kHalf>
+// kScaleQ: the first q_heads heads (the query heads) are also multiplied by q_scale, a power of two (exact in bf16), in
+// both directions.
+template <bool kBwd, int kHalf, bool kScaleQ = false>
 __global__ void __launch_bounds__(kRopeThreads) rotary_kernel(const __nv_bfloat16* __restrict__ x, const int* __restrict__ pos,
                                                               const float* __restrict__ table, int max_pos, size_t rows, int rot_heads,
-                                                              int heads, __nv_bfloat16* __restrict__ y) {
+                                                              int heads, __nv_bfloat16* __restrict__ y, int q_heads = 0,
+                                                              float q_scale = 1.f) {
   constexpr int kParts = kHalf / 8, kShift = kParts == 4 ? 2 : 3;
   static_assert(kParts == 1 << kShift, "kHalf is 32 or 64");
   const size_t n = rows * (size_t)heads * kParts;
@@ -49,6 +54,12 @@ __global__ void __launch_bounds__(kRopeThreads) rotary_kernel(const __nv_bfloat1
       olo[i] = lo[i] * cv[i] - hi[i] * sn;
       ohi[i] = hi[i] * cv[i] + lo[i] * sn;
     }
+    if constexpr (kScaleQ) {
+      if (hh < q_heads) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { olo[i] *= q_scale; ohi[i] *= q_scale; }
+      }
+    }
     *reinterpret_cast<Bf16x8*>(y + off) = pack8(olo);
     *reinterpret_cast<Bf16x8*>(y + off + kHalf) = pack8(ohi);
   }
@@ -56,12 +67,17 @@ __global__ void __launch_bounds__(kRopeThreads) rotary_kernel(const __nv_bfloat1
 
 template <int kHalf>
 void rotary_launch(const __nv_bfloat16* x, const int* pos, const float* table, int max_pos, size_t rows, int heads, int kv_heads,
-                   __nv_bfloat16* y, bool backward, cudaStream_t s) {
+                   __nv_bfloat16* y, bool backward, float q_scale, cudaStream_t s) {
   const int all = heads + 2 * kv_heads;
   size_t b = (rows * all * (kHalf / 8) + kRopeThreads - 1) / kRopeThreads;
   if (b < 1) b = 1;
   if (b > (size_t)16 * kNumSMs) b = (size_t)16 * kNumSMs;
-  if (backward)
+  if (q_scale != 1.f) {
+    if (backward)
+      rotary_kernel<true, kHalf, true><<<(int)b, kRopeThreads, 0, s>>>(x, pos, table, max_pos, rows, heads + kv_heads, all, y, heads, q_scale);
+    else
+      rotary_kernel<false, kHalf, true><<<(int)b, kRopeThreads, 0, s>>>(x, pos, table, max_pos, rows, heads + kv_heads, all, y, heads, q_scale);
+  } else if (backward)
     rotary_kernel<true, kHalf><<<(int)b, kRopeThreads, 0, s>>>(x, pos, table, max_pos, rows, heads + kv_heads, all, y);
   else
     rotary_kernel<false, kHalf><<<(int)b, kRopeThreads, 0, s>>>(x, pos, table, max_pos, rows, heads + kv_heads, all, y);
@@ -70,14 +86,17 @@ void rotary_launch(const __nv_bfloat16* x, const int* pos, const float* table, i
 }  // namespace
 
 void launch_rotary(const void* x, const int* pos, const float* table, int max_pos, size_t rows, int heads, int kv_heads, int head_dim,
-                   void* y, bool backward, cudaStream_t s) {
+                   void* y, bool backward, cudaStream_t s, float q_scale) {
   if (max_pos < 1 || heads < 1 || kv_heads < 1 || (head_dim != 64 && head_dim != 128) ||
       ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15u) != 0 || (reinterpret_cast<uintptr_t>(table) & 15u) != 0)
     throw std::runtime_error("rotary: needs heads, kv_heads, max_pos >= 1, head dim 64 or 128, 16-byte aligned qkv / out and table");
+  int e2 = 0;
+  if (!(q_scale > 0.f) || std::frexp(q_scale, &e2) != 0.5f)
+    throw std::runtime_error("rotary: the query scale must be a positive power of two (exact in bf16), got " + std::to_string(q_scale));
   const auto* xi = reinterpret_cast<const __nv_bfloat16*>(x);
   auto* yo = reinterpret_cast<__nv_bfloat16*>(y);
-  if (head_dim == 64) rotary_launch<32>(xi, pos, table, max_pos, rows, heads, kv_heads, yo, backward, s);
-  else rotary_launch<64>(xi, pos, table, max_pos, rows, heads, kv_heads, yo, backward, s);
+  if (head_dim == 64) rotary_launch<32>(xi, pos, table, max_pos, rows, heads, kv_heads, yo, backward, q_scale, s);
+  else rotary_launch<64>(xi, pos, table, max_pos, rows, heads, kv_heads, yo, backward, q_scale, s);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 

@@ -67,18 +67,22 @@ def build_parser() -> argparse.ArgumentParser:
                    help="BERT encoder / GPT-2 / SmolLM block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs "
                         "--model bert-base, gpt2, smollm-135m or qwen2.5-1.5b, --fp16 and a GPU")
     p.add_argument("--min_seq_len", type=int, default=None,
-                   help="BERT / GPT-2 / SmolLM / Qwen2.5 on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
+                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Granite on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
                         "keys are hidden from attention (native key-padding or causal kernel on the GPU; needs --fp16 and "
                         "--seq_len %% 128 == 0 there).  Default: fixed-length rows")
     p.add_argument("--pack", action="store_true",
-                   help="BERT / GPT-2 / SmolLM / Qwen2.5 on packed documents: documents with lengths uniform in [--min_seq_len, "
-                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2, Qwen2.5) or <s> (SmolLM), packed "
+                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Granite on packed documents: documents with lengths uniform in [--min_seq_len, "
+                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2, Qwen2.5) or <s> (SmolLM; also Granite, "
+                        "whose own <|end_of_text|> is the padding id 0), packed "
                         "first-fit decreasing into rows; "
                         "attention stays inside a document (native document-boundary or causal kernel on the GPU).  Needs "
-                        "--model bert-base, gpt2, smollm-135m or qwen2.5-1.5b and --min_seq_len < --seq_len")
+                        "--model bert-base, gpt2, smollm-135m, qwen2.5-1.5b or granite-3.0-1b-a400m and --min_seq_len < --seq_len")
     p.add_argument("--fused_lm_loss", action="store_true",
-                   help="GPT-2 / SmolLM / Qwen2.5: LM head and cross-entropy in one op that never builds the [tokens, vocab] "
+                   help="GPT-2 / SmolLM / Qwen2.5 / Granite: LM head and cross-entropy in one op that never builds the [tokens, vocab] "
                         "logits (the head GEMM runs once more in the backward); needs --loss ce, and --fp16 on a GPU")
+    p.add_argument("--router_aux_loss_coef", type=float, default=None,
+                   help="mixture-of-experts models (granite-3.0-1b-a400m): weight of the router load-balancing loss added to "
+                        "the training loss (default: the preset's, 0.001); 0 turns it off and skips its statistics")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -139,6 +143,7 @@ def setup(args):
     check_min_seq_len_args(args)
     check_pack_args(args)
     check_fused_lm_loss_args(args)
+    check_moe_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -146,12 +151,15 @@ def setup(args):
 
 
 # models whose token rows can be right-padded or packed, and whose block linears can run on FP8
-TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m", "qwen2.5-1.5b")
+TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m", "qwen2.5-1.5b", "granite-3.0-1b-a400m")
 # causal LMs: their packed documents start with a BOS id
-CAUSAL_MODELS = ("gpt2", "smollm-135m", "qwen2.5-1.5b")
+CAUSAL_MODELS = ("gpt2", "smollm-135m", "qwen2.5-1.5b", "granite-3.0-1b-a400m")
+# sparse mixture-of-experts LMs: no FP8 path, and a router load-balancing loss
+MOE_MODELS = ("granite-3.0-1b-a400m",)
 GPT2_MAX_SEQ_LEN = 1024
 SMOLLM_MAX_SEQ_LEN = 2048
 QWEN_MAX_SEQ_LEN = 32768
+GRANITE_MAX_SEQ_LEN = 4096
 
 
 def check_gpt_args(args) -> None:
@@ -165,12 +173,18 @@ def check_gpt_args(args) -> None:
     if args.model == "qwen2.5-1.5b" and args.seq_len > QWEN_MAX_SEQ_LEN:
         raise ValueError(f"--model qwen2.5-1.5b has {QWEN_MAX_SEQ_LEN} positions; --seq_len must be at most "
                          f"{QWEN_MAX_SEQ_LEN} (got {args.seq_len})")
+    if args.model == "granite-3.0-1b-a400m" and args.seq_len > GRANITE_MAX_SEQ_LEN:
+        raise ValueError(f"--model granite-3.0-1b-a400m has {GRANITE_MAX_SEQ_LEN} positions; --seq_len must be at most "
+                         f"{GRANITE_MAX_SEQ_LEN} (got {args.seq_len})")
 
 
 def check_fp8_args(args) -> None:
     """``--fp8`` is a BERT / GPT-2 feature on top of bf16 weights on a GPU: reject every other combination up front."""
     if not getattr(args, "fp8", False):
         return
+    if args.model in MOE_MODELS:
+        raise ValueError(f"--fp8 covers dense block linears; --model {args.model} is a mixture of experts, whose expert GEMMs "
+                         f"have no FP8 path")
     if args.model not in TOKEN_MODELS:
         raise ValueError(f"--fp8 covers the block linears of the token models; it needs --model bert-base, gpt2, "
                          f"smollm-135m or qwen2.5-1.5b (got --model {args.model})")
@@ -187,8 +201,8 @@ def check_min_seq_len_args(args) -> None:
     if n is None:
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (or smollm-135m; got --model "
-                         f"{args.model})")
+        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b or "
+                         f"granite-3.0-1b-a400m; got --model {args.model})")
     if not 1 <= n <= args.seq_len:
         raise ValueError(f"--min_seq_len must lie in [1, --seq_len = {args.seq_len}], got {n}")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -204,8 +218,8 @@ def check_pack_args(args) -> None:
     if not getattr(args, "pack", False):
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (or smollm-135m; got --model "
-                         f"{args.model})")
+        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b or "
+                         f"granite-3.0-1b-a400m; got --model {args.model})")
     if not padding_on(args):
         raise ValueError("--pack needs --min_seq_len below --seq_len (documents have lengths in [--min_seq_len, --seq_len])")
     check_min_seq_len_args(args)
@@ -218,8 +232,8 @@ def check_fused_lm_loss_args(args) -> None:
     if not getattr(args, "fused_lm_loss", False):
         return
     if args.model not in CAUSAL_MODELS:
-        raise ValueError(f"--fused_lm_loss fuses a causal LM's head into its loss; it needs --model gpt2, smollm-135m or "
-                         f"qwen2.5-1.5b (got --model {args.model})")
+        raise ValueError(f"--fused_lm_loss fuses a causal LM's head into its loss; it needs --model gpt2, smollm-135m, "
+                         f"qwen2.5-1.5b or granite-3.0-1b-a400m (got --model {args.model})")
     if getattr(args, "loss", None) not in (None, "ce"):
         raise ValueError(f"--fused_lm_loss computes cross-entropy; it needs --loss ce (got --loss {args.loss})")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -228,6 +242,23 @@ def check_fused_lm_loss_args(args) -> None:
         if args.local_rank == -1 and getattr(args, "n_gpu", 1) > 1:
             raise ValueError("--fused_lm_loss does not run under single-process multi-GPU DataParallel; launch one process "
                              "per GPU (torchrun) or make one GPU visible")
+
+
+def check_moe_args(args) -> None:
+    """``--router_aux_loss_coef`` weights a mixture-of-experts model's load-balancing loss: it needs such a model and a
+    non-negative value.  The loss (on by default) reads statistics the MoE layers keep from their forward, which
+    single-process multi-GPU ``DataParallel`` leaves on its per-GPU replicas: that mode needs the loss turned off."""
+    coef = getattr(args, "router_aux_loss_coef", None)
+    if coef is not None and args.model not in MOE_MODELS:
+        raise ValueError(f"--router_aux_loss_coef weights a mixture-of-experts router's loss; it needs --model "
+                         f"{' or '.join(MOE_MODELS)} (got --model {args.model})")
+    if coef is not None and not coef >= 0:
+        raise ValueError(f"--router_aux_loss_coef must be >= 0, got {coef}")
+    if args.model in MOE_MODELS and coef != 0 and getattr(args, "device", None) is not None and args.device.type == "cuda" \
+            and args.local_rank == -1 and getattr(args, "n_gpu", 1) > 1:
+        raise ValueError(f"--model {args.model} with its router load-balancing loss does not run under single-process "
+                         f"multi-GPU DataParallel; launch one process per GPU (torchrun), make one GPU visible, or pass "
+                         f"--router_aux_loss_coef 0")
 
 
 def padding_on(args) -> bool:
@@ -258,12 +289,14 @@ def main(argv=None) -> int:
     kwargs = {"fp8": True} if args.fp8 else {}
     if args.fused_lm_loss:
         kwargs["fused_lm_loss"] = True
+    if args.router_aux_loss_coef is not None:
+        kwargs["router_aux_loss_coef"] = args.router_aux_loss_coef
     if padding_on(args):
         from ..data import SyntheticTokens
         kwargs["pad_token_id"] = SyntheticTokens.PAD_ID
         if args.pack and args.model == "gpt2":
             kwargs["bos_token_id"] = SyntheticTokens.BOS_ID
-        elif args.pack and args.model == "smollm-135m":
+        elif args.pack and args.model in ("smollm-135m", "granite-3.0-1b-a400m"):
             kwargs["bos_token_id"] = SyntheticTokens.LLAMA_BOS_ID
         elif args.pack and args.model == "qwen2.5-1.5b":
             kwargs["bos_token_id"] = SyntheticTokens.QWEN_BOS_ID

@@ -66,6 +66,11 @@ def build_dataset(args):
         return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=151936,
                                min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
                                causal=True, bos_token_id=SyntheticTokens.QWEN_BOS_ID)
+    if name == "granite-3.0-1b-a400m":                        # causal-LM rows over Granite's vocabulary; Granite's own start id,
+        # <|end_of_text|> = 0, is PAD_ID here, so packed documents start with LLAMA_BOS_ID (1) instead
+        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=49155,
+                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
+                               causal=True, bos_token_id=SyntheticTokens.LLAMA_BOS_ID)
     raise ValueError(f"no default dataset for model {name!r}")
 
 
@@ -74,13 +79,31 @@ def loss_kind(args) -> str:
     return getattr(args, "loss", None) or ("mse" if getattr(args, "model", "foo") == "foo" else "ce")
 
 
+class RouterAuxLoss:
+    """``criterion(out, y) + coef * model.router_aux_loss()``: a mixture-of-experts LM's training loss with its
+    load-balancing term, as Hugging Face's GraniteMoe reports it with ``output_router_logits=True``."""
+
+    def __init__(self, criterion, model: torch.nn.Module, coef: float):
+        self.criterion, self.coef = criterion, float(coef)
+        self._model = [model]                                  # not a submodule: the criterion owns no parameters
+
+    def __call__(self, out, y):
+        return self.criterion(out, y) + self.coef * self._model[0].router_aux_loss()
+
+
 def build_criterion(args, model: Optional[torch.nn.Module] = None):
-    """``--loss``'s criterion; with ``--fused_lm_loss`` the model's own head-plus-cross-entropy (``lm_head_loss``)."""
+    """``--loss``'s criterion; with ``--fused_lm_loss`` the model's own head-plus-cross-entropy (``lm_head_loss``).  A
+    model with ``config.router_aux_loss_coef > 0`` (mixture of experts) adds its load-balancing loss (``RouterAuxLoss``)."""
     if getattr(args, "fused_lm_loss", False):
         if model is None or not getattr(getattr(model, "config", None), "fused_lm_loss", False):
             raise ValueError("--fused_lm_loss needs a causal LM built with fused_lm_loss=True (it has lm_head_loss)")
-        return model.lm_head_loss()
-    return CrossEntropyLoss() if loss_kind(args) == "ce" else MSELoss()
+        criterion = model.lm_head_loss()
+    else:
+        criterion = CrossEntropyLoss() if loss_kind(args) == "ce" else MSELoss()
+    coef = getattr(getattr(model, "config", None), "router_aux_loss_coef", 0.0) if model is not None else 0.0
+    if coef > 0:
+        criterion = RouterAuxLoss(criterion, model, coef)
+    return criterion
 
 
 class Trainer:

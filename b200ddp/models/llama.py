@@ -11,15 +11,21 @@ position ids restarting in each) with ``LlamaConfig.bos_token_id``.  ``load_hf_s
 
 ``qwen2_5_1_5b`` is Qwen2.5-1.5B: the same blocks with a bias on the q | k | v projection (``attention_bias``), head dim
 128 (12 query heads over 2 K/V heads at hidden 1536), SwiGLU intermediate 8960, vocabulary 151936, rope theta 1e6, RMSNorm
-eps 1e-6 and tied embeddings: 1,543,714,304 parameters."""
+eps 1e-6 and tied embeddings: 1,543,714,304 parameters.
+
+``granite_3_0_1b_a400m`` is Granite-3.0-1B-A400M, a sparse mixture of experts: every block's SwiGLU is 32 experts of
+width 512 of which each token uses 8 (``ops.MoE``: native routing, expert sort and grouped wgmma GEMMs), 16 query heads
+over 8 K/V heads at hidden 1024, 24 layers, Granite's four multipliers and a vocabulary of 49155 padded to 49216:
+1,334,690,816 parameters.  ``load_hf_state_dict`` also reads ``transformers.GraniteMoeForCausalLM``'s state dicts."""
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 
 import torch
 import torch.nn as nn
 
-from ..ops import Linear, LinearCrossEntropyLoss, RMSNorm, causal_attention, document_bounds, linear, rotary, rotary_cos_sin, swiglu
+from ..ops import Linear, LinearCrossEntropyLoss, MoE, RMSNorm, causal_attention, document_bounds, linear, rotary, rotary_cos_sin, swiglu
 
 
 @dataclass
@@ -38,10 +44,32 @@ class LlamaConfig:
     pad_token_id: int | None = None  # right-padded input: length = non-pad count per row
     bos_token_id: int | None = None  # packed input: a document starts at each such id (and at 0), attention stays inside it
     fused_lm_loss: bool = False    # forward returns the final hidden states; ``lm_head_loss`` applies the head inside the loss
+    # sparse mixture of experts: with num_experts > 0 every block's SwiGLU is num_experts experts of width `intermediate`,
+    # experts_per_token of them per token; router_aux_loss_coef > 0 keeps the load-balancing statistics (router_aux_loss)
+    num_experts: int = 0
+    experts_per_token: int = 0
+    router_aux_loss_coef: float = 0.0
+    # Granite's multipliers (the defaults leave the model as it is, with no extra op): embedding output, attention scores
+    # (None = 1 / sqrt(head_dim)), both residual branches, and 1 / logits_scaling on the final hidden states
+    embedding_multiplier: float = 1.0
+    attention_multiplier: float | None = None
+    residual_multiplier: float = 1.0
+    logits_scaling: float = 1.0
+    pad_vocab_to: int = 1          # embedding / LM-head rows padded to a multiple of this (GPT-2's mechanism)
 
     @property
     def head_dim(self) -> int:
         return self.hidden // self.heads
+
+    @property
+    def padded_vocab(self) -> int:
+        m = max(1, self.pad_vocab_to)
+        return (self.vocab_size + m - 1) // m * m
+
+    @property
+    def q_scale(self) -> float:
+        """Factor on q that turns the attention kernels' 1 / sqrt(head_dim) into ``attention_multiplier``."""
+        return 1.0 if self.attention_multiplier is None else self.attention_multiplier * math.sqrt(self.head_dim)
 
 
 class LlamaBlock(nn.Module):
@@ -54,13 +82,21 @@ class LlamaBlock(nn.Module):
         self.qkv = Linear(c.hidden, (c.heads + 2 * c.kv_heads) * d, bias=c.attention_bias, fp8=c.fp8)
         self.o_proj = Linear(c.heads * d, c.hidden, bias=False, fp8=c.fp8)
         self.post_attention_layernorm = RMSNorm(c.hidden, eps=c.eps)
-        self.gate_up = Linear(c.hidden, 2 * c.intermediate, bias=False, fp8=c.fp8)   # gate | up
-        self.down_proj = Linear(c.intermediate, c.hidden, bias=False, fp8=c.fp8)
+        if c.num_experts > 0:
+            self.moe = MoE(c.hidden, c.intermediate, c.num_experts, c.experts_per_token, aux=c.router_aux_loss_coef > 0)
+        else:
+            self.gate_up = Linear(c.hidden, 2 * c.intermediate, bias=False, fp8=c.fp8)   # gate | up
+            self.down_proj = Linear(c.intermediate, c.hidden, bias=False, fp8=c.fp8)
+        self.q_scale, self.residual = c.q_scale, c.residual_multiplier
+
+    def _add(self, x, y):
+        return x + y if self.residual == 1.0 else torch.add(x, y, alpha=self.residual)
 
     def forward(self, x, bounds, position_ids, cos_sin):
-        qkv = rotary(self.qkv(self.input_layernorm(x)), position_ids, cos_sin, self.heads, self.kv_heads)
-        x = x + self.o_proj(causal_attention(qkv, bounds, self.heads, self.kv_heads))
-        return x + self.down_proj(swiglu(self.gate_up(self.post_attention_layernorm(x))))
+        qkv = rotary(self.qkv(self.input_layernorm(x)), position_ids, cos_sin, self.heads, self.kv_heads, self.q_scale)
+        x = self._add(x, self.o_proj(causal_attention(qkv, bounds, self.heads, self.kv_heads)))
+        h = self.post_attention_layernorm(x)
+        return self._add(x, self.moe(h) if hasattr(self, "moe") else self.down_proj(swiglu(self.gate_up(h))))
 
 
 class LlamaModel(nn.Module):
@@ -70,7 +106,14 @@ class LlamaModel(nn.Module):
         if c.hidden % c.heads or c.heads % c.kv_heads:
             raise ValueError(f"LlamaConfig: heads must divide hidden and kv_heads must divide heads, got hidden={c.hidden}, "
                              f"heads={c.heads}, kv_heads={c.kv_heads}")
-        self.embed_tokens = nn.Embedding(c.vocab_size, c.hidden)
+        if not (c.q_scale > 0 and math.frexp(c.q_scale)[0] == 0.5):
+            raise ValueError(f"LlamaConfig: attention_multiplier * sqrt(head_dim) must be a power of two (it scales q exactly in "
+                             f"bf16), got {c.attention_multiplier} * sqrt({c.head_dim})")
+        if c.num_experts > 0 and not 1 <= c.experts_per_token <= c.num_experts:
+            raise ValueError(f"LlamaConfig: experts_per_token must lie in [1, num_experts = {c.num_experts}], got {c.experts_per_token}")
+        if c.num_experts > 0 and c.fp8:
+            raise ValueError("LlamaConfig: fp8 covers dense block linears; the mixture-of-experts layers have no FP8 path")
+        self.embed_tokens = nn.Embedding(c.padded_vocab, c.hidden)
         self.layers = nn.ModuleList([LlamaBlock(c) for _ in range(c.layers)])
         self.norm = RMSNorm(c.hidden, eps=c.eps)
         self.register_buffer("cos_sin", rotary_cos_sin(c.max_position, c.head_dim, c.rope_theta), persistent=False)
@@ -100,6 +143,8 @@ class LlamaModel(nn.Module):
         bounds, position_ids = document_bounds(input_ids, c.bos_token_id, c.pad_token_id)
         position_ids = position_ids.to(torch.int32)
         x = self.embed_tokens(input_ids)
+        if c.embedding_multiplier != 1.0:
+            x = x * c.embedding_multiplier
         for layer in self.layers:
             x = layer(x, bounds, position_ids, self.cos_sin)
         return self.norm(x)
@@ -107,11 +152,22 @@ class LlamaModel(nn.Module):
 
 class LlamaForCausalLM(nn.Module):
     """Decoder + LM head tied to the token embedding (no bias); forward returns logits [B, S, vocab], or with
-    ``LlamaConfig.fused_lm_loss`` the final hidden states [B, S, hidden], to be scored by ``lm_head_loss()``."""
+    ``LlamaConfig.fused_lm_loss`` the final hidden states [B, S, hidden], to be scored by ``lm_head_loss()``.
+
+    With ``pad_vocab_to`` padding the vocabulary, the logits are [B, S, padded vocab] and the padded rows get a -1e4 logit
+    bias (a non-persistent buffer, as GPT-2's), so they take no probability.  ``logits_scaling`` multiplies the final
+    hidden states by 1 / logits_scaling before the head, in both paths; Hugging Face divides the logits instead, so the
+    two differ by bf16 rounding only."""
 
     def __init__(self, config: LlamaConfig | None = None):
         super().__init__()
         self.model = LlamaModel(config)
+        c = self.model.config
+        bias = None
+        if c.padded_vocab != c.vocab_size:
+            bias = torch.zeros(c.padded_vocab)
+            bias[c.vocab_size:] = -1e4
+        self.register_buffer("vocab_bias", bias, persistent=False)
 
     @property
     def config(self) -> LlamaConfig:
@@ -119,26 +175,59 @@ class LlamaForCausalLM(nn.Module):
 
     def forward(self, input_ids):
         h = self.model(input_ids)
-        return h if self.config.fused_lm_loss else linear(h, self.model.embed_tokens.weight)
+        if self.config.logits_scaling != 1.0:
+            h = h * (1.0 / self.config.logits_scaling)
+        if self.config.fused_lm_loss:
+            return h
+        bias = None if self.vocab_bias is None else self.vocab_bias.to(h.dtype)
+        return linear(h, self.model.embed_tokens.weight, bias)
 
     def lm_head_loss(self, ignore_index: int = -100) -> LinearCrossEntropyLoss:
-        """Criterion over ``forward``'s hidden states with ``fused_lm_loss``: the tied head, read from this model at every call."""
-        return LinearCrossEntropyLoss(lambda: (self.model.embed_tokens.weight, None), ignore_index)
+        """Criterion over ``forward``'s hidden states with ``fused_lm_loss``: the tied head (and the padded-vocabulary bias),
+        read from this model at every call."""
+        return LinearCrossEntropyLoss(lambda: (self.model.embed_tokens.weight, self.vocab_bias), ignore_index)
+
+    def router_aux_loss(self) -> torch.Tensor:
+        """Hugging Face's ``load_balancing_loss_func`` over every layer of the last forward (``attention_mask=None``): E times
+        the sum over experts of (fraction of token slots routed to the expert) x (mean router probability), both averaged over
+        all layers' tokens together.  Needs ``router_aux_loss_coef > 0``.  Takes the statistics out of the layers, so one
+        forward gives one aux loss: left behind, they would keep that forward's autograd graph (and its parameters' gradient
+        accumulators) alive into the next step, which a CUDA-graph capture cannot take."""
+        states = [layer.moe.aux_state for layer in self.model.layers]
+        if any(s is None for s in states):
+            raise RuntimeError("router_aux_loss needs a forward of a model built with num_experts > 0 and router_aux_loss_coef > 0, "
+                               "and takes that forward's statistics once")
+        for layer in self.model.layers:
+            layer.moe.aux_state = None
+        n = float(sum(s[2] for s in states))
+        probs = torch.stack([s[0] for s in states]).sum(0)
+        counts = torch.stack([s[1] for s in states]).sum(0).float()
+        return (counts * probs).sum() * (self.config.num_experts / (n * n))
 
     def load_hf_state_dict(self, hf: dict) -> None:
-        """Load a ``transformers.LlamaForCausalLM`` or ``transformers.Qwen2ForCausalLM`` state dict: q / k / v (weights, and
-        biases when the config has ``attention_bias``) and gate / up are concatenated into the fused projections, a tied
-        ``lm_head.weight`` is ignored."""
+        """Load a ``transformers.LlamaForCausalLM``, ``transformers.Qwen2ForCausalLM`` or ``transformers.GraniteMoeForCausalLM``
+        state dict: q / k / v (weights, and biases when the config has ``attention_bias``) and gate / up are concatenated into
+        the fused projections, GraniteMoe's ``block_sparse_moe`` router and expert weights are taken as they are, embedding
+        rows beyond the checkpoint's vocabulary are zero, and a tied ``lm_head.weight`` is ignored."""
         own = self.state_dict()
-        out = {"model.embed_tokens.weight": hf["model.embed_tokens.weight"], "model.norm.weight": hf["model.norm.weight"]}
+        emb = hf["model.embed_tokens.weight"]
+        if emb.shape[0] != own["model.embed_tokens.weight"].shape[0]:       # padded vocabulary: zero rows beyond the checkpoint's
+            emb = torch.cat([emb, emb.new_zeros(own["model.embed_tokens.weight"].shape[0] - emb.shape[0], emb.shape[1])])
+        out = {"model.embed_tokens.weight": emb, "model.norm.weight": hf["model.norm.weight"]}
         for i in range(self.config.layers):
             src, dst = f"model.layers.{i}.", f"model.layers.{i}."
             out[dst + "qkv.weight"] = torch.cat([hf[src + f"self_attn.{n}_proj.weight"] for n in "qkv"], 0)
             if self.config.attention_bias:
                 out[dst + "qkv.bias"] = torch.cat([hf[src + f"self_attn.{n}_proj.bias"] for n in "qkv"], 0)
             out[dst + "o_proj.weight"] = hf[src + "self_attn.o_proj.weight"]
-            out[dst + "gate_up.weight"] = torch.cat([hf[src + "mlp.gate_proj.weight"], hf[src + "mlp.up_proj.weight"]], 0)
-            out[dst + "down_proj.weight"] = hf[src + "mlp.down_proj.weight"]
+            if self.config.num_experts > 0:
+                moe = src + "block_sparse_moe."
+                out[dst + "moe.router.weight"] = hf[moe + "router.layer.weight"]
+                out[dst + "moe.w_gate_up"] = hf[moe + "input_linear.weight"]
+                out[dst + "moe.w_down"] = hf[moe + "output_linear.weight"]
+            else:
+                out[dst + "gate_up.weight"] = torch.cat([hf[src + "mlp.gate_proj.weight"], hf[src + "mlp.up_proj.weight"]], 0)
+                out[dst + "down_proj.weight"] = hf[src + "mlp.down_proj.weight"]
             for n in ("input_layernorm", "post_attention_layernorm"):
                 out[dst + f"{n}.weight"] = hf[src + f"{n}.weight"]
         self.load_state_dict({k: v.to(own[k].dtype).contiguous() for k, v in out.items()}, strict=True)
@@ -160,3 +249,18 @@ def qwen2_5_1_5b(fp8: bool = False, pad_token_id: int | None = None, bos_token_i
     return LlamaForCausalLM(LlamaConfig(vocab_size=151936, max_position=32768, hidden=1536, layers=28, heads=12, kv_heads=2,
                                         intermediate=8960, eps=1e-6, rope_theta=1e6, attention_bias=True, fp8=fp8,
                                         pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))
+
+
+def granite_3_0_1b_a400m(pad_token_id: int | None = None, bos_token_id: int | None = None, fused_lm_loss: bool = False,
+                         router_aux_loss_coef: float = 0.001) -> nn.Module:
+    """Granite-3.0-1B-A400M with its tied LM head (4096 positions): 24 blocks of grouped-query attention (16 query heads
+    over 8 K/V heads, head dim 64) and a mixture of 32 SwiGLU experts of width 512, 8 per token; embedding multiplier 12,
+    attention multiplier 1/64, residual multiplier 0.22, logits scaling 6; vocabulary 49155 padded to 49216.
+    ``router_aux_loss_coef`` (transformers' default 0.001; 0 turns it off) weights ``router_aux_loss`` in the training
+    loss.  ``pad_token_id``, ``bos_token_id`` and ``fused_lm_loss`` as for ``smollm_135m``."""
+    return LlamaForCausalLM(LlamaConfig(vocab_size=49155, max_position=4096, hidden=1024, layers=24, heads=16, kv_heads=8,
+                                        intermediate=512, eps=1e-6, rope_theta=10000.0, num_experts=32, experts_per_token=8,
+                                        router_aux_loss_coef=router_aux_loss_coef, embedding_multiplier=12.0,
+                                        attention_multiplier=0.015625, residual_multiplier=0.22, logits_scaling=6.0,
+                                        pad_vocab_to=64, pad_token_id=pad_token_id, bos_token_id=bos_token_id,
+                                        fused_lm_loss=fused_lm_loss))

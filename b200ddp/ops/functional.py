@@ -580,7 +580,7 @@ def rotary_cos_sin(max_position: int, head_dim: int = ATTENTION_HEAD_DIM, theta:
 
 
 def _rotary_reference(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor, heads: int, kv_heads: int,
-                      inverse: bool = False) -> torch.Tensor:
+                      inverse: bool = False, q_scale: float = 1.0) -> torch.Tensor:
     B, S, Wd = qkv.shape
     d = Wd // (heads + 2 * kv_heads)
     half = d // 2
@@ -593,38 +593,47 @@ def _rotary_reference(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: to
     qk, v = qkv.to(ct).split([(heads + kv_heads) * d, kv_heads * d], dim=-1)
     x = qk.reshape(B, S, heads + kv_heads, d)
     lo, hi = x[..., :half], x[..., half:]
-    out = torch.cat([lo * cos - hi * sin, hi * cos + lo * sin], -1).reshape(B, S, -1)
-    return torch.cat([out, v], -1).to(qkv.dtype)
+    out = torch.cat([lo * cos - hi * sin, hi * cos + lo * sin], -1)
+    if q_scale != 1.0:
+        out = torch.cat([out[:, :, :heads] * q_scale, out[:, :, heads:]], 2)
+    return torch.cat([out.reshape(B, S, -1), v], -1).to(qkv.dtype)
 
 
 class _Rotary(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, position_ids, cos_sin, heads, kv_heads):
-        ctx.heads, ctx.kv_heads = heads, kv_heads
+    def forward(ctx, qkv, position_ids, cos_sin, heads, kv_heads, q_scale):
+        ctx.heads, ctx.kv_heads, ctx.q_scale = heads, kv_heads, q_scale
         if qkv.is_cuda:
             B, S, Wd = qkv.shape
             pos = position_ids.to(device=qkv.device, dtype=torch.int32).reshape(-1).contiguous()
             table = cos_sin.to(device=qkv.device, dtype=torch.float32).contiguous()
             ctx.save_for_backward(pos, table)
-            return _C().rotary(qkv.reshape(B * S, Wd).contiguous(), pos, table, heads, kv_heads, False).view(B, S, Wd)
+            return _C().rotary(qkv.reshape(B * S, Wd).contiguous(), pos, table, heads, kv_heads, False, q_scale).view(B, S, Wd)
         ctx.save_for_backward(position_ids, cos_sin)
-        return _rotary_reference(qkv, position_ids, cos_sin, heads, kv_heads)
+        return _rotary_reference(qkv, position_ids, cos_sin, heads, kv_heads, q_scale=q_scale)
 
     @staticmethod
     def backward(ctx, dy):
         pos, table = ctx.saved_tensors
         if dy.is_cuda:
             B, S, Wd = dy.shape
-            dx = _C().rotary(dy.reshape(B * S, Wd).to(torch.bfloat16).contiguous(), pos, table, ctx.heads, ctx.kv_heads, True)
-            return dx.view(B, S, Wd), None, None, None, None
-        return _rotary_reference(dy, pos, table, ctx.heads, ctx.kv_heads, inverse=True), None, None, None, None
+            dx = _C().rotary(dy.reshape(B * S, Wd).to(torch.bfloat16).contiguous(), pos, table, ctx.heads, ctx.kv_heads, True, ctx.q_scale)
+            return dx.view(B, S, Wd), None, None, None, None, None
+        return (_rotary_reference(dy, pos, table, ctx.heads, ctx.kv_heads, inverse=True, q_scale=ctx.q_scale),
+                None, None, None, None, None)
 
 
-def rotary(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor, heads: int, kv_heads: int) -> torch.Tensor:
+def rotary(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor, heads: int, kv_heads: int,
+           q_scale: float = 1.0) -> torch.Tensor:
     """Rotary position embedding (Hugging Face's ``rotate_half`` convention: element i of a head pairs with i + d/2) of
     the query and key heads of qkv [B, S, (heads + 2 * kv_heads) * d]; the value heads pass through.  position_ids
     integer [B, S] (clamped to the table), cos_sin fp32 [max_position, 2, d / 2] (``rotary_cos_sin``).  Out of place.  On
-    CUDA: bf16 and d = 64 or 128, else ``ValueError``; positions stay on the device (CUDA-graph safe)."""
+    CUDA: bf16 and d = 64 or 128, else ``ValueError``; positions stay on the device (CUDA-graph safe).
+
+    ``q_scale``, a positive power of two (exact in bf16, else ``ValueError``), also multiplies the query heads: it folds
+    an attention score scale other than 1 / sqrt(d) (Granite's ``attention_multiplier``) into q."""
+    if not (q_scale > 0 and math.frexp(q_scale)[0] == 0.5):
+        raise ValueError(f"rotary: q_scale must be a positive power of two (exact in bf16), got {q_scale}")
     if qkv.dim() != 3 or heads < 1 or kv_heads < 1 or qkv.shape[-1] % (heads + 2 * kv_heads) or \
             (qkv.shape[-1] // (heads + 2 * kv_heads)) % 2:
         raise ValueError(f"rotary needs qkv [B, S, (heads + 2 * kv_heads) * d] with an even d, got {tuple(qkv.shape)} for "
@@ -637,7 +646,7 @@ def rotary(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor,
     if qkv.is_cuda and (qkv.dtype != torch.bfloat16 or d not in (ATTENTION_HEAD_DIM, CAUSAL_WIDE_HEAD_DIM)):
         raise ValueError(f"rotary on CUDA needs bf16 qkv and head dim {ATTENTION_HEAD_DIM} or {CAUSAL_WIDE_HEAD_DIM}, got {qkv.dtype}, "
                          f"head dim {d}")
-    return _Rotary.apply(qkv, position_ids, cos_sin, heads, kv_heads)
+    return _Rotary.apply(qkv, position_ids, cos_sin, heads, kv_heads, float(q_scale))
 
 
 def _rms_norm_reference(x: torch.Tensor, weight: torch.Tensor, eps: float) -> torch.Tensor:
@@ -705,6 +714,159 @@ def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
             raise ValueError(f"swiglu on CUDA needs bf16 and I % 8 == 0, got {gate_up.dtype} {tuple(gate_up.shape)}")
         return _SwiGLU.apply(gate_up)
     return _swiglu_reference(gate_up)
+
+
+# ------------------------------------------------------------------------------------------------
+# Mixture of experts (csrc/moe.cu routing / permutation / combine, csrc/gemm_wgmma.cu grouped GEMMs)
+# ------------------------------------------------------------------------------------------------
+MOE_MAX_EXPERTS = 64
+MOE_MAX_TOP_K = 8
+MOE_ALIGN = 128            # each expert's segment of the permuted rows starts at a multiple of this
+
+
+def moe_capacity(tokens: int, experts: int, top_k: int) -> int:
+    """Rows of the permuted buffers: every expert's segment padded to a multiple of 128, for any routing."""
+    return (tokens * top_k + experts * (MOE_ALIGN - 1) + MOE_ALIGN - 1) // MOE_ALIGN * MOE_ALIGN
+
+
+def moe_route_reference(logits: torch.Tensor, top_k: int):
+    """(ids [T, k] long, gates [T, k] fp32): the top-k logits of each row, ties to the lower expert (a stable sort), and
+    the softmax over them in fp32.  Differentiable in the gates."""
+    ids = torch.sort(logits.float(), dim=-1, descending=True, stable=True).indices[:, :top_k]
+    return ids, torch.softmax(logits.float().gather(1, ids), dim=-1)
+
+
+def moe_permute_reference(ids: torch.Tensor, experts: int):
+    """The expert-sorted layout the native permutation writes, from ids [T, k]: (counts [E], offsets [E + 1] (segment
+    starts, multiples of 128), fwd_map [capacity] (row -> t * k + j, -1 in padding), inv_map [T, k] (t * k + j -> row),
+    tile_expert [capacity / 128] (-1 for unused tiles)), all int32.  Within an expert, rows keep the order of t * k + j."""
+    T, k = ids.shape
+    flat = ids.reshape(-1).long()
+    counts = torch.bincount(flat, minlength=experts)
+    padded = (counts + MOE_ALIGN - 1) // MOE_ALIGN * MOE_ALIGN
+    offsets = torch.cat([padded.new_zeros(1), padded.cumsum(0)])
+    cap = moe_capacity(T, experts, k)
+    order = torch.sort(flat, stable=True).indices                     # assignments grouped by expert, in order
+    starts = torch.cat([counts.new_zeros(1), counts.cumsum(0)])[:-1]
+    sorted_e = flat[order]
+    rows = offsets[sorted_e] + torch.arange(T * k) - starts[sorted_e]
+    fwd = torch.full((cap,), -1, dtype=torch.long)
+    fwd[rows] = order
+    inv = torch.empty(T * k, dtype=torch.long)
+    inv[order] = rows
+    tile0 = torch.arange(cap // MOE_ALIGN) * MOE_ALIGN
+    owner = ((tile0[:, None] >= offsets[None, :-1]) & (tile0[:, None] < offsets[None, 1:])).int()
+    tiles = torch.where(owner.any(1), owner.argmax(1), -1)
+    return tuple(t.to(torch.int32) for t in (counts, offsets, fwd, inv.view(T, k), tiles))
+
+
+def _moe_reference(x, router_weight, w_gate_up, w_down, top_k, aux=False, routing_logits=None):
+    """Hugging Face's ``GraniteMoeMoE`` with the stable tie rule: the router logits in x's dtype, then in fp32; top-k and
+    a softmax over the chosen logits in fp32, rounded to x's dtype; each expert a SwiGLU over its rows (w_gate_up [E, 2I,
+    H], gate | up, and w_down [E, H, I]); the k gated outputs of a token summed in fp32 in slot order.  With ``aux`` also
+    returns each expert's sum of full-softmax probabilities (fp32, differentiable) and its token count (int32).
+    ``routing_logits`` [T, E], if given, decides which experts each token takes (the gates still come from this call's
+    logits): an fp32 reference then routes exactly like the bf16 run it checks."""
+    H = x.shape[-1]
+    E = router_weight.shape[0]
+    x2 = x.reshape(-1, H)
+    T = x2.shape[0]
+    logits = F.linear(x2, router_weight).float()
+    ids = moe_route_reference(logits if routing_logits is None else routing_logits, top_k)[0]
+    gates = torch.softmax(logits.gather(1, ids), dim=-1).to(x.dtype)
+    slots = x2.new_zeros(T, top_k, H)
+    for e in range(E):
+        tok, slot = (ids == e).nonzero(as_tuple=True)
+        if tok.numel() == 0:
+            continue
+        g, u = F.linear(x2[tok], w_gate_up[e]).chunk(2, dim=-1)
+        y = F.linear(F.silu(g) * u, w_down[e])
+        slots = slots.index_put((tok, slot), y * gates[tok, slot, None])
+    out = slots.float().sum(1).to(x.dtype).view(x.shape)
+    if not aux:
+        return out
+    return out, torch.softmax(logits, dim=-1).sum(0), torch.bincount(ids.reshape(-1), minlength=E).to(torch.int32)
+
+
+class _MoE(torch.autograd.Function):
+    """CUDA body of ``moe``: route, permute, gather, grouped gate|up GEMM, SwiGLU, grouped down GEMM, combine.  The backward
+    gathers the permuted input again from x rather than keeping it (one more memory-bound pass instead of [capacity, H]
+    per layer alive until the backward).  No host synchronisation: every shape follows from (T, E, k)."""
+
+    @staticmethod
+    def forward(ctx, x2, logits, w_gate_up, w_down, top_k, aux):
+        C = _C()
+        ctx.set_materialize_grads(False)
+        E = w_gate_up.shape[0]
+        ids, gates, probsum = C.moe_route(logits, top_k, aux)
+        counts, offsets, fwd, inv, tiles = C.moe_permute(ids, E)
+        gu = C.moe_gemm(C.moe_gather(x2, fwd, top_k), w_gate_up, tiles, False)
+        h = C.swiglu_fwd(gu)
+        y = C.moe_gemm(h, w_down, tiles, False)
+        out = C.moe_combine(y, inv, gates)
+        ctx.save_for_backward(x2, logits, w_gate_up, w_down, ids, gates, offsets, fwd, inv, tiles, gu, h, y)
+        ctx.top_k, ctx.aux = top_k, aux
+        if not aux:
+            return out
+        ctx.mark_non_differentiable(counts)
+        return out, probsum, counts
+
+    @staticmethod
+    def backward(ctx, dout, dprobsum=None, _dcounts=None):
+        C = _C()
+        x2, logits, w_gate_up, w_down, ids, gates, offsets, fwd, inv, tiles, gu, h, y = ctx.saved_tensors
+        if dout is None:
+            dout = torch.zeros_like(x2)
+        dy, dgates = C.moe_combine_bwd(dout.to(torch.bfloat16).contiguous(), y, fwd, gates)
+        dw_down = C.moe_gemm_wgrad(dy, h, offsets) if ctx.needs_input_grad[3] else None
+        dgu = C.swiglu_bwd(C.moe_gemm(dy, w_down, tiles, True), gu)
+        dx = dw_gu = None
+        if ctx.needs_input_grad[0]:
+            dx = C.moe_combine(C.moe_gemm(dgu, w_gate_up, tiles, True), inv, None)
+        if ctx.needs_input_grad[2]:
+            dw_gu = C.moe_gemm_wgrad(dgu, C.moe_gather(x2, fwd, ctx.top_k), offsets)
+        dp = dprobsum.float().contiguous() if ctx.aux and dprobsum is not None else None
+        dlogits = C.moe_router_bwd(logits, ids, dgates, dp) if ctx.needs_input_grad[1] else None
+        return dx, dlogits, dw_gu, dw_down, None, None
+
+
+def moe(x: torch.Tensor, router_weight: torch.Tensor, w_gate_up: torch.Tensor, w_down: torch.Tensor, top_k: int,
+        aux: bool = False):
+    """Sparse mixture-of-experts SwiGLU layer (Hugging Face's ``GraniteMoeMoE``), dropless: x [..., H], router_weight
+    [E, H], w_gate_up [E, 2I, H] (rows gate | up), w_down [E, H, I].  Each token goes to its top_k experts by router logit
+    (ties to the lower expert), weighted by the softmax over those k logits in fp32 rounded to x's dtype; the k outputs
+    are summed in fp32 in slot order.  Returns the output [..., H]; with ``aux=True`` also each expert's sum over tokens
+    of the full router softmax (fp32 [E], differentiable: the load-balancing loss) and its token count (int32 [E]).
+
+    On CUDA (bf16; E <= 64 and a multiple of 8, 1 <= top_k <= min(E, 8), H and I multiples of 64, tokens a multiple of
+    8, else ``ValueError``): native routing, a stable expert sort into 128-aligned segments, grouped wgmma GEMMs and a
+    gather-based combine; deterministic, no atomics and no host synchronisation (CUDA-graph safe).  CPU: ``_moe_reference``."""
+    H = x.shape[-1] if x.dim() >= 1 else -1
+    E = router_weight.shape[0] if router_weight.dim() == 2 else -1
+    if router_weight.dim() != 2 or router_weight.shape[1] != H or w_gate_up.dim() != 3 or w_down.dim() != 3 or \
+            w_gate_up.shape[0] != E or w_down.shape[0] != E or w_gate_up.shape[2] != H or w_gate_up.shape[1] % 2 or \
+            tuple(w_down.shape[1:]) != (H, w_gate_up.shape[1] // 2):
+        raise ValueError(f"moe needs x [..., H], router_weight [E, H], w_gate_up [E, 2I, H] and w_down [E, H, I], got x "
+                         f"{tuple(x.shape)}, router {tuple(router_weight.shape)}, gate_up {tuple(w_gate_up.shape)}, down "
+                         f"{tuple(w_down.shape)}")
+    if not 1 <= top_k <= min(E, MOE_MAX_TOP_K):
+        raise ValueError(f"moe needs 1 <= top_k <= min(experts, {MOE_MAX_TOP_K}), got top_k={top_k} with {E} experts")
+    if not x.is_cuda:
+        return _moe_reference(x, router_weight, w_gate_up, w_down, top_k, aux)
+    I = w_down.shape[2]
+    T = x.numel() // H
+    if any(t.dtype != torch.bfloat16 for t in (x, router_weight, w_gate_up, w_down)):
+        raise ValueError(f"moe on CUDA needs bf16 x and weights, got {x.dtype}, {router_weight.dtype}, {w_gate_up.dtype}, {w_down.dtype}")
+    if E > MOE_MAX_EXPERTS or E % 8 or H % 64 or I % 64 or T == 0 or T % 8:
+        raise ValueError(f"moe on CUDA needs E <= {MOE_MAX_EXPERTS} and a multiple of 8, H and I multiples of 64 and a positive "
+                         f"token count that is a multiple of 8, got E={E}, H={H}, I={I}, tokens={T}")
+    x2 = x.reshape(T, H).contiguous()
+    logits = linear(x2, router_weight)                               # bf16 [T, E] on the wgmma GEMM, as Hugging Face's router
+    outs = _MoE.apply(x2, logits, w_gate_up.contiguous(), w_down.contiguous(), int(top_k), bool(aux))
+    if not aux:
+        return outs.view(x.shape)
+    out, probsum, counts = outs
+    return out.view(x.shape), probsum, counts
 
 
 # ------------------------------------------------------------------------------------------------

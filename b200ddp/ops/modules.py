@@ -43,6 +43,35 @@ class Linear(nn.Module):
                 + (", fp8=True" if self.fp8 else ""))
 
 
+class MoE(nn.Module):
+    """Sparse mixture-of-experts SwiGLU feed-forward (``Fn.moe``): a bias-free router ``Linear(hidden, experts)`` and the
+    expert weights ``w_gate_up`` [E, 2I, H] (rows gate | up) and ``w_down`` [E, H, I], laid out like Hugging Face's
+    GraniteMoe ``input_linear`` / ``output_linear``.  With ``aux=True`` every forward leaves the load-balancing statistics
+    in ``aux_state``: (each expert's sum of router probabilities, fp32 [E] and differentiable; its token count, int32 [E];
+    the number of tokens)."""
+
+    def __init__(self, hidden: int, intermediate: int, experts: int, top_k: int, aux: bool = False):
+        super().__init__()
+        self.top_k, self.aux = top_k, aux
+        self.router = Linear(hidden, experts, bias=False)
+        self.w_gate_up = nn.Parameter(torch.empty(experts, 2 * intermediate, hidden))
+        self.w_down = nn.Parameter(torch.empty(experts, hidden, intermediate))
+        nn.init.normal_(self.w_gate_up, std=0.02)
+        nn.init.normal_(self.w_down, std=0.02)
+        self.aux_state = None
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if not self.aux:
+            return Fn.moe(x, self.router.weight, self.w_gate_up, self.w_down, self.top_k)
+        out, probsum, counts = Fn.moe(x, self.router.weight, self.w_gate_up, self.w_down, self.top_k, aux=True)
+        self.aux_state = (probsum, counts, x.numel() // x.shape[-1])
+        return out
+
+    def extra_repr(self) -> str:
+        return (f"experts={self.w_gate_up.shape[0]}, top_k={self.top_k}, hidden={self.w_gate_up.shape[2]}, "
+                f"intermediate={self.w_down.shape[2]}, aux={self.aux}")
+
+
 class Conv2dTC(nn.Conv2d):
     """Bias-free ``nn.Conv2d`` (same parameter name, shape and init, so checkpoints and DDP bucket layouts are unchanged)
     whose stride-1 1x1 / 3x3 instances run forward, data gradient and (where it wins) weight gradient on the hand-written

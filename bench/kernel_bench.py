@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,conv,bn,sgd,adamw,ln,xent,lmloss,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,conv,bn,sgd,adamw,ln,xent,lmloss,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -622,6 +622,81 @@ def main():
                     ms = timeit(lambda: C_.lm_loss_bwd(h.detach(), w.detach(), tt, None, lse, rl, g1, -100, sl), args.iters)
                     record(f"lm-loss qwen bwd slice {sl}", ms, flops=3 * gemm, note=f"dlogits buffer {N * sl * 2 / 1e6:.0f} MB")
             del h, w
+
+    if "moe" in want:
+        # Granite-3.0-1B-A400M's MoE layer at batch 8 x 2048: T = 16384 tokens, k = 8 of E = 32 experts, H = 1024, I = 512.
+        # TFLOP/s count the routed rows only (T * k), not the padding of the 128-aligned segments.  Baselines: torch._grouped_mm
+        # on the same permuted rows and offsets, and our dense GEMM over the same total M with one weight.  Uniform routing
+        # (random logits) and skewed routing (a bias falling by 0.25 per expert index).
+        print(f"moe on {card()}", flush=True)
+        T, k, E, H, I = 16384, 8, 32, 1024, 512
+        R = T * k
+        gen = torch.Generator(device=dev).manual_seed(0)
+        x = torch.randn(T, H, device=dev, generator=gen).to(torch.bfloat16)
+        wgu = (torch.randn(E, 2 * I, H, device=dev, generator=gen) * 0.02).to(torch.bfloat16)
+        wd = (torch.randn(E, H, I, device=dev, generator=gen) * 0.02).to(torch.bfloat16)
+        for routing in ("uniform", "skewed"):
+            logits = torch.randn(T, E, device=dev, generator=gen)
+            if routing == "skewed":
+                logits = logits - 0.25 * torch.arange(E, device=dev)
+            logits = logits.to(torch.bfloat16)
+            ids, gates, _ = C.moe_route(logits, k, True)
+            counts, offsets, fwd, inv, tiles = C.moe_permute(ids, E)
+            cap = fwd.numel()
+            c = counts.tolist()
+            print(f"  {routing}: rows per expert min {min(c)} max {max(c)}, {int(offsets[-1])} of {cap} permuted rows used", flush=True)
+            xp = C.moe_gather(x, fwd, k)
+            gu = C.moe_gemm(xp, wgu, tiles, False)
+            h = C.swiglu_fwd(gu)
+            y = C.moe_gemm(h, wd, tiles, False)
+            dy = torch.randn(cap, H, device=dev, generator=gen).to(torch.bfloat16)
+            dgu = torch.randn(cap, 2 * I, device=dev, generator=gen).to(torch.bfloat16)
+            ends = offsets[1:].contiguous()
+
+            def grouped(tag, ours, flops, lib, lib_note):
+                lib_ms = None
+                note = ""
+                try:
+                    lib_ms = timeit(lib, args.iters)
+                    note = f"lib = {lib_note}"
+                except Exception as err:                          # report the baseline as missing, never substitute it
+                    note = f"{lib_note} did not run: {type(err).__name__}: {str(err).splitlines()[0][:120]}"
+                record(f"moe {routing} {tag}", timeit(ours, args.iters), flops=flops, lib_ms=lib_ms, note=note)
+
+            f_gu, f_dn = 2.0 * R * 2 * I * H, 2.0 * R * H * I
+            grouped("fwd gate_up", lambda: C.moe_gemm(xp, wgu, tiles, False), f_gu,
+                    lambda: torch._grouped_mm(xp, wgu.transpose(1, 2), offs=ends), "torch._grouped_mm")
+            grouped("fwd down", lambda: C.moe_gemm(h, wd, tiles, False), f_dn,
+                    lambda: torch._grouped_mm(h, wd.transpose(1, 2), offs=ends), "torch._grouped_mm")
+            grouped("dgrad gate_up", lambda: C.moe_gemm(dgu, wgu, tiles, True), f_gu,
+                    lambda: torch._grouped_mm(dgu, wgu, offs=ends), "torch._grouped_mm")
+            grouped("dgrad down", lambda: C.moe_gemm(dy, wd, tiles, True), f_dn,
+                    lambda: torch._grouped_mm(dy, wd, offs=ends), "torch._grouped_mm")
+            grouped("wgrad gate_up", lambda: C.moe_gemm_wgrad(dgu, xp, offsets), f_gu,
+                    lambda: torch._grouped_mm(dgu.t(), xp, offs=ends), "torch._grouped_mm")
+            grouped("wgrad down", lambda: C.moe_gemm_wgrad(dy, h, offsets), f_dn,
+                    lambda: torch._grouped_mm(dy.t(), h, offs=ends), "torch._grouped_mm")
+            if routing == "uniform":                              # our dense GEMM over the same total M, one weight
+                a, b = xp[:R].contiguous(), wgu[0].contiguous()
+                record(f"moe dense gemm_nt {R}x{2 * I}x{H}", timeit(lambda: C.gemm(a, b, None, False, False, 0, False, None),
+                                                                     args.iters), flops=f_gu, note="dense reference at equal M")
+            # memory-bound passes: bytes each kernel must move
+            dout = torch.randn(T, H, device=dev, generator=gen).to(torch.bfloat16)
+            dgates = torch.randn(T, k, device=dev, generator=gen)
+            dprob = torch.randn(E, device=dev, generator=gen)
+            record(f"moe {routing} router fwd (+aux sums)", timeit(lambda: C.moe_route(logits, k, True), args.iters),
+                   bytes_=T * E * 2 + T * k * (4 + 2))
+            record(f"moe {routing} router bwd", timeit(lambda: C.moe_router_bwd(logits, ids, dgates, dprob), args.iters),
+                   bytes_=T * E * 2 * 2 + T * k * (4 + 4))
+            record(f"moe {routing} permute (3 kernels + memset)", timeit(lambda: C.moe_permute(ids, E), args.iters),
+                   bytes_=R * 4 * 2 + cap * 4 + R * 4, note="bytes: ids read twice, both row maps written")
+            record(f"moe {routing} gather", timeit(lambda: C.moe_gather(x, fwd, k), args.iters),
+                   bytes_=R * H * 2 + cap * H * 2 + cap * 4)
+            record(f"moe {routing} combine", timeit(lambda: C.moe_combine(y, inv, gates), args.iters),
+                   bytes_=R * H * 2 + T * H * 2 + R * (4 + 2))
+            record(f"moe {routing} combine bwd", timeit(lambda: C.moe_combine_bwd(dout, y, fwd, gates), args.iters),
+                   bytes_=R * H * 2 * 2 + cap * H * 2 + R * (4 + 2 + 4), note="dout read once per routed row")
+            del xp, gu, h, y, dy, dgu
 
     if "mse" in want:
         n = 64 * 1024 * 1024
