@@ -847,6 +847,50 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return y;
   }, py::arg("x"), py::arg("position_ids"), py::arg("cos_sin"), py::arg("heads"), py::arg("kv_heads"), py::arg("backward") = false,
      py::arg("q_scale") = 1.0);
+  // Qwen3's per-head q / k RMSNorm + rotary, d = 128: (y, rstd fp32 [rows, heads + kv_heads]) = fwd(qkv, wq, wk, ...);
+  // (dqkv, dwq, dwk) = bwd(dy, qkv, rstd, wq, wk, ...) with qkv the forward's input
+  auto qk_norm_check = [](const char* name, at::Tensor x, at::Tensor wq, at::Tensor wk, at::Tensor pos, at::Tensor table, int heads,
+                          int kv_heads) {
+    check_cuda(x, "x"); check_cuda(wq, "q_weight"); check_cuda(wk, "k_weight"); check_cuda(pos, "position_ids"); check_cuda(table, "cos_sin");
+    TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == 2 && table.size(2) == 64,
+                name, ": cos_sin must be contiguous fp32 [max_position, 2, 64]");
+    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous() && heads >= 1 && kv_heads >= 1 &&
+                x.size(1) == (int64_t)(heads + 2 * kv_heads) * 128, name, ": x must be contiguous bf16 [rows, (heads + 2*kv_heads)*128]");
+    for (const at::Tensor& w : {wq, wk})
+      TORCH_CHECK(w.scalar_type() == at::kBFloat16 && w.is_contiguous() && w.numel() == 128 && w.device() == x.device(), name,
+                  ": q_weight and k_weight must be contiguous bf16 [128] on x's device");
+    TORCH_CHECK(pos.scalar_type() == at::kInt && pos.is_contiguous() && pos.numel() == x.size(0), name, ": position_ids must be int32 [rows]");
+  };
+  m.def("qk_norm_rotary_fwd", [qk_norm_check](at::Tensor x, at::Tensor wq, at::Tensor wk, at::Tensor pos, at::Tensor table, int heads,
+                                              int kv_heads, double eps) {
+    qk_norm_check("qk_norm_rotary_fwd", x, wq, wk, pos, table, heads, kv_heads);
+    c10::cuda::CUDAGuard guard(x.device());
+    at::Tensor y = at::empty_like(x);
+    at::Tensor rstd = at::empty({x.size(0), heads + kv_heads}, x.options().dtype(at::kFloat));
+    launch_qk_norm_rotary_fwd(x.data_ptr(), wq.data_ptr(), wk.data_ptr(), pos.data_ptr<int>(), table.data_ptr<float>(), (int)table.size(0),
+                              (size_t)x.size(0), heads, kv_heads, 128, (float)eps, y.data_ptr(), rstd.data_ptr<float>(), cur_stream());
+    return std::make_tuple(y, rstd);
+  }, py::arg("x"), py::arg("q_weight"), py::arg("k_weight"), py::arg("position_ids"), py::arg("cos_sin"), py::arg("heads"),
+     py::arg("kv_heads"), py::arg("eps"));
+  m.def("qk_norm_rotary_bwd", [qk_norm_check](at::Tensor dy, at::Tensor x, at::Tensor rstd, at::Tensor wq, at::Tensor wk, at::Tensor pos,
+                                              at::Tensor table, int heads, int kv_heads) {
+    qk_norm_check("qk_norm_rotary_bwd", x, wq, wk, pos, table, heads, kv_heads);
+    check_cuda(dy, "dy"); check_cuda(rstd, "rstd");
+    TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && dy.is_contiguous() && dy.sizes() == x.sizes() && dy.device() == x.device(),
+                "qk_norm_rotary_bwd: dy must be contiguous bf16 shaped like x");
+    TORCH_CHECK(rstd.scalar_type() == at::kFloat && rstd.is_contiguous() && rstd.device() == x.device() &&
+                rstd.numel() == x.size(0) * (int64_t)(heads + kv_heads), "qk_norm_rotary_bwd: rstd must be fp32 [rows, heads + kv_heads]");
+    c10::cuda::CUDAGuard guard(x.device());
+    const int parts = qk_norm_rotary_partials((size_t)x.size(0));
+    at::Tensor dx = at::empty_like(x);
+    at::Tensor partial = at::empty({2, parts, 128}, x.options().dtype(at::kFloat));
+    at::Tensor dwq = at::empty_like(wq), dwk = at::empty_like(wk);
+    launch_qk_norm_rotary_bwd(dy.data_ptr(), x.data_ptr(), rstd.data_ptr<float>(), wq.data_ptr(), wk.data_ptr(), pos.data_ptr<int>(),
+                              table.data_ptr<float>(), (int)table.size(0), (size_t)x.size(0), heads, kv_heads, 128, dx.data_ptr(),
+                              partial.data_ptr<float>(), dwq.data_ptr(), dwk.data_ptr(), cur_stream());
+    return std::make_tuple(dx, dwq, dwk);
+  }, py::arg("dy"), py::arg("x"), py::arg("rstd"), py::arg("q_weight"), py::arg("k_weight"), py::arg("position_ids"), py::arg("cos_sin"),
+     py::arg("heads"), py::arg("kv_heads"));
   auto aligned32 = [](at::Tensor t) { return (reinterpret_cast<uintptr_t>(t.data_ptr()) & 31) != 0 ? t.clone() : t; };
   m.def("rmsnorm_fwd", [aligned32](at::Tensor x, at::Tensor gamma, double eps) {
     check_cuda(x, "x"); check_cuda(gamma, "gamma");

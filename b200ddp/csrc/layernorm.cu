@@ -439,6 +439,13 @@ LnBwdGeometry ln_bwd_geometry(int rows, int cols, int max_gy) {
   return g;
 }
 
+void launch_column_sum_pair_bf16(const float* partial_a, const float* partial_b, int parts, int cols, void* out_a, void* out_b,
+                                 cudaStream_t s) {
+  layernorm_bwd_finish_kernel<__nv_bfloat16><<<(cols + 255) / 256, 256, 0, s>>>(partial_a, partial_b, parts, cols, (__nv_bfloat16*)out_a,
+                                                                              (__nv_bfloat16*)out_b);
+  B200_CUDA_CHECK(cudaGetLastError());
+}
+
 int layernorm_partial_rows(int rows) {
   int p = (rows + 63) / 64;
   if (p > 2 * kNumSMs) p = 2 * kNumSMs;

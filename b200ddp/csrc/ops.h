@@ -82,6 +82,18 @@ void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, 
 // (Granite's attention multiplier folded into q).
 void launch_rotary(const void* x, const int* pos, const float* table, int max_pos, size_t rows, int heads, int kv_heads, int head_dim,
                    void* y, bool backward, cudaStream_t s, float q_scale = 1.f);
+// Qwen3's per-head q / k RMSNorm fused with rotary, head_dim 128 only, same layouts, positions and table as launch_rotary.
+// Forward: y = rope(x * rstd * w) per query head (w = wq [128]) and key head (w = wk [128]), rstd = rsqrt(mean(x^2) + eps)
+// over the head in fp32, one bf16 rounding; value heads copied; rstd fp32 [rows, heads + kv_heads].  Backward from dy and
+// the forward's x and rstd: dx (value heads pass through), dwq / dwk bf16 [128] = sum of rope^-1(dy) * x * rstd over rows
+// and query / key heads, with no atomics: per-CTA partials in partial fp32 [2, qk_norm_rotary_partials(rows), 128],
+// summed in CTA order; the grid depends on rows only, so repeated calls are bitwise identical.
+int qk_norm_rotary_partials(size_t rows);
+void launch_qk_norm_rotary_fwd(const void* x, const void* wq, const void* wk, const int* pos, const float* table, int max_pos, size_t rows,
+                               int heads, int kv_heads, int head_dim, float eps, void* y, float* rstd, cudaStream_t s);
+void launch_qk_norm_rotary_bwd(const void* dy, const void* x, const float* rstd, const void* wq, const void* wk, const int* pos,
+                               const float* table, int max_pos, size_t rows, int heads, int kv_heads, int head_dim, void* dx,
+                               float* partial, void* dwq, void* dwk, cudaStream_t s);
 
 // ---------------- mixture-of-experts routing, permutation and combine (moe.cu) -----------------------------
 // T tokens, E <= 64 experts, k <= min(E, 8) experts per token, hidden H % 64 == 0.  Deterministic, no atomics, no host
@@ -117,6 +129,10 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
                           DType dt, int rows, int cols, void* dx, float* dgamma_partial, float* dbeta_partial,
                           int partial_rows, void* dgamma, void* dbeta, cudaStream_t s);
 int layernorm_partial_rows(int rows);
+// out_a / out_b bf16 [cols] = sum over p < parts of partial_a / partial_b fp32 [parts, cols], in part order (the general
+// LayerNorm backward's finish kernel)
+void launch_column_sum_pair_bf16(const float* partial_a, const float* partial_b, int parts, int cols, void* out_a, void* out_b,
+                                 cudaStream_t s);
 // RMSNorm, y = x * rsqrt(mean(x^2) + eps) * gamma, on the LayerNorm fast path up to 1024 columns and on one CTA per row
 // above that: cols % 8 == 0, cols <= 4096, 32-byte aligned tensors.  rstd fp32 [rows]; backward workspace partial fp32
 // [2 * partial_rows, cols], counters uint32 [cols / 8].

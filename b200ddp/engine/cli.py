@@ -65,20 +65,20 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--cuda_graph", action="store_true", help="capture the whole optimizer step in a CUDA graph")
     p.add_argument("--fp8", action="store_true",
                    help="BERT encoder / GPT-2 / SmolLM block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs "
-                        "--model bert-base, gpt2, smollm-135m or qwen2.5-1.5b, --fp16 and a GPU")
+                        "--model bert-base, gpt2, smollm-135m, qwen2.5-1.5b or qwen3-0.6b, --fp16 and a GPU")
     p.add_argument("--min_seq_len", type=int, default=None,
-                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Granite on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
+                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Qwen3 / Granite on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
                         "keys are hidden from attention (native key-padding or causal kernel on the GPU; needs --fp16 and "
                         "--seq_len %% 128 == 0 there).  Default: fixed-length rows")
     p.add_argument("--pack", action="store_true",
-                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Granite on packed documents: documents with lengths uniform in [--min_seq_len, "
-                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2, Qwen2.5) or <s> (SmolLM; also Granite, "
+                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Qwen3 / Granite on packed documents: documents with lengths uniform in [--min_seq_len, "
+                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2, Qwen2.5, Qwen3) or <s> (SmolLM; also Granite, "
                         "whose own <|end_of_text|> is the padding id 0), packed "
                         "first-fit decreasing into rows; "
                         "attention stays inside a document (native document-boundary or causal kernel on the GPU).  Needs "
-                        "--model bert-base, gpt2, smollm-135m, qwen2.5-1.5b or granite-3.0-1b-a400m and --min_seq_len < --seq_len")
+                        "--model bert-base, gpt2, smollm-135m, qwen2.5-1.5b, qwen3-0.6b or granite-3.0-1b-a400m and --min_seq_len < --seq_len")
     p.add_argument("--fused_lm_loss", action="store_true",
-                   help="GPT-2 / SmolLM / Qwen2.5 / Granite: LM head and cross-entropy in one op that never builds the [tokens, vocab] "
+                   help="GPT-2 / SmolLM / Qwen2.5 / Qwen3 / Granite: LM head and cross-entropy in one op that never builds the [tokens, vocab] "
                         "logits (the head GEMM runs once more in the backward); needs --loss ce, and --fp16 on a GPU")
     p.add_argument("--router_aux_loss_coef", type=float, default=None,
                    help="mixture-of-experts models (granite-3.0-1b-a400m): weight of the router load-balancing loss added to "
@@ -151,14 +151,16 @@ def setup(args):
 
 
 # models whose token rows can be right-padded or packed, and whose block linears can run on FP8
-TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m", "qwen2.5-1.5b", "granite-3.0-1b-a400m")
+TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m", "qwen2.5-1.5b", "qwen3-0.6b", "granite-3.0-1b-a400m")
 # causal LMs: their packed documents start with a BOS id
-CAUSAL_MODELS = ("gpt2", "smollm-135m", "qwen2.5-1.5b", "granite-3.0-1b-a400m")
+CAUSAL_MODELS = ("gpt2", "smollm-135m", "qwen2.5-1.5b", "qwen3-0.6b", "granite-3.0-1b-a400m")
 # sparse mixture-of-experts LMs: no FP8 path, and a router load-balancing loss
 MOE_MODELS = ("granite-3.0-1b-a400m",)
+# Qwen models: Qwen's vocabulary, <|endoftext|> starts a packed document, at most QWEN_MAX_SEQ_LEN positions
+QWEN_MODELS = ("qwen2.5-1.5b", "qwen3-0.6b")
 GPT2_MAX_SEQ_LEN = 1024
 SMOLLM_MAX_SEQ_LEN = 2048
-QWEN_MAX_SEQ_LEN = 32768
+QWEN_MAX_SEQ_LEN = 32768          # Qwen2.5's positions and Qwen3's native context
 GRANITE_MAX_SEQ_LEN = 4096
 
 
@@ -170,8 +172,8 @@ def check_gpt_args(args) -> None:
     if args.model == "smollm-135m" and args.seq_len > SMOLLM_MAX_SEQ_LEN:
         raise ValueError(f"--model smollm-135m has {SMOLLM_MAX_SEQ_LEN} positions; --seq_len must be at most "
                          f"{SMOLLM_MAX_SEQ_LEN} (got {args.seq_len})")
-    if args.model == "qwen2.5-1.5b" and args.seq_len > QWEN_MAX_SEQ_LEN:
-        raise ValueError(f"--model qwen2.5-1.5b has {QWEN_MAX_SEQ_LEN} positions; --seq_len must be at most "
+    if args.model in QWEN_MODELS and args.seq_len > QWEN_MAX_SEQ_LEN:
+        raise ValueError(f"--model {args.model} trains on up to {QWEN_MAX_SEQ_LEN} positions; --seq_len must be at most "
                          f"{QWEN_MAX_SEQ_LEN} (got {args.seq_len})")
     if args.model == "granite-3.0-1b-a400m" and args.seq_len > GRANITE_MAX_SEQ_LEN:
         raise ValueError(f"--model granite-3.0-1b-a400m has {GRANITE_MAX_SEQ_LEN} positions; --seq_len must be at most "
@@ -187,7 +189,7 @@ def check_fp8_args(args) -> None:
                          f"have no FP8 path")
     if args.model not in TOKEN_MODELS:
         raise ValueError(f"--fp8 covers the block linears of the token models; it needs --model bert-base, gpt2, "
-                         f"smollm-135m or qwen2.5-1.5b (got --model {args.model})")
+                         f"smollm-135m, qwen2.5-1.5b or qwen3-0.6b (got --model {args.model})")
     if not args.fp16:
         raise ValueError("--fp8 needs --fp16: the FP8 GEMMs read bf16 activations and weights")
     if getattr(args, "device", None) is None or args.device.type != "cuda":
@@ -201,8 +203,8 @@ def check_min_seq_len_args(args) -> None:
     if n is None:
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b or "
-                         f"granite-3.0-1b-a400m; got --model {args.model})")
+        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b, "
+                         f"qwen3-0.6b or granite-3.0-1b-a400m; got --model {args.model})")
     if not 1 <= n <= args.seq_len:
         raise ValueError(f"--min_seq_len must lie in [1, --seq_len = {args.seq_len}], got {n}")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -218,8 +220,8 @@ def check_pack_args(args) -> None:
     if not getattr(args, "pack", False):
         return
     if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b or "
-                         f"granite-3.0-1b-a400m; got --model {args.model})")
+        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b, "
+                         f"qwen3-0.6b or granite-3.0-1b-a400m; got --model {args.model})")
     if not padding_on(args):
         raise ValueError("--pack needs --min_seq_len below --seq_len (documents have lengths in [--min_seq_len, --seq_len])")
     check_min_seq_len_args(args)
@@ -233,7 +235,7 @@ def check_fused_lm_loss_args(args) -> None:
         return
     if args.model not in CAUSAL_MODELS:
         raise ValueError(f"--fused_lm_loss fuses a causal LM's head into its loss; it needs --model gpt2, smollm-135m, "
-                         f"qwen2.5-1.5b or granite-3.0-1b-a400m (got --model {args.model})")
+                         f"qwen2.5-1.5b, qwen3-0.6b or granite-3.0-1b-a400m (got --model {args.model})")
     if getattr(args, "loss", None) not in (None, "ce"):
         raise ValueError(f"--fused_lm_loss computes cross-entropy; it needs --loss ce (got --loss {args.loss})")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -298,7 +300,7 @@ def main(argv=None) -> int:
             kwargs["bos_token_id"] = SyntheticTokens.BOS_ID
         elif args.pack and args.model in ("smollm-135m", "granite-3.0-1b-a400m"):
             kwargs["bos_token_id"] = SyntheticTokens.LLAMA_BOS_ID
-        elif args.pack and args.model == "qwen2.5-1.5b":
+        elif args.pack and args.model in QWEN_MODELS:
             kwargs["bos_token_id"] = SyntheticTokens.QWEN_BOS_ID
         elif args.pack:
             kwargs["cls_token_id"] = SyntheticTokens.CLS_ID

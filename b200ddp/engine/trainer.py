@@ -62,7 +62,7 @@ def build_dataset(args):
         return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=49152,
                                min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
                                causal=True, bos_token_id=SyntheticTokens.LLAMA_BOS_ID)
-    if name == "qwen2.5-1.5b":                                # causal-LM rows over Qwen2.5's vocabulary, <|endoftext|> starts a document
+    if name in ("qwen2.5-1.5b", "qwen3-0.6b"):                # causal-LM rows over Qwen's vocabulary, <|endoftext|> starts a document
         return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=151936,
                                min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
                                causal=True, bos_token_id=SyntheticTokens.QWEN_BOS_ID)

@@ -3,7 +3,7 @@ from .foo import FooModel, BranchyFooModel
 from .resnet import ResNet, resnet50, resnet152
 from .bert import BertConfig, BertModel, BertForMaskedLM, bert_base
 from .gpt import GPTConfig, GPTModel, GPTLMHeadModel, gpt2
-from .llama import LlamaConfig, LlamaModel, LlamaForCausalLM, smollm_135m, qwen2_5_1_5b, granite_3_0_1b_a400m
+from .llama import LlamaConfig, LlamaModel, LlamaForCausalLM, smollm_135m, qwen2_5_1_5b, qwen3_0_6b, granite_3_0_1b_a400m
 
 MODEL_REGISTRY = {
     "foo": FooModel,
@@ -13,6 +13,7 @@ MODEL_REGISTRY = {
     "gpt2": gpt2,
     "smollm-135m": smollm_135m,
     "qwen2.5-1.5b": qwen2_5_1_5b,
+    "qwen3-0.6b": qwen3_0_6b,
     "granite-3.0-1b-a400m": granite_3_0_1b_a400m,
 }
 
@@ -25,4 +26,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "granite_3_0_1b_a400m", "MODEL_REGISTRY", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "MODEL_REGISTRY", "build_model"]

@@ -16,7 +16,13 @@ eps 1e-6 and tied embeddings: 1,543,714,304 parameters.
 ``granite_3_0_1b_a400m`` is Granite-3.0-1B-A400M, a sparse mixture of experts: every block's SwiGLU is 32 experts of
 width 512 of which each token uses 8 (``ops.MoE``: native routing, expert sort and grouped wgmma GEMMs), 16 query heads
 over 8 K/V heads at hidden 1024, 24 layers, Granite's four multipliers and a vocabulary of 49155 padded to 49216:
-1,334,690,816 parameters.  ``load_hf_state_dict`` also reads ``transformers.GraniteMoeForCausalLM``'s state dicts."""
+1,334,690,816 parameters.  ``load_hf_state_dict`` also reads ``transformers.GraniteMoeForCausalLM``'s state dicts.
+
+``qwen3_0_6b`` is Qwen3-0.6B: 16 query heads over 8 K/V heads of dim 128 at hidden 1024 (``explicit_head_dim``: the
+heads are 2048 wide together), each query and key head RMS-normalised over its 128 elements with a learned weight
+before rotary (``qk_norm``: ``ops.qk_norm_rotary``, one fused kernel per direction), 28 layers, SwiGLU intermediate 3072,
+vocabulary 151936, rope theta 1e6, RMSNorm eps 1e-6 and tied embeddings: 596,049,920 parameters.
+``load_hf_state_dict`` also reads ``transformers.Qwen3ForCausalLM``'s state dicts."""
 from __future__ import annotations
 
 import math
@@ -25,7 +31,8 @@ from dataclasses import dataclass
 import torch
 import torch.nn as nn
 
-from ..ops import Linear, LinearCrossEntropyLoss, MoE, RMSNorm, causal_attention, document_bounds, linear, rotary, rotary_cos_sin, swiglu
+from ..ops import (Linear, LinearCrossEntropyLoss, MoE, RMSNorm, causal_attention, document_bounds, linear, qk_norm_rotary, rotary,
+                   rotary_cos_sin, swiglu)
 
 
 @dataclass
@@ -56,10 +63,13 @@ class LlamaConfig:
     residual_multiplier: float = 1.0
     logits_scaling: float = 1.0
     pad_vocab_to: int = 1          # embedding / LM-head rows padded to a multiple of this (GPT-2's mechanism)
+    # attention head width when it is not hidden // heads (Qwen3: 16 heads of 128 at hidden 1024); None = hidden // heads
+    explicit_head_dim: int | None = None
+    qk_norm: bool = False          # per-head RMSNorm of q and k (weights q_norm / k_norm [head_dim]) before rotary (Qwen3)
 
     @property
     def head_dim(self) -> int:
-        return self.hidden // self.heads
+        return self.hidden // self.heads if self.explicit_head_dim is None else self.explicit_head_dim
 
     @property
     def padded_vocab(self) -> int:
@@ -87,13 +97,21 @@ class LlamaBlock(nn.Module):
         else:
             self.gate_up = Linear(c.hidden, 2 * c.intermediate, bias=False, fp8=c.fp8)   # gate | up
             self.down_proj = Linear(c.intermediate, c.hidden, bias=False, fp8=c.fp8)
+        if c.qk_norm:
+            self.q_norm = RMSNorm(d, eps=c.eps)
+            self.k_norm = RMSNorm(d, eps=c.eps)
         self.q_scale, self.residual = c.q_scale, c.residual_multiplier
 
     def _add(self, x, y):
         return x + y if self.residual == 1.0 else torch.add(x, y, alpha=self.residual)
 
     def forward(self, x, bounds, position_ids, cos_sin):
-        qkv = rotary(self.qkv(self.input_layernorm(x)), position_ids, cos_sin, self.heads, self.kv_heads, self.q_scale)
+        qkv = self.qkv(self.input_layernorm(x))
+        if hasattr(self, "q_norm"):
+            qkv = qk_norm_rotary(qkv, self.q_norm.weight, self.k_norm.weight, position_ids, cos_sin, self.heads, self.kv_heads,
+                                 self.q_norm.eps)
+        else:
+            qkv = rotary(qkv, position_ids, cos_sin, self.heads, self.kv_heads, self.q_scale)
         x = self._add(x, self.o_proj(causal_attention(qkv, bounds, self.heads, self.kv_heads)))
         h = self.post_attention_layernorm(x)
         return self._add(x, self.moe(h) if hasattr(self, "moe") else self.down_proj(swiglu(self.gate_up(h))))
@@ -103,9 +121,13 @@ class LlamaModel(nn.Module):
     def __init__(self, config: LlamaConfig | None = None):
         super().__init__()
         c = self.config = config or LlamaConfig()
-        if c.hidden % c.heads or c.heads % c.kv_heads:
-            raise ValueError(f"LlamaConfig: heads must divide hidden and kv_heads must divide heads, got hidden={c.hidden}, "
-                             f"heads={c.heads}, kv_heads={c.kv_heads}")
+        if (c.explicit_head_dim is None and c.hidden % c.heads) or c.heads % c.kv_heads:
+            raise ValueError(f"LlamaConfig: heads must divide hidden (unless explicit_head_dim is set) and kv_heads must divide "
+                             f"heads, got hidden={c.hidden}, heads={c.heads}, kv_heads={c.kv_heads}")
+        if c.explicit_head_dim is not None and (c.explicit_head_dim < 2 or c.explicit_head_dim % 2):
+            raise ValueError(f"LlamaConfig: explicit_head_dim must be a positive even number, got {c.explicit_head_dim}")
+        if c.qk_norm and c.q_scale != 1.0:
+            raise ValueError("LlamaConfig: qk_norm has no query-scale variant; leave attention_multiplier at None")
         if not (c.q_scale > 0 and math.frexp(c.q_scale)[0] == 0.5):
             raise ValueError(f"LlamaConfig: attention_multiplier * sqrt(head_dim) must be a power of two (it scales q exactly in "
                              f"bf16), got {c.attention_multiplier} * sqrt({c.head_dim})")
@@ -205,10 +227,11 @@ class LlamaForCausalLM(nn.Module):
         return (counts * probs).sum() * (self.config.num_experts / (n * n))
 
     def load_hf_state_dict(self, hf: dict) -> None:
-        """Load a ``transformers.LlamaForCausalLM``, ``transformers.Qwen2ForCausalLM`` or ``transformers.GraniteMoeForCausalLM``
-        state dict: q / k / v (weights, and biases when the config has ``attention_bias``) and gate / up are concatenated into
-        the fused projections, GraniteMoe's ``block_sparse_moe`` router and expert weights are taken as they are, embedding
-        rows beyond the checkpoint's vocabulary are zero, and a tied ``lm_head.weight`` is ignored."""
+        """Load a ``transformers.LlamaForCausalLM``, ``transformers.Qwen2ForCausalLM``, ``transformers.Qwen3ForCausalLM`` or
+        ``transformers.GraniteMoeForCausalLM`` state dict: q / k / v (weights, and biases when the config has
+        ``attention_bias``) and gate / up are concatenated into the fused projections, Qwen3's ``self_attn.q_norm`` /
+        ``k_norm`` weights (with ``qk_norm``) and GraniteMoe's ``block_sparse_moe`` router and expert weights are taken as
+        they are, embedding rows beyond the checkpoint's vocabulary are zero, and a tied ``lm_head.weight`` is ignored."""
         own = self.state_dict()
         emb = hf["model.embed_tokens.weight"]
         if emb.shape[0] != own["model.embed_tokens.weight"].shape[0]:       # padded vocabulary: zero rows beyond the checkpoint's
@@ -230,6 +253,9 @@ class LlamaForCausalLM(nn.Module):
                 out[dst + "down_proj.weight"] = hf[src + "mlp.down_proj.weight"]
             for n in ("input_layernorm", "post_attention_layernorm"):
                 out[dst + f"{n}.weight"] = hf[src + f"{n}.weight"]
+            if self.config.qk_norm:
+                for n in ("q_norm", "k_norm"):
+                    out[dst + f"{n}.weight"] = hf[src + f"self_attn.{n}.weight"]
         self.load_state_dict({k: v.to(own[k].dtype).contiguous() for k, v in out.items()}, strict=True)
 
 
@@ -249,6 +275,18 @@ def qwen2_5_1_5b(fp8: bool = False, pad_token_id: int | None = None, bos_token_i
     return LlamaForCausalLM(LlamaConfig(vocab_size=151936, max_position=32768, hidden=1536, layers=28, heads=12, kv_heads=2,
                                         intermediate=8960, eps=1e-6, rope_theta=1e6, attention_bias=True, fp8=fp8,
                                         pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))
+
+
+def qwen3_0_6b(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
+               fused_lm_loss: bool = False) -> nn.Module:
+    """Qwen3-0.6B with its tied LM head (40960 positions): 28 blocks of grouped-query attention (16 query heads over 8 K/V
+    heads of dim 128 at hidden 1024, so heads * head_dim = 2048 is not the hidden size) with per-head q / k RMSNorm before
+    rotary, SwiGLU intermediate 3072, vocabulary 151936; ``fp8=True`` puts the 112 block linears on FP8 tensor cores.
+    ``pad_token_id``, ``bos_token_id`` and ``fused_lm_loss`` as for ``smollm_135m``."""
+    return LlamaForCausalLM(LlamaConfig(vocab_size=151936, max_position=40960, hidden=1024, layers=28, heads=16, kv_heads=8,
+                                        intermediate=3072, eps=1e-6, rope_theta=1e6, explicit_head_dim=128, qk_norm=True,
+                                        fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id,
+                                        fused_lm_loss=fused_lm_loss))
 
 
 def granite_3_0_1b_a400m(pad_token_id: int | None = None, bos_token_id: int | None = None, fused_lm_loss: bool = False,

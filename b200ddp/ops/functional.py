@@ -649,6 +649,89 @@ def rotary(qkv: torch.Tensor, position_ids: torch.Tensor, cos_sin: torch.Tensor,
     return _Rotary.apply(qkv, position_ids, cos_sin, heads, kv_heads, float(q_scale))
 
 
+def _qk_norm_rotary_reference(qkv: torch.Tensor, q_weight: torch.Tensor, k_weight: torch.Tensor, position_ids: torch.Tensor,
+                              cos_sin: torch.Tensor, heads: int, kv_heads: int, eps: float) -> torch.Tensor:
+    B, S, Wd = qkv.shape
+    d = Wd // (heads + 2 * kv_heads)
+    ct = torch.promote_types(qkv.dtype, torch.float32)
+    x = qkv.to(ct)
+    qk, v = x.split([(heads + kv_heads) * d, kv_heads * d], dim=-1)
+    qk = qk.reshape(B, S, heads + kv_heads, d)
+    w = torch.cat([q_weight.to(ct).expand(heads, d), k_weight.to(ct).expand(kv_heads, d)])
+    qk = qk * torch.rsqrt(qk.pow(2).mean(-1, keepdim=True) + eps) * w
+    normed = torch.cat([qk.reshape(B, S, -1), v], -1)
+    return _rotary_reference(normed, position_ids, cos_sin, heads, kv_heads).to(qkv.dtype)
+
+
+class _QkNormRotary(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, qkv, q_weight, k_weight, position_ids, cos_sin, heads, kv_heads, eps):
+        ctx.heads, ctx.kv_heads, ctx.eps = heads, kv_heads, eps
+        if qkv.is_cuda:
+            B, S, Wd = qkv.shape
+            x = qkv.reshape(B * S, Wd).contiguous()
+            pos = position_ids.to(device=qkv.device, dtype=torch.int32).reshape(-1).contiguous()
+            table = cos_sin.to(device=qkv.device, dtype=torch.float32).contiguous()
+            wq, wk = q_weight.contiguous(), k_weight.contiguous()
+            y, rstd = _C().qk_norm_rotary_fwd(x, wq, wk, pos, table, heads, kv_heads, eps)
+            ctx.save_for_backward(x, rstd, wq, wk, pos, table)
+            return y.view(B, S, Wd)
+        ctx.save_for_backward(qkv, q_weight, k_weight, position_ids, cos_sin)
+        return _qk_norm_rotary_reference(qkv, q_weight, k_weight, position_ids, cos_sin, heads, kv_heads, eps)
+
+    @staticmethod
+    def backward(ctx, dy):
+        if dy.is_cuda:
+            x, rstd, wq, wk, pos, table = ctx.saved_tensors
+            B, S, Wd = dy.shape
+            dx, dwq, dwk = _C().qk_norm_rotary_bwd(dy.reshape(B * S, Wd).to(torch.bfloat16).contiguous(), x, rstd, wq, wk, pos, table,
+                                                   ctx.heads, ctx.kv_heads)
+            return dx.view(B, S, Wd), dwq, dwk, None, None, None, None, None
+        qkv, q_weight, k_weight, position_ids, cos_sin = ctx.saved_tensors
+        with torch.enable_grad():                    # the CPU body's gradient is autograd through the reference
+            ins = [t.detach().requires_grad_(True) for t in (qkv, q_weight, k_weight)]
+            y = _qk_norm_rotary_reference(*ins, position_ids, cos_sin, ctx.heads, ctx.kv_heads, ctx.eps)
+            grads = torch.autograd.grad(y, ins, dy)
+        return (*grads, None, None, None, None, None)
+
+
+def qk_norm_rotary(qkv: torch.Tensor, q_weight: torch.Tensor, k_weight: torch.Tensor, position_ids: torch.Tensor,
+                   cos_sin: torch.Tensor, heads: int, kv_heads: int, eps: float = 1e-6) -> torch.Tensor:
+    """Qwen3's per-head q / k RMSNorm followed by rotary, in Hugging Face's ``Qwen3Attention`` order (norm, then rope):
+    every query head h of qkv [B, S, (heads + 2 * kv_heads) * d] becomes rope(x * rsqrt(mean(x^2) + eps) * q_weight) over
+    its d elements, every key head the same with k_weight ([d] each); value heads pass through.  position_ids and cos_sin
+    as for ``rotary``.  Out of place.
+
+    On CUDA one kernel per direction (statistics and rotation in fp32, one bf16 rounding), with bf16 qkv, d = 128,
+    16-byte aligned qkv and bf16 weights on qkv's device, else ``ValueError``; positions stay on the device (CUDA-graph
+    safe).  The weight gradients are deterministic (per-CTA partials summed in a fixed order).  The backward keeps the
+    pre-norm qkv and fp32 rstd [B * S, heads + kv_heads]: at 16,384 tokens and Qwen3-0.6B's 4096-wide qkv, about 134 MB
+    per layer (plus 1.6 MB of rstd)."""
+    if qkv.dim() != 3 or heads < 1 or kv_heads < 1 or qkv.shape[-1] % (heads + 2 * kv_heads) or \
+            (qkv.shape[-1] // (heads + 2 * kv_heads)) % 2:
+        raise ValueError(f"qk_norm_rotary needs qkv [B, S, (heads + 2 * kv_heads) * d] with an even d, got {tuple(qkv.shape)} for "
+                         f"heads={heads}, kv_heads={kv_heads}")
+    d = qkv.shape[-1] // (heads + 2 * kv_heads)
+    if q_weight.shape != (d,) or k_weight.shape != (d,):
+        raise ValueError(f"qk_norm_rotary needs q_weight and k_weight [{d}], got {tuple(q_weight.shape)} and {tuple(k_weight.shape)}")
+    if tuple(position_ids.shape) != tuple(qkv.shape[:2]) or position_ids.is_floating_point() or position_ids.is_complex():
+        raise ValueError(f"qk_norm_rotary needs integer position_ids {tuple(qkv.shape[:2])}, got {position_ids.dtype} "
+                         f"{tuple(position_ids.shape)}")
+    if cos_sin.dim() != 3 or tuple(cos_sin.shape[1:]) != (2, d // 2) or cos_sin.shape[0] < 1:
+        raise ValueError(f"qk_norm_rotary needs cos_sin [max_position, 2, {d // 2}], got {tuple(cos_sin.shape)}")
+    if not eps > 0:
+        raise ValueError(f"qk_norm_rotary needs eps > 0, got {eps}")
+    if qkv.is_cuda:
+        if qkv.dtype != torch.bfloat16 or d != CAUSAL_WIDE_HEAD_DIM:
+            raise ValueError(f"qk_norm_rotary on CUDA needs bf16 qkv and head dim {CAUSAL_WIDE_HEAD_DIM}, got {qkv.dtype}, head dim {d}")
+        if any(w.dtype != torch.bfloat16 or w.device != qkv.device for w in (q_weight, k_weight)):
+            raise ValueError(f"qk_norm_rotary on CUDA needs bf16 weights on qkv's device ({qkv.device}), got "
+                             f"{q_weight.dtype} on {q_weight.device} and {k_weight.dtype} on {k_weight.device}")
+        if qkv.is_contiguous() and qkv.data_ptr() % 16:
+            raise ValueError("qk_norm_rotary on CUDA needs 16-byte aligned qkv")
+    return _QkNormRotary.apply(qkv, q_weight, k_weight, position_ids, cos_sin, heads, kv_heads, float(eps))
+
+
 def _rms_norm_reference(x: torch.Tensor, weight: torch.Tensor, eps: float) -> torch.Tensor:
     xf = x.float()
     return (xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps) * weight.float()).to(x.dtype)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,conv,bn,sgd,adamw,ln,xent,lmloss,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,conv,bn,sgd,adamw,ln,xent,lmloss,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -411,6 +411,47 @@ def main():
                                   C.causal_attention_d128_bwd)
         rmsnorm_rows(8192, hidden, 1e-6)
         rotary_rows(qkv, H, Hkv, d, S, 1e6)
+
+    if "qwen3" in want:
+        # Qwen3-0.6B's per-head q / k RMSNorm + rotary at batch 8 x 2048: qkv [16384, (16 + 2 * 8) * 128] bf16.  Baselines:
+        # the torch expression (F.rms_norm on the head views, then rotate_half with bf16 cos / sin, autograd for the
+        # backward) and our rotary kernel alone, the floor the fusion should approach.  Algorithmic bytes: forward qkv in,
+        # out and rstd out; backward dy, qkv, rstd in and dqkv out (weights and the [2, parts, 128] partials are noise).
+        import torch.nn.functional as F
+        print(f"qwen3 kernels on {card()}", flush=True)
+        M, H, Hkv, d, eps = 16384, 16, 8, 128, 1e-6
+        W, normed = (H + 2 * Hkv) * d, H + Hkv
+        g = torch.Generator(device="cuda").manual_seed(0)
+        x = torch.randn(M, W, device=dev, generator=g).to(torch.bfloat16)
+        dy = torch.randn(M, W, device=dev, generator=g).to(torch.bfloat16)
+        wq, wk = ((torch.rand(d, device=dev, generator=g) + 0.5).to(torch.bfloat16) for _ in range(2))
+        pos = (torch.arange(M, device=dev, dtype=torch.int32) % 2048).contiguous()
+        table = Fn.rotary_cos_sin(2048, d, 1e6).to(dev)
+        cos = torch.cat([table[pos.long(), 0]] * 2, -1)[:, None].to(torch.bfloat16)
+        sin = torch.cat([table[pos.long(), 1]] * 2, -1)[:, None].to(torch.bfloat16)
+
+        def torch_fwd(t, a, b):
+            h = t.view(M, H + 2 * Hkv, d)
+            qk = torch.cat([F.rms_norm(h[:, :H], (d,), a, eps), F.rms_norm(h[:, H:normed], (d,), b, eps)], 1)
+            rot = torch.cat([-qk[..., d // 2:], qk[..., :d // 2]], -1)
+            return torch.cat([(qk * cos + rot * sin).view(M, -1), t[:, normed * d:]], -1)
+        io = M * W * 2
+        y, rstd = C.qk_norm_rotary_fwd(x, wq, wk, pos, table, H, Hkv, eps)
+        record(f"qk_norm_rotary fwd {M}x{W} bf16", timeit(lambda: C.qk_norm_rotary_fwd(x, wq, wk, pos, table, H, Hkv, eps), args.iters),
+               bytes_=2 * io + M * normed * 4, lib_ms=timeit(lambda: torch_fwd(x, wq, wk), args.iters),
+               note="lib = F.rms_norm per head view + rotate_half")
+        record(f"rotary alone fwd {M}x{W} bf16", timeit(lambda: C.rotary(x, pos, table, H, Hkv, False), args.iters), bytes_=2 * io,
+               note="the floor: rotation without the norm")
+        xg, ag, bg = (t.clone().requires_grad_(True) for t in (x, wq, wk))
+        yt = torch_fwd(xg, ag, bg)
+        record(f"qk_norm_rotary bwd {M}x{W} bf16",
+               timeit(lambda: C.qk_norm_rotary_bwd(dy, x, rstd, wq, wk, pos, table, H, Hkv), args.iters),
+               bytes_=3 * io + M * normed * 4,
+               lib_ms=timeit(lambda: torch.autograd.grad(yt, (xg, ag, bg), dy, retain_graph=True), args.iters),
+               note="lib = the torch expression's autograd (dqkv, dw_q, dw_k)")
+        record(f"rotary alone bwd {M}x{W} bf16", timeit(lambda: C.rotary(dy, pos, table, H, Hkv, True), args.iters), bytes_=2 * io,
+               note="the floor: rotation without the norm")
+        del xg, ag, bg, yt
 
     if "conv" in want:
         import torch.nn.functional as F
