@@ -84,14 +84,12 @@ class SyntheticTokens(Dataset):
     ``causal=True`` gives causal-LM rows (GPT) in the same three layouts: within a document ``labels[t] = ids[t + 1]``,
     and each document's last token and the padding are labelled -100.  Tokens come from [1, vocab); packed documents
     start with ``BOS_ID`` instead of ``CLS_ID`` (and hold no other ``BOS_ID``), and ``bos_token_id`` is set instead of
-    ``cls_token_id``.  ``bos_token_id`` picks another start id for causal packed documents (1, Llama's ``<s>``, for
-    SmolLM; 151643, ``<|endoftext|>``, for Qwen2.5); GPT-2's 50256 stays the default."""
+    ``cls_token_id``.  ``bos_token_id`` picks another start id for causal packed documents (a model's own, from its
+    entry in ``b200ddp.models.MODEL_REGISTRY``); ``BOS_ID`` is the default."""
 
     PAD_ID = 0
     CLS_ID = 101                   # [CLS] in the BERT vocabulary
     BOS_ID = 50256                 # <|endoftext|> in the GPT-2 vocabulary, which starts each GPT-2 document
-    LLAMA_BOS_ID = 1               # <s> in the Llama / SmolLM vocabularies
-    QWEN_BOS_ID = 151643           # <|endoftext|> in the Qwen2.5 vocabulary, which starts each Qwen2.5 document
 
     def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 30522, mask_prob: float = 0.15, seed: int = 1234,
                  min_len: int | None = None, pack: bool = False, causal: bool = False, bos_token_id: int | None = None):

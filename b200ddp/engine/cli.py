@@ -17,7 +17,7 @@ import sys
 import torch
 import torch.distributed as dist
 
-from ..models import MODEL_REGISTRY, build_model
+from ..models import MODEL_REGISTRY, build_model, model_entry
 from ..utils import (get_logger_with_rank, redirect_warnings_to_logger, resolve_local_rank, env_int, set_seed)
 
 log = None
@@ -64,25 +64,25 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--channels_last", action="store_true")
     p.add_argument("--cuda_graph", action="store_true", help="capture the whole optimizer step in a CUDA graph")
     p.add_argument("--fp8", action="store_true",
-                   help="BERT encoder / GPT-2 / SmolLM block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs "
-                        "--model bert-base, gpt2, smollm-135m, qwen2.5-1.5b or qwen3-0.6b, --fp16 and a GPU")
+                   help="block linears on FP8 tensor cores (E4M3 x / W, E5M2 gradients); needs --model "
+                        f"{_names(lambda e: e.fp8)}, --fp16 and a GPU")
     p.add_argument("--min_seq_len", type=int, default=None,
-                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Qwen3 / Granite on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
+                   help="token models on right-padded rows: each row's length is uniform in [min_seq_len, --seq_len], padded "
                         "keys are hidden from attention (native key-padding or causal kernel on the GPU; needs --fp16 and "
-                        "--seq_len %% 128 == 0 there).  Default: fixed-length rows")
+                        f"--seq_len %% 128 == 0 there).  Needs --model {_names(lambda e: e.token_model)}.  Default: "
+                        "fixed-length rows")
     p.add_argument("--pack", action="store_true",
-                   help="BERT / GPT-2 / SmolLM / Qwen2.5 / Qwen3 / Granite on packed documents: documents with lengths uniform in [--min_seq_len, "
-                        "--seq_len], each starting with [CLS] (BERT), <|endoftext|> (GPT-2, Qwen2.5, Qwen3) or <s> (SmolLM; also Granite, "
-                        "whose own <|end_of_text|> is the padding id 0), packed "
-                        "first-fit decreasing into rows; "
+                   help="token models on packed documents: documents with lengths uniform in [--min_seq_len, --seq_len], each "
+                        "starting with the model's start id ([CLS] for BERT), packed first-fit decreasing into rows; "
                         "attention stays inside a document (native document-boundary or causal kernel on the GPU).  Needs "
-                        "--model bert-base, gpt2, smollm-135m, qwen2.5-1.5b, qwen3-0.6b or granite-3.0-1b-a400m and --min_seq_len < --seq_len")
+                        f"--model {_names(lambda e: e.token_model)} and --min_seq_len < --seq_len")
     p.add_argument("--fused_lm_loss", action="store_true",
-                   help="GPT-2 / SmolLM / Qwen2.5 / Qwen3 / Granite: LM head and cross-entropy in one op that never builds the [tokens, vocab] "
-                        "logits (the head GEMM runs once more in the backward); needs --loss ce, and --fp16 on a GPU")
+                   help="LM head and cross-entropy in one op that never builds the [tokens, vocab] logits (the head GEMM runs "
+                        f"once more in the backward); needs --model {_names(lambda e: e.kind == 'causal')}, --loss ce, and "
+                        "--fp16 on a GPU")
     p.add_argument("--router_aux_loss_coef", type=float, default=None,
-                   help="mixture-of-experts models (granite-3.0-1b-a400m): weight of the router load-balancing loss added to "
-                        "the training loss (default: the preset's, 0.001); 0 turns it off and skips its statistics")
+                   help=f"mixture-of-experts models ({_names(lambda e: e.moe)}): weight of the router load-balancing loss "
+                        "added to the training loss (default: the preset's, 0.001); 0 turns it off and skips its statistics")
     p.add_argument("--resume_from", type=str, default=None, help="checkpoint dir, or 'latest' under --output_dir")
     p.add_argument("--log_file", type=str, default=None, help="also log to this file ({rank} is substituted)")
     p.add_argument("--no_tensorboard", action="store_true")
@@ -138,7 +138,7 @@ def setup(args):
                                                                         transport=args.backend))
         args.n_gpu = 1 if have_cuda else 0
     args.device = device
-    check_gpt_args(args)
+    check_seq_len_args(args)
     check_fp8_args(args)
     check_min_seq_len_args(args)
     check_pack_args(args)
@@ -150,46 +150,36 @@ def setup(args):
     return log
 
 
-# models whose token rows can be right-padded or packed, and whose block linears can run on FP8
-TOKEN_MODELS = ("bert-base", "gpt2", "smollm-135m", "qwen2.5-1.5b", "qwen3-0.6b", "granite-3.0-1b-a400m")
-# causal LMs: their packed documents start with a BOS id
-CAUSAL_MODELS = ("gpt2", "smollm-135m", "qwen2.5-1.5b", "qwen3-0.6b", "granite-3.0-1b-a400m")
-# sparse mixture-of-experts LMs: no FP8 path, and a router load-balancing loss
-MOE_MODELS = ("granite-3.0-1b-a400m",)
-# Qwen models: Qwen's vocabulary, <|endoftext|> starts a packed document, at most QWEN_MAX_SEQ_LEN positions
-QWEN_MODELS = ("qwen2.5-1.5b", "qwen3-0.6b")
-GPT2_MAX_SEQ_LEN = 1024
-SMOLLM_MAX_SEQ_LEN = 2048
-QWEN_MAX_SEQ_LEN = 32768          # Qwen2.5's positions and Qwen3's native context
-GRANITE_MAX_SEQ_LEN = 4096
+def _names(pick) -> str:
+    """The registered models whose entries ``pick`` selects, as "a, b or c"."""
+    names = [n for n, e in MODEL_REGISTRY.items() if pick(e)]
+    return " or ".join([", ".join(names[:-1]), names[-1]]) if len(names) > 1 else names[0]
 
 
-def check_gpt_args(args) -> None:
-    """GPT-2 has 1024 learned positions: reject a longer ``--seq_len`` up front."""
-    if args.model == "gpt2" and args.seq_len > GPT2_MAX_SEQ_LEN:
-        raise ValueError(f"--model gpt2 has {GPT2_MAX_SEQ_LEN} positions; --seq_len must be at most {GPT2_MAX_SEQ_LEN} "
+def check_seq_len_args(args) -> None:
+    """A token model trains on at most its position table's rows (or its entry's lower ``max_seq_len``): reject a longer
+    ``--seq_len`` up front instead of indexing past the table."""
+    entry = model_entry(args.model)
+    if not entry.token_model:
+        return
+    limit = entry.max_seq_len or entry.config.max_position
+    if args.seq_len > limit:
+        raise ValueError(f"--model {args.model} trains on up to {limit} positions; --seq_len must be at most {limit} "
                          f"(got {args.seq_len})")
-    if args.model == "smollm-135m" and args.seq_len > SMOLLM_MAX_SEQ_LEN:
-        raise ValueError(f"--model smollm-135m has {SMOLLM_MAX_SEQ_LEN} positions; --seq_len must be at most "
-                         f"{SMOLLM_MAX_SEQ_LEN} (got {args.seq_len})")
-    if args.model in QWEN_MODELS and args.seq_len > QWEN_MAX_SEQ_LEN:
-        raise ValueError(f"--model {args.model} trains on up to {QWEN_MAX_SEQ_LEN} positions; --seq_len must be at most "
-                         f"{QWEN_MAX_SEQ_LEN} (got {args.seq_len})")
-    if args.model == "granite-3.0-1b-a400m" and args.seq_len > GRANITE_MAX_SEQ_LEN:
-        raise ValueError(f"--model granite-3.0-1b-a400m has {GRANITE_MAX_SEQ_LEN} positions; --seq_len must be at most "
-                         f"{GRANITE_MAX_SEQ_LEN} (got {args.seq_len})")
 
 
 def check_fp8_args(args) -> None:
-    """``--fp8`` is a BERT / GPT-2 feature on top of bf16 weights on a GPU: reject every other combination up front."""
+    """``--fp8`` runs a dense token model's block linears on FP8 tensor cores, on top of bf16 weights on a GPU: reject
+    every other combination up front."""
     if not getattr(args, "fp8", False):
         return
-    if args.model in MOE_MODELS:
+    entry = model_entry(args.model)
+    if entry.moe:
         raise ValueError(f"--fp8 covers dense block linears; --model {args.model} is a mixture of experts, whose expert GEMMs "
                          f"have no FP8 path")
-    if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--fp8 covers the block linears of the token models; it needs --model bert-base, gpt2, "
-                         f"smollm-135m, qwen2.5-1.5b or qwen3-0.6b (got --model {args.model})")
+    if not entry.fp8:
+        raise ValueError(f"--fp8 covers the block linears of the token models; it needs --model {_names(lambda e: e.fp8)} "
+                         f"(got --model {args.model})")
     if not args.fp16:
         raise ValueError("--fp8 needs --fp16: the FP8 GEMMs read bf16 activations and weights")
     if getattr(args, "device", None) is None or args.device.type != "cuda":
@@ -197,14 +187,14 @@ def check_fp8_args(args) -> None:
 
 
 def check_min_seq_len_args(args) -> None:
-    """``--min_seq_len`` pads BERT / GPT-2 rows; on the GPU their attention runs on the bf16 key-padding or causal
-    kernel (head dim 64, sequence length a multiple of 128): reject every other combination up front."""
+    """``--min_seq_len`` pads a token model's rows; on the GPU their attention runs on the bf16 key-padding or causal
+    kernels (sequence length a multiple of 128): reject every other combination up front."""
     n = getattr(args, "min_seq_len", None)
     if n is None:
         return
-    if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--min_seq_len pads token rows; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b, "
-                         f"qwen3-0.6b or granite-3.0-1b-a400m; got --model {args.model})")
+    if not model_entry(args.model).token_model:
+        raise ValueError(f"--min_seq_len pads token rows; it needs --model {_names(lambda e: e.token_model)} "
+                         f"(got --model {args.model})")
     if not 1 <= n <= args.seq_len:
         raise ValueError(f"--min_seq_len must lie in [1, --seq_len = {args.seq_len}], got {n}")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -215,13 +205,13 @@ def check_min_seq_len_args(args) -> None:
 
 
 def check_pack_args(args) -> None:
-    """``--pack`` packs documents into padded BERT / GPT-2 rows, so it needs everything ``--min_seq_len`` needs (on the
-    GPU: ``--fp16``, ``--seq_len`` % 128 == 0) and a ``--min_seq_len`` below ``--seq_len``."""
+    """``--pack`` packs documents into a token model's padded rows, so it needs everything ``--min_seq_len`` needs (on
+    the GPU: ``--fp16``, ``--seq_len`` % 128 == 0) and a ``--min_seq_len`` below ``--seq_len``."""
     if not getattr(args, "pack", False):
         return
-    if args.model not in TOKEN_MODELS:
-        raise ValueError(f"--pack packs token documents; it needs --model bert-base or gpt2 (or smollm-135m, qwen2.5-1.5b, "
-                         f"qwen3-0.6b or granite-3.0-1b-a400m; got --model {args.model})")
+    if not model_entry(args.model).token_model:
+        raise ValueError(f"--pack packs token documents; it needs --model {_names(lambda e: e.token_model)} "
+                         f"(got --model {args.model})")
     if not padding_on(args):
         raise ValueError("--pack needs --min_seq_len below --seq_len (documents have lengths in [--min_seq_len, --seq_len])")
     check_min_seq_len_args(args)
@@ -233,9 +223,9 @@ def check_fused_lm_loss_args(args) -> None:
     across GPUs and gather them back to one)."""
     if not getattr(args, "fused_lm_loss", False):
         return
-    if args.model not in CAUSAL_MODELS:
-        raise ValueError(f"--fused_lm_loss fuses a causal LM's head into its loss; it needs --model gpt2, smollm-135m, "
-                         f"qwen2.5-1.5b, qwen3-0.6b or granite-3.0-1b-a400m (got --model {args.model})")
+    if model_entry(args.model).kind != "causal":
+        raise ValueError(f"--fused_lm_loss fuses a causal LM's head into its loss; it needs --model "
+                         f"{_names(lambda e: e.kind == 'causal')} (got --model {args.model})")
     if getattr(args, "loss", None) not in (None, "ce"):
         raise ValueError(f"--fused_lm_loss computes cross-entropy; it needs --loss ce (got --loss {args.loss})")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -251,12 +241,13 @@ def check_moe_args(args) -> None:
     non-negative value.  The loss (on by default) reads statistics the MoE layers keep from their forward, which
     single-process multi-GPU ``DataParallel`` leaves on its per-GPU replicas: that mode needs the loss turned off."""
     coef = getattr(args, "router_aux_loss_coef", None)
-    if coef is not None and args.model not in MOE_MODELS:
+    moe = model_entry(args.model).moe
+    if coef is not None and not moe:
         raise ValueError(f"--router_aux_loss_coef weights a mixture-of-experts router's loss; it needs --model "
-                         f"{' or '.join(MOE_MODELS)} (got --model {args.model})")
+                         f"{_names(lambda e: e.moe)} (got --model {args.model})")
     if coef is not None and not coef >= 0:
         raise ValueError(f"--router_aux_loss_coef must be >= 0, got {coef}")
-    if args.model in MOE_MODELS and coef != 0 and getattr(args, "device", None) is not None and args.device.type == "cuda" \
+    if moe and coef != 0 and getattr(args, "device", None) is not None and args.device.type == "cuda" \
             and args.local_rank == -1 and getattr(args, "n_gpu", 1) > 1:
         raise ValueError(f"--model {args.model} with its router load-balancing loss does not run under single-process "
                          f"multi-GPU DataParallel; launch one process per GPU (torchrun), make one GPU visible, or pass "
@@ -296,14 +287,9 @@ def main(argv=None) -> int:
     if padding_on(args):
         from ..data import SyntheticTokens
         kwargs["pad_token_id"] = SyntheticTokens.PAD_ID
-        if args.pack and args.model == "gpt2":
-            kwargs["bos_token_id"] = SyntheticTokens.BOS_ID
-        elif args.pack and args.model in ("smollm-135m", "granite-3.0-1b-a400m"):
-            kwargs["bos_token_id"] = SyntheticTokens.LLAMA_BOS_ID
-        elif args.pack and args.model in QWEN_MODELS:
-            kwargs["bos_token_id"] = SyntheticTokens.QWEN_BOS_ID
-        elif args.pack:
-            kwargs["cls_token_id"] = SyntheticTokens.CLS_ID
+        if args.pack:
+            entry = model_entry(args.model)
+            kwargs["cls_token_id" if entry.kind == "encoder" else "bos_token_id"] = entry.start_id
     model = build_model(args.model, **kwargs)
     trainer = Trainer(args, model, log)
     trainer.train()

@@ -23,6 +23,7 @@ from tqdm import tqdm
 from tqdm.auto import trange
 
 from ..data import BatchLoader, DevicePrefetcher, FooDataset, SyntheticImageNet, SyntheticTokens
+from ..models import model_entry
 from ..ops import CrossEntropyLoss, MSELoss
 from ..optim import FusedAdamW, FusedSGD, get_linear_schedule_with_warmup, weight_decay_groups
 from ..parallel import DataParallel, DistributedDataParallel, ShardedSampler
@@ -43,40 +44,24 @@ def _summary_writer():
 
 
 def build_dataset(args):
-    # (loss_kind is defined below; resolved at call time)
-    name = getattr(args, "model", "foo")
+    """``args.model``'s synthetic data: the reference's ``FooDataset``, ImageNet-shaped images, or token rows over the
+    model's vocabulary whose packed documents start with its registry entry's ``start_id``."""
+    entry = model_entry(getattr(args, "model", "foo"))
     n = int(getattr(args, "dataset_size", 100000))
-    if name == "foo":
+    if entry.kind == "foo":
         return FooDataset(n)
-    if name.startswith("resnet"):
+    if entry.kind == "image":
         dense = loss_kind(args) == "mse"
         return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
-    if name.startswith("bert"):
-        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)),
-                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)))
-    if name == "gpt2":                                        # causal-LM rows over GPT-2's vocabulary
-        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=50257,
-                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
-                               causal=True)
-    if name == "smollm-135m":                                 # causal-LM rows over SmolLM's vocabulary, <s> starts a document
-        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=49152,
-                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
-                               causal=True, bos_token_id=SyntheticTokens.LLAMA_BOS_ID)
-    if name in ("qwen2.5-1.5b", "qwen3-0.6b"):                # causal-LM rows over Qwen's vocabulary, <|endoftext|> starts a document
-        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=151936,
-                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
-                               causal=True, bos_token_id=SyntheticTokens.QWEN_BOS_ID)
-    if name == "granite-3.0-1b-a400m":                        # causal-LM rows over Granite's vocabulary; Granite's own start id,
-        # <|end_of_text|> = 0, is PAD_ID here, so packed documents start with LLAMA_BOS_ID (1) instead
-        return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=49155,
-                               min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
-                               causal=True, bos_token_id=SyntheticTokens.LLAMA_BOS_ID)
-    raise ValueError(f"no default dataset for model {name!r}")
+    causal = entry.kind == "causal"
+    return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=entry.config.vocab_size,
+                           min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
+                           causal=causal, bos_token_id=entry.start_id if causal else None)
 
 
 def loss_kind(args) -> str:
     """``--loss`` or the model's default: MSE for the reference's FooModel (``ddp.py:164``), cross-entropy otherwise."""
-    return getattr(args, "loss", None) or ("mse" if getattr(args, "model", "foo") == "foo" else "ce")
+    return getattr(args, "loss", None) or ("mse" if model_entry(getattr(args, "model", "foo")).kind == "foo" else "ce")
 
 
 class RouterAuxLoss:
@@ -185,7 +170,7 @@ class Trainer:
             self._resume_state = load_checkpoint(self.resume_dir, None, self.optimizer, self.scheduler)
             log.info("Resumed from checkpoint.", dict(path=self.resume_dir, global_step=self._resume_state.get("global_step")))
         self.model = model
-        if input_transform is None and self.device.type == "cuda" and getattr(args, "model", "foo").startswith("resnet"):
+        if input_transform is None and self.device.type == "cuda" and model_entry(getattr(args, "model", "foo")).kind == "image":
             input_transform = self._make_image_transform()
         self.step_fn = TrainStep(model, self.criterion, self.optimizer, self.device,
                                  accumulation=args.gradient_accumulation_steps, use_graph=getattr(args, "cuda_graph", False),

@@ -1,29 +1,58 @@
 """Model registry: the reference hard-codes ``FooModel()`` (``ddp.py:311``); ``--model`` selects here."""
+from __future__ import annotations
+
+from dataclasses import dataclass
+from typing import Any, Callable
+
 from .foo import FooModel, BranchyFooModel
 from .resnet import ResNet, resnet50, resnet152
-from .bert import BertConfig, BertModel, BertForMaskedLM, bert_base
-from .gpt import GPTConfig, GPTModel, GPTLMHeadModel, gpt2
-from .llama import LlamaConfig, LlamaModel, LlamaForCausalLM, smollm_135m, qwen2_5_1_5b, qwen3_0_6b, granite_3_0_1b_a400m
+from .bert import BERT_BASE, BertConfig, BertModel, BertForMaskedLM, bert_base
+from .gpt import GPT2, GPTConfig, GPTModel, GPTLMHeadModel, gpt2
+from .llama import (GRANITE_3_0_1B_A400M, QWEN2_5_1_5B, QWEN3_0_6B, SMOLLM_135M, LlamaConfig, LlamaModel, LlamaForCausalLM,
+                    smollm_135m, qwen2_5_1_5b, qwen3_0_6b, granite_3_0_1b_a400m)
+
+
+@dataclass(frozen=True)
+class ModelEntry:
+    """A registered model: its builder and what training needs to know about it without building it."""
+    build: Callable[..., Any]
+    kind: str                          # "foo", "image", "encoder" (BERT) or "causal" (the language models)
+    config: Any = None                 # token models: the preset config, whose vocab_size and max_position training reads
+    start_id: int | None = None        # token models: the id each packed document starts with
+    fp8: bool = False                  # build takes fp8=True (block linears on FP8 tensor cores)
+    moe: bool = False                  # mixture of experts: build takes router_aux_loss_coef
+    max_seq_len: int | None = None     # a training cap on --seq_len below config.max_position
+
+    @property
+    def token_model(self) -> bool:
+        return self.kind in ("encoder", "causal")
+
 
 MODEL_REGISTRY = {
-    "foo": FooModel,
-    "resnet50": resnet50,
-    "resnet152": resnet152,
-    "bert-base": bert_base,
-    "gpt2": gpt2,
-    "smollm-135m": smollm_135m,
-    "qwen2.5-1.5b": qwen2_5_1_5b,
-    "qwen3-0.6b": qwen3_0_6b,
-    "granite-3.0-1b-a400m": granite_3_0_1b_a400m,
+    "foo": ModelEntry(FooModel, "foo"),
+    "resnet50": ModelEntry(resnet50, "image"),
+    "resnet152": ModelEntry(resnet152, "image"),
+    "bert-base": ModelEntry(bert_base, "encoder", BERT_BASE, start_id=101, fp8=True),                 # [CLS]
+    "gpt2": ModelEntry(gpt2, "causal", GPT2, start_id=50256, fp8=True),                               # <|endoftext|>
+    "smollm-135m": ModelEntry(smollm_135m, "causal", SMOLLM_135M, start_id=1, fp8=True),              # <s>
+    "qwen2.5-1.5b": ModelEntry(qwen2_5_1_5b, "causal", QWEN2_5_1_5B, start_id=151643, fp8=True),      # <|endoftext|>
+    # Qwen3's native context is 32768 tokens; the position table's 40960 rows leave room to generate past it
+    "qwen3-0.6b": ModelEntry(qwen3_0_6b, "causal", QWEN3_0_6B, start_id=151643, fp8=True, max_seq_len=32768),
+    # Granite's own start id, <|end_of_text|> = 0, is the padding id here, so packed documents start with id 1 instead
+    "granite-3.0-1b-a400m": ModelEntry(granite_3_0_1b_a400m, "causal", GRANITE_3_0_1B_A400M, start_id=1, moe=True),
 }
 
 
-def build_model(name: str, **kwargs):
+def model_entry(name: str) -> ModelEntry:
     try:
-        return MODEL_REGISTRY[name](**kwargs)
+        return MODEL_REGISTRY[name]
     except KeyError:
         raise ValueError(f"unknown model {name!r}; choose from {sorted(MODEL_REGISTRY)}") from None
 
 
+def build_model(name: str, **kwargs):
+    return model_entry(name).build(**kwargs)
+
+
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "MODEL_REGISTRY", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

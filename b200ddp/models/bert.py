@@ -8,7 +8,7 @@ document-boundary kernel (``ops.packed_attention``), with position ids restartin
 (199 tensors in the stock naming; 151 here because Q / K / V are one stored parameter) when built with ``with_mlm_head=False``."""
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 
 import torch
 import torch.nn as nn
@@ -195,12 +195,14 @@ def split_qkv_state_dict(state: dict) -> dict:
     return out
 
 
+BERT_BASE = BertConfig()
+
+
 def bert_base(with_mlm_head: bool = True, fp8: bool = False, pad_token_id: int | None = None,
               cls_token_id: int | None = None) -> nn.Module:
     """BERT-base; ``fp8=True`` puts the 48 encoder linears on FP8 tensor cores (embeddings, MLM transform and the tied
     decoder stay bf16).  ``pad_token_id`` takes right-padded input (padded keys are hidden from attention);
     ``cls_token_id`` takes packed documents, each starting with that id (attention stays inside a document and position
     ids restart in each).  The state dict is the same either way."""
-    if with_mlm_head:
-        return BertForMaskedLM(BertConfig(pad_vocab_to=64, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id))
-    return BertModel(BertConfig(fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id))
+    c = replace(BERT_BASE, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id)
+    return BertForMaskedLM(replace(c, pad_vocab_to=64)) if with_mlm_head else BertModel(c)

@@ -8,7 +8,7 @@ packed documents (each starting with that id), attention is causal inside each d
 each.  The state dict is the same in every mode; ``load_hf_state_dict`` reads ``transformers.GPT2LMHeadModel``'s."""
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 
 import torch
 import torch.nn as nn
@@ -155,10 +155,13 @@ class GPTLMHeadModel(nn.Module):
         self.load_state_dict(out, strict=True)
 
 
+GPT2 = GPTConfig()
+
+
 def gpt2(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
          fused_lm_loss: bool = False) -> nn.Module:
     """GPT-2 small (124 M) with its LM head; ``fp8=True`` puts the 48 block linears on FP8 tensor cores (embeddings and
     the tied LM head stay bf16).  ``pad_token_id`` takes right-padded input; ``bos_token_id`` takes packed documents,
     each starting with that id (causal attention stays inside a document and position ids restart in each).
     ``fused_lm_loss=True``: forward returns hidden states and ``lm_head_loss()`` computes the loss without the logits."""
-    return GPTLMHeadModel(GPTConfig(fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))
+    return GPTLMHeadModel(replace(GPT2, fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))

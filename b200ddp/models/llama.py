@@ -26,7 +26,7 @@ vocabulary 151936, rope theta 1e6, RMSNorm eps 1e-6 and tied embeddings: 596,049
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 
 import torch
 import torch.nn as nn
@@ -259,22 +259,33 @@ class LlamaForCausalLM(nn.Module):
         self.load_state_dict({k: v.to(own[k].dtype).contiguous() for k, v in out.items()}, strict=True)
 
 
+SMOLLM_135M = LlamaConfig()
+QWEN2_5_1_5B = LlamaConfig(vocab_size=151936, max_position=32768, hidden=1536, layers=28, heads=12, kv_heads=2,
+                           intermediate=8960, eps=1e-6, rope_theta=1e6, attention_bias=True)
+QWEN3_0_6B = LlamaConfig(vocab_size=151936, max_position=40960, hidden=1024, layers=28, heads=16, kv_heads=8,
+                         intermediate=3072, eps=1e-6, rope_theta=1e6, explicit_head_dim=128, qk_norm=True)
+GRANITE_3_0_1B_A400M = LlamaConfig(vocab_size=49155, max_position=4096, hidden=1024, layers=24, heads=16, kv_heads=8,
+                                   intermediate=512, eps=1e-6, rope_theta=10000.0, num_experts=32, experts_per_token=8,
+                                   router_aux_loss_coef=0.001, embedding_multiplier=12.0, attention_multiplier=0.015625,
+                                   residual_multiplier=0.22, logits_scaling=6.0, pad_vocab_to=64)
+
+
 def smollm_135m(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
                 fused_lm_loss: bool = False) -> nn.Module:
     """SmolLM-135M with its tied LM head; ``fp8=True`` puts the 120 block linears on FP8 tensor cores (embedding and LM
     head stay bf16).  ``pad_token_id`` takes right-padded input; ``bos_token_id`` takes packed documents, each starting
     with that id (attention stays inside a document and position ids restart in each).  ``fused_lm_loss=True``: forward
     returns hidden states and ``lm_head_loss()`` computes the loss without the logits."""
-    return LlamaForCausalLM(LlamaConfig(fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))
+    return LlamaForCausalLM(replace(SMOLLM_135M, fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id,
+                                    fused_lm_loss=fused_lm_loss))
 
 
 def qwen2_5_1_5b(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
                  fused_lm_loss: bool = False) -> nn.Module:
     """Qwen2.5-1.5B with its tied LM head (32768 positions); ``fp8=True`` puts the 112 block linears on FP8 tensor cores.
     ``pad_token_id``, ``bos_token_id`` and ``fused_lm_loss`` as for ``smollm_135m``."""
-    return LlamaForCausalLM(LlamaConfig(vocab_size=151936, max_position=32768, hidden=1536, layers=28, heads=12, kv_heads=2,
-                                        intermediate=8960, eps=1e-6, rope_theta=1e6, attention_bias=True, fp8=fp8,
-                                        pad_token_id=pad_token_id, bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))
+    return LlamaForCausalLM(replace(QWEN2_5_1_5B, fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id,
+                                    fused_lm_loss=fused_lm_loss))
 
 
 def qwen3_0_6b(fp8: bool = False, pad_token_id: int | None = None, bos_token_id: int | None = None,
@@ -283,22 +294,16 @@ def qwen3_0_6b(fp8: bool = False, pad_token_id: int | None = None, bos_token_id:
     heads of dim 128 at hidden 1024, so heads * head_dim = 2048 is not the hidden size) with per-head q / k RMSNorm before
     rotary, SwiGLU intermediate 3072, vocabulary 151936; ``fp8=True`` puts the 112 block linears on FP8 tensor cores.
     ``pad_token_id``, ``bos_token_id`` and ``fused_lm_loss`` as for ``smollm_135m``."""
-    return LlamaForCausalLM(LlamaConfig(vocab_size=151936, max_position=40960, hidden=1024, layers=28, heads=16, kv_heads=8,
-                                        intermediate=3072, eps=1e-6, rope_theta=1e6, explicit_head_dim=128, qk_norm=True,
-                                        fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id,
-                                        fused_lm_loss=fused_lm_loss))
+    return LlamaForCausalLM(replace(QWEN3_0_6B, fp8=fp8, pad_token_id=pad_token_id, bos_token_id=bos_token_id,
+                                    fused_lm_loss=fused_lm_loss))
 
 
 def granite_3_0_1b_a400m(pad_token_id: int | None = None, bos_token_id: int | None = None, fused_lm_loss: bool = False,
-                         router_aux_loss_coef: float = 0.001) -> nn.Module:
+                         router_aux_loss_coef: float = GRANITE_3_0_1B_A400M.router_aux_loss_coef) -> nn.Module:
     """Granite-3.0-1B-A400M with its tied LM head (4096 positions): 24 blocks of grouped-query attention (16 query heads
     over 8 K/V heads, head dim 64) and a mixture of 32 SwiGLU experts of width 512, 8 per token; embedding multiplier 12,
     attention multiplier 1/64, residual multiplier 0.22, logits scaling 6; vocabulary 49155 padded to 49216.
     ``router_aux_loss_coef`` (transformers' default 0.001; 0 turns it off) weights ``router_aux_loss`` in the training
     loss.  ``pad_token_id``, ``bos_token_id`` and ``fused_lm_loss`` as for ``smollm_135m``."""
-    return LlamaForCausalLM(LlamaConfig(vocab_size=49155, max_position=4096, hidden=1024, layers=24, heads=16, kv_heads=8,
-                                        intermediate=512, eps=1e-6, rope_theta=10000.0, num_experts=32, experts_per_token=8,
-                                        router_aux_loss_coef=router_aux_loss_coef, embedding_multiplier=12.0,
-                                        attention_multiplier=0.015625, residual_multiplier=0.22, logits_scaling=6.0,
-                                        pad_vocab_to=64, pad_token_id=pad_token_id, bos_token_id=bos_token_id,
-                                        fused_lm_loss=fused_lm_loss))
+    return LlamaForCausalLM(replace(GRANITE_3_0_1B_A400M, router_aux_loss_coef=router_aux_loss_coef, pad_token_id=pad_token_id,
+                                    bos_token_id=bos_token_id, fused_lm_loss=fused_lm_loss))

@@ -377,11 +377,12 @@ def main():
         # SmolLM-135M's hot ops at batch 8 x 2048 (9 query heads over 3 K/V heads, d 64, hidden 576, SwiGLU 1536), each
         # against its torch equivalent.  The card and its power limit are part of every number below.
         import torch.nn.functional as F
-        from b200ddp.data import SyntheticTokens
+        from b200ddp.models import MODEL_REGISTRY
         print(f"llama kernels on {card()}", flush=True)
         B, S, H, Hkv, d, hidden, inter = 8, 2048, 9, 3, 64, 576, 1536
         M = B * S
-        qkv = causal_lm_attention("gqa", B, S, H, Hkv, d, 49152, SyntheticTokens.LLAMA_BOS_ID, C.causal_gqa_attention_fwd,
+        smollm = MODEL_REGISTRY["smollm-135m"]
+        qkv = causal_lm_attention("gqa", B, S, H, Hkv, d, smollm.config.vocab_size, smollm.start_id, C.causal_gqa_attention_fwd,
                                   C.causal_gqa_attention_bwd)
         rmsnorm_rows(M, hidden, 1e-5)
         rotary_rows(qkv, H, Hkv, d, S, 10000.0)
@@ -404,10 +405,11 @@ def main():
     if "qwen" in want:
         # Qwen2.5-1.5B's head-dim-128 ops at batch 4 x 2048 (12 query heads over 2 K/V heads, hidden 1536), each against
         # its torch equivalent.  The card and its power limit are part of every number below.
-        from b200ddp.data import SyntheticTokens
+        from b200ddp.models import MODEL_REGISTRY
         print(f"qwen kernels on {card()}", flush=True)
         B, S, H, Hkv, d, hidden = 4, 2048, 12, 2, 128, 1536
-        qkv = causal_lm_attention("d128", B, S, H, Hkv, d, 151936, SyntheticTokens.QWEN_BOS_ID, C.causal_attention_d128_fwd,
+        qwen = MODEL_REGISTRY["qwen2.5-1.5b"]
+        qkv = causal_lm_attention("d128", B, S, H, Hkv, d, qwen.config.vocab_size, qwen.start_id, C.causal_attention_d128_fwd,
                                   C.causal_attention_d128_bwd)
         rmsnorm_rows(8192, hidden, 1e-6)
         rotary_rows(qkv, H, Hkv, d, S, 1e6)

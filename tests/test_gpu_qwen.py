@@ -353,7 +353,7 @@ def test_qwen_step_has_no_host_synchronisation():
 
 
 @pytest.mark.parametrize("pack,fp8", [(False, False), (True, False), (False, True), (True, True)])
-def test_qwen_graph_training_lowers_the_loss(tmp_path, pack, fp8):
+def test_qwen_graph_training_on_its_cli_dataset_lowers_the_loss(tmp_path, pack, fp8):
     """What `python ddp.py --model qwen2.5-1.5b --fp16 --optimizer adamw --cuda_graph --max_steps 30 --seq_len 256
     --min_seq_len 32 [--pack] [--fp8]` runs, on a two-layer Qwen-shaped model (head dim 128, q / k / v bias)."""
     from b200ddp.data import SyntheticTokens
@@ -367,9 +367,9 @@ def test_qwen_graph_training_lowers_the_loss(tmp_path, pack, fp8):
     args = cli.build_parser().parse_args(argv)
     cli.setup(args)
     ds = build_dataset(args)
-    assert isinstance(ds, SyntheticTokens) and ds.bos_token_id == (SyntheticTokens.QWEN_BOS_ID if pack else None)
+    assert isinstance(ds, SyntheticTokens) and ds.bos_token_id == (151643 if pack else None)
     # a small alphabet leaves something to learn; the start id maps to the small model's 1
-    ds.X = torch.where(ds.X == SyntheticTokens.QWEN_BOS_ID, torch.ones_like(ds.X), torch.where(ds.X > 0, ds.X % 64 + 2, ds.X))
+    ds.X = torch.where(ds.X == 151643, torch.ones_like(ds.X), torch.where(ds.X > 0, ds.X % 64 + 2, ds.X))
     ds.Y = torch.where(ds.Y > 0, ds.Y % 64 + 2, ds.Y)
     if pack:
         ds.bos_token_id = 1

@@ -201,11 +201,10 @@ def test_granite_cli_accepts_its_flags_and_rejects_the_rest(tmp_path):
     assert not isinstance(build_criterion(on, LlamaForCausalLM(_tiny_cfg(router_aux_loss_coef=0.0))), RouterAuxLoss)
 
 
-def test_granite_dataset_start_id():
-    from b200ddp.data import SyntheticTokens
+def test_granite_dataset_documents_start_with_id_1():
     from b200ddp.engine.trainer import build_dataset
     ds = build_dataset(types.SimpleNamespace(model="granite-3.0-1b-a400m", dataset_size=40, seq_len=64, min_seq_len=4, pack=True))
-    assert ds.bos_token_id == SyntheticTokens.LLAMA_BOS_ID and ds.pad_token_id == 0 and int(ds.X.max()) < 49155
+    assert ds.bos_token_id == 1 and ds.pad_token_id == 0 and int(ds.X.max()) < 49155
 
 
 def test_short_cpu_training_run_lowers_the_loss(tmp_path):

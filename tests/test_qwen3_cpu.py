@@ -202,11 +202,10 @@ def test_qwen3_cli_accepts_its_flags_and_rejects_long_rows(tmp_path):
         cli.setup(_args(tmp_path, "--model", "resnet50", "--no_cuda", "--fused_lm_loss"))
 
 
-def test_qwen3_dataset_start_id():
-    from b200ddp.data import SyntheticTokens
+def test_qwen3_dataset_documents_start_with_endoftext():
     from b200ddp.engine.trainer import build_dataset
     ds = build_dataset(types.SimpleNamespace(model="qwen3-0.6b", dataset_size=40, seq_len=64, min_seq_len=4, pack=True))
-    assert ds.bos_token_id == QWEN_BOS == SyntheticTokens.QWEN_BOS_ID and ds.pad_token_id == 0 and int(ds.X.max()) < 151936
+    assert ds.bos_token_id == QWEN_BOS and ds.pad_token_id == 0 and int(ds.X.max()) < 151936
     for x, docs in zip(ds.X, ds.doc_lengths):
         at = 0
         for n in docs:

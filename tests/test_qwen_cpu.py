@@ -117,10 +117,10 @@ def test_qwen_cli_accepts_its_flags_and_rejects_long_rows(tmp_path):
         cli.setup(_args(tmp_path, "--model", "resnet50", "--no_cuda", "--fp16", "--fp8"))
 
 
-def test_qwen_dataset_start_id():
-    from b200ddp.data import SyntheticTokens
+def test_qwen_dataset_documents_start_with_endoftext():
     from b200ddp.engine.trainer import build_dataset
-    assert SyntheticTokens.QWEN_BOS_ID == QWEN_BOS
+    from b200ddp.models import MODEL_REGISTRY
+    assert MODEL_REGISTRY["qwen2.5-1.5b"].start_id == QWEN_BOS
     ds = build_dataset(types.SimpleNamespace(model="qwen2.5-1.5b", dataset_size=40, seq_len=64, min_seq_len=4, pack=True))
     assert ds.bos_token_id == QWEN_BOS and ds.pad_token_id == 0 and int(ds.X.max()) < 151936
     for x, y, docs in zip(ds.X, ds.Y, ds.doc_lengths):
