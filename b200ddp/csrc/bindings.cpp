@@ -925,34 +925,39 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                        cur_stream());
     return std::make_tuple(dx, dgamma);
   });
-  // out [M, I] = silu(gate) * up from gate_up bf16 [M, 2I]
-  m.def("swiglu_fwd", [](at::Tensor gate_up) {
+  // Gated linear units on one projection [M, 2I]: SwiGLU (gate | up, out = silu(gate) * up) and GeGLU (input | gate,
+  // out = gelu(input) * gate).  Forward: out [M, I]; backward: the gradient of both column blocks [M, 2I] from dy [M, I].
+  using GluLaunch = void (*)(const void*, const void*, void*, size_t, int, bool, cudaStream_t);
+  auto glu_fwd = [](at::Tensor gate_up, GluLaunch launch, const char* name) {
     check_cuda(gate_up, "gate_up");
     TORCH_CHECK(gate_up.scalar_type() == at::kBFloat16 && gate_up.is_contiguous() && gate_up.size(-1) % 16 == 0,
-                "swiglu_fwd: contiguous bf16 [..., 2I] with I % 8 == 0");
+                name, "_fwd: contiguous bf16 [..., 2I] with I % 8 == 0");
     c10::cuda::CUDAGuard guard(gate_up.device());
     if ((reinterpret_cast<uintptr_t>(gate_up.data_ptr()) & 15) != 0) gate_up = gate_up.clone();
     auto sizes = gate_up.sizes().vec();
     const int inter = (int)(sizes.back() / 2);
     sizes.back() = inter;
     at::Tensor out = at::empty(sizes, gate_up.options());
-    launch_swiglu(gate_up.data_ptr(), nullptr, out.data_ptr(), (size_t)(gate_up.numel() / (2 * inter)), inter, false, cur_stream());
+    launch(gate_up.data_ptr(), nullptr, out.data_ptr(), (size_t)(gate_up.numel() / (2 * inter)), inter, false, cur_stream());
     return out;
-  });
-  // d[gate | up] [M, 2I] from dy [M, I]
-  m.def("swiglu_bwd", [](at::Tensor dy, at::Tensor gate_up) {
+  };
+  auto glu_bwd = [](at::Tensor dy, at::Tensor gate_up, GluLaunch launch, const char* name) {
     check_cuda(dy, "dy"); check_cuda(gate_up, "gate_up");
     TORCH_CHECK(gate_up.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && gate_up.is_contiguous() &&
                 dy.is_contiguous() && gate_up.size(-1) % 16 == 0 && dy.numel() * 2 == gate_up.numel() && dy.size(-1) * 2 == gate_up.size(-1),
-                "swiglu_bwd: contiguous bf16 dy [..., I] and gate_up [..., 2I]");
+                name, "_bwd: contiguous bf16 dy [..., I] and gate_up [..., 2I]");
     c10::cuda::CUDAGuard guard(gate_up.device());
     if ((reinterpret_cast<uintptr_t>(gate_up.data_ptr()) & 15) != 0) gate_up = gate_up.clone();
     if ((reinterpret_cast<uintptr_t>(dy.data_ptr()) & 15) != 0) dy = dy.clone();
     const int inter = (int)dy.size(-1);
     at::Tensor out = at::empty_like(gate_up);
-    launch_swiglu(gate_up.data_ptr(), dy.data_ptr(), out.data_ptr(), (size_t)(dy.numel() / inter), inter, true, cur_stream());
+    launch(gate_up.data_ptr(), dy.data_ptr(), out.data_ptr(), (size_t)(dy.numel() / inter), inter, true, cur_stream());
     return out;
-  });
+  };
+  m.def("swiglu_fwd", [glu_fwd](at::Tensor gate_up) { return glu_fwd(gate_up, launch_swiglu, "swiglu"); });
+  m.def("swiglu_bwd", [glu_bwd](at::Tensor dy, at::Tensor gate_up) { return glu_bwd(dy, gate_up, launch_swiglu, "swiglu"); });
+  m.def("geglu_fwd", [glu_fwd](at::Tensor input_gate) { return glu_fwd(input_gate, launch_geglu, "geglu"); });
+  m.def("geglu_bwd", [glu_bwd](at::Tensor dy, at::Tensor input_gate) { return glu_bwd(dy, input_gate, launch_geglu, "geglu"); });
 
   // ---- mixture of experts (moe.cu, grouped GEMMs in gemm_wgmma.cu) -------------------------------------------------
   auto moe_tensor = [](const at::Tensor& t, at::ScalarType st, int64_t numel, const char* what) {

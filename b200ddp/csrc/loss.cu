@@ -381,10 +381,14 @@ void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n,
 // SwiGLU (Llama MLP): in = [M, 2I] bf16 with column blocks gate | up, out = silu(gate) * up [M, I].  The backward writes
 // d[gate | up] [M, 2I] in one pass: dgate = dy * up * silu'(gate), dup = dy * silu(gate), silu'(g) = s (1 + g (1 - s)),
 // s = sigmoid(g).  One thread per 8 consecutive columns (I % 8 == 0), 16-byte loads and stores.
+// GeGLU (ModernBERT MLP) is the same kernel with the erf-form GELU on the first block: out = gelu(input) * gate, and
+// d[input | gate] = [dy * gate * gelu'(input), dy * gelu(input)].
 namespace b200 {
 namespace {
 
-template <bool BWD>
+enum class GluAct { kSilu, kGelu };
+
+template <bool BWD, GluAct ACT = GluAct::kSilu>
 __global__ void __launch_bounds__(kLossThreads) swiglu_kernel(const __nv_bfloat16* __restrict__ in, const __nv_bfloat16* __restrict__ dy,
                                                               __nv_bfloat16* __restrict__ out, size_t rows, int inter) {
   const int vpr = inter / 8;                                    // 8-column vectors per row
@@ -401,9 +405,14 @@ __global__ void __launch_bounds__(kLossThreads) swiglu_kernel(const __nv_bfloat1
       unpack8(*reinterpret_cast<const Bf16x8*>(dy + r * inter + c), d);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float sg = 1.f / (1.f + expf(-g[i]));
-        du[i] = d[i] * g[i] * sg;
-        dg[i] = d[i] * u[i] * sg * (1.f + g[i] * (1.f - sg));
+        if constexpr (ACT == GluAct::kGelu) {
+          du[i] = d[i] * gelu_f(g[i]);
+          dg[i] = d[i] * u[i] * gelu_grad_f(g[i]);
+        } else {
+          const float sg = 1.f / (1.f + expf(-g[i]));
+          du[i] = d[i] * g[i] * sg;
+          dg[i] = d[i] * u[i] * sg * (1.f + g[i] * (1.f - sg));
+        }
       }
       __nv_bfloat16* op = out + r * 2 * inter + c;
       *reinterpret_cast<Bf16x8*>(op) = pack8(dg);
@@ -411,28 +420,40 @@ __global__ void __launch_bounds__(kLossThreads) swiglu_kernel(const __nv_bfloat1
     } else {
       float o[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) o[i] = g[i] / (1.f + expf(-g[i])) * u[i];
+      for (int i = 0; i < 8; ++i) {
+        if constexpr (ACT == GluAct::kGelu) o[i] = gelu_f(g[i]) * u[i];
+        else o[i] = g[i] / (1.f + expf(-g[i])) * u[i];
+      }
       *reinterpret_cast<Bf16x8*>(out + r * inter + c) = pack8(o);
     }
   }
 }
 
-}  // namespace
-
-void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s) {
-  if (inter % 8 != 0 || ((reinterpret_cast<uintptr_t>(gate_up) | reinterpret_cast<uintptr_t>(out) |
+template <GluAct ACT>
+void launch_glu(const char* name, const void* in_act, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s) {
+  if (inter % 8 != 0 || ((reinterpret_cast<uintptr_t>(in_act) | reinterpret_cast<uintptr_t>(out) |
                           reinterpret_cast<uintptr_t>(dy)) & 15u) != 0)
-    throw std::runtime_error("swiglu: needs the intermediate size a multiple of 8 and 16-byte aligned tensors (inter=" +
+    throw std::runtime_error(std::string(name) + ": needs the intermediate size a multiple of 8 and 16-byte aligned tensors (inter=" +
                              std::to_string(inter) + ")");
   size_t b = (rows * (inter / 8) + kLossThreads - 1) / kLossThreads;
   if (b < 1) b = 1;
   if (b > (size_t)16 * kNumSMs) b = (size_t)16 * kNumSMs;
-  const auto* in = reinterpret_cast<const __nv_bfloat16*>(gate_up);
+  const auto* in = reinterpret_cast<const __nv_bfloat16*>(in_act);
   if (backward)
-    swiglu_kernel<true><<<(int)b, kLossThreads, 0, s>>>(in, reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<__nv_bfloat16*>(out), rows, inter);
+    swiglu_kernel<true, ACT><<<(int)b, kLossThreads, 0, s>>>(in, reinterpret_cast<const __nv_bfloat16*>(dy), reinterpret_cast<__nv_bfloat16*>(out), rows, inter);
   else
-    swiglu_kernel<false><<<(int)b, kLossThreads, 0, s>>>(in, nullptr, reinterpret_cast<__nv_bfloat16*>(out), rows, inter);
+    swiglu_kernel<false, ACT><<<(int)b, kLossThreads, 0, s>>>(in, nullptr, reinterpret_cast<__nv_bfloat16*>(out), rows, inter);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+}  // namespace
+
+void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s) {
+  launch_glu<GluAct::kSilu>("swiglu", gate_up, dy, out, rows, inter, backward, s);
+}
+
+void launch_geglu(const void* input_gate, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s) {
+  launch_glu<GluAct::kGelu>("geglu", input_gate, dy, out, rows, inter, backward, s);
 }
 
 }  // namespace b200

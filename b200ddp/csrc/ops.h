@@ -74,6 +74,9 @@ void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n,
 // SwiGLU: forward out[M, I] = silu(gate) * up from gate_up bf16 [M, 2I] (gate | up); backward out[M, 2I] = d[gate | up]
 // from dy [M, I].  I % 8 == 0, 16-byte aligned tensors (loss.cu).
 void launch_swiglu(const void* gate_up, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s);
+// GeGLU: the same with the erf-form GELU, forward out[M, I] = gelu(input) * gate from input_gate bf16 [M, 2I]
+// (input | gate); backward out[M, 2I] = d[input | gate] from dy [M, I].  I % 8 == 0, 16-byte aligned tensors (loss.cu).
+void launch_geglu(const void* input_gate, const void* dy, void* out, size_t rows, int inter, bool backward, cudaStream_t s);
 
 // ---------------- rotary position embedding (rotary.cu) ----------------------------------------------
 // qkv bf16 [rows, (heads + 2*kv_heads)*head_dim] -> y (same shape), head_dim 64 or 128: query and key heads rotated by

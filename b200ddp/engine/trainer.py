@@ -56,7 +56,8 @@ def build_dataset(args):
     causal = entry.kind == "causal"
     return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=entry.config.vocab_size,
                            min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
-                           causal=causal, bos_token_id=entry.start_id if causal else None)
+                           causal=causal, bos_token_id=entry.start_id if causal else None,
+                           cls_token_id=SyntheticTokens.CLS_ID if causal else entry.start_id)
 
 
 def loss_kind(args) -> str:

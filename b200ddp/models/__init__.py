@@ -10,13 +10,15 @@ from .bert import BERT_BASE, BertConfig, BertModel, BertForMaskedLM, bert_base
 from .gpt import GPT2, GPTConfig, GPTModel, GPTLMHeadModel, gpt2
 from .llama import (GRANITE_3_0_1B_A400M, QWEN2_5_1_5B, QWEN3_0_6B, SMOLLM_135M, LlamaConfig, LlamaModel, LlamaForCausalLM,
                     smollm_135m, qwen2_5_1_5b, qwen3_0_6b, granite_3_0_1b_a400m)
+from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, ModernBertModel, ModernBertForMaskedLM, modernbert_base,
+                         modernbert_large)
 
 
 @dataclass(frozen=True)
 class ModelEntry:
     """A registered model: its builder and what training needs to know about it without building it."""
     build: Callable[..., Any]
-    kind: str                          # "foo", "image", "encoder" (BERT) or "causal" (the language models)
+    kind: str                          # "foo", "image", "encoder" (BERT, ModernBERT) or "causal" (the language models)
     config: Any = None                 # token models: the preset config, whose vocab_size and max_position training reads
     start_id: int | None = None        # token models: the id each packed document starts with
     fp8: bool = False                  # build takes fp8=True (block linears on FP8 tensor cores)
@@ -33,6 +35,8 @@ MODEL_REGISTRY = {
     "resnet50": ModelEntry(resnet50, "image"),
     "resnet152": ModelEntry(resnet152, "image"),
     "bert-base": ModelEntry(bert_base, "encoder", BERT_BASE, start_id=101, fp8=True),                 # [CLS]
+    "modernbert-base": ModelEntry(modernbert_base, "encoder", MODERNBERT_BASE, start_id=50281, fp8=True),   # [CLS]
+    "modernbert-large": ModelEntry(modernbert_large, "encoder", MODERNBERT_LARGE, start_id=50281, fp8=True),
     "gpt2": ModelEntry(gpt2, "causal", GPT2, start_id=50256, fp8=True),                               # <|endoftext|>
     "smollm-135m": ModelEntry(smollm_135m, "causal", SMOLLM_135M, start_id=1, fp8=True),              # <s>
     "qwen2.5-1.5b": ModelEntry(qwen2_5_1_5b, "causal", QWEN2_5_1_5B, start_id=151643, fp8=True),      # <|endoftext|>
@@ -55,4 +59,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

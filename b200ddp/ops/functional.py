@@ -56,11 +56,11 @@ class _LinearTC(torch.autograd.Function):
         x2 = x.reshape(-1, x.shape[-1])
         if not x2.is_contiguous():
             x2 = x2.contiguous()
-        if bias is None and activation is not None:
+        if bias is None and activation not in (None, *_GELU_TANH):
             raise ValueError("fused activation needs a bias (use bias=True)")
         if activation in _GELU_TANH:
             # keep the pre-activation for the backward (GELU' needs it): two launches, one extra tensor
-            pre = C.gemm_nt(x2, weight, bias, EPI_BIAS, None)
+            pre = C.gemm_nt(x2, weight, bias, EPI_BIAS if bias is not None else EPI_NONE, None)
             y = C.gelu_fwd(pre, _GELU_TANH[activation])
             ctx.save_for_backward(x2, weight, pre)
         else:
@@ -266,7 +266,7 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
         N, K = weight.shape
         M = x.numel() // K
         if x.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and _tc_ok(M, N, K) \
-                and (bias is not None or activation is None) and os.environ.get("B200DDP_DISABLE_TC", "0") != "1":
+                and (bias is not None or activation in (None, *_GELU_TANH)) and os.environ.get("B200DDP_DISABLE_TC", "0") != "1":
             return _LinearTC.apply(x, weight, bias, activation)
         if x.dtype == torch.float32 and weight.dtype == torch.float32 and N * (K + 1) * 4 <= 48 * 1024 and M * N * 4 <= 48 * 1024 \
                 and activation in (None, "relu"):
@@ -418,6 +418,27 @@ def document_bounds(input_ids: torch.Tensor, cls_token_id: Optional[int], pad_to
     end = torch.minimum(nxt, lens)
     bounds = torch.stack([torch.where(valid, start, 0), torch.where(valid, end, 0)], -1).to(torch.int32)
     return bounds, torch.where(valid, pos - start, 0)
+
+
+def window_bounds(bounds: torch.Tensor, window: int) -> torch.Tensor:
+    """Bidirectional sliding-window bounds inside documents: int32 [B, S, 2] where position i's interval (start, end)
+    becomes (max(start, i - window), min(end, i + window + 1)), so query i sees key j iff both lie in one document and
+    |i - j| <= window (ModernBERT's local attention with ``window = local_attention // 2``).  The mask stays symmetric,
+    which is what ``packed_attention``'s key-side gradient needs, and its kernels skip every tile outside the window.
+    Padding rows (start == end) stay empty; ``window >= S - 1`` returns ``bounds`` itself.  Torch ops on bounds' device,
+    no host synchronisation (CUDA-graph safe).  A negative or non-integer window raises ``ValueError``."""
+    if isinstance(window, bool) or not isinstance(window, int) or window < 0:
+        raise ValueError(f"window_bounds needs a non-negative integer window, got {window!r}")
+    if bounds.dim() != 3 or bounds.shape[-1] != 2 or bounds.is_floating_point() or bounds.is_complex():
+        raise ValueError(f"window_bounds needs integer bounds [B, S, 2], got {bounds.dtype} {tuple(bounds.shape)}")
+    S = bounds.shape[1]
+    if window >= S - 1:
+        return bounds
+    b = bounds.to(torch.int32)
+    i = torch.arange(S, device=b.device, dtype=torch.int32)[None, :]
+    start, end = b[..., 0], b[..., 1]
+    win = torch.stack([torch.maximum(start, i - window), torch.minimum(end, i + window + 1)], -1)
+    return torch.where((start == end)[..., None], b, win)
 
 
 def _bounds_mask(bounds: torch.Tensor, S: int, device) -> torch.Tensor:
@@ -797,6 +818,39 @@ def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
             raise ValueError(f"swiglu on CUDA needs bf16 and I % 8 == 0, got {gate_up.dtype} {tuple(gate_up.shape)}")
         return _SwiGLU.apply(gate_up)
     return _swiglu_reference(gate_up)
+
+
+class _GeGLU(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, input_gate):
+        ctx.save_for_backward(input_gate)
+        return _C().geglu_fwd(input_gate)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (ig,) = ctx.saved_tensors
+        return _C().geglu_bwd(dy.to(ig.dtype).contiguous(), ig)
+
+
+def _geglu_reference(input_gate: torch.Tensor) -> torch.Tensor:
+    a, g = input_gate.to(torch.promote_types(input_gate.dtype, torch.float32)).chunk(2, dim=-1)
+    return (F.gelu(a) * g).to(input_gate.dtype)
+
+
+def geglu(input_gate: torch.Tensor) -> torch.Tensor:
+    """gelu(input) * gate (the erf form of GELU) from one projection [..., 2 * I] with column blocks input | gate; returns
+    [..., I] (ModernBERT's MLP).  CPU: the fp32 reference, differentiated by autograd.  On CUDA: one vectorised pass each
+    way (the backward writes d[input | gate] together); bf16, I % 8 == 0 and a contiguous 16-byte aligned input, else
+    ``ValueError``."""
+    if input_gate.dim() < 1 or input_gate.shape[-1] % 2:
+        raise ValueError(f"geglu needs [..., 2 * I] (input | gate), got {tuple(input_gate.shape)}")
+    if input_gate.is_cuda:
+        if input_gate.dtype != torch.bfloat16 or (input_gate.shape[-1] // 2) % 8:
+            raise ValueError(f"geglu on CUDA needs bf16 and I % 8 == 0, got {input_gate.dtype} {tuple(input_gate.shape)}")
+        if not input_gate.is_contiguous() or input_gate.data_ptr() % 16:
+            raise ValueError("geglu on CUDA needs a contiguous, 16-byte aligned input")
+        return _GeGLU.apply(input_gate)
+    return _geglu_reference(input_gate)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -1254,7 +1308,9 @@ class _LayerNormFused(torch.autograd.Function):
         return dx, dgamma, dbeta, None
 
 
-def layer_norm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
+def layer_norm(x: torch.Tensor, gamma: torch.Tensor, beta: Optional[torch.Tensor], eps: float = 1e-5) -> torch.Tensor:
+    """LayerNorm over the last dimension; ``beta=None`` is the bias-free form (ModernBERT's), which on CUDA runs the same
+    fused kernel with a zero beta whose gradient is dropped."""
     if x.is_cuda and x.dtype in (torch.float32, torch.bfloat16) and gamma.dtype == x.dtype and x.shape[-1] * 8 <= 96 * 1024:
-        return _LayerNormFused.apply(x, gamma, beta, eps)
+        return _LayerNormFused.apply(x, gamma, gamma.new_zeros(gamma.shape) if beta is None else beta, eps)
     return F.layer_norm(x, (x.shape[-1],), gamma, beta, eps)

@@ -129,11 +129,13 @@ class StemConv7x7(nn.Conv2d):
 
 
 class LayerNorm(nn.Module):
-    def __init__(self, hidden: int, eps: float = 1e-5, device=None, dtype=None):
+    """``nn.LayerNorm`` over the last dimension; ``bias=False`` registers only ``weight`` (``nn.LayerNorm(bias=False)``)."""
+
+    def __init__(self, hidden: int, eps: float = 1e-5, device=None, dtype=None, bias: bool = True):
         super().__init__()
         self.eps = eps
         self.weight = nn.Parameter(torch.ones(hidden, device=device, dtype=dtype))
-        self.bias = nn.Parameter(torch.zeros(hidden, device=device, dtype=dtype))
+        self.bias = nn.Parameter(torch.zeros(hidden, device=device, dtype=dtype)) if bias else None
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         return Fn.layer_norm(x, self.weight, self.bias, self.eps)

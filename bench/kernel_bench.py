@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,conv,bn,sgd,adamw,ln,xent,lmloss,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,conv,bn,sgd,adamw,ln,xent,lmloss,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -454,6 +454,76 @@ def main():
         record(f"rotary alone bwd {M}x{W} bf16", timeit(lambda: C.rotary(dy, pos, table, H, Hkv, True), args.iters), bytes_=2 * io,
                note="the floor: rotation without the norm")
         del xg, ag, bg, yt
+
+    if "modernbert" in want:
+        # ModernBERT-base's attention at 2 x 8192 tokens (12 heads, d 64): local layers (window_bounds, +-64) and global
+        # layers on the native document-bounds kernels, against SDPA with the dense [B, 1, S, S] mask each would need
+        # (flash for global attention on fixed rows).  Fixed rows, right-padded rows (lengths U[1024, 8192]) and packed
+        # documents (the CLI's packing, U[1024, 8192]).  FLOPs count the visible pairs only: forward 4 d H sum(end - start),
+        # backward 2.5x that.  Then GeGLU at [16384, 2 x 1152] against F.gelu(a) * g.  The card and its power limit are
+        # part of every number below.
+        import torch.nn.functional as F
+        from b200ddp.data import SyntheticTokens
+        from b200ddp.models import MODEL_REGISTRY
+        from b200ddp.ops import document_bounds, window_bounds
+        print(f"modernbert kernels on {card()}", flush=True)
+        entry = MODEL_REGISTRY["modernbert-base"]
+        B, S, H, d, inter = 2, 8192, 12, 64, entry.config.intermediate
+        w = entry.config.local_attention // 2
+        g = torch.Generator(device="cuda").manual_seed(2)
+        qkv = torch.randn(B * S, 3 * H * d, device=dev, generator=g).to(torch.bfloat16)
+        dout = torch.randn(B * S, H * d, device=dev, generator=g).to(torch.bfloat16)
+        j = torch.arange(S, device=dev)
+        lens = torch.randint(1024, S + 1, (B,), generator=torch.Generator().manual_seed(0)).to(dev)
+        packed = SyntheticTokens(samples=64, seq_len=S, min_len=1024, vocab=entry.config.vocab_size, pack=True,
+                                 cls_token_id=entry.start_id)
+        prow = torch.linspace(0, len(packed) - 1, B).long().tolist()
+        layouts = [("fixed", document_bounds(torch.ones(B, S, dtype=torch.long, device=dev), None, None)[0]),
+                   ("padded U[1024,8192]", document_bounds(torch.where(j[None, :] < lens[:, None], 1, 0), None, 0)[0]),
+                   (f"packed {sum(len(packed.doc_lengths[r]) for r in prow)} docs U[1024,8192]",
+                    document_bounds(packed.X[prow].to(dev), packed.cls_token_id, packed.pad_token_id)[0])]
+        for label, bounds in layouts:
+            for kind, bnd in (("local", window_bounds(bounds, w)), ("global", bounds)):
+                fwd_flops = 4.0 * float((bnd[..., 1] - bnd[..., 0]).sum()) * d * H
+                x = qkv.view(B, S, -1).detach().clone().requires_grad_(True)
+                q, k, v = (t.reshape(B, S, H, d).transpose(1, 2) for t in x.split(H * d, dim=-1))
+                if kind == "global" and label == "fixed":
+                    mask, lib_name = None, "SDPA flash"
+                else:
+                    mask = ((j >= bnd[..., :1]) & (j < bnd[..., 1:]))[:, None]
+                    mask |= torch.eye(S, dtype=torch.bool, device=dev)     # padding rows: their own key, not a NaN row
+                    lib_name = f"SDPA dense {'band' if kind == 'local' else 'block-diagonal'} bool mask"
+
+                def sdpa():
+                    return F.scaled_dot_product_attention(q, k, v, attn_mask=mask).transpose(1, 2).reshape(B, S, H * d)
+                lib = timeit(lambda: sdpa().detach(), args.iters)
+                record(f"modernbert {kind} attention fwd {label} B{B} S{S}",
+                       timeit(lambda: C.packed_attention_fwd(qkv, bnd, H), args.iters), flops=fwd_flops, lib_ms=lib,
+                       note=f"lib = {lib_name} + output transpose")
+                o, lse = C.packed_attention_fwd(qkv, bnd, H)
+                y = sdpa()
+                dy = dout.view(B, S, H * d)
+                lib = timeit(lambda: torch.autograd.grad(y, x, dy, retain_graph=True), args.iters)
+                record(f"modernbert {kind} attention bwd {label} B{B} S{S}",
+                       timeit(lambda: C.packed_attention_bwd(dout, qkv, o, lse, bnd, H), args.iters),
+                       flops=2.5 * fwd_flops, lib_ms=lib, note=f"lib = {lib_name} backward into qkv")
+                del x, q, k, v, y, mask
+        # GeGLU [16384, 2 x 1152] (bytes: input_gate, out; backward input_gate, dy, d[input | gate])
+        M = B * S
+        ig = torch.randn(M, 2 * inter, device=dev).to(torch.bfloat16)
+        dyg = torch.randn(M, inter, device=dev).to(torch.bfloat16)
+
+        def geglu_lib(t):
+            a, b = t.chunk(2, -1)
+            return F.gelu(a) * b
+        record(f"geglu fwd {M}x{inter} bf16", timeit(lambda: C.geglu_fwd(ig), args.iters), bytes_=M * inter * 3 * 2,
+               lib_ms=timeit(lambda: geglu_lib(ig), args.iters), note="lib = F.gelu(a) * g")
+        gg = ig.clone().requires_grad_(True)
+        yg = geglu_lib(gg)
+        record(f"geglu bwd {M}x{inter} bf16", timeit(lambda: C.geglu_bwd(dyg, ig), args.iters), bytes_=M * inter * 5 * 2,
+               lib_ms=timeit(lambda: torch.autograd.grad(yg, gg, dyg, retain_graph=True), args.iters),
+               note="lib = F.gelu(a) * g autograd")
+        del gg, yg
 
     if "conv" in want:
         import torch.nn.functional as F
