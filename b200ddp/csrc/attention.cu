@@ -48,14 +48,11 @@
 #include <cuda.h>
 
 #include "common.h"
-#include "drv.h"
 #include "ops.h"
 #include "tc_primitives.cuh"
+#include "tensor_map.h"
 
 namespace b200 {
-
-CUtensorMap conv_encode_map(const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box);   // conv_wgmma.cu
-
 namespace {
 using namespace tc;
 
@@ -1263,7 +1260,7 @@ CUtensorMap rows_map(const void* ptr, int rows, int cols) {
   const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows};
   const uint64_t strides[1] = {(uint64_t)cols * 2};
   const uint32_t box[2] = {(uint32_t)kHd, (uint32_t)kBoxRows};
-  return conv_encode_map(ptr, 2, dims, strides, box);
+  return encode_tensor_map(ptr, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 2, dims, strides, box);
 }
 
 // heads query heads and kv_heads K/V heads (equal for multi-head attention; a divisor of heads for GQA) of width hd

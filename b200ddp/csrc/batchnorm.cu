@@ -23,8 +23,8 @@
 // partials, a grid barrier makes the partials visible, every CTA reduces its tile's partials in a fixed order and then
 // normalises / applies the gradient straight from shared memory, writing the result back in place and TMA-storing it.
 #include "ops.h"
-#include "drv.h"
 #include "tc_primitives.cuh"
+#include "tensor_map.h"
 
 #include <algorithm>
 #include <cstdlib>
@@ -37,23 +37,6 @@ namespace {
 
 constexpr int kBnThreads = 256;
 constexpr int kVec = 8;              // channels per thread
-
-template <typename T> __device__ __forceinline__ void bn_load8(const T* p, float* f);
-template <> __device__ __forceinline__ void bn_load8<__nv_bfloat16>(const __nv_bfloat16* p, float* f) {
-  unpack8(*reinterpret_cast<const Bf16x8*>(p), f);
-}
-template <> __device__ __forceinline__ void bn_load8<float>(const float* p, float* f) {
-  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-template <typename T> __device__ __forceinline__ void bn_store8(T* p, const float* f);
-template <> __device__ __forceinline__ void bn_store8<__nv_bfloat16>(__nv_bfloat16* p, const float* f) {
-  *reinterpret_cast<Bf16x8*>(p) = pack8(f);
-}
-template <> __device__ __forceinline__ void bn_store8<float>(float* p, const float* f) {
-  reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
-  reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
-}
 
 struct Tile {
   int cvb;       // channel vectors handled by a block (threads along x)
@@ -142,7 +125,7 @@ __global__ void __launch_bounds__(kBnThreads, 2) bn_stats_kernel(const T* __rest
     for (; r + 3 * ty < r1; r += 4 * ty) {              // 4 independent 16-byte loads in flight
       float f[4][kVec];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) bn_load8<T>(base + (size_t)(r + u * ty) * C, f[u]);
+      for (int u = 0; u < 4; ++u) load8<T>(base + (size_t)(r + u * ty) * C, f[u]);
 #pragma unroll
       for (int u = 0; u < 4; ++u)
 #pragma unroll
@@ -150,7 +133,7 @@ __global__ void __launch_bounds__(kBnThreads, 2) bn_stats_kernel(const T* __rest
     }
     for (; r < r1; r += ty) {
       float f[kVec];
-      bn_load8<T>(base + (size_t)r * C, f);
+      load8<T>(base + (size_t)r * C, f);
 #pragma unroll
       for (int i = 0; i < kVec; ++i) { acc[0][i] += f[i]; acc[1][i] = fmaf(f[i], f[i], acc[1][i]); }
     }
@@ -228,16 +211,16 @@ __device__ __forceinline__ void bn_apply_rows(const T* __restrict__ x, const T* 
                                               unsigned char* __restrict__ mask, const float* __restrict__ scale,
                                               const float* __restrict__ shift, int C, int cv, int r0, int r1, int tyi, int ty, int relu) {
   float sc[kVec], sh[kVec];                       // per-channel constants stay in registers for the whole row loop
-  bn_load8<float>(scale + cv * kVec, sc);
-  bn_load8<float>(shift + cv * kVec, sh);
+  load8<float>(scale + cv * kVec, sc);
+  load8<float>(shift + cv * kVec, sh);
   const size_t col = (size_t)cv * kVec;
   int r = r0 + tyi;
   for (; r + 3 * ty < r1; r += 4 * ty) {
     float f[4][kVec], rs[4][kVec];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
-      bn_load8<T>(x + (size_t)(r + u * ty) * C + col, f[u]);
-      if (residual != nullptr) bn_load8<T>(residual + (size_t)(r + u * ty) * C + col, rs[u]);
+      load8<T>(x + (size_t)(r + u * ty) * C + col, f[u]);
+      if (residual != nullptr) load8<T>(residual + (size_t)(r + u * ty) * C + col, rs[u]);
     }
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -249,14 +232,14 @@ __device__ __forceinline__ void bn_apply_rows(const T* __restrict__ x, const T* 
         bits |= (v > 0.f ? 1u : 0u) << i;
         f[u][i] = relu ? fmaxf(v, 0.f) : v;
       }
-      bn_store8<T>(y + (size_t)(r + u * ty) * C + col, f[u]);
+      store8<T>(y + (size_t)(r + u * ty) * C + col, f[u]);
       if (mask != nullptr) mask[(size_t)(r + u * ty) * (C / kVec) + cv] = (unsigned char)bits;
     }
   }
   for (; r < r1; r += ty) {
     float f[kVec], rs[kVec];
-    bn_load8<T>(x + (size_t)r * C + col, f);
-    if (residual != nullptr) bn_load8<T>(residual + (size_t)r * C + col, rs);
+    load8<T>(x + (size_t)r * C + col, f);
+    if (residual != nullptr) load8<T>(residual + (size_t)r * C + col, rs);
     unsigned int bits = 0;
 #pragma unroll
     for (int i = 0; i < kVec; ++i) {
@@ -265,7 +248,7 @@ __device__ __forceinline__ void bn_apply_rows(const T* __restrict__ x, const T* 
       bits |= (v > 0.f ? 1u : 0u) << i;
       f[i] = relu ? fmaxf(v, 0.f) : v;
     }
-    bn_store8<T>(y + (size_t)r * C + col, f);
+    store8<T>(y + (size_t)r * C + col, f);
     if (mask != nullptr) mask[(size_t)r * (C / kVec) + cv] = (unsigned char)bits;
   }
 }
@@ -332,8 +315,8 @@ __global__ void __launch_bounds__(kBnThreads, 2) bn_bwd_reduce_kernel(const T* _
   for (int i = 0; i < kVec; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
   if (cv * kVec < C) {
     float mean[kVec], rstd[kVec];
-    bn_load8<float>(save_mean + cv * kVec, mean);
-    bn_load8<float>(save_rstd + cv * kVec, rstd);
+    load8<float>(save_mean + cv * kVec, mean);
+    load8<float>(save_rstd + cv * kVec, rstd);
     const size_t col = (size_t)cv * kVec;
     int r = r0 + tyi;
     for (; r + ty < r1; r += 2 * ty) {                  // 2 rows x 3 streams = 6 independent 16-byte loads in flight
@@ -342,8 +325,8 @@ __global__ void __launch_bounds__(kBnThreads, 2) bn_bwd_reduce_kernel(const T* _
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
         const size_t off = (size_t)(r + u * ty) * C + col;
-        bn_load8<T>(dy + off, g[u]);
-        bn_load8<T>(x + off, xv[u]);
+        load8<T>(dy + off, g[u]);
+        load8<T>(x + off, xv[u]);
         if (relu) mk[u] = y[(size_t)(r + u * ty) * (C / kVec) + cv];
       }
 #pragma unroll
@@ -358,8 +341,8 @@ __global__ void __launch_bounds__(kBnThreads, 2) bn_bwd_reduce_kernel(const T* _
     for (; r < r1; r += ty) {
       float g[kVec], xv[kVec];
       const size_t off = (size_t)r * C + col;
-      bn_load8<T>(dy + off, g);
-      bn_load8<T>(x + off, xv);
+      load8<T>(dy + off, g);
+      load8<T>(x + off, xv);
       const unsigned int mk = relu ? y[(size_t)r * (C / kVec) + cv] : 0xffu;
 #pragma unroll
       for (int i = 0; i < kVec; ++i) {
@@ -437,11 +420,11 @@ __device__ __forceinline__ void bn_bwd_apply_rows_coef(const T* __restrict__ dy,
   float ka[kVec], kb[kVec], kc[kVec];
   {
     float mean[kVec], rstd[kVec], gam[kVec], c1[kVec], c2[kVec];
-    bn_load8<float>(save_mean + cv * kVec, mean);
-    bn_load8<float>(save_rstd + cv * kVec, rstd);
-    bn_load8<float>(gamma + cv * kVec, gam);
-    bn_load8<float>(c1p, c1);
-    bn_load8<float>(c2p, c2);
+    load8<float>(save_mean + cv * kVec, mean);
+    load8<float>(save_rstd + cv * kVec, rstd);
+    load8<float>(gamma + cv * kVec, gam);
+    load8<float>(c1p, c1);
+    load8<float>(c2p, c2);
 #pragma unroll
     for (int i = 0; i < kVec; ++i) {
       ka[i] = gam[i] * rstd[i];
@@ -457,8 +440,8 @@ __device__ __forceinline__ void bn_bwd_apply_rows_coef(const T* __restrict__ dy,
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
       const size_t off = (size_t)(r + u * ty) * C + col;
-      bn_load8<T>(dy + off, g[u]);
-      bn_load8<T>(x + off, xv[u]);
+      load8<T>(dy + off, g[u]);
+      load8<T>(x + off, xv[u]);
       if (relu) mk[u] = y[(size_t)(r + u * ty) * (C / kVec) + cv];
     }
 #pragma unroll
@@ -470,23 +453,23 @@ __device__ __forceinline__ void bn_bwd_apply_rows_coef(const T* __restrict__ dy,
         if (!((mk[u] >> i) & 1u)) g[u][i] = 0.f;
         o[i] = fmaf(ka[i], g[u][i], fmaf(kb[i], xv[u][i], kc[i]));
       }
-      if (dres != nullptr) bn_store8<T>(dres + off, g[u]);          // gradient of the residual branch = masked dy
-      bn_store8<T>(dx + off, o);
+      if (dres != nullptr) store8<T>(dres + off, g[u]);          // gradient of the residual branch = masked dy
+      store8<T>(dx + off, o);
     }
   }
   for (; r < r1; r += ty) {
     const size_t off = (size_t)r * C + col;
     float g[kVec], xv[kVec], o[kVec];
-    bn_load8<T>(dy + off, g);
-    bn_load8<T>(x + off, xv);
+    load8<T>(dy + off, g);
+    load8<T>(x + off, xv);
     const unsigned int mk = relu ? y[(size_t)r * (C / kVec) + cv] : 0xffu;
 #pragma unroll
     for (int i = 0; i < kVec; ++i) {
       if (!((mk >> i) & 1u)) g[i] = 0.f;
       o[i] = fmaf(ka[i], g[i], fmaf(kb[i], xv[i], kc[i]));
     }
-    if (dres != nullptr) bn_store8<T>(dres + off, g);
-    bn_store8<T>(dx + off, o);
+    if (dres != nullptr) store8<T>(dres + off, g);
+    store8<T>(dx + off, o);
   }
 }
 
@@ -950,7 +933,7 @@ bn_resident_bwd_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_
       float mean[kVec], rstd[kVec];
 #pragma unroll
       for (int i = 0; i < kVec; ++i) { mean[i] = 0.f; rstd[i] = 0.f; }
-      if (live_cv) { bn_load8<float>(save_mean + cvg * kVec, mean); bn_load8<float>(save_rstd + cvg * kVec, rstd); }
+      if (live_cv) { load8<float>(save_mean + cvg * kVec, mean); load8<float>(save_rstd + cvg * kVec, rstd); }
       for (int b = 0; b < nlive; ++b) {
         tc::mbar_wait(&mbar[b], (uint32_t)(w & 1));
         // rows past R and channels past C hold zero dy (TMA zero fill): they add nothing whatever their mask byte says
@@ -1125,17 +1108,10 @@ ResGeom res_launch(const ResPlan& plan, int k) {
 
 // [R, C] bf16, row-major, 64-channel x box_rows boxes, no swizzle; out-of-range rows / channels read as zero, stores clip.
 CUtensorMap res_map(const void* ptr, int R, int C, int box_rows) {
-  auto& drv = Driver::get();
-  if (!drv.TensorMapEncodeTiled) throw std::runtime_error("batch norm: cuTensorMapEncodeTiled unavailable");
-  CUtensorMap map;
-  cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)R};
-  cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-  cuuint32_t box[2] = {(cuuint32_t)kResTile, (cuuint32_t)box_rows};
-  cuuint32_t es[2] = {1, 1};
-  B200_DRV_CHECK(drv.TensorMapEncodeTiled(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, es,
-                                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-  return map;
+  const uint64_t dims[2] = {(uint64_t)C, (uint64_t)R};
+  const uint64_t strides[1] = {(uint64_t)C * 2};
+  const uint32_t box[2] = {(uint32_t)kResTile, (uint32_t)box_rows};
+  return encode_tensor_map(ptr, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_NONE, 2, dims, strides, box);
 }
 
 int res_smem_limit() {
@@ -1187,8 +1163,8 @@ __global__ void __launch_bounds__(kBnThreads) bn_apply_partials_kernel(const T* 
   if (live) {
     for (int g = tyi; g < G; g += ty) {
       float a[kVec], b[kVec];
-      bn_load8<float>(partial + (size_t)g * C + cv * kVec, a);
-      bn_load8<float>(partial + ((size_t)G + g) * C + cv * kVec, b);
+      load8<float>(partial + (size_t)g * C + cv * kVec, a);
+      load8<float>(partial + ((size_t)G + g) * C + cv * kVec, b);
 #pragma unroll
       for (int i = 0; i < kVec; ++i) { acc[0][i] += a[i]; acc[1][i] += b[i]; }
     }
@@ -1249,8 +1225,8 @@ __global__ void __launch_bounds__(kBnThreads) bn_bwd_apply_partials_kernel(const
   if (live) {
     for (int g = tyi; g < G; g += ty) {
       float a[kVec], b[kVec];
-      bn_load8<float>(partial + (size_t)g * C + cv * kVec, a);
-      bn_load8<float>(partial + ((size_t)G + g) * C + cv * kVec, b);
+      load8<float>(partial + (size_t)g * C + cv * kVec, a);
+      load8<float>(partial + ((size_t)G + g) * C + cv * kVec, b);
 #pragma unroll
       for (int i = 0; i < kVec; ++i) { acc[0][i] += a[i]; acc[1][i] += b[i]; }
     }

@@ -11,6 +11,7 @@
 #include "ops.h"
 #include "peer_mem.h"
 #include "reducer.h"
+#include "tensor_map.h"
 
 namespace py = pybind11;
 using namespace b200;
@@ -274,6 +275,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   m.def("launch_count", []() { return (long long)launch_counter().load(); });
   m.def("assign_by_size", &assign_by_size, py::arg("nbytes"), py::arg("keys"), py::arg("limits"), py::arg("max_tensors") = 0);
+  // the 128 bytes of the tensor map the kernels would get for this geometry (tests compare them with recorded ones)
+  m.def("_tensor_map_bytes", [](uintptr_t ptr, int dtype, int swizzle, const std::vector<uint64_t>& dims, const std::vector<uint64_t>& strides,
+                                const std::vector<uint32_t>& box) {
+    TORCH_CHECK(!dims.empty() && dims.size() <= 4 && box.size() == dims.size() && strides.size() + 1 == dims.size(), "tensor map: bad rank");
+    const CUtensorMap map = encode_tensor_map(reinterpret_cast<const void*>(ptr), (CUtensorMapDataType)dtype, (CUtensorMapSwizzle)swizzle,
+                                              (int)dims.size(), dims.data(), strides.data(), box.data());
+    return py::bytes(reinterpret_cast<const char*>(&map), sizeof(map));
+  });
 
   py::class_<PeerArena>(m, "PeerArena")
       .def(py::init<int, int, int, size_t, const std::string&>())

@@ -117,6 +117,23 @@ __device__ __forceinline__ Bf16x8 pack8(const float* f) {
   for (int i = 0; i < 4; ++i) v.h[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
   return v;
 }
+// 8 consecutive elements <-> registers (16-byte / 32-byte vector accesses)
+template <typename T> __device__ __forceinline__ void load8(const T* p, float* f);
+template <> __device__ __forceinline__ void load8<float>(const float* p, float* f) {
+  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+template <> __device__ __forceinline__ void load8<__nv_bfloat16>(const __nv_bfloat16* p, float* f) {
+  unpack8(*reinterpret_cast<const Bf16x8*>(p), f);
+}
+template <typename T> __device__ __forceinline__ void store8(T* p, const float* f);
+template <> __device__ __forceinline__ void store8<float>(float* p, const float* f) {
+  reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
+  reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
+}
+template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16* p, const float* f) {
+  *reinterpret_cast<Bf16x8*>(p) = pack8(f);
+}
 #endif
 
 }  // namespace b200

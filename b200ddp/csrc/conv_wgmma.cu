@@ -23,12 +23,10 @@
 #include "conv.h"
 
 #include <cuda.h>
-#include <mutex>
-#include <unordered_map>
 #include <vector>
 
-#include "drv.h"
 #include "tc_primitives.cuh"
+#include "tensor_map.h"
 
 namespace b200 {
 namespace {
@@ -510,59 +508,9 @@ conv_tap_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
 #undef B200_T0
 #undef B200_T1
 
-// ---------------- host side ------------------------------------------------------------------------
-struct MapKey {
-  const void* ptr; uint64_t d[4]; uint64_t s[3]; uint32_t b[4]; int rank;
-  bool operator==(const MapKey& o) const {
-    if (ptr != o.ptr || rank != o.rank) return false;
-    for (int i = 0; i < 4; ++i) if (d[i] != o.d[i] || b[i] != o.b[i]) return false;
-    for (int i = 0; i < 3; ++i) if (s[i] != o.s[i]) return false;
-    return true;
-  }
-};
-struct MapKeyHash {
-  size_t operator()(const MapKey& k) const {
-    size_t h = std::hash<const void*>()(k.ptr) ^ (size_t)k.rank;
-    for (int i = 0; i < 4; ++i) h = (h * 1000003u) ^ (size_t)k.d[i] ^ ((size_t)k.b[i] << 20);
-    for (int i = 0; i < 3; ++i) h = (h * 1000003u) ^ (size_t)k.s[i];
-    return h;
-  }
-};
-
 }  // namespace
 
-// bf16 tiled tensor map, 128B swizzle, rank <= 4 (dims / box innermost first; strides in bytes for dims 1..rank-1).  Cached:
-// encoding costs a few microseconds on the host and the same (pointer, shape) recurs every step.
-CUtensorMap conv_encode_map(const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box) {
-  static std::mutex mu;
-  static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
-  MapKey key{};
-  key.ptr = ptr; key.rank = rank;
-  for (int i = 0; i < rank; ++i) { key.d[i] = dims[i]; key.b[i] = box[i]; }
-  for (int i = 0; i + 1 < rank; ++i) key.s[i] = strides[i];
-  {
-    std::lock_guard<std::mutex> g(mu);
-    auto it = cache.find(key);
-    if (it != cache.end()) return it->second;
-  }
-  auto& drv = Driver::get();
-  if (!drv.TensorMapEncodeTiled) throw std::runtime_error("conv: cuTensorMapEncodeTiled unavailable");
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) { B200_CUDA_CHECK(cudaFree(nullptr)); ctx_bound = true; }
-  CUtensorMap map;
-  cuuint64_t d[4], s[3];
-  cuuint32_t b[4], es[4] = {1, 1, 1, 1};
-  for (int i = 0; i < rank; ++i) { d[i] = dims[i]; b[i] = box[i]; }
-  for (int i = 0; i + 1 < rank; ++i) s[i] = strides[i];
-  B200_DRV_CHECK(drv.TensorMapEncodeTiled(&map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), d, s, b, es,
-                                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-  std::lock_guard<std::mutex> g(mu);
-  if (cache.size() > 8192) cache.clear();
-  cache.emplace(key, map);
-  return map;
-}
-
+// ---------------- host side ------------------------------------------------------------------------
 bool conv_tile_plan(int N, int H, int W, int R, int S, int want_mode, ConvTilePlan* plan) {
   ConvTilePlan pl;
   const int taps = R * S;
@@ -743,12 +691,12 @@ void launch_conv_tap_gemm(const void* a, const void* w, void* d, int N, int H, i
     uint64_t dm[4] = {(uint64_t)Kc, (uint64_t)M_total, 1, 1};
     uint64_t st[3] = {(uint64_t)Kc * 2, (uint64_t)Kc * 2 * (uint64_t)M_total, (uint64_t)Kc * 2 * (uint64_t)M_total};
     uint32_t bx[4] = {64, 128, 1, 1};
-    ma = conv_encode_map(a, 4, dm, st, bx);
+    ma = encode_tensor_map(a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, dm, st, bx);
   } else {
     uint64_t dm[4] = {(uint64_t)Kc, (uint64_t)W, (uint64_t)H, (uint64_t)N};
     uint64_t st[3] = {(uint64_t)Kc * 2, (uint64_t)W * Kc * 2, (uint64_t)H * W * Kc * 2};
     uint32_t bx[4] = {64, (uint32_t)(pl.mode == 2 ? pl.Wp : W), (uint32_t)(pl.mode == 2 ? pl.BH + 2 : pl.BH), (uint32_t)pl.BI};
-    ma = conv_encode_map(a, 4, dm, st, bx);
+    ma = encode_tensor_map(a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, dm, st, bx);
   }
   // filter map: [Cout, R*S*Cin] row-major
   CUtensorMap mb;
@@ -756,7 +704,7 @@ void launch_conv_tap_gemm(const void* a, const void* w, void* d, int N, int H, i
     uint64_t dm[2] = {(uint64_t)R * S * Cin, (uint64_t)Cout};
     uint64_t st[1] = {(uint64_t)R * S * Cin * 2};
     uint32_t bx[2] = {64, (uint32_t)(dgrad ? 64 : block_n)};
-    mb = conv_encode_map(w, 2, dm, st, bx);
+    mb = encode_tensor_map(w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 2, dm, st, bx);
   }
   // output map: [M_total, Nc] row-major, one dense tile per store
   CUtensorMap md;
@@ -764,7 +712,7 @@ void launch_conv_tap_gemm(const void* a, const void* w, void* d, int N, int H, i
     uint64_t dm[2] = {(uint64_t)Nc, (uint64_t)M_total};
     uint64_t st[1] = {(uint64_t)Nc * 2};
     uint32_t bx[2] = {64, (uint32_t)pl.dense_rows};
-    md = conv_encode_map(d, 2, dm, st, bx);
+    md = encode_tensor_map(d, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 2, dm, st, bx);
   }
 #define B200_CONV_DISPATCH(BN)                                                                         \
   if (block_n == BN) {                                                                                 \
@@ -813,19 +761,19 @@ void launch_stem_conv_fprop(const void* xp, const void* w2, void* y, int N, int 
     uint64_t dm[4] = {64, (uint64_t)g.Wo, (uint64_t)g.Hp2, (uint64_t)N};
     uint64_t st[3] = {32, row_pitch, row_pitch * (uint64_t)g.Hp2};
     uint32_t bx[4] = {64, (uint32_t)g.Wo, 1, 1};
-    ma = conv_encode_map(xp, 4, dm, st, bx);
+    ma = encode_tensor_map(xp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, dm, st, bx);
   }
   {
     uint64_t dm[2] = {(uint64_t)kStemK, (uint64_t)Cout};
     uint64_t st[1] = {(uint64_t)kStemK * 2};
     uint32_t bx[2] = {64, 64};
-    mb = conv_encode_map(w2, 2, dm, st, bx);
+    mb = encode_tensor_map(w2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 2, dm, st, bx);
   }
   {
     uint64_t dm[2] = {(uint64_t)Cout, (uint64_t)M_total};
     uint64_t st[1] = {(uint64_t)Cout * 2};
     uint32_t bx[2] = {64, (uint32_t)g.Wo};
-    md = conv_encode_map(y, 2, dm, st, bx);
+    md = encode_tensor_map(y, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 2, dm, st, bx);
   }
   if (col_stats != nullptr) launch_variant<64, false, 1>(ma, mb, md, p, 0, stream);
   else launch_variant<64, false, 0>(ma, mb, md, p, 0, stream);

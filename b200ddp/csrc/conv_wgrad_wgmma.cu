@@ -14,13 +14,10 @@
 
 #include <cuda.h>
 
-#include "drv.h"
 #include "tc_primitives.cuh"
+#include "tensor_map.h"
 
 namespace b200 {
-
-CUtensorMap conv_encode_map(const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides, const uint32_t* box);   // conv_wgmma.cu
-
 namespace {
 using namespace tc;
 
@@ -321,18 +318,18 @@ void launch_conv_wgrad(const void* dy, const void* x, void* dw, int N, int H, in
     uint64_t dd[4] = {(uint64_t)Cout, (uint64_t)M_total, 1, 1};
     uint64_t ds[3] = {(uint64_t)Cout * 2, (uint64_t)Cout * 2 * (uint64_t)M_total, (uint64_t)Cout * 2 * (uint64_t)M_total};
     uint32_t bx[4] = {64, (uint32_t)p.KB, 1, 1};
-    mdy = conv_encode_map(dy, 4, dd, ds, bx);
+    mdy = encode_tensor_map(dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, dd, ds, bx);
     uint64_t xd[4] = {(uint64_t)Cin, (uint64_t)M_total, 1, 1};
     uint64_t xs[3] = {(uint64_t)Cin * 2, (uint64_t)Cin * 2 * (uint64_t)M_total, (uint64_t)Cin * 2 * (uint64_t)M_total};
-    mx = conv_encode_map(x, 4, xd, xs, bx);
+    mx = encode_tensor_map(x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, xd, xs, bx);
   } else {
     uint32_t bx[4] = {64, (uint32_t)W, (uint32_t)p.BH, (uint32_t)p.BI};
     uint64_t dd[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)N};
     uint64_t ds[3] = {(uint64_t)Cout * 2, (uint64_t)W * Cout * 2, (uint64_t)H * W * Cout * 2};
-    mdy = conv_encode_map(dy, 4, dd, ds, bx);
+    mdy = encode_tensor_map(dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, dd, ds, bx);
     uint64_t xd[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
     uint64_t xs[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-    mx = conv_encode_map(x, 4, xd, xs, bx);
+    mx = encode_tensor_map(x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, xd, xs, bx);
   }
   launch_wgrad_kernel(mdy, mx, pl, stream);
   B200_CUDA_CHECK(cudaGetLastError());
@@ -523,13 +520,13 @@ void launch_stem_conv_wgrad(const void* dy, const void* xp, void* dw2, int N, in
   {
     uint64_t dd[4] = {(uint64_t)Cout, (uint64_t)g.Wo, (uint64_t)g.Ho, (uint64_t)N};
     uint64_t ds[3] = {(uint64_t)Cout * 2, (uint64_t)g.Wo * Cout * 2, (uint64_t)g.Ho * g.Wo * Cout * 2};
-    mdy = conv_encode_map(dy, 4, dd, ds, bx);
+    mdy = encode_tensor_map(dy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, dd, ds, bx);
   }
   {
     const uint64_t row_pitch = (uint64_t)g.Wp * 16;
     uint64_t xd[4] = {64, (uint64_t)g.Wo, (uint64_t)g.Hp2, (uint64_t)N};
     uint64_t xs[3] = {32, row_pitch, row_pitch * (uint64_t)g.Hp2};
-    mx = conv_encode_map(xp, 4, xd, xs, bx);
+    mx = encode_tensor_map(xp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, 4, xd, xs, bx);
   }
   const size_t n = (size_t)Cout * kStemK;
   int split = 0;

@@ -24,11 +24,9 @@
 
 #include <cuda.h>
 #include <cstdlib>
-#include <mutex>
-#include <unordered_map>
 
-#include "drv.h"
 #include "tc_primitives.cuh"
+#include "tensor_map.h"
 
 namespace b200 {
 namespace {
@@ -521,49 +519,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 }
 
 // ---------------- host side ------------------------------------------------------------------------
-struct MapKey {
-  const void* ptr; int rows, cols, box_rows, box_cols, elem_bytes;
-  bool operator==(const MapKey& o) const {
-    return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows && box_cols == o.box_cols && elem_bytes == o.elem_bytes;
-  }
-};
-struct MapKeyHash {
-  size_t operator()(const MapKey& k) const {
-    size_t h = std::hash<const void*>()(k.ptr);
-    for (int v : {k.rows, k.cols, k.box_rows, k.box_cols, k.elem_bytes}) h = h * 1000003u ^ (size_t)v;
-    return h;
-  }
-};
-
 // 2-D row-major tensor [rows, cols] of bf16 (elem_bytes 2) or 8-bit (elem_bytes 1) elements; box = [box_rows, box_cols]
 // with box_cols * elem_bytes == 128 bytes.
 CUtensorMap make_map(const void* ptr, int rows, int cols, int box_rows, int box_cols, int elem_bytes = 2) {
-  static std::mutex mu;
-  static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
-  MapKey key{ptr, rows, cols, box_rows, box_cols, elem_bytes};
-  {
-    std::lock_guard<std::mutex> g(mu);
-    auto it = cache.find(key);
-    if (it != cache.end()) return it->second;
-  }
-  auto& drv = Driver::get();
-  if (!drv.TensorMapEncodeTiled) throw std::runtime_error("gemm: cuTensorMapEncodeTiled unavailable");
-  // driver-API calls need a current context; autograd worker threads only get one lazily from the runtime
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) { B200_CUDA_CHECK(cudaFree(nullptr)); ctx_bound = true; }
-  CUtensorMap map;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * elem_bytes};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t elem_strides[2] = {1, 1};
+  const uint64_t dims[2] = {(uint64_t)cols, (uint64_t)rows};
+  const uint64_t strides[1] = {(uint64_t)cols * elem_bytes};
+  const uint32_t box[2] = {(uint32_t)box_cols, (uint32_t)box_rows};
   const CUtensorMapDataType dt = elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  B200_DRV_CHECK(drv.TensorMapEncodeTiled(&map, dt, 2, const_cast<void*>(ptr), dims, strides, box,
-                                          elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
-  std::lock_guard<std::mutex> g(mu);
-  if (cache.size() > 4096) cache.clear();
-  cache.emplace(key, map);
-  return map;
+  return encode_tensor_map(ptr, dt, CU_TENSOR_MAP_SWIZZLE_128B, 2, dims, strides, box);
 }
 
 // TMA_ST: epilogue through shared memory + TMA store (bf16 output, N % 8 == 0); the D map's box is one warp slab.

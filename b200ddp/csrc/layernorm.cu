@@ -88,23 +88,6 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_bwd_kernel(const T* __re
 // dx = rs * (dy*gamma - xn * mean(dy*gamma*xn)) and dgamma = sum dy * xn from the same column reduction.
 constexpr int kLnChunks = 4;
 
-template <typename T> __device__ __forceinline__ void ln_load8(const T* p, float* f);
-template <> __device__ __forceinline__ void ln_load8<float>(const float* p, float* f) {
-  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-template <> __device__ __forceinline__ void ln_load8<__nv_bfloat16>(const __nv_bfloat16* p, float* f) {
-  unpack8(*reinterpret_cast<const Bf16x8*>(p), f);
-}
-template <typename T> __device__ __forceinline__ void ln_store8(T* p, const float* f);
-template <> __device__ __forceinline__ void ln_store8<float>(float* p, const float* f) {
-  reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
-  reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
-}
-template <> __device__ __forceinline__ void ln_store8<__nv_bfloat16>(__nv_bfloat16* p, const float* f) {
-  *reinterpret_cast<Bf16x8*>(p) = pack8(f);
-}
-
 template <typename T, bool kRms = false>
 __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T* __restrict__ x, const T* __restrict__ gamma,
                                                                         const T* __restrict__ beta, int rows, int cols, float eps,
@@ -116,12 +99,12 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T*
   for (int c = 0; c < kLnChunks; ++c) {
     const int ch = lane + 32 * c;
     if (ch < nchunk) {
-      ln_load8<T>(gamma + 8 * ch, g[c]);
+      load8<T>(gamma + 8 * ch, g[c]);
       if constexpr (kRms) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) b[c][j] = 0.f;
       } else {
-        ln_load8<T>(beta + 8 * ch, b[c]);
+        load8<T>(beta + 8 * ch, b[c]);
       }
     }
   }
@@ -134,7 +117,7 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T*
     for (int c = 0; c < kLnChunks; ++c) {
       const int ch = lane + 32 * c;
       if (ch < nchunk) {
-        ln_load8<T>(xr + 8 * ch, v[c]);
+        load8<T>(xr + 8 * ch, v[c]);
 #pragma unroll
         for (int j = 0; j < 8; ++j) s += v[c][j];
       }
@@ -157,7 +140,7 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_fast_kernel(const T*
         float o[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = kRms ? v[c][j] * rs * g[c][j] : (v[c][j] - mu) * rs * g[c][j] + b[c][j];
-        ln_store8<T>(yr + 8 * ch, o);
+        store8<T>(yr + 8 * ch, o);
       }
     }
     if (lane == 0) {
@@ -178,7 +161,7 @@ __global__ void __launch_bounds__(kLnThreads, 2) layernorm_bwd_dx_kernel(const T
 #pragma unroll
   for (int c = 0; c < kLnChunks; ++c) {
     const int ch = lane + 32 * c;
-    if (ch < nchunk) ln_load8<T>(gamma + 8 * ch, g[c]);
+    if (ch < nchunk) load8<T>(gamma + 8 * ch, g[c]);
   }
   const float inv = 1.f / (float)cols;
   for (int row = blockIdx.x * warps + (threadIdx.x >> 5); row < rows; row += gridDim.x * warps) {
@@ -191,8 +174,8 @@ __global__ void __launch_bounds__(kLnThreads, 2) layernorm_bwd_dx_kernel(const T
     for (int c = 0; c < kLnChunks; ++c) {
       const int ch = lane + 32 * c;
       if (ch < nchunk) {
-        ln_load8<T>(xr + 8 * ch, xn[c]);
-        ln_load8<T>(dyr + 8 * ch, d[c]);
+        load8<T>(xr + 8 * ch, xn[c]);
+        load8<T>(dyr + 8 * ch, d[c]);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           xn[c][j] = (xn[c][j] - mu) * rs;
@@ -212,7 +195,7 @@ __global__ void __launch_bounds__(kLnThreads, 2) layernorm_bwd_dx_kernel(const T
         float o[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = rs * (d[c][j] - s1 - xn[c][j] * s2);
-        ln_store8<T>(dxr + 8 * ch, o);
+        store8<T>(dxr + 8 * ch, o);
       }
     }
   }
@@ -242,10 +225,10 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_param_grad_kernel(const 
     int r = r0 + tyi;
     for (; r + ty < r1; r += 2 * ty) {
       float d0[8], x0[8], d1[8], x1[8];
-      ln_load8<T>(dy + (size_t)r * cols + col, d0);
-      ln_load8<T>(x + (size_t)r * cols + col, x0);
-      ln_load8<T>(dy + (size_t)(r + ty) * cols + col, d1);
-      ln_load8<T>(x + (size_t)(r + ty) * cols + col, x1);
+      load8<T>(dy + (size_t)r * cols + col, d0);
+      load8<T>(x + (size_t)r * cols + col, x0);
+      load8<T>(dy + (size_t)(r + ty) * cols + col, d1);
+      load8<T>(x + (size_t)(r + ty) * cols + col, x1);
       const float m0 = kRms ? 0.f : mean[r], s0 = rstd[r], m1 = kRms ? 0.f : mean[r + ty], s1 = rstd[r + ty];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -256,8 +239,8 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_param_grad_kernel(const 
     }
     for (; r < r1; r += ty) {
       float d0[8], x0[8];
-      ln_load8<T>(dy + (size_t)r * cols + col, d0);
-      ln_load8<T>(x + (size_t)r * cols + col, x0);
+      load8<T>(dy + (size_t)r * cols + col, d0);
+      load8<T>(x + (size_t)r * cols + col, x0);
       const float m0 = kRms ? 0.f : mean[r], s0 = rstd[r];
 #pragma unroll
       for (int i = 0; i < 8; ++i) { ab[i] += d0[i]; ag[i] = fmaf(d0[i], (x0[i] - m0) * s0, ag[i]); }
@@ -320,7 +303,7 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const
 #pragma unroll
   for (int c = 0; c < kRmsWideChunks; ++c) {
     const int ch = threadIdx.x + kRmsWideThreads * c;
-    if (ch < nchunk) ln_load8<T>(gamma + 8 * ch, g[c]);
+    if (ch < nchunk) load8<T>(gamma + 8 * ch, g[c]);
   }
   const float inv = 1.f / (float)cols;
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
@@ -331,7 +314,7 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const
     for (int c = 0; c < kRmsWideChunks; ++c) {
       const int ch = threadIdx.x + kRmsWideThreads * c;
       if (ch < nchunk) {
-        ln_load8<T>(xr + 8 * ch, v[c]);
+        load8<T>(xr + 8 * ch, v[c]);
 #pragma unroll
         for (int j = 0; j < 8; ++j) q += v[c][j] * v[c][j];
       }
@@ -345,7 +328,7 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const
         float o[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = v[c][j] * rs * g[c][j];
-        ln_store8<T>(yr + 8 * ch, o);
+        store8<T>(yr + 8 * ch, o);
       }
     }
     if (threadIdx.x == 0) rstd[row] = rs;
@@ -363,7 +346,7 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(co
 #pragma unroll
   for (int c = 0; c < kRmsWideChunks; ++c) {
     const int ch = threadIdx.x + kRmsWideThreads * c;
-    if (ch < nchunk) ln_load8<T>(gamma + 8 * ch, g[c]);
+    if (ch < nchunk) load8<T>(gamma + 8 * ch, g[c]);
   }
   const float inv = 1.f / (float)cols;
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
@@ -376,8 +359,8 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(co
     for (int c = 0; c < kRmsWideChunks; ++c) {
       const int ch = threadIdx.x + kRmsWideThreads * c;
       if (ch < nchunk) {
-        ln_load8<T>(xr + 8 * ch, xn[c]);
-        ln_load8<T>(dyr + 8 * ch, d[c]);
+        load8<T>(xr + 8 * ch, xn[c]);
+        load8<T>(dyr + 8 * ch, d[c]);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           xn[c][j] *= rs;
@@ -395,7 +378,7 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(co
         float o[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = rs * (d[c][j] - xn[c][j] * s2);
-        ln_store8<T>(dxr + 8 * ch, o);
+        store8<T>(dxr + 8 * ch, o);
       }
     }
   }

@@ -9,19 +9,6 @@ namespace {
 
 constexpr int kLossThreads = 256;
 
-template <typename T> __device__ __forceinline__ void loss_load8(const T* p, float* f);
-template <> __device__ __forceinline__ void loss_load8<__nv_bfloat16>(const __nv_bfloat16* p, float* f) { unpack8(*reinterpret_cast<const Bf16x8*>(p), f); }
-template <> __device__ __forceinline__ void loss_load8<float>(const float* p, float* f) {
-  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-template <typename T> __device__ __forceinline__ void loss_store8(T* p, const float* f);
-template <> __device__ __forceinline__ void loss_store8<__nv_bfloat16>(__nv_bfloat16* p, const float* f) { *reinterpret_cast<Bf16x8*>(p) = pack8(f); }
-template <> __device__ __forceinline__ void loss_store8<float>(float* p, const float* f) {
-  reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
-  reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
-}
-
 template <typename T>
 __global__ void __launch_bounds__(kLossThreads) mse_fwd_bwd_kernel(const T* __restrict__ out, const T* __restrict__ tgt, size_t n,
                                                                    float gscale, float* __restrict__ loss, T* __restrict__ dout,
@@ -40,19 +27,19 @@ __global__ void __launch_bounds__(kLossThreads) mse_fwd_bwd_kernel(const T* __re
     size_t v = tid;
     for (; v + stride < nvec; v += 2 * stride) {            // two independent vector pairs in flight
       float a0[8], b0[8], a1[8], b1[8];
-      loss_load8<T>(out + v * 8, a0); loss_load8<T>(tgt + v * 8, b0);
-      loss_load8<T>(out + (v + stride) * 8, a1); loss_load8<T>(tgt + (v + stride) * 8, b1);
+      load8<T>(out + v * 8, a0); load8<T>(tgt + v * 8, b0);
+      load8<T>(out + (v + stride) * 8, a1); load8<T>(tgt + (v + stride) * 8, b1);
 #pragma unroll
       for (int i = 0; i < 8; ++i) { a0[i] -= b0[i]; acc = fmaf(a0[i], a0[i], acc); a0[i] *= k; a1[i] -= b1[i]; acc = fmaf(a1[i], a1[i], acc); a1[i] *= k; }
-      loss_store8<T>(dout + v * 8, a0);
-      loss_store8<T>(dout + (v + stride) * 8, a1);
+      store8<T>(dout + v * 8, a0);
+      store8<T>(dout + (v + stride) * 8, a1);
     }
     for (; v < nvec; v += stride) {
       float a0[8], b0[8];
-      loss_load8<T>(out + v * 8, a0); loss_load8<T>(tgt + v * 8, b0);
+      load8<T>(out + v * 8, a0); load8<T>(tgt + v * 8, b0);
 #pragma unroll
       for (int i = 0; i < 8; ++i) { a0[i] -= b0[i]; acc = fmaf(a0[i], a0[i], acc); a0[i] *= k; }
-      loss_store8<T>(dout + v * 8, a0);
+      store8<T>(dout + v * 8, a0);
     }
     done = nvec * 8;
   }
@@ -338,11 +325,11 @@ __global__ void __launch_bounds__(kLossThreads) gelu_kernel(const T* __restrict_
     const size_t nvec = n / 8;
     for (size_t v = tid; v < nvec; v += stride) {
       float a[8], g[8];
-      loss_load8<T>(pre + v * 8, a);
-      if (BWD) loss_load8<T>(dy + v * 8, g);
+      load8<T>(pre + v * 8, a);
+      if (BWD) load8<T>(dy + v * 8, g);
 #pragma unroll
       for (int i = 0; i < 8; ++i) a[i] = gelu_op<BWD, TANH>(a[i], g[i]);
-      loss_store8<T>(out + v * 8, a);
+      store8<T>(out + v * 8, a);
     }
     done = nvec * 8;
   }

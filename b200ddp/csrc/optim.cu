@@ -22,23 +22,12 @@ __device__ __forceinline__ int find_tensor(const uint32_t* blk0, int count, uint
   return lo;
 }
 
-// 8 consecutive elements <-> registers (16-byte / 32-byte vector accesses)
-template <typename T> __device__ __forceinline__ void load8(const T* p, float* f);
-template <> __device__ __forceinline__ void load8<float>(const float* p, float* f) {
-  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-template <> __device__ __forceinline__ void load8<__nv_bfloat16>(const __nv_bfloat16* p, float* f) {
+// load8 that copies a bf16 vector into registers before unpacking it, where common.h's load8 unpacks through the pointer.
+// nvcc compiles the two to different code in these kernels, so the optimizer keeps the form it was measured with.
+template <typename T> __device__ __forceinline__ void load8_copy(const T* p, float* f) { load8<T>(p, f); }
+template <> __device__ __forceinline__ void load8_copy<__nv_bfloat16>(const __nv_bfloat16* p, float* f) {
   const Bf16x8 v = *reinterpret_cast<const Bf16x8*>(p);
   unpack8(v, f);
-}
-template <typename T> __device__ __forceinline__ void store8(T* p, const float* f);
-template <> __device__ __forceinline__ void store8<float>(float* p, const float* f) {
-  reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
-  reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
-}
-template <> __device__ __forceinline__ void store8<__nv_bfloat16>(__nv_bfloat16* p, const float* f) {
-  *reinterpret_cast<Bf16x8*>(p) = pack8(f);
 }
 
 template <typename GT>
@@ -59,7 +48,7 @@ __global__ void __launch_bounds__(kOptThreads) multi_sqnorm_kernel(const __grid_
       const uint32_t vend = begin + ((end - begin) & ~7u);
       for (uint32_t v = begin + threadIdx.x * 8; v < vend; v += blockDim.x * 8) {
         float f[8];
-        load8<GT>(g + v, f);
+        load8_copy<GT>(g + v, f);
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc += f[j] * f[j];
       }
@@ -136,8 +125,8 @@ __global__ void __launch_bounds__(kOptThreads) multi_sgd_kernel(const __grid_con
     const uint32_t vend = begin + ((end - begin) & ~7u);
     for (i = begin + threadIdx.x * 8; i < vend; i += blockDim.x * 8) {
       float w[8], gr[8], m[8];
-      load8<GT>(g + i, gr);
-      if (master) load8<float>(master + i, w); else load8<PT>(p + i, w);
+      load8_copy<GT>(g + i, gr);
+      if (master) load8<float>(master + i, w); else load8_copy<PT>(p + i, w);
       if (has_mom) load8<float>(mom + i, m);
 #pragma unroll
       for (int j = 0; j < 8; ++j) w[j] = sgd_update(w[j], gr[j], &m[j], c, has_mom);
@@ -219,8 +208,8 @@ __global__ void __launch_bounds__(kOptThreads) multi_adamw_kernel(const __grid_c
     const uint32_t vend = begin + ((end - begin) & ~7u);
     for (i = begin + threadIdx.x * 8; i < vend; i += blockDim.x * 8) {
       float w[8], gr[8], m[8], v[8];
-      load8<GT>(g + i, gr);
-      if (master) load8<float>(master + i, w); else load8<PT>(p + i, w);
+      load8_copy<GT>(g + i, gr);
+      if (master) load8<float>(master + i, w); else load8_copy<PT>(p + i, w);
       load8<float>(m1 + i, m);
       load8<float>(m2 + i, v);
 #pragma unroll

@@ -10,19 +10,6 @@ namespace {
 
 constexpr int kPoolThreads = 256;
 
-template <typename T> __device__ __forceinline__ void pl_load8(const T* p, float* f);
-template <> __device__ __forceinline__ void pl_load8<__nv_bfloat16>(const __nv_bfloat16* p, float* f) { unpack8(*reinterpret_cast<const Bf16x8*>(p), f); }
-template <> __device__ __forceinline__ void pl_load8<float>(const float* p, float* f) {
-  const float4 a = reinterpret_cast<const float4*>(p)[0], b = reinterpret_cast<const float4*>(p)[1];
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-template <typename T> __device__ __forceinline__ void pl_store8(T* p, const float* f);
-template <> __device__ __forceinline__ void pl_store8<__nv_bfloat16>(__nv_bfloat16* p, const float* f) { *reinterpret_cast<Bf16x8*>(p) = pack8(f); }
-template <> __device__ __forceinline__ void pl_store8<float>(float* p, const float* f) {
-  reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
-  reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
-}
-
 // x [N,H,W,C] -> y [N,OH,OW,C], idx [N,OH,OW,C] (uint8 slot = ky*3+kx)
 template <typename T>
 __global__ void __launch_bounds__(kPoolThreads) maxpool3x3s2_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, unsigned char* __restrict__ idx,
@@ -48,14 +35,14 @@ __global__ void __launch_bounds__(kPoolThreads) maxpool3x3s2_fwd_kernel(const T*
         const int iw = ow * 2 - 1 + kx;
         if (iw < 0 || iw >= W) continue;
         float f[8];
-        pl_load8<T>(x + (((size_t)n * H + ih) * W + iw) * C + cv * 8, f);
+        load8<T>(x + (((size_t)n * H + ih) * W + iw) * C + cv * 8, f);
 #pragma unroll
         for (int i = 0; i < 8; ++i)
           if (f[i] > best[i] || (f[i] != f[i])) { best[i] = f[i]; slot[i] = ky * 3 + kx; }     // first max wins, NaN propagates (torch semantics)
       }
     }
     const size_t o = (((size_t)n * OH + oh) * OW + ow) * C + cv * 8;
-    pl_store8<T>(y + o, best);
+    store8<T>(y + o, best);
     uint2 packed;
     packed.x = slot[0] | (slot[1] << 8) | (slot[2] << 16) | (slot[3] << 24);
     packed.y = slot[4] | (slot[5] << 8) | (slot[6] << 16) | (slot[7] << 24);
@@ -88,7 +75,7 @@ __global__ void __launch_bounds__(kPoolThreads) maxpool3x3s2_bwd_kernel(const T*
         const size_t o = (((size_t)n * OH + oh) * OW + ow) * C + cv * 8;
         const uint2 packed = *reinterpret_cast<const uint2*>(idx + o);
         float g[8];
-        pl_load8<T>(dy + o, g);
+        load8<T>(dy + o, g);
         const unsigned int want = ky * 3 + kx;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -97,7 +84,7 @@ __global__ void __launch_bounds__(kPoolThreads) maxpool3x3s2_bwd_kernel(const T*
         }
       }
     }
-    pl_store8<T>(dx + (((size_t)n * H + ih) * W + iw) * C + cv * 8, acc);
+    store8<T>(dx + (((size_t)n * H + ih) * W + iw) * C + cv * 8, acc);
   }
 }
 
