@@ -444,9 +444,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                 "lm_loss: bad ", name, " output");
     return *given;
   };
-  m.def("lm_loss_fwd", [lm_check, lm_out](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
-                                          long long ignore_index, c10::optional<at::Tensor> lse_out, c10::optional<at::Tensor> row_loss_out) {
+  // rows (optional): int32 [1] device count of the leading rows that carry labels (compact_rows' count).  Only the 128-row tiles
+  // below it are computed; the rows at or past it must be ignored ones, and get lse = row_loss = 0 (dh: zeros).
+  auto rows_ptr = [](const c10::optional<at::Tensor>& rows, const at::Tensor& hidden) -> const int* {
+    if (!rows.has_value()) return nullptr;
+    check_cuda(*rows, "rows");
+    TORCH_CHECK(rows->scalar_type() == at::kInt && rows->numel() == 1 && rows->device() == hidden.device(),
+                "lm_loss: rows must be an int32 [1] tensor on the hidden states' device");
+    return rows->data_ptr<int>();
+  };
+  m.def("lm_loss_fwd", [lm_check, lm_out, rows_ptr](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
+                                                    long long ignore_index, c10::optional<at::Tensor> lse_out, c10::optional<at::Tensor> row_loss_out,
+                                                    c10::optional<at::Tensor> rows) {
     lm_check(hidden, weight, targets, bias);
+    const int* bound = rows_ptr(rows, hidden);
     c10::cuda::CUDAGuard guard(hidden.device());
     const int N = (int)hidden.size(0), H = (int)hidden.size(1), V = (int)weight.size(0), tiles = (V + 127) / 128;
     const auto f32 = hidden.options().dtype(at::kFloat);
@@ -457,20 +468,23 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     at::Tensor target_logit = at::empty({N}, f32);
     const auto* t = (const long long*)targets.data_ptr<int64_t>();
     launch_gemm_lm_lse(hidden.data_ptr(), weight.data_ptr(), bias.has_value() ? bias->data_ptr() : nullptr, N, V, H, t,
-                       partial.data_ptr<float>(), target_logit.data_ptr<float>(), cur_stream());
+                       partial.data_ptr<float>(), target_logit.data_ptr<float>(), cur_stream(), bound);
     launch_lm_loss_combine(partial.data_ptr<float>(), target_logit.data_ptr<float>(), t, N, tiles, V, ignore_index, lse.data_ptr<float>(),
-                           row_loss.data_ptr<float>(), loss.data_ptr<float>(), cur_stream());
+                           row_loss.data_ptr<float>(), loss.data_ptr<float>(), cur_stream(), bound);
     return std::make_tuple(loss, lse, row_loss);
   }, py::arg("hidden"), py::arg("weight"), py::arg("targets"), py::arg("bias") = py::none(), py::arg("ignore_index") = -100,
-     py::arg("lse_out") = py::none(), py::arg("row_loss_out") = py::none());
+     py::arg("lse_out") = py::none(), py::arg("row_loss_out") = py::none(), py::arg("rows") = py::none());
   // Backward, `slice` vocabulary columns at a time: recompute the slice's logits into its bf16 gradient (one GEMM), then
-  // dh += dlogits . weight[slice] (fp32, cast to bf16 once at the end) and dweight[slice] = dlogits^T . hidden.  gscale:
-  // fp32 device scalar (the upstream gradient).  Returns (dh bf16 [N,H] or None, dweight bf16 [V,H] or None).
-  m.def("lm_loss_bwd", [lm_check, lm_out](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
-                                          at::Tensor lse, at::Tensor row_loss, at::Tensor gscale, long long ignore_index, int slice,
-                                          bool need_dh, bool need_dweight, c10::optional<at::Tensor> dh_out,
-                                          c10::optional<at::Tensor> dweight_out) {
+  // dh += dlogits . weight[slice] (fp32, cast to bf16 once at the end), dweight[slice] = dlogits^T . hidden and, with
+  // need_dbias, dbias[slice] = the column sums of dlogits (fixed order).  gscale: fp32 device scalar (the upstream
+  // gradient).  rows: as for lm_loss_fwd.  Returns (dh bf16 [N,H], dweight bf16 [V,H], dbias bf16 [V]; each None when not asked for).
+  m.def("lm_loss_bwd", [lm_check, lm_out, rows_ptr](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
+                                                    at::Tensor lse, at::Tensor row_loss, at::Tensor gscale, long long ignore_index, int slice,
+                                                    bool need_dh, bool need_dweight, c10::optional<at::Tensor> dh_out,
+                                                    c10::optional<at::Tensor> dweight_out, c10::optional<at::Tensor> rows, bool need_dbias) {
     lm_check(hidden, weight, targets, bias);
+    TORCH_CHECK(!need_dbias || bias.has_value(), "lm_loss_bwd: need_dbias needs the bias");
+    const int* bound = rows_ptr(rows, hidden);
     const int N = (int)hidden.size(0), H = (int)hidden.size(1), V = (int)weight.size(0);
     TORCH_CHECK(slice >= 128 && slice % 128 == 0, "lm_loss_bwd: slice must be a positive multiple of 128, got ", slice);
     for (const at::Tensor* t : {&lse, &row_loss, &gscale}) {
@@ -480,36 +494,89 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(lse.numel() == N && row_loss.numel() == N + 1 && gscale.numel() == 1, "lm_loss_bwd: lse [N], row_loss [N+1], gscale [1]");
     c10::cuda::CUDAGuard guard(hidden.device());
     const auto bf16 = hidden.options();
-    at::Tensor dh, dweight, dh32;
+    at::Tensor dh, dweight, dbias, dh32, colsum;
     if (need_dh) {
       dh = lm_out(dh_out, {N, H}, bf16, "dh");
-      dh32 = at::empty({N, H}, bf16.dtype(at::kFloat));
+      // row-bounded: the data-gradient GEMM skips the tiles past the count, whose rows must read as zeros
+      dh32 = bound != nullptr ? at::zeros({N, H}, bf16.dtype(at::kFloat)) : at::empty({N, H}, bf16.dtype(at::kFloat));
     }
     if (need_dweight) dweight = lm_out(dweight_out, {V, H}, bf16, "dweight");
-    if (!need_dh && !need_dweight) return std::make_tuple(dh, dweight);
+    if (need_dbias) dbias = at::empty({V}, bf16);
+    if (!need_dh && !need_dweight && !need_dbias) return std::make_tuple(dh, dweight, dbias);
     const int width = slice < V ? slice : V;
     at::Tensor dlogits = at::empty({(int64_t)N * width}, bf16);
+    if (need_dbias) colsum = at::empty({(int64_t)column_sum_workspace(N, width)}, bf16.dtype(at::kFloat));
     const auto* t = (const long long*)targets.data_ptr<int64_t>();
     const auto* w = reinterpret_cast<const __nv_bfloat16*>(weight.data_ptr());
     const auto* b = bias.has_value() ? reinterpret_cast<const __nv_bfloat16*>(bias->data_ptr()) : nullptr;
     for (int v0 = 0; v0 < V; v0 += width) {
       const int vs = V - v0 < width ? V - v0 : width;
       launch_gemm_lm_dlogits(hidden.data_ptr(), w + (size_t)v0 * H, b ? b + v0 : nullptr, N, vs, H, v0, V, t, ignore_index,
-                             lse.data_ptr<float>(), gscale.data_ptr<float>(), row_loss.data_ptr<float>() + N, dlogits.data_ptr(), cur_stream());
+                             lse.data_ptr<float>(), gscale.data_ptr<float>(), row_loss.data_ptr<float>() + N, dlogits.data_ptr(), cur_stream(),
+                             bound);
       // dh [N,H] (+)= dlogits [N,vs] . weight[v0:v0+vs] (stored [vs,H]: MN-major B)
-      if (need_dh)
+      if (need_dh && bound != nullptr)
+        launch_gemm_bf16_rows(dlogits.data_ptr(), w + (size_t)v0 * H, dh32.data_ptr(), N, H, vs, false, DType::F32, v0 > 0, bound, cur_stream());
+      else if (need_dh)
         launch_gemm_bf16(dlogits.data_ptr(), w + (size_t)v0 * H, dh32.data_ptr(), nullptr, N, H, vs, false, true, 0, DType::F32, v0 > 0,
                          cur_stream());
       // dweight[v0:v0+vs] [vs,H] = dlogits^T (stored [N,vs]: MN-major A) . hidden (stored [N,H]: MN-major B)
-      if (need_dweight)
-        launch_gemm_bf16(dlogits.data_ptr(), hidden.data_ptr(), reinterpret_cast<__nv_bfloat16*>(dweight.data_ptr()) + (size_t)v0 * H,
-                         nullptr, vs, H, N, true, true, 0, DType::BF16, false, cur_stream());
+      auto* dw = need_dweight ? reinterpret_cast<__nv_bfloat16*>(dweight.data_ptr()) + (size_t)v0 * H : nullptr;
+      if (need_dweight && bound != nullptr)
+        launch_gemm_bf16_rows(dlogits.data_ptr(), hidden.data_ptr(), dw, vs, H, N, true, DType::BF16, false, bound, cur_stream());
+      else if (need_dweight)
+        launch_gemm_bf16(dlogits.data_ptr(), hidden.data_ptr(), dw, nullptr, vs, H, N, true, true, 0, DType::BF16, false, cur_stream());
+      if (need_dbias)
+        launch_column_sum(dlogits.data_ptr(), N, vs, bound, colsum.data_ptr<float>(),
+                          reinterpret_cast<__nv_bfloat16*>(dbias.data_ptr()) + v0, cur_stream());
     }
     if (need_dh) dh.copy_(dh32);
-    return std::make_tuple(dh, dweight);
+    return std::make_tuple(dh, dweight, dbias);
   }, py::arg("hidden"), py::arg("weight"), py::arg("targets"), py::arg("bias"), py::arg("lse"), py::arg("row_loss"), py::arg("gscale"),
      py::arg("ignore_index"), py::arg("slice"), py::arg("need_dh") = true, py::arg("need_dweight") = true, py::arg("dh_out") = py::none(),
-     py::arg("dweight_out") = py::none());
+     py::arg("dweight_out") = py::none(), py::arg("rows") = py::none(), py::arg("need_dbias") = false);
+  // Sparse prediction: compact_rows(targets int64 [T], ignore_index, vocab) -> (index int32 [T], count int32 [1], targets int64
+  // [T]): a stable partition of the rows, those whose target is not ignore_index and lies in [0, vocab) first; the compacted
+  // targets hold ignore_index from count on.  No host synchronisation.
+  m.def("compact_rows", [](at::Tensor targets, long long ignore_index, long long vocab) {
+    check_cuda(targets, "targets");
+    TORCH_CHECK(targets.scalar_type() == at::kLong && targets.dim() == 1 && targets.is_contiguous() && targets.numel() >= 1 &&
+                targets.numel() < (1LL << 31), "compact_rows: targets int64 [T], contiguous, 1 <= T < 2^31");
+    TORCH_CHECK(vocab >= 1, "compact_rows: vocab must be positive, got ", vocab);
+    c10::cuda::CUDAGuard guard(targets.device());
+    const int T = (int)targets.numel();
+    const auto i32 = targets.options().dtype(at::kInt);
+    at::Tensor index = at::empty({T}, i32), count = at::empty({1}, i32), out = at::empty_like(targets);
+    at::Tensor work = at::empty({2 * compact_chunks(T)}, i32);
+    launch_compact_rows((const long long*)targets.data_ptr<int64_t>(), T, ignore_index, vocab, work.data_ptr<int>(), index.data_ptr<int>(),
+                        count.data_ptr<int>(), (long long*)out.data_ptr<int64_t>(), cur_stream());
+    return std::make_tuple(index, count, out);
+  }, py::arg("targets"), py::arg("ignore_index"), py::arg("vocab"));
+  auto rows_check = [](const at::Tensor& x, const at::Tensor& index, const at::Tensor& count, const char* name) {
+    check_cuda(x, name); check_cuda(index, "index"); check_cuda(count, "count");
+    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous() && x.size(1) % 8 == 0,
+                name, ": bf16 [T, H] contiguous with H % 8 == 0");
+    TORCH_CHECK(index.scalar_type() == at::kInt && index.is_contiguous() && index.numel() == x.size(0) &&
+                count.scalar_type() == at::kInt && count.numel() == 1, name, ": index int32 [T] and count int32 [1] (compact_rows)");
+    TORCH_CHECK(index.device() == x.device() && count.device() == x.device(), name, ": tensors on different devices");
+  };
+  // gather_rows(x [T, H], index, count): out[r] = x[index[r]] for r < count, zero rows from count on
+  m.def("gather_rows", [rows_check](at::Tensor x, at::Tensor index, at::Tensor count) {
+    rows_check(x, index, count, "gather_rows");
+    c10::cuda::CUDAGuard guard(x.device());
+    at::Tensor out = at::empty_like(x);
+    launch_gather_rows(x.data_ptr(), index.data_ptr<int>(), count.data_ptr<int>(), (int)x.size(0), (int)x.size(1), out.data_ptr(), cur_stream());
+    return out;
+  }, py::arg("x"), py::arg("index"), py::arg("count"));
+  // scatter_rows(dy [T, H], index, count): dx[index[r]] = dy[r] for r < count, every other row of dx zero
+  m.def("scatter_rows", [rows_check](at::Tensor dy, at::Tensor index, at::Tensor count) {
+    rows_check(dy, index, count, "scatter_rows");
+    c10::cuda::CUDAGuard guard(dy.device());
+    at::Tensor dx = at::empty_like(dy);
+    launch_scatter_rows(dy.data_ptr(), index.data_ptr<int>(), count.data_ptr<int>(), (int)dy.size(0), (int)dy.size(1), dx.data_ptr(),
+                        cur_stream());
+    return dx;
+  }, py::arg("dy"), py::arg("index"), py::arg("count"));
 
   // tanh = false: the erf form; true: the tanh approximation
   m.def("gelu_fwd", [](at::Tensor pre, bool tanh) {

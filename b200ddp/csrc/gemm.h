@@ -30,14 +30,23 @@ void launch_gemm_fp8(const void* a, const void* b, void* d, const void* bias, co
 // Fused LM-head cross-entropy GEMMs: logits x = bf16(hidden[M,K] . weight[V,K]^T + bias) on 128 x 128 tiles, never stored.
 // LSE: partial fp32 [ceil(V/128)][M][2] gets each row's (max, sum exp(x - max)) per 128-column tile; target_logit [M] gets
 // x[row, targets[row]] for targets in [0, V) (other rows are not written).  K % 8 == 0.
+// rows (optional): int32 device count; only the 128-row tiles below it are computed, and the other rows of partial and
+// target_logit are not written.
 void launch_gemm_lm_lse(const void* hidden, const void* weight, const void* bias, int M, int V, int K, const long long* targets,
-                        float* partial, float* target_logit, cudaStream_t stream);
+                        float* partial, float* target_logit, cudaStream_t stream, const int* rows = nullptr);
 // Logit gradient of vocabulary columns [col_offset, col_offset + N): weight and bias point at that slice's first row.
 // dlogits bf16 [M, N] = (exp(x - lse[row]) - [col == target]) * gscale / valid, zero for rows whose target is ignore_index
-// or outside [0, vocab); gscale and valid are fp32 device scalars (valid <= 0 gives zeros).
+// or outside [0, vocab); gscale and valid are fp32 device scalars (valid <= 0 gives zeros).  rows (optional): as for the LSE
+// GEMM; the dlogits rows of skipped tiles are not written.
 void launch_gemm_lm_dlogits(const void* hidden, const void* weight, const void* bias, int M, int N, int K, int col_offset, int vocab,
                             const long long* targets, long long ignore_index, const float* lse, const float* gscale,
-                            const float* valid, void* dlogits, cudaStream_t stream);
+                            const float* valid, void* dlogits, cudaStream_t stream, const int* rows = nullptr);
+// The two backward GEMMs of the row-bounded LM loss, bf16 operands, B MN-major, 128 x 128 tiles; rows: int32 device count.
+// a_mn=false (data gradient): A [M, K] K-major, only the 128-row tiles below *rows are computed, D's other rows are not
+// written.  a_mn=true (weight gradient): A stored [K, M], B stored [K, N], the k-loop runs over the first *rows rows rounded
+// up to 64 (those rows must be finite; zero-padded beyond *rows), and zero rows store zeros.
+void launch_gemm_bf16_rows(const void* a, const void* b, void* d, int M, int N, int K, bool a_mn, DType out_dtype, bool accumulate,
+                           const int* rows, cudaStream_t stream);
 
 // Grouped (mixture-of-experts) GEMMs on 128 x 128 tiles, bf16 in and out.  A's rows are sorted by expert into segments that
 // start at multiples of 128, so each 128-row tile belongs to one expert; rows % 128 == 0, N and K multiples of 64.

@@ -51,7 +51,9 @@ struct GemmParams {
   float* col_stats;       // [2][stat_groups][N] per-32-row partial column sums / sums of squares of the stored output, or nullptr
   void* d;
   const __nv_bfloat16* bias;
-  const float* scale_a;   // FP8 only: device scalars 1/s_a, 1/s_b (dequantisation factors)
+  // FP8 only: device scalars 1/s_a, 1/s_b (dequantisation factors).  The row-bounded bf16 modes (kBoundRows, kBoundK)
+  // never dequantise, so their device row count `bound_rows` shares scale_a's bytes.
+  union { const float* scale_a; const int* bound_rows; };
   const float* scale_b;
   // fused LM-head cross-entropy (LM != kLmNone).  Appended after the fields above so that their offsets stay as they
   // were, and kept to 56 bytes: at 128 bytes or less the struct's parameter loads, and the code of every other variant,
@@ -77,6 +79,11 @@ constexpr int kLmNone = 0, kLmLse = 1, kLmDlogits = 2;
 // segments, so every 128-row tile multiplies one expert's B.  kGrpWgrad: D_e = A_e^T B_e per expert e, both operands
 // MN-major, the k-loop running over expert e's segment only.
 constexpr int kGrpNone = 0, kGrpRows = 1, kGrpWgrad = 2;
+// Row-bounded modes, the same tile-schedule slot: only the first *bound_rows rows of A (a device count, so the host never
+// reads it back) carry data.  kBoundRows (A K-major): the schedule walks the 128-row tiles below the count only, so no CTA
+// waits on skipped tiles; D's rows in skipped tiles are not written.  kBoundK (A and B MN-major, the token dimension as K):
+// the k-loop stops at the count rounded up to the k-block; an empty loop stores zeros.
+constexpr int kBoundRows = 3, kBoundK = 4;
 
 // bias / activation on 32 consecutive accumulator columns starting at `col0`
 __device__ __forceinline__ void epilogue_math(const GemmParams& p, int col0, const uint32_t* r, float* v) {
@@ -313,6 +320,15 @@ __device__ __forceinline__ bool grouped_tile(const GemmParams& p, int tile, int 
     *e = __ldg(p.grp_tile_expert + *mb);
     *b_off = *e * p.grp_rows;
     return *e >= 0;
+  } else if constexpr (GRP == kBoundRows) {                    // the live tiles are numbered first, m-fastest
+    const int live_m = min(num_m, (__ldg(p.bound_rows) + BLOCK_M - 1) / BLOCK_M);
+    if (tile >= live_m * num_n) return false;
+    gemm_tile_coords(tile, live_m, num_n, 0, mb, nb);
+    return true;
+  } else if constexpr (GRP == kBoundK) {
+    gemm_tile_coords(tile, num_m, num_n, 0, mb, nb);
+    *kb1 = min(*kb1, (__ldg(p.bound_rows) + BLOCK_K - 1) / BLOCK_K);
+    return true;
   } else {                                                     // expert-major: all tiles of expert 0, then expert 1, ...
     const int per_expert = num_m * num_n;
     *e = tile / per_expert;
@@ -353,9 +369,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   static_assert(sizeof(GemmParams) <= 128, "GemmParams: see the note on the LM-head fields");
   static_assert(LM == kLmNone || (!kFP8 && !A_MN && !B_MN && !TMA_ST && !STATS && !PAIR && BLOCK_N == 128),
                 "LM-head epilogues: bf16 K-major operands, direct epilogue, single-CTA 128 x 128 tiles");
-  static_assert(GRP == kGrpNone || (!kFP8 && LM == kLmNone && !TMA_ST && !STATS && !PAIR && BLOCK_N == 128 &&
-                                    (GRP == kGrpRows ? !A_MN : (A_MN && B_MN))),
+  static_assert(GRP == kGrpNone || GRP >= kBoundRows ||
+                    (!kFP8 && LM == kLmNone && !TMA_ST && !STATS && !PAIR && BLOCK_N == 128 && (GRP == kGrpRows ? !A_MN : (A_MN && B_MN))),
                 "grouped GEMMs: bf16, direct epilogue, single-CTA 128 x 128 tiles; A K-major (rows) or A and B MN-major (wgrad)");
+  static_assert(GRP < kBoundRows || (!kFP8 && !TMA_ST && !STATS && !PAIR && BLOCK_N == 128 &&
+                                     (GRP == kBoundRows ? !A_MN : (A_MN && B_MN && LM == kLmNone))),
+                "row-bounded GEMMs: bf16, direct epilogue, single-CTA 128 x 128 tiles; A K-major (rows) or A and B MN-major (k)");
   constexpr int kBK = kFP8 ? 2 * BLOCK_K : BLOCK_K;            // elements per k-block: one 128-byte row either way
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -447,7 +466,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       const int n0 = nb * BLOCK_N;
       WgAcc<BLOCK_N> acc;
       [[maybe_unused]] WgAcc<BLOCK_N> part;                    // FP8: this k-block's products before promotion
-      if constexpr (kFP8 || GRP == kGrpWgrad) {                // wgrad: an expert without rows runs no wgmma and stores zeros
+      if constexpr (kFP8 || GRP == kGrpWgrad || GRP == kBoundK) {   // an empty k-loop (no rows) runs no wgmma and stores zeros
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 2; ++i) { acc.h[0][i] = 0.f; acc.h[1][i] = 0.f; }
       }
@@ -530,7 +549,8 @@ CUtensorMap make_map(const void* ptr, int rows, int cols, int box_rows, int box_
 }
 
 // TMA_ST: epilogue through shared memory + TMA store (bf16 output, N % 8 == 0); the D map's box is one warp slab.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS = false, bool PAIR = false, int OP = kOpBF16, int LM = kLmNone>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool TMA_ST, bool STATS = false, bool PAIR = false, int OP = kOpBF16, int LM = kLmNone,
+          int GRP = kGrpNone>
 void launch_variant(const void* a, const void* b, const GemmParams& p, cudaStream_t stream) {
   using L = SmemLayout<BLOCK_N, A_MN, B_MN, TMA_ST>;
   constexpr int kSmem = L::kTotal;
@@ -542,7 +562,7 @@ void launch_variant(const void* a, const void* b, const GemmParams& p, cudaStrea
   CUtensorMap map_a = A_MN ? make_map(a, p.K, p.M, BLOCK_K, 64) : make_map(a, p.M, p.K, BLOCK_M, kBK, kEB);
   CUtensorMap map_b = B_MN ? make_map(b, p.K, p.N, BLOCK_K, 64) : make_map(b, p.N, p.K, PAIR ? BLOCK_N / 2 : BLOCK_N, kBK, kEB);
   CUtensorMap map_d = TMA_ST ? make_map(p.d, p.M, p.N, 32, 64) : map_a;       // unused by the direct epilogue
-  auto kernel = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, TMA_ST, STATS, PAIR, OP, LM>;
+  auto kernel = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, TMA_ST, STATS, PAIR, OP, LM, GRP>;
   static std::atomic<unsigned long long> configured{0};
   ensure_max_dynamic_smem(kernel, kSmem, configured);
   if constexpr (PAIR) {
@@ -696,16 +716,18 @@ GemmParams lm_params(int M, int N, int K, const void* bias, const long long* tar
 }  // namespace
 
 void launch_gemm_lm_lse(const void* hidden, const void* weight, const void* bias, int M, int V, int K, const long long* targets,
-                        float* partial, float* target_logit, cudaStream_t stream) {
+                        float* partial, float* target_logit, cudaStream_t stream, const int* rows) {
   GemmParams p = lm_params(M, V, K, bias, targets);
   p.d = partial;
   p.lm_target_logit = target_logit;
-  launch_variant<128, false, false, false, false, false, kOpBF16, kLmLse>(hidden, weight, p, stream);
+  p.bound_rows = rows;
+  if (rows != nullptr) launch_variant<128, false, false, false, false, false, kOpBF16, kLmLse, kBoundRows>(hidden, weight, p, stream);
+  else launch_variant<128, false, false, false, false, false, kOpBF16, kLmLse>(hidden, weight, p, stream);
 }
 
 void launch_gemm_lm_dlogits(const void* hidden, const void* weight, const void* bias, int M, int N, int K, int col_offset, int vocab,
                             const long long* targets, long long ignore_index, const float* lse, const float* gscale,
-                            const float* valid, void* dlogits, cudaStream_t stream) {
+                            const float* valid, void* dlogits, cudaStream_t stream, const int* rows) {
   GemmParams p = lm_params(M, N, K, bias, targets);
   p.d = dlogits;
   p.lm_lse = lse;
@@ -714,7 +736,25 @@ void launch_gemm_lm_dlogits(const void* hidden, const void* weight, const void* 
   p.lm_ignore_index = ignore_index >= 0 && ignore_index < vocab ? (int)ignore_index : -1;
   p.lm_col_offset = col_offset;
   p.lm_vocab = vocab;
-  launch_variant<128, false, false, false, false, false, kOpBF16, kLmDlogits>(hidden, weight, p, stream);
+  p.bound_rows = rows;
+  if (rows != nullptr) launch_variant<128, false, false, false, false, false, kOpBF16, kLmDlogits, kBoundRows>(hidden, weight, p, stream);
+  else launch_variant<128, false, false, false, false, false, kOpBF16, kLmDlogits>(hidden, weight, p, stream);
+}
+
+void launch_gemm_bf16_rows(const void* a, const void* b, void* d, int M, int N, int K, bool a_mn, DType out_dtype, bool accumulate,
+                           const int* rows, cudaStream_t stream) {
+  if (!gemm_shape_supported(M, N, K, a_mn, true)) throw std::runtime_error("gemm_bf16_rows: shape not TMA-compatible (row pitch % 16 B)");
+  if (out_dtype != DType::BF16 && out_dtype != DType::F32) throw std::runtime_error("gemm_bf16_rows: output must be bf16 or fp32");
+  if (accumulate && out_dtype != DType::F32) throw std::runtime_error("gemm_bf16_rows: accumulate needs fp32 output");
+  if (rows == nullptr) throw std::runtime_error("gemm_bf16_rows: missing the device row count");
+  GemmParams p = {};
+  p.M = M; p.N = N; p.K = K;
+  p.out_fp32 = out_dtype == DType::F32 ? 1 : 0;
+  p.accumulate = accumulate ? 1 : 0;
+  p.d = d;
+  p.bound_rows = rows;
+  if (a_mn) launch_variant<128, true, true, false, false, false, kOpBF16, kLmNone, kBoundK>(a, b, p, stream);
+  else launch_variant<128, false, true, false, false, false, kOpBF16, kLmNone, kBoundRows>(a, b, p, stream);
 }
 
 namespace {

@@ -199,19 +199,28 @@ __device__ __forceinline__ float2 lse_merge(float2 a, float2 b) {
 
 // Block = 32 rows x 8 tile groups: thread (x, y) merges tiles y, y + 8, ... of row x in order (a warp reads 32 consecutive
 // rows of one tile: coalesced), then the 8 group results are merged in order.  Deterministic: a fixed order per row.
+// BOUNDED: only the rows below the device count *bound have partials (the row-bounded LSE GEMM skipped the other tiles);
+// the rest get lse = row_loss = 0 without reading them.
 constexpr int kCombineGroups = 8;
+template <bool BOUNDED>
 __global__ void __launch_bounds__(32 * kCombineGroups) lm_lse_combine_kernel(const float2* __restrict__ partial, const float* __restrict__ target_logit,
                                                                              const long long* __restrict__ targets, int rows, int tiles, int cols,
                                                                              long long ignore_index, float* __restrict__ lse,
-                                                                             float* __restrict__ row_loss) {
+                                                                             float* __restrict__ row_loss, const int* __restrict__ bound) {
   __shared__ float2 part[kCombineGroups][32];
   const int row = blockIdx.x * 32 + threadIdx.x;
+  const bool live = row < rows && (!BOUNDED || row < __ldg(bound));
   float2 acc = make_float2(-INFINITY, 0.f);
-  if (row < rows)
+  if (live)
     for (int i = threadIdx.y; i < tiles; i += kCombineGroups) acc = lse_merge(acc, partial[(size_t)i * rows + row]);
   part[threadIdx.y][threadIdx.x] = acc;
   __syncthreads();
   if (threadIdx.y != 0 || row >= rows) return;
+  if (BOUNDED && !live) {
+    lse[row] = 0.f;
+    row_loss[row] = 0.f;
+    return;
+  }
 #pragma unroll
   for (int g = 1; g < kCombineGroups; ++g) acc = lse_merge(acc, part[g][threadIdx.x]);
   const float l = acc.x + __logf(acc.y);
@@ -273,14 +282,226 @@ void launch_xent_fwd_bwd(const void* logits, const long long* targets, DType dt,
 }
 
 void launch_lm_loss_combine(const float* partial, const float* target_logit, const long long* targets, int rows, int tiles, int cols,
-                            long long ignore_index, float* lse, float* row_loss, float* loss, cudaStream_t s) {
+                            long long ignore_index, float* lse, float* row_loss, float* loss, cudaStream_t s, const int* bound) {
   count_valid_kernel<<<1, 1024, 0, s>>>(targets, rows, cols, ignore_index, row_loss + rows);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
-  lm_lse_combine_kernel<<<(rows + 31) / 32, dim3(32, kCombineGroups), 0, s>>>(reinterpret_cast<const float2*>(partial), target_logit, targets,
-                                                                             rows, tiles, cols, ignore_index, lse, row_loss);
+  const auto* pf2 = reinterpret_cast<const float2*>(partial);
+  if (bound != nullptr)
+    lm_lse_combine_kernel<true><<<(rows + 31) / 32, dim3(32, kCombineGroups), 0, s>>>(pf2, target_logit, targets, rows, tiles, cols, ignore_index,
+                                                                                    lse, row_loss, bound);
+  else
+    lm_lse_combine_kernel<false><<<(rows + 31) / 32, dim3(32, kCombineGroups), 0, s>>>(pf2, target_logit, targets, rows, tiles, cols, ignore_index,
+                                                                                     lse, row_loss, nullptr);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
   xent_finish_kernel<<<1, 1024, 0, s>>>(row_loss, targets, rows, cols, ignore_index, loss);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+}  // namespace b200
+
+// ---------------------------------------------------------------------------------------------------------
+// Sparse (masked-row) prediction: the rows that carry a label are compacted to the front on the device, so the LM-head
+// loss runs on them alone, and the bias gradient of the fused loss.  Nothing is read back to the host: the number of
+// labelled rows is a device scalar that the kernels read, and every buffer is sized for all rows.
+//   compact : a stable partition of the rows, labelled first.  Three launches, as the mixture-of-experts sort does it:
+//             per-chunk counts, a one-warp scan over the chunks, and a scatter that re-derives each row's rank with
+//             warp ballots.  No atomics.
+//   gather / scatter : one warp per row, 16-byte copies; rows past the count are written as zeros.
+//   column sum : d[rows, cols] bf16 summed over the rows below the count, per 128-row chunk and then over the chunks,
+//             both in a fixed order (bitwise repeatable).
+namespace b200 {
+namespace {
+
+constexpr int kCompactThreads = 256, kCompactWarps = kCompactThreads / 32;
+constexpr int kCompactChunk = 4 * kCompactThreads;             // rows per count / scatter block: 4 rounds of 256
+
+__device__ __forceinline__ bool labelled(long long t, long long ignore_index, long long vocab) {
+  return t != ignore_index && t >= 0 && t < vocab;
+}
+
+__global__ void __launch_bounds__(kCompactThreads) compact_count_kernel(const long long* __restrict__ targets, int n, long long ignore_index,
+                                                                        long long vocab, int* __restrict__ chunk_counts) {
+  int c = 0;
+#pragma unroll
+  for (int r = 0; r < kCompactChunk / kCompactThreads; ++r) {
+    const int i = blockIdx.x * kCompactChunk + r * kCompactThreads + threadIdx.x;
+    c += __syncthreads_count(i < n && labelled(__ldg(targets + i), ignore_index, vocab));
+  }
+  if (threadIdx.x == 0) chunk_counts[blockIdx.x] = c;
+}
+
+// One warp: exclusive prefix sums of the chunk counts in chunk order, and the total.
+__global__ void __launch_bounds__(32) compact_scan_kernel(const int* __restrict__ chunk_counts, int chunks, int* __restrict__ chunk_base,
+                                                          int* __restrict__ count) {
+  const int lane = threadIdx.x;
+  int run = 0;
+  for (int c0 = 0; c0 < chunks; c0 += 32) {
+    const int v = c0 + lane < chunks ? chunk_counts[c0 + lane] : 0;
+    int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += y;
+    }
+    if (c0 + lane < chunks) chunk_base[c0 + lane] = run + inc - v;
+    run += __shfl_sync(0xffffffffu, inc, 31);
+  }
+  if (lane == 0) *count = run;
+}
+
+// Labelled row i goes to position (labelled rows before it); unlabelled row i to count + (unlabelled rows before it), with
+// its target replaced by ignore_index.  Every position gets exactly one writer.
+__global__ void __launch_bounds__(kCompactThreads) compact_scatter_kernel(const long long* __restrict__ targets, int n, long long ignore_index,
+                                                                          long long vocab, const int* __restrict__ chunk_base,
+                                                                          const int* __restrict__ count, int* __restrict__ index,
+                                                                          long long* __restrict__ targets_out) {
+  __shared__ int warp_counts[kCompactWarps];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int total = __ldg(count);
+  int base = __ldg(chunk_base + blockIdx.x);                   // labelled rows before this round
+#pragma unroll 1
+  for (int r = 0; r < kCompactChunk / kCompactThreads; ++r) {
+    const int i = blockIdx.x * kCompactChunk + r * kCompactThreads + threadIdx.x;
+    const long long t = i < n ? __ldg(targets + i) : ignore_index;
+    const bool lab = i < n && labelled(t, ignore_index, vocab);
+    const unsigned ballot = __ballot_sync(0xffffffffu, lab);
+    if (lane == 0) warp_counts[warp] = __popc(ballot);
+    __syncthreads();
+    int before = base + __popc(ballot & ((1u << lane) - 1u)), round = 0;
+#pragma unroll
+    for (int w = 0; w < kCompactWarps; ++w) {
+      before += w < warp ? warp_counts[w] : 0;
+      round += warp_counts[w];
+    }
+    __syncthreads();                                           // warp_counts is rewritten by the next round
+    if (i < n) {
+      const int pos = lab ? before : total + (i - before);
+      index[pos] = i;
+      targets_out[pos] = lab ? t : ignore_index;
+    }
+    base += round;
+  }
+}
+
+int row_grid(long long rows) {
+  const long long b = (rows + kCompactWarps - 1) / kCompactWarps;
+  return (int)(b < 1 ? 1 : (b > 16LL * kNumSMs ? 16LL * kNumSMs : b));
+}
+
+// out[r] = x[index[r]] for r < *count, zeros after.
+__global__ void __launch_bounds__(kCompactThreads) gather_rows_kernel(const __nv_bfloat16* __restrict__ x, const int* __restrict__ index,
+                                                                      const int* __restrict__ count, int T, int H,
+                                                                      __nv_bfloat16* __restrict__ out) {
+  const int lane = threadIdx.x & 31, vecs = H / 8, live = __ldg(count);
+  for (int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < T; r += (gridDim.x * blockDim.x) >> 5) {
+    Bf16x8* o = reinterpret_cast<Bf16x8*>(out + (size_t)r * H);
+    if (r < live) {
+      const Bf16x8* in = reinterpret_cast<const Bf16x8*>(x + (size_t)__ldg(index + r) * H);
+      for (int v = lane; v < vecs; v += 32) o[v] = in[v];
+    } else {
+      const Bf16x8 z = {};
+      for (int v = lane; v < vecs; v += 32) o[v] = z;
+    }
+  }
+}
+
+// dx[index[r]] = dy[r] for r < *count, zeros for the other rows (index is a permutation: one writer per row of dx).
+__global__ void __launch_bounds__(kCompactThreads) scatter_rows_kernel(const __nv_bfloat16* __restrict__ dy, const int* __restrict__ index,
+                                                                       const int* __restrict__ count, int T, int H,
+                                                                       __nv_bfloat16* __restrict__ dx) {
+  const int lane = threadIdx.x & 31, vecs = H / 8, live = __ldg(count);
+  for (int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < T; r += (gridDim.x * blockDim.x) >> 5) {
+    Bf16x8* o = reinterpret_cast<Bf16x8*>(dx + (size_t)__ldg(index + r) * H);
+    if (r < live) {
+      const Bf16x8* in = reinterpret_cast<const Bf16x8*>(dy + (size_t)r * H);
+      for (int v = lane; v < vecs; v += 32) o[v] = in[v];
+    } else {
+      const Bf16x8 z = {};
+      for (int v = lane; v < vecs; v += 32) o[v] = z;
+    }
+  }
+}
+
+constexpr int kColSumRows = 128, kColSumThreads = 128;
+
+// partial[chunk][col] = sum of d[row, col] over the chunk's rows below the count, in row order; 8 columns per thread.
+__global__ void __launch_bounds__(kColSumThreads) column_sum_kernel(const __nv_bfloat16* __restrict__ d, int rows, int cols,
+                                                                    const int* __restrict__ bound, float* __restrict__ partial) {
+  const int col = (blockIdx.x * kColSumThreads + threadIdx.x) * 8;
+  const int end = bound != nullptr ? min(rows, __ldg(bound)) : rows;
+  const int r0 = blockIdx.y * kColSumRows;
+  if (col >= cols || r0 >= end) return;
+  const int r1 = min(end, r0 + kColSumRows);
+  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll 4
+  for (int r = r0; r < r1; ++r) {
+    float v[8];
+    unpack8(*reinterpret_cast<const Bf16x8*>(d + (size_t)r * cols + col), v);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i] += v[i];
+  }
+  float4* out = reinterpret_cast<float4*>(partial + (size_t)blockIdx.y * cols + col);
+  out[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+  out[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+__global__ void __launch_bounds__(256) column_sum_finish_kernel(const float* __restrict__ partial, int rows, int cols,
+                                                                const int* __restrict__ bound, __nv_bfloat16* __restrict__ out) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x;
+  if (col >= cols) return;
+  const int end = bound != nullptr ? min(rows, __ldg(bound)) : rows;
+  float s = 0.f;
+  for (int c = 0; c * kColSumRows < end; ++c) s += partial[(size_t)c * cols + col];
+  out[col] = __float2bfloat16_rn(s);
+}
+
+void rows_check(const char* name, int T, int H, const void* a, const void* b) {
+  if (T < 1 || H < 8 || H % 8 != 0 || ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15u) != 0)
+    throw std::runtime_error(std::string(name) + ": needs T >= 1, H a positive multiple of 8 and 16-byte aligned rows, got T=" +
+                             std::to_string(T) + " H=" + std::to_string(H));
+}
+
+}  // namespace
+
+int compact_chunks(int T) { return ceil_div(T, kCompactChunk); }
+
+void launch_compact_rows(const long long* targets, int T, long long ignore_index, long long vocab, int* workspace, int* index, int* count,
+                         long long* targets_out, cudaStream_t s) {
+  if (T < 1) throw std::runtime_error("compact_rows: no rows");
+  const int chunks = compact_chunks(T);
+  int* chunk_counts = workspace;
+  int* chunk_base = workspace + chunks;
+  compact_count_kernel<<<chunks, kCompactThreads, 0, s>>>(targets, T, ignore_index, vocab, chunk_counts);
+  B200_CUDA_CHECK(cudaGetLastError());
+  compact_scan_kernel<<<1, 32, 0, s>>>(chunk_counts, chunks, chunk_base, count);
+  B200_CUDA_CHECK(cudaGetLastError());
+  compact_scatter_kernel<<<chunks, kCompactThreads, 0, s>>>(targets, T, ignore_index, vocab, chunk_base, count, index, targets_out);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(3);
+}
+
+void launch_gather_rows(const void* x, const int* index, const int* count, int T, int H, void* out, cudaStream_t s) {
+  rows_check("gather_rows", T, H, x, out);
+  gather_rows_kernel<<<row_grid(T), kCompactThreads, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(x), index, count, T, H,
+                                                             reinterpret_cast<__nv_bfloat16*>(out));
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void launch_scatter_rows(const void* dy, const int* index, const int* count, int T, int H, void* dx, cudaStream_t s) {
+  rows_check("scatter_rows", T, H, dy, dx);
+  scatter_rows_kernel<<<row_grid(T), kCompactThreads, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dy), index, count, T, H,
+                                                              reinterpret_cast<__nv_bfloat16*>(dx));
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+size_t column_sum_workspace(int rows, int cols) { return (size_t)ceil_div(rows, kColSumRows) * cols; }
+
+void launch_column_sum(const void* d, int rows, int cols, const int* bound, float* workspace, void* out, cudaStream_t s) {
+  rows_check("column_sum", rows, cols, d, workspace);
+  const dim3 grid(ceil_div(cols, 8 * kColSumThreads), ceil_div(rows, kColSumRows));
+  column_sum_kernel<<<grid, kColSumThreads, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(d), rows, cols, bound, workspace);
+  B200_CUDA_CHECK(cudaGetLastError());
+  column_sum_finish_kernel<<<ceil_div(cols, 256), 256, 0, s>>>(workspace, rows, cols, bound, reinterpret_cast<__nv_bfloat16*>(out));
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(2);
 }
 
 }  // namespace b200

@@ -64,8 +64,24 @@ void launch_xent_fwd_bwd(const void* logits, const long long* targets, DType dt,
 // Fused LM-head cross-entropy, after launch_gemm_lm_lse (gemm.h): lse[row] from the per-tile partials fp32
 // [tiles][rows][2] (a fixed-order merge), row_loss [rows+1] (lse - target logit, 0 for ignored rows; row_loss[rows] = the
 // number of non-ignored rows) and loss = their mean (0 when every row is ignored).
+// bound (optional): int32 device count; rows at or past it get lse = row_loss = 0 and their partials are not read.
 void launch_lm_loss_combine(const float* partial, const float* target_logit, const long long* targets, int rows, int tiles, int cols,
-                            long long ignore_index, float* lse, float* row_loss, float* loss, cudaStream_t s);
+                            long long ignore_index, float* lse, float* row_loss, float* loss, cudaStream_t s, const int* bound = nullptr);
+
+// Sparse prediction (loss.cu).  compact_rows: a stable partition of T rows, those whose target is not ignore_index and lies
+// in [0, vocab) first.  index int32 [T] (the original row at each position), count int32 [1] (labelled rows), targets_out
+// int64 [T] (the labelled targets, then ignore_index); workspace int32 [2 * compact_chunks(T)].
+int compact_chunks(int T);
+void launch_compact_rows(const long long* targets, int T, long long ignore_index, long long vocab, int* workspace, int* index, int* count,
+                         long long* targets_out, cudaStream_t s);
+// gather_rows: out[r] = x[index[r]] for r < *count, zero rows after; scatter_rows: dx[index[r]] = dy[r] for r < *count and
+// zeros for the other rows of dx (index a permutation of [0, T)).  bf16 [T, H], H % 8 == 0.
+void launch_gather_rows(const void* x, const int* index, const int* count, int T, int H, void* out, cudaStream_t s);
+void launch_scatter_rows(const void* dy, const int* index, const int* count, int T, int H, void* dx, cudaStream_t s);
+// column_sum: out bf16 [cols] = sum over rows r < min(rows, *bound) (all rows when bound is null) of d bf16 [rows, cols],
+// in a fixed order; cols % 8 == 0; workspace fp32 [column_sum_workspace(rows, cols)].
+size_t column_sum_workspace(int rows, int cols);
+void launch_column_sum(const void* d, int rows, int cols, const int* bound, float* workspace, void* out, cudaStream_t s);
 
 // GELU forward: out = gelu(pre); backward: out = dy * gelu'(pre).  One vectorised pass each (loss.cu).  The erf form, or
 // with `tanh` the tanh approximation 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3))) (GPT-2's MLP).

@@ -80,6 +80,10 @@ def build_parser() -> argparse.ArgumentParser:
                    help="LM head and cross-entropy in one op that never builds the [tokens, vocab] logits (the head GEMM runs "
                         f"once more in the backward); needs --model {_names(lambda e: e.kind == 'causal')}, --loss ce, and "
                         "--fp16 on a GPU")
+    p.add_argument("--sparse_prediction", action="store_true",
+                   help="masked-LM encoders: run the vocabulary decoder and its cross-entropy on the labelled (masked) rows "
+                        f"only, compacted on the device; needs --model {_names(lambda e: e.kind == 'encoder')}, --loss ce, and "
+                        "--fp16 on a GPU")
     p.add_argument("--router_aux_loss_coef", type=float, default=None,
                    help=f"mixture-of-experts models ({_names(lambda e: e.moe)}): weight of the router load-balancing loss "
                         "added to the training loss (default: the preset's, 0.001); 0 turns it off and skips its statistics")
@@ -143,6 +147,7 @@ def setup(args):
     check_min_seq_len_args(args)
     check_pack_args(args)
     check_fused_lm_loss_args(args)
+    check_sparse_prediction_args(args)
     check_moe_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
@@ -225,7 +230,8 @@ def check_fused_lm_loss_args(args) -> None:
         return
     if model_entry(args.model).kind != "causal":
         raise ValueError(f"--fused_lm_loss fuses a causal LM's head into its loss; it needs --model "
-                         f"{_names(lambda e: e.kind == 'causal')} (got --model {args.model})")
+                         f"{_names(lambda e: e.kind == 'causal')} (got --model {args.model}); masked-LM encoders decode "
+                         f"their labelled rows only with --sparse_prediction")
     if getattr(args, "loss", None) not in (None, "ce"):
         raise ValueError(f"--fused_lm_loss computes cross-entropy; it needs --loss ce (got --loss {args.loss})")
     if getattr(args, "device", None) is not None and args.device.type == "cuda":
@@ -233,6 +239,25 @@ def check_fused_lm_loss_args(args) -> None:
             raise ValueError("--fused_lm_loss on a GPU needs --fp16: the fused head reads bf16 hidden states and weights")
         if args.local_rank == -1 and getattr(args, "n_gpu", 1) > 1:
             raise ValueError("--fused_lm_loss does not run under single-process multi-GPU DataParallel; launch one process "
+                             "per GPU (torchrun) or make one GPU visible")
+
+
+def check_sparse_prediction_args(args) -> None:
+    """``--sparse_prediction`` moves a masked-LM encoder's decoder into a criterion that scores the labelled rows alone: it
+    needs such a model and ``--loss ce``, bf16 weights on a GPU (the native op is bf16), and a process per GPU
+    (``DataParallel`` would split the head's output across GPUs and gather it back to one)."""
+    if not getattr(args, "sparse_prediction", False):
+        return
+    if model_entry(args.model).kind != "encoder":
+        raise ValueError(f"--sparse_prediction decodes a masked-LM encoder's labelled rows only; it needs --model "
+                         f"{_names(lambda e: e.kind == 'encoder')} (got --model {args.model})")
+    if getattr(args, "loss", None) not in (None, "ce"):
+        raise ValueError(f"--sparse_prediction computes cross-entropy; it needs --loss ce (got --loss {args.loss})")
+    if getattr(args, "device", None) is not None and args.device.type == "cuda":
+        if not args.fp16:
+            raise ValueError("--sparse_prediction on a GPU needs --fp16: the fused decoder reads bf16 hidden states and weights")
+        if args.local_rank == -1 and getattr(args, "n_gpu", 1) > 1:
+            raise ValueError("--sparse_prediction does not run under single-process multi-GPU DataParallel; launch one process "
                              "per GPU (torchrun) or make one GPU visible")
 
 
@@ -282,6 +307,8 @@ def main(argv=None) -> int:
     kwargs = {"fp8": True} if args.fp8 else {}
     if args.fused_lm_loss:
         kwargs["fused_lm_loss"] = True
+    if args.sparse_prediction:
+        kwargs["sparse_prediction"] = True
     if args.router_aux_loss_coef is not None:
         kwargs["router_aux_loss_coef"] = args.router_aux_loss_coef
     if padding_on(args):

@@ -78,11 +78,17 @@ class RouterAuxLoss:
 
 
 def build_criterion(args, model: Optional[torch.nn.Module] = None):
-    """``--loss``'s criterion; with ``--fused_lm_loss`` the model's own head-plus-cross-entropy (``lm_head_loss``).  A
-    model with ``config.router_aux_loss_coef > 0`` (mixture of experts) adds its load-balancing loss (``RouterAuxLoss``)."""
+    """``--loss``'s criterion; with ``--fused_lm_loss`` or ``--sparse_prediction`` the model's own head-plus-cross-entropy
+    (``lm_head_loss``).  A model with ``config.router_aux_loss_coef > 0`` (mixture of experts) adds its load-balancing loss
+    (``RouterAuxLoss``)."""
     if getattr(args, "fused_lm_loss", False):
         if model is None or not getattr(getattr(model, "config", None), "fused_lm_loss", False):
             raise ValueError("--fused_lm_loss needs a causal LM built with fused_lm_loss=True (it has lm_head_loss)")
+        criterion = model.lm_head_loss()
+    elif getattr(args, "sparse_prediction", False):
+        config = getattr(getattr(model, "bert", model), "config", None)
+        if model is None or not getattr(config, "sparse_prediction", False):
+            raise ValueError("--sparse_prediction needs a masked-LM encoder built with sparse_prediction=True (it has lm_head_loss)")
         criterion = model.lm_head_loss()
     else:
         criterion = CrossEntropyLoss() if loss_kind(args) == "ce" else MSELoss()

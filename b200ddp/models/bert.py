@@ -14,7 +14,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops import LayerNorm, Linear, attention, document_bounds, packed_attention
+from ..ops import LayerNorm, Linear, LinearCrossEntropyLoss, attention, document_bounds, packed_attention
 
 
 @dataclass
@@ -32,6 +32,7 @@ class BertConfig:
     fp8: bool = False              # encoder linears (qkv, attn_out, ffn_in, ffn_out) on FP8 tensor cores; same parameters
     pad_token_id: int | None = None  # right-padded input: lengths = non-pad count per row, padded keys hidden (ops.attention)
     cls_token_id: int | None = None  # packed input: a document starts at each such id (and at 0), attention stays inside it
+    sparse_prediction: bool = False  # forward returns the prediction head's output; ``lm_head_loss`` decodes the labelled rows only
 
     @property
     def padded_vocab(self) -> int:
@@ -128,7 +129,9 @@ class BertModel(nn.Module):
 
 
 class BertForMaskedLM(nn.Module):
-    """Encoder + tied-embedding MLM head; forward returns logits [B, S, vocab]."""
+    """Encoder + tied-embedding MLM head; forward returns logits [B, S, vocab].  With ``BertConfig.sparse_prediction``
+    forward stops before the decoder and returns the prediction head's output [B, S, hidden]; ``lm_head_loss()`` is the
+    criterion that decodes only the rows that carry a label (``ops.linear_cross_entropy(sparse=True)``)."""
 
     def __init__(self, config: BertConfig | None = None):
         super().__init__()
@@ -142,8 +145,14 @@ class BertForMaskedLM(nn.Module):
     def forward(self, input_ids, token_type_ids=None, attn_mask=None):
         from ..ops import linear
         h = self.transform_norm(self.transform(self.bert(input_ids, token_type_ids, attn_mask)))
+        if self.bert.config.sparse_prediction:
+            return h
         return linear(h, self.bert.embeddings.word_embeddings.weight, self.decoder_bias)
 
+    def lm_head_loss(self, ignore_index: int = -100) -> LinearCrossEntropyLoss:
+        """Criterion over ``forward``'s head output with ``sparse_prediction``: the tied decoder and its trained bias, read
+        from this model at every call, on the labelled rows only."""
+        return LinearCrossEntropyLoss(lambda: (self.bert.embeddings.word_embeddings.weight, self.decoder_bias), ignore_index, sparse=True)
 
     # ---- interchange with the stock (Hugging Face) parameter naming ---------------------------------------
     _LAYER_MAP = (("attention.output.dense", "attn_out"), ("attention.output.LayerNorm", "attn_norm"),
@@ -199,10 +208,11 @@ BERT_BASE = BertConfig()
 
 
 def bert_base(with_mlm_head: bool = True, fp8: bool = False, pad_token_id: int | None = None,
-              cls_token_id: int | None = None) -> nn.Module:
+              cls_token_id: int | None = None, sparse_prediction: bool = False) -> nn.Module:
     """BERT-base; ``fp8=True`` puts the 48 encoder linears on FP8 tensor cores (embeddings, MLM transform and the tied
     decoder stay bf16).  ``pad_token_id`` takes right-padded input (padded keys are hidden from attention);
     ``cls_token_id`` takes packed documents, each starting with that id (attention stays inside a document and position
-    ids restart in each).  The state dict is the same either way."""
-    c = replace(BERT_BASE, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id)
+    ids restart in each).  ``sparse_prediction=True``: forward returns the MLM head's output and ``lm_head_loss()`` decodes
+    the labelled rows only.  The state dict is the same either way."""
+    c = replace(BERT_BASE, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id, sparse_prediction=sparse_prediction)
     return BertForMaskedLM(replace(c, pad_vocab_to=64)) if with_mlm_head else BertModel(c)

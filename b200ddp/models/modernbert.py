@@ -16,7 +16,7 @@ from dataclasses import dataclass, replace
 import torch
 import torch.nn as nn
 
-from ..ops import LayerNorm, Linear, document_bounds, geglu, linear, packed_attention, rotary, rotary_cos_sin, window_bounds
+from ..ops import LayerNorm, Linear, LinearCrossEntropyLoss, document_bounds, geglu, linear, packed_attention, rotary, rotary_cos_sin, window_bounds
 
 
 @dataclass
@@ -35,6 +35,7 @@ class ModernBertConfig:
     fp8: bool = False                # block linears (Wqkv, attn.Wo, mlp.Wi, mlp.Wo) on FP8 tensor cores; same parameters
     pad_token_id: int | None = None  # right-padded input: length = non-pad count per row
     cls_token_id: int | None = None  # packed input: a document starts at each such id (and at 0), attention stays inside it
+    sparse_prediction: bool = False  # forward returns the head's output; ``lm_head_loss`` decodes the labelled rows only
 
     @property
     def head_dim(self) -> int:
@@ -142,7 +143,9 @@ class ModernBertPredictionHead(nn.Module):
 
 class ModernBertForMaskedLM(nn.Module):
     """Encoder + MLM head; forward returns logits [B, S, vocab].  The decoder's weight is ``tok_embeddings.weight``, so
-    ``state_dict()`` holds Hugging Face's keys without ``decoder.weight``."""
+    ``state_dict()`` holds Hugging Face's keys without ``decoder.weight``.  With ``ModernBertConfig.sparse_prediction``
+    (Hugging Face's name) forward returns the head's output [B, S, hidden] and ``lm_head_loss()`` is the criterion that
+    decodes only the rows that carry a label (``ops.linear_cross_entropy(sparse=True)``)."""
 
     def __init__(self, config: ModernBertConfig | None = None):
         super().__init__()
@@ -174,7 +177,14 @@ class ModernBertForMaskedLM(nn.Module):
 
     def forward(self, input_ids):
         h = self.head(self.model(input_ids))
+        if self.config.sparse_prediction:
+            return h
         return linear(h, self.model.embeddings.tok_embeddings.weight, self.decoder.bias)
+
+    def lm_head_loss(self, ignore_index: int = -100) -> LinearCrossEntropyLoss:
+        """Criterion over ``forward``'s head output with ``sparse_prediction``: the tied decoder and its trained bias, read
+        from this model at every call, on the labelled rows only."""
+        return LinearCrossEntropyLoss(lambda: (self.model.embeddings.tok_embeddings.weight, self.decoder.bias), ignore_index, sparse=True)
 
     def load_hf_state_dict(self, hf: dict) -> None:
         """Load a ``transformers.ModernBertForMaskedLM`` state dict, strictly: the names are the same (``Wqkv`` is fused
@@ -193,14 +203,20 @@ MODERNBERT_BASE = ModernBertConfig()
 MODERNBERT_LARGE = ModernBertConfig(hidden=1024, layers=28, heads=16, intermediate=2624)
 
 
-def modernbert_base(fp8: bool = False, pad_token_id: int | None = None, cls_token_id: int | None = None) -> nn.Module:
+def modernbert_base(fp8: bool = False, pad_token_id: int | None = None, cls_token_id: int | None = None,
+                    sparse_prediction: bool = False) -> nn.Module:
     """ModernBERT-base with its MLM head (8192 positions); ``fp8=True`` puts the 88 block linears on FP8 tensor cores
     (embedding, head and decoder stay bf16).  ``pad_token_id`` takes right-padded input; ``cls_token_id`` takes packed
-    documents, each starting with that id (attention stays inside a document and position ids restart in each)."""
-    return ModernBertForMaskedLM(replace(MODERNBERT_BASE, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id))
+    documents, each starting with that id (attention stays inside a document and position ids restart in each).
+    ``sparse_prediction=True``: forward returns the head's output and ``lm_head_loss()`` decodes the labelled rows only;
+    the state dict is the same."""
+    return ModernBertForMaskedLM(replace(MODERNBERT_BASE, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id,
+                                         sparse_prediction=sparse_prediction))
 
 
-def modernbert_large(fp8: bool = False, pad_token_id: int | None = None, cls_token_id: int | None = None) -> nn.Module:
+def modernbert_large(fp8: bool = False, pad_token_id: int | None = None, cls_token_id: int | None = None,
+                     sparse_prediction: bool = False) -> nn.Module:
     """ModernBERT-large (hidden 1024, 28 layers, 16 heads, GeGLU intermediate 2624; 395,881,664 parameters) with its MLM
     head; ``fp8=True`` puts the 112 block linears on FP8 tensor cores.  The other arguments as for ``modernbert_base``."""
-    return ModernBertForMaskedLM(replace(MODERNBERT_LARGE, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id))
+    return ModernBertForMaskedLM(replace(MODERNBERT_LARGE, fp8=fp8, pad_token_id=pad_token_id, cls_token_id=cls_token_id,
+                                         sparse_prediction=sparse_prediction))

@@ -1228,27 +1228,66 @@ LM_LOSS_SLICE = 4096
 class _LinearCrossEntropy(torch.autograd.Function):
     """Forward: one GEMM whose epilogue reduces each row's logits per 128-column tile to (max, sum exp), then a fixed-order
     merge to the row log-sum-exp and the mean loss.  Backward, per vocabulary slice: the GEMM again, its epilogue writing
-    the bf16 logit gradient, then dh += dlogits . weight[slice] (fp32) and dweight[slice] = dlogits^T . hidden.  The upstream
-    gradient and the valid-row count stay on the device (CUDA-graph safe).  Nothing of size [tokens, vocab] is allocated."""
+    the bf16 logit gradient, then dh += dlogits . weight[slice] (fp32), dweight[slice] = dlogits^T . hidden and, for a
+    trained bias, dbias[slice] = the column sums of dlogits.  The upstream gradient and the valid-row count stay on the
+    device (CUDA-graph safe).  Nothing of size [tokens, vocab] is allocated.  ``rows`` (int32 [1] on the device, or None):
+    only the leading rows below it carry labels, and every GEMM visits only the 128-row tiles below it."""
 
     @staticmethod
-    def forward(ctx, hidden, weight, targets, bias, ignore_index):
+    def forward(ctx, hidden, weight, targets, bias, ignore_index, rows):
         h2 = hidden.reshape(-1, hidden.shape[-1]).contiguous()
         t = targets.reshape(-1).to(torch.long).contiguous()
         w = weight.contiguous()
-        loss, lse, row_loss = _C().lm_loss_fwd(h2, w, t, bias, int(ignore_index))
-        ctx.save_for_backward(h2, w, t, bias, lse, row_loss)
+        b = bias.detach().contiguous() if bias is not None else None
+        loss, lse, row_loss = _C().lm_loss_fwd(h2, w, t, b, int(ignore_index), rows=rows)
+        ctx.save_for_backward(h2, w, t, b, lse, row_loss, rows)
         ctx.ignore_index = int(ignore_index)
         ctx.h_shape = hidden.shape
         return loss
 
     @staticmethod
     def backward(ctx, g):
-        h2, w, t, bias, lse, row_loss = ctx.saved_tensors
+        h2, w, t, b, lse, row_loss, rows = ctx.saved_tensors
         gs = g.detach().float().reshape(1).contiguous()
-        dh, dw = _C().lm_loss_bwd(h2, w, t, bias, lse, row_loss, gs, ctx.ignore_index, LM_LOSS_SLICE,
-                                  ctx.needs_input_grad[0], ctx.needs_input_grad[1])
-        return (dh.view(ctx.h_shape) if dh is not None else None), dw, None, None, None
+        dh, dw, db = _C().lm_loss_bwd(h2, w, t, b, lse, row_loss, gs, ctx.ignore_index, LM_LOSS_SLICE,
+                                      ctx.needs_input_grad[0], ctx.needs_input_grad[1], rows=rows,
+                                      need_dbias=ctx.needs_input_grad[3])
+        return (dh.view(ctx.h_shape) if dh is not None else None), dw, None, db, None, None
+
+
+class _GatherRows(torch.autograd.Function):
+    """out[r] = x[index[r]] for r < count, zero rows after (``compact_rows``' order); the backward scatters the gradient
+    back, exactly zero on the other rows of x."""
+
+    @staticmethod
+    def forward(ctx, x, index, count):
+        ctx.save_for_backward(index, count)
+        return _C().gather_rows(x, index, count)
+
+    @staticmethod
+    def backward(ctx, g):
+        index, count = ctx.saved_tensors
+        return _C().scatter_rows(g.contiguous(), index, count), None, None
+
+
+def compact_rows(targets: torch.Tensor, ignore_index: int = -100, num_classes: Optional[int] = None):
+    """The rows that carry a label, first and in their original order: ``(index int32 [T], count int32 [1], compacted
+    targets int64 [T])`` for targets [T].  A row is labelled by ``cross_entropy``'s rule: its target is not
+    ``ignore_index``, not negative and below ``num_classes`` (no upper bound when None).  ``index`` is a permutation of the
+    rows (the unlabelled ones follow, also in order) and the compacted targets hold ``ignore_index`` from ``count`` on.
+    On CUDA it runs on the device with no host synchronisation, so ``count`` stays there; the CPU body uses
+    ``torch.nonzero``."""
+    if targets.dim() != 1 or targets.is_floating_point() or targets.is_complex() or targets.numel() == 0:
+        raise ValueError(f"compact_rows needs integer targets [T] with T >= 1, got {targets.dtype} {tuple(targets.shape)}")
+    vocab = num_classes if num_classes is not None else torch.iinfo(torch.int64).max
+    t = targets.to(torch.long).contiguous()
+    if t.is_cuda:
+        return _C().compact_rows(t, int(ignore_index), int(vocab))
+    valid = (t != ignore_index) & (t >= 0) & (t < vocab)
+    index = torch.cat([torch.nonzero(valid)[:, 0], torch.nonzero(~valid)[:, 0]]).to(torch.int32)
+    count = valid.sum(dtype=torch.int32).reshape(1)
+    out = torch.where(torch.arange(t.numel()) < count, t[index.long()], torch.full_like(t, ignore_index))
+    return index, count, out
 
 
 def _linear_cross_entropy_reference(hidden, weight, targets, bias, ignore_index):
@@ -1263,12 +1302,17 @@ def _linear_cross_entropy_reference(hidden, weight, targets, bias, ignore_index)
 
 
 def linear_cross_entropy(hidden: torch.Tensor, weight: torch.Tensor, targets: torch.Tensor, bias: Optional[torch.Tensor] = None,
-                         ignore_index: int = -100) -> torch.Tensor:
+                         ignore_index: int = -100, sparse: bool = False) -> torch.Tensor:
     """Mean over non-ignored rows of ``cross_entropy(linear(hidden, weight, bias), targets)``: hidden [..., H], weight [V, H],
     bias [V] or None, targets [...] integer.  Targets equal to ``ignore_index``, negative or >= V are ignored; when every row
     is ignored the loss and the gradients are 0.  On CUDA the [tokens, V] logits are never allocated (``_LinearCrossEntropy``):
-    bf16 hidden / weight / bias, H and V multiples of 8, else ``ValueError``.  The bias is a constant (GPT-2's
-    padded-vocabulary mask): it gets no gradient on CUDA."""
+    bf16 hidden / weight / bias, H and V multiples of 8, else ``ValueError``.  The bias gets a gradient when it requires one
+    (a trained decoder bias); a bias without one (GPT-2's padded-vocabulary mask) is a constant.
+
+    ``sparse=True`` scores the labelled rows alone (masked-LM prediction, where most rows are ignored): they are compacted
+    to the front (``compact_rows``), the head runs on the tiles that hold them, and the hidden-state gradient is scattered
+    back, exactly zero on the other rows.  Same loss and gradients as ``sparse=False``; on CUDA the number of labelled rows
+    stays on the device, so the call captures into a CUDA graph that replays on batches with other counts."""
     if hidden.dim() < 1 or weight.dim() != 2 or weight.shape[1] != hidden.shape[-1] or \
             tuple(targets.shape) != tuple(hidden.shape[:-1]) or (bias is not None and tuple(bias.shape) != (weight.shape[0],)):
         raise ValueError(f"linear_cross_entropy needs hidden [..., H], weight [V, H], targets [...] and bias [V], got hidden "
@@ -1276,18 +1320,24 @@ def linear_cross_entropy(hidden: torch.Tensor, weight: torch.Tensor, targets: to
                          f"{None if bias is None else tuple(bias.shape)}")
     if targets.is_floating_point() or targets.is_complex():
         raise ValueError(f"linear_cross_entropy needs integer targets, got {targets.dtype}")
+    V, H = weight.shape
+    if sparse and hidden.numel() > 0:
+        index, count, targets = compact_rows(targets.reshape(-1), ignore_index, V)
+        h2 = hidden.reshape(-1, H)
+        if not hidden.is_cuda:
+            return _linear_cross_entropy_reference(h2[index.long()], weight, targets, bias, ignore_index)
+        hidden, rows = _GatherRows.apply(h2.contiguous(), index, count), count
+    else:
+        rows = None
     if not hidden.is_cuda:
         return _linear_cross_entropy_reference(hidden, weight, targets, bias, ignore_index)
-    V, H = weight.shape
     if hidden.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16 or (bias is not None and bias.dtype != torch.bfloat16):
         raise ValueError(f"linear_cross_entropy on CUDA needs bf16 hidden, weight and bias, got {hidden.dtype}, {weight.dtype}, "
                          f"{None if bias is None else bias.dtype}")
     if H % 8 or V % 8 or hidden.numel() == 0:
         raise ValueError(f"linear_cross_entropy on CUDA needs H and V multiples of 8 and at least one row, got weight "
                          f"{tuple(weight.shape)}, hidden {tuple(hidden.shape)}")
-    if bias is not None:
-        bias = bias.detach().contiguous()
-    return _LinearCrossEntropy.apply(hidden, weight, targets, bias, ignore_index)
+    return _LinearCrossEntropy.apply(hidden, weight, targets, bias, ignore_index, rows)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -168,17 +168,19 @@ class CrossEntropyLoss(nn.Module):
 
 
 class LinearCrossEntropyLoss(nn.Module):
-    """Criterion over final hidden states: ``linear_cross_entropy(hidden, weight, target, bias)``, where ``head()`` returns
-    the model's current ``(weight, bias or None)`` at every call, so casts and moves of the model (``.to()``,
-    ``to_mixed_bf16``) are followed.  Holds no parameters; the bias is cast to the hidden states' dtype."""
+    """Criterion over final hidden states: ``linear_cross_entropy(hidden, weight, target, bias, sparse=sparse)``, where
+    ``head()`` returns the model's current ``(weight, bias or None)`` at every call, so casts and moves of the model
+    (``.to()``, ``to_mixed_bf16``) are followed.  Holds no parameters; the bias is cast to the hidden states' dtype and
+    gets a gradient when it is a trained parameter.  ``sparse=True`` scores the labelled rows alone (masked-LM heads)."""
 
-    def __init__(self, head, ignore_index: int = -100):
+    def __init__(self, head, ignore_index: int = -100, sparse: bool = False):
         super().__init__()
         self.head = head
         self.ignore_index = ignore_index
+        self.sparse = sparse
 
     def forward(self, hidden: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
         weight, bias = self.head()
         if bias is not None:
             bias = bias.to(hidden.dtype)
-        return Fn.linear_cross_entropy(hidden, weight, target, bias, self.ignore_index)
+        return Fn.linear_cross_entropy(hidden, weight, target, bias, self.ignore_index, sparse=self.sparse)

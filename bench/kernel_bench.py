@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,conv,bn,sgd,adamw,ln,xent,lmloss,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -735,6 +735,55 @@ def main():
                     ms = timeit(lambda: C_.lm_loss_bwd(h.detach(), w.detach(), tt, None, lse, rl, g1, -100, sl), args.iters)
                     record(f"lm-loss qwen bwd slice {sl}", ms, flops=3 * gemm, note=f"dlogits buffer {N * sl * 2 / 1e6:.0f} MB")
             del h, w
+
+    if "sparse" in want:
+        # Sparse masked-LM prediction: the decoder + cross-entropy on the labelled rows only, at the BERT-base (16 x 512,
+        # padded vocabulary 30528) and ModernBERT-base (2 x 8192, 50368) head shapes with 15 % and 30 % of the rows labelled,
+        # against the unfused linear + cross_entropy and the dense fused op, all with the decoder bias trained.  FLOPs count
+        # the useful work: 3 head GEMMs over the labelled rows.  Then compaction + gather + scatter alone, and the rise of
+        # the peak memory over fwd+bwd of each.
+        print(f"sparse prediction on {card()}", flush=True)
+        for label, N, V, H in (("bert", 8192, 30528, 768), ("modernbert", 16384, 50368, 768)):
+            h = torch.randn(N, H, device=dev).to(torch.bfloat16).requires_grad_(True)
+            w = (torch.randn(V, H, device=dev) * 0.02).to(torch.bfloat16).requires_grad_(True)
+            b = torch.zeros(V, device=dev, dtype=torch.bfloat16).requires_grad_(True)
+            for frac in (0.15, 0.30):
+                g = torch.Generator(device=dev).manual_seed(0)
+                t = torch.randint(0, V, (N,), device=dev, generator=g)
+                t = torch.where(torch.rand(N, device=dev, generator=g) < frac, t, torch.full_like(t, -100))
+                labelled = int((t >= 0).sum())
+
+                def unfused():
+                    torch.autograd.grad(Fn.cross_entropy(Fn.linear(h, w, b), t), (h, w, b))
+
+                def dense():
+                    torch.autograd.grad(Fn.linear_cross_entropy(h, w, t, b), (h, w, b))
+
+                def sparse():
+                    torch.autograd.grad(Fn.linear_cross_entropy(h, w, t, b, sparse=True), (h, w, b))
+
+                def compaction():
+                    index, count, _ = Fn.compact_rows(t, -100, V)
+                    C.scatter_rows(C.gather_rows(h.detach(), index, count), index, count)
+
+                def peak_rise(fn):
+                    torch.cuda.synchronize()
+                    base = torch.cuda.memory_allocated()
+                    torch.cuda.reset_peak_memory_stats()
+                    fn()
+                    torch.cuda.synchronize()
+                    return (torch.cuda.max_memory_allocated() - base) / 1e9
+                useful = 3 * 2.0 * labelled * V * H
+                rise = {n: peak_rise(f) for n, f in (("unfused", unfused), ("dense", dense), ("sparse", sparse))}
+                tag = f"{label} {N}x{V}x{H} {int(frac * 100)}% ({labelled} rows)"
+                lib = timeit(unfused, args.iters)
+                dense_ms = timeit(dense, args.iters)
+                record(f"sparse lm-loss {tag}", timeit(sparse, args.iters), flops=useful, lib_ms=lib,
+                       note=f"lib = unfused linear + cross_entropy; dense fused {dense_ms:.3f} ms; peak rise sparse "
+                            f"{rise['sparse']:.2f} GB, dense {rise['dense']:.2f} GB, unfused {rise['unfused']:.2f} GB")
+                record(f"compact+gather+scatter {tag}", timeit(compaction, args.iters), bytes_=N * 8 + 4 * N * H * 2,
+                       note="bytes: targets, and the [T, H] gather and scatter (read + write each)")
+            del h, w, b
 
     if "moe" in want:
         # Granite-3.0-1B-A400M's MoE layer at batch 8 x 2048: T = 16384 tokens, k = 8 of E = 32 experts, H = 1024, I = 512.
