@@ -30,10 +30,145 @@ DType dtype_of(const at::Tensor& t) {
 
 cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
-void check_cuda(const at::Tensor& t, const char* name) {
-  TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor");
-  TORCH_CHECK(t.is_contiguous() || t.is_non_overlapping_and_dense(), name, " must be dense");
+// ---- the argument contract: what every binding accepts -------------------------------------------------------------
+// A binding first checks each tensor argument's dtype, sizes, layout and alignment (Args::operator()), then that all of
+// them are CUDA tensors on one device (Args::device(), which also sets the device guard); only after that does it allocate,
+// take pointers or launch.  Errors read "<binding>: <argument> must be <expected>, got <actual>".
+constexpr int64_t kAny = -1;   // a size that matches any extent
+// kDense: any non-overlapping dense order (the comm bindings); kStrided: any strides, for inputs the binding repairs
+enum Layout { kContiguous, kChannelsLast, kDense, kStrided };
+using Dtypes = std::initializer_list<at::ScalarType>;   // empty: any dtype
+constexpr at::ScalarType kBF16 = at::kBFloat16, kF32 = at::kFloat, kI32 = at::kInt, kI64 = at::kLong, kU8 = at::kByte;
+
+struct Shape {
+  enum Kind { kSizes, kNumel, kMinNumel, kLastDim } kind;
+  at::IntArrayRef sizes;   // kSizes: a view of the caller's list, used within the call
+  int64_t n = 0;
+  Shape(std::initializer_list<int64_t> s) : kind(kSizes), sizes(s) {}
+  Shape(at::IntArrayRef s) : kind(kSizes), sizes(s) {}
+  Shape(Kind k, int64_t v) : kind(k), n(v) {}
+};
+Shape numel(int64_t n) { return Shape(Shape::kNumel, n); }
+Shape min_numel(int64_t n) { return Shape(Shape::kMinNumel, n); }
+Shape last_dim(int64_t n) { return Shape(Shape::kLastDim, n); }   // [..., n]; kAny: any tensor of at least one dim
+
+bool misaligned(const at::Tensor& t, int align) { return align > 1 && reinterpret_cast<uintptr_t>(t.data_ptr()) % align != 0; }
+
+// a copy of t when its address is not a multiple of `align` bytes (the kernel's vector width)
+at::Tensor aligned(const at::Tensor& t, int align) { return misaligned(t, align) ? t.clone() : t; }
+
+// "[2, *, 4]" (kAny as *)
+std::string sizes_str(at::IntArrayRef sizes) {
+  std::string s = "[";
+  for (size_t i = 0; i < sizes.size(); ++i) s += (i ? ", " : "") + (sizes[i] == kAny ? std::string("*") : std::to_string(sizes[i]));
+  return s + "]";
 }
+
+std::string describe(const at::Tensor& t, int align = 0) {
+  std::string s = std::string(c10::toString(t.scalar_type())) + " " + sizes_str(t.sizes()) +
+                  (t.is_contiguous() ? " contiguous" : t.dim() == 4 && t.is_contiguous(at::MemoryFormat::ChannelsLast) ? " channels_last" : " strided");
+  if (misaligned(t, align))
+    s += " at an address " + std::to_string(reinterpret_cast<uintptr_t>(t.data_ptr()) % align) + " bytes past a multiple of " + std::to_string(align);
+  return s;
+}
+
+class Args {
+ public:
+  explicit Args(const char* fn) : fn_(fn) {}
+  const char* fn() const { return fn_; }
+
+  // shape check of one tensor argument
+  Args& operator()(const char* name, const at::Tensor& t, Dtypes dtypes, const Shape& shape, Layout layout = kContiguous, int align = 0) {
+    const bool ok = (dtypes.size() == 0 || std::find(dtypes.begin(), dtypes.end(), t.scalar_type()) != dtypes.end()) && fits(t, shape) &&
+                    laid_out(t, layout) && !misaligned(t, align);
+    if (!ok) fail(name, expected(dtypes, shape, layout, align), describe(t, align));
+    seen_.push_back({name, &t});
+    return *this;
+  }
+  // an optional argument is checked only when present
+  Args& operator()(const char* name, const c10::optional<at::Tensor>& t, Dtypes dtypes, const Shape& shape, Layout layout = kContiguous,
+                   int align = 0) {
+    return t.has_value() ? (*this)(name, *t, dtypes, shape, layout, align) : *this;
+  }
+  // an optional argument this call needs
+  const at::Tensor& required(const char* name, const c10::optional<at::Tensor>& t) const {
+    if (!t.has_value()) fail(name, "a tensor", "None");
+    return *t;
+  }
+  // a relation between arguments that their shapes cannot state
+  void expect(bool ok, const char* name, const char* what, const at::Tensor& t) const {
+    if (!ok) fail(name, what, describe(t));
+  }
+  // A caller-owned output: when given, it is checked like an argument (contiguous, as many elements as `sizes`, opt's dtype
+  // or one of `accept`) and used; otherwise device() allocates it with `sizes` and `opt`.
+  void out(at::Tensor& dst, const char* name, const c10::optional<at::Tensor>& given, at::IntArrayRef sizes, const at::TensorOptions& opt,
+           int align = 0, Dtypes accept = {}) {
+    if (!given.has_value()) {
+      pending_.push_back({&dst, c10::SmallVector<int64_t, 4>(sizes.begin(), sizes.end()), opt});
+      return;
+    }
+    const Shape count = numel(c10::multiply_integers(sizes));
+    if (accept.size() == 0) (*this)(name, *given, {opt.dtype().toScalarType()}, count, kContiguous, align);
+    else (*this)(name, *given, accept, count, kContiguous, align);
+    dst = *given;
+  }
+  // Every tensor argument is a CUDA tensor on one device: set the guard to it, then allocate the outputs not given.
+  void device() {
+    const at::Tensor& first = *seen_[0].second;
+    for (const auto& [name, t] : seen_) {
+      if (!t->is_cuda()) fail(name, "a CUDA tensor", t->device().str());
+      if (t->device() != first.device()) fail(name, std::string("on ") + seen_[0].first + "'s device " + first.device().str(), t->device().str());
+    }
+    guard_.set_device(first.device());
+    for (auto& p : pending_) *p.dst = at::empty(p.sizes, p.opt);
+  }
+  [[noreturn]] void fail(const char* name, const std::string& want, const std::string& got) const {
+    TORCH_CHECK(false, fn_, ": ", name, " must be ", want, ", got ", got);
+  }
+
+ private:
+  static bool fits(const at::Tensor& t, const Shape& s) {
+    switch (s.kind) {
+      case Shape::kNumel: return t.numel() == s.n;
+      case Shape::kMinNumel: return t.numel() >= s.n;
+      case Shape::kLastDim: return t.dim() >= 1 && (s.n == kAny || t.size(-1) == s.n);
+      default:
+        if (t.dim() != (int64_t)s.sizes.size()) return false;
+        for (size_t i = 0; i < s.sizes.size(); ++i)
+          if (s.sizes[i] != kAny && s.sizes[i] != t.size((int64_t)i)) return false;
+        return true;
+    }
+  }
+  static bool laid_out(const at::Tensor& t, Layout l) {
+    switch (l) {
+      case kContiguous: return t.is_contiguous();
+      case kChannelsLast: return t.dim() == 4 && t.is_contiguous(at::MemoryFormat::ChannelsLast);
+      case kDense: return t.is_contiguous() || t.is_non_overlapping_and_dense();
+      default: return true;
+    }
+  }
+  static std::string expected(Dtypes dtypes, const Shape& s, Layout l, int align) {
+    std::string o = dtypes.size() == 0 ? "any dtype" : "";
+    for (auto it = dtypes.begin(); it != dtypes.end(); ++it) o += (it == dtypes.begin() ? "" : " or ") + std::string(c10::toString(*it));
+    switch (s.kind) {
+      case Shape::kNumel: o += " of " + std::to_string(s.n) + " elements"; break;
+      case Shape::kMinNumel: o += " of at least " + std::to_string(s.n) + " elements"; break;
+      case Shape::kLastDim: o += " [..., " + (s.n == kAny ? std::string("*") : std::to_string(s.n)) + "]"; break;
+      default: o += " " + sizes_str(s.sizes);
+    }
+    o += l == kContiguous ? " contiguous" : l == kChannelsLast ? " channels_last" : l == kDense ? " dense" : "";
+    return align > 1 ? o + ", " + std::to_string(align) + "-byte aligned" : o;
+  }
+  struct Pending {
+    at::Tensor* dst;
+    c10::SmallVector<int64_t, 4> sizes;
+    at::TensorOptions opt;
+  };
+  const char* fn_;
+  c10::SmallVector<std::pair<const char*, const at::Tensor*>, 8> seen_;
+  c10::SmallVector<Pending, 2> pending_;
+  c10::cuda::OptionalCUDAGuard guard_;
+};
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
   CommCtx c;
@@ -54,6 +189,11 @@ void allreduce_tensors(PeerArena& arena, const std::vector<at::Tensor>& tensors,
                        int blocks, size_t stage_off, size_t stage_bytes, double scale, int pad_set, double timeout_s,
                        c10::optional<at::Tensor> sq_partials) {
   TORCH_CHECK(!tensors.empty() && (int)tensors.size() <= kMaxBucketTensors, "allreduce_tensors: 1..", kMaxBucketTensors, " tensors");
+  Args args("allreduce_tensors");
+  args("tensors", tensors[0], {kF32, kBF16}, min_numel(0), kDense);
+  for (const at::Tensor& t : tensors) args("tensors", t, {tensors[0].scalar_type()}, min_numel(0), kDense);
+  args("sq_partials", sq_partials, {kF32}, min_numel(0));
+  args.device();
   const DType in_dt = dtype_of(tensors[0]);
   const DType wire_dt = wire == "fp32" ? DType::F32 : DType::BF16;
   BucketTable tab;
@@ -61,8 +201,6 @@ void allreduce_tensors(PeerArena& arena, const std::vector<at::Tensor>& tensors,
   tab.count = (int)tensors.size();
   for (int k = 0; k < tab.count; ++k) {
     const at::Tensor& t = tensors[k];
-    check_cuda(t, "tensor");
-    TORCH_CHECK(dtype_of(t) == in_dt, "allreduce_tensors: mixed dtypes in one bucket");
     tab.t[k].ptr = t.data_ptr();
     tab.t[k].numel = (uint32_t)t.numel();
     tab.t[k].off = off;
@@ -82,6 +220,10 @@ void allreduce_tensors(PeerArena& arena, const std::vector<at::Tensor>& tensors,
 // Broadcast arbitrary tensors from `src`; chunked through the staging region.
 int broadcast_tensors(PeerArena& arena, const std::vector<at::Tensor>& tensors, int src, size_t stage_off,
                       size_t stage_bytes, bool use_mc, int blocks, int pad_set, double timeout_s) {
+  if (tensors.empty()) return 0;
+  Args args("broadcast_tensors");
+  for (const at::Tensor& t : tensors) args("tensors", t, {}, min_numel(0), kDense);
+  args.device();
   CommCtx ctx = make_ctx(arena, (size_t)pad_set * kPadSetBytes, timeout_s);
   int launches = 0;
   size_t i = 0;
@@ -94,7 +236,6 @@ int broadcast_tensors(PeerArena& arena, const std::vector<at::Tensor>& tensors, 
     uint32_t off = 0;
     while (i < n && tab.count < kMaxBucketTensors) {
       const at::Tensor& t = tensors[i];
-      check_cuda(t, "tensor");
       const size_t nbytes = (size_t)t.numel() * t.element_size() - piece_off;
       const size_t room = stage_bytes - off;
       if (room < 16) break;
@@ -115,6 +256,14 @@ int broadcast_tensors(PeerArena& arena, const std::vector<at::Tensor>& tensors, 
     ++launches;
   }
   return launches;
+}
+
+// peer_pull / peer_push: `bytes` between the arena and one dense tensor, which must hold them
+void peer_copy_args(Args& args, const char* name, const at::Tensor& t, size_t bytes) {
+  args(name, t, {}, min_numel(0), kDense);
+  if (bytes > (size_t)t.numel() * t.element_size())
+    args.fail("bytes", std::string("at most ") + name + "'s " + std::to_string(t.numel() * t.element_size()), std::to_string(bytes));
+  args.device();
 }
 
 // ---- optimizer ---------------------------------------------------------------------------------
@@ -200,62 +349,57 @@ struct OptPlan {
   }
 };
 
-// grouped-query causal documents: qkv [B*S, (heads + 2*kv_heads)*hd] with head dim hd = 64 (causal_gqa_attention_*) or
-// 128 (causal_attention_d128_*, kv_heads == heads included); the same bounds as the packed pair
-int gqa_check(const at::Tensor& qkv, const at::Tensor& bounds, int heads, int kv_heads, int hd, const char* who) {
-  check_cuda(qkv, "qkv");
-  TORCH_CHECK(qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 2 && qkv.is_contiguous(), who,
-              ": qkv must be contiguous bf16 [B*S, (heads + 2*kv_heads)*", hd, "]");
-  TORCH_CHECK(heads >= 1 && kv_heads >= 1 && heads % kv_heads == 0, who, ": kv_heads (", kv_heads, ") must divide heads (", heads, ")");
-  TORCH_CHECK(qkv.size(1) == (int64_t)(heads + 2 * kv_heads) * hd, who, ": qkv has ", qkv.size(1),
-              " columns, expected (heads + 2 * kv_heads) * ", hd, " with heads = ", heads, ", kv_heads = ", kv_heads);
-  check_cuda(bounds, "bounds");
-  TORCH_CHECK(bounds.scalar_type() == at::kInt && bounds.dim() == 3 && bounds.size(2) == 2 && bounds.is_contiguous() && bounds.numel() >= 2,
-              who, ": bounds must be contiguous int32 [B, S, 2]");
-  TORCH_CHECK(qkv.size(0) == bounds.size(0) * bounds.size(1), who, ": qkv rows (", qkv.size(0), ") are not B * S for bounds [",
-              bounds.size(0), ", ", bounds.size(1), ", 2]");
-  TORCH_CHECK(bounds.device() == qkv.device(), who, ": bounds must be on qkv's device");
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(qkv.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(bounds.data_ptr()) & 7) == 0,
-              who, ": qkv must be 16-byte and bounds 8-byte aligned");
-  return (int)bounds.size(0);
+// ---- attention (attention.cu): one body per direction for every mask and head layout ------------------------------
+// qkv bf16 [B*S, (heads + 2*kv_heads)*hd], query | key | value column blocks (kv_heads == heads: multi-head), S % 128 == 0;
+// the mask is seq_lens int32 [B] (key padding) or bounds int32 [B, S, 2] (documents: packed, causal, grouped-query, head
+// dim 128).  The multi-head launchers, which take no kv_heads, are adapted by captureless lambdas at their m.def.
+using AttnFwd = void (*)(const void*, const int*, int, int, int, int, void*, float*, cudaStream_t);
+using AttnBwd = void (*)(const void*, const void*, const void*, const float*, const int*, int, int, int, int, float*, void*, cudaStream_t);
+enum class Mask { kSeqLens, kBounds };
+
+// checks qkv and the mask; returns (B, S)
+std::pair<int, int> attn_args(Args& args, const at::Tensor& qkv, const at::Tensor& mask, Mask kind, int heads, int kv_heads, int hd) {
+  TORCH_CHECK(heads >= 1 && kv_heads >= 1 && heads % kv_heads == 0, args.fn(), ": kv_heads (", kv_heads, ") must divide heads (", heads, ")");
+  const int64_t cols = (int64_t)(heads + 2 * kv_heads) * hd;
+  if (kind == Mask::kSeqLens) {
+    args("seq_lens", mask, {kI32}, {kAny})("qkv", qkv, {kBF16}, {kAny, cols}, kContiguous, 16);
+    const int64_t B = mask.size(0);
+    args.expect(B >= 1 && qkv.size(0) % B == 0, "seq_lens", "int32 [B] with B >= 1 dividing qkv's rows", mask);
+    return {(int)B, (int)(qkv.size(0) / B)};
+  }
+  args("bounds", mask, {kI32}, {kAny, kAny, 2}, kContiguous, 8);
+  args.expect(mask.numel() >= 2, "bounds", "int32 [B, S, 2] with B, S >= 1", mask);
+  args("qkv", qkv, {kBF16}, {mask.size(0) * mask.size(1), cols}, kContiguous, 16);
+  return {(int)mask.size(0), (int)mask.size(1)};
 }
 
-using GqaFwd = void (*)(const void*, const int*, int, int, int, int, void*, float*, cudaStream_t);
-using GqaBwd = void (*)(const void*, const void*, const void*, const float*, const int*, int, int, int, int, float*, void*, cudaStream_t);
-
-std::tuple<at::Tensor, at::Tensor> gqa_fwd(GqaFwd launch, int hd, const char* who, const at::Tensor& qkv, const at::Tensor& bounds,
-                                           int heads, int kv_heads, c10::optional<at::Tensor> o_out, c10::optional<at::Tensor> lse_out) {
-  const int B = gqa_check(qkv, bounds, heads, kv_heads, hd, who);
-  c10::cuda::CUDAGuard guard(qkv.device());
-  const int S = (int)(qkv.size(0) / B);
-  at::Tensor o = o_out.has_value() ? *o_out : at::empty({qkv.size(0), (int64_t)heads * hd}, qkv.options());
-  at::Tensor lse = lse_out.has_value() ? *lse_out : at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-  TORCH_CHECK(o.is_cuda() && o.scalar_type() == at::kBFloat16 && o.is_contiguous() && o.numel() == qkv.size(0) * heads * hd, who, ": bad o");
-  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S, who, ": bad lse");
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(o.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0,
-              who, ": o must be 16-byte and lse 8-byte aligned");
-  launch(qkv.data_ptr(), bounds.data_ptr<int>(), B, S, heads, kv_heads, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
+// (o bf16 [B*S, heads*hd], lse fp32 [B, heads, S]); optional caller-owned outputs
+std::tuple<at::Tensor, at::Tensor> attn_fwd(const char* fn, AttnFwd launch, int hd, Mask kind, const at::Tensor& qkv, const at::Tensor& mask,
+                                            int heads, int kv_heads, const c10::optional<at::Tensor>& o_out,
+                                            const c10::optional<at::Tensor>& lse_out) {
+  Args args(fn);
+  const auto [B, S] = attn_args(args, qkv, mask, kind, heads, kv_heads, hd);
+  at::Tensor o, lse;
+  args.out(o, "o", o_out, {qkv.size(0), (int64_t)heads * hd}, qkv.options(), 16);
+  args.out(lse, "lse", lse_out, {B, heads, S}, qkv.options().dtype(kF32), 8);
+  args.device();
+  launch(qkv.data_ptr(), mask.data_ptr<int>(), B, S, heads, kv_heads, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
   return std::make_tuple(o, lse);
 }
 
-at::Tensor gqa_bwd(GqaBwd launch, int hd, const char* who, const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o,
-                   const at::Tensor& lse, const at::Tensor& bounds, int heads, int kv_heads, c10::optional<at::Tensor> dqkv_out) {
-  const int B = gqa_check(qkv, bounds, heads, kv_heads, hd, who);
-  c10::cuda::CUDAGuard guard(qkv.device());
-  const int S = (int)(qkv.size(0) / B);
-  for (const at::Tensor* t : {&dout, &o}) {
-    check_cuda(*t, "dout / o");
-    TORCH_CHECK(t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->numel() == qkv.size(0) * heads * hd &&
-                (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, who, ": dout and o must be 16-byte aligned contiguous bf16 [B*S, heads*",
-                hd, "]");
-  }
-  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S &&
-              (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0, who, ": lse must be 8-byte aligned contiguous fp32 [B, heads, S]");
-  at::Tensor dqkv = dqkv_out.has_value() ? *dqkv_out : at::empty_like(qkv);
-  TORCH_CHECK(dqkv.is_cuda() && dqkv.scalar_type() == at::kBFloat16 && dqkv.is_contiguous() && dqkv.numel() == qkv.numel() &&
-              (reinterpret_cast<uintptr_t>(dqkv.data_ptr()) & 3) == 0, who, ": bad dqkv");
-  at::Tensor dsum = at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-  launch(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), bounds.data_ptr<int>(), B, S, heads, kv_heads,
+// dqkv shaped like qkv: the query / key / value column blocks hold dQ / dK / dV
+at::Tensor attn_bwd(const char* fn, AttnBwd launch, int hd, Mask kind, const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o,
+                    const at::Tensor& lse, const at::Tensor& mask, int heads, int kv_heads, const c10::optional<at::Tensor>& dqkv_out) {
+  Args args(fn);
+  const auto [B, S] = attn_args(args, qkv, mask, kind, heads, kv_heads, hd);
+  args("dout", dout, {kBF16}, numel(qkv.size(0) * heads * hd), kContiguous, 16);
+  args("o", o, {kBF16}, numel(qkv.size(0) * heads * hd), kContiguous, 16);
+  args("lse", lse, {kF32}, numel((int64_t)B * heads * S), kContiguous, 8);
+  at::Tensor dqkv;
+  args.out(dqkv, "dqkv", dqkv_out, qkv.sizes(), qkv.options(), 4);
+  args.device();
+  at::Tensor dsum = at::empty({B, heads, S}, qkv.options().dtype(kF32));
+  launch(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), mask.data_ptr<int>(), B, S, heads, kv_heads,
          dsum.data_ptr<float>(), dqkv.data_ptr(), cur_stream());
   return dqkv;
 }
@@ -311,12 +455,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("algo") = (int)kAlgoAuto, py::arg("blocks") = 32, py::arg("stage_off"), py::arg("stage_bytes"),
         py::arg("scale") = 1.0, py::arg("pad_set") = 1, py::arg("timeout_s") = 30.0, py::arg("sq_partials") = py::none());
   m.def("arena_tensor", [](PeerArena& a, size_t offset, int64_t numel, int dtype_code) {
-    auto dt = dtype_code == 1 ? at::kBFloat16 : dtype_code == 2 ? at::kByte : at::kFloat;
+    auto dt = dtype_code == 1 ? kBF16 : dtype_code == 2 ? kU8 : kF32;
     auto opts = at::TensorOptions().dtype(dt).device(at::kCUDA, a.device());
     return at::from_blob(a.local() + offset, {numel}, [](void*) {}, opts);
   });
   m.def("allreduce_symmetric", [](PeerArena& a, size_t buf_off, int64_t numel, int dtype_code, int algo, int blocks, double scale,
                                   int pad_set, double timeout_s) {
+    c10::cuda::CUDAGuard guard((c10::DeviceIndex)a.device());
     CommCtx ctx = make_ctx(a, (size_t)pad_set * kPadSetBytes, timeout_s);
     if (algo == kAlgoAuto) algo = a.has_multicast() ? kAlgoNvls : kAlgoTwoShot;
     launch_symmetric_allreduce(ctx, buf_off, (size_t)numel, (DType)dtype_code, algo, blocks, (float)scale, cur_stream());
@@ -325,9 +470,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("stage_bytes"), py::arg("use_mc") = false, py::arg("blocks") = 32, py::arg("pad_set") = 1,
         py::arg("timeout_s") = 30.0);
   m.def("peer_pull", [](PeerArena& a, int peer, size_t src_off, at::Tensor dst, size_t bytes, int blocks) {
+    Args args("peer_pull");
+    peer_copy_args(args, "dst", dst, bytes);
     launch_peer_pull(make_ctx(a, 0, 30.0), peer, src_off, dst.data_ptr(), bytes, blocks, cur_stream());
   });
   m.def("peer_push", [](PeerArena& a, int peer, size_t dst_off, at::Tensor src, size_t bytes, int blocks) {
+    Args args("peer_push");
+    peer_copy_args(args, "src", src, bytes);
     launch_peer_push(make_ctx(a, 0, 30.0), peer, dst_off, src.data_ptr(), bytes, blocks, cur_stream());
   });
   m.def("peer_barrier", [](PeerArena& a, int blocks, int pad_set, double timeout_s) {
@@ -391,79 +540,64 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def("step", &OptPlan::step)
       .def("adamw", &OptPlan::adamw);
   m.def("clip_coef", [](at::Tensor partials, int n, double max_norm, double grad_scale, at::Tensor coef, at::Tensor norm) {
+    Args args("clip_coef");
+    args("partials", partials, {kF32}, min_numel(n))("coef", coef, {kF32}, min_numel(1))("norm", norm, {kF32}, min_numel(1));
+    args.device();
     launch_clip_coef(partials.data_ptr<float>(), n, (float)max_norm, (float)grad_scale, coef.data_ptr<float>(),
                      norm.data_ptr<float>(), cur_stream());
   });
 
   // ---- losses -----------------------------------------------------------------------------------
   m.def("mse_fwd_bwd", [](at::Tensor out, at::Tensor target, double gscale) {
-    check_cuda(out, "out"); check_cuda(target, "target");
-    TORCH_CHECK(out.is_contiguous() && target.is_contiguous() && out.sizes() == target.sizes() && out.dtype() == target.dtype(),
-                "mse_fwd_bwd: out/target must be contiguous with equal shape and dtype");
-    c10::cuda::CUDAGuard guard(out.device());
+    Args args("mse_fwd_bwd");
+    args("out", out, {kF32, kBF16}, min_numel(0))("target", target, {out.scalar_type()}, out.sizes());
+    args.device();
     const size_t n = (size_t)out.numel();
     const int blocks = mse_blocks(n);
-    at::Tensor loss = at::empty({}, out.options().dtype(at::kFloat));
+    at::Tensor loss = at::empty({}, out.options().dtype(kF32));
     at::Tensor dout = at::empty_like(out);
-    at::Tensor scratch = at::zeros({blocks + 1}, out.options().dtype(at::kFloat));
+    at::Tensor scratch = at::zeros({blocks + 1}, out.options().dtype(kF32));
     launch_mse_fwd_bwd(out.data_ptr(), target.data_ptr(), dtype_of(out), n, (float)gscale, loss.data_ptr<float>(), dout.data_ptr(),
                        scratch.data_ptr<float>(), blocks, cur_stream());
     return std::make_tuple(loss, dout);
   });
   m.def("xent_fwd_bwd", [](at::Tensor logits, at::Tensor targets, long long ignore_index, double gscale) {
-    check_cuda(logits, "logits"); check_cuda(targets, "targets");
-    TORCH_CHECK(logits.dim() == 2 && logits.is_contiguous() && targets.is_contiguous() && targets.scalar_type() == at::kLong &&
-                targets.numel() == logits.size(0), "xent_fwd_bwd: logits [rows, cols] contiguous, targets int64 [rows]");
-    c10::cuda::CUDAGuard guard(logits.device());
+    Args args("xent_fwd_bwd");
+    args("logits", logits, {kF32, kBF16}, {kAny, kAny})("targets", targets, {kI64}, numel(logits.size(0)));
+    args.device();
     const int rows = (int)logits.size(0), cols = (int)logits.size(1);
-    at::Tensor loss = at::empty({}, logits.options().dtype(at::kFloat));
-    at::Tensor row_loss = at::empty({rows + 1}, logits.options().dtype(at::kFloat));
+    at::Tensor loss = at::empty({}, logits.options().dtype(kF32));
+    at::Tensor row_loss = at::empty({rows + 1}, logits.options().dtype(kF32));
     at::Tensor dlogits = at::empty_like(logits);
-    launch_xent_fwd_bwd(logits.data_ptr(), targets.data_ptr<int64_t>() ? (const long long*)targets.data_ptr<int64_t>() : nullptr,
-                        dtype_of(logits), rows, cols, ignore_index, (float)gscale, row_loss.data_ptr<float>(), loss.data_ptr<float>(),
-                        dlogits.data_ptr(), cur_stream());
+    launch_xent_fwd_bwd(logits.data_ptr(), (const long long*)targets.data_ptr<int64_t>(), dtype_of(logits), rows, cols, ignore_index,
+                        (float)gscale, row_loss.data_ptr<float>(), loss.data_ptr<float>(), dlogits.data_ptr(), cur_stream());
     return std::make_tuple(loss, dlogits);
   });
   // Fused LM-head cross-entropy: mean over non-ignored rows of cross_entropy(hidden [N,H] . weight [V,H]^T + bias [V]) without
   // the [N, V] logits.  Forward -> (loss fp32 [], lse fp32 [N], row_loss fp32 [N+1], row_loss[N] = non-ignored rows).
-  auto lm_check = [](const at::Tensor& hidden, const at::Tensor& weight, const at::Tensor& targets, const c10::optional<at::Tensor>& bias) {
-    check_cuda(hidden, "hidden"); check_cuda(weight, "weight"); check_cuda(targets, "targets");
-    TORCH_CHECK(hidden.scalar_type() == at::kBFloat16 && weight.scalar_type() == at::kBFloat16 && hidden.dim() == 2 && weight.dim() == 2 &&
-                hidden.is_contiguous() && weight.is_contiguous() && hidden.size(1) == weight.size(1),
-                "lm_loss: hidden [N,H] and weight [V,H], bf16 contiguous");
-    TORCH_CHECK(hidden.size(1) % 8 == 0 && weight.size(0) % 8 == 0, "lm_loss: H and V must be multiples of 8 (16-byte rows), got H=",
-                hidden.size(1), ", V=", weight.size(0));
-    TORCH_CHECK(hidden.size(0) >= 1, "lm_loss: no rows");
-    TORCH_CHECK(targets.scalar_type() == at::kLong && targets.is_contiguous() && targets.numel() == hidden.size(0), "lm_loss: targets int64 [N]");
-    if (bias.has_value())
-      TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->is_contiguous() && bias->numel() == weight.size(0), "lm_loss: bias bf16 [V]");
-  };
-  auto lm_out = [](const c10::optional<at::Tensor>& given, at::IntArrayRef sizes, const at::TensorOptions& opt, const char* name) {
-    if (!given.has_value()) return at::empty(sizes, opt);
-    TORCH_CHECK(given->is_contiguous() && given->sizes() == sizes && given->scalar_type() == opt.dtype().toScalarType(),
-                "lm_loss: bad ", name, " output");
-    return *given;
-  };
   // rows (optional): int32 [1] device count of the leading rows that carry labels (compact_rows' count).  Only the 128-row tiles
   // below it are computed; the rows at or past it must be ignored ones, and get lse = row_loss = 0 (dh: zeros).
-  auto rows_ptr = [](const c10::optional<at::Tensor>& rows, const at::Tensor& hidden) -> const int* {
-    if (!rows.has_value()) return nullptr;
-    check_cuda(*rows, "rows");
-    TORCH_CHECK(rows->scalar_type() == at::kInt && rows->numel() == 1 && rows->device() == hidden.device(),
-                "lm_loss: rows must be an int32 [1] tensor on the hidden states' device");
-    return rows->data_ptr<int>();
+  auto lm_args = [](Args& args, const at::Tensor& hidden, const at::Tensor& weight, const at::Tensor& targets,
+                    const c10::optional<at::Tensor>& bias, const c10::optional<at::Tensor>& rows) {
+    args("hidden", hidden, {kBF16}, {kAny, kAny});
+    args.expect(hidden.size(0) >= 1 && hidden.size(1) % 8 == 0, "hidden", "[N, H] with N >= 1 and H % 8 == 0 (16-byte rows)", hidden);
+    args("weight", weight, {kBF16}, {kAny, hidden.size(1)});
+    args.expect(weight.size(0) % 8 == 0, "weight", "[V, H] with V % 8 == 0", weight);
+    args("targets", targets, {kI64}, numel(hidden.size(0)))("bias", bias, {kBF16}, numel(weight.size(0)))("rows", rows, {kI32}, numel(1));
   };
-  m.def("lm_loss_fwd", [lm_check, lm_out, rows_ptr](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
-                                                    long long ignore_index, c10::optional<at::Tensor> lse_out, c10::optional<at::Tensor> row_loss_out,
-                                                    c10::optional<at::Tensor> rows) {
-    lm_check(hidden, weight, targets, bias);
-    const int* bound = rows_ptr(rows, hidden);
-    c10::cuda::CUDAGuard guard(hidden.device());
+  m.def("lm_loss_fwd", [lm_args](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
+                                 long long ignore_index, c10::optional<at::Tensor> lse_out, c10::optional<at::Tensor> row_loss_out,
+                                 c10::optional<at::Tensor> rows) {
+    Args args("lm_loss_fwd");
+    lm_args(args, hidden, weight, targets, bias, rows);
     const int N = (int)hidden.size(0), H = (int)hidden.size(1), V = (int)weight.size(0), tiles = (V + 127) / 128;
-    const auto f32 = hidden.options().dtype(at::kFloat);
+    const auto f32 = hidden.options().dtype(kF32);
+    at::Tensor lse, row_loss;
+    args.out(lse, "lse_out", lse_out, {N}, f32);
+    args.out(row_loss, "row_loss_out", row_loss_out, {N + 1}, f32);
+    args.device();
+    const int* bound = rows.has_value() ? rows->data_ptr<int>() : nullptr;
     at::Tensor loss = at::empty({}, f32);
-    at::Tensor lse = lm_out(lse_out, {N}, f32, "lse");
-    at::Tensor row_loss = lm_out(row_loss_out, {N + 1}, f32, "row_loss");
     at::Tensor partial = at::empty({tiles, N, 2}, f32);
     at::Tensor target_logit = at::empty({N}, f32);
     const auto* t = (const long long*)targets.data_ptr<int64_t>();
@@ -478,34 +612,29 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // dh += dlogits . weight[slice] (fp32, cast to bf16 once at the end), dweight[slice] = dlogits^T . hidden and, with
   // need_dbias, dbias[slice] = the column sums of dlogits (fixed order).  gscale: fp32 device scalar (the upstream
   // gradient).  rows: as for lm_loss_fwd.  Returns (dh bf16 [N,H], dweight bf16 [V,H], dbias bf16 [V]; each None when not asked for).
-  m.def("lm_loss_bwd", [lm_check, lm_out, rows_ptr](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
-                                                    at::Tensor lse, at::Tensor row_loss, at::Tensor gscale, long long ignore_index, int slice,
-                                                    bool need_dh, bool need_dweight, c10::optional<at::Tensor> dh_out,
-                                                    c10::optional<at::Tensor> dweight_out, c10::optional<at::Tensor> rows, bool need_dbias) {
-    lm_check(hidden, weight, targets, bias);
-    TORCH_CHECK(!need_dbias || bias.has_value(), "lm_loss_bwd: need_dbias needs the bias");
-    const int* bound = rows_ptr(rows, hidden);
+  m.def("lm_loss_bwd", [lm_args](at::Tensor hidden, at::Tensor weight, at::Tensor targets, c10::optional<at::Tensor> bias,
+                                 at::Tensor lse, at::Tensor row_loss, at::Tensor gscale, long long ignore_index, int slice,
+                                 bool need_dh, bool need_dweight, c10::optional<at::Tensor> dh_out,
+                                 c10::optional<at::Tensor> dweight_out, c10::optional<at::Tensor> rows, bool need_dbias) {
+    Args args("lm_loss_bwd");
+    lm_args(args, hidden, weight, targets, bias, rows);
+    if (need_dbias) args.required("bias", bias);
     const int N = (int)hidden.size(0), H = (int)hidden.size(1), V = (int)weight.size(0);
     TORCH_CHECK(slice >= 128 && slice % 128 == 0, "lm_loss_bwd: slice must be a positive multiple of 128, got ", slice);
-    for (const at::Tensor* t : {&lse, &row_loss, &gscale}) {
-      check_cuda(*t, "lse / row_loss / gscale");
-      TORCH_CHECK(t->scalar_type() == at::kFloat && t->is_contiguous(), "lm_loss_bwd: lse, row_loss and gscale are contiguous fp32");
-    }
-    TORCH_CHECK(lse.numel() == N && row_loss.numel() == N + 1 && gscale.numel() == 1, "lm_loss_bwd: lse [N], row_loss [N+1], gscale [1]");
-    c10::cuda::CUDAGuard guard(hidden.device());
+    args("lse", lse, {kF32}, numel(N))("row_loss", row_loss, {kF32}, numel(N + 1))("gscale", gscale, {kF32}, numel(1));
     const auto bf16 = hidden.options();
     at::Tensor dh, dweight, dbias, dh32, colsum;
-    if (need_dh) {
-      dh = lm_out(dh_out, {N, H}, bf16, "dh");
-      // row-bounded: the data-gradient GEMM skips the tiles past the count, whose rows must read as zeros
-      dh32 = bound != nullptr ? at::zeros({N, H}, bf16.dtype(at::kFloat)) : at::empty({N, H}, bf16.dtype(at::kFloat));
-    }
-    if (need_dweight) dweight = lm_out(dweight_out, {V, H}, bf16, "dweight");
+    if (need_dh) args.out(dh, "dh_out", dh_out, {N, H}, bf16);
+    if (need_dweight) args.out(dweight, "dweight_out", dweight_out, {V, H}, bf16);
+    args.device();
+    const int* bound = rows.has_value() ? rows->data_ptr<int>() : nullptr;
+    // row-bounded: the data-gradient GEMM skips the tiles past the count, whose rows must read as zeros
+    if (need_dh) dh32 = bound != nullptr ? at::zeros({N, H}, bf16.dtype(kF32)) : at::empty({N, H}, bf16.dtype(kF32));
     if (need_dbias) dbias = at::empty({V}, bf16);
     if (!need_dh && !need_dweight && !need_dbias) return std::make_tuple(dh, dweight, dbias);
     const int width = slice < V ? slice : V;
     at::Tensor dlogits = at::empty({(int64_t)N * width}, bf16);
-    if (need_dbias) colsum = at::empty({(int64_t)column_sum_workspace(N, width)}, bf16.dtype(at::kFloat));
+    if (need_dbias) colsum = at::empty({(int64_t)column_sum_workspace(N, width)}, bf16.dtype(kF32));
     const auto* t = (const long long*)targets.data_ptr<int64_t>();
     const auto* w = reinterpret_cast<const __nv_bfloat16*>(weight.data_ptr());
     const auto* b = bias.has_value() ? reinterpret_cast<const __nv_bfloat16*>(bias->data_ptr()) : nullptr;
@@ -539,39 +668,38 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // [T]): a stable partition of the rows, those whose target is not ignore_index and lies in [0, vocab) first; the compacted
   // targets hold ignore_index from count on.  No host synchronisation.
   m.def("compact_rows", [](at::Tensor targets, long long ignore_index, long long vocab) {
-    check_cuda(targets, "targets");
-    TORCH_CHECK(targets.scalar_type() == at::kLong && targets.dim() == 1 && targets.is_contiguous() && targets.numel() >= 1 &&
-                targets.numel() < (1LL << 31), "compact_rows: targets int64 [T], contiguous, 1 <= T < 2^31");
+    Args args("compact_rows");
+    args("targets", targets, {kI64}, {kAny});
+    args.expect(targets.numel() >= 1 && targets.numel() < (1LL << 31), "targets", "int64 [T] with 1 <= T < 2^31", targets);
     TORCH_CHECK(vocab >= 1, "compact_rows: vocab must be positive, got ", vocab);
-    c10::cuda::CUDAGuard guard(targets.device());
+    args.device();
     const int T = (int)targets.numel();
-    const auto i32 = targets.options().dtype(at::kInt);
+    const auto i32 = targets.options().dtype(kI32);
     at::Tensor index = at::empty({T}, i32), count = at::empty({1}, i32), out = at::empty_like(targets);
     at::Tensor work = at::empty({2 * compact_chunks(T)}, i32);
     launch_compact_rows((const long long*)targets.data_ptr<int64_t>(), T, ignore_index, vocab, work.data_ptr<int>(), index.data_ptr<int>(),
                         count.data_ptr<int>(), (long long*)out.data_ptr<int64_t>(), cur_stream());
     return std::make_tuple(index, count, out);
   }, py::arg("targets"), py::arg("ignore_index"), py::arg("vocab"));
-  auto rows_check = [](const at::Tensor& x, const at::Tensor& index, const at::Tensor& count, const char* name) {
-    check_cuda(x, name); check_cuda(index, "index"); check_cuda(count, "count");
-    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous() && x.size(1) % 8 == 0,
-                name, ": bf16 [T, H] contiguous with H % 8 == 0");
-    TORCH_CHECK(index.scalar_type() == at::kInt && index.is_contiguous() && index.numel() == x.size(0) &&
-                count.scalar_type() == at::kInt && count.numel() == 1, name, ": index int32 [T] and count int32 [1] (compact_rows)");
-    TORCH_CHECK(index.device() == x.device() && count.device() == x.device(), name, ": tensors on different devices");
+  // x bf16 [T, H] (H % 8 == 0), index int32 [T] and count int32 [1] from compact_rows
+  auto rows_args = [](Args& args, const char* name, const at::Tensor& x, const at::Tensor& index, const at::Tensor& count) {
+    args(name, x, {kBF16}, {kAny, kAny});
+    args.expect(x.size(1) % 8 == 0, name, "bf16 [T, H] with H % 8 == 0", x);
+    args("index", index, {kI32}, numel(x.size(0)))("count", count, {kI32}, numel(1));
+    args.device();
   };
   // gather_rows(x [T, H], index, count): out[r] = x[index[r]] for r < count, zero rows from count on
-  m.def("gather_rows", [rows_check](at::Tensor x, at::Tensor index, at::Tensor count) {
-    rows_check(x, index, count, "gather_rows");
-    c10::cuda::CUDAGuard guard(x.device());
+  m.def("gather_rows", [rows_args](at::Tensor x, at::Tensor index, at::Tensor count) {
+    Args args("gather_rows");
+    rows_args(args, "x", x, index, count);
     at::Tensor out = at::empty_like(x);
     launch_gather_rows(x.data_ptr(), index.data_ptr<int>(), count.data_ptr<int>(), (int)x.size(0), (int)x.size(1), out.data_ptr(), cur_stream());
     return out;
   }, py::arg("x"), py::arg("index"), py::arg("count"));
   // scatter_rows(dy [T, H], index, count): dx[index[r]] = dy[r] for r < count, every other row of dx zero
-  m.def("scatter_rows", [rows_check](at::Tensor dy, at::Tensor index, at::Tensor count) {
-    rows_check(dy, index, count, "scatter_rows");
-    c10::cuda::CUDAGuard guard(dy.device());
+  m.def("scatter_rows", [rows_args](at::Tensor dy, at::Tensor index, at::Tensor count) {
+    Args args("scatter_rows");
+    rows_args(args, "dy", dy, index, count);
     at::Tensor dx = at::empty_like(dy);
     launch_scatter_rows(dy.data_ptr(), index.data_ptr<int>(), count.data_ptr<int>(), (int)dy.size(0), (int)dy.size(1), dx.data_ptr(),
                         cur_stream());
@@ -580,17 +708,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // tanh = false: the erf form; true: the tanh approximation
   m.def("gelu_fwd", [](at::Tensor pre, bool tanh) {
-    check_cuda(pre, "pre");
-    TORCH_CHECK(pre.is_contiguous(), "gelu_fwd: contiguous input");
-    c10::cuda::CUDAGuard guard(pre.device());
+    Args args("gelu_fwd");
+    args("pre", pre, {kF32, kBF16}, min_numel(0));
+    args.device();
     at::Tensor out = at::empty_like(pre);
     launch_gelu(pre.data_ptr(), nullptr, out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), false, cur_stream(), tanh);
     return out;
   }, py::arg("pre"), py::arg("tanh") = false);
   m.def("gelu_bwd", [](at::Tensor dy, at::Tensor pre, bool tanh) {
-    check_cuda(pre, "pre");
-    TORCH_CHECK(pre.is_contiguous() && dy.is_contiguous() && dy.dtype() == pre.dtype() && dy.numel() == pre.numel(), "gelu_bwd: matching contiguous tensors");
-    c10::cuda::CUDAGuard guard(pre.device());
+    Args args("gelu_bwd");
+    args("pre", pre, {kF32, kBF16}, min_numel(0))("dy", dy, {pre.scalar_type()}, numel(pre.numel()));
+    args.device();
     at::Tensor out = at::empty_like(pre);
     launch_gelu(pre.data_ptr(), dy.data_ptr(), out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), true, cur_stream(), tanh);
     return out;
@@ -598,29 +726,31 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ---- layer norm -------------------------------------------------------------------------------
   m.def("layernorm_fwd", [](at::Tensor x, at::Tensor gamma, at::Tensor beta, double eps) {
-    check_cuda(x, "x");
-    TORCH_CHECK(x.is_contiguous() && gamma.is_contiguous() && beta.is_contiguous(), "layernorm_fwd: contiguous inputs");
-    TORCH_CHECK(gamma.dtype() == x.dtype() && beta.dtype() == x.dtype(), "layernorm_fwd: gamma/beta dtype must match x");
-    c10::cuda::CUDAGuard guard(x.device());
+    Args args("layernorm_fwd");
+    args("x", x, {kF32, kBF16}, last_dim(kAny))("gamma", gamma, {x.scalar_type()}, numel(x.size(-1)));
+    args("beta", beta, {x.scalar_type()}, numel(x.size(-1)));
+    args.device();
     const int cols = (int)x.size(-1);
     const int rows = (int)(x.numel() / cols);
     at::Tensor y = at::empty_like(x);
-    at::Tensor mean = at::empty({rows}, x.options().dtype(at::kFloat));
-    at::Tensor rstd = at::empty({rows}, x.options().dtype(at::kFloat));
+    at::Tensor mean = at::empty({rows}, x.options().dtype(kF32));
+    at::Tensor rstd = at::empty({rows}, x.options().dtype(kF32));
     launch_layernorm_fwd(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), dtype_of(x), rows, cols, (float)eps, y.data_ptr(),
                          mean.data_ptr<float>(), rstd.data_ptr<float>(), cur_stream());
     return std::make_tuple(y, mean, rstd);
   });
   m.def("layernorm_bwd", [](at::Tensor dy, at::Tensor x, at::Tensor gamma, at::Tensor mean, at::Tensor rstd) {
-    check_cuda(dy, "dy");
-    TORCH_CHECK(dy.is_contiguous() && x.is_contiguous(), "layernorm_bwd: contiguous inputs");
-    c10::cuda::CUDAGuard guard(x.device());
+    Args args("layernorm_bwd");
+    args("x", x, {kF32, kBF16}, last_dim(kAny));
     const int cols = (int)x.size(-1);
     const int rows = (int)(x.numel() / cols);
+    args("dy", dy, {x.scalar_type()}, x.sizes())("gamma", gamma, {x.scalar_type()}, numel(cols))("mean", mean, {kF32}, numel(rows));
+    args("rstd", rstd, {kF32}, numel(rows));
+    args.device();
     const int parts = layernorm_partial_rows(rows);
     at::Tensor dx = at::empty_like(x);
-    at::Tensor dgp = at::empty({parts, cols}, x.options().dtype(at::kFloat));
-    at::Tensor dbp = at::empty({parts, cols}, x.options().dtype(at::kFloat));
+    at::Tensor dgp = at::empty({parts, cols}, x.options().dtype(kF32));
+    at::Tensor dbp = at::empty({parts, cols}, x.options().dtype(kF32));
     at::Tensor dgamma = at::empty_like(gamma);
     at::Tensor dbeta = at::empty_like(gamma);
     launch_layernorm_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), dtype_of(x),
@@ -631,10 +761,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ---- linears ----------------------------------------------------------------------------------
   m.def("small_linear_fwd", [](at::Tensor x, at::Tensor w, c10::optional<at::Tensor> b, bool relu) {
-    check_cuda(x, "x");
-    TORCH_CHECK(x.scalar_type() == at::kFloat && w.scalar_type() == at::kFloat && x.is_contiguous() && w.is_contiguous(),
-                "small_linear_fwd: fp32 contiguous");
-    c10::cuda::CUDAGuard guard(x.device());
+    Args args("small_linear_fwd");
+    args("x", x, {kF32}, last_dim(kAny))("w", w, {kF32}, {kAny, x.size(-1)})("b", b, {kF32}, numel(w.size(0)));
+    args.device();
     const int K = (int)x.size(-1), N = (int)w.size(0);
     const int M = (int)(x.numel() / K);
     auto sizes = x.sizes().vec();
@@ -645,10 +774,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return y;
   });
   m.def("small_linear_bwd", [](at::Tensor dy, at::Tensor x, at::Tensor w, at::Tensor y, bool relu, bool need_dx, bool has_bias) {
-    check_cuda(dy, "dy");
-    c10::cuda::CUDAGuard guard(x.device());
+    Args args("small_linear_bwd");
+    args("x", x, {kF32}, last_dim(kAny))("w", w, {kF32}, {kAny, x.size(-1)});
     const int K = (int)x.size(-1), N = (int)w.size(0);
     const int M = (int)(x.numel() / K);
+    args("y", y, {kF32}, numel((int64_t)M * N))("dy", dy, {kF32}, numel((int64_t)M * N), kStrided);
+    args.device();
     at::Tensor dyc = dy.contiguous();
     at::Tensor dx = need_dx ? at::empty_like(x) : at::Tensor();
     at::Tensor dw = at::empty_like(w);
@@ -661,245 +792,172 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // wgmma GEMM: D[M,N] = act(A[M,K] @ B[N,K]^T + bias) ; all bf16 row-major, fp32 accumulate in registers
   m.def("gemm_nt", [](at::Tensor a, at::Tensor b, c10::optional<at::Tensor> bias, int epilogue, c10::optional<at::Tensor> out) {
-    check_cuda(a, "a"); check_cuda(b, "b");
-    TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm_nt: bf16 operands");
-    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.size(1) == b.size(1) && a.is_contiguous() && b.is_contiguous(),
-                "gemm_nt: A [M,K], B [N,K], both K-major contiguous");
-    c10::cuda::CUDAGuard guard(a.device());
+    Args args("gemm_nt");
+    args("a", a, {kBF16}, {kAny, kAny})("b", b, {kBF16}, {kAny, a.size(1)});
     const int M = (int)a.size(0), K = (int)a.size(1), N = (int)b.size(0);
-    at::Tensor d = out.has_value() ? *out : at::empty({M, N}, a.options());
-    TORCH_CHECK(d.is_contiguous() && d.size(0) == M && d.size(1) == N, "gemm_nt: bad output");
-    const void* bias_ptr = nullptr;
-    if (bias.has_value()) {
-      TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N, "gemm_nt: bias bf16 [N]");
-      bias_ptr = bias->data_ptr();
-    }
-    launch_gemm_nt_bf16(a.data_ptr(), b.data_ptr(), d.data_ptr(), bias_ptr, M, N, K, epilogue, dtype_of(d), cur_stream());
+    args("bias", bias, {kBF16}, numel(N));
+    at::Tensor d;
+    args.out(d, "out", out, {M, N}, a.options(), 0, {kBF16, kF32});
+    args.device();
+    launch_gemm_nt_bf16(a.data_ptr(), b.data_ptr(), d.data_ptr(), bias.has_value() ? bias->data_ptr() : nullptr, M, N, K, epilogue,
+                        dtype_of(d), cur_stream());
     return d;
   }, py::arg("a"), py::arg("b"), py::arg("bias") = py::none(), py::arg("epilogue") = 0, py::arg("out") = py::none());
   // general form: a_mn=false -> a is [M,K]; true -> a is stored [K,M].  b_mn=false -> b is [N,K]; true -> stored [K,N].
+  // A given fp32 `out` with out_fp32 is accumulated into.
   m.def("gemm", [](at::Tensor a, at::Tensor b, c10::optional<at::Tensor> bias, bool a_mn, bool b_mn, int epilogue, bool out_fp32,
                    c10::optional<at::Tensor> out) {
-    check_cuda(a, "a"); check_cuda(b, "b");
-    TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm: bf16 operands");
-    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.is_contiguous() && b.is_contiguous(), "gemm: 2-D contiguous operands");
-    c10::cuda::CUDAGuard guard(a.device());
+    Args args("gemm");
+    args("a", a, {kBF16}, {kAny, kAny});
     const int M = (int)(a_mn ? a.size(1) : a.size(0)), K = (int)(a_mn ? a.size(0) : a.size(1));
-    const int N = (int)(b_mn ? b.size(1) : b.size(0)), Kb = (int)(b_mn ? b.size(0) : b.size(1));
-    TORCH_CHECK(K == Kb, "gemm: reduction dims differ (", K, " vs ", Kb, ")");
-    bool accumulate = false;
+    if (b_mn) args("b", b, {kBF16}, {K, kAny});
+    else args("b", b, {kBF16}, {kAny, K});
+    const int N = (int)(b_mn ? b.size(1) : b.size(0));
+    args("bias", bias, {kBF16}, numel(N));
     at::Tensor d;
-    if (out.has_value()) { d = *out; accumulate = d.scalar_type() == at::kFloat && out_fp32; }
-    else d = at::empty({M, N}, a.options().dtype(out_fp32 ? at::kFloat : at::kBFloat16));
-    TORCH_CHECK(d.is_contiguous() && d.size(0) == M && d.size(1) == N, "gemm: bad output");
-    const void* bias_ptr = nullptr;
-    if (bias.has_value()) {
-      TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N, "gemm: bias bf16 [N]");
-      bias_ptr = bias->data_ptr();
-    }
-    launch_gemm_bf16(a.data_ptr(), b.data_ptr(), d.data_ptr(), bias_ptr, M, N, K, a_mn, b_mn, epilogue, dtype_of(d), accumulate,
-                     cur_stream());
+    args.out(d, "out", out, {M, N}, a.options().dtype(out_fp32 ? kF32 : kBF16), 0, {kBF16, kF32});
+    args.device();
+    const bool accumulate = out.has_value() && out_fp32 && d.scalar_type() == kF32;
+    launch_gemm_bf16(a.data_ptr(), b.data_ptr(), d.data_ptr(), bias.has_value() ? bias->data_ptr() : nullptr, M, N, K, a_mn, b_mn, epilogue,
+                     dtype_of(d), accumulate, cur_stream());
     return d;
   }, py::arg("a"), py::arg("b"), py::arg("bias") = py::none(), py::arg("a_mn") = false, py::arg("b_mn") = false,
      py::arg("epilogue") = 0, py::arg("out_fp32") = false, py::arg("out") = py::none());
   // forward GEMM (a [M,K], b [N,K]) that also returns per-32-row partial column statistics of its output: [2][ceil(M/32)][N]
   m.def("gemm_stats", [](at::Tensor a, at::Tensor b) {
-    check_cuda(a, "a"); check_cuda(b, "b");
-    TORCH_CHECK(a.scalar_type() == at::kBFloat16 && b.scalar_type() == at::kBFloat16, "gemm_stats: bf16 operands");
-    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.is_contiguous() && b.is_contiguous() && a.size(1) == b.size(1), "gemm_stats: [M,K] x [N,K]");
-    c10::cuda::CUDAGuard guard(a.device());
+    Args args("gemm_stats");
+    args("a", a, {kBF16}, {kAny, kAny})("b", b, {kBF16}, {kAny, a.size(1)});
+    args.device();
     const int M = (int)a.size(0), K = (int)a.size(1), N = (int)b.size(0);
     at::Tensor d = at::empty({M, N}, a.options());
-    at::Tensor stats = at::empty({2, (M + 31) / 32, N}, a.options().dtype(at::kFloat));
+    at::Tensor stats = at::empty({2, (M + 31) / 32, N}, a.options().dtype(kF32));
     launch_gemm_bf16(a.data_ptr(), b.data_ptr(), d.data_ptr(), nullptr, M, N, K, false, false, 0, DType::BF16, false, cur_stream(),
                      stats.data_ptr<float>());
     return std::make_tuple(d, stats);
   });
   // ---- FP8 (fp8.cu, gemm_wgmma.cu): E4M3 activations / weights, E5M2 gradients, power-of-two per-tensor scales ------------
   m.def("fp8_amax", [](at::Tensor t) {
-    check_cuda(t, "t");
-    TORCH_CHECK(t.scalar_type() == at::kBFloat16 && t.is_contiguous(), "fp8_amax: contiguous bf16 tensor");
-    c10::cuda::CUDAGuard guard(t.device());
-    if ((reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) != 0) t = t.clone();
-    at::Tensor amax = at::empty({1}, t.options().dtype(at::kFloat));
+    Args args("fp8_amax");
+    args("t", t, {kBF16}, min_numel(0));
+    args.device();
+    t = aligned(t, 16);
+    at::Tensor amax = at::empty({1}, t.options().dtype(kF32));
     launch_fp8_amax(t.data_ptr(), (size_t)t.numel(), amax.data_ptr<float>(), cur_stream());
     return amax;
   });
   // q (t's shape), q^T [cols, rows] or None, scale_inv [1] (= 1/s), fp32 column sums [cols] or None; s comes from `amax`
-  auto fp8_cast = [](at::Tensor t, at::Tensor amax, const std::string& fmt, bool want_transpose, bool want_colsum) {
-    TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "fp8: format must be 'e4m3' or 'e5m2', got '", fmt, "'");
-    TORCH_CHECK(amax.is_cuda() && amax.scalar_type() == at::kFloat && amax.numel() == 1, "fp8: amax must be a 1-element fp32 CUDA tensor");
-    const bool e5m2 = fmt == "e5m2";
+  auto fp8_cast = [](const at::Tensor& t, const at::Tensor& amax, bool e5m2, bool want_transpose, bool want_colsum) {
     const int cols = (int)t.size(-1);
     const int rows = (int)(t.numel() / cols);
     at::Tensor q = at::empty(t.sizes(), t.options().dtype(e5m2 ? at::kFloat8_e5m2 : at::kFloat8_e4m3fn));
     at::Tensor qt = want_transpose ? at::empty({cols, rows}, q.options()) : at::Tensor();
-    at::Tensor scale_inv = at::empty({1}, t.options().dtype(at::kFloat));
+    at::Tensor scale_inv = at::empty({1}, t.options().dtype(kF32));
     at::Tensor colsum, partial;
     if (want_colsum) {
-      colsum = at::empty({cols}, t.options().dtype(at::kFloat));
-      partial = at::empty({fp8_colsum_parts(rows), cols}, t.options().dtype(at::kFloat));
+      colsum = at::empty({cols}, t.options().dtype(kF32));
+      partial = at::empty({fp8_colsum_parts(rows), cols}, t.options().dtype(kF32));
     }
     launch_fp8_cast_transpose(t.data_ptr(), rows, cols, amax.data_ptr<float>(), e5m2, q.data_ptr(),
                               want_transpose ? qt.data_ptr() : nullptr, want_colsum ? partial.data_ptr<float>() : nullptr,
                               want_colsum ? colsum.data_ptr<float>() : nullptr, scale_inv.data_ptr<float>(), cur_stream());
     return py::make_tuple(q, want_transpose ? py::cast(qt) : py::none(), scale_inv, want_colsum ? py::cast(colsum) : py::none());
   };
-  auto fp8_input = [](at::Tensor t) {
-    check_cuda(t, "t");
-    TORCH_CHECK(t.scalar_type() == at::kBFloat16 && t.is_contiguous() && t.dim() >= 1, "fp8: contiguous bf16 tensor");
-    return (reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) != 0 ? t.clone() : t;
-  };
-  m.def("fp8_cast_transpose", [fp8_cast, fp8_input](at::Tensor t, at::Tensor amax, const std::string& fmt, bool want_transpose, bool want_colsum) {
-    t = fp8_input(t);
-    c10::cuda::CUDAGuard guard(t.device());
-    return fp8_cast(t, amax, fmt, want_transpose, want_colsum);
+  m.def("fp8_cast_transpose", [fp8_cast](at::Tensor t, at::Tensor amax, const std::string& fmt, bool want_transpose, bool want_colsum) {
+    TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "fp8: format must be 'e4m3' or 'e5m2', got '", fmt, "'");
+    Args args("fp8_cast_transpose");
+    args("t", t, {kBF16}, last_dim(kAny))("amax", amax, {kF32}, numel(1));
+    args.device();
+    return fp8_cast(aligned(t, 16), amax, fmt == "e5m2", want_transpose, want_colsum);
   }, py::arg("t"), py::arg("amax"), py::arg("fmt"), py::arg("want_transpose") = false, py::arg("want_colsum") = false);
-  m.def("fp8_quantize", [fp8_cast, fp8_input](at::Tensor t, const std::string& fmt, bool want_transpose, bool want_colsum) {
-    t = fp8_input(t);
-    c10::cuda::CUDAGuard guard(t.device());
-    at::Tensor amax = at::empty({1}, t.options().dtype(at::kFloat));
+  m.def("fp8_quantize", [fp8_cast](at::Tensor t, const std::string& fmt, bool want_transpose, bool want_colsum) {
+    TORCH_CHECK(fmt == "e4m3" || fmt == "e5m2", "fp8: format must be 'e4m3' or 'e5m2', got '", fmt, "'");
+    Args args("fp8_quantize");
+    args("t", t, {kBF16}, last_dim(kAny));
+    args.device();
+    t = aligned(t, 16);
+    at::Tensor amax = at::empty({1}, t.options().dtype(kF32));
     launch_fp8_amax(t.data_ptr(), (size_t)t.numel(), amax.data_ptr<float>(), cur_stream());
-    return fp8_cast(t, amax, fmt, want_transpose, want_colsum);
+    return fp8_cast(t, amax, fmt == "e5m2", want_transpose, want_colsum);
   }, py::arg("t"), py::arg("fmt"), py::arg("want_transpose") = false, py::arg("want_colsum") = false);
   // D[M,N] bf16 = epi(a_scale_inv * b_scale_inv * A[M,K] @ B[N,K]^T + bias): A e4m3 or e5m2, B e4m3, both K-major
   m.def("gemm_fp8", [](at::Tensor a, at::Tensor b, at::Tensor a_scale_inv, at::Tensor b_scale_inv, c10::optional<at::Tensor> bias,
                        int epilogue) {
-    check_cuda(a, "a"); check_cuda(b, "b");
-    TORCH_CHECK(a.scalar_type() == at::kFloat8_e4m3fn || a.scalar_type() == at::kFloat8_e5m2, "gemm_fp8: A must be float8_e4m3fn or float8_e5m2");
-    TORCH_CHECK(b.scalar_type() == at::kFloat8_e4m3fn, "gemm_fp8: B must be float8_e4m3fn");
-    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.is_contiguous() && b.is_contiguous() && a.size(1) == b.size(1),
-                "gemm_fp8: A [M,K], B [N,K], both K-major contiguous");
-    for (const at::Tensor* s : {&a_scale_inv, &b_scale_inv})
-      TORCH_CHECK(s->is_cuda() && s->scalar_type() == at::kFloat && s->numel() == 1, "gemm_fp8: scale factors are 1-element fp32 CUDA tensors");
-    c10::cuda::CUDAGuard guard(a.device());
+    Args args("gemm_fp8");
+    args("a", a, {at::kFloat8_e4m3fn, at::kFloat8_e5m2}, {kAny, kAny}, kContiguous, 16);
+    args("b", b, {at::kFloat8_e4m3fn}, {kAny, a.size(1)}, kContiguous, 16)("a_scale_inv", a_scale_inv, {kF32}, numel(1));
+    args("b_scale_inv", b_scale_inv, {kF32}, numel(1));
     const int M = (int)a.size(0), K = (int)a.size(1), N = (int)b.size(0);
     TORCH_CHECK(K % 16 == 0, "gemm_fp8: K = ", K, " must be a multiple of 16 (row pitch of the 8-bit operands)");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(a.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(b.data_ptr()) & 15) == 0,
-                "gemm_fp8: operands must be 16-byte aligned");
-    at::Tensor d = at::empty({M, N}, a.options().dtype(at::kBFloat16));
-    const void* bias_ptr = nullptr;
-    if (bias.has_value()) {
-      TORCH_CHECK(bias->scalar_type() == at::kBFloat16 && bias->numel() == N && bias->is_contiguous(), "gemm_fp8: bias bf16 [N]");
-      bias_ptr = bias->data_ptr();
-    }
-    launch_gemm_fp8(a.data_ptr(), b.data_ptr(), d.data_ptr(), bias_ptr, a_scale_inv.data_ptr<float>(), b_scale_inv.data_ptr<float>(),
-                    M, N, K, a.scalar_type() == at::kFloat8_e5m2, epilogue, cur_stream());
+    args("bias", bias, {kBF16}, numel(N));
+    args.device();
+    at::Tensor d = at::empty({M, N}, a.options().dtype(kBF16));
+    launch_gemm_fp8(a.data_ptr(), b.data_ptr(), d.data_ptr(), bias.has_value() ? bias->data_ptr() : nullptr, a_scale_inv.data_ptr<float>(),
+                    b_scale_inv.data_ptr<float>(), M, N, K, a.scalar_type() == at::kFloat8_e5m2, epilogue, cur_stream());
     return d;
   }, py::arg("a"), py::arg("b"), py::arg("a_scale_inv"), py::arg("b_scale_inv"), py::arg("bias") = py::none(), py::arg("epilogue") = 0);
-  // ---- attention (attention.cu): head dim 64, S % 128 == 0, masks on the device ----------------------------------------
-  auto attn_qkv_check = [](const at::Tensor& qkv, int heads, const char* who) {
-    check_cuda(qkv, "qkv");
-    TORCH_CHECK(qkv.scalar_type() == at::kBFloat16 && qkv.dim() == 2 && qkv.is_contiguous(), who, ": qkv must be contiguous bf16 [B*S, 3*heads*64]");
-    TORCH_CHECK(heads >= 1 && qkv.size(1) == 3LL * heads * 64, who, ": qkv has ", qkv.size(1), " columns, expected 3 * heads * 64 with heads = ", heads);
+
+  // ---- attention (attention.cu): head dim 64 or 128, S % 128 == 0, masks on the device --------------------------------
+  constexpr AttnFwd kPaddedFwd = [](const void* qkv, const int* m, int B, int S, int h, int, void* o, float* l, cudaStream_t s) {
+    launch_attention_fwd(qkv, m, B, S, h, o, l, s);
   };
-  // key padding: seq_lens int32 [B]; returns B
-  auto attn_check = [attn_qkv_check](const at::Tensor& qkv, const at::Tensor& seq_lens, int heads, const char* who) {
-    attn_qkv_check(qkv, heads, who);
-    check_cuda(seq_lens, "seq_lens");
-    TORCH_CHECK(seq_lens.scalar_type() == at::kInt && seq_lens.dim() == 1 && seq_lens.is_contiguous() && seq_lens.numel() >= 1, who, ": seq_lens must be int32 [B]");
-    TORCH_CHECK(qkv.size(0) % seq_lens.numel() == 0, who, ": qkv rows (", qkv.size(0), ") are not B * S for B = ", seq_lens.numel());
-    TORCH_CHECK(seq_lens.device() == qkv.device(), who, ": seq_lens must be on qkv's device");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(qkv.data_ptr()) & 15) == 0, who, ": qkv must be 16-byte aligned");
-    return (int)seq_lens.numel();
+  constexpr AttnFwd kPackedFwd = [](const void* qkv, const int* m, int B, int S, int h, int, void* o, float* l, cudaStream_t s) {
+    launch_packed_attention_fwd(qkv, m, B, S, h, o, l, s);
   };
-  // packed documents: bounds int32 [B, S, 2] (contiguous, so [B*S, 2] rows of (start, end)); returns B
-  auto packed_check = [attn_qkv_check](const at::Tensor& qkv, const at::Tensor& bounds, int heads, const char* who) {
-    attn_qkv_check(qkv, heads, who);
-    check_cuda(bounds, "bounds");
-    TORCH_CHECK(bounds.scalar_type() == at::kInt && bounds.dim() == 3 && bounds.size(2) == 2 && bounds.is_contiguous() && bounds.numel() >= 2,
-                who, ": bounds must be contiguous int32 [B, S, 2]");
-    TORCH_CHECK(qkv.size(0) == bounds.size(0) * bounds.size(1), who, ": qkv rows (", qkv.size(0), ") are not B * S for bounds [",
-                bounds.size(0), ", ", bounds.size(1), ", 2]");
-    TORCH_CHECK(bounds.device() == qkv.device(), who, ": bounds must be on qkv's device");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(qkv.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(bounds.data_ptr()) & 7) == 0,
-                who, ": qkv must be 16-byte and bounds 8-byte aligned");
-    return (int)bounds.size(0);
+  constexpr AttnFwd kCausalFwd = [](const void* qkv, const int* m, int B, int S, int h, int, void* o, float* l, cudaStream_t s) {
+    launch_causal_attention_fwd(qkv, m, B, S, h, o, l, s);
   };
-  using AttnFwd = void (*)(const void*, const int*, int, int, int, void*, float*, cudaStream_t);
-  using AttnBwd = void (*)(const void*, const void*, const void*, const float*, const int*, int, int, int, float*, void*, cudaStream_t);
-  // (o [B*S, heads*64] bf16, lse [B, heads, S] fp32); optional caller-owned outputs
-  auto attn_fwd = [](AttnFwd launch, const char* who, const at::Tensor& qkv, const at::Tensor& mask, int B, int heads,
-                     c10::optional<at::Tensor> o_out, c10::optional<at::Tensor> lse_out) {
-    c10::cuda::CUDAGuard guard(qkv.device());
-    const int S = (int)(qkv.size(0) / B);
-    at::Tensor o = o_out.has_value() ? *o_out : at::empty({qkv.size(0), (int64_t)heads * 64}, qkv.options());
-    at::Tensor lse = lse_out.has_value() ? *lse_out : at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-    TORCH_CHECK(o.is_cuda() && o.scalar_type() == at::kBFloat16 && o.is_contiguous() && o.numel() == qkv.numel() / 3, who, ": bad o");
-    TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S, who, ": bad lse");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(o.data_ptr()) & 15) == 0 && (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0,
-                who, ": o must be 16-byte and lse 8-byte aligned");
-    launch(qkv.data_ptr(), mask.data_ptr<int>(), B, S, heads, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
-    return std::make_tuple(o, lse);
-  };
-  // dqkv [B*S, 3*heads*64] bf16: the query / key / value column blocks hold dQ / dK / dV
-  auto attn_bwd = [](AttnBwd launch, const char* who, const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o,
-                     const at::Tensor& lse, const at::Tensor& mask, int B, int heads, c10::optional<at::Tensor> dqkv_out) {
-    c10::cuda::CUDAGuard guard(qkv.device());
-    const int S = (int)(qkv.size(0) / B);
-    for (const at::Tensor* t : {&dout, &o}) {
-      check_cuda(*t, "dout / o");
-      TORCH_CHECK(t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->numel() == qkv.numel() / 3 &&
-                  (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, who, ": dout and o must be 16-byte aligned contiguous bf16 [B*S, heads*64]");
-    }
-    TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == (int64_t)B * heads * S &&
-                (reinterpret_cast<uintptr_t>(lse.data_ptr()) & 7) == 0, who, ": lse must be 8-byte aligned contiguous fp32 [B, heads, S]");
-    at::Tensor dqkv = dqkv_out.has_value() ? *dqkv_out : at::empty_like(qkv);
-    TORCH_CHECK(dqkv.is_cuda() && dqkv.scalar_type() == at::kBFloat16 && dqkv.is_contiguous() && dqkv.numel() == qkv.numel() &&
-                (reinterpret_cast<uintptr_t>(dqkv.data_ptr()) & 3) == 0, who, ": bad dqkv");
-    at::Tensor dsum = at::empty({B, heads, S}, qkv.options().dtype(at::kFloat));
-    launch(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), mask.data_ptr<int>(), B, S, heads,
-           dsum.data_ptr<float>(), dqkv.data_ptr(), cur_stream());
-    return dqkv;
-  };
-  m.def("attention_fwd", [attn_check, attn_fwd](at::Tensor qkv, at::Tensor seq_lens, int heads, c10::optional<at::Tensor> o_out,
-                                                c10::optional<at::Tensor> lse_out) {
-    const int B = attn_check(qkv, seq_lens, heads, "attention_fwd");
-    return attn_fwd(&launch_attention_fwd, "attention_fwd", qkv, seq_lens, B, heads, o_out, lse_out);
+  constexpr AttnBwd kPaddedBwd = [](const void* d, const void* qkv, const void* o, const float* l, const int* m, int B, int S, int h, int,
+                                    float* dsum, void* dqkv, cudaStream_t s) { launch_attention_bwd(d, qkv, o, l, m, B, S, h, dsum, dqkv, s); };
+  constexpr AttnBwd kPackedBwd = [](const void* d, const void* qkv, const void* o, const float* l, const int* m, int B, int S, int h, int,
+                                    float* dsum, void* dqkv, cudaStream_t s) { launch_packed_attention_bwd(d, qkv, o, l, m, B, S, h, dsum, dqkv, s); };
+  constexpr AttnBwd kCausalBwd = [](const void* d, const void* qkv, const void* o, const float* l, const int* m, int B, int S, int h, int,
+                                    float* dsum, void* dqkv, cudaStream_t s) { launch_causal_attention_bwd(d, qkv, o, l, m, B, S, h, dsum, dqkv, s); };
+  // key padding: seq_lens int32 [B]
+  m.def("attention_fwd", [](at::Tensor qkv, at::Tensor seq_lens, int heads, c10::optional<at::Tensor> o_out, c10::optional<at::Tensor> lse_out) {
+    return attn_fwd("attention_fwd", kPaddedFwd, 64, Mask::kSeqLens, qkv, seq_lens, heads, heads, o_out, lse_out);
   }, py::arg("qkv"), py::arg("seq_lens"), py::arg("heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
-  m.def("attention_bwd", [attn_check, attn_bwd](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor seq_lens,
-                                                int heads, c10::optional<at::Tensor> dqkv_out) {
-    const int B = attn_check(qkv, seq_lens, heads, "attention_bwd");
-    return attn_bwd(&launch_attention_bwd, "attention_bwd", dout, qkv, o, lse, seq_lens, B, heads, dqkv_out);
+  m.def("attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor seq_lens, int heads,
+                            c10::optional<at::Tensor> dqkv_out) {
+    return attn_bwd("attention_bwd", kPaddedBwd, 64, Mask::kSeqLens, dout, qkv, o, lse, seq_lens, heads, heads, dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("seq_lens"), py::arg("heads"), py::arg("dqkv") = py::none());
-  m.def("packed_attention_fwd", [packed_check, attn_fwd](at::Tensor qkv, at::Tensor bounds, int heads, c10::optional<at::Tensor> o_out,
-                                                         c10::optional<at::Tensor> lse_out) {
-    const int B = packed_check(qkv, bounds, heads, "packed_attention_fwd");
-    return attn_fwd(&launch_packed_attention_fwd, "packed_attention_fwd", qkv, bounds, B, heads, o_out, lse_out);
+  // packed documents: bounds int32 [B, S, 2] (contiguous, so [B*S, 2] rows of (start, end))
+  m.def("packed_attention_fwd", [](at::Tensor qkv, at::Tensor bounds, int heads, c10::optional<at::Tensor> o_out,
+                                   c10::optional<at::Tensor> lse_out) {
+    return attn_fwd("packed_attention_fwd", kPackedFwd, 64, Mask::kBounds, qkv, bounds, heads, heads, o_out, lse_out);
   }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
-  m.def("packed_attention_bwd", [packed_check, attn_bwd](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds,
-                                                         int heads, c10::optional<at::Tensor> dqkv_out) {
-    const int B = packed_check(qkv, bounds, heads, "packed_attention_bwd");
-    return attn_bwd(&launch_packed_attention_bwd, "packed_attention_bwd", dout, qkv, o, lse, bounds, B, heads, dqkv_out);
+  m.def("packed_attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds, int heads,
+                                   c10::optional<at::Tensor> dqkv_out) {
+    return attn_bwd("packed_attention_bwd", kPackedBwd, 64, Mask::kBounds, dout, qkv, o, lse, bounds, heads, heads, dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("dqkv") = py::none());
-  // causal documents: the same bounds and checks as the packed pair
-  m.def("causal_attention_fwd", [packed_check, attn_fwd](at::Tensor qkv, at::Tensor bounds, int heads, c10::optional<at::Tensor> o_out,
-                                                         c10::optional<at::Tensor> lse_out) {
-    const int B = packed_check(qkv, bounds, heads, "causal_attention_fwd");
-    return attn_fwd(&launch_causal_attention_fwd, "causal_attention_fwd", qkv, bounds, B, heads, o_out, lse_out);
+  // causal documents: the same bounds as the packed pair
+  m.def("causal_attention_fwd", [](at::Tensor qkv, at::Tensor bounds, int heads, c10::optional<at::Tensor> o_out,
+                                   c10::optional<at::Tensor> lse_out) {
+    return attn_fwd("causal_attention_fwd", kCausalFwd, 64, Mask::kBounds, qkv, bounds, heads, heads, o_out, lse_out);
   }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
-  m.def("causal_attention_bwd", [packed_check, attn_bwd](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds,
-                                                         int heads, c10::optional<at::Tensor> dqkv_out) {
-    const int B = packed_check(qkv, bounds, heads, "causal_attention_bwd");
-    return attn_bwd(&launch_causal_attention_bwd, "causal_attention_bwd", dout, qkv, o, lse, bounds, B, heads, dqkv_out);
+  m.def("causal_attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds, int heads,
+                                   c10::optional<at::Tensor> dqkv_out) {
+    return attn_bwd("causal_attention_bwd", kCausalBwd, 64, Mask::kBounds, dout, qkv, o, lse, bounds, heads, heads, dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("dqkv") = py::none());
+  // grouped-query causal documents at head dim 64, and causal documents at head dim 128 (kv_heads == heads included)
   m.def("causal_gqa_attention_fwd", [](at::Tensor qkv, at::Tensor bounds, int heads, int kv_heads, c10::optional<at::Tensor> o_out,
-                                              c10::optional<at::Tensor> lse_out) {
-    return gqa_fwd(&launch_causal_gqa_attention_fwd, 64, "causal_gqa_attention_fwd", qkv, bounds, heads, kv_heads, o_out, lse_out);
+                                       c10::optional<at::Tensor> lse_out) {
+    return attn_fwd("causal_gqa_attention_fwd", &launch_causal_gqa_attention_fwd, 64, Mask::kBounds, qkv, bounds, heads, kv_heads, o_out, lse_out);
   }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
   m.def("causal_gqa_attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds, int heads,
-                                              int kv_heads, c10::optional<at::Tensor> dqkv_out) {
-    return gqa_bwd(&launch_causal_gqa_attention_bwd, 64, "causal_gqa_attention_bwd", dout, qkv, o, lse, bounds, heads, kv_heads, dqkv_out);
+                                       int kv_heads, c10::optional<at::Tensor> dqkv_out) {
+    return attn_bwd("causal_gqa_attention_bwd", &launch_causal_gqa_attention_bwd, 64, Mask::kBounds, dout, qkv, o, lse, bounds, heads, kv_heads,
+                    dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"),
      py::arg("dqkv") = py::none());
   m.def("causal_attention_d128_fwd", [](at::Tensor qkv, at::Tensor bounds, int heads, int kv_heads, c10::optional<at::Tensor> o_out,
-                                               c10::optional<at::Tensor> lse_out) {
-    return gqa_fwd(&launch_causal_attention_d128_fwd, 128, "causal_attention_d128_fwd", qkv, bounds, heads, kv_heads, o_out, lse_out);
+                                        c10::optional<at::Tensor> lse_out) {
+    return attn_fwd("causal_attention_d128_fwd", &launch_causal_attention_d128_fwd, 128, Mask::kBounds, qkv, bounds, heads, kv_heads, o_out,
+                    lse_out);
   }, py::arg("qkv"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"), py::arg("o") = py::none(), py::arg("lse") = py::none());
   m.def("causal_attention_d128_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds, int heads,
-                                               int kv_heads, c10::optional<at::Tensor> dqkv_out) {
-    return gqa_bwd(&launch_causal_attention_d128_bwd, 128, "causal_attention_d128_bwd", dout, qkv, o, lse, bounds, heads, kv_heads,
-                   dqkv_out);
+                                        int kv_heads, c10::optional<at::Tensor> dqkv_out) {
+    return attn_bwd("causal_attention_d128_bwd", &launch_causal_attention_d128_bwd, 128, Mask::kBounds, dout, qkv, o, lse, bounds, heads,
+                    kv_heads, dqkv_out);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("heads"), py::arg("kv_heads"),
      py::arg("dqkv") = py::none());
 
@@ -907,16 +965,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // y = rope(qkv) (backward: the transpose rotation); qkv bf16 [rows, (heads + 2*kv_heads)*d] with d = 64 or 128, positions
   // int32 [rows], table fp32 [max_pos, 2, d/2]
   m.def("rotary", [](at::Tensor x, at::Tensor pos, at::Tensor table, int heads, int kv_heads, bool backward, double q_scale) {
-    check_cuda(x, "x"); check_cuda(pos, "position_ids"); check_cuda(table, "cos_sin");
-    TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == 2 &&
-                (table.size(2) == 32 || table.size(2) == 64), "rotary: cos_sin must be contiguous fp32 [max_position, 2, d/2], d = 64 or 128");
+    Args args("rotary");
+    TORCH_CHECK(heads >= 1 && kv_heads >= 1, "rotary: heads and kv_heads must be positive, got ", heads, " and ", kv_heads);
+    args("cos_sin", table, {kF32}, {kAny, 2, kAny});
+    args.expect(table.size(2) == 32 || table.size(2) == 64, "cos_sin", "fp32 [max_position, 2, d/2] with d = 64 or 128", table);
     const int d = (int)table.size(2) * 2;
-    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous() && heads >= 1 && kv_heads >= 1 &&
-                x.size(1) == (int64_t)(heads + 2 * kv_heads) * d, "rotary: x must be contiguous bf16 [rows, (heads + 2*kv_heads)*d] for the "
-                "table's head dim d = ", d);
-    TORCH_CHECK(pos.scalar_type() == at::kInt && pos.is_contiguous() && pos.numel() == x.size(0), "rotary: position_ids must be int32 [rows]");
-    c10::cuda::CUDAGuard guard(x.device());
-    if ((reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) != 0) x = x.clone();
+    args("x", x, {kBF16}, {kAny, (int64_t)(heads + 2 * kv_heads) * d})("position_ids", pos, {kI32}, numel(x.size(0)));
+    args.device();
+    x = aligned(x, 16);
     at::Tensor y = at::empty_like(x);
     launch_rotary(x.data_ptr(), pos.data_ptr<int>(), table.data_ptr<float>(), (int)table.size(0), (size_t)x.size(0), heads, kv_heads, d,
                   y.data_ptr(), backward, cur_stream(), (float)q_scale);
@@ -925,41 +981,33 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("q_scale") = 1.0);
   // Qwen3's per-head q / k RMSNorm + rotary, d = 128: (y, rstd fp32 [rows, heads + kv_heads]) = fwd(qkv, wq, wk, ...);
   // (dqkv, dwq, dwk) = bwd(dy, qkv, rstd, wq, wk, ...) with qkv the forward's input
-  auto qk_norm_check = [](const char* name, at::Tensor x, at::Tensor wq, at::Tensor wk, at::Tensor pos, at::Tensor table, int heads,
-                          int kv_heads) {
-    check_cuda(x, "x"); check_cuda(wq, "q_weight"); check_cuda(wk, "k_weight"); check_cuda(pos, "position_ids"); check_cuda(table, "cos_sin");
-    TORCH_CHECK(table.scalar_type() == at::kFloat && table.is_contiguous() && table.dim() == 3 && table.size(1) == 2 && table.size(2) == 64,
-                name, ": cos_sin must be contiguous fp32 [max_position, 2, 64]");
-    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 2 && x.is_contiguous() && heads >= 1 && kv_heads >= 1 &&
-                x.size(1) == (int64_t)(heads + 2 * kv_heads) * 128, name, ": x must be contiguous bf16 [rows, (heads + 2*kv_heads)*128]");
-    for (const at::Tensor& w : {wq, wk})
-      TORCH_CHECK(w.scalar_type() == at::kBFloat16 && w.is_contiguous() && w.numel() == 128 && w.device() == x.device(), name,
-                  ": q_weight and k_weight must be contiguous bf16 [128] on x's device");
-    TORCH_CHECK(pos.scalar_type() == at::kInt && pos.is_contiguous() && pos.numel() == x.size(0), name, ": position_ids must be int32 [rows]");
+  auto qk_norm_args = [](Args& args, const at::Tensor& x, const at::Tensor& wq, const at::Tensor& wk, const at::Tensor& pos,
+                         const at::Tensor& table, int heads, int kv_heads) {
+    TORCH_CHECK(heads >= 1 && kv_heads >= 1, args.fn(), ": heads and kv_heads must be positive, got ", heads, " and ", kv_heads);
+    args("cos_sin", table, {kF32}, {kAny, 2, 64})("x", x, {kBF16}, {kAny, (int64_t)(heads + 2 * kv_heads) * 128});
+    args("q_weight", wq, {kBF16}, numel(128))("k_weight", wk, {kBF16}, numel(128))("position_ids", pos, {kI32}, numel(x.size(0)));
   };
-  m.def("qk_norm_rotary_fwd", [qk_norm_check](at::Tensor x, at::Tensor wq, at::Tensor wk, at::Tensor pos, at::Tensor table, int heads,
-                                              int kv_heads, double eps) {
-    qk_norm_check("qk_norm_rotary_fwd", x, wq, wk, pos, table, heads, kv_heads);
-    c10::cuda::CUDAGuard guard(x.device());
+  m.def("qk_norm_rotary_fwd", [qk_norm_args](at::Tensor x, at::Tensor wq, at::Tensor wk, at::Tensor pos, at::Tensor table, int heads,
+                                             int kv_heads, double eps) {
+    Args args("qk_norm_rotary_fwd");
+    qk_norm_args(args, x, wq, wk, pos, table, heads, kv_heads);
+    args.device();
     at::Tensor y = at::empty_like(x);
-    at::Tensor rstd = at::empty({x.size(0), heads + kv_heads}, x.options().dtype(at::kFloat));
+    at::Tensor rstd = at::empty({x.size(0), heads + kv_heads}, x.options().dtype(kF32));
     launch_qk_norm_rotary_fwd(x.data_ptr(), wq.data_ptr(), wk.data_ptr(), pos.data_ptr<int>(), table.data_ptr<float>(), (int)table.size(0),
                               (size_t)x.size(0), heads, kv_heads, 128, (float)eps, y.data_ptr(), rstd.data_ptr<float>(), cur_stream());
     return std::make_tuple(y, rstd);
   }, py::arg("x"), py::arg("q_weight"), py::arg("k_weight"), py::arg("position_ids"), py::arg("cos_sin"), py::arg("heads"),
      py::arg("kv_heads"), py::arg("eps"));
-  m.def("qk_norm_rotary_bwd", [qk_norm_check](at::Tensor dy, at::Tensor x, at::Tensor rstd, at::Tensor wq, at::Tensor wk, at::Tensor pos,
-                                              at::Tensor table, int heads, int kv_heads) {
-    qk_norm_check("qk_norm_rotary_bwd", x, wq, wk, pos, table, heads, kv_heads);
-    check_cuda(dy, "dy"); check_cuda(rstd, "rstd");
-    TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && dy.is_contiguous() && dy.sizes() == x.sizes() && dy.device() == x.device(),
-                "qk_norm_rotary_bwd: dy must be contiguous bf16 shaped like x");
-    TORCH_CHECK(rstd.scalar_type() == at::kFloat && rstd.is_contiguous() && rstd.device() == x.device() &&
-                rstd.numel() == x.size(0) * (int64_t)(heads + kv_heads), "qk_norm_rotary_bwd: rstd must be fp32 [rows, heads + kv_heads]");
-    c10::cuda::CUDAGuard guard(x.device());
+  m.def("qk_norm_rotary_bwd", [qk_norm_args](at::Tensor dy, at::Tensor x, at::Tensor rstd, at::Tensor wq, at::Tensor wk, at::Tensor pos,
+                                             at::Tensor table, int heads, int kv_heads) {
+    Args args("qk_norm_rotary_bwd");
+    qk_norm_args(args, x, wq, wk, pos, table, heads, kv_heads);
+    args("dy", dy, {kBF16}, x.sizes())("rstd", rstd, {kF32}, numel(x.size(0) * (int64_t)(heads + kv_heads)));
+    args.device();
     const int parts = qk_norm_rotary_partials((size_t)x.size(0));
     at::Tensor dx = at::empty_like(x);
-    at::Tensor partial = at::empty({2, parts, 128}, x.options().dtype(at::kFloat));
+    at::Tensor partial = at::empty({2, parts, 128}, x.options().dtype(kF32));
     at::Tensor dwq = at::empty_like(wq), dwk = at::empty_like(wk);
     launch_qk_norm_rotary_bwd(dy.data_ptr(), x.data_ptr(), rstd.data_ptr<float>(), wq.data_ptr(), wk.data_ptr(), pos.data_ptr<int>(),
                               table.data_ptr<float>(), (int)table.size(0), (size_t)x.size(0), heads, kv_heads, 128, dx.data_ptr(),
@@ -967,34 +1015,33 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(dx, dwq, dwk);
   }, py::arg("dy"), py::arg("x"), py::arg("rstd"), py::arg("q_weight"), py::arg("k_weight"), py::arg("position_ids"), py::arg("cos_sin"),
      py::arg("heads"), py::arg("kv_heads"));
-  auto aligned32 = [](at::Tensor t) { return (reinterpret_cast<uintptr_t>(t.data_ptr()) & 31) != 0 ? t.clone() : t; };
-  m.def("rmsnorm_fwd", [aligned32](at::Tensor x, at::Tensor gamma, double eps) {
-    check_cuda(x, "x"); check_cuda(gamma, "gamma");
-    TORCH_CHECK(gamma.device() == x.device(), "rmsnorm_fwd: gamma must be on x's device");
-    TORCH_CHECK(x.is_contiguous() && gamma.is_contiguous() && gamma.dtype() == x.dtype() && gamma.numel() == x.size(-1),
-                "rmsnorm_fwd: contiguous x [..., cols] and gamma [cols] of one dtype");
-    c10::cuda::CUDAGuard guard(x.device());
-    x = aligned32(x); gamma = aligned32(gamma);
+  m.def("rmsnorm_fwd", [](at::Tensor x, at::Tensor gamma, double eps) {
+    Args args("rmsnorm_fwd");
+    args("x", x, {kF32, kBF16}, last_dim(kAny))("gamma", gamma, {x.scalar_type()}, numel(x.size(-1)));
+    args.device();
+    x = aligned(x, 32);
+    gamma = aligned(gamma, 32);
     const int cols = (int)x.size(-1);
     const int rows = (int)(x.numel() / cols);
     at::Tensor y = at::empty_like(x);
-    at::Tensor rstd = at::empty({rows}, x.options().dtype(at::kFloat));
+    at::Tensor rstd = at::empty({rows}, x.options().dtype(kF32));
     launch_rmsnorm_fwd(x.data_ptr(), gamma.data_ptr(), dtype_of(x), rows, cols, (float)eps, y.data_ptr(), rstd.data_ptr<float>(), cur_stream());
     return std::make_tuple(y, rstd);
   });
-  m.def("rmsnorm_bwd", [aligned32](at::Tensor dy, at::Tensor x, at::Tensor gamma, at::Tensor rstd) {
-    check_cuda(dy, "dy"); check_cuda(x, "x"); check_cuda(gamma, "gamma"); check_cuda(rstd, "rstd");
-    TORCH_CHECK(gamma.device() == x.device() && dy.device() == x.device() && rstd.device() == x.device() &&
-                rstd.scalar_type() == at::kFloat && rstd.numel() == x.numel() / x.size(-1), "rmsnorm_bwd: dy, gamma and fp32 rstd [rows] on x's device");
-    TORCH_CHECK(dy.is_contiguous() && x.is_contiguous() && dy.sizes() == x.sizes() && dy.dtype() == x.dtype(), "rmsnorm_bwd: matching contiguous inputs");
-    c10::cuda::CUDAGuard guard(x.device());
-    dy = aligned32(dy); x = aligned32(x); gamma = aligned32(gamma.contiguous());
+  m.def("rmsnorm_bwd", [](at::Tensor dy, at::Tensor x, at::Tensor gamma, at::Tensor rstd) {
+    Args args("rmsnorm_bwd");
+    args("x", x, {kF32, kBF16}, last_dim(kAny));
     const int cols = (int)x.size(-1);
     const int rows = (int)(x.numel() / cols);
+    args("dy", dy, {x.scalar_type()}, x.sizes())("gamma", gamma, {x.scalar_type()}, numel(cols), kStrided)("rstd", rstd, {kF32}, numel(rows));
+    args.device();
+    dy = aligned(dy, 32);
+    x = aligned(x, 32);
+    gamma = aligned(gamma.contiguous(), 32);
     const int parts = layernorm_partial_rows(rows);
     at::Tensor dx = at::empty_like(x);
-    at::Tensor partial = at::empty({2 * parts, cols}, x.options().dtype(at::kFloat));
-    at::Tensor counters = at::empty({(cols + 7) / 8}, x.options().dtype(at::kInt));
+    at::Tensor partial = at::empty({2 * parts, cols}, x.options().dtype(kF32));
+    at::Tensor counters = at::empty({(cols + 7) / 8}, x.options().dtype(kI32));
     at::Tensor dgamma = at::empty_like(gamma);
     launch_rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr(), rstd.data_ptr<float>(), dtype_of(x), rows, cols, dx.data_ptr(),
                        partial.data_ptr<float>(), reinterpret_cast<unsigned int*>(counters.data_ptr<int>()), parts, dgamma.data_ptr(),
@@ -1004,12 +1051,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // Gated linear units on one projection [M, 2I]: SwiGLU (gate | up, out = silu(gate) * up) and GeGLU (input | gate,
   // out = gelu(input) * gate).  Forward: out [M, I]; backward: the gradient of both column blocks [M, 2I] from dy [M, I].
   using GluLaunch = void (*)(const void*, const void*, void*, size_t, int, bool, cudaStream_t);
-  auto glu_fwd = [](at::Tensor gate_up, GluLaunch launch, const char* name) {
-    check_cuda(gate_up, "gate_up");
-    TORCH_CHECK(gate_up.scalar_type() == at::kBFloat16 && gate_up.is_contiguous() && gate_up.size(-1) % 16 == 0,
-                name, "_fwd: contiguous bf16 [..., 2I] with I % 8 == 0");
-    c10::cuda::CUDAGuard guard(gate_up.device());
-    if ((reinterpret_cast<uintptr_t>(gate_up.data_ptr()) & 15) != 0) gate_up = gate_up.clone();
+  auto glu_fwd = [](const char* fn, const char* name, at::Tensor gate_up, GluLaunch launch) {
+    Args args(fn);
+    args(name, gate_up, {kBF16}, last_dim(kAny));
+    args.expect(gate_up.size(-1) % 16 == 0, name, "bf16 [..., 2I] with I % 8 == 0", gate_up);
+    args.device();
+    gate_up = aligned(gate_up, 16);
     auto sizes = gate_up.sizes().vec();
     const int inter = (int)(sizes.back() / 2);
     sizes.back() = inter;
@@ -1017,70 +1064,64 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     launch(gate_up.data_ptr(), nullptr, out.data_ptr(), (size_t)(gate_up.numel() / (2 * inter)), inter, false, cur_stream());
     return out;
   };
-  auto glu_bwd = [](at::Tensor dy, at::Tensor gate_up, GluLaunch launch, const char* name) {
-    check_cuda(dy, "dy"); check_cuda(gate_up, "gate_up");
-    TORCH_CHECK(gate_up.scalar_type() == at::kBFloat16 && dy.scalar_type() == at::kBFloat16 && gate_up.is_contiguous() &&
-                dy.is_contiguous() && gate_up.size(-1) % 16 == 0 && dy.numel() * 2 == gate_up.numel() && dy.size(-1) * 2 == gate_up.size(-1),
-                name, "_bwd: contiguous bf16 dy [..., I] and gate_up [..., 2I]");
-    c10::cuda::CUDAGuard guard(gate_up.device());
-    if ((reinterpret_cast<uintptr_t>(gate_up.data_ptr()) & 15) != 0) gate_up = gate_up.clone();
-    if ((reinterpret_cast<uintptr_t>(dy.data_ptr()) & 15) != 0) dy = dy.clone();
+  auto glu_bwd = [](const char* fn, const char* name, at::Tensor dy, at::Tensor gate_up, GluLaunch launch) {
+    Args args(fn);
+    args(name, gate_up, {kBF16}, last_dim(kAny));
+    args.expect(gate_up.size(-1) % 16 == 0, name, "bf16 [..., 2I] with I % 8 == 0", gate_up);
+    args("dy", dy, {kBF16}, last_dim(gate_up.size(-1) / 2));
+    args.expect(dy.numel() * 2 == gate_up.numel(), "dy", "bf16 [..., I] with half the elements of gate_up", dy);
+    args.device();
+    gate_up = aligned(gate_up, 16);
+    dy = aligned(dy, 16);
     const int inter = (int)dy.size(-1);
     at::Tensor out = at::empty_like(gate_up);
     launch(gate_up.data_ptr(), dy.data_ptr(), out.data_ptr(), (size_t)(dy.numel() / inter), inter, true, cur_stream());
     return out;
   };
-  m.def("swiglu_fwd", [glu_fwd](at::Tensor gate_up) { return glu_fwd(gate_up, launch_swiglu, "swiglu"); });
-  m.def("swiglu_bwd", [glu_bwd](at::Tensor dy, at::Tensor gate_up) { return glu_bwd(dy, gate_up, launch_swiglu, "swiglu"); });
-  m.def("geglu_fwd", [glu_fwd](at::Tensor input_gate) { return glu_fwd(input_gate, launch_geglu, "geglu"); });
-  m.def("geglu_bwd", [glu_bwd](at::Tensor dy, at::Tensor input_gate) { return glu_bwd(dy, input_gate, launch_geglu, "geglu"); });
+  m.def("swiglu_fwd", [glu_fwd](at::Tensor gate_up) { return glu_fwd("swiglu_fwd", "gate_up", gate_up, launch_swiglu); });
+  m.def("swiglu_bwd", [glu_bwd](at::Tensor dy, at::Tensor gate_up) { return glu_bwd("swiglu_bwd", "gate_up", dy, gate_up, launch_swiglu); });
+  m.def("geglu_fwd", [glu_fwd](at::Tensor input_gate) { return glu_fwd("geglu_fwd", "input_gate", input_gate, launch_geglu); });
+  m.def("geglu_bwd", [glu_bwd](at::Tensor dy, at::Tensor input_gate) { return glu_bwd("geglu_bwd", "input_gate", dy, input_gate, launch_geglu); });
 
   // ---- mixture of experts (moe.cu, grouped GEMMs in gemm_wgmma.cu) -------------------------------------------------
-  auto moe_tensor = [](const at::Tensor& t, at::ScalarType st, int64_t numel, const char* what) {
-    check_cuda(t, what);
-    TORCH_CHECK(t.scalar_type() == st && t.is_contiguous() && t.numel() == numel, "moe: ", what, " must be a contiguous ",
-                c10::toString(st), " tensor of ", numel, " elements, got ", c10::toString(t.scalar_type()), " ", t.sizes());
-  };
   // logits bf16 [T, E] -> (ids int32 [T, k], gates bf16 [T, k], probsum fp32 [E] (aux) or None)
-  m.def("moe_route", [moe_tensor](at::Tensor logits, int k, bool aux) {
-    TORCH_CHECK(logits.dim() == 2, "moe_route: logits [T, E]");
+  m.def("moe_route", [](at::Tensor logits, int k, bool aux) {
+    Args args("moe_route");
+    args("logits", logits, {kBF16}, {kAny, kAny});
+    args.device();
     const int T = (int)logits.size(0), E = (int)logits.size(1);
-    moe_tensor(logits, at::kBFloat16, (int64_t)T * E, "logits");
-    c10::cuda::CUDAGuard guard(logits.device());
-    at::Tensor ids = at::empty({T, k}, logits.options().dtype(at::kInt));
+    at::Tensor ids = at::empty({T, k}, logits.options().dtype(kI32));
     at::Tensor gates = at::empty({T, k}, logits.options());
     c10::optional<at::Tensor> probsum;
     at::Tensor partial;
     if (aux) {
-      probsum = at::empty({E}, logits.options().dtype(at::kFloat));
-      partial = at::empty({(T + 63) / 64, E}, logits.options().dtype(at::kFloat));
+      probsum = at::empty({E}, logits.options().dtype(kF32));
+      partial = at::empty({(T + 63) / 64, E}, logits.options().dtype(kF32));
     }
     launch_moe_router_fwd(logits.data_ptr(), T, E, k, ids.data_ptr<int>(), gates.data_ptr(), aux ? partial.data_ptr<float>() : nullptr,
                           aux ? probsum->data_ptr<float>() : nullptr, cur_stream());
     return std::make_tuple(ids, gates, probsum);
   });
   // dlogits bf16 [T, E] from d(gates) fp32 [T, k] and d(probsum) fp32 [E] (or None)
-  m.def("moe_router_bwd", [moe_tensor](at::Tensor logits, at::Tensor ids, at::Tensor dgates, c10::optional<at::Tensor> dprobsum) {
-    TORCH_CHECK(logits.dim() == 2 && ids.dim() == 2 && ids.size(0) == logits.size(0), "moe_router_bwd: logits [T, E], ids [T, k]");
+  m.def("moe_router_bwd", [](at::Tensor logits, at::Tensor ids, at::Tensor dgates, c10::optional<at::Tensor> dprobsum) {
+    Args args("moe_router_bwd");
+    args("logits", logits, {kBF16}, {kAny, kAny})("ids", ids, {kI32}, {logits.size(0), kAny});
     const int T = (int)logits.size(0), E = (int)logits.size(1), k = (int)ids.size(1);
-    moe_tensor(logits, at::kBFloat16, (int64_t)T * E, "logits");
-    moe_tensor(ids, at::kInt, (int64_t)T * k, "ids");
-    moe_tensor(dgates, at::kFloat, (int64_t)T * k, "dgates");
-    if (dprobsum.has_value()) moe_tensor(*dprobsum, at::kFloat, E, "dprobsum");
-    c10::cuda::CUDAGuard guard(logits.device());
+    args("dgates", dgates, {kF32}, numel((int64_t)T * k))("dprobsum", dprobsum, {kF32}, numel(E));
+    args.device();
     at::Tensor dlogits = at::empty_like(logits);
     launch_moe_router_bwd(logits.data_ptr(), T, E, k, ids.data_ptr<int>(), dgates.data_ptr<float>(),
                           dprobsum.has_value() ? dprobsum->data_ptr<float>() : nullptr, dlogits.data_ptr(), cur_stream());
     return dlogits;
   });
   // ids int32 [T, k] -> (counts [E], offsets [E + 1], fwd_map [capacity], inv_map [T, k], tile_expert [capacity / 128]), int32
-  m.def("moe_permute", [moe_tensor](at::Tensor ids, int E) {
-    TORCH_CHECK(ids.dim() == 2, "moe_permute: ids [T, k]");
+  m.def("moe_permute", [](at::Tensor ids, int E) {
+    Args args("moe_permute");
+    args("ids", ids, {kI32}, {kAny, kAny});
     const int T = (int)ids.size(0), k = (int)ids.size(1);
-    moe_tensor(ids, at::kInt, (int64_t)T * k, "ids");
     TORCH_CHECK(T >= 1 && E >= 1 && E <= kMoeMaxExperts && k >= 1 && k <= kMoeMaxTopK && k <= E,
                 "moe_permute: needs T >= 1, 1 <= E <= 64, 1 <= k <= min(E, 8), got T=", T, " E=", E, " k=", k);
-    c10::cuda::CUDAGuard guard(ids.device());
+    args.device();
     const int cap = moe_capacity(T, E, k), chunks = moe_chunks(T, k);
     auto opt = ids.options();
     at::Tensor work = at::empty({2, chunks, E}, opt), counts = at::empty({E}, opt), offsets = at::empty({E + 1}, opt);
@@ -1091,69 +1132,61 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   });
   m.def("moe_capacity", [](int T, int E, int k) { return moe_capacity(T, E, k); });
   // x bf16 [T, H] -> x_perm [capacity, H]
-  m.def("moe_gather", [moe_tensor](at::Tensor x, at::Tensor fwd_map, int k) {
-    TORCH_CHECK(x.dim() == 2 && fwd_map.dim() == 1, "moe_gather: x [T, H], fwd_map [capacity]");
-    moe_tensor(x, at::kBFloat16, x.numel(), "x");
-    moe_tensor(fwd_map, at::kInt, fwd_map.numel(), "fwd_map");
-    c10::cuda::CUDAGuard guard(x.device());
+  m.def("moe_gather", [](at::Tensor x, at::Tensor fwd_map, int k) {
+    Args args("moe_gather");
+    args("x", x, {kBF16}, {kAny, kAny})("fwd_map", fwd_map, {kI32}, {kAny});
+    args.device();
     const int H = (int)x.size(1), cap = (int)fwd_map.numel();
     at::Tensor out = at::empty({cap, H}, x.options());
     launch_moe_gather(x.data_ptr(), fwd_map.data_ptr<int>(), cap, H, k, out.data_ptr(), cur_stream());
     return out;
   });
   // forward: a [capacity, K] . w_e^T with w [E, N, K] -> [capacity, N]; dgrad: a [capacity, K] . w_e with w [E, K, N] -> [capacity, N]
-  m.def("moe_gemm", [moe_tensor](at::Tensor a, at::Tensor w, at::Tensor tile_expert, bool dgrad, c10::optional<at::Tensor> out) {
-    TORCH_CHECK(a.dim() == 2 && w.dim() == 3, "moe_gemm: a [rows, K], w [E, *, *]");
-    const int rows = (int)a.size(0), E = (int)w.size(0);
-    const int K = (int)(dgrad ? w.size(1) : w.size(2)), N = (int)(dgrad ? w.size(2) : w.size(1));
-    TORCH_CHECK(a.size(1) == K, "moe_gemm: a has ", a.size(1), " columns, the weight's reduction dim is ", K);
-    moe_tensor(a, at::kBFloat16, a.numel(), "a");
-    moe_tensor(w, at::kBFloat16, w.numel(), "w");
-    moe_tensor(tile_expert, at::kInt, rows / kMoeAlign, "tile_expert");
-    c10::cuda::CUDAGuard guard(a.device());
-    at::Tensor d = out.has_value() ? *out : at::empty({rows, N}, a.options());
-    if (out.has_value()) moe_tensor(d, at::kBFloat16, (int64_t)rows * N, "out");
+  m.def("moe_gemm", [](at::Tensor a, at::Tensor w, at::Tensor tile_expert, bool dgrad, c10::optional<at::Tensor> out) {
+    Args args("moe_gemm");
+    args("w", w, {kBF16}, {kAny, kAny, kAny});
+    const int E = (int)w.size(0), K = (int)(dgrad ? w.size(1) : w.size(2)), N = (int)(dgrad ? w.size(2) : w.size(1));
+    args("a", a, {kBF16}, {kAny, K});
+    const int rows = (int)a.size(0);
+    args("tile_expert", tile_expert, {kI32}, numel(rows / kMoeAlign));
+    at::Tensor d;
+    args.out(d, "out", out, {rows, N}, a.options());
+    args.device();
     launch_gemm_grouped(a.data_ptr(), w.data_ptr(), d.data_ptr(), rows, N, K, E, dgrad, tile_expert.data_ptr<int>(), cur_stream());
     return d;
   }, py::arg("a"), py::arg("w"), py::arg("tile_expert"), py::arg("dgrad"), py::arg("out") = py::none());
   // weight gradient: dw [E, M, N] (bf16), dw_e = a[s_e]^T . b[s_e] over expert e's segment of a [capacity, M] and b [capacity, N]
-  m.def("moe_gemm_wgrad", [moe_tensor](at::Tensor a, at::Tensor b, at::Tensor offsets, c10::optional<at::Tensor> out) {
-    TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.size(0) == b.size(0) && offsets.dim() == 1, "moe_gemm_wgrad: a [rows, M], b [rows, N], offsets [E + 1]");
-    moe_tensor(a, at::kBFloat16, a.numel(), "a");
-    moe_tensor(b, at::kBFloat16, b.numel(), "b");
-    moe_tensor(offsets, at::kInt, offsets.numel(), "offsets");
-    c10::cuda::CUDAGuard guard(a.device());
+  m.def("moe_gemm_wgrad", [](at::Tensor a, at::Tensor b, at::Tensor offsets, c10::optional<at::Tensor> out) {
+    Args args("moe_gemm_wgrad");
+    args("a", a, {kBF16}, {kAny, kAny})("b", b, {kBF16}, {a.size(0), kAny})("offsets", offsets, {kI32}, {kAny});
     const int rows = (int)a.size(0), M = (int)a.size(1), N = (int)b.size(1), E = (int)offsets.numel() - 1;
-    at::Tensor d = out.has_value() ? *out : at::empty({E, M, N}, a.options());
-    if (out.has_value()) moe_tensor(d, at::kBFloat16, (int64_t)E * M * N, "out");
+    at::Tensor d;
+    args.out(d, "out", out, {E, M, N}, a.options());
+    args.device();
     launch_gemm_grouped_wgrad(a.data_ptr(), b.data_ptr(), d.data_ptr(), rows, M, N, E, offsets.data_ptr<int>(), cur_stream());
     return d;
   }, py::arg("a"), py::arg("b"), py::arg("offsets"), py::arg("out") = py::none());
   // out [T, H] = sum_j gate[t, j] * y_perm[inv[t, j]] (gates None: weight 1)
-  m.def("moe_combine", [moe_tensor](at::Tensor y_perm, at::Tensor inv_map, c10::optional<at::Tensor> gates) {
-    TORCH_CHECK(y_perm.dim() == 2 && inv_map.dim() == 2, "moe_combine: y_perm [capacity, H], inv_map [T, k]");
+  m.def("moe_combine", [](at::Tensor y_perm, at::Tensor inv_map, c10::optional<at::Tensor> gates) {
+    Args args("moe_combine");
+    args("y_perm", y_perm, {kBF16}, {kAny, kAny})("inv_map", inv_map, {kI32}, {kAny, kAny});
     const int T = (int)inv_map.size(0), k = (int)inv_map.size(1), H = (int)y_perm.size(1);
-    moe_tensor(y_perm, at::kBFloat16, y_perm.numel(), "y_perm");
-    moe_tensor(inv_map, at::kInt, (int64_t)T * k, "inv_map");
-    if (gates.has_value()) moe_tensor(*gates, at::kBFloat16, (int64_t)T * k, "gates");
-    c10::cuda::CUDAGuard guard(y_perm.device());
+    args("gates", gates, {kBF16}, numel((int64_t)T * k));
+    args.device();
     at::Tensor out = at::empty({T, H}, y_perm.options());
     launch_moe_combine(y_perm.data_ptr(), inv_map.data_ptr<int>(), gates.has_value() ? gates->data_ptr() : nullptr, T, H, k, out.data_ptr(),
                        cur_stream());
     return out;
   });
   // (dy_perm bf16 [capacity, H], dgates fp32 [T, k]) from dout bf16 [T, H]
-  m.def("moe_combine_bwd", [moe_tensor](at::Tensor dout, at::Tensor y_perm, at::Tensor fwd_map, at::Tensor gates) {
-    TORCH_CHECK(dout.dim() == 2 && y_perm.dim() == 2 && gates.dim() == 2 && dout.size(1) == y_perm.size(1) && gates.size(0) == dout.size(0),
-                "moe_combine_bwd: dout [T, H], y_perm [capacity, H], gates [T, k]");
+  m.def("moe_combine_bwd", [](at::Tensor dout, at::Tensor y_perm, at::Tensor fwd_map, at::Tensor gates) {
+    Args args("moe_combine_bwd");
+    args("dout", dout, {kBF16}, {kAny, kAny})("y_perm", y_perm, {kBF16}, {kAny, dout.size(1)})("gates", gates, {kBF16}, {dout.size(0), kAny});
     const int T = (int)dout.size(0), H = (int)dout.size(1), k = (int)gates.size(1), cap = (int)y_perm.size(0);
-    moe_tensor(dout, at::kBFloat16, dout.numel(), "dout");
-    moe_tensor(y_perm, at::kBFloat16, y_perm.numel(), "y_perm");
-    moe_tensor(fwd_map, at::kInt, cap, "fwd_map");
-    moe_tensor(gates, at::kBFloat16, (int64_t)T * k, "gates");
-    c10::cuda::CUDAGuard guard(dout.device());
+    args("fwd_map", fwd_map, {kI32}, numel(cap));
+    args.device();
     at::Tensor dy = at::empty_like(y_perm);
-    at::Tensor dgates = at::empty({T, k}, dout.options().dtype(at::kFloat));
+    at::Tensor dgates = at::empty({T, k}, dout.options().dtype(kF32));
     launch_moe_combine_bwd(dout.data_ptr(), y_perm.data_ptr(), fwd_map.data_ptr<int>(), gates.data_ptr(), cap, H, k, dy.data_ptr(),
                            dgates.data_ptr<float>(), cur_stream());
     return std::make_tuple(dy, dgates);
@@ -1172,23 +1205,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // ---- convolutions on wgmma (conv_wgmma.cu / conv_wgrad_wgmma.cu): channels_last bf16, stride 1, 1x1 or 3x3 ------
   m.def("conv_fprop", [](at::Tensor x, at::Tensor w, int stride, int pad, int mode, int block_n, int base_offset, bool stats,
                          c10::optional<at::Tensor> debug, int kc) {
-    check_cuda(x, "x"); check_cuda(w, "w");
-    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16, "conv_fprop: bf16 tensors");
-    TORCH_CHECK(x.dim() == 4 && x.is_contiguous(at::MemoryFormat::ChannelsLast), "conv_fprop: x must be 4-D channels_last");
-    TORCH_CHECK(w.dim() == 4 && w.size(1) == x.size(1) && w.is_contiguous(at::MemoryFormat::ChannelsLast), "conv_fprop: filter must be [K, C, R, S] channels_last");
+    Args args("conv_fprop");
+    args("x", x, {kBF16}, {kAny, kAny, kAny, kAny}, kChannelsLast)("w", w, {kBF16}, {kAny, x.size(1), kAny, kAny}, kChannelsLast);
+    args("debug", debug, {kI64}, min_numel(16));
     const int R = (int)w.size(2), S = (int)w.size(3);
     TORCH_CHECK(stride == 1 && R == S && pad == (R - 1) / 2, "conv_fprop: stride 1, 'same' padding");
-    c10::cuda::CUDAGuard guard(x.device());
+    args.device();
     const int N = (int)x.size(0), C = (int)x.size(1), H = (int)x.size(2), W = (int)x.size(3), K = (int)w.size(0);
     at::Tensor y = at::empty({N, K, H, W}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
     ConvLaunchCfg cfg; cfg.mode = mode; cfg.block_n = block_n; cfg.set_base_offset = base_offset; cfg.kc = kc;
-    if (debug.has_value()) { TORCH_CHECK(debug->scalar_type() == at::kLong && debug->numel() >= 16 && debug->is_cuda(), "debug: int64[16] cuda"); cfg.debug_counters = debug->data_ptr(); }
+    if (debug.has_value()) cfg.debug_counters = debug->data_ptr();
     at::Tensor st;
     float* stp = nullptr;
     if (stats) {
       const int groups = conv_stat_groups(N, H, W, C, K, R, S, cfg);
       TORCH_CHECK(groups > 0, "conv_fprop: no tile plan");
-      st = at::empty({2, groups, K}, x.options().dtype(at::kFloat));
+      st = at::empty({2, groups, K}, x.options().dtype(kF32));
       stp = st.data_ptr<float>();
     }
     launch_conv_tap_gemm(x.data_ptr(), w.data_ptr(), y.data_ptr(), N, H, W, C, K, R, S, false, cfg, stp, cur_stream());
@@ -1200,41 +1232,34 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("conv_dgrad", [](at::Tensor dy, at::Tensor w, int stride, int pad, int mode, int block_n, int base_offset, int kc,
                          c10::optional<at::Tensor> addend, c10::optional<at::Tensor> bn_x, c10::optional<at::Tensor> bn_mask,
                          c10::optional<at::Tensor> bn_stats) {
-    check_cuda(dy, "dy"); check_cuda(w, "w");
-    TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16, "conv_dgrad: bf16 tensors");
-    TORCH_CHECK(dy.dim() == 4 && dy.is_contiguous(at::MemoryFormat::ChannelsLast), "conv_dgrad: dy must be 4-D channels_last");
-    TORCH_CHECK(w.dim() == 4 && w.size(0) == dy.size(1) && w.is_contiguous(at::MemoryFormat::ChannelsLast), "conv_dgrad: filter must be [K, C, R, S] channels_last");
+    Args args("conv_dgrad");
+    args("dy", dy, {kBF16}, {kAny, kAny, kAny, kAny}, kChannelsLast)("w", w, {kBF16}, {dy.size(1), kAny, kAny, kAny}, kChannelsLast);
     const int R = (int)w.size(2), S = (int)w.size(3);
     TORCH_CHECK(stride == 1 && R == S && pad == (R - 1) / 2, "conv_dgrad: stride 1, 'same' padding");
-    c10::cuda::CUDAGuard guard(dy.device());
     const int N = (int)dy.size(0), K = (int)dy.size(1), H = (int)dy.size(2), W = (int)dy.size(3), C = (int)w.size(1);
+    args("addend", addend, {kBF16}, {N, C, H, W}, kChannelsLast)("bn_x", bn_x, {kBF16}, {N, C, H, W}, kChannelsLast);
+    args("bn_mask", bn_mask, {kU8}, numel((int64_t)N * H * W * (C / 8)));
+    if (bn_x.has_value()) {
+      args("bn_stats", args.required("bn_stats", bn_stats), {kF32}, {kAny, C});
+      args.expect(bn_stats->size(0) >= 2, "bn_stats", "fp32 [>= 2, C] (rows: mean, rstd)", *bn_stats);
+    }
+    args.device();
     at::Tensor dx = at::empty({N, C, H, W}, dy.options().memory_format(at::MemoryFormat::ChannelsLast));
     ConvLaunchCfg cfg; cfg.mode = mode; cfg.block_n = block_n; cfg.set_base_offset = base_offset; cfg.kc = kc;
     ConvBwdFusion fuse;
     bool any = false;
     at::Tensor part;
     float* pp = nullptr;
-    if (addend.has_value()) {
-      TORCH_CHECK(addend->sizes() == dx.sizes() && addend->scalar_type() == at::kBFloat16 && addend->is_contiguous(at::MemoryFormat::ChannelsLast),
-                  "conv_dgrad: addend must match dx (bf16, channels_last)");
-      fuse.addend = addend->data_ptr(); any = true;
-    }
+    if (addend.has_value()) { fuse.addend = addend->data_ptr(); any = true; }
     if (bn_x.has_value()) {
-      TORCH_CHECK(bn_stats.has_value() && bn_stats->scalar_type() == at::kFloat && bn_stats->dim() == 2 && bn_stats->size(1) == C && bn_stats->size(0) >= 2,
-                  "conv_dgrad: bn_stats must be fp32 [>=2, C] (rows: mean, rstd)");
-      TORCH_CHECK(bn_x->sizes() == dx.sizes() && bn_x->scalar_type() == at::kBFloat16 && bn_x->is_contiguous(at::MemoryFormat::ChannelsLast),
-                  "conv_dgrad: bn_x must match dx (bf16, channels_last)");
       fuse.bn_x = bn_x->data_ptr();
-      if (bn_mask.has_value()) {
-        TORCH_CHECK(bn_mask->scalar_type() == at::kByte && bn_mask->numel() == (int64_t)N * H * W * (C / 8), "conv_dgrad: bn_mask must be uint8 [N*H*W, C/8]");
-        fuse.bn_mask = bn_mask->data_ptr();
-      }
+      if (bn_mask.has_value()) fuse.bn_mask = bn_mask->data_ptr();
       fuse.bn_mean = bn_stats->data_ptr<float>();
       fuse.bn_rstd = bn_stats->data_ptr<float>() + C;
       // the statistics workspace of the data gradient has one row per CTA of an n-tile over the Cin columns
       const int groups = conv_stat_groups(N, H, W, K, C, R, S, cfg);
       TORCH_CHECK(groups > 0, "conv_dgrad: no tile plan");
-      part = at::empty({2, groups, C}, dy.options().dtype(at::kFloat));
+      part = at::empty({2, groups, C}, dy.options().dtype(kF32));
       pp = part.data_ptr<float>();
       any = true;
     }
@@ -1244,18 +1269,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
      py::arg("base_offset") = 0, py::arg("kc") = 0, py::arg("addend") = py::none(), py::arg("bn_x") = py::none(),
      py::arg("bn_mask") = py::none(), py::arg("bn_stats") = py::none());
   m.def("conv_wgrad", [](at::Tensor dy, at::Tensor x, int ksize, int stride, int pad, int split, int tile_m, int tile_n) {
-    check_cuda(dy, "dy"); check_cuda(x, "x");
-    TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && x.scalar_type() == at::kBFloat16, "conv_wgrad: bf16 tensors");
-    TORCH_CHECK(dy.dim() == 4 && dy.is_contiguous(at::MemoryFormat::ChannelsLast) && x.dim() == 4 && x.is_contiguous(at::MemoryFormat::ChannelsLast),
-                "conv_wgrad: channels_last 4-D tensors");
-    TORCH_CHECK(stride == 1 && pad == (ksize - 1) / 2 && dy.size(0) == x.size(0) && dy.size(2) == x.size(2) && dy.size(3) == x.size(3),
-                "conv_wgrad: stride 1, 'same' padding");
-    c10::cuda::CUDAGuard guard(dy.device());
+    Args args("conv_wgrad");
+    args("dy", dy, {kBF16}, {kAny, kAny, kAny, kAny}, kChannelsLast)("x", x, {kBF16}, {dy.size(0), kAny, dy.size(2), dy.size(3)}, kChannelsLast);
+    TORCH_CHECK(stride == 1 && pad == (ksize - 1) / 2, "conv_wgrad: stride 1, 'same' padding");
+    args.device();
     const int N = (int)x.size(0), C = (int)x.size(1), H = (int)x.size(2), W = (int)x.size(3), K = (int)dy.size(1);
     WgradCfg cfg; cfg.split = split; cfg.tile_m = tile_m; cfg.tile_n = tile_n;
     const size_t ws = conv_wgrad_workspace_floats(N, H, W, C, K, ksize, ksize, cfg);
     TORCH_CHECK(ws > 0, "conv_wgrad: unsupported geometry / tiling");
-    at::Tensor work = at::empty({(int64_t)ws}, x.options().dtype(at::kFloat));
+    at::Tensor work = at::empty({(int64_t)ws}, x.options().dtype(kF32));
     at::Tensor dw = at::empty({K, C, ksize, ksize}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
     launch_conv_wgrad(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), N, H, W, C, K, ksize, ksize, cfg, work.data_ptr<float>(), cur_stream());
     return dw;
@@ -1264,58 +1286,52 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   // strided 7x7 stem (3 -> 64 channels, stride 2, padding 3) on the wgmma tap-GEMM through an overlapping-window tensor map
   m.def("stem_conv_supported", [](int H, int W) { StemGeom g; return stem_geom(H, W, &g); });
   m.def("stem_pack_input", [](at::Tensor x) {
-    check_cuda(x, "x");
-    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && x.dim() == 4 && x.size(1) == 3 && x.is_contiguous(at::MemoryFormat::ChannelsLast),
-                "stem_pack_input: x must be bf16 [N,3,H,W] channels_last");
-    c10::cuda::CUDAGuard guard(x.device());
+    Args args("stem_pack_input");
+    args("x", x, {kBF16}, {kAny, 3, kAny, kAny}, kChannelsLast);
     const int N = (int)x.size(0), H = (int)x.size(2), W = (int)x.size(3);
     StemGeom g;
     TORCH_CHECK(stem_geom(H, W, &g), "stem_pack_input: unsupported image size ", H, "x", W);
+    args.device();
     at::Tensor xp = at::empty({N, g.Hp2, g.Wp, 8}, x.options());
     launch_stem_pack_input(x.data_ptr(), xp.data_ptr(), N, H, W, cur_stream());
     return xp;
   });
   m.def("stem_pack_weight", [](at::Tensor w) {
-    check_cuda(w, "w");
-    TORCH_CHECK(w.scalar_type() == at::kBFloat16 && w.dim() == 4 && w.size(0) == 64 && w.size(1) == 3 && w.size(2) == 7 && w.size(3) == 7 &&
-                w.is_contiguous(at::MemoryFormat::ChannelsLast), "stem_pack_weight: w must be bf16 [64,3,7,7] channels_last");
-    c10::cuda::CUDAGuard guard(w.device());
+    Args args("stem_pack_weight");
+    args("w", w, {kBF16}, {64, 3, 7, 7}, kChannelsLast);
+    args.device();
     at::Tensor w2 = at::empty({w.size(0), (int64_t)kStemK}, w.options().memory_format(at::MemoryFormat::Contiguous));
     launch_stem_pack_weight(w.data_ptr(), w2.data_ptr(), (int)w.size(0), cur_stream());
     return w2;
   });
   m.def("stem_conv_fprop_packed", [](at::Tensor xp, at::Tensor w2, int H, int W, bool stats, bool resident, bool debug) {
-    check_cuda(xp, "xp"); check_cuda(w2, "w2");
-    c10::cuda::CUDAGuard guard(xp.device());
+    Args args("stem_conv_fprop_packed");
     StemGeom g;
+    TORCH_CHECK(stem_geom(H, W, &g), "stem_conv_fprop_packed: unsupported image size ", H, "x", W);
+    args("xp", xp, {kBF16}, {kAny, g.Hp2, g.Wp, 8})("w2", w2, {kBF16}, {kAny, kStemK});
+    args.device();
     const int N = (int)xp.size(0), K = (int)w2.size(0);
-    TORCH_CHECK(stem_geom(H, W, &g) && xp.dim() == 4 && xp.size(1) == g.Hp2 && xp.size(2) == g.Wp && xp.size(3) == 8 && xp.is_contiguous() &&
-                w2.dim() == 2 && w2.size(1) == kStemK && w2.is_contiguous() && xp.scalar_type() == at::kBFloat16 && w2.scalar_type() == at::kBFloat16,
-                "stem_conv_fprop_packed: operands do not match the packed layout");
     at::Tensor y = at::empty({N, K, g.Ho, g.Wo}, xp.options().memory_format(at::MemoryFormat::ChannelsLast));
     at::Tensor part, dbg;
     float* sp = nullptr;
-    if (stats) { part = at::empty({2, stem_stat_groups(N, H, W), K}, xp.options().dtype(at::kFloat)); sp = part.data_ptr<float>(); }
-    if (debug) dbg = at::zeros({16}, xp.options().dtype(at::kLong));
+    if (stats) { part = at::empty({2, stem_stat_groups(N, H, W), K}, xp.options().dtype(kF32)); sp = part.data_ptr<float>(); }
+    if (debug) dbg = at::zeros({16}, xp.options().dtype(kI64));
     launch_stem_conv_fprop(xp.data_ptr(), w2.data_ptr(), y.data_ptr(), N, H, W, K, sp, resident, debug ? dbg.data_ptr() : nullptr, cur_stream());
     return std::make_tuple(y, part, dbg);
   }, py::arg("xp"), py::arg("w2"), py::arg("H"), py::arg("W"), py::arg("stats") = false, py::arg("resident") = true, py::arg("debug") = false);
   m.def("stem_conv_fprop", [](at::Tensor x, at::Tensor w, bool stats, bool resident) {
-    check_cuda(x, "x"); check_cuda(w, "w");
-    TORCH_CHECK(x.scalar_type() == at::kBFloat16 && w.scalar_type() == at::kBFloat16, "stem_conv_fprop: bf16 tensors");
-    TORCH_CHECK(x.dim() == 4 && x.size(1) == 3 && x.is_contiguous(at::MemoryFormat::ChannelsLast), "stem_conv_fprop: x must be [N,3,H,W] channels_last");
-    TORCH_CHECK(w.dim() == 4 && w.size(0) == 64 && w.size(1) == 3 && w.size(2) == 7 && w.size(3) == 7 && w.is_contiguous(at::MemoryFormat::ChannelsLast),
-                "stem_conv_fprop: w must be [64,3,7,7] channels_last");
-    c10::cuda::CUDAGuard guard(x.device());
+    Args args("stem_conv_fprop");
+    args("x", x, {kBF16}, {kAny, 3, kAny, kAny}, kChannelsLast)("w", w, {kBF16}, {64, 3, 7, 7}, kChannelsLast);
     const int N = (int)x.size(0), H = (int)x.size(2), W = (int)x.size(3), K = (int)w.size(0);
     StemGeom g;
     TORCH_CHECK(stem_geom(H, W, &g), "stem_conv_fprop: unsupported image size ", H, "x", W);
+    args.device();
     at::Tensor xp = at::empty({N, g.Hp2, g.Wp, 8}, x.options().memory_format(at::MemoryFormat::Contiguous));
     at::Tensor w2 = at::empty({K, (int64_t)kStemK}, x.options().memory_format(at::MemoryFormat::Contiguous));
     at::Tensor y = at::empty({N, K, g.Ho, g.Wo}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
     at::Tensor part;
     float* sp = nullptr;
-    if (stats) { part = at::empty({2, stem_stat_groups(N, H, W), K}, x.options().dtype(at::kFloat).memory_format(at::MemoryFormat::Contiguous)); sp = part.data_ptr<float>(); }
+    if (stats) { part = at::empty({2, stem_stat_groups(N, H, W), K}, x.options().dtype(kF32).memory_format(at::MemoryFormat::Contiguous)); sp = part.data_ptr<float>(); }
     cudaStream_t st = cur_stream();
     launch_stem_pack_input(x.data_ptr(), xp.data_ptr(), N, H, W, st);
     launch_stem_pack_weight(w.data_ptr(), w2.data_ptr(), K, st);
@@ -1323,19 +1339,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(y, part, xp);
   }, py::arg("x"), py::arg("w"), py::arg("stats") = false, py::arg("resident") = true);
   m.def("stem_conv_wgrad", [](at::Tensor dy, at::Tensor xp, int H, int W, int variant, bool unpack) {
-    check_cuda(dy, "dy"); check_cuda(xp, "xp");
-    TORCH_CHECK(dy.scalar_type() == at::kBFloat16 && xp.scalar_type() == at::kBFloat16, "stem_conv_wgrad: bf16 tensors");
-    TORCH_CHECK(dy.dim() == 4 && dy.is_contiguous(at::MemoryFormat::ChannelsLast) && xp.is_contiguous(), "stem_conv_wgrad: dy channels_last, xp packed");
+    Args args("stem_conv_wgrad");
     TORCH_CHECK(variant == 0 || variant == 1, "stem_conv_wgrad: variant 0 (dedicated kernel) or 1 (generic kernel)");
-    c10::cuda::CUDAGuard guard(dy.device());
-    const int N = (int)dy.size(0), K = (int)dy.size(1);
     StemGeom g;
-    TORCH_CHECK(stem_geom(H, W, &g) && dy.size(2) == g.Ho && dy.size(3) == g.Wo && xp.dim() == 4 && xp.size(0) == N && xp.size(1) == g.Hp2 &&
-                xp.size(2) == g.Wp && xp.size(3) == 8, "stem_conv_wgrad: geometry mismatch");
+    TORCH_CHECK(stem_geom(H, W, &g), "stem_conv_wgrad: unsupported image size ", H, "x", W);
+    args("dy", dy, {kBF16}, {kAny, kAny, g.Ho, g.Wo}, kChannelsLast)("xp", xp, {kBF16}, {dy.size(0), g.Hp2, g.Wp, 8});
+    args.device();
+    const int N = (int)dy.size(0), K = (int)dy.size(1);
     const size_t ws = stem_wgrad_workspace_floats(N, H, W, K, variant);
     TORCH_CHECK(ws > 0, "stem_conv_wgrad: unsupported geometry");
     auto plain = dy.options().memory_format(at::MemoryFormat::Contiguous);
-    at::Tensor work = at::empty({(int64_t)ws}, plain.dtype(at::kFloat));
+    at::Tensor work = at::empty({(int64_t)ws}, plain.dtype(kF32));
     at::Tensor dw2 = variant == 0 ? at::empty({(int64_t)kStemK, K}, plain) : at::empty({K, (int64_t)kStemK}, plain);
     cudaStream_t st = cur_stream();
     launch_stem_conv_wgrad(dy.data_ptr(), xp.data_ptr(), dw2.data_ptr(), N, H, W, K, variant, work.data_ptr<float>(), st);
@@ -1350,7 +1364,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(ok, pl.mode, pl.BH, pl.BI, pl.num_m_tiles, pl.dense_rows, pl.acc_rows, pl.a_rows);
   });
 
-  // ---- fused BatchNorm ---------------------------------------------------------------------------
+  // ---- fused BatchNorm: x [N, C, H, W] channels_last viewed as [R = N*H*W, C]; gamma, beta and statistics fp32 ----------------
   m.def("set_bn_pdl", &set_bn_pdl);
   m.def("set_bn_two_pass", &set_bn_two_pass);
   m.def("bn_resident_error", &bn_resident_error);
@@ -1359,97 +1373,106 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     bn_workspace_sizes(R, C, &pf, &cn);
     return std::make_tuple((long long)pf, (long long)cn);
   });
-  m.def("bn_forward", [](at::Tensor x, c10::optional<at::Tensor> residual, at::Tensor gamma, at::Tensor beta,
-                         c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
-                         c10::optional<at::Tensor> num_batches, double eps, double momentum, bool relu, at::Tensor partial,
-                         at::Tensor counters) {
-    check_cuda(x, "x");
-    TORCH_CHECK(x.dim() == 4 && x.is_contiguous(at::MemoryFormat::ChannelsLast), "bn_forward: x must be 4-D channels_last");
-    TORCH_CHECK(gamma.scalar_type() == at::kFloat && beta.scalar_type() == at::kFloat, "bn_forward: fp32 affine parameters");
-    c10::cuda::CUDAGuard guard(x.device());
+  // the forward's x, residual and affine / running statistics
+  auto bn_fwd_args = [](Args& args, const at::Tensor& x, const c10::optional<at::Tensor>& residual, const at::Tensor& gamma,
+                        const at::Tensor& beta, const c10::optional<at::Tensor>& running_mean, const c10::optional<at::Tensor>& running_var,
+                        const c10::optional<at::Tensor>& num_batches) {
+    args("x", x, {kF32, kBF16}, {kAny, kAny, kAny, kAny}, kChannelsLast);
+    const int64_t C = x.size(1);
+    args("residual", residual, {x.scalar_type()}, x.sizes(), kChannelsLast)("gamma", gamma, {kF32}, numel(C))("beta", beta, {kF32}, numel(C));
+    args("running_mean", running_mean, {kF32}, numel(C))("running_var", running_var, {kF32}, numel(C))("num_batches", num_batches, {kI64}, numel(1));
+  };
+  // the backward's dy (`dy_layout`: kStrided when the binding makes it channels_last), x, ReLU mask (uint8 [R, C/8], read with
+  // relu), gamma and the forward's statistics (save_mean, save_rstd, ...)
+  auto bn_bwd_args = [](Args& args, const at::Tensor& dy, Layout dy_layout, const at::Tensor& x, const c10::optional<at::Tensor>& mask, bool relu,
+                        const at::Tensor& gamma, const at::Tensor& stats) {
+    args("x", x, {kF32, kBF16}, {kAny, kAny, kAny, kAny}, kChannelsLast);
+    const int64_t C = x.size(1), R = x.numel() / std::max<int64_t>(C, 1);
+    args("dy", dy, {x.scalar_type()}, x.sizes(), dy_layout);
+    if (relu) args("y", args.required("y", mask), {kU8}, {R, C / 8});
+    args("gamma", gamma, {kF32}, numel(C))("stats", stats, {kF32}, min_numel(2 * C));
+  };
+  m.def("bn_forward", [bn_fwd_args](at::Tensor x, c10::optional<at::Tensor> residual, at::Tensor gamma, at::Tensor beta,
+                                    c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
+                                    c10::optional<at::Tensor> num_batches, double eps, double momentum, bool relu, at::Tensor partial,
+                                    at::Tensor counters) {
+    Args args("bn_forward");
+    bn_fwd_args(args, x, residual, gamma, beta, running_mean, running_var, num_batches);
+    args("partial", partial, {kF32}, min_numel(0))("counters", counters, {kI32}, min_numel(0));
+    args.device();
     const int C = (int)x.size(1);
     const int R = (int)(x.numel() / C);
+    size_t pf = 0, cn = 0;
+    bn_workspace_sizes(R, C, &pf, &cn);   // reads the device's limits, so after the guard
+    args("partial", partial, {kF32}, min_numel((int64_t)pf))("counters", counters, {kI32}, min_numel((int64_t)cn));
     at::Tensor y = at::empty_like(x);
-    auto fopt = x.options().dtype(at::kFloat);
-    at::Tensor stats = at::empty({4, C}, fopt);   // rows: save_mean, save_rstd, scale, shift
-    const void* res = nullptr;
-    if (residual.has_value()) {
-      TORCH_CHECK(residual->sizes() == x.sizes() && residual->dtype() == x.dtype() && residual->is_contiguous(at::MemoryFormat::ChannelsLast),
-                  "bn_forward: residual must match x (shape, dtype, channels_last)");
-      res = residual->data_ptr();
-    }
+    at::Tensor stats = at::empty({4, C}, x.options().dtype(kF32));   // rows: save_mean, save_rstd, scale, shift
     float* st = stats.data_ptr<float>();
-    at::Tensor mask = relu ? at::empty({(int64_t)R, (int64_t)(C / 8)}, x.options().dtype(at::kByte)) : at::Tensor();
-    launch_bn_forward(x.data_ptr(), res, y.data_ptr(), relu ? mask.data_ptr<uint8_t>() : nullptr, dtype_of(x), R, C, gamma.data_ptr<float>(), beta.data_ptr<float>(),
+    at::Tensor mask = relu ? at::empty({(int64_t)R, (int64_t)(C / 8)}, x.options().dtype(kU8)) : at::Tensor();
+    launch_bn_forward(x.data_ptr(), residual.has_value() ? residual->data_ptr() : nullptr, y.data_ptr(), relu ? mask.data_ptr<uint8_t>() : nullptr,
+                      dtype_of(x), R, C, gamma.data_ptr<float>(), beta.data_ptr<float>(),
                       running_mean.has_value() ? running_mean->data_ptr<float>() : nullptr,
                       running_var.has_value() ? running_var->data_ptr<float>() : nullptr,
                       num_batches.has_value() ? (long long*)num_batches->data_ptr<int64_t>() : nullptr, st, st + C, st + 2 * C, st + 3 * C,
                       partial.data_ptr<float>(), (unsigned int*)counters.data_ptr<int>(), (float)eps, (float)momentum, relu, cur_stream());
     return std::make_tuple(y, stats, mask);
   });
-  m.def("bn_forward_partials", [](at::Tensor x, c10::optional<at::Tensor> residual, at::Tensor gamma, at::Tensor beta,
-                                  c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
-                                  c10::optional<at::Tensor> num_batches, double eps, double momentum, bool relu, at::Tensor partial) {
-    check_cuda(x, "x"); check_cuda(partial, "partial");
-    TORCH_CHECK(x.dim() == 4 && x.is_contiguous(at::MemoryFormat::ChannelsLast), "bn_forward_partials: x must be 4-D channels_last");
-    TORCH_CHECK(gamma.scalar_type() == at::kFloat && beta.scalar_type() == at::kFloat, "bn_forward_partials: fp32 affine parameters");
+  m.def("bn_forward_partials", [bn_fwd_args](at::Tensor x, c10::optional<at::Tensor> residual, at::Tensor gamma, at::Tensor beta,
+                                             c10::optional<at::Tensor> running_mean, c10::optional<at::Tensor> running_var,
+                                             c10::optional<at::Tensor> num_batches, double eps, double momentum, bool relu, at::Tensor partial) {
+    Args args("bn_forward_partials");
+    bn_fwd_args(args, x, residual, gamma, beta, running_mean, running_var, num_batches);
+    args("partial", partial, {kF32}, {2, kAny, x.size(1)});   // [2, groups, C]
+    args.device();
     const int C = (int)x.size(1);
     const int R = (int)(x.numel() / C);
-    TORCH_CHECK(partial.scalar_type() == at::kFloat && partial.dim() == 3 && partial.size(0) == 2 && partial.size(2) == C &&
-                partial.is_contiguous(), "bn_forward_partials: partial statistics must be fp32 [2, groups, C]");
-    c10::cuda::CUDAGuard guard(x.device());
     at::Tensor y = at::empty_like(x);
-    at::Tensor stats = at::empty({4, C}, x.options().dtype(at::kFloat));   // rows: save_mean, save_rstd, scale, shift
-    const void* res = nullptr;
-    if (residual.has_value()) {
-      TORCH_CHECK(residual->sizes() == x.sizes() && residual->dtype() == x.dtype() && residual->is_contiguous(at::MemoryFormat::ChannelsLast),
-                  "bn_forward_partials: residual must match x (shape, dtype, channels_last)");
-      res = residual->data_ptr();
-    }
+    at::Tensor stats = at::empty({4, C}, x.options().dtype(kF32));   // rows: save_mean, save_rstd, scale, shift
     float* st = stats.data_ptr<float>();
-    at::Tensor mask = relu ? at::empty({(int64_t)R, (int64_t)(C / 8)}, x.options().dtype(at::kByte)) : at::Tensor();
-    launch_bn_forward_from_partials(x.data_ptr(), res, y.data_ptr(), relu ? mask.data_ptr<uint8_t>() : nullptr, dtype_of(x), R, C,
-                                    gamma.data_ptr<float>(), beta.data_ptr<float>(),
+    at::Tensor mask = relu ? at::empty({(int64_t)R, (int64_t)(C / 8)}, x.options().dtype(kU8)) : at::Tensor();
+    launch_bn_forward_from_partials(x.data_ptr(), residual.has_value() ? residual->data_ptr() : nullptr, y.data_ptr(),
+                                    relu ? mask.data_ptr<uint8_t>() : nullptr, dtype_of(x), R, C, gamma.data_ptr<float>(), beta.data_ptr<float>(),
                                     running_mean.has_value() ? running_mean->data_ptr<float>() : nullptr,
                                     running_var.has_value() ? running_var->data_ptr<float>() : nullptr,
                                     num_batches.has_value() ? (long long*)num_batches->data_ptr<int64_t>() : nullptr, st, st + C, st + 2 * C,
                                     st + 3 * C, partial.data_ptr<float>(), (int)partial.size(1), (float)eps, (float)momentum, relu, cur_stream());
     return std::make_tuple(y, stats, mask);
   });
-  m.def("bn_backward_partials", [](at::Tensor dy, at::Tensor x, c10::optional<at::Tensor> y, at::Tensor gamma, at::Tensor stats, bool relu,
-                                   bool need_dres, at::Tensor partial) {
-    check_cuda(dy, "dy"); check_cuda(partial, "partial");
-    c10::cuda::CUDAGuard guard(x.device());
+  m.def("bn_backward_partials", [bn_bwd_args](at::Tensor dy, at::Tensor x, c10::optional<at::Tensor> y, at::Tensor gamma, at::Tensor stats,
+                                              bool relu, bool need_dres, at::Tensor partial) {
+    Args args("bn_backward_partials");
+    bn_bwd_args(args, dy, kChannelsLast, x, y, relu, gamma, stats);
+    args("partial", partial, {kF32}, {2, kAny, x.size(1)});   // [2, groups, C]
+    args.device();
     const int C = (int)x.size(1);
     const int R = (int)(x.numel() / C);
-    TORCH_CHECK(partial.scalar_type() == at::kFloat && partial.dim() == 3 && partial.size(0) == 2 && partial.size(2) == C && partial.is_contiguous(),
-                "bn_backward_partials: partial sums must be fp32 [2, groups, C]");
-    TORCH_CHECK(dy.is_contiguous(at::MemoryFormat::ChannelsLast) && dy.sizes() == x.sizes() && dy.dtype() == x.dtype(), "bn_backward_partials: dy must match x");
     at::Tensor dx = at::empty_like(x);
     at::Tensor dres = need_dres ? at::empty_like(x) : at::Tensor();
-    at::Tensor dparams = at::empty({2, C}, x.options().dtype(at::kFloat));   // rows: dgamma, dbeta
+    at::Tensor dparams = at::empty({2, C}, x.options().dtype(kF32));   // rows: dgamma, dbeta
     float* dp = dparams.data_ptr<float>();
     const float* st = stats.data_ptr<float>();
-    TORCH_CHECK(!relu || (y.has_value() && y->scalar_type() == at::kByte), "bn_backward_partials: needs the ReLU bitmask written by bn_forward");
     launch_bn_backward_from_partials(dy.data_ptr(), x.data_ptr(), relu ? y->data_ptr() : nullptr, dx.data_ptr(), need_dres ? dres.data_ptr() : nullptr,
                                      dtype_of(x), R, C, gamma.data_ptr<float>(), st, st + C, dp, dp + C, partial.data_ptr<float>(), (int)partial.size(1),
                                      relu, cur_stream());
     return std::make_tuple(dx, dres, dparams);
   });
-  m.def("bn_backward", [](at::Tensor dy, at::Tensor x, c10::optional<at::Tensor> y, at::Tensor gamma, at::Tensor stats, bool relu,
-                          bool need_dres, at::Tensor partial, at::Tensor counters) {
-    check_cuda(dy, "dy");
-    c10::cuda::CUDAGuard guard(x.device());
+  m.def("bn_backward", [bn_bwd_args](at::Tensor dy, at::Tensor x, c10::optional<at::Tensor> y, at::Tensor gamma, at::Tensor stats, bool relu,
+                                     bool need_dres, at::Tensor partial, at::Tensor counters) {
+    Args args("bn_backward");
+    bn_bwd_args(args, dy, kStrided, x, y, relu, gamma, stats);
+    args("partial", partial, {kF32}, min_numel(0))("counters", counters, {kI32}, min_numel(0));
+    args.device();
     const int C = (int)x.size(1);
     const int R = (int)(x.numel() / C);
+    size_t pf = 0, cn = 0;
+    bn_workspace_sizes(R, C, &pf, &cn);   // reads the device's limits, so after the guard
+    args("partial", partial, {kF32}, min_numel((int64_t)pf))("counters", counters, {kI32}, min_numel((int64_t)cn));
     at::Tensor dyc = dy.is_contiguous(at::MemoryFormat::ChannelsLast) ? dy : dy.contiguous(at::MemoryFormat::ChannelsLast);
     at::Tensor dx = at::empty_like(x);
     at::Tensor dres = need_dres ? at::empty_like(x) : at::Tensor();
-    auto fopt = x.options().dtype(at::kFloat);
-    at::Tensor dparams = at::empty({4, C}, fopt);   // rows: dgamma, dbeta, coef1, coef2
+    at::Tensor dparams = at::empty({4, C}, x.options().dtype(kF32));   // rows: dgamma, dbeta, coef1, coef2
     float* dp = dparams.data_ptr<float>();
     const float* st = stats.data_ptr<float>();
-    TORCH_CHECK(!relu || (y.has_value() && y->scalar_type() == at::kByte), "bn_backward: needs the ReLU bitmask written by bn_forward");
     launch_bn_backward(dyc.data_ptr(), x.data_ptr(), relu ? y->data_ptr() : nullptr, dx.data_ptr(), need_dres ? dres.data_ptr() : nullptr,
                        dtype_of(x), R, C, gamma.data_ptr<float>(), st, st + C, dp, dp + C, dp + 2 * C, partial.data_ptr<float>(),
                        (unsigned int*)counters.data_ptr<int>(), relu, cur_stream());
@@ -1458,19 +1481,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ---- max pooling ------------------------------------------------------------------------------
   m.def("maxpool3x3s2_fwd", [](at::Tensor x) {
-    check_cuda(x, "x");
-    TORCH_CHECK(x.dim() == 4 && x.is_contiguous(at::MemoryFormat::ChannelsLast), "maxpool3x3s2_fwd: 4-D channels_last input");
-    c10::cuda::CUDAGuard guard(x.device());
+    Args args("maxpool3x3s2_fwd");
+    args("x", x, {kF32, kBF16}, {kAny, kAny, kAny, kAny}, kChannelsLast);
+    args.device();
     const int N = (int)x.size(0), C = (int)x.size(1), H = (int)x.size(2), W = (int)x.size(3);
     const int OH = (H + 2 - 3) / 2 + 1, OW = (W + 2 - 3) / 2 + 1;
     at::Tensor y = at::empty({N, C, OH, OW}, x.options().memory_format(at::MemoryFormat::ChannelsLast));
-    at::Tensor idx = at::empty({N, C, OH, OW}, x.options().dtype(at::kByte).memory_format(at::MemoryFormat::ChannelsLast));
+    at::Tensor idx = at::empty({N, C, OH, OW}, x.options().dtype(kU8).memory_format(at::MemoryFormat::ChannelsLast));
     launch_maxpool3x3s2_fwd(x.data_ptr(), y.data_ptr(), idx.data_ptr<uint8_t>(), dtype_of(x), N, H, W, C, cur_stream());
     return std::make_tuple(y, idx);
   });
   m.def("maxpool3x3s2_bwd", [](at::Tensor dy, at::Tensor idx, int64_t H, int64_t W) {
-    check_cuda(dy, "dy");
-    c10::cuda::CUDAGuard guard(dy.device());
+    Args args("maxpool3x3s2_bwd");
+    args("dy", dy, {kF32, kBF16}, {kAny, kAny, (H + 1) / 2, (W + 1) / 2}, kStrided)("idx", idx, {kU8}, dy.sizes(), kChannelsLast);
+    args.device();
     at::Tensor dyc = dy.is_contiguous(at::MemoryFormat::ChannelsLast) ? dy : dy.contiguous(at::MemoryFormat::ChannelsLast);
     const int N = (int)dy.size(0), C = (int)dy.size(1);
     at::Tensor dx = at::empty({N, C, H, W}, dy.options().memory_format(at::MemoryFormat::ChannelsLast));
@@ -1480,14 +1504,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
 
   // ---- input pipeline ---------------------------------------------------------------------------
   m.def("normalize_to_channels_last", [](at::Tensor src, at::Tensor dst, at::Tensor mean, at::Tensor inv_std, double in_scale) {
-    check_cuda(src, "src"); check_cuda(dst, "dst");
-    TORCH_CHECK(src.dim() == 4 && src.is_contiguous(), "normalize_to_channels_last: src NCHW contiguous");
+    Args args("normalize_to_channels_last");
+    args("src", src, {kU8, kF32}, {kAny, kAny, kAny, kAny});
     // dst may carry extra (zero-filled) channels: [N, C_out >= C, H, W]
-    TORCH_CHECK(dst.dim() == 4 && dst.is_contiguous(at::MemoryFormat::ChannelsLast) && dst.size(0) == src.size(0) &&
-                dst.size(1) >= src.size(1) && dst.size(2) == src.size(2) && dst.size(3) == src.size(3),
-                "normalize_to_channels_last: dst must be channels_last [N, C_out >= C, H, W]");
-    TORCH_CHECK(mean.numel() >= src.size(1) && inv_std.numel() >= src.size(1), "normalize_to_channels_last: mean/inv_std per source channel");
-    c10::cuda::CUDAGuard guard(src.device());
+    args("dst", dst, {kBF16, kF32}, {src.size(0), kAny, src.size(2), src.size(3)}, kChannelsLast);
+    args.expect(dst.size(1) >= src.size(1), "dst", "channels_last [N, C_out >= C, H, W]", dst);
+    args("mean", mean, {kF32}, min_numel(src.size(1)))("inv_std", inv_std, {kF32}, min_numel(src.size(1)));
+    args.device();
     launch_normalize_to_channels_last(src.data_ptr(), dtype_of(src), dst.data_ptr(), dtype_of(dst), (int)src.size(0), (int)src.size(1),
                                       (int)dst.size(1), (int)src.size(2), (int)src.size(3), mean.data_ptr<float>(), inv_std.data_ptr<float>(),
                                       (float)in_scale, cur_stream());

@@ -229,3 +229,22 @@ def test_normalize_pads_channels_with_zeros():
     ref = ((x - mean.view(1, 3, 1, 1)) * istd.view(1, 3, 1, 1)).to(torch.bfloat16)
     assert torch.allclose(dst[:, :3].float(), ref.float(), atol=1e-2, rtol=1e-2)
     assert float(dst[:, 3:].abs().max()) == 0.0
+
+
+def test_peer_copy_bytes_bounded_by_tensor():
+    """peer_pull / peer_push refuse to move more bytes than their tensor holds.  The tensor is a narrow view of a larger
+    allocation, so even a missed check would stay inside allocated memory."""
+    import os
+    from b200ddp import _ext
+    C = _ext.get()
+    arena = C.PeerArena(0, 1, torch.cuda.current_device(), 1 << 21, os.urandom(8).hex())
+    try:
+        arena.bind_socket()
+        arena.exchange()
+        view = torch.zeros(1024, device="cuda")[256:512]
+        for fn in (C.peer_pull, C.peer_push):
+            with pytest.raises(RuntimeError, match=rf"^{fn.__name__}: bytes must be at most"):
+                fn(arena, 0, 0, view, view.numel() * view.element_size() + 4, 1)
+        torch.cuda.synchronize()
+    finally:
+        arena.close()
