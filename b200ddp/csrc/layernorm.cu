@@ -1,7 +1,7 @@
 // LayerNorm forward / backward (needed by the BERT
 // config).  One warp per row, 16-byte vector loads, fp32 statistics; backward produces dx in the same
-// pass as per-CTA partial dgamma/dbeta, finished by a small column-reduce kernel (no atomics, so the
-// result is deterministic).
+// kernel as per-CTA partial dgamma/dbeta, finished by a small column-reduce kernel (no floating-point
+// atomics, so the result is deterministic).
 #include "ops.h"
 
 namespace b200 {
@@ -33,18 +33,15 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_fwd_kernel(const T* __re
   }
 }
 
-// Each CTA owns a contiguous stripe of rows.  Warps compute dx for their rows and accumulate
-// dgamma/dbeta for the columns they touch into registers -> shared -> one partial row per CTA.
+// Each CTA owns a contiguous stripe of rows.  Warps compute dx for their rows; then each thread sums dgamma/dbeta over
+// the stripe for its columns, row by row, into one partial row per CTA.  The order is fixed (no atomics), so the
+// partials, and dgamma/dbeta, are bitwise repeatable.  The second pass re-reads the stripe, which the first just
+// brought into L2.
 template <typename T>
 __global__ void __launch_bounds__(kLnThreads) layernorm_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ gamma,
                                                                    const float* __restrict__ mean, const float* __restrict__ rstd, int rows, int cols,
                                                                    T* __restrict__ dx, float* __restrict__ dgamma_partial,
                                                                    float* __restrict__ dbeta_partial) {
-  extern __shared__ float smem[];            // [2][cols] per-CTA column accumulators
-  float* sg = smem;
-  float* sb = smem + cols;
-  for (int i = threadIdx.x; i < 2 * cols; i += blockDim.x) smem[i] = 0.f;
-  __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
   const int rows_per_cta = (rows + gridDim.x - 1) / gridDim.x;
   const int r0 = blockIdx.x * rows_per_cta;
@@ -65,18 +62,20 @@ __global__ void __launch_bounds__(kLnThreads) layernorm_bwd_kernel(const T* __re
     T* dxr = dx + (size_t)row * cols;
     for (int i = lane; i < cols; i += 32) {
       const float xn = (to_f32<T>(xr[i]) - mu) * rs;
-      const float dyv = to_f32<T>(dyr[i]);
-      const float dg = dyv * to_f32<T>(gamma[i]);
+      const float dg = to_f32<T>(dyr[i]) * to_f32<T>(gamma[i]);
       dxr[i] = from_f32<T>(rs * (dg - s1 - xn * s2));
-      // column i is only ever touched by lane (i % 32) of each warp: shared atomics across warps
-      atomicAdd(&sg[i], dyv * xn);
-      atomicAdd(&sb[i], dyv);
     }
   }
-  __syncthreads();
   for (int i = threadIdx.x; i < cols; i += blockDim.x) {
-    dgamma_partial[(size_t)blockIdx.x * cols + i] = sg[i];
-    dbeta_partial[(size_t)blockIdx.x * cols + i] = sb[i];
+    float sg = 0.f, sb = 0.f;
+    for (int row = r0; row < r1; ++row) {
+      const size_t o = (size_t)row * cols + i;
+      const float dyv = to_f32<T>(dy[o]);
+      sg += dyv * ((to_f32<T>(x[o]) - mean[row]) * rstd[row]);
+      sb += dyv;
+    }
+    dgamma_partial[(size_t)blockIdx.x * cols + i] = sg;
+    dbeta_partial[(size_t)blockIdx.x * cols + i] = sb;
   }
 }
 
@@ -462,7 +461,6 @@ void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, DT
 void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, const float* mean, const float* rstd, DType dt, int rows,
                           int cols, void* dx, float* dgamma_partial, float* dbeta_partial, int partial_rows, void* dgamma,
                           void* dbeta, cudaStream_t s) {
-  const size_t smem = 2 * (size_t)cols * sizeof(float);
   const bool fast = (cols % 8 == 0) && cols <= 8 * 32 * kLnChunks &&
                     ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx) |
                       reinterpret_cast<uintptr_t>(gamma)) & 31u) == 0;
@@ -486,13 +484,13 @@ void launch_layernorm_bwd(const void* dy, const void* x, const void* gamma, cons
                                                                                  dgamma_partial, counters, (float*)dgamma, (float*)dbeta);
     }
   } else if (dt == DType::BF16) {
-    layernorm_bwd_kernel<__nv_bfloat16><<<partial_rows, kLnThreads, smem, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
+    layernorm_bwd_kernel<__nv_bfloat16><<<partial_rows, kLnThreads, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
                                                                              (const __nv_bfloat16*)gamma, mean, rstd, rows, cols,
                                                                              (__nv_bfloat16*)dx, dgamma_partial, dbeta_partial);
     layernorm_bwd_finish_kernel<__nv_bfloat16><<<(cols + 255) / 256, 256, 0, s>>>(dgamma_partial, dbeta_partial, partial_rows, cols,
                                                                                 (__nv_bfloat16*)dgamma, (__nv_bfloat16*)dbeta);
   } else {
-    layernorm_bwd_kernel<float><<<partial_rows, kLnThreads, smem, s>>>((const float*)dy, (const float*)x, (const float*)gamma, mean, rstd,
+    layernorm_bwd_kernel<float><<<partial_rows, kLnThreads, 0, s>>>((const float*)dy, (const float*)x, (const float*)gamma, mean, rstd,
                                                                      rows, cols, (float*)dx, dgamma_partial, dbeta_partial);
     layernorm_bwd_finish_kernel<float><<<(cols + 255) / 256, 256, 0, s>>>(dgamma_partial, dbeta_partial, partial_rows, cols,
                                                                         (float*)dgamma, (float*)dbeta);
