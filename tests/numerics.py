@@ -17,6 +17,11 @@ bf16 outputs reach about 0.99 of theirs: the half-ulp rounding term is exact, so
 
 The norms accumulate on the CUDA cores in IEEE fp32, so their sums take the plain worst-case bound n · u · Σ|terms|.
 
+Attention (the last section) reuses C_ACC for its tensor-core products.  On the same H100, test_gpu_attention_elementwise.py
+reaches at most 0.037 of the lse bound at C_ACC = 2 and 0.23 at C_ACC = 0.25, and fails it at C_ACC = 0 (2.2): the lse
+has no bf16 rounding to hide behind, so it is what calibrates C_ACC there.  EXP_ULPS = 0 passes as well as 2: no bound
+is filled by the exp2 terms, so EXP_ULPS stays at exp2f's documented maximum.  Its bf16 outputs reach 0.95.
+
 Set B200DDP_NUMERICS_LOG to a file path to append "<group> <largest error / bound>" for every check, which is how C_ACC
 is recalibrated after a kernel change.
 """
@@ -173,3 +178,187 @@ def layernorm_bwd_reference(dy, x, gamma, mean, rstd, rms=False):
 def rel_err(a, b):
     """The global relative error the older GEMM tests assert below 1e-2: it cannot see a local error."""
     return float((a.double() - b.double()).norm() / (b.double().norm() + 1e-12))
+
+
+# ---- attention ----------------------------------------------------------------------------------------------------------
+# Per (batch row, query head), with scale c, visible set V_i of query i and n_i = |V_i|.  The kernels compute the scores
+# s = c q kᵀ in fp32 on the tensor cores, p = exp2(s log2e - m log2e) against the running row maximum m (rescaling the
+# accumulators by alpha = exp2((m_old - m) log2e) once per key tile of 128 they visit), round p to bf16 for P V, and
+# divide by the fp32 sum of the unrounded p.  The backward recomputes P' = exp(s - lse) from the forward's own lse, forms
+# dS = P' (dO vᵀ - D) with D = rowsum(dO o) from the forward's own o, and rounds P' and dS to bf16 before the products
+# dV = P'ᵀ dO, dK = c dSᵀ q and dQ = c dS k.  So, with A = C_ACC d u |q||k|ᵀ the score error:
+#   rho_ij   relative error of one unnormalised p: c A_ij + u (EXP_ULPS + 3 + 2 (|s_ij| + max_j |s_ij|)) + (EXP_ULPS + 3) u T_i
+#            (the exponent's rounding is absolute, so it grows with |s| and the maximum; T_i key tiles rescale the sums)
+#   o        (P (2⁻⁸ + rho)) |V| + C_ACC (n_i + 1) u P|V| + |o| (sum_j P_ij rho_ij + (n_i + 2) u), then the bf16 rounding
+#   lse      sum_j P_ij rho_ij + (n_i + 2) u + 2 u (|lse| + 1)
+#   dS       P' rho' |dP - D| + P' (err dP + err D) + 2 u |dS|, plus 2⁻⁸ for its bf16 rounding (rho': |lse| for the maximum,
+#            no rescale), with err dP = C_ACC d u |dO||v|ᵀ and err D = d u sum |dO o|
+#   dV dK dQ that error times |dO|, |q| or |k|, plus C_ACC (m + 1) u times the absolute product over the m summed terms,
+#            plus u for the multiply by c when c is not a power of two, then the bf16 rounding
+# EXP_ULPS is exp2f's documented maximum error; the build does not use --use_fast_math, so exp2f, logf and 1 / l are the
+# accurate versions.
+EXP_ULPS = 2.0
+BF16_U = 2.0 ** -8            # P and dS are rounded to bf16 before their products
+ATTN_BLOCK = 1 << 22          # elements of one [B, H, rows, S] block of the attention references (32 MB in float64)
+KEY_TILE = 128                # keys per forward tile (one online-softmax rescale each)
+
+
+def attention_visible(mask, S, causal=False):
+    """[B, S, S] bool, query i sees key j.  mask: seq_lens int [B] (key j is visible iff j < len, len clamped to [0, S] as
+    the kernels' clamped_len does) or bounds int [B, S, 2] (start clamped to [0, S], end to [start, S] as row_bounds
+    does); causal also needs j <= i."""
+    j = torch.arange(S, device=mask.device)
+    if mask.dim() == 1:
+        n = mask.long().clamp(0, S)
+        return (j[None, None, :] < n[:, None, None]).expand(-1, S, -1).contiguous()
+    b = mask.long().reshape(-1, S, 2)
+    start = b[..., 0].clamp(0, S)
+    end = torch.maximum(b[..., 1], start).clamp(max=S)
+    vis = (j >= start[..., None]) & (j < end[..., None])
+    if causal:
+        vis &= j[None, None, :] <= j[None, :, None]
+    return vis
+
+
+def _attn_chunks(B, H, S):
+    rows = max(16, min(1024, ATTN_BLOCK // (B * H * S)))
+    return [(r, min(r + rows, S)) for r in range(0, S, rows)]
+
+
+def _by_batch_row(fn, tensors, visible, args):
+    """fn on one batch row at a time, its (ref, bound) pairs concatenated: keeps the [B, H, S, d] terms of a wide problem
+    small."""
+    parts = [fn(*(t[b:b + 1] for t in tensors), visible[b:b + 1], *args) for b in range(visible.shape[0])]
+    return {key: tuple(torch.cat([p[key][i] for p in parts]) for i in range(2)) for key in parts[0]}
+
+
+def _kv_per_query_head(t, H):
+    """K or V [B, Hkv, S, d] as float64 [B, H, S, d]: query head h reads K/V head h // (H // Hkv)."""
+    return t.double().repeat_interleave(H // t.shape[1], dim=1)
+
+
+def _scale_ulps(scale):
+    return 0.0 if math.frexp(scale)[0] == 0.5 else 1.0
+
+
+def attention_reference(q, k, v, visible, scale, c_acc=None, exp_ulps=None):
+    """fp64 softmax attention of q [B, H, S, d] over k, v [B, Hkv, S, d] (bf16) where visible [B, S, S] allows, and the
+    element-wise bounds of the kernels' arithmetic: {"o": (ref, acc) [B, H, S, d], "lse": (ref, bnd) [B, H, S]}.  A row
+    that sees no key has o = 0 and lse = -inf, with bound 0 (plus bound()'s floor for o)."""
+    c_acc = C_ACC if c_acc is None else c_acc
+    e = EXP_ULPS if exp_ulps is None else exp_ulps
+    B, H, S, d = q.shape
+    if B > 1 and B * H * S * d > ATTN_BLOCK:
+        return _by_batch_row(attention_reference, (q, k, v), visible, (scale, c_acc, exp_ulps))
+    K, V = _kv_per_query_head(k, H), _kv_per_query_head(v, H)
+    o = torch.zeros(B, H, S, d, dtype=torch.float64, device=q.device)
+    o_acc = torch.zeros_like(o)
+    lse = torch.zeros(B, H, S, dtype=torch.float64, device=q.device)
+    lse_bnd = torch.zeros_like(lse)
+    for r0, r1 in _attn_chunks(B, H, S):
+        Q = q[:, :, r0:r1].double()
+        vis = visible[:, None, r0:r1]
+        s = scale * (Q @ K.transpose(-1, -2))
+        A = c_acc * d * U * (Q.abs() @ K.abs().transpose(-1, -2))
+        n = vis.sum(-1).double()
+        tiles = vis.reshape(B, 1, r1 - r0, S // KEY_TILE, KEY_TILE).any(-1).sum(-1).double()
+        l = torch.logsumexp(s.masked_fill(~vis, -math.inf), -1)
+        live = torch.isfinite(l)
+        P = torch.where(vis, torch.exp(s - torch.where(live, l, 0.0)[..., None]), 0.0)
+        smax = torch.where(vis, s.abs(), 0.0).amax(-1, keepdim=True)
+        rho = scale * A + U * (e + 3 + 2 * (s.abs() + smax)) + (e + 3) * U * tiles[..., None]
+        Prho = P * rho
+        sum_prho = Prho.sum(-1)
+        oc = P @ V
+        o[:, :, r0:r1] = oc
+        Va = V.abs()
+        o_acc[:, :, r0:r1] = ((BF16_U * P + Prho) @ Va + (c_acc * U * (n + 1))[..., None] * (P @ Va)
+                              + oc.abs() * (sum_prho + (n + 2) * U)[..., None])
+        lse[:, :, r0:r1] = l
+        lse_bnd[:, :, r0:r1] = torch.where(live, sum_prho + (n + 2) * U + 2 * U * (torch.where(live, l, 0.0).abs() + 1), 0.0)
+    return {"o": (o, o_acc), "lse": (lse, lse_bnd)}
+
+
+def attention_bwd_reference(q, k, v, o, lse, dout, visible, scale, c_acc=None, exp_ulps=None):
+    """fp64 gradients of attention_reference at the kernel's own o [B, H, S, d] (bf16) and lse [B, H, S] (fp32), taken
+    as exact inputs, for the output gradient dout [B, H, S, d] (bf16), and the bounds of the kernels' arithmetic before
+    output rounding: {"dq": (ref, acc) [B, H, S, d], "dk": ..., "dv": ... [B, Hkv, S, d]}; dK and dV sum each group of
+    query heads.  A query whose lse is -inf has P' = 0."""
+    c_acc = C_ACC if c_acc is None else c_acc
+    e = EXP_ULPS if exp_ulps is None else exp_ulps
+    B, H, S, d = q.shape
+    if B > 1 and B * H * S * d > ATTN_BLOCK:
+        return _by_batch_row(attention_bwd_reference, (q, k, v, o, lse, dout), visible, (scale, c_acc, exp_ulps))
+    Hkv = k.shape[1]
+    K, V = _kv_per_query_head(k, H), _kv_per_query_head(v, H)
+    su = _scale_ulps(scale)
+    dq = torch.zeros(B, H, S, d, dtype=torch.float64, device=q.device)
+    dq_acc = torch.zeros_like(dq)
+    dk, dk_mag, dk_err, dv, dv_mag, dv_err = (torch.zeros(B, Hkv, S, d, dtype=torch.float64, device=q.device)
+                                              for _ in range(6))
+    m = torch.zeros(B, Hkv, S, dtype=torch.float64, device=q.device)
+
+    def group(t):                                               # the sum over each group of query heads
+        return t.reshape(B, Hkv, H // Hkv, *t.shape[2:]).sum(2)
+    for r0, r1 in _attn_chunks(B, H, S):
+        Q, dO, O = (t[:, :, r0:r1].double() for t in (q, dout, o))
+        L = lse[:, :, r0:r1].double()
+        live = torch.isfinite(L)
+        Lz = torch.where(live, L, 0.0)[..., None]
+        vis = visible[:, None, r0:r1] & live[..., None]
+        s = scale * (Q @ K.transpose(-1, -2))
+        A = c_acc * d * U * (Q.abs() @ K.abs().transpose(-1, -2))
+        P = torch.where(vis, torch.exp(s - Lz), 0.0)
+        dP = dO @ V.transpose(-1, -2)
+        err_dP = c_acc * d * U * (dO.abs() @ V.abs().transpose(-1, -2))
+        D = (dO * O).sum(-1, keepdim=True)
+        err_D = d * U * (dO * O).abs().sum(-1, keepdim=True)
+        dS = P * (dP - D)
+        rho = scale * A + U * (e + 3 + 2 * (s.abs() + Lz.abs()))
+        err_dS = P * rho * (dP - D).abs() + P * (err_dP + err_D) + 2 * U * dS.abs()
+        err_dS = err_dS + BF16_U * (dS.abs() + err_dS)
+        err_P = P * (rho + BF16_U * (1 + rho))
+        dSa = dS.abs()
+        n = vis.sum(-1).double()
+        dq[:, :, r0:r1] = scale * (dS @ K)
+        Ka = K.abs()
+        dq_acc[:, :, r0:r1] = scale * (err_dS @ Ka + (U * (c_acc * (n + 1) + su))[..., None] * (dSa @ Ka))
+        m += group(vis.sum(-2).double())
+        Pt, dSt = P.transpose(-1, -2), dS.transpose(-1, -2)
+        dv += group(Pt @ dO)
+        dv_mag += group(Pt @ dO.abs())
+        dv_err += group(err_P.transpose(-1, -2) @ dO.abs())
+        dk += group(dSt @ Q)
+        dk_mag += group(dSa.transpose(-1, -2) @ Q.abs())
+        dk_err += group(err_dS.transpose(-1, -2) @ Q.abs())
+    m = m[..., None]
+    return {"dq": (dq, dq_acc),
+            "dk": (scale * dk, scale * (dk_err + U * (c_acc * (m + 1) + su) * dk_mag)),
+            "dv": (dv, dv_err + c_acc * U * (m + 1) * dv_mag)}
+
+
+def check_lse(name, got, ref, bnd, group=None):
+    """check() of an lse [B, H, S]: -inf exactly where the reference is -inf, the finite entries element by element."""
+    dead = torch.isneginf(ref)
+    wrong = torch.isneginf(got) != dead
+    if wrong.any():
+        i = int(wrong.reshape(-1).nonzero()[0])
+        raise AssertionError(f"{name}: {int(wrong.sum())} of {ref.numel()} entries are -inf where the reference is not or "
+                             f"the reverse; first at {_where(i, tuple(ref.shape))}: got {float(got.reshape(-1)[i])!r}, "
+                             f"reference {float(ref.reshape(-1)[i])!r}")
+    return check(name, torch.where(dead, 0.0, got.double()), torch.where(dead, 0.0, ref), bnd + FLOOR, group)
+
+
+def check_attention(name, got, ref, group=None):
+    """Checks every output in `got` ({"o", "lse"} or {"dq", "dk", "dv"}, kernel outputs in the references' layouts) against
+    the (ref, acc) pairs of attention_reference / attention_bwd_reference; groups log as "<group> <output>".  Returns the
+    largest error / bound per output."""
+    worst = {}
+    for key, t in got.items():
+        r, a = ref[key]
+        g = None if group is None else f"{group} {key}"
+        if key == "lse":
+            worst[key] = check_lse(f"{name}: lse [b, h, s]", t, r, a, g)
+        else:
+            worst[key] = check(f"{name}: {key} [b, h, s, d]", t, r, bound(r, a, t.dtype), g)
+    return worst
