@@ -17,10 +17,35 @@ bf16 outputs reach about 0.99 of theirs: the half-ulp rounding term is exact, so
 
 The norms accumulate on the CUDA cores in IEEE fp32, so their sums take the plain worst-case bound n · u · Σ|terms|.
 
-Attention (the last section) reuses C_ACC for its tensor-core products.  On the same H100, test_gpu_attention_elementwise.py
+Attention reuses C_ACC for its tensor-core products.  On the same H100, test_gpu_attention_elementwise.py
 reaches at most 0.037 of the lse bound at C_ACC = 2 and 0.23 at C_ACC = 0.25, and fails it at C_ACC = 0 (2.2): the lse
 has no bf16 rounding to hide behind, so it is what calibrates C_ACC there.  EXP_ULPS = 0 passes as well as 2: no bound
 is filled by the exp2 terms, so EXP_ULPS stays at exp2f's documented maximum.  Its bf16 outputs reach 0.95.
+
+ResNet-50 (the last section).  The convolutions (conv_wgmma.cu, conv_wgrad_wgmma.cu, the stem) are GEMMs on the tensor
+cores and take the GEMM bound with the same C_ACC, P being the same convolution of the absolute values:
+  fprop   K = R S Cin (the stem: 147; its packed layout only adds exact zero products)
+  dgrad   K = R S Cout, plus one term for the fp32 addend the epilogue adds before rounding
+  wgrad   K = the pixels one split sums on the tensor cores, plus the fixed-order fp32 reduction of the split partials
+          (its longest chain, split lanes + 8, times u P)
+then the bf16 rounding of the output.  The epilogue statistics (column sums of the stored bf16 output, and S1 / S2 of the
+BatchNorm backward fused into dgrad) are fp32 chains of 32 rows per warp + one add per tile the CTA ran + the 4 epilogue
+warps: conv_epilogue_depth().
+BatchNorm (batchnorm.cu) sums x and x² (backward: dy* and dy* x̂) per channel in fp32 in an order fixed by its launch path;
+D is the longest chain of fp32 additions any term goes through in that order (bn_two_pass_depth here, the resident and
+from-partials depths in test_gpu_batchnorm_elementwise.py), so each sum is within D u Σ|terms|.  The forward then forms
+mean = Σx / R, var = max(Σx²/R - mean², 0), rstd = rsqrtf(var + eps) (2 ulp), scale = γ rstd, shift = β - mean scale and
+y = relu(x scale + shift (+ residual)); the bound carries every rounding at the magnitude it meets: the variance error is
+relative to Σx²/R (not to var, which cancels when |mean| >> σ), rstd is bounded over the interval of var, and y's error is
+relative to |x scale|, |mean scale| and |β| (not to |x̂|).  The backward takes the kernel's own mean, rstd and ReLU mask
+as exact inputs and follows its dx = a dy* + b x + c, a = γ rstd, b = -a rstd S2/R, c = -a (S1/R - mean rstd S2/R), whose
+b x and c also cancel when |mean| >> σ.  Max pool 3x3/s2/p1: the forward is exact (bitwise, the first maximum in (ky, kx)
+order wins); the backward sums at most four dy per input in fp32.  MSE: dout = 2 (out - t) gscale / n; the loss is a
+two-stage fp32 sum.
+On an H100 80GB HBM3 (700 W power limit) test_gpu_conv_elementwise.py and test_gpu_batchnorm_elementwise.py reach at most,
+at C_ACC = 2: conv fprop 0.992, dgrad 0.993, wgrad 0.994 and stem 0.984 / 0.926 (bf16 outputs, filled by their rounding
+term); epilogue statistics 0.065, fused S1 / S2 0.037; BatchNorm y and dx 0.996, mean 0.11, rstd 0.12 (0.061 with every
+channel at |mean| = 64σ), running statistics 0.38, dgamma / dbeta 0.073; max pool 0.996; MSE dout 0.996, loss 0.033.
 
 Set B200DDP_NUMERICS_LOG to a file path to append "<group> <largest error / bound>" for every check, which is how C_ACC
 is recalibrated after a kernel change.
@@ -362,3 +387,217 @@ def check_attention(name, got, ref, group=None):
         else:
             worst[key] = check(f"{name}: {key} [b, h, s, d]", t, r, bound(r, a, t.dtype), g)
     return worst
+
+
+# ---- ResNet-50: convolutions, BatchNorm, max pool, MSE --------------------------------------------------------------------
+# (The bounds of this section are documented in the module docstring.)
+
+
+def _conv64(t):
+    return t.double().contiguous()
+
+
+def conv_reference(direction, a, b, stride=1, pad=0, shape=None, addend=None, k_pixels=None, reduce_depth=0, c_acc=None):
+    """fp64 reference and accumulation bound (before output rounding) of one convolution, both float64 in the output's logical
+    NCHW shape.  direction "fprop": a = x, b = w; "dgrad": a = dy, b = w, shape = x's shape, optional fp32 addend added
+    before rounding; "wgrad": a = dy, b = x, shape = w's shape, k_pixels = the pixels one split sums, reduce_depth = the
+    longest fp32 chain of the split reduction."""
+    from torch.nn.grad import conv2d_input, conv2d_weight
+    c_acc = C_ACC if c_acc is None else c_acc
+    A, B = _conv64(a), _conv64(b)
+    if direction == "fprop":
+        ref = F.conv2d(A, B, None, stride, pad)
+        P = F.conv2d(A.abs(), B.abs(), None, stride, pad)
+        K = b.shape[1] * b.shape[2] * b.shape[3]
+    elif direction == "dgrad":
+        ref = conv2d_input(tuple(shape), B, A, stride, pad)
+        P = conv2d_input(tuple(shape), B.abs(), A.abs(), stride, pad)
+        K = b.shape[0] * b.shape[2] * b.shape[3]
+        if addend is not None:
+            ref = ref + addend.double()
+            P = P + addend.double().abs()
+            K += 1
+    elif direction == "wgrad":
+        ref = conv2d_weight(B, tuple(shape), A, stride, pad)
+        P = conv2d_weight(B.abs(), tuple(shape), A.abs(), stride, pad)
+        K = k_pixels
+    else:
+        raise ValueError(direction)
+    return ref, (c_acc * (K + 1) + reduce_depth) * U * P
+
+
+def conv_epilogue_depth(tiles_per_cta):
+    """Longest fp32 chain of the conv epilogue's per-CTA column sums: 32 rows per warp, one add per tile, 4 warps."""
+    return 32 + tiles_per_cta + 4
+
+
+SMS = 132                     # kNumSMs: the persistent and two-pass grids are sized for the H100 SXM
+
+
+def _ceil(a, b):
+    return -(-a // b)
+
+
+def conv_grid_tiles(num_m_tiles, num_n_tiles, stats=True):
+    """(grid, tiles per CTA) of conv_grid_size: the persistent conv grid, a multiple of the n-tiles with statistics."""
+    tiles = num_m_tiles * num_n_tiles
+    grid = min(tiles, SMS)
+    if stats and num_n_tiles > 1:
+        grid = max((grid // num_n_tiles) * num_n_tiles, num_n_tiles)
+    return grid, _ceil(tiles, grid)
+
+
+def bn_pick_tile(R, C):
+    """(cvb, ty, grid_x, grid_y) of batchnorm.cu's pick_tile: channel vectors per block, row lanes, channel tiles, row splits."""
+    cv = C // 8
+    cvb = min(cv, 8)
+    while 256 % cvb:
+        cvb -= 1
+    ty = 256 // cvb
+    grid_x = _ceil(cv, cvb)
+    return cvb, ty, grid_x, min(_ceil(4 * SMS, grid_x), max(R // (ty * 4), 1), 256)
+
+
+def bn_two_pass_depth(R, C, fused=False):
+    """Longest fp32 chain of the two-pass (and fused) stats / reduce kernels: rows per thread + row lanes + the finishing
+    block's strided split lanes + its combine of the lanes."""
+    cvb, ty, grid_x, S = bn_pick_tile(R, C)
+    if fused:
+        S = min(S, max(1, (2 * SMS) // grid_x))
+    lanes = max(1, 256 // (cvb * 8))
+    return _ceil(_ceil(R, S), ty) + ty + _ceil(S, lanes) + lanes
+
+
+def as_rows(t):
+    """A channels_last activation [N, C, H, W] as the [N*H*W, C] matrix the BatchNorm kernels see."""
+    return t.permute(0, 2, 3, 1).reshape(-1, t.shape[1])
+
+
+def unpack_mask(mask, C):
+    """uint8 [R, C/8] ReLU bitmask (bit i of byte v = channel 8 v + i) as bool [R, C]."""
+    bits = torch.arange(8, device=mask.device, dtype=torch.uint8)
+    return ((mask.reshape(-1, C // 8, 1) >> bits) & 1).bool().reshape(-1, C)
+
+
+def batchnorm_reference(x, gamma, beta, eps, depth, residual=None, relu=False, momentum=0.0, running_mean=None,
+                        running_var=None):
+    """fp64 training BatchNorm of x [R, C] (the stored input) and the bounds of the kernels' fp32 arithmetic, with `depth`
+    the longest chain of the per-channel sums: {"y": (ref, acc) [R, C] before output rounding, "mean", "rstd",
+    "running_mean", "running_var": (ref, bnd) [C]}."""
+    X = x.double()
+    R = X.shape[0]
+    g, b = gamma.double(), beta.double()
+    A1, A2 = X.abs().sum(0), (X * X).sum(0)
+    mean = X.sum(0) / R
+    E2 = A2 / R
+    var = torch.clamp(E2 - mean * mean, min=0.0)
+    d_mean = (depth * U * A1 + 3 * U * A1) / R
+    d_E2 = (depth * U * A2 + 3 * U * A2) / R
+    d_var = d_E2 + (2 * mean.abs() + d_mean) * d_mean + U * (mean.abs() + d_mean) ** 2 + U * (E2 + d_E2)
+    rs = 1.0 / torch.sqrt(var + eps)
+    v_lo = (torch.clamp(var - d_var, min=0.0) + eps) * (1 - U)
+    v_hi = (var + d_var + eps) * (1 + U)
+    d_rs = torch.maximum(v_lo.rsqrt() - rs, rs - v_hi.rsqrt()) + 4 * U * v_lo.rsqrt()
+    sc = g * rs
+    d_sc = g.abs() * d_rs + U * g.abs() * (rs + d_rs)
+    ms = mean * sc
+    d_ms = mean.abs() * d_sc + sc.abs() * d_mean + d_mean * d_sc + U * (mean.abs() + d_mean) * (sc.abs() + d_sc)
+    sh = b - ms
+    d_sh = d_ms + U * (b.abs() + ms.abs() + d_ms)
+    xs = X * sc
+    z = xs + sh
+    acc = X.abs() * d_sc + d_sh + U * (X.abs() * (sc.abs() + d_sc) + sh.abs() + d_sh)
+    if residual is not None:
+        Rr = residual.double()
+        z = z + Rr
+        acc = acc + U * (z.abs() + acc)
+    y = torch.relu(z) if relu else z
+    out = {"y": (y, acc), "mean": (mean, d_mean + FLOOR), "rstd": (rs, d_rs + FLOOR)}
+    if running_mean is not None:
+        m = float(torch.tensor(momentum, dtype=torch.float32))
+        rm0, rv0 = running_mean.double(), running_var.double()
+        f = R / (R - 1) if R > 1 else 1.0
+        rm = (1 - m) * rm0 + m * mean
+        rv = (1 - m) * rv0 + m * f * var
+        out["running_mean"] = (rm, m * d_mean + 4 * U * ((1 - m) * rm0.abs() + m * mean.abs()) + FLOOR)
+        out["running_var"] = (rv, m * f * d_var + 6 * U * ((1 - m) * rv0.abs() + m * f * var) + FLOOR)
+    return out
+
+
+def batchnorm_bwd_reference(dy, x, mask, gamma, mean, rstd, depth):
+    """fp64 BatchNorm backward of dy, x [R, C] at the kernel's own fp32 mean / rstd [C] and ReLU mask (bool [R, C] or None),
+    all taken as exact inputs, with `depth` the longest chain of the sums S1 = Σ dy*, S2 = Σ dy* x̂ (dy* = dy m), and the bounds
+    of the kernels' fp32 arithmetic before output rounding: {"dx": (ref, acc) [R, C], "dgamma": S2, "dbeta": S1 (ref, acc) [C]}."""
+    X, DY = x.double(), dy.double()
+    R = X.shape[0]
+    G = DY if mask is None else torch.where(mask, DY, 0.0)
+    m, s, gam = mean.double(), rstd.double(), gamma.double()
+    xh = (X - m) * s
+    gx = G * xh
+    S1, S2 = G.sum(0), gx.sum(0)
+    A1, A2 = G.abs().sum(0), gx.abs().sum(0)
+    e1 = depth * U * A1
+    e2 = (depth + 3) * U * A2
+    c1, c2 = S1 / R, S2 / R
+    d_c1, d_c2 = (e1 + 3 * U * A1) / R, (e2 + 3 * U * A2) / R
+    ka = gam * s
+    d_ka = U * ka.abs()
+    kr = (ka * s).abs()
+    d_kb = kr * d_c2 + 3 * U * kr * (c2.abs() + d_c2)
+    mr = (m * s).abs()
+    t = m * s * c2
+    d_t = mr * d_c2 + 3 * U * mr * (c2.abs() + d_c2)
+    inner = (c1 - t).abs()
+    d_inner = d_c1 + d_t + U * (c1.abs() + t.abs() + d_c1 + d_t)
+    d_kc = ka.abs() * d_inner + 2 * U * ka.abs() * (inner + d_inner)
+    kb, kc = -ka * s * c2, -ka * (c1 - t)
+    zx = kb * X + kc
+    d_z = X.abs() * d_kb + d_kc + U * ((kb * X).abs() + kc.abs() + X.abs() * d_kb + d_kc)
+    dx = ka * (G - c1 - xh * c2)
+    acc = G.abs() * d_ka + d_z + U * ((ka * G).abs() + zx.abs() + G.abs() * d_ka + d_z)
+    return {"dx": (dx, acc * (1 + 8 * U)), "dgamma": (S2, e2 + FLOOR), "dbeta": (S1, e1 + FLOOR)}
+
+
+def maxpool_reference(x):
+    """3x3 / stride 2 / pad 1 max pool of x [N, C, H, W]: (y, slot) with the first maximum in (ky, kx) order winning, exact."""
+    N, C, H, W = x.shape
+    OH, OW = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    xp = F.pad(x.double(), (1, 1, 1, 1), value=-math.inf)
+    best = torch.full((N, C, OH, OW), -math.inf, dtype=torch.float64, device=x.device)
+    slot = torch.zeros(N, C, OH, OW, dtype=torch.uint8, device=x.device)
+    for ky in range(3):
+        for kx in range(3):
+            v = xp[:, :, ky:ky + 2 * OH - 1:2, kx:kx + 2 * OW - 1:2]
+            take = v > best
+            best = torch.where(take, v, best)
+            slot = torch.where(take, ky * 3 + kx, slot).to(torch.uint8)
+    return best.to(x.dtype), slot
+
+
+def maxpool_bwd_reference(dy, slot, H, W):
+    """fp64 gradient of the max pool at its recorded window slots, and the bound of summing <= 4 dy per input in fp32."""
+    N, C, OH, OW = dy.shape
+    D = dy.double()
+    dx = torch.zeros(N, C, 2 * OH + 1, 2 * OW + 1, dtype=torch.float64, device=dy.device)
+    mag = torch.zeros_like(dx)
+    for ky in range(3):
+        for kx in range(3):
+            g = torch.where(slot == ky * 3 + kx, D, 0.0)
+            dx[:, :, ky:ky + 2 * OH:2, kx:kx + 2 * OW:2] += g
+            mag[:, :, ky:ky + 2 * OH:2, kx:kx + 2 * OW:2] += g.abs()
+    dx, mag = dx[:, :, 1:H + 1, 1:W + 1], mag[:, :, 1:H + 1, 1:W + 1]
+    return dx, 4 * U * mag
+
+
+def mse_reference(out, target, gscale, blocks, threads=256):
+    """fp64 MSE loss and gradient 2 (out - t) gscale / n of out, target (any shape) and the bounds of the kernel's fp32
+    arithmetic before output rounding: {"loss": (ref, bnd), "dout": (ref, acc)}.  The loss is a per-thread chain over a
+    grid-stride loop, two warp trees per block, then the last block's chain over the block partials."""
+    O, T = out.double(), target.double()
+    n = O.numel()
+    d = O - T
+    dout = 2.0 * gscale / n * d
+    stride = blocks * threads
+    depth = -(-n // stride) + 8 + 10 + -(-blocks // threads) + 10
+    loss = (d * d).sum() / n
+    return {"loss": (loss, (depth + 6) * U * loss + FLOOR), "dout": (dout, 6 * U * dout.abs())}
