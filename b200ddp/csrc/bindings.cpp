@@ -1515,4 +1515,53 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                       (int)dst.size(1), (int)src.size(2), (int)src.size(3), mean.data_ptr<float>(), inv_std.data_ptr<float>(),
                                       (float)in_scale, cur_stream());
   });
+
+  // ---- Vision Transformer patch embedding (vit.cu): images as documents of one token stream ------------------------------
+  // The submodule _C.vit holds these entry points; they follow the same argument contract (tests/test_vit_bindings_cpu.py).
+  py::module_ vit = m.def_submodule("vit", "Vision Transformer patch embedding (vit.cu)");
+  vit.def("patchify", [](at::Tensor images, int64_t patch, int64_t tokens) {
+    Args args("patchify");
+    args("images", images, {kBF16}, {kAny, kAny, kAny, kAny}, kStrided, 16);
+    const bool cl = !images.is_contiguous();
+    args.expect(!cl || images.is_contiguous(at::MemoryFormat::ChannelsLast), "images", "contiguous or channels_last", images);
+    const int64_t B = images.size(0), C = images.size(1), H = images.size(2), W = images.size(3);
+    if (patch < 8 || patch % 8 || H % patch || W % patch)
+      args.fail("patch", "a multiple of 8 that divides the image's height and width", std::to_string(patch) + " for " + sizes_str(images.sizes()));
+    const int64_t per = (H / patch) * (W / patch) + 1;
+    if (tokens < B * per) args.fail("tokens", "at least batch * (patches + 1) = " + std::to_string(B * per), std::to_string(tokens));
+    args.device();
+    at::Tensor out = at::empty({tokens, C * patch * patch}, images.options().memory_format(at::MemoryFormat::Contiguous));
+    launch_patchify(images.data_ptr(), cl, (int)B, (int)C, (int)H, (int)W, (int)patch, (int)tokens, out.data_ptr(), cur_stream());
+    return out;
+  }, py::arg("images"), py::arg("patch"), py::arg("tokens"));
+  vit.def("patch_assemble", [](at::Tensor y, at::Tensor class_token, at::Tensor pos_embedding, int64_t batch) {
+    Args args("patch_assemble");
+    args("y", y, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t T = y.size(0), D = y.size(1);
+    if (D % 8) args.fail("y", "bf16 [T, D] with D % 8 == 0", describe(y));
+    args("class_token", class_token, {kBF16}, numel(D), kContiguous, 16)("pos_embedding", pos_embedding, {kBF16}, last_dim(D), kContiguous, 16);
+    const int64_t per = pos_embedding.numel() / D;
+    if (per < 1 || batch < 0 || batch * per > T)
+      args.fail("batch", "at most T / tokens_per_image = " + std::to_string(T / std::max<int64_t>(per, 1)), std::to_string(batch));
+    args.device();
+    at::Tensor out = at::empty_like(y);
+    launch_patch_assemble(y.data_ptr(), class_token.data_ptr(), pos_embedding.data_ptr(), (int)batch, (int)per, (int)D, (int)T, out.data_ptr(),
+                          cur_stream());
+    return out;
+  }, py::arg("y"), py::arg("class_token"), py::arg("pos_embedding"), py::arg("batch"));
+  vit.def("patch_embed_bwd", [](at::Tensor dy, int64_t batch, int64_t tokens_per_image) {
+    Args args("patch_embed_bwd");
+    args("dy", dy, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t T = dy.size(0), D = dy.size(1);
+    if (D % 8) args.fail("dy", "bf16 [T, D] with D % 8 == 0", describe(dy));
+    if (tokens_per_image < 1 || batch < 0 || batch * tokens_per_image > T)
+      args.fail("batch", "batch * tokens_per_image <= T = " + std::to_string(T), std::to_string(batch) + " * " + std::to_string(tokens_per_image));
+    args.device();
+    at::Tensor dpatch = at::empty_like(dy);
+    at::Tensor dpos = at::empty({tokens_per_image, D}, dy.options());
+    at::Tensor dcls = at::empty({D}, dy.options());
+    launch_patch_embed_bwd(dy.data_ptr(), (int)batch, (int)tokens_per_image, (int)D, (int)T, dpatch.data_ptr(), dpos.data_ptr(), dcls.data_ptr(),
+                           cur_stream());
+    return std::make_tuple(dpatch, dpos, dcls);
+  }, py::arg("dy"), py::arg("batch"), py::arg("tokens_per_image"));
 }

@@ -247,4 +247,14 @@ void launch_normalize_to_channels_last(const void* src, DType src_dt, void* dst,
                                        int h, int w, const float* mean, const float* inv_std, float in_scale,
                                        cudaStream_t s);
 
+// ---------------- Vision Transformer patch embedding (vit.cu), bf16 --------------------------------
+// Token stream of T rows (T >= B (N + 1), N = (H / p) (W / p) patches, per = N + 1): image b owns rows [b per, (b + 1) per),
+// its class token first; rows past B per are padding.  p % 8 == 0, H % p == W % p == 0, D % 8 == 0, 16-byte aligned rows.
+// out [T, C p p] = the patches in token order, k = (c, ky, kx); zero at class and padding rows
+void launch_patchify(const void* img, bool channels_last, int B, int C, int H, int W, int p, int T, void* out, cudaStream_t s);
+// out [T, D] = cls + pos[0] at class rows, y + pos[j] at patch rows (fp32 add), 0 at padding rows
+void launch_patch_assemble(const void* y, const void* cls, const void* pos, int B, int per, int D, int T, void* out, cudaStream_t s);
+// dpatch [T, D] = dy at patch rows, 0 elsewhere; dpos [per, D] = fixed-order fp32 sums over the B images; dcls [D] = dpos[0]
+void launch_patch_embed_bwd(const void* dy, int B, int per, int D, int T, void* dpatch, void* dpos, void* dcls, cudaStream_t s);
+
 }  // namespace b200

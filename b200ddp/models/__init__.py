@@ -12,6 +12,7 @@ from .llama import (GRANITE_3_0_1B_A400M, QWEN2_5_1_5B, QWEN3_0_6B, SMOLLM_135M,
                     smollm_135m, qwen2_5_1_5b, qwen3_0_6b, granite_3_0_1b_a400m)
 from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, ModernBertModel, ModernBertForMaskedLM, modernbert_base,
                          modernbert_large)
+from .vit import VIT_B_16, VIT_B_32, VIT_L_16, ViTConfig, VisionTransformer, vit_b_16, vit_b_32, vit_l_16
 
 
 @dataclass(frozen=True)
@@ -34,6 +35,9 @@ MODEL_REGISTRY = {
     "foo": ModelEntry(FooModel, "foo"),
     "resnet50": ModelEntry(resnet50, "image"),
     "resnet152": ModelEntry(resnet152, "image"),
+    "vit-b-16": ModelEntry(vit_b_16, "image"),
+    "vit-b-32": ModelEntry(vit_b_32, "image"),
+    "vit-l-16": ModelEntry(vit_l_16, "image"),
     "bert-base": ModelEntry(bert_base, "encoder", BERT_BASE, start_id=101, fp8=True),                 # [CLS]
     "modernbert-base": ModelEntry(modernbert_base, "encoder", MODERNBERT_BASE, start_id=50281, fp8=True),   # [CLS]
     "modernbert-large": ModelEntry(modernbert_large, "encoder", MODERNBERT_LARGE, start_id=50281, fp8=True),
@@ -59,4 +63,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

@@ -1364,3 +1364,106 @@ def layer_norm(x: torch.Tensor, gamma: torch.Tensor, beta: Optional[torch.Tensor
     if x.is_cuda and x.dtype in (torch.float32, torch.bfloat16) and gamma.dtype == x.dtype and x.shape[-1] * 8 <= 96 * 1024:
         return _LayerNormFused.apply(x, gamma, gamma.new_zeros(gamma.shape) if beta is None else beta, eps)
     return F.layer_norm(x, (x.shape[-1],), gamma, beta, eps)
+
+
+# ------------------------------------------------------------------------------------------------
+# Vision Transformer patch embedding (csrc/vit.cu): the images of a batch as documents of one token stream
+# ------------------------------------------------------------------------------------------------
+def image_token_rows(batch: int, tokens_per_image: int) -> int:
+    """Rows of the token stream of `batch` images of `tokens_per_image` tokens each: their count rounded up to a multiple
+    of 128, the row multiple of the attention kernels."""
+    return -(-batch * tokens_per_image // ATTENTION_SEQ_MULTIPLE) * ATTENTION_SEQ_MULTIPLE
+
+
+def image_token_bounds(batch: int, tokens_per_image: int, device=None) -> torch.Tensor:
+    """Document bounds int32 [1, T, 2] (T = ``image_token_rows``) of `batch` images laid out one after another in one token
+    stream: the rows of image b, [b n, (b + 1) n) with n = tokens_per_image, hold (b n, (b + 1) n); the padding rows past
+    batch n hold (0, 0).  ``packed_attention(qkv.view(1, T, 3 * hidden), bounds, heads)`` then attends within each image.
+    Torch ops on static shapes: no host synchronisation (CUDA-graph safe)."""
+    if batch < 1 or tokens_per_image < 1:
+        raise ValueError(f"image_token_bounds needs batch >= 1 and tokens_per_image >= 1, got {batch}, {tokens_per_image}")
+    T = image_token_rows(batch, tokens_per_image)
+    t = torch.arange(T, device=device, dtype=torch.int32)
+    start = t - t % tokens_per_image
+    real = t < batch * tokens_per_image
+    zero = torch.zeros((), device=device, dtype=torch.int32)
+    return torch.stack([torch.where(real, start, zero), torch.where(real, start + tokens_per_image, zero)], -1).view(1, T, 2)
+
+
+def patch_embed_reference(images: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], class_token: torch.Tensor,
+                          pos_embedding: torch.Tensor) -> torch.Tensor:
+    """torchvision's ViT input stage (``conv_proj``, flatten, class token, position embedding) laid out as ``patch_embed``'s
+    token stream [T, D]: image b's class token at row b (N + 1), its N patches after it, zero rows past B (N + 1).
+    Differentiable."""
+    B = images.shape[0]
+    D, p = weight.shape[0], weight.shape[-1]
+    x = F.conv2d(images, weight, bias, stride=p).flatten(2).transpose(1, 2)
+    x = torch.cat([class_token.expand(B, -1, -1), x], 1) + pos_embedding
+    per = x.shape[1]
+    return F.pad(x.reshape(B * per, D), (0, 0, 0, image_token_rows(B, per) - B * per))
+
+
+def _patch_embed_check(images, weight, bias, class_token, pos_embedding) -> None:
+    if images.dim() != 4 or weight.dim() != 4 or weight.shape[1] != images.shape[1] or weight.shape[2] != weight.shape[3]:
+        raise ValueError(f"patch_embed needs images [B, C, H, W] and a square weight [D, C, p, p], got {tuple(images.shape)} "
+                         f"and {tuple(weight.shape)}")
+    B, C, H, W = images.shape
+    D, p = weight.shape[0], weight.shape[-1]
+    if p % 8 or H % p or W % p or D % 8:
+        raise ValueError(f"patch_embed on CUDA needs a patch size p % 8 == 0 that divides H and W, and D % 8 == 0, got p = {p}, "
+                         f"image {H}x{W}, D = {D}")
+    per = (H // p) * (W // p) + 1
+    if class_token.numel() != D or pos_embedding.numel() != per * D or (bias is not None and bias.numel() != D):
+        raise ValueError(f"patch_embed needs class_token of {D} elements, pos_embedding [1, {per}, {D}] and bias [{D}], got "
+                         f"{tuple(class_token.shape)}, {tuple(pos_embedding.shape)}, {None if bias is None else tuple(bias.shape)}")
+    ts = [images, weight, class_token, pos_embedding] + ([bias] if bias is not None else [])
+    if any(t.dtype != torch.bfloat16 for t in ts):
+        raise ValueError(f"patch_embed on CUDA needs bf16 tensors, got {[t.dtype for t in ts]}")
+    if not (images.is_contiguous() or images.is_contiguous(memory_format=torch.channels_last)):
+        raise ValueError("patch_embed on CUDA needs contiguous or channels_last images")
+    if images.requires_grad and torch.is_grad_enabled():
+        raise ValueError("patch_embed gives the images no gradient; pass images that do not require one")
+
+
+class _PatchAssemble(torch.autograd.Function):
+    """GEMM output [T, D] -> tokens: class token + pos[0], patch + pos[1 + i], zero padding rows (csrc/vit.cu).  Backward is
+    one launch: the patch rows' gradient (zero at class and padding rows, so the linear's weight and bias gradients sum
+    patch rows only) and d pos / d class_token as fixed-order fp32 sums over the images."""
+
+    @staticmethod
+    def forward(ctx, y, class_token, pos_embedding, batch):
+        ctx.batch, ctx.per = batch, pos_embedding.numel() // y.shape[1]
+        ctx.shapes = class_token.shape, pos_embedding.shape
+        return _C().vit.patch_assemble(y, class_token.contiguous(), pos_embedding.contiguous(), batch)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dy = dy.contiguous()
+        if dy.data_ptr() % 16:                                    # the kernel reads dy in 16-byte vectors
+            dy = dy.clone()
+        dpatch, dpos, dcls = _C().vit.patch_embed_bwd(dy, ctx.batch, ctx.per)
+        return dpatch, dcls.view(ctx.shapes[0]), dpos.view(ctx.shapes[1]), None
+
+
+def patch_embed(images: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], class_token: torch.Tensor,
+                pos_embedding: torch.Tensor) -> torch.Tensor:
+    """A Vision Transformer's input stage as one token stream: images [B, C, H, W], the patch convolution's weight
+    [D, C, p, p] (stride p) and bias [D], class_token [1, 1, D] and pos_embedding [1, N + 1, D] (N = H W / p²; torchvision's
+    ``conv_proj``, ``class_token`` and ``encoder.pos_embedding``).  Returns tokens [T, D], T = ``image_token_rows(B, N + 1)``:
+    image b's class token (class_token + pos[0]) at row b (N + 1), its patches (patch + pos[1 + i], raster order) after it,
+    exact zeros in the padding rows past B (N + 1); ``image_token_bounds(B, N + 1)`` are its attention bounds.
+
+    On CUDA (bf16, contiguous or channels_last images, p % 8 == 0, D % 8 == 0, else ``ValueError``): one kernel writes the
+    patch matrix [T, C p²] in token order (zero class and padding rows) in the flattened weight's K order, the wgmma
+    ``linear`` runs on all T rows, and one kernel adds the class token and the position embedding.  The gradients of the
+    weight, bias, class token and position embedding do not depend on the output gradient at padding rows; the images get
+    none.  On CPU: ``patch_embed_reference``."""
+    if not images.is_cuda:
+        return patch_embed_reference(images, weight, bias, class_token, pos_embedding)
+    _patch_embed_check(images, weight, bias, class_token, pos_embedding)
+    B, _, H, W = images.shape
+    D, p = weight.shape[0], weight.shape[-1]
+    per = (H // p) * (W // p) + 1
+    patches = _C().vit.patchify(images, p, image_token_rows(B, per))
+    y = linear(patches, weight.reshape(D, -1), bias)               # a channels_last weight is copied into (c, ky, kx) order
+    return _PatchAssemble.apply(y, class_token, pos_embedding, B)

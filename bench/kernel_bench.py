@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -859,6 +859,60 @@ def main():
             record(f"moe {routing} combine bwd", timeit(lambda: C.moe_combine_bwd(dout, y, fwd, gates), args.iters),
                    bytes_=R * H * 2 * 2 + cap * H * 2 + R * (4 + 2 + 4), note="dout read once per routed row")
             del xp, gu, h, y, dy, dgu
+
+    if "vit" in want:
+        # ViT-B/16 at batch 64: the patch embedding (patchify + wgmma linear + assembly, and its backward) against torchvision's
+        # conv_proj + flatten + cat + position add in bf16, and attention on the image-as-document stream against SDPA flash
+        # per image on [64, 12, 197, 64]
+        import torch.nn.functional as F
+        print(f"vit kernels on {card()}", flush=True)
+        B, p, D, H, d, per = 64, 16, 768, 12, 64, 197
+        T = Fn.image_token_rows(B, per)
+        g = torch.Generator(device="cuda").manual_seed(4)
+        images = torch.randn(B, 3, 224, 224, device=dev, generator=g).to(torch.bfloat16)
+        w = (torch.randn(D, 3, p, p, device=dev, generator=g) / 28).to(torch.bfloat16).requires_grad_(True)
+        bias, cls, pos = (torch.randn(*s, device=dev, generator=g).to(torch.bfloat16).requires_grad_(True)
+                          for s in ((D,), (1, 1, D), (1, per, D)))
+        K = 3 * p * p
+
+        def tv_embed():
+            x = F.conv2d(images, w, bias, stride=p).flatten(2).transpose(1, 2)
+            return torch.cat([cls.expand(B, -1, -1), x], 1) + pos
+        # bytes: image read, patch matrix write + read, GEMM output write + read, tokens write (weights are small)
+        fwd_bytes = 2 * (B * 3 * 224 * 224 + 2 * T * K + 3 * T * D)
+        with torch.no_grad():
+            record(f"vit patch_embed fwd B{B} p{p}", timeit(lambda: Fn.patch_embed(images, w, bias, cls, pos), args.iters),
+                   bytes_=fwd_bytes, lib_ms=timeit(tv_embed, args.iters), note="lib = conv2d + flatten + cat + pos add")
+        y = Fn.patch_embed(images, w, bias, cls, pos)
+        dy = torch.randn(T, D, device=dev, generator=g).to(torch.bfloat16)
+        yl = tv_embed()
+        dyl = dy[:B * per].view(B, per, D)
+        # bytes: dy read, patch-row gradient write + read, patch matrix read (the wgrad GEMM), d pos write
+        bwd_bytes = 2 * (3 * T * D + T * K + per * D)
+        record(f"vit patch_embed bwd B{B} p{p}", timeit(lambda: torch.autograd.grad(y, (w, bias, cls, pos), dy, retain_graph=True),
+                                                          args.iters),
+               bytes_=bwd_bytes, lib_ms=timeit(lambda: torch.autograd.grad(yl, (w, bias, cls, pos), dyl, retain_graph=True), args.iters),
+               note="lib = the same through conv2d's backward")
+        bounds = Fn.image_token_bounds(B, per, dev)
+        qkv = torch.randn(T, 3 * H * d, device=dev, generator=g).to(torch.bfloat16)
+        dout = torch.randn(T, H * d, device=dev, generator=g).to(torch.bfloat16)
+        fwd_flops = 4.0 * d * H * B * per * per                   # the visible pairs only
+        x = qkv[:B * per].view(B, per, -1).detach().clone().requires_grad_(True)
+        q, k, v = (t.reshape(B, per, H, d).transpose(1, 2) for t in x.split(H * d, dim=-1))
+
+        def sdpa():
+            return F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, per, H * d)
+        with torch.nn.attention.sdpa_kernel(torch.nn.attention.SDPBackend.FLASH_ATTENTION):
+            lib = timeit(lambda: sdpa().detach(), args.iters)
+            record(f"vit attention fwd B{B} {per} tokens/image", timeit(lambda: C.packed_attention_fwd(qkv, bounds, H), args.iters),
+                   flops=fwd_flops, lib_ms=lib, note=f"stream of {T} rows; lib = SDPA flash [{B}, {H}, {per}, {d}] + output transpose")
+            o, lse = C.packed_attention_fwd(qkv, bounds, H)
+            ya = sdpa()
+            lib = timeit(lambda: torch.autograd.grad(ya, x, dout[:B * per].view(B, per, -1), retain_graph=True), args.iters)
+            record(f"vit attention bwd B{B} {per} tokens/image",
+                   timeit(lambda: C.packed_attention_bwd(dout, qkv, o, lse, bounds, H), args.iters), flops=2.5 * fwd_flops,
+                   lib_ms=lib, note="lib = SDPA flash backward into qkv")
+        del x, q, k, v, ya, y, yl
 
     if "mse" in want:
         n = 64 * 1024 * 1024
