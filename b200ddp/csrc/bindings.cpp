@@ -170,6 +170,9 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
+// the type behind the _C.clip namespace of static entry points
+struct ClipNamespace {};
+
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
   CommCtx c;
   c.base = a.base();
@@ -712,7 +715,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     args("pre", pre, {kF32, kBF16}, min_numel(0));
     args.device();
     at::Tensor out = at::empty_like(pre);
-    launch_gelu(pre.data_ptr(), nullptr, out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), false, cur_stream(), tanh);
+    launch_gelu(pre.data_ptr(), nullptr, out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), false, cur_stream(),
+                tanh ? GeluForm::kTanh : GeluForm::kErf);
     return out;
   }, py::arg("pre"), py::arg("tanh") = false);
   m.def("gelu_bwd", [](at::Tensor dy, at::Tensor pre, bool tanh) {
@@ -720,7 +724,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     args("pre", pre, {kF32, kBF16}, min_numel(0))("dy", dy, {pre.scalar_type()}, numel(pre.numel()));
     args.device();
     at::Tensor out = at::empty_like(pre);
-    launch_gelu(pre.data_ptr(), dy.data_ptr(), out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), true, cur_stream(), tanh);
+    launch_gelu(pre.data_ptr(), dy.data_ptr(), out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), true, cur_stream(),
+                tanh ? GeluForm::kTanh : GeluForm::kErf);
     return out;
   }, py::arg("dy"), py::arg("pre"), py::arg("tanh") = false);
 
@@ -1564,4 +1569,68 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                            cur_stream());
     return std::make_tuple(dpatch, dpos, dcls);
   }, py::arg("dy"), py::arg("batch"), py::arg("tokens_per_image"));
+
+  // ---- CLIP (clip.cu, and QuickGELU in loss.cu): the contrastive loss over the global batch ----------------------------
+  // _C.clip is a namespace of static entry points (a class that is never instantiated), not a submodule: the argument-contract
+  // tests of the top-level functions and of the vit submodule each list exactly their own bindings, and these have their
+  // rows, and their own check that every one has a row, in tests/test_clip_bindings_cpu.py.  Same argument contract.
+  py::class_<ClipNamespace> clip(m, "clip", "CLIP contrastive loss and QuickGELU (clip.cu, loss.cu)");
+  clip.def_static("quick_gelu_fwd", [](at::Tensor pre) {
+    Args args("quick_gelu_fwd");
+    args("pre", pre, {kF32, kBF16}, min_numel(0));
+    args.device();
+    at::Tensor out = at::empty_like(pre);
+    launch_gelu(pre.data_ptr(), nullptr, out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), false, cur_stream(), GeluForm::kQuick);
+    return out;
+  }, py::arg("pre"));
+  clip.def_static("quick_gelu_bwd", [](at::Tensor dy, at::Tensor pre) {
+    Args args("quick_gelu_bwd");
+    args("pre", pre, {kF32, kBF16}, min_numel(0))("dy", dy, {pre.scalar_type()}, numel(pre.numel()));
+    args.device();
+    at::Tensor out = at::empty_like(pre);
+    launch_gelu(pre.data_ptr(), dy.data_ptr(), out.data_ptr(), dtype_of(pre), (size_t)pre.numel(), true, cur_stream(), GeluForm::kQuick);
+    return out;
+  }, py::arg("dy"), py::arg("pre"));
+  clip.def_static("l2norm_fwd", [](at::Tensor x) {
+    Args args("l2norm_fwd");
+    args("x", x, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t B = x.size(0), D = x.size(1);
+    if (B < 1 || D < 8 || D % 8) args.fail("x", "bf16 [B, D] with B >= 1 and D % 8 == 0", describe(x));
+    args.device();
+    at::Tensor u = at::empty_like(x);
+    at::Tensor rnorm = at::empty({B}, x.options().dtype(kF32));
+    launch_l2norm_fwd(x.data_ptr(), (int)B, (int)D, u.data_ptr(), rnorm.data_ptr<float>(), cur_stream());
+    return std::make_tuple(u, rnorm);
+  }, py::arg("x"));
+  clip.def_static("l2norm_bwd", [](at::Tensor du, at::Tensor x, at::Tensor rnorm) {
+    Args args("l2norm_bwd");
+    args("x", x, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t B = x.size(0), D = x.size(1);
+    if (B < 1 || D < 8 || D % 8) args.fail("x", "bf16 [B, D] with B >= 1 and D % 8 == 0", describe(x));
+    args("du", du, {kBF16}, {B, D}, kContiguous, 16)("rnorm", rnorm, {kF32}, {B});
+    args.device();
+    at::Tensor dx = at::empty_like(x);
+    launch_l2norm_bwd(du.data_ptr(), x.data_ptr(), rnorm.data_ptr<float>(), (int)B, (int)D, dx.data_ptr(), cur_stream());
+    return dx;
+  }, py::arg("du"), py::arg("x"), py::arg("rnorm"));
+  // (loss fp32 [], dscale fp32 [], dz_img bf16 [B, N], dz_txt bf16 [B, N])
+  clip.def_static("contrastive_xent", [](at::Tensor z_img, at::Tensor z_txt, at::Tensor logit_scale, int64_t label_offset) {
+    Args args("contrastive_xent");
+    args("z_img", z_img, {kF32}, {kAny, kAny});
+    const int64_t B = z_img.size(0), N = z_img.size(1);
+    if (B < 1 || N < B) args.fail("z_img", "fp32 [B, N] with 1 <= B <= N", describe(z_img));
+    args("z_txt", z_txt, {kF32}, {B, N})("logit_scale", logit_scale, {kF32}, numel(1));
+    if (label_offset < 0 || label_offset + B > N)
+      args.fail("label_offset", "in [0, N - B] = [0, " + std::to_string(N - B) + "]", std::to_string(label_offset));
+    args.device();
+    at::Tensor dz_img = at::empty({B, N}, z_img.options().dtype(kBF16));
+    at::Tensor dz_txt = at::empty({B, N}, z_img.options().dtype(kBF16));
+    at::Tensor partials = at::empty({4 * B}, z_img.options());
+    at::Tensor loss = at::empty({}, z_img.options());
+    at::Tensor dscale = at::empty({}, z_img.options());
+    launch_contrastive_xent(z_img.data_ptr<float>(), z_txt.data_ptr<float>(), logit_scale.data_ptr<float>(), (int)B, (int)N, (int)label_offset,
+                            dz_img.data_ptr(), dz_txt.data_ptr(), partials.data_ptr<float>(), loss.data_ptr<float>(), dscale.data_ptr<float>(),
+                            cur_stream());
+    return std::make_tuple(loss, dscale, dz_img, dz_txt);
+  }, py::arg("z_img"), py::arg("z_txt"), py::arg("logit_scale"), py::arg("label_offset"));
 }

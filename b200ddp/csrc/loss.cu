@@ -507,9 +507,9 @@ void launch_column_sum(const void* d, int rows, int cols, const int* bound, floa
 }  // namespace b200
 
 // ---------------------------------------------------------------------------------------------------------
-// GELU forward and backward as single vectorised passes, erf form (BERT) or tanh approximation (GPT-2).  The stock
-// autograd formula for the backward (cast to fp32, erf, exp, three multiplies, cast back) is ~8 launches over a
-// [tokens, 3072] tensor per BERT layer.
+// GELU forward and backward as single vectorised passes, erf form (BERT), tanh approximation (GPT-2) or QuickGELU
+// (CLIP).  The stock autograd formula for the backward (cast to fp32, erf, exp, three multiplies, cast back) is ~8 launches
+// over a [tokens, 3072] tensor per BERT layer.
 namespace b200 {
 namespace {
 
@@ -530,13 +530,21 @@ __device__ __forceinline__ float gelu_tanh_grad_f(float x) {
   const float t = tanhf(kSqrt2OverPi * (x + kGeluTanhC * x * x * x));
   return 0.5f * (1.f + t) + 0.5f * x * (1.f - t * t) * kSqrt2OverPi * (1.f + 3.f * kGeluTanhC * x * x);
 }
-template <bool BWD, bool TANH>
+// QuickGELU: x sigmoid(1.702 x); its derivative s + 1.702 x s (1 - s) with s = sigmoid(1.702 x)
+constexpr float kQuickGeluC = 1.702f;
+__device__ __forceinline__ float quick_gelu_f(float x) { return x / (1.f + __expf(-kQuickGeluC * x)); }
+__device__ __forceinline__ float quick_gelu_grad_f(float x) {
+  const float s = 1.f / (1.f + __expf(-kQuickGeluC * x));
+  return s + kQuickGeluC * x * s * (1.f - s);
+}
+template <bool BWD, GeluForm FORM>
 __device__ __forceinline__ float gelu_op(float x, float g) {
-  if constexpr (TANH) return BWD ? g * gelu_tanh_grad_f(x) : gelu_tanh_f(x);
+  if constexpr (FORM == GeluForm::kTanh) return BWD ? g * gelu_tanh_grad_f(x) : gelu_tanh_f(x);
+  else if constexpr (FORM == GeluForm::kQuick) return BWD ? g * quick_gelu_grad_f(x) : quick_gelu_f(x);
   else return BWD ? g * gelu_grad_f(x) : gelu_f(x);
 }
 
-template <typename T, bool BWD, bool TANH>
+template <typename T, bool BWD, GeluForm FORM>
 __global__ void __launch_bounds__(kLossThreads) gelu_kernel(const T* __restrict__ pre, const T* __restrict__ dy, T* __restrict__ out, size_t n) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -549,37 +557,38 @@ __global__ void __launch_bounds__(kLossThreads) gelu_kernel(const T* __restrict_
       load8<T>(pre + v * 8, a);
       if (BWD) load8<T>(dy + v * 8, g);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) a[i] = gelu_op<BWD, TANH>(a[i], g[i]);
+      for (int i = 0; i < 8; ++i) a[i] = gelu_op<BWD, FORM>(a[i], g[i]);
       store8<T>(out + v * 8, a);
     }
     done = nvec * 8;
   }
   for (size_t i = done + tid; i < n; i += stride) {
     const float x = to_f32<T>(pre[i]);
-    out[i] = from_f32<T>(gelu_op<BWD, TANH>(x, BWD ? to_f32<T>(dy[i]) : 0.f));
+    out[i] = from_f32<T>(gelu_op<BWD, FORM>(x, BWD ? to_f32<T>(dy[i]) : 0.f));
   }
 }
 
 }  // namespace
 
-template <bool TANH>
+template <GeluForm FORM>
 void gelu_dispatch(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, int blocks, cudaStream_t s) {
   if (dt == DType::BF16) {
-    if (backward) gelu_kernel<__nv_bfloat16, true, TANH><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, (const __nv_bfloat16*)dy, (__nv_bfloat16*)out, n);
-    else gelu_kernel<__nv_bfloat16, false, TANH><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, nullptr, (__nv_bfloat16*)out, n);
+    if (backward) gelu_kernel<__nv_bfloat16, true, FORM><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, (const __nv_bfloat16*)dy, (__nv_bfloat16*)out, n);
+    else gelu_kernel<__nv_bfloat16, false, FORM><<<blocks, kLossThreads, 0, s>>>((const __nv_bfloat16*)pre, nullptr, (__nv_bfloat16*)out, n);
   } else {
-    if (backward) gelu_kernel<float, true, TANH><<<blocks, kLossThreads, 0, s>>>((const float*)pre, (const float*)dy, (float*)out, n);
-    else gelu_kernel<float, false, TANH><<<blocks, kLossThreads, 0, s>>>((const float*)pre, nullptr, (float*)out, n);
+    if (backward) gelu_kernel<float, true, FORM><<<blocks, kLossThreads, 0, s>>>((const float*)pre, (const float*)dy, (float*)out, n);
+    else gelu_kernel<float, false, FORM><<<blocks, kLossThreads, 0, s>>>((const float*)pre, nullptr, (float*)out, n);
   }
 }
 
-void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s, bool tanh) {
+void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s, GeluForm form) {
   size_t b = (n / 8 + kLossThreads - 1) / kLossThreads;
   if (b < 1) b = 1;
   if (b > (size_t)16 * kNumSMs) b = (size_t)16 * kNumSMs;
   const int blocks = (int)b;
-  if (tanh) gelu_dispatch<true>(pre, dy, out, dt, n, backward, blocks, s);
-  else gelu_dispatch<false>(pre, dy, out, dt, n, backward, blocks, s);
+  if (form == GeluForm::kTanh) gelu_dispatch<GeluForm::kTanh>(pre, dy, out, dt, n, backward, blocks, s);
+  else if (form == GeluForm::kQuick) gelu_dispatch<GeluForm::kQuick>(pre, dy, out, dt, n, backward, blocks, s);
+  else gelu_dispatch<GeluForm::kErf>(pre, dy, out, dt, n, backward, blocks, s);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 

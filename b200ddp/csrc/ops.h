@@ -83,9 +83,11 @@ void launch_scatter_rows(const void* dy, const int* index, const int* count, int
 size_t column_sum_workspace(int rows, int cols);
 void launch_column_sum(const void* d, int rows, int cols, const int* bound, float* workspace, void* out, cudaStream_t s);
 
-// GELU forward: out = gelu(pre); backward: out = dy * gelu'(pre).  One vectorised pass each (loss.cu).  The erf form, or
-// with `tanh` the tanh approximation 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3))) (GPT-2's MLP).
-void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s, bool tanh = false);
+// GELU forward: out = gelu(pre); backward: out = dy * gelu'(pre).  One vectorised pass each (loss.cu).  The erf form, the
+// tanh approximation 0.5 x (1 + tanh(sqrt(2 / pi) (x + 0.044715 x^3))) (GPT-2's MLP) or QuickGELU x sigmoid(1.702 x) (CLIP's).
+enum class GeluForm { kErf, kTanh, kQuick };
+void launch_gelu(const void* pre, const void* dy, void* out, DType dt, size_t n, bool backward, cudaStream_t s,
+                 GeluForm form = GeluForm::kErf);
 
 // SwiGLU: forward out[M, I] = silu(gate) * up from gate_up bf16 [M, 2I] (gate | up); backward out[M, 2I] = d[gate | up]
 // from dy [M, I].  I % 8 == 0, 16-byte aligned tensors (loss.cu).
@@ -256,5 +258,16 @@ void launch_patchify(const void* img, bool channels_last, int B, int C, int H, i
 void launch_patch_assemble(const void* y, const void* cls, const void* pos, int B, int per, int D, int T, void* out, cudaStream_t s);
 // dpatch [T, D] = dy at patch rows, 0 elsewhere; dpos [per, D] = fixed-order fp32 sums over the B images; dcls [D] = dpos[0]
 void launch_patch_embed_bwd(const void* dy, int B, int per, int D, int T, void* dpatch, void* dpos, void* dcls, cudaStream_t s);
+
+// ---------------- CLIP contrastive loss (clip.cu) ---------------------------------------------------
+// u bf16 [B, D] = x / ||x|| per row (fp32, one rounding), rnorm fp32 [B] = 1 / ||x||; D % 8 == 0, 16-byte aligned rows
+void launch_l2norm_fwd(const void* x, int B, int D, void* u, float* rnorm, cudaStream_t s);
+// dx bf16 [B, D] = rnorm (du - u <u, du>) with u = x rnorm in fp32
+void launch_l2norm_bwd(const void* du, const void* x, const float* rnorm, int B, int D, void* dx, cudaStream_t s);
+// z_img, z_txt fp32 [B, N] (unscaled similarities), logit_scale fp32 [1], labels offset + r (0 <= offset, offset + B <= N):
+// dz_* bf16 [B, N] = s (softmax(s z) - onehot) / (2B), loss fp32 [1] = mean of the 2B cross-entropies, dscale fp32 [1] =
+// d loss / d logit_scale; row_partials fp32 [4B] is scratch.  Two launches, fixed-order sums.
+void launch_contrastive_xent(const float* z_img, const float* z_txt, const float* logit_scale, int B, int N, int offset, void* dz_img,
+                             void* dz_txt, float* row_partials, float* loss, float* dscale, cudaStream_t s);
 
 }  // namespace b200

@@ -68,6 +68,46 @@ class SyntheticImageNet(Dataset):
         torch.index_select(self.Y, 0, indices, out=outs[1])
 
 
+class SyntheticImageText(Dataset):
+    """Image-caption pairs for CLIP: ``X`` images fp32 [3, size, size] as in ``SyntheticImageNet`` and ``Y`` caption ids
+    int64 [context] (seeded).  A caption is ``SOT_ID``, tokens from [1, SOT_ID), ``EOT_ID``, then pad 0, with total lengths
+    (SOT and EOT included) uniform in [8, context].  ``samples`` is rounded down to a multiple of ``batch`` (at least one
+    batch): with ``batch`` the global batch, every batch holds whole pairs and no partial batch reaches the loss."""
+
+    SOT_ID = 49406                 # <|startoftext|> in CLIP's vocabulary
+    EOT_ID = 49407                 # <|endoftext|>
+    PAD_ID = 0
+
+    def __init__(self, samples: int = 1024, batch: int = 1, size: int = 224, context: int = 77, min_len: int = 8, seed: int = 1234):
+        if not 2 <= min_len <= context:
+            raise ValueError(f"SyntheticImageText: min_len must lie in [2, context = {context}], got {min_len}")
+        g = torch.Generator().manual_seed(seed)
+        batch = max(1, int(batch))
+        self.samples = max(batch, int(samples) // batch * batch)
+        self.X = torch.randn(self.samples, 3, size, size, generator=g)
+        lens = torch.randint(min_len, context + 1, (self.samples,), generator=g)
+        pos = torch.arange(context)[None, :]
+        ids = torch.randint(1, self.SOT_ID, (self.samples, context), generator=g)
+        ids[:, 0] = self.SOT_ID
+        ids = torch.where(pos == (lens - 1)[:, None], torch.full_like(ids, self.EOT_ID), ids)
+        self.Y = torch.where(pos >= lens[:, None], torch.full_like(ids, self.PAD_ID), ids)
+        self.caption_lengths = lens
+
+    def __len__(self) -> int:
+        return self.samples
+
+    def __getitem__(self, index):
+        return self.X[index], self.Y[index]
+
+    def batch(self, indices: torch.Tensor):
+        return self.X.index_select(0, indices), self.Y.index_select(0, indices)
+
+    def batch_into(self, indices: torch.Tensor, outs) -> None:
+        """Gather straight into caller-owned (pinned) buffers: one pass over the data."""
+        torch.index_select(self.X, 0, indices, out=outs[0])
+        torch.index_select(self.Y, 0, indices, out=outs[1])
+
+
 class SyntheticTokens(Dataset):
     """Token ids [seq] + MLM labels [seq] (-100 = not predicted) for the BERT config.
 

@@ -23,6 +23,15 @@ from ..utils import (get_logger_with_rank, redirect_warnings_to_logger, resolve_
 log = None
 
 
+class _StoreGiven(argparse.Action):
+    """Stores the value and records that the flag was given (``args.<dest>_given``), so a check can reject a flag that
+    was passed even when its value equals the default."""
+
+    def __call__(self, parser, namespace, values, option_string=None):
+        setattr(namespace, self.dest, values)
+        setattr(namespace, self.dest + "_given", True)
+
+
 def build_parser() -> argparse.ArgumentParser:
     p = argparse.ArgumentParser(description="H100-native DDP training template")
     # ---- reference flags (ddp.py:293-308), same names and defaults -----------------------------
@@ -54,7 +63,8 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--adam_beta2", type=float, default=0.999)
     p.add_argument("--adam_epsilon", type=float, default=1e-8)
     p.add_argument("--dataset_size", type=int, default=100000)
-    p.add_argument("--seq_len", type=int, default=512)
+    p.add_argument("--seq_len", type=int, default=512, action=_StoreGiven,
+                   help="token models: tokens per row (CLIP's captions are always 77 tokens and take no --seq_len)")
     p.add_argument("--backend", type=str, default="auto", choices=["auto", "b200", "nccl", "gloo"])
     p.add_argument("--bucket_cap_mb", type=float, default=None)
     p.add_argument("--gradient_as_bucket_view", action="store_true")
@@ -149,6 +159,7 @@ def setup(args):
     check_fused_lm_loss_args(args)
     check_sparse_prediction_args(args)
     check_moe_args(args)
+    check_contrastive_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -277,6 +288,29 @@ def check_moe_args(args) -> None:
         raise ValueError(f"--model {args.model} with its router load-balancing loss does not run under single-process "
                          f"multi-GPU DataParallel; launch one process per GPU (torchrun), make one GPU visible, or pass "
                          f"--router_aux_loss_coef 0")
+
+
+def check_contrastive_args(args) -> None:
+    """A contrastive model (CLIP) trains on image-caption pairs with its own loss over the global batch: the token-row
+    flags, ``--fp8`` and an explicit ``--loss`` do not apply, single-process multi-GPU ``DataParallel`` would split the
+    pairs across GPUs without gathering their features, and on a GPU the native loss needs a batch that is a multiple of 8."""
+    if not model_entry(args.model).contrastive:
+        return
+    for flag, given in (("--fp8", getattr(args, "fp8", False)), ("--pack", getattr(args, "pack", False)),
+                        ("--min_seq_len", getattr(args, "min_seq_len", None) is not None),
+                        ("--fused_lm_loss", getattr(args, "fused_lm_loss", False)),
+                        ("--sparse_prediction", getattr(args, "sparse_prediction", False)),
+                        ("--seq_len", getattr(args, "seq_len_given", False)), ("--loss", getattr(args, "loss", None) is not None)):
+        if given:
+            raise ValueError(f"{flag} does not apply to --model {args.model}: CLIP trains on image-caption pairs (77-token "
+                             f"captions) with its own contrastive loss")
+    if getattr(args, "device", None) is not None and args.device.type == "cuda":
+        if args.local_rank == -1 and getattr(args, "n_gpu", 1) > 1:
+            raise ValueError(f"--model {args.model} does not run under single-process multi-GPU DataParallel (its loss gathers "
+                             f"every rank's features); launch one process per GPU (torchrun) or make one GPU visible")
+        if args.per_gpu_train_batch_size % 8:
+            raise ValueError(f"--model {args.model} on a GPU needs --per_gpu_train_batch_size to be a multiple of 8 (the native "
+                             f"contrastive loss), got {args.per_gpu_train_batch_size}")
 
 
 def padding_on(args) -> bool:

@@ -21,8 +21,10 @@ import torch
 class TrainStep:
     def __init__(self, model, criterion, optimizer, device: torch.device, accumulation: int = 1, use_graph: bool = False,
                  input_transform: Optional[Callable] = None, target_transform: Optional[Callable] = None,
-                 graph_warmup: int = 3, loss_scale: float = 1.0):
+                 graph_warmup: int = 3, loss_scale: float = 1.0, paired: bool = False):
         self.model = model
+        # paired inputs (CLIP's image-caption pairs): the model takes both, model(x, y), and the criterion scores its output
+        self.paired = bool(paired)
         self.criterion = criterion
         self.optimizer = optimizer
         self.device = torch.device(device)
@@ -66,7 +68,7 @@ class TrainStep:
 
     def _fwd_bwd(self, x, y, boundary: bool) -> torch.Tensor:
         with self._sync_ctx(boundary):
-            out = self.model(x)
+            out = self.model(x, y) if self.paired else self.model(x)
             loss = self.criterion(out, y)
             if self.accumulation > 1:
                 loss = loss / self.accumulation
@@ -108,7 +110,10 @@ class TrainStep:
                 boundary = kind in ("single", "last")
                 # "first" is captured with .grad == None, so autograd leaves freshly written gradients in static (pool)
                 # buffers; the later captures find those tensors in .grad and accumulate into them in place
-                with torch.cuda.graph(g, stream=side, pool=pool):
+                # thread_local: the loader's helper threads keep gathering batches while this thread captures, and they
+                # wait on a pinned slot's copy event before refilling it; in the default global mode that wait, from
+                # another thread, invalidates the capture
+                with torch.cuda.graph(g, stream=side, pool=pool, capture_error_mode="thread_local"):
                     loss = self._fwd_bwd(self._static_x, self._static_y, boundary)
                     if boundary:
                         self._apply_optimizer()

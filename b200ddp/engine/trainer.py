@@ -22,9 +22,9 @@ import torch.distributed as dist
 from tqdm import tqdm
 from tqdm.auto import trange
 
-from ..data import BatchLoader, DevicePrefetcher, FooDataset, SyntheticImageNet, SyntheticTokens
+from ..data import BatchLoader, DevicePrefetcher, FooDataset, SyntheticImageNet, SyntheticImageText, SyntheticTokens
 from ..models import model_entry
-from ..ops import CrossEntropyLoss, MSELoss
+from ..ops import ClipLoss, CrossEntropyLoss, MSELoss
 from ..optim import FusedAdamW, FusedSGD, get_linear_schedule_with_warmup, weight_decay_groups
 from ..parallel import DataParallel, DistributedDataParallel, ShardedSampler
 from ..utils import StepTimer, is_main_process, nvtx_range, rng_state, restore_rng_state, to_mixed_bf16
@@ -44,12 +44,17 @@ def _summary_writer():
 
 
 def build_dataset(args):
-    """``args.model``'s synthetic data: the reference's ``FooDataset``, ImageNet-shaped images, or token rows over the
-    model's vocabulary whose packed documents start with its registry entry's ``start_id``."""
+    """``args.model``'s synthetic data: the reference's ``FooDataset``, ImageNet-shaped images, image-caption pairs (a whole
+    number of global batches), or token rows over the model's vocabulary whose packed documents start with its registry
+    entry's ``start_id``."""
     entry = model_entry(getattr(args, "model", "foo"))
     n = int(getattr(args, "dataset_size", 100000))
     if entry.kind == "foo":
         return FooDataset(n)
+    if entry.contrastive:
+        world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+        return SyntheticImageText(samples=min(n, int(getattr(args, "image_samples", 1024))),
+                                  batch=int(getattr(args, "train_batch_size", 1)) * world)
     if entry.kind == "image":
         dense = loss_kind(args) == "mse"
         return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
@@ -79,9 +84,11 @@ class RouterAuxLoss:
 
 def build_criterion(args, model: Optional[torch.nn.Module] = None):
     """``--loss``'s criterion; with ``--fused_lm_loss`` or ``--sparse_prediction`` the model's own head-plus-cross-entropy
-    (``lm_head_loss``).  A model with ``config.router_aux_loss_coef > 0`` (mixture of experts) adds its load-balancing loss
-    (``RouterAuxLoss``)."""
-    if getattr(args, "fused_lm_loss", False):
+    (``lm_head_loss``); for a contrastive model (CLIP) its contrastive loss over the global batch (``ClipLoss``).  A model
+    with ``config.router_aux_loss_coef > 0`` (mixture of experts) adds its load-balancing loss (``RouterAuxLoss``)."""
+    if model_entry(getattr(args, "model", "foo")).contrastive:
+        criterion = ClipLoss()
+    elif getattr(args, "fused_lm_loss", False):
         if model is None or not getattr(getattr(model, "config", None), "fused_lm_loss", False):
             raise ValueError("--fused_lm_loss needs a causal LM built with fused_lm_loss=True (it has lm_head_loss)")
         criterion = model.lm_head_loss()
@@ -177,11 +184,12 @@ class Trainer:
             self._resume_state = load_checkpoint(self.resume_dir, None, self.optimizer, self.scheduler)
             log.info("Resumed from checkpoint.", dict(path=self.resume_dir, global_step=self._resume_state.get("global_step")))
         self.model = model
+        self.paired = model_entry(getattr(args, "model", "foo")).contrastive
         if input_transform is None and self.device.type == "cuda" and model_entry(getattr(args, "model", "foo")).kind == "image":
             input_transform = self._make_image_transform()
         self.step_fn = TrainStep(model, self.criterion, self.optimizer, self.device,
                                  accumulation=args.gradient_accumulation_steps, use_graph=getattr(args, "cuda_graph", False),
-                                 input_transform=input_transform,
+                                 input_transform=input_transform, paired=self.paired,
                                  loss_scale=float(getattr(args, "loss_scale", 0) or 0) if getattr(args, "fp16", False) else 1.0)
         self.global_step = 1
         self.tr_loss_host = 0.0
@@ -429,7 +437,7 @@ class Trainer:
             x, y = self._to_compute(x), self._to_compute(y)
             if self.step_fn.input_transform is not None:
                 x = self.step_fn.input_transform(x)
-            loss = self.criterion(inner(x), y)
+            loss = self.criterion(inner(x, y) if self.paired else inner(x), y)
             total[0] += loss.double() * x.shape[0]
             total[1] += x.shape[0]
         if self.distributed:

@@ -13,6 +13,7 @@ from .llama import (GRANITE_3_0_1B_A400M, QWEN2_5_1_5B, QWEN3_0_6B, SMOLLM_135M,
 from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, ModernBertModel, ModernBertForMaskedLM, modernbert_base,
                          modernbert_large)
 from .vit import VIT_B_16, VIT_B_32, VIT_L_16, ViTConfig, VisionTransformer, vit_b_16, vit_b_32, vit_l_16
+from .clip import CLIP_VIT_B_16, CLIP_VIT_B_32, CLIPConfig, CLIPModel, clip_vit_b_16, clip_vit_b_32
 
 
 @dataclass(frozen=True)
@@ -25,6 +26,8 @@ class ModelEntry:
     fp8: bool = False                  # build takes fp8=True (block linears on FP8 tensor cores)
     moe: bool = False                  # mixture of experts: build takes router_aux_loss_coef
     max_seq_len: int | None = None     # a training cap on --seq_len below config.max_position
+    contrastive: bool = False          # image models trained on image-caption pairs with their own contrastive loss
+                                       # (CLIP): forward(images, input_ids), the criterion ops.ClipLoss
 
     @property
     def token_model(self) -> bool:
@@ -38,6 +41,8 @@ MODEL_REGISTRY = {
     "vit-b-16": ModelEntry(vit_b_16, "image"),
     "vit-b-32": ModelEntry(vit_b_32, "image"),
     "vit-l-16": ModelEntry(vit_l_16, "image"),
+    "clip-vit-b-32": ModelEntry(clip_vit_b_32, "image", contrastive=True),
+    "clip-vit-b-16": ModelEntry(clip_vit_b_16, "image", contrastive=True),
     "bert-base": ModelEntry(bert_base, "encoder", BERT_BASE, start_id=101, fp8=True),                 # [CLS]
     "modernbert-base": ModelEntry(modernbert_base, "encoder", MODERNBERT_BASE, start_id=50281, fp8=True),   # [CLS]
     "modernbert-large": ModelEntry(modernbert_large, "encoder", MODERNBERT_LARGE, start_id=50281, fp8=True),
@@ -63,4 +68,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

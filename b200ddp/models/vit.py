@@ -17,7 +17,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops import LayerNorm, Linear, image_token_bounds, linear, packed_attention, patch_embed
+from ..ops import LayerNorm, Linear, causal_attention, image_token_bounds, linear, packed_attention, patch_embed
 
 
 @dataclass(frozen=True)
@@ -44,11 +44,13 @@ VIT_L_16 = ViTConfig(patch_size=16, layers=24, heads=16, hidden=1024, mlp_dim=40
 
 class SelfAttention(nn.Module):
     """``nn.MultiheadAttention``'s parameters: the fused q | k | v projection ``in_proj_weight`` [3D, D] (the column layout
-    the attention kernels read) with ``in_proj_bias``, and ``out_proj``."""
+    the attention kernels read) with ``in_proj_bias``, and ``out_proj``.  ``causal=True`` (CLIP's text tower) attends
+    causally: ``causal_attention`` on the token stream, SDPA's causal mask per sequence."""
 
-    def __init__(self, hidden: int, heads: int):
+    def __init__(self, hidden: int, heads: int, causal: bool = False):
         super().__init__()
         self.heads = heads
+        self.causal = causal
         self.in_proj_weight = nn.Parameter(torch.empty(3 * hidden, hidden))
         self.in_proj_bias = nn.Parameter(torch.empty(3 * hidden))
         self.out_proj = Linear(hidden, hidden)
@@ -60,19 +62,21 @@ class SelfAttention(nn.Module):
         qkv = linear(x, self.in_proj_weight, self.in_proj_bias)
         if bounds is not None:                       # the token stream [T, D]: each image one document
             T = qkv.shape[0]
-            return self.out_proj(packed_attention(qkv.view(1, T, -1), bounds, self.heads).view(T, -1))
-        B, S, W = qkv.shape                          # [B, N + 1, 3D]: per image, no mask
+            attend = causal_attention if self.causal else packed_attention
+            return self.out_proj(attend(qkv.view(1, T, -1), bounds, self.heads).view(T, -1))
+        B, S, W = qkv.shape                          # [B, N + 1, 3D]: per image (or caption), no mask or the causal one
         q, k, v = (t.view(B, S, self.heads, -1).transpose(1, 2) for t in qkv.split(W // 3, dim=-1))
-        return self.out_proj(F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, S, W // 3))
+        o = F.scaled_dot_product_attention(q, k, v, is_causal=self.causal)
+        return self.out_proj(o.transpose(1, 2).reshape(B, S, W // 3))
 
 
 class MLPBlock(nn.Module):
-    """torchvision's ``MLPBlock`` keys: ``0`` (with the erf GELU, torchvision's ``1``, in its epilogue) and ``3``; its
-    dropouts (``2``, ``4``) are identities at torchvision's default rate 0."""
+    """torchvision's ``MLPBlock`` keys: ``0`` (with the erf GELU, torchvision's ``1``, in its epilogue, or another
+    ``activation`` of ``ops.linear``) and ``3``; its dropouts (``2``, ``4``) are identities at torchvision's default rate 0."""
 
-    def __init__(self, hidden: int, mlp_dim: int):
+    def __init__(self, hidden: int, mlp_dim: int, activation: str = "gelu"):
         super().__init__()
-        self.add_module("0", Linear(hidden, mlp_dim, activation="gelu"))
+        self.add_module("0", Linear(hidden, mlp_dim, activation=activation))
         self.add_module("3", Linear(mlp_dim, hidden))
         for m in (self[0], self[3]):
             nn.init.xavier_uniform_(m.weight)
@@ -86,12 +90,15 @@ class MLPBlock(nn.Module):
 
 
 class EncoderBlock(nn.Module):
-    def __init__(self, c: ViTConfig):
+    """A pre-norm block on any config with ``hidden``, ``heads``, ``mlp_dim`` and ``eps``; ``activation`` is the MLP's and
+    ``causal`` the attention's (CLIP's towers use QuickGELU, its text tower causal attention)."""
+
+    def __init__(self, c: ViTConfig, activation: str = "gelu", causal: bool = False):
         super().__init__()
         self.ln_1 = LayerNorm(c.hidden, eps=c.eps)
-        self.self_attention = SelfAttention(c.hidden, c.heads)
+        self.self_attention = SelfAttention(c.hidden, c.heads, causal)
         self.ln_2 = LayerNorm(c.hidden, eps=c.eps)
-        self.mlp = MLPBlock(c.hidden, c.mlp_dim)
+        self.mlp = MLPBlock(c.hidden, c.mlp_dim, activation)
 
     def forward(self, x: torch.Tensor, bounds: torch.Tensor | None = None) -> torch.Tensor:
         x = x + self.self_attention(self.ln_1(x), bounds)

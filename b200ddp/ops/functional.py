@@ -22,9 +22,20 @@ from .. import _ext
 
 EPI_NONE, EPI_BIAS, EPI_BIAS_RELU, EPI_BIAS_GELU = 0, 1, 2, 3
 _ACT_TO_EPI = {None: EPI_BIAS, "relu": EPI_BIAS_RELU, "gelu": EPI_BIAS_GELU}
-# GELU variants: the erf form ("gelu", BERT) and the tanh approximation ("gelu_tanh", GPT-2's ``gelu_new``).  Both run as
-# a bias epilogue plus one elementwise pass (csrc/loss.cu) that keeps the pre-activation for the backward.
+# GELU variants: the erf form ("gelu", BERT), the tanh approximation ("gelu_tanh", GPT-2's ``gelu_new``) and QuickGELU
+# ("quick_gelu", x sigmoid(1.702 x), CLIP's).  All run as a bias epilogue plus one elementwise pass (csrc/loss.cu) that keeps
+# the pre-activation for the backward.
 _GELU_TANH = {"gelu": False, "gelu_tanh": True}
+_GELUS = (*_GELU_TANH, "quick_gelu")
+QUICK_GELU_C = 1.702
+
+
+def _gelu_fwd(C, pre: torch.Tensor, activation: str) -> torch.Tensor:
+    return C.clip.quick_gelu_fwd(pre) if activation == "quick_gelu" else C.gelu_fwd(pre, _GELU_TANH[activation])
+
+
+def _gelu_bwd(C, dy: torch.Tensor, pre: torch.Tensor, activation: str) -> torch.Tensor:
+    return C.clip.quick_gelu_bwd(dy, pre) if activation == "quick_gelu" else C.gelu_bwd(dy, pre, _GELU_TANH[activation])
 
 
 def _gelu_tanh_grad(p: torch.Tensor) -> torch.Tensor:
@@ -56,12 +67,12 @@ class _LinearTC(torch.autograd.Function):
         x2 = x.reshape(-1, x.shape[-1])
         if not x2.is_contiguous():
             x2 = x2.contiguous()
-        if bias is None and activation not in (None, *_GELU_TANH):
+        if bias is None and activation not in (None, *_GELUS):
             raise ValueError("fused activation needs a bias (use bias=True)")
-        if activation in _GELU_TANH:
+        if activation in _GELUS:
             # keep the pre-activation for the backward (GELU' needs it): two launches, one extra tensor
             pre = C.gemm_nt(x2, weight, bias, EPI_BIAS if bias is not None else EPI_NONE, None)
-            y = C.gelu_fwd(pre, _GELU_TANH[activation])
+            y = _gelu_fwd(C, pre, activation)
             ctx.save_for_backward(x2, weight, pre)
         else:
             y = C.gemm_nt(x2, weight, bias, _ACT_TO_EPI[activation] if bias is not None else EPI_NONE, None)
@@ -78,8 +89,8 @@ class _LinearTC(torch.autograd.Function):
         dy2 = dy.reshape(-1, dy.shape[-1])
         if ctx.activation == "relu":
             dy2 = dy2 * (aux > 0).to(dy2.dtype)
-        elif ctx.activation in _GELU_TANH:
-            dy2 = C.gelu_bwd(dy2.contiguous(), aux, _GELU_TANH[ctx.activation])   # dy * gelu'(pre) in one pass
+        elif ctx.activation in _GELUS:
+            dy2 = _gelu_bwd(C, dy2.contiguous(), aux, ctx.activation)          # dy * gelu'(pre) in one pass
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
         dx = dw = db = None
@@ -257,16 +268,19 @@ class _LinearFP8(torch.autograd.Function):
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None,
            activation: Optional[str] = None, fp8: bool = False) -> torch.Tensor:
-    """y = act(x @ weight.T + bias), activation in {None, "relu", "gelu", "gelu_tanh"} ("gelu" is the erf form,
-    "gelu_tanh" the tanh approximation).  ``fp8=True`` runs the three GEMMs on FP8 tensor cores (``_LinearFP8``); on CUDA
-    it needs bf16 tensors and raises ``ValueError`` for anything else."""
+    """y = act(x @ weight.T + bias), activation in {None, "relu", "gelu", "gelu_tanh", "quick_gelu"} ("gelu" is the erf
+    form, "gelu_tanh" the tanh approximation, "quick_gelu" x sigmoid(1.702 x)).  ``fp8=True`` runs the three GEMMs on FP8
+    tensor cores (``_LinearFP8``); on CUDA it needs bf16 tensors and raises ``ValueError`` for anything else, and it has no
+    QuickGELU."""
     if fp8:
+        if activation == "quick_gelu":
+            raise ValueError("fp8 linear has no quick_gelu activation")
         return _LinearFP8.apply(x, weight, bias, activation, torch.is_grad_enabled())
     if x.is_cuda:
         N, K = weight.shape
         M = x.numel() // K
         if x.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and _tc_ok(M, N, K) \
-                and (bias is not None or activation in (None, *_GELU_TANH)) and os.environ.get("B200DDP_DISABLE_TC", "0") != "1":
+                and (bias is not None or activation in (None, *_GELUS)) and os.environ.get("B200DDP_DISABLE_TC", "0") != "1":
             return _LinearTC.apply(x, weight, bias, activation)
         if x.dtype == torch.float32 and weight.dtype == torch.float32 and N * (K + 1) * 4 <= 48 * 1024 and M * N * 4 <= 48 * 1024 \
                 and activation in (None, "relu"):
@@ -281,6 +295,8 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
         y = F.gelu(y)
     elif activation == "gelu_tanh":
         y = F.gelu(y, approximate="tanh")
+    elif activation == "quick_gelu":
+        y = y * torch.sigmoid(QUICK_GELU_C * y)                       # transformers' QuickGELUActivation
     return y
 
 
@@ -1467,3 +1483,130 @@ def patch_embed(images: torch.Tensor, weight: torch.Tensor, bias: Optional[torch
     patches = _C().vit.patchify(images, p, image_token_rows(B, per))
     y = linear(patches, weight.reshape(D, -1), bias)               # a channels_last weight is copied into (c, ky, kx) order
     return _PatchAssemble.apply(y, class_token, pos_embedding, B)
+
+
+# ------------------------------------------------------------------------------------------------
+# CLIP (csrc/clip.cu): captions as causal documents of one token stream, the contrastive loss over the global batch
+# ------------------------------------------------------------------------------------------------
+def caption_token_bounds(input_ids: torch.Tensor, eos_token_id: int):
+    """Causal-document bounds of B captions laid out one after another in one token stream: ``(bounds int32 [1, T, 2],
+    pooled long [B])`` for input_ids [B, L], T = ``image_token_rows(B, L)``.  Caption b owns rows [L b, L (b + 1)); with e_b
+    its first ``eos_token_id`` (transformers' ``(ids == eos).int().argmax(-1)``, so 0 for a caption without one), rows
+    L b + j with j <= e_b hold (L b, L b + e_b + 1) and every later row, and the padding past L B, holds (0, 0).
+    ``causal_attention(qkv.view(1, T, 3 * hidden), bounds, heads)`` then gives the pooled row L b + e_b (``pooled[b]``) the
+    same keys as the dense L x L causal mask, and never visits a row past an EOT.  Torch ops on input_ids' device: no host
+    synchronisation (CUDA-graph safe)."""
+    if input_ids.dim() != 2 or input_ids.is_floating_point() or input_ids.is_complex() or input_ids.numel() == 0:
+        raise ValueError(f"caption_token_bounds needs integer input_ids [B, L], got {input_ids.dtype} {tuple(input_ids.shape)}")
+    B, L = input_ids.shape
+    dev = input_ids.device
+    eot = (input_ids == eos_token_id).int().argmax(-1)
+    T = image_token_rows(B, L)
+    t = torch.arange(T, device=dev)
+    b = torch.clamp(t // L, max=B - 1)
+    first = b * L
+    e = eot[b]
+    keep = (t < B * L) & (t - first <= e)
+    zero = torch.zeros((), device=dev, dtype=torch.long)
+    bounds = torch.stack([torch.where(keep, first, zero), torch.where(keep, first + e + 1, zero)], -1).to(torch.int32)
+    return bounds.view(1, T, 2), torch.arange(B, device=dev) * L + eot
+
+
+def _vector_norm(x: torch.Tensor) -> torch.Tensor:
+    """transformers' ``_get_vector_norm``: sqrt(sum(x^2)) over the last dimension, kept."""
+    return torch.pow(torch.sum(torch.pow(x, 2), dim=-1, keepdim=True), 0.5)
+
+
+class _L2Normalize(torch.autograd.Function):
+    """u = x / ||x|| per row (csrc/clip.cu); the backward rnorm (du - u <u, du>) recomputes u from x in fp32."""
+
+    @staticmethod
+    def forward(ctx, x):
+        u, rnorm = _C().clip.l2norm_fwd(x)
+        ctx.save_for_backward(x, rnorm)
+        return u
+
+    @staticmethod
+    def backward(ctx, du):
+        x, rnorm = ctx.saved_tensors
+        return _C().clip.l2norm_bwd(du.to(torch.bfloat16).contiguous(), x, rnorm)
+
+
+class _ContrastiveLoss(torch.autograd.Function):
+    """Forward: z_img = u_img U_txt^T and z_txt = u_txt U_img^T on the wgmma GEMM (fp32 out), then one fused cross-entropy
+    (csrc/clip.cu) that writes the loss, both bf16 logit gradients and d logit_scale.  Backward: the four products
+    du_img = dz_img U_txt, dU_txt = dz_img^T u_img, du_txt = dz_txt U_img and dU_img = dz_txt^T u_txt on the same GEMM
+    (MN-major operands, no transposed copies), each dz first scaled by the upstream gradient on the device."""
+
+    @staticmethod
+    def forward(ctx, u_img, u_txt, U_img, U_txt, logit_scale, offset):
+        C = _C()
+        z_img = C.gemm(u_img, U_txt, None, False, False, EPI_NONE, True, None)
+        z_txt = C.gemm(u_txt, U_img, None, False, False, EPI_NONE, True, None)
+        loss, dscale, dz_img, dz_txt = C.clip.contrastive_xent(z_img, z_txt, logit_scale.reshape(1), int(offset))
+        ctx.save_for_backward(u_img, u_txt, U_img, U_txt, dz_img, dz_txt, dscale)
+        ctx.scale_shape = logit_scale.shape
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        C = _C()
+        u_img, u_txt, U_img, U_txt, dz_img, dz_txt, dscale = ctx.saved_tensors
+        g = g.detach().float()
+        dz_img, dz_txt = dz_img * g, dz_txt * g                   # bf16 out, one rounding of the fp32 product
+        du_img = C.gemm(dz_img, U_txt, None, False, True, EPI_NONE, False, None)
+        du_txt = C.gemm(dz_txt, U_img, None, False, True, EPI_NONE, False, None)
+        dU_txt = C.gemm(dz_img, u_img, None, True, True, EPI_NONE, False, None)
+        dU_img = C.gemm(dz_txt, u_txt, None, True, True, EPI_NONE, False, None)
+        return du_img, du_txt, dU_img, dU_txt, (dscale * g).view(ctx.scale_shape), None
+
+
+def _gather_features(x: torch.Tensor, group) -> torch.Tensor:
+    """The rows of every rank of ``group``, in rank order, with autograd: the backward sums the gradient of the gathered
+    rows across ranks and returns this rank's slice (``torch.distributed.nn.functional.all_gather``)."""
+    from torch.distributed.nn.functional import all_gather
+    return torch.cat(all_gather(x.contiguous(), group=group), 0)
+
+
+def clip_loss(image_embeds: torch.Tensor, text_embeds: torch.Tensor, logit_scale: torch.Tensor, group=None) -> torch.Tensor:
+    """CLIP's contrastive loss over the global batch: with u = x / ||x|| per row, s = exp(logit_scale) (no clamp), and the
+    N = world B normalised features of every rank gathered in rank order (U_img, U_txt),
+    (CE(s u_img U_txt^T, rank B + r) + CE(s u_txt U_img^T, rank B + r)) / 2 averaged over the B local rows -
+    transformers' ``clip_loss`` on the global batch's similarity rows this rank owns.  image_embeds, text_embeds [B, D]
+    (unnormalised), logit_scale a one-element tensor.
+
+    Ranks: ``group``, or the default process group when one is initialised.  Above one rank the gather is
+    ``torch.distributed.nn.functional.all_gather``, whose backward sums the features' gradients over the ranks, so that
+    averaging the parameter gradients across ranks (DDP) gives the gradient of the global-batch mean loss.  One rank runs
+    no collective.
+
+    On CUDA: bf16 embeds with B % 8 == 0 and D % 8 == 0, else ``ValueError``.  The normalisation, the cross-entropy with its
+    gradients (``_ContrastiveLoss``) and the GEMMs are native and read nothing back to the host.  On CPU: torch ops."""
+    if image_embeds.dim() != 2 or tuple(text_embeds.shape) != tuple(image_embeds.shape) or image_embeds.shape[0] < 1:
+        raise ValueError(f"clip_loss needs image_embeds and text_embeds [B, D] of one shape with B >= 1, got "
+                         f"{tuple(image_embeds.shape)} and {tuple(text_embeds.shape)}")
+    if logit_scale.numel() != 1:
+        raise ValueError(f"clip_loss needs a one-element logit_scale, got {tuple(logit_scale.shape)}")
+    world, rank = 1, 0
+    if torch.distributed.is_available() and torch.distributed.is_initialized():
+        group = torch.distributed.group.WORLD if group is None else group
+        world, rank = torch.distributed.get_world_size(group), torch.distributed.get_rank(group)
+    B, D = image_embeds.shape
+    if image_embeds.is_cuda:
+        if image_embeds.dtype != torch.bfloat16 or text_embeds.dtype != torch.bfloat16 or B % 8 or D % 8:
+            raise ValueError(f"clip_loss on CUDA needs bf16 embeds with B % 8 == 0 and D % 8 == 0, got {image_embeds.dtype} and "
+                             f"{text_embeds.dtype} [{B}, {D}]")
+        if logit_scale.device != image_embeds.device:
+            raise ValueError(f"clip_loss needs logit_scale on the embeds' device ({image_embeds.device}), got {logit_scale.device}")
+        u_img, u_txt = _L2Normalize.apply(image_embeds.contiguous()), _L2Normalize.apply(text_embeds.contiguous())
+    else:
+        u_img, u_txt = image_embeds / _vector_norm(image_embeds), text_embeds / _vector_norm(text_embeds)
+    if world > 1:
+        U_img, U_txt = _gather_features(u_img, group), _gather_features(u_txt, group)
+    else:
+        U_img, U_txt = u_img, u_txt
+    if image_embeds.is_cuda:
+        return _ContrastiveLoss.apply(u_img, u_txt, U_img, U_txt, logit_scale.float(), rank * B)
+    s = logit_scale.exp()
+    labels = torch.arange(B, device=image_embeds.device) + rank * B
+    return (F.cross_entropy((u_img @ U_txt.t()) * s, labels) + F.cross_entropy((u_txt @ U_img.t()) * s, labels)) / 2.0

@@ -167,6 +167,19 @@ class CrossEntropyLoss(nn.Module):
         return Fn.cross_entropy(logits, target, self.ignore_index)
 
 
+class ClipLoss(nn.Module):
+    """Criterion over a CLIP model's output ``(image_embeds, text_embeds, logit_scale)``: ``clip_loss`` over the global
+    batch of ``group`` (the default process group when None).  The target argument is ignored: the labels are the pairs."""
+
+    def __init__(self, group=None):
+        super().__init__()
+        self.group = group
+
+    def forward(self, out, target=None) -> torch.Tensor:
+        image_embeds, text_embeds, logit_scale = out
+        return Fn.clip_loss(image_embeds, text_embeds, logit_scale, self.group)
+
+
 class LinearCrossEntropyLoss(nn.Module):
     """Criterion over final hidden states: ``linear_cross_entropy(hidden, weight, target, bias, sparse=sparse)``, where
     ``head()`` returns the model's current ``(weight, bias or None)`` at every call, so casts and moves of the model

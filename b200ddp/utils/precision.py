@@ -11,11 +11,17 @@ _KEEP_FP32 = (nn.modules.batchnorm._BatchNorm,)
 
 
 def to_mixed_bf16(model: nn.Module, keep_norm_fp32: bool = True) -> nn.Module:
+    """bf16 weights, with BatchNorm (``keep_norm_fp32``) and the parameters a module names in ``keep_fp32_params`` (CLIP's
+    ``logit_scale``, whose exponential bf16 would round) left in fp32."""
     model.to(torch.bfloat16)
     if keep_norm_fp32:
         for m in model.modules():
             if isinstance(m, _KEEP_FP32):
                 m.float()
+    for m in model.modules():
+        for name in getattr(m, "keep_fp32_params", ()):
+            p = getattr(m, name)
+            p.data = p.data.float()
     return model
 
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -913,6 +913,57 @@ def main():
                    timeit(lambda: C.packed_attention_bwd(dout, qkv, o, lse, bounds, H), args.iters), flops=2.5 * fwd_flops,
                    lib_ms=lib, note="lib = SDPA flash backward into qkv")
         del x, q, k, v, ya, y, yl
+
+    if "clip" in want:
+        # CLIP's contrastive loss at B = 256 pairs per rank, 512-wide features: clip_loss forward and backward against the
+        # torch expression in bf16 (normalise, two logit matrices, two cross-entropies); N = 2048 stands for 8 ranks through
+        # the label offset (the gathered features are inputs here, no collective).  And QuickGELU at CLIP-B's MLP width.
+        import torch.nn.functional as F
+        print(f"clip kernels on {card()}", flush=True)
+        B, D = 256, 512
+        g = torch.Generator(device="cuda").manual_seed(5)
+        for N in (256, 2048):
+            rank = N // B - 1
+            u_img = torch.nn.functional.normalize(torch.randn(B, D, device=dev, generator=g), dim=-1).to(torch.bfloat16).requires_grad_(True)
+            u_txt = torch.nn.functional.normalize(torch.randn(B, D, device=dev, generator=g), dim=-1).to(torch.bfloat16).requires_grad_(True)
+            others = [torch.nn.functional.normalize(torch.randn(N - B, D, device=dev, generator=g), dim=-1).to(torch.bfloat16) for _ in range(2)]
+            scale = torch.tensor(2.6592, device=dev, requires_grad=True)
+
+            def gathered():
+                return (torch.cat([others[0][:rank * B], u_img, others[0][rank * B:]]),
+                        torch.cat([others[1][:rank * B], u_txt, others[1][rank * B:]]))
+
+            def native():
+                U_img, U_txt = gathered()
+                return Fn._ContrastiveLoss.apply(u_img, u_txt, U_img, U_txt, scale, rank * B)
+
+            labels = torch.arange(B, device=dev) + rank * B
+
+            def torch_expr():
+                U_img, U_txt = gathered()
+                s = scale.exp()
+                return (F.cross_entropy((u_img @ U_txt.t()).float() * s, labels) +
+                        F.cross_entropy((u_txt @ U_img.t()).float() * s, labels)) / 2
+            flops = 2 * 2.0 * B * N * D                             # the two similarity GEMMs
+            with torch.no_grad():
+                record(f"clip loss fwd B{B} N{N}", timeit(native, args.iters), flops=flops, lib_ms=timeit(torch_expr, args.iters),
+                       note="fused cross-entropy on wgmma similarities; lib = bf16 matmuls + F.cross_entropy")
+            ln, lt = native(), torch_expr()
+            record(f"clip loss bwd B{B} N{N}",
+                   timeit(lambda: torch.autograd.grad(ln, (u_img, u_txt, scale), retain_graph=True), args.iters), flops=2 * flops,
+                   lib_ms=timeit(lambda: torch.autograd.grad(lt, (u_img, u_txt, scale), retain_graph=True), args.iters),
+                   note="four GEMMs from the forward's dz; lib = autograd through the torch expression")
+            del ln, lt
+        x = torch.randn(256 * 50, 3072, device=dev, generator=g).to(torch.bfloat16)
+        dy = torch.randn_like(x)
+        n = x.numel()
+        record("quick_gelu fwd 12800x3072 bf16", timeit(lambda: C.clip.quick_gelu_fwd(x), args.iters), bytes_=n * 4,
+               lib_ms=timeit(lambda: x * torch.sigmoid(1.702 * x), args.iters), note="lib = x * torch.sigmoid(1.702 * x)")
+        xr = x.detach().clone().requires_grad_(True)
+        yl = xr * torch.sigmoid(1.702 * xr)
+        record("quick_gelu bwd 12800x3072 bf16", timeit(lambda: C.clip.quick_gelu_bwd(dy, x), args.iters), bytes_=n * 6,
+               lib_ms=timeit(lambda: torch.autograd.grad(yl, xr, dy, retain_graph=True), args.iters), note="lib = autograd of the same")
+        del x, dy, xr, yl
 
     if "mse" in want:
         n = 64 * 1024 * 1024
