@@ -170,8 +170,9 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the type behind the _C.clip namespace of static entry points
+// the types behind the _C.clip and _C.cross namespaces of static entry points
 struct ClipNamespace {};
+struct CrossNamespace {};
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
   CommCtx c;
@@ -405,6 +406,17 @@ at::Tensor attn_bwd(const char* fn, AttnBwd launch, int hd, Mask kind, const at:
   launch(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), mask.data_ptr<int>(), B, S, heads, kv_heads,
          dsum.data_ptr<float>(), dqkv.data_ptr(), cur_stream());
   return dqkv;
+}
+
+// checks q, kv and q_bounds of a cross-attention binding (heads * 64 columns per query row); returns (B, Sq, Sk)
+std::tuple<int, int, int> cross_args(Args& args, const at::Tensor& q, const at::Tensor& kv, const at::Tensor& q_bounds, int heads) {
+  if (heads < 1) args.fail("heads", ">= 1", std::to_string(heads));
+  args("q_bounds", q_bounds, {kI32}, {kAny, kAny, 2}, kContiguous, 8);
+  args.expect(q_bounds.numel() >= 2, "q_bounds", "int32 [B, Sq, 2] with B, Sq >= 1", q_bounds);
+  const int64_t B = q_bounds.size(0), Sq = q_bounds.size(1), hidden = (int64_t)heads * 64;
+  args("q", q, {kBF16}, {B * Sq, hidden}, kContiguous, 16)("kv", kv, {kBF16}, {kAny, 2 * hidden}, kContiguous, 16);
+  args.expect(kv.size(0) % B == 0 && kv.size(0) >= B, "kv", "bf16 [B*Sk, 2*heads*64] with Sk >= 1", kv);
+  return std::make_tuple((int)B, (int)Sq, (int)(kv.size(0) / B));
 }
 
 }  // namespace
@@ -1633,4 +1645,37 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                             cur_stream());
     return std::make_tuple(loss, dscale, dz_img, dz_txt);
   }, py::arg("z_img"), py::arg("z_txt"), py::arg("logit_scale"), py::arg("label_offset"));
+
+  // ---- cross-attention (cross_attention.cu): decoder queries over another sequence's keys and values, head dim 64 ------
+  // _C.cross is a namespace of static entry points like _C.clip; its contract rows are in tests/test_cross_bindings_cpu.py.
+  // q bf16 [B*Sq, heads*64], kv bf16 [B*Sk, 2*heads*64] (key | value), q_bounds int32 [B, Sq, 2], kv_bounds int32
+  // [B, Sk, 2]; Sq, Sk multiples of 128 (the launcher checks them).
+  py::class_<CrossNamespace> cross(m, "cross", "Cross-attention of an encoder-decoder (cross_attention.cu)");
+  // (o bf16 [B*Sq, heads*64], lse fp32 [B, heads, Sq])
+  cross.def_static("cross_attention_fwd", [](at::Tensor q, at::Tensor kv, at::Tensor q_bounds, int heads) {
+    Args args("cross_attention_fwd");
+    const auto [B, Sq, Sk] = cross_args(args, q, kv, q_bounds, heads);
+    args.device();
+    at::Tensor o = at::empty_like(q);
+    at::Tensor lse = at::empty({B, heads, Sq}, q.options().dtype(kF32));
+    launch_cross_attention_fwd(q.data_ptr(), kv.data_ptr(), q_bounds.data_ptr<int>(), B, Sq, Sk, heads, o.data_ptr(), lse.data_ptr<float>(),
+                               cur_stream());
+    return std::make_tuple(o, lse);
+  }, py::arg("q"), py::arg("kv"), py::arg("q_bounds"), py::arg("heads"));
+  // (dq like q, dkv like kv)
+  cross.def_static("cross_attention_bwd", [](at::Tensor dout, at::Tensor q, at::Tensor kv, at::Tensor o, at::Tensor lse,
+                                                       at::Tensor q_bounds, at::Tensor kv_bounds, int heads) {
+    Args args("cross_attention_bwd");
+    const auto [B, Sq, Sk] = cross_args(args, q, kv, q_bounds, heads);
+    args("kv_bounds", kv_bounds, {kI32}, {B, Sk, 2}, kContiguous, 8);
+    args("dout", dout, {kBF16}, numel(q.numel()), kContiguous, 16)("o", o, {kBF16}, numel(q.numel()), kContiguous, 16);
+    args("lse", lse, {kF32}, numel((int64_t)B * heads * Sq), kContiguous, 8);
+    args.device();
+    at::Tensor dq = at::empty_like(q);
+    at::Tensor dkv = at::empty_like(kv);
+    at::Tensor dsum = at::empty({B, heads, Sq}, q.options().dtype(kF32));
+    launch_cross_attention_bwd(dout.data_ptr(), q.data_ptr(), kv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), q_bounds.data_ptr<int>(),
+                               kv_bounds.data_ptr<int>(), B, Sq, Sk, heads, dsum.data_ptr<float>(), dq.data_ptr(), dkv.data_ptr(), cur_stream());
+    return std::make_tuple(dq, dkv);
+  }, py::arg("dout"), py::arg("q"), py::arg("kv"), py::arg("o"), py::arg("lse"), py::arg("q_bounds"), py::arg("kv_bounds"), py::arg("heads"));
 }

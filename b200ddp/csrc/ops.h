@@ -270,4 +270,13 @@ void launch_l2norm_bwd(const void* du, const void* x, const float* rnorm, int B,
 void launch_contrastive_xent(const float* z_img, const float* z_txt, const float* logit_scale, int B, int N, int offset, void* dz_img,
                              void* dz_txt, float* row_partials, float* loss, float* dscale, cudaStream_t s);
 
+// ---------------- cross-attention on wgmma, head dim 64 (cross_attention.cu) ------------------------
+// q bf16 [B*Sq, heads*64], kv bf16 [B*Sk, 2*heads*64] (key block | value block), o bf16 [B*Sq, heads*64], lse fp32
+// [B, heads, Sq]; q_bounds int32 [B*Sq, 2] (the keys each query sees), kv_bounds int32 [B*Sk, 2] (the queries that see
+// each key, the same mask); Sq, Sk multiples of 128.  Backward: dsum fp32 [B, heads, Sq] scratch, dq like q, dkv like kv.
+void launch_cross_attention_fwd(const void* q, const void* kv, const int* q_bounds, int B, int Sq, int Sk, int heads, void* o, float* lse,
+                                cudaStream_t s);
+void launch_cross_attention_bwd(const void* dout, const void* q, const void* kv, const void* o, const float* lse, const int* q_bounds,
+                                const int* kv_bounds, int B, int Sq, int Sk, int heads, float* dsum, void* dq, void* dkv, cudaStream_t s);
+
 }  // namespace b200

@@ -239,3 +239,108 @@ class SyntheticTokens(Dataset):
         """Gather straight into caller-owned (pinned) buffers: one pass over the data."""
         torch.index_select(self.X, 0, indices, out=outs[0])
         torch.index_select(self.Y, 0, indices, out=outs[1])
+
+
+class SyntheticDenoising(Dataset):
+    """Source / target pairs for BART's text-infilling objective (seeded): ``X`` source ids [seq_len], right-padded with
+    ``PAD_ID``; ``Y`` labels [seq_len], the target ids, -100 at padding.
+
+    A target document is ``start_id`` followed by tokens from [4, vocab) other than ``start_id`` and ``mask_id`` (BART's
+    special ids are 0 to 3 and its <mask>); ``start_id`` is neither ``PAD_ID`` nor BART's decoder start id 2.  Its source is the same document with spans of the tokens after the start
+    replaced, each span by one ``mask_id``: span lengths are Poisson(3) clipped to at least 1 (the last one cut to the
+    budget), covering ``round(0.3 n)`` of the document's n tokens, so a source is never longer than its target.
+
+    Targets are ``seq_len`` tokens long, or uniform in [``min_len``, ``seq_len``] with ``min_len``.  ``pack=True`` places
+    the pairs into rows by first-fit decreasing target length (longest first, ties in pair order); the k-th source and
+    the k-th target of a row are one pair, and since no source is longer than its target every source fits.
+    ``bos_token_id`` is then ``start_id`` and ``doc_ids`` / ``doc_lengths`` list each row's pairs and target lengths.
+    ``pad_token_id`` is always ``PAD_ID`` (sources are shorter than their targets) and ``lengths`` holds each row's
+    filled target length."""
+
+    PAD_ID = 0
+
+    def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 50265, start_id: int = 3, mask_id: int = 50264,
+                 min_len: int | None = None, pack: bool = False, mask_ratio: float = 0.3, mean_span: float = 3.0, seed: int = 1234):
+        if min_len is not None and not 1 <= min_len <= seq_len:
+            raise ValueError(f"SyntheticDenoising: min_len must lie in [1, seq_len = {seq_len}], got {min_len}")
+        if not (0 < start_id < vocab and start_id != 2 and 4 <= mask_id < vocab and start_id != mask_id):
+            raise ValueError(f"SyntheticDenoising: start_id must lie in [1, vocab = {vocab}) other than the pad id 0 and the decoder "
+                             f"start id 2, mask_id in [4, vocab), and the two must differ; got {start_id} and {mask_id}")
+        g = torch.Generator().manual_seed(seed)
+        n = int(samples)
+        lens = torch.full((n,), seq_len) if min_len is None else torch.randint(min_len, seq_len + 1, (n,), generator=g)
+        lens_l = lens.tolist()
+        excluded = sorted(i for i in (start_id, mask_id) if i >= 4)
+        targets, sources = [], []
+        for L in lens_l:
+            body = torch.randint(4, vocab - len(excluded), (L - 1,), generator=g)
+            for e in excluded:                                      # [4, vocab) without start_id and mask_id
+                body += body >= e
+            targets.append(torch.cat([torch.tensor([start_id]), body]))
+            sources.append(torch.cat([torch.tensor([start_id]), self._infill(body, g, mask_id, mask_ratio, mean_span)]))
+        self.pad_token_id = self.PAD_ID
+        self.bos_token_id = None
+        self.doc_ids = self.doc_lengths = None
+        if pack:
+            rows, free = [], []
+            for i in sorted(range(n), key=lambda i: (-lens_l[i], i)):   # first-fit decreasing by target length
+                r = next((r for r, f in enumerate(free) if f >= lens_l[i]), len(rows))
+                if r == len(rows):
+                    rows.append([])
+                    free.append(seq_len)
+                rows[r].append(i)
+                free[r] -= lens_l[i]
+            self.doc_ids = rows
+            self.doc_lengths = [[lens_l[i] for i in docs] for docs in rows]
+            self.bos_token_id = start_id
+        else:
+            rows = [[i] for i in range(n)]
+        self.samples = len(rows)
+        self.X = torch.full((self.samples, seq_len), self.PAD_ID, dtype=torch.long)
+        self.Y = torch.full((self.samples, seq_len), -100, dtype=torch.long)
+        for r, docs in enumerate(rows):
+            a = b = 0
+            for i in docs:
+                s, t = sources[i], targets[i]
+                self.X[r, a:a + len(s)] = s
+                self.Y[r, b:b + len(t)] = t
+                a, b = a + len(s), b + len(t)
+        self.lengths = (self.Y != -100).sum(1)
+
+    @staticmethod
+    def _infill(body: torch.Tensor, g: torch.Generator, mask_id: int, ratio: float, mean_span: float) -> torch.Tensor:
+        """body with spans covering round(ratio * len) of its tokens replaced by one mask_id each."""
+        n = body.numel()
+        budget = int(round(ratio * n))
+        spans = []
+        while sum(spans) < budget:
+            spans += torch.poisson(torch.full((16,), mean_span), generator=g).clamp(min=1).long().tolist()
+        out, total = [], 0
+        for s in spans:
+            if total >= budget:
+                break
+            out.append(min(s, budget - total))
+            total += out[-1]
+        spans = out
+        # the n - budget kept tokens and the spans in a random interleaving (stars and bars)
+        slots = len(spans) + n - budget
+        is_span = torch.zeros(slots, dtype=torch.bool)
+        is_span[torch.randperm(slots, generator=g)[:len(spans)]] = True
+        width = torch.ones(slots, dtype=torch.long)
+        width[is_span] = torch.tensor(spans, dtype=torch.long)
+        first = torch.cumsum(width, 0) - width                    # each slot's first token in body
+        return torch.where(is_span, torch.full_like(first, mask_id), body[first.clamp(max=max(n - 1, 0))] if n else first)
+
+    def __len__(self) -> int:
+        return self.samples
+
+    def __getitem__(self, index):
+        return self.X[index], self.Y[index]
+
+    def batch(self, indices: torch.Tensor):
+        return self.X.index_select(0, indices), self.Y.index_select(0, indices)
+
+    def batch_into(self, indices: torch.Tensor, outs) -> None:
+        """Gather straight into caller-owned (pinned) buffers: one pass over the data."""
+        torch.index_select(self.X, 0, indices, out=outs[0])
+        torch.index_select(self.Y, 0, indices, out=outs[1])

@@ -160,6 +160,7 @@ def setup(args):
     check_sparse_prediction_args(args)
     check_moe_args(args)
     check_contrastive_args(args)
+    check_seq2seq_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -313,6 +314,19 @@ def check_contrastive_args(args) -> None:
                              f"contrastive loss), got {args.per_gpu_train_batch_size}")
 
 
+def check_seq2seq_args(args) -> None:
+    """An encoder-decoder (BART) trains on source / target pairs whose sources are always right-padded, so on the GPU its
+    attention always runs on the bf16 document kernels: it needs ``--fp16`` and ``--seq_len`` a multiple of 128 there.
+    ``--seq_len`` bounds both sides (the position table's check covers it)."""
+    if not model_entry(args.model).seq2seq:
+        return
+    if getattr(args, "device", None) is not None and args.device.type == "cuda":
+        if not args.fp16:
+            raise ValueError(f"--model {args.model} on a GPU needs --fp16: its attention kernels read bf16 activations")
+        if args.seq_len % 128:
+            raise ValueError(f"--model {args.model} on a GPU needs --seq_len to be a multiple of 128 (got {args.seq_len})")
+
+
 def padding_on(args) -> bool:
     """Rows are padded (and the model must hide padded keys) when some row can be shorter than --seq_len."""
     n = getattr(args, "min_seq_len", None)
@@ -345,7 +359,7 @@ def main(argv=None) -> int:
         kwargs["sparse_prediction"] = True
     if args.router_aux_loss_coef is not None:
         kwargs["router_aux_loss_coef"] = args.router_aux_loss_coef
-    if padding_on(args):
+    if padding_on(args) or model_entry(args.model).seq2seq:      # an encoder-decoder's sources are always padded
         from ..data import SyntheticTokens
         kwargs["pad_token_id"] = SyntheticTokens.PAD_ID
         if args.pack:

@@ -23,7 +23,8 @@ class TrainStep:
                  input_transform: Optional[Callable] = None, target_transform: Optional[Callable] = None,
                  graph_warmup: int = 3, loss_scale: float = 1.0, paired: bool = False):
         self.model = model
-        # paired inputs (CLIP's image-caption pairs): the model takes both, model(x, y), and the criterion scores its output
+        # paired inputs (CLIP's image-caption pairs, an encoder-decoder's source ids and labels): the model takes both,
+        # model(x, y), and the criterion scores its output
         self.paired = bool(paired)
         self.criterion = criterion
         self.optimizer = optimizer

@@ -22,7 +22,7 @@ import torch.distributed as dist
 from tqdm import tqdm
 from tqdm.auto import trange
 
-from ..data import BatchLoader, DevicePrefetcher, FooDataset, SyntheticImageNet, SyntheticImageText, SyntheticTokens
+from ..data import BatchLoader, DevicePrefetcher, FooDataset, SyntheticDenoising, SyntheticImageNet, SyntheticImageText, SyntheticTokens
 from ..models import model_entry
 from ..ops import ClipLoss, CrossEntropyLoss, MSELoss
 from ..optim import FusedAdamW, FusedSGD, get_linear_schedule_with_warmup, weight_decay_groups
@@ -45,8 +45,8 @@ def _summary_writer():
 
 def build_dataset(args):
     """``args.model``'s synthetic data: the reference's ``FooDataset``, ImageNet-shaped images, image-caption pairs (a whole
-    number of global batches), or token rows over the model's vocabulary whose packed documents start with its registry
-    entry's ``start_id``."""
+    number of global batches), source / target pairs for an encoder-decoder, or token rows over the model's vocabulary
+    whose packed documents start with its registry entry's ``start_id``."""
     entry = model_entry(getattr(args, "model", "foo"))
     n = int(getattr(args, "dataset_size", 100000))
     if entry.kind == "foo":
@@ -58,6 +58,9 @@ def build_dataset(args):
     if entry.kind == "image":
         dense = loss_kind(args) == "mse"
         return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
+    if entry.seq2seq:
+        return SyntheticDenoising(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=entry.config.vocab_size,
+                                  start_id=entry.start_id, min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)))
     causal = entry.kind == "causal"
     return SyntheticTokens(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=entry.config.vocab_size,
                            min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)),
@@ -184,7 +187,8 @@ class Trainer:
             self._resume_state = load_checkpoint(self.resume_dir, None, self.optimizer, self.scheduler)
             log.info("Resumed from checkpoint.", dict(path=self.resume_dir, global_step=self._resume_state.get("global_step")))
         self.model = model
-        self.paired = model_entry(getattr(args, "model", "foo")).contrastive
+        entry = model_entry(getattr(args, "model", "foo"))
+        self.paired = entry.contrastive or entry.seq2seq
         if input_transform is None and self.device.type == "cuda" and model_entry(getattr(args, "model", "foo")).kind == "image":
             input_transform = self._make_image_transform()
         self.step_fn = TrainStep(model, self.criterion, self.optimizer, self.device,

@@ -14,6 +14,7 @@ from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, Mo
                          modernbert_large)
 from .vit import VIT_B_16, VIT_B_32, VIT_L_16, ViTConfig, VisionTransformer, vit_b_16, vit_b_32, vit_l_16
 from .clip import CLIP_VIT_B_16, CLIP_VIT_B_32, CLIPConfig, CLIPModel, clip_vit_b_16, clip_vit_b_32
+from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneration, bart_base, bart_large
 
 
 @dataclass(frozen=True)
@@ -28,6 +29,8 @@ class ModelEntry:
     max_seq_len: int | None = None     # a training cap on --seq_len below config.max_position
     contrastive: bool = False          # image models trained on image-caption pairs with their own contrastive loss
                                        # (CLIP): forward(images, input_ids), the criterion ops.ClipLoss
+    seq2seq: bool = False              # encoder-decoder trained on source / target pairs (BART): forward(source_ids, labels),
+                                       # kind "causal" (the decoder is a causal LM over the target)
 
     @property
     def token_model(self) -> bool:
@@ -53,6 +56,10 @@ MODEL_REGISTRY = {
     "qwen3-0.6b": ModelEntry(qwen3_0_6b, "causal", QWEN3_0_6B, start_id=151643, fp8=True, max_seq_len=32768),
     # Granite's own start id, <|end_of_text|> = 0, is the padding id here, so packed documents start with id 1 instead
     "granite-3.0-1b-a400m": ModelEntry(granite_3_0_1b_a400m, "causal", GRANITE_3_0_1B_A400M, start_id=1, moe=True),
+    # BART's own <s> = 0 is the padding id here and </s> = 2 starts every decoder input, so packed documents start with
+    # id 3 (<unk>), which the synthetic text never holds otherwise
+    "bart-base": ModelEntry(bart_base, "causal", BART_BASE, start_id=3, seq2seq=True),
+    "bart-large": ModelEntry(bart_large, "causal", BART_LARGE, start_id=3, seq2seq=True),
 }
 
 
@@ -68,4 +75,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

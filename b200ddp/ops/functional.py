@@ -607,6 +607,142 @@ def causal_attention(qkv: torch.Tensor, bounds: torch.Tensor, heads: int, kv_hea
 
 
 # ------------------------------------------------------------------------------------------------
+# Cross-attention (csrc/cross_attention.cu): queries of one sequence attend to the keys / values of another
+# ------------------------------------------------------------------------------------------------
+def _interval_mask(bounds: torch.Tensor, n: int, device) -> torch.Tensor:
+    """[B, R, n] bool: row r sees column j iff start[r] <= j < end[r] (start clamped to [0, n], end to [start, n], like
+    the kernels)."""
+    b = bounds.to(device=device, dtype=torch.long)
+    start = b[..., 0].clamp(0, n)
+    end = torch.maximum(b[..., 1].clamp(max=n), start)
+    j = torch.arange(n, device=device)
+    return (j >= start[..., None]) & (j < end[..., None])
+
+
+def cross_attention_reference(q: torch.Tensor, kv: torch.Tensor, q_bounds: torch.Tensor, heads: int) -> torch.Tensor:
+    """softmax(Q K^T / sqrt(d)) V where query i of row b sees key j of row b iff q_bounds[b, i, 0] <= j < q_bounds[b, i, 1],
+    as a dense mask in fp32 (fp64 stays fp64); a query that sees no key gives zeros.  q [B, Sq, hidden], kv
+    [B, Sk, 2 * hidden] (key | value column blocks), q_bounds integer [B, Sq, 2]; returns [B, Sq, hidden] in q's dtype.
+    Differentiable."""
+    B, Sq, hidden = q.shape
+    Sk = kv.shape[1]
+    hd = hidden // heads
+    ct = torch.promote_types(q.dtype, torch.float32)
+    qh = q.to(ct).reshape(B, Sq, heads, hd).transpose(1, 2)
+    k, v = (t.to(ct).reshape(B, Sk, heads, hd).transpose(1, 2) for t in kv.split(hidden, dim=-1))
+    keep = _interval_mask(q_bounds, Sk, q.device)[:, None]
+    scores = (qh @ k.transpose(-1, -2)) * (1.0 / math.sqrt(hd))
+    p = torch.softmax(scores.masked_fill(~keep, torch.finfo(ct).min), dim=-1) * keep
+    return (p @ v).transpose(1, 2).reshape(B, Sq, hidden).to(q.dtype)
+
+
+def _cross_check(q: torch.Tensor, kv: torch.Tensor, q_bounds: torch.Tensor, kv_bounds: torch.Tensor, heads: int) -> None:
+    if q.dim() != 3 or kv.dim() != 3 or q.shape[0] != kv.shape[0] or kv.shape[-1] != 2 * q.shape[-1]:
+        raise ValueError(f"cross attention needs q [B, Sq, hidden] and kv [B, Sk, 2 * hidden], got {tuple(q.shape)} and {tuple(kv.shape)}")
+    B, Sq, hidden = q.shape
+    Sk = kv.shape[1]
+    if heads < 1 or hidden % heads or hidden // heads != ATTENTION_HEAD_DIM:
+        raise ValueError(f"cross attention on CUDA supports head dim {ATTENTION_HEAD_DIM} only, got hidden {hidden} over {heads} heads")
+    if q.dtype != torch.bfloat16 or kv.dtype != torch.bfloat16:
+        raise ValueError(f"cross attention on CUDA needs bf16 q and kv, got {q.dtype} and {kv.dtype}")
+    if Sq == 0 or Sk == 0 or Sq % ATTENTION_SEQ_MULTIPLE or Sk % ATTENTION_SEQ_MULTIPLE:
+        raise ValueError(f"cross attention on CUDA needs both lengths to be multiples of {ATTENTION_SEQ_MULTIPLE}, got Sq={Sq}, Sk={Sk}")
+    if not q.is_contiguous() or not kv.is_contiguous():
+        raise ValueError("cross attention on CUDA needs contiguous q and kv (the projections' outputs)")
+    for name, t, S in (("q_bounds", q_bounds, Sq), ("kv_bounds", kv_bounds, Sk)):
+        if tuple(t.shape) != (B, S, 2) or t.is_floating_point() or t.is_complex():
+            raise ValueError(f"cross attention needs integer {name} [B, {'Sq' if S == Sq else 'Sk'}, 2] = [{B}, {S}, 2], "
+                             f"got {t.dtype} {tuple(t.shape)}")
+
+
+class _CrossAttention(torch.autograd.Function):
+    """CUDA body: the sm_90a cross-attention kernels (forward keeps the row log-sum-exp; backward is four deterministic
+    launches writing dq and dkv, the gradients the two projections consume).  CPU body: ``cross_attention_reference``
+    (backward by recomputation through autograd)."""
+
+    @staticmethod
+    def forward(ctx, q, kv, q_bounds, kv_bounds, heads):
+        ctx.heads = heads
+        if q.is_cuda:
+            B, Sq, hidden = q.shape
+            Sk = kv.shape[1]
+            qb = q_bounds.to(device=q.device, dtype=torch.int32).contiguous()
+            kb = kv_bounds.to(device=q.device, dtype=torch.int32).contiguous()
+            o, lse = _C().cross.cross_attention_fwd(q.view(B * Sq, hidden), kv.view(B * Sk, 2 * hidden), qb, heads)
+            ctx.save_for_backward(q, kv, o, lse, qb, kb)
+            return o.view(B, Sq, hidden)
+        ctx.save_for_backward(q, kv, q_bounds)
+        return cross_attention_reference(q, kv, q_bounds, heads)
+
+    @staticmethod
+    def backward(ctx, dy):
+        if dy.is_cuda:
+            q, kv, o, lse, qb, kb = ctx.saved_tensors
+            B, Sq, hidden = q.shape
+            Sk = kv.shape[1]
+            do = dy.reshape(B * Sq, hidden).to(torch.bfloat16).contiguous()
+            if do.data_ptr() % 16:                                # the kernels read dO in 16-byte vectors / TMA boxes
+                do = do.clone()
+            dq, dkv = _C().cross.cross_attention_bwd(do, q.view(B * Sq, hidden), kv.view(B * Sk, 2 * hidden), o, lse, qb, kb, ctx.heads)
+            return dq.view(B, Sq, hidden), dkv.view(B, Sk, 2 * hidden), None, None, None
+        q, kv, q_bounds = ctx.saved_tensors
+        with torch.enable_grad():
+            x, y = q.detach().requires_grad_(True), kv.detach().requires_grad_(True)
+            dq, dkv = torch.autograd.grad(cross_attention_reference(x, y, q_bounds, ctx.heads), (x, y), dy)
+        return dq, dkv, None, None, None
+
+
+def cross_attention(q: torch.Tensor, kv: torch.Tensor, q_bounds: torch.Tensor, kv_bounds: torch.Tensor, heads: int) -> torch.Tensor:
+    """Multi-head cross-attention: q [B, Sq, hidden] (the query projection's output), kv [B, Sk, 2 * hidden] (the fused
+    key | value projection of the other sequence), q_bounds integer [B, Sq, 2]: query i of row b sees key j of row b iff
+    q_bounds[b, i, 0] <= j < q_bounds[b, i, 1]; kv_bounds integer [B, Sk, 2]: for key j, the interval of queries that see
+    it.  The two must describe the same mask (``cross_bounds`` builds such a pair); the kernels trust it rather than
+    check it, which would need a host synchronisation.  A query that sees no key gives zeros; a key no query sees gets
+    zero gradients.  Returns [B, Sq, hidden].  On CUDA: bf16, head dim 64, Sq and Sk multiples of 128, contiguous q and
+    kv, else ``ValueError``; bounds stay on the device (CUDA-graph safe)."""
+    if q.is_cuda:
+        _cross_check(q, kv, q_bounds, kv_bounds, heads)
+    return _CrossAttention.apply(q, kv, q_bounds, kv_bounds, heads)
+
+
+def _document_table(bounds: torch.Tensor, slots: int):
+    """Per position, the index of its document in its row (counting from 0, -1 for padding), and a table
+    [B, slots + 1, 2] (slots >= S) of each row's k-th document's (start, end), (0, 0) where the row has no k-th document."""
+    B, S, _ = bounds.shape
+    b = bounds.to(torch.long)
+    start, end = b[..., 0], b[..., 1]
+    pos = torch.arange(S, device=b.device)
+    is_start = (start == pos) & (end > start)
+    index = torch.where(end > start, is_start.long().cumsum(1) - 1, -1)
+    slot = torch.where(is_start, index, slots)
+    table = torch.zeros(B, slots + 1, 2, dtype=torch.long, device=b.device)
+    table.scatter_(1, slot[..., None].expand(B, S, 2), torch.where(is_start[..., None], b, 0))
+    table[:, slots] = 0
+    return index, table
+
+
+def cross_bounds(enc_bounds: torch.Tensor, dec_bounds: torch.Tensor):
+    """Cross-attention bounds of paired documents: the k-th decoder document of a row sees the k-th encoder document of
+    the same row.  enc_bounds [B, Sk, 2] and dec_bounds [B, Sq, 2] are the two sides' ``document_bounds``.  Returns
+    ``(q_bounds, kv_bounds)`` int32 [B, Sq, 2] and [B, Sk, 2]: each decoder position gets its partner document's (start,
+    end), each encoder position its partner's; padding positions and documents without a partner get (0, 0).  Both
+    describe the same mask, as ``cross_attention`` requires.  Torch ops on the bounds' device, no host synchronisation."""
+    if enc_bounds.dim() != 3 or dec_bounds.dim() != 3 or enc_bounds.shape[0] != dec_bounds.shape[0] or enc_bounds.shape[-1] != 2 \
+            or dec_bounds.shape[-1] != 2:
+        raise ValueError(f"cross_bounds needs enc_bounds [B, Sk, 2] and dec_bounds [B, Sq, 2], got {tuple(enc_bounds.shape)} "
+                         f"and {tuple(dec_bounds.shape)}")
+    slots = max(enc_bounds.shape[1], dec_bounds.shape[1])
+    enc_index, enc_table = _document_table(enc_bounds, slots)
+    dec_index, dec_table = _document_table(dec_bounds, slots)
+
+    def partner(index, table):
+        got = torch.gather(table, 1, torch.where(index >= 0, index, slots)[..., None].expand(*index.shape, 2))
+        return got.to(torch.int32)
+
+    return partner(dec_index, enc_table), partner(enc_index, dec_table)
+
+
+# ------------------------------------------------------------------------------------------------
 # Llama building blocks: rotary position embedding (csrc/rotary.cu), RMSNorm (csrc/layernorm.cu), SwiGLU (csrc/loss.cu)
 # ------------------------------------------------------------------------------------------------
 def rotary_cos_sin(max_position: int, head_dim: int = ATTENTION_HEAD_DIM, theta: float = 10000.0) -> torch.Tensor:

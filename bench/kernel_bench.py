@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -965,6 +965,59 @@ def main():
                lib_ms=timeit(lambda: torch.autograd.grad(yl, xr, dy, retain_graph=True), args.iters), note="lib = autograd of the same")
         del x, dy, xr, yl
 
+    if "cross" in want:
+        # Cross-attention at bart-base's shape (12 heads, batch 16): Sq = Sk = 512, and Sq 128 over Sk 1024.  Full rows
+        # against SDPA (flash); right-padded rows (source / target lengths U[S/4, S]) and packed rows (the denoising data's
+        # pairs, documents U[64, S]) against SDPA with the dense [B, 1, Sq, Sk] mask.  FLOPs count the visible pairs only:
+        # forward 4 d H sum(q_end - q_start), backward 2.5x that.
+        import torch.nn.functional as F
+        from b200ddp.data import SyntheticDenoising
+        from b200ddp.ops import cross_bounds, document_bounds
+        H, d, B = 12, 64, 16
+        g = torch.Generator(device=dev).manual_seed(0)
+        for Sq, Sk in ((512, 512), (128, 1024)):
+            q = torch.randn(B * Sq, H * d, device=dev, generator=g).to(torch.bfloat16)
+            kv = torch.randn(B * Sk, 2 * H * d, device=dev, generator=g).to(torch.bfloat16)
+            dout = torch.randn(B * Sq, H * d, device=dev, generator=g).to(torch.bfloat16)
+            rng = torch.Generator().manual_seed(1)
+            src_l = torch.randint(Sk // 4, Sk + 1, (B,), generator=rng)
+            tgt_l = torch.randint(Sq // 4, Sq + 1, (B,), generator=rng)
+            pad = lambda n, S: (torch.arange(S)[None, :] < n[:, None]).long()
+            packed = SyntheticDenoising(samples=4 * B, seq_len=min(Sq, Sk), min_len=64, pack=True)
+            pick = torch.linspace(0, len(packed) - 1, B).long()
+            ids = lambda t, S: torch.nn.functional.pad(t, (0, S - t.shape[1]))
+            cases = [("full", torch.ones(B, Sk, dtype=torch.long), torch.ones(B, Sq, dtype=torch.long), None),
+                     ("padded", pad(src_l, Sk), pad(tgt_l, Sq), None),
+                     ("packed", ids(packed.X[pick], Sk), ids(packed.Y[pick].clamp(min=0), Sq), packed.bos_token_id)]
+            for label, src, tgt, bos in cases:
+                enc, _ = document_bounds(src.to(dev), bos, 0)
+                dec, _ = document_bounds(tgt.to(dev), bos, 0)
+                qb, kb = cross_bounds(enc, dec)
+                vis = float((qb[..., 1] - qb[..., 0]).sum())
+                fwd_flops = 4.0 * d * H * vis
+                xq = q.view(B, Sq, H * d).detach().clone().requires_grad_(True)
+                xkv = kv.view(B, Sk, 2 * H * d).detach().clone().requires_grad_(True)
+                qh = xq.view(B, Sq, H, d).transpose(1, 2)
+                kh, vh = (t.reshape(B, Sk, H, d).transpose(1, 2) for t in xkv.split(H * d, -1))
+                j = torch.arange(Sk, device=dev)
+                mask = None if label == "full" else ((j >= qb[..., :1]) & (j < qb[..., 1:]))[:, None]
+                if mask is not None:
+                    mask |= ~mask.any(-1, keepdim=True) & (j == 0)      # a query that sees nothing: one key, not a NaN row
+
+                def sdpa():
+                    return F.scaled_dot_product_attention(qh, kh, vh, attn_mask=mask).transpose(1, 2).reshape(B, Sq, H * d)
+                lib_name = "SDPA flash" if mask is None else "SDPA dense bool mask"
+                name = f"cross {label} B{B} Sq{Sq} Sk{Sk} H{H}"
+                lib = timeit(lambda: sdpa().detach(), args.iters)
+                record(f"{name} fwd", timeit(lambda: C.cross.cross_attention_fwd(q, kv, qb, H), args.iters), flops=fwd_flops,
+                       lib_ms=lib, note=f"lib = {lib_name} + output transpose")
+                o, lse = C.cross.cross_attention_fwd(q, kv, qb, H)
+                y = sdpa()
+                dy = dout.view(B, Sq, H * d)
+                lib = timeit(lambda: torch.autograd.grad(y, (xq, xkv), dy, retain_graph=True), args.iters)
+                record(f"{name} bwd", timeit(lambda: C.cross.cross_attention_bwd(dout, q, kv, o, lse, qb, kb, H), args.iters),
+                       flops=2.5 * fwd_flops, lib_ms=lib, note=f"lib = {lib_name} backward into q and kv")
+                del xq, xkv, y
     if "mse" in want:
         n = 64 * 1024 * 1024
         o = torch.randn(n, device=dev, dtype=torch.bfloat16)
