@@ -80,12 +80,67 @@ __device__ __forceinline__ int2 kv_cols(int h, int H, int HD, int Hkv) {
   }
 }
 
+// ============================================== relative position bias ===============================================
+// kBias (kSegment / kCausal, multi-head): T5's learned relative position bias.  table fp32 [H, 257] holds head h's bias
+// for the clamped distance k - i in [-128, 128] at column k - i + 128; the score of a visible pair is q.k + table[h, .]
+// with no 1/sqrt(d) scale, so lse, P and the gradients are those of the unscaled, biased scores.  Each CTA keeps its
+// head's row in shared memory (after the 256 bytes of barriers and scratch every layout reserves), widened to the
+// distances [-264, 264] so that a thread's lookups need no clamp: a thread with any distance inside (-128, 128) has all
+// of them within 129 of it.
+constexpr int kRelMax = 128;
+constexpr int kRelCols = 2 * kRelMax + 1;                       // 257
+constexpr int kRelMid = kRelMax + 136;                          // the widened row: distance d at kRelMid + d
+constexpr int kBiasTable = 2304;                                // 2 kRelMid + 1 entries, then 16 floats of far-sum scratch
+constexpr int kFarRed = 2 * kRelMid + 4;                        // the scratch's offset in floats
+constexpr int kPartStride = 25;                                 // dQ: floats per thread in a diagonal-fold buffer (odd: no bank conflicts)
+constexpr int kPartBytes = 2 * 256 * kPartStride * 4;           // dQ: two buffers of 256 consumer threads
+
+// Copies head h's table row, widened, into shared memory; every thread calls it before the kernel's first __syncthreads.
+__device__ __forceinline__ void load_bias_table(float* tbl, const float* __restrict__ table, int h) {
+  for (int i = threadIdx.x; i <= 2 * kRelMid; i += blockDim.x)
+    tbl[i] = __ldg(table + (size_t)h * kRelCols + min(max(i - kRelMid, -kRelMax), kRelMax) + kRelMax);
+}
+
+// Adds the bias to one thread's fragment of 4 * kJ scores.  Element (i, j, e) (s[4 j + 2 i + e]: row half i, column
+// 8 j + e from the thread's first) lies at distance base + i * kDi + kSign * (8 j + e), in [base + kLo, base + kHi].  A
+// thread whose distances all lie beyond +-128 on one side has a constant bias: its base is moved to where its nearest
+// distance is +-128, which reads that same entry everywhere from the widened row, so one branch-free path serves both.
+// rel_bias_row gives the thread's row pointer t: the bias of element (i, j, e) is t[i * kDi + kSign * (8 j + e)].
+template <int kJ, int kSign, int kDi>
+__device__ __forceinline__ const float* rel_bias_row(const float* tbl, int base) {
+  constexpr int kSpan = 8 * (kJ - 1);
+  constexpr int kLo = (kDi < 0 ? kDi : 0) - (kSign < 0 ? kSpan + 1 : 0), kHi = (kDi > 0 ? kDi : 0) + (kSign > 0 ? kSpan + 1 : 0);
+  static_assert(kHi - kLo <= kRelMid - kRelMax, "the widened row must cover a thread's distances");
+  return tbl + kRelMid + min(max(base, -kRelMax - kHi), kRelMax - kLo);
+}
+__device__ __forceinline__ float lds_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+  return v;
+}
+template <int kJ, int kSign, int kDi>
+__device__ __forceinline__ void add_rel_bias(float (&s)[4 * kJ], const float* tbl, int base) {
+  const float* t = rel_bias_row<kJ, kSign, kDi>(tbl, base);
+#pragma unroll
+  for (int j = 0; j < kJ; ++j) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) s[4 * j + 2 * i + e] += t[i * kDi + kSign * (8 * j + e)];
+    }
+  }
+}
+
 // ============================================== forward ==============================================================
-// mask: seq_lens [B] (kKeyPadding) or bounds [B*S, 2] (kSegment, kCausal); Hkv: K/V heads (read only when kGqa)
-template <int kMode, bool kGqa = false>
+// mask: seq_lens [B] (kKeyPadding) or bounds [B*S, 2] (kSegment, kCausal); Hkv: K/V heads (read only when kGqa);
+// table: the relative bias (read only when kBias)
+template <int kMode, bool kGqa = false, bool kBias = false>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restrict__ mask, int S, int H,
-                __nv_bfloat16* __restrict__ o, float* __restrict__ lse, int Hkv) {
+                __nv_bfloat16* __restrict__ o, float* __restrict__ lse, int Hkv, const float* __restrict__ table) {
+  static_assert(!kBias || (kMode != kKeyPadding && !kGqa), "the relative bias is a document-mode, multi-head instantiation");
+  constexpr float kSc = kBias ? 1.f : kScale;                   // natural-log units per score unit
+  constexpr float kSL = kSc * kLog2e;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sq = smem;                                           // 128 query rows
@@ -93,6 +148,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
   uint64_t* q_bar = reinterpret_cast<uint64_t*>(ring + kFwdStages * 4 * kBoxBytes);
   uint64_t* full_bar = q_bar + 1;
   uint64_t* empty_bar = full_bar + kFwdStages;
+  float* tbl = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(q_bar) + 256);   // kBias
 
   const int3 tc = tile_coords<kMode, false>();
   const int qt = tc.x, h = tc.y, b = tc.z;
@@ -119,6 +175,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
     for (int i = 0; i < kFwdStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerArrivals); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  if constexpr (kBias) load_bias_table(tbl, table, h);
   __syncthreads();
 
   if (warp == 0) {
@@ -173,6 +230,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
       wgmma_commit();
       wgmma_wait<0>();
       const int key0 = kt * 128;
+      if constexpr (kBias) add_rel_bias<16, 1, -8>(s, tbl, key0 + c0 - (qt * 128 + wg * 64 + r0));
       if constexpr (kMode == kKeyPadding) {
         if (key0 + 128 > len) {                                 // partial tile: hide keys at or beyond the length
 #pragma unroll
@@ -209,23 +267,23 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
         mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
         mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
         if constexpr (kMode == kKeyPadding) {
-          alpha[i] = exp2f((m[i] - mx[i]) * kScaleLog2);        // key 0 is visible, so mx is finite; 0 on the first tile
+          alpha[i] = exp2f((m[i] - mx[i]) * kSL);               // key 0 is visible, so mx is finite; 0 on the first tile
           m[i] = mx[i];
-          mb[i] = mx[i] * kScaleLog2;
+          mb[i] = mx[i] * kSL;
         } else {
           // a row may have seen no visible key yet (mx = -inf): subtract 0 instead, so exp2 gives 0 rather than NaN
           const float base = mx[i] == -INFINITY ? 0.f : mx[i];
-          alpha[i] = exp2f((m[i] - base) * kScaleLog2);
+          alpha[i] = exp2f((m[i] - base) * kSL);
           m[i] = mx[i];
-          mb[i] = base * kScaleLog2;
+          mb[i] = base * kSL;
         }
       }
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        s[4 * j] = exp2f(s[4 * j] * kScaleLog2 - mb[0]);
-        s[4 * j + 1] = exp2f(s[4 * j + 1] * kScaleLog2 - mb[0]);
-        s[4 * j + 2] = exp2f(s[4 * j + 2] * kScaleLog2 - mb[1]);
-        s[4 * j + 3] = exp2f(s[4 * j + 3] * kScaleLog2 - mb[1]);
+        s[4 * j] = exp2f(s[4 * j] * kSL - mb[0]);
+        s[4 * j + 1] = exp2f(s[4 * j + 1] * kSL - mb[0]);
+        s[4 * j + 2] = exp2f(s[4 * j + 2] * kSL - mb[1]);
+        s[4 * j + 3] = exp2f(s[4 * j + 3] * kSL - mb[1]);
         rs[0] += s[4 * j] + s[4 * j + 1];
         rs[1] += s[4 * j + 2] + s[4 * j + 3];
       }
@@ -259,14 +317,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, const int* __restri
     if constexpr (kMode == kKeyPadding) {
       store_frag(acc, 1.f / l[0], 1.f / l[1], o + (seq_row + row) * HD + h * kHd, HD, c0);
       if ((lane & 3) == 0) {
-        lse_bh[row] = m[0] * kScale + logf(l[0]);
-        lse_bh[row + 8] = m[1] * kScale + logf(l[1]);
+        lse_bh[row] = m[0] * kSc + logf(l[0]);
+        lse_bh[row + 8] = m[1] * kSc + logf(l[1]);
       }
     } else {                                                    // a row that saw no key: zeros and -inf
       store_frag(acc, l[0] > 0.f ? 1.f / l[0] : 0.f, l[1] > 0.f ? 1.f / l[1] : 0.f, o + (seq_row + row) * HD + h * kHd, HD, c0);
       if ((lane & 3) == 0) {
-        lse_bh[row] = l[0] > 0.f ? m[0] * kScale + logf(l[0]) : -INFINITY;
-        lse_bh[row + 8] = l[1] > 0.f ? m[1] * kScale + logf(l[1]) : -INFINITY;
+        lse_bh[row] = l[0] > 0.f ? m[0] * kSc + logf(l[0]) : -INFINITY;
+        lse_bh[row + 8] = l[1] > 0.f ? m[1] * kSc + logf(l[1]) : -INFINITY;
       }
     }
   }
@@ -371,14 +429,18 @@ __device__ __forceinline__ void dkdv_consume_group(const BwdSmem& L, const int* 
 
 // dK, dV for one tile of 128 keys.  Fixed: K, V.  Ring: (Q, dO) tiles of 64 queries: all S / 64 of them (kKeyPadding),
 // or those inside the union of the key rows' intervals (kSegment, kCausal); with kGqa, those tiles of every query head
-// of the K/V head's group in turn (h is then the K/V head).
-template <int kMode, bool kGqa = false>
+// of the K/V head's group in turn (h is then the K/V head).  kBias: P recomputed with the relative bias.
+template <int kMode, bool kGqa = false, bool kBias = false>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
                      const int* __restrict__ mask, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
-                     __nv_bfloat16* __restrict__ dqkv, int Hkv) {
+                     __nv_bfloat16* __restrict__ dqkv, int Hkv, const float* __restrict__ table) {
+  static_assert(!kBias || (kMode != kKeyPadding && !kGqa), "the relative bias is a document-mode, multi-head instantiation");
+  constexpr float kSc = kBias ? 1.f : kScale;
+  constexpr float kSL = kSc * kLog2e;
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
+  float* tbl = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(L.fixed_bar) + 256);   // kBias
   const int3 tc = tile_coords<kMode, true>();
   const int kt = tc.x, h = tc.y, b = tc.z;
   const int HD = H * kHd;
@@ -410,6 +472,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
   }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 1 && lane == 0) bwd_init_barriers(L);
+  if constexpr (kBias) load_bias_table(tbl, table, h);
   __syncthreads();
 
   if (warp == 0) {
@@ -452,8 +515,9 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
       // key, 16-31: row key + 8), so the mask costs one register while the accumulators are live
       uint32_t vis = 0;
       if constexpr (kMode != kKeyPadding) {
-        const int2 kb0 = mask_interval<kMode, true>(mask, seq_row + key, key, S);
-        const int2 kb1 = mask_interval<kMode, true>(mask, seq_row + key + 8, key + 8, S);
+        const size_t mrow = kBias ? (size_t)(unsigned)(b * S + key) : seq_row + key;   // kBias: a 32-bit row (no spills)
+        const int2 kb0 = mask_interval<kMode, true>(mask, mrow, key, S);
+        const int2 kb1 = mask_interval<kMode, true>(mask, mrow + 8, key + 8, S);
         const int q0 = qt * 64 + c0;
         vis = frag_mask16(kb0.x - q0, kb0.y - q0) | (frag_mask16(kb1.x - q0, kb1.y - q0) << 16);
       }
@@ -465,12 +529,16 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
       mma_hd_n64(dpt, v_addr, do_addr);                         // dP^T = V dO^T
       wgmma_commit();
       wgmma_wait<0>();
+      uint32_t bias_t = 0;                                      // kBias: a 32-bit shared address, and the bias added column
+      if constexpr (kBias) bias_t = smem_u32(rel_bias_row<8, -1, 8>(tbl, key - (qt * 64 + c0)));   // by column: no spills
       uint32_t pa[16], dsa[16];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {                             // query columns 8 j + c0, + 1
         const int q = qt * 64 + 8 * j + c0;
-        const float2 lq = *reinterpret_cast<const float2*>(lse_bh + q);
-        const float2 dq = *reinterpret_cast<const float2*>(D_bh + q);
+        // kBias: lse and D at a 32-bit offset from the kernel parameters (B * H * S < 2^31), as in dkdv_consume_group
+        const int bhq = (b * H + h) * S + q;
+        const float2 lq = *reinterpret_cast<const float2*>(kBias ? lse + bhq : lse_bh + q);
+        const float2 dq = *reinterpret_cast<const float2*>(kBias ? Dsum + bhq : D_bh + q);
         float l0 = lq.x * kLog2e, l1 = lq.y * kLog2e;
         if constexpr (kMode != kKeyPadding) {                   // a query that saw no key (lse = -inf) gets P = 0, even
           l0 = lq.x == -INFINITY ? INFINITY : l0;               // where malformed bounds put it inside a key's interval
@@ -484,10 +552,14 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
           v00 = (vis >> (2 * j)) & 1u; v01 = (vis >> (2 * j + 1)) & 1u;
           v10 = (vis >> (16 + 2 * j)) & 1u; v11 = (vis >> (17 + 2 * j)) & 1u;
         }
-        const float p00 = v00 ? exp2f(st[4 * j] * kScaleLog2 - l0) : 0.f;
-        const float p01 = v01 ? exp2f(st[4 * j + 1] * kScaleLog2 - l1) : 0.f;
-        const float p10 = v10 ? exp2f(st[4 * j + 2] * kScaleLog2 - l0) : 0.f;
-        const float p11 = v11 ? exp2f(st[4 * j + 3] * kScaleLog2 - l1) : 0.f;
+        if constexpr (kBias) {
+          st[4 * j] += lds_f32(bias_t - 32 * j); st[4 * j + 1] += lds_f32(bias_t - 32 * j - 4);
+          st[4 * j + 2] += lds_f32(bias_t + 32 - 32 * j); st[4 * j + 3] += lds_f32(bias_t + 28 - 32 * j);
+        }
+        const float p00 = v00 ? exp2f(st[4 * j] * kSL - l0) : 0.f;
+        const float p01 = v01 ? exp2f(st[4 * j + 1] * kSL - l1) : 0.f;
+        const float p10 = v10 ? exp2f(st[4 * j + 2] * kSL - l0) : 0.f;
+        const float p11 = v11 ? exp2f(st[4 * j + 3] * kSL - l1) : 0.f;
         pa[2 * j] = pack_bf16x2(p00, p01);
         pa[2 * j + 1] = pack_bf16x2(p10, p11);
         dsa[2 * j] = pack_bf16x2(p00 * (dpt[4 * j] - dq.x), p01 * (dpt[4 * j + 1] - dq.y));
@@ -505,25 +577,40 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_c
       if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
     }
     __nv_bfloat16* krow = dqkv + (seq_row + key) * pitch + h * kHd;
-    store_frag(dk, kScale, kScale, krow + HD, pitch, c0);
+    store_frag(dk, kSc, kSc, krow + HD, pitch, c0);
     store_frag(dv, 1.f, 1.f, krow + 2 * HD, pitch, c0);
   }
 }
 
 // dQ for one tile of 128 queries.  Fixed: Q, dO.  Ring: (K, V) tiles of 64 keys below the length (kKeyPadding), or
 // inside the union of the query rows' intervals (kSegment, kCausal).  kGqa: K / V from the query head's K/V head.
-template <int kMode, bool kGqa = false>
+//
+// kBias: P recomputed with the relative bias, and this CTA's share of the bias gradient: dtable_part[b, qt, h, c] =
+// the sum of fp32 dS over its visible pairs at clamped distance c - 128, with no atomics.  A thread's 32 dS values of a
+// 128 x 64 tile lie on 18 diagonals (slot 2 m + e: distance kt * 64 + c0 - row + 8 (m - 1) + e), which it folds in
+// registers.  Slots at distance beyond +-128, and whole tiles beyond it, go to two running sums per thread (columns 0
+// and 256).  For the other tiles the slots go through shared memory, where the owner of column c (consumer thread c - 1)
+// adds the up to 64 slots of its diagonal in a fixed order to a register.  The tiles are walked in key order, so every
+// sum has one fixed order.
+template <int kMode, bool kGqa = false, bool kBias = false>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_constant__ CUtensorMap map_do,
                    const int* __restrict__ mask, int S, int H, const float* __restrict__ lse, const float* __restrict__ Dsum,
-                   __nv_bfloat16* __restrict__ dqkv, int Hkv) {
+                   __nv_bfloat16* __restrict__ dqkv, int Hkv, const float* __restrict__ table, float* __restrict__ dtable_part) {
+  static_assert(!kBias || (kMode != kKeyPadding && !kGqa), "the relative bias is a document-mode, multi-head instantiation");
+  constexpr float kSc = kBias ? 1.f : kScale;
+  constexpr float kSL = kSc * kLog2e;
   extern __shared__ uint8_t smem_raw[];
   const BwdSmem L = bwd_smem(smem_raw);
+  float* tbl = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(L.fixed_bar) + 256);   // kBias: table, far-sum scratch,
+  float* far_red = tbl + kFarRed;                                                           // then the two fold buffers
+  float* fold = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(tbl) + kBiasTable);
   const int3 tc = tile_coords<kMode, false>();
   const int qt = tc.x, h = tc.y, b = tc.z;
   const int HD = H * kHd;
   const size_t pitch = kGqa ? (size_t)(H + 2 * Hkv) * kHd : (size_t)3 * HD;
   const size_t seq_row = (size_t)b * S;
+  float* part_out = kBias ? dtable_part + (((size_t)b * (S / 128) + qt) * H + h) * kRelCols : nullptr;
   int len = 0, kt0 = 0, kt_end = 0;
   bool hidden;
   if constexpr (kMode == kKeyPadding) {
@@ -537,11 +624,14 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
   }
   if (hidden) {
     zero_rows(dqkv + h * kHd, pitch, seq_row + qt * 128, 128);
+    if constexpr (kBias)
+      for (int i = threadIdx.x; i < kRelCols; i += blockDim.x) part_out[i] = 0.f;
     return;
   }
   const int n_kt = kMode == kKeyPadding ? (len + 63) / 64 : kt_end - kt0;   // key tiles kt0 .. kt0 + n_kt - 1
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 1 && lane == 0) bwd_init_barriers(L);
+  if constexpr (kBias) load_bias_table(tbl, table, h);
   __syncthreads();
 
   if (warp == 0) {
@@ -574,6 +664,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
     float dq[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+    const int u = threadIdx.x - 128;                            // kBias: consumer thread index; owns column u + 1 (u < 255)
+    float col_sum = 0.f, far_lo = 0.f, far_hi = 0.f;            // kBias: column u + 1, columns 0 and 256
     mbar_wait(L.fixed_bar, 0);
     int stage = 0;
     uint32_t phase = 0;
@@ -586,6 +678,11 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
       mma_hd_n64(dp, do_addr, v_addr);                          // dP = dO V^T
       wgmma_commit();
       wgmma_wait<0>();
+      const int tile_rel = kt * 64 - qt * 128;                  // distance of the tile's key 0 from its query 0
+      if constexpr (kBias) add_rel_bias<8, 1, -8>(s, tbl, tile_rel + c0 - (wg * 64 + r0));
+      float slot[18];
+#pragma unroll
+      for (int t = 0; t < 18; ++t) slot[t] = 0.f;
       uint32_t dsa[16];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -598,23 +695,79 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_qkv, const __grid_con
           v00 = inside(k0, qb0); v01 = inside(k0 + 1, qb0);
           v10 = inside(k0, qb1); v11 = inside(k0 + 1, qb1);
         }
-        const float p00 = v00 ? exp2f(s[4 * j] * kScaleLog2 - l0) : 0.f;
-        const float p01 = v01 ? exp2f(s[4 * j + 1] * kScaleLog2 - l0) : 0.f;
-        const float p10 = v10 ? exp2f(s[4 * j + 2] * kScaleLog2 - l1) : 0.f;
-        const float p11 = v11 ? exp2f(s[4 * j + 3] * kScaleLog2 - l1) : 0.f;
-        dsa[2 * j] = pack_bf16x2(p00 * (dp[4 * j] - d0), p01 * (dp[4 * j + 1] - d0));
-        dsa[2 * j + 1] = pack_bf16x2(p10 * (dp[4 * j + 2] - d1), p11 * (dp[4 * j + 3] - d1));
+        const float p00 = v00 ? exp2f(s[4 * j] * kSL - l0) : 0.f;
+        const float p01 = v01 ? exp2f(s[4 * j + 1] * kSL - l0) : 0.f;
+        const float p10 = v10 ? exp2f(s[4 * j + 2] * kSL - l1) : 0.f;
+        const float p11 = v11 ? exp2f(s[4 * j + 3] * kSL - l1) : 0.f;
+        if constexpr (kBias) {
+          const float ds00 = p00 * (dp[4 * j] - d0), ds01 = p01 * (dp[4 * j + 1] - d0);
+          const float ds10 = p10 * (dp[4 * j + 2] - d1), ds11 = p11 * (dp[4 * j + 3] - d1);
+          dsa[2 * j] = pack_bf16x2(ds00, ds01);
+          dsa[2 * j + 1] = pack_bf16x2(ds10, ds11);
+          slot[2 * j + 2] += ds00; slot[2 * j + 3] += ds01;     // row r0: m = j + 1
+          slot[2 * j] += ds10; slot[2 * j + 1] += ds11;         // row r0 + 8: m = j
+        } else {
+          dsa[2 * j] = pack_bf16x2(p00 * (dp[4 * j] - d0), p01 * (dp[4 * j + 1] - d0));
+          dsa[2 * j + 1] = pack_bf16x2(p10 * (dp[4 * j + 2] - d1), p11 * (dp[4 * j + 3] - d1));
+        }
       }
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) wgmma_n64_rs<1>(dq, dsa + 4 * kk, desc_mn(k_addr + kk * kStepMN), 1u);  // dQ += dS K
       wgmma_commit();
+      if constexpr (kBias) {
+        if (tile_rel + 63 <= -kRelMax) {                        // the whole tile lies at distance <= -128 (CTA-uniform)
+#pragma unroll
+          for (int t = 0; t < 18; ++t) far_lo += slot[t];
+        } else if (tile_rel - 127 >= kRelMax) {                 // ... or >= 128
+#pragma unroll
+          for (int t = 0; t < 18; ++t) far_hi += slot[t];
+        } else {
+          float* buf = fold + (kt & 1) * 256 * kPartStride;
+          const int d_slot0 = tile_rel + c0 - (wg * 64 + r0) - 8;
+#pragma unroll
+          for (int t = 0; t < 18; ++t) {
+            const int d = d_slot0 + 8 * (t >> 1) + (t & 1);
+            if (d <= -kRelMax) far_lo += slot[t];
+            else if (d >= kRelMax) far_hi += slot[t];
+            buf[u * kPartStride + t] = slot[t];
+          }
+          asm volatile("bar.sync 1, 256;" ::: "memory");        // the consumer warpgroups' slots are in buf
+          // Column u + 1 is tile diagonal dl = key - row (tile-local).  The thread group of warp w, quad q (rows
+          // 16 w + q and 16 w + q + 8) holds it at kk = 16 w + q + dl + 8 if that lies in [0, 72): lane 4 q + (kk & 7) / 2,
+          // slot 2 (kk >> 3) + (kk & 1).  Only the quads in that range are visited, in increasing (w, q).
+          const int dl = u - (kRelMax - 1) - tile_rel;
+          if (u < 2 * kRelMax - 1 && dl >= -127 && dl <= 63) {
+            for (int w = 0; w < 8; ++w) {
+              const int kk0 = 16 * w + dl + 8;
+              for (int kk = max(kk0, 0); kk < min(kk0 + 8, 72); ++kk)
+                col_sum += buf[(32 * w + 4 * (kk - kk0) + ((kk & 7) >> 1)) * kPartStride + 2 * (kk >> 3) + (kk & 1)];
+            }
+          }
+        }
+      }
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(&L.empty_bar[stage]);
       if (++stage == kBwdStages) { stage = 0; phase ^= 1; }
     }
-    store_frag(dq, kScale, kScale, dqkv + (seq_row + row) * pitch + h * kHd, pitch, c0);
+    store_frag(dq, kSc, kSc, dqkv + (seq_row + row) * pitch + h * kHd, pitch, c0);
+    if constexpr (kBias) {
+      if (u < 2 * kRelMax - 1) part_out[u + 1] = col_sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        far_lo += __shfl_xor_sync(0xffffffffu, far_lo, o);
+        far_hi += __shfl_xor_sync(0xffffffffu, far_hi, o);
+      }
+      if (lane == 0) { far_red[warp - 4] = far_lo; far_red[8 + warp - 4] = far_hi; }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (u == 0) {
+        float lo = 0.f, hi = 0.f;
+        for (int w = 0; w < 8; ++w) { lo += far_red[w]; hi += far_red[8 + w]; }
+        part_out[0] = lo;
+        part_out[2 * kRelMax] = hi;
+      }
+    }
   }
 }
 
@@ -1100,7 +1253,7 @@ void attention_fwd(const char* who, const void* qkv, const int* mask, int B, int
   static std::atomic<unsigned long long> configured{0};
   ensure_max_dynamic_smem(attn_fwd_kernel<kMode, kGqa>, kFwdSmem, configured);
   attn_fwd_kernel<kMode, kGqa><<<dim3(S / 128, heads, B), kThreads, kFwdSmem, s>>>(
-      map_qkv, mask, S, heads, reinterpret_cast<__nv_bfloat16*>(o), lse, kv_heads);
+      map_qkv, mask, S, heads, reinterpret_cast<__nv_bfloat16*>(o), lse, kv_heads, nullptr);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 
@@ -1121,14 +1274,122 @@ void attention_bwd(const char* who, const void* dout, const void* qkv, const voi
   ensure_max_dynamic_smem(attn_bwd_dq_kernel<kMode, kGqa>, kBwdSmem, configured_dq);
   // dK / dV: one CTA per (key tile, K/V head, batch)
   attn_bwd_dkdv_kernel<kMode, kGqa><<<dim3(S / 128, kGqa ? kv_heads : heads, B), kThreads, kBwdSmem, s>>>(
-      map_qkv, map_do, mask, S, heads, lse, dsum, dq, kv_heads);
+      map_qkv, map_do, mask, S, heads, lse, dsum, dq, kv_heads, nullptr);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
   attn_bwd_dq_kernel<kMode, kGqa><<<dim3(S / 128, heads, B), kThreads, kBwdSmem, s>>>(
-      map_qkv, map_do, mask, S, heads, lse, dsum, dq, kv_heads);
+      map_qkv, map_do, mask, S, heads, lse, dsum, dq, kv_heads, nullptr, nullptr);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+// ---- relative position bias (T5) ----
+constexpr int kRelFwdSmem = kFwdSmem + kBiasTable;
+constexpr int kRelDkdvSmem = kBwdSmem + kBiasTable;
+constexpr int kRelDqSmem = kBwdSmem + kBiasTable + kPartBytes;
+
+// dtable[h, c] = sum over (b, query tile) of part[b, qt, h, c], in that order
+__global__ void rel_bias_finish_kernel(const float* __restrict__ part, int n, int H, float* __restrict__ dtable) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;          // h * 257 + c
+  if (i >= H * kRelCols) return;
+  float acc = 0.f;
+  for (int k = 0; k < n; ++k) acc += part[(size_t)k * H * kRelCols + i];
+  dtable[i] = acc;
+}
+
+// table[h, c] = weight[bucket[c], h]: weight [num_buckets, H] fp32 or bf16
+template <typename T>
+__global__ void rel_table_gather_kernel(const T* __restrict__ weight, const int* __restrict__ bucket, int H, float* __restrict__ table) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= H * kRelCols) return;
+  const int h = i / kRelCols, c = i - h * kRelCols;
+  table[i] = static_cast<float>(weight[(size_t)__ldg(bucket + c) * H + h]);
+}
+
+// dweight[k, h] = sum of dtable[h, c] over the columns c of bucket k, in increasing c (one writer per element)
+template <typename T>
+__global__ void rel_table_fold_kernel(const float* __restrict__ dtable, const int* __restrict__ bucket, int num_buckets, int H,
+                                      T* __restrict__ dweight) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;          // k * H + h
+  if (i >= num_buckets * H) return;
+  const int k = i / H, h = i - k * H;
+  float acc = 0.f;
+  for (int c = 0; c < kRelCols; ++c)
+    if (__ldg(bucket + c) == k) acc += dtable[(size_t)h * kRelCols + c];
+  dweight[i] = static_cast<T>(acc);
+}
+
+template <int kMode>
+void relative_fwd(const char* who, const void* qkv, const int* bounds, const float* table, int B, int S, int heads, void* o,
+                  float* lse, cudaStream_t s) {
+  check_shape(who, B, S, heads, heads);
+  const CUtensorMap map_qkv = rows_map(qkv, B * S, 3 * heads * kHd);
+  static std::atomic<unsigned long long> configured{0};
+  ensure_max_dynamic_smem(attn_fwd_kernel<kMode, false, true>, kRelFwdSmem, configured);
+  attn_fwd_kernel<kMode, false, true><<<dim3(S / 128, heads, B), kThreads, kRelFwdSmem, s>>>(
+      map_qkv, bounds, S, heads, reinterpret_cast<__nv_bfloat16*>(o), lse, heads, table);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+template <int kMode>
+void relative_bwd(const char* who, const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds,
+                  const float* table, int B, int S, int heads, float* dsum, float* dtable_part, void* dqkv, float* dtable,
+                  cudaStream_t s) {
+  check_shape(who, B, S, heads, heads);
+  const int rows = B * S;
+  const long long items = (long long)rows * heads * 8;
+  attn_bwd_dot_kernel<<<ceil_div(items, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(dout),
+                                                           reinterpret_cast<const __nv_bfloat16*>(o), rows, S, heads, dsum);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  const CUtensorMap map_qkv = rows_map(qkv, rows, 3 * heads * kHd);
+  const CUtensorMap map_do = rows_map(dout, rows, heads * kHd);
+  auto* dq = reinterpret_cast<__nv_bfloat16*>(dqkv);
+  static std::atomic<unsigned long long> configured_dkdv{0}, configured_dq{0};
+  ensure_max_dynamic_smem(attn_bwd_dkdv_kernel<kMode, false, true>, kRelDkdvSmem, configured_dkdv);
+  ensure_max_dynamic_smem(attn_bwd_dq_kernel<kMode, false, true>, kRelDqSmem, configured_dq);
+  attn_bwd_dkdv_kernel<kMode, false, true><<<dim3(S / 128, heads, B), kThreads, kRelDkdvSmem, s>>>(
+      map_qkv, map_do, bounds, S, heads, lse, dsum, dq, heads, table);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  attn_bwd_dq_kernel<kMode, false, true><<<dim3(S / 128, heads, B), kThreads, kRelDqSmem, s>>>(
+      map_qkv, map_do, bounds, S, heads, lse, dsum, dq, heads, table, dtable_part);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+  rel_bias_finish_kernel<<<ceil_div((long long)heads * kRelCols, 256), 256, 0, s>>>(dtable_part, B * (S / 128), heads, dtable);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
 }
 
 }  // namespace
+
+void launch_relative_attention_fwd(const void* qkv, const int* bounds, const float* table, int B, int S, int heads, bool causal,
+                                   void* o, float* lse, cudaStream_t s) {
+  if (causal) relative_fwd<kCausal>("relative_attention_fwd", qkv, bounds, table, B, S, heads, o, lse, s);
+  else relative_fwd<kSegment>("relative_attention_fwd", qkv, bounds, table, B, S, heads, o, lse, s);
+}
+
+void launch_relative_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds,
+                                   const float* table, int B, int S, int heads, bool causal, float* dsum, float* dtable_part,
+                                   void* dqkv, float* dtable, cudaStream_t s) {
+  if (causal)
+    relative_bwd<kCausal>("relative_attention_bwd", dout, qkv, o, lse, bounds, table, B, S, heads, dsum, dtable_part, dqkv, dtable, s);
+  else
+    relative_bwd<kSegment>("relative_attention_bwd", dout, qkv, o, lse, bounds, table, B, S, heads, dsum, dtable_part, dqkv, dtable, s);
+}
+
+void launch_relative_table_fwd(const void* weight, bool bf16, const int* bucket, int heads, float* table, cudaStream_t s) {
+  const int n = heads * kRelCols;
+  if (bf16)
+    rel_table_gather_kernel<<<ceil_div(n, 256), 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(weight), bucket, heads, table);
+  else
+    rel_table_gather_kernel<<<ceil_div(n, 256), 256, 0, s>>>(reinterpret_cast<const float*>(weight), bucket, heads, table);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void launch_relative_table_bwd(const float* dtable, const int* bucket, int num_buckets, int heads, bool bf16, void* dweight,
+                               cudaStream_t s) {
+  const int n = num_buckets * heads;
+  if (bf16)
+    rel_table_fold_kernel<<<ceil_div(n, 256), 256, 0, s>>>(dtable, bucket, num_buckets, heads, reinterpret_cast<__nv_bfloat16*>(dweight));
+  else
+    rel_table_fold_kernel<<<ceil_div(n, 256), 256, 0, s>>>(dtable, bucket, num_buckets, heads, reinterpret_cast<float*>(dweight));
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
 
 void launch_causal_attention_d128_fwd(const void* qkv, const int* bounds, int B, int S, int heads, int kv_heads, void* o, float* lse, cudaStream_t s) {
   check_shape("causal_attention_d128_fwd", B, S, heads, kv_heads, kHd128);

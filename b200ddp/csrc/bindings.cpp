@@ -170,9 +170,10 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip and _C.cross namespaces of static entry points
+// the types behind the _C.clip, _C.cross and _C.t5 namespaces of static entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
+struct T5Namespace {};
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
   CommCtx c;
@@ -417,6 +418,14 @@ std::tuple<int, int, int> cross_args(Args& args, const at::Tensor& q, const at::
   args("q", q, {kBF16}, {B * Sq, hidden}, kContiguous, 16)("kv", kv, {kBF16}, {kAny, 2 * hidden}, kContiguous, 16);
   args.expect(kv.size(0) % B == 0 && kv.size(0) >= B, "kv", "bf16 [B*Sk, 2*heads*64] with Sk >= 1", kv);
   return std::make_tuple((int)B, (int)Sq, (int)(kv.size(0) / B));
+}
+
+// checks qkv, bounds and table of a relative-bias attention binding (multi-head, head dim 64); returns (B, S)
+std::pair<int, int> relative_args(Args& args, const at::Tensor& qkv, const at::Tensor& bounds, const at::Tensor& table, int heads) {
+  if (heads < 1) args.fail("heads", ">= 1", std::to_string(heads));
+  const auto [B, S] = attn_args(args, qkv, bounds, Mask::kBounds, heads, heads, 64);
+  args("table", table, {kF32}, {heads, 257});
+  return {B, S};
 }
 
 }  // namespace
@@ -1678,4 +1687,61 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                kv_bounds.data_ptr<int>(), B, Sq, Sk, heads, dsum.data_ptr<float>(), dq.data_ptr(), dkv.data_ptr(), cur_stream());
     return std::make_tuple(dq, dkv);
   }, py::arg("dout"), py::arg("q"), py::arg("kv"), py::arg("o"), py::arg("lse"), py::arg("q_bounds"), py::arg("kv_bounds"), py::arg("heads"));
+
+  // ---- T5's relative position bias (attention.cu): document attention with a learned bias table, head dim 64 ---------
+  // _C.t5 is a namespace of static entry points like _C.cross; its contract rows are in tests/test_t5_bindings_cpu.py.
+  // qkv bf16 [B*S, 3*heads*64], bounds int32 [B, S, 2] (segment, or causal inside documents), table fp32 [heads, 257]
+  // (launch_relative_attention_fwd); S a multiple of 128 (the launcher checks it).
+  py::class_<T5Namespace> t5(m, "t5", "T5's relative position bias inside the attention kernels (attention.cu)");
+  // (o bf16 [B*S, heads*64], lse fp32 [B, heads, S])
+  t5.def_static("relative_attention_fwd", [](at::Tensor qkv, at::Tensor bounds, at::Tensor table, int heads, bool causal) {
+    Args args("relative_attention_fwd");
+    const auto [B, S] = relative_args(args, qkv, bounds, table, heads);
+    args.device();
+    at::Tensor o = at::empty({qkv.size(0), (int64_t)heads * 64}, qkv.options());
+    at::Tensor lse = at::empty({B, heads, S}, qkv.options().dtype(kF32));
+    launch_relative_attention_fwd(qkv.data_ptr(), bounds.data_ptr<int>(), table.data_ptr<float>(), B, S, heads, causal, o.data_ptr(),
+                                  lse.data_ptr<float>(), cur_stream());
+    return std::make_tuple(o, lse);
+  }, py::arg("qkv"), py::arg("bounds"), py::arg("table"), py::arg("heads"), py::arg("causal"));
+  // (dqkv like qkv, dtable fp32 [heads, 257])
+  t5.def_static("relative_attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor bounds,
+                                             at::Tensor table, int heads, bool causal) {
+    Args args("relative_attention_bwd");
+    const auto [B, S] = relative_args(args, qkv, bounds, table, heads);
+    args("dout", dout, {kBF16}, numel(qkv.size(0) * heads * 64), kContiguous, 16)("o", o, {kBF16}, numel(qkv.size(0) * heads * 64), kContiguous, 16);
+    args("lse", lse, {kF32}, numel((int64_t)B * heads * S), kContiguous, 8);
+    args.device();
+    at::Tensor dqkv = at::empty_like(qkv);
+    at::Tensor dtable = at::empty({heads, 257}, qkv.options().dtype(kF32));
+    at::Tensor dsum = at::empty({B, heads, S}, qkv.options().dtype(kF32));
+    at::Tensor part = at::empty({B, S / 128, heads, 257}, qkv.options().dtype(kF32));
+    launch_relative_attention_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), bounds.data_ptr<int>(),
+                                  table.data_ptr<float>(), B, S, heads, causal, dsum.data_ptr<float>(), part.data_ptr<float>(),
+                                  dqkv.data_ptr(), dtable.data_ptr<float>(), cur_stream());
+    return std::make_tuple(dqkv, dtable);
+  }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("bounds"), py::arg("table"), py::arg("heads"), py::arg("causal"));
+  // table fp32 [H, 257] = weight[bucket[c], h]: weight fp32 or bf16 [num_buckets, H], bucket int32 [257] in [0, num_buckets)
+  t5.def_static("relative_table_fwd", [](at::Tensor weight, at::Tensor bucket) {
+    Args args("relative_table_fwd");
+    args("weight", weight, {kF32, kBF16}, {kAny, kAny})("bucket", bucket, {kI32}, {257});
+    args.expect(weight.size(0) >= 1 && weight.size(1) >= 1, "weight", "[num_buckets, heads] with both >= 1", weight);
+    args.device();
+    at::Tensor table = at::empty({weight.size(1), 257}, weight.options().dtype(kF32));
+    launch_relative_table_fwd(weight.data_ptr(), weight.scalar_type() == kBF16, bucket.data_ptr<int>(), (int)weight.size(1),
+                              table.data_ptr<float>(), cur_stream());
+    return table;
+  }, py::arg("weight"), py::arg("bucket"));
+  // d weight like weight: the sum of dtable[h, c] over the c of each bucket, in increasing c
+  t5.def_static("relative_table_bwd", [](at::Tensor dtable, at::Tensor bucket, at::Tensor weight) {
+    Args args("relative_table_bwd");
+    args("weight", weight, {kF32, kBF16}, {kAny, kAny});
+    args.expect(weight.size(0) >= 1 && weight.size(1) >= 1, "weight", "[num_buckets, heads] with both >= 1", weight);
+    args("dtable", dtable, {kF32}, {weight.size(1), 257})("bucket", bucket, {kI32}, {257});
+    args.device();
+    at::Tensor dweight = at::empty_like(weight, at::MemoryFormat::Contiguous);
+    launch_relative_table_bwd(dtable.data_ptr<float>(), bucket.data_ptr<int>(), (int)weight.size(0), (int)weight.size(1),
+                              weight.scalar_type() == kBF16, dweight.data_ptr(), cur_stream());
+    return dweight;
+  }, py::arg("dtable"), py::arg("bucket"), py::arg("weight"));
 }

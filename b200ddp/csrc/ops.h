@@ -270,6 +270,22 @@ void launch_l2norm_bwd(const void* du, const void* x, const float* rnorm, int B,
 void launch_contrastive_xent(const float* z_img, const float* z_txt, const float* logit_scale, int B, int N, int offset, void* dz_img,
                              void* dz_txt, float* row_partials, float* loss, float* dscale, cudaStream_t s);
 
+// ---------------- T5 relative position bias (attention.cu) ------------------------
+// The segment (causal = false) or causal attention of launch_packed_attention_* / launch_causal_attention_*, multi-head
+// at head dim 64, with table fp32 [heads, 257] added to the unscaled scores: score(i, j) = q_i . k_j + table[h, clamp(j - i,
+// -128, 128) + 128].  lse is that of the biased scores.  The backward also writes dtable fp32 [heads, 257], the sum of dS
+// over the pairs at each clamped distance, through dtable_part fp32 [B, S / 128, heads, 257]; no atomics.
+void launch_relative_attention_fwd(const void* qkv, const int* bounds, const float* table, int B, int S, int heads, bool causal,
+                                   void* o, float* lse, cudaStream_t s);
+void launch_relative_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const int* bounds,
+                                   const float* table, int B, int S, int heads, bool causal, float* dsum, float* dtable_part,
+                                   void* dqkv, float* dtable, cudaStream_t s);
+// table fp32 [heads, 257] = weight[bucket[c], h] (weight [num_buckets, heads], fp32 or bf16; bucket int32 [257]), and its
+// backward: dweight[k, h] = the sum of dtable[h, c] over the c with bucket[c] == k, in increasing c
+void launch_relative_table_fwd(const void* weight, bool bf16, const int* bucket, int heads, float* table, cudaStream_t s);
+void launch_relative_table_bwd(const float* dtable, const int* bucket, int num_buckets, int heads, bool bf16, void* dweight,
+                               cudaStream_t s);
+
 // ---------------- cross-attention on wgmma, head dim 64 (cross_attention.cu) ------------------------
 // q bf16 [B*Sq, heads*64], kv bf16 [B*Sk, 2*heads*64] (key block | value block), o bf16 [B*Sq, heads*64], lse fp32
 // [B, heads, Sq]; q_bounds int32 [B*Sq, 2] (the keys each query sees), kv_bounds int32 [B*Sk, 2] (the queries that see

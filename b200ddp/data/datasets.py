@@ -241,6 +241,147 @@ class SyntheticTokens(Dataset):
         torch.index_select(self.Y, 0, indices, out=outs[1])
 
 
+class SyntheticSpanCorruption(Dataset):
+    """Source / target pairs for T5's span-corruption objective (seeded): ``X`` source ids [seq_len], right-padded with
+    ``PAD_ID``; ``Y`` labels [target_width], the target ids, -100 at padding.
+
+    A document is n text tokens from [3, 32000) (T5's special ids are 0 to 2; its sentinels 32099, 32098, ... sit above
+    the text vocabulary).  ``round(0.15 n)`` of them (at least 1, at most n - 1) are noise, in ``max(round(noise / 3),
+    1)`` spans; noise and kept tokens are each split into that many non-empty runs by a random segmentation, and the
+    runs alternate kept, noise, kept, noise ... as in T5's ``random_spans_noise_mask``.  The source is ``start_id`` +
+    the kept runs with each noise span replaced by the next sentinel + ``EOS_ID``; the target is ``start_id`` + (sentinel,
+    its span's tokens) for every span + the next sentinel + ``EOS_ID``.  ``start_id`` (2, <unk>) never occurs in the text,
+    so packed documents can be found on both sides.
+
+    Sources are ``seq_len`` tokens long (the longest n whose source fits), or uniform in [``min_len``, ``seq_len``].
+    Targets are right-padded to ``target_width(seq_len)``: the longest target a source of ``seq_len`` tokens can have,
+    rounded up to 128 (128 at 512, 256 at 1024).  ``pack=True`` places the pairs first-fit decreasing by source length
+    (ties in pair order) into the first row where both the source and the target still fit: short documents have a
+    larger target-to-source ratio, so the source alone does not bound the target row.  ``bos_token_id`` is then
+    ``start_id``, and ``doc_ids`` / ``doc_lengths`` list each row's pairs and source lengths.  ``lengths`` holds each
+    row's filled source length."""
+
+    PAD_ID = 0
+    EOS_ID = 1
+    TEXT_END = 32000
+    FIRST_SENTINEL = 32099
+
+    def __init__(self, samples: int = 512, seq_len: int = 512, vocab: int = 32128, start_id: int = 2, min_len: int | None = None,
+                 pack: bool = False, noise_density: float = 0.15, mean_span: float = 3.0, seed: int = 1234):
+        if min_len is not None and not 4 <= min_len <= seq_len:
+            raise ValueError(f"SyntheticSpanCorruption: min_len must lie in [4, seq_len = {seq_len}], got {min_len}")
+        if vocab <= self.FIRST_SENTINEL or not 1 < start_id < 3:
+            raise ValueError(f"SyntheticSpanCorruption: needs T5's vocabulary (> {self.FIRST_SENTINEL} ids) and start_id 2, "
+                             f"got vocab {vocab} and start_id {start_id}")
+        self.noise_density, self.mean_span = noise_density, mean_span
+        g = torch.Generator().manual_seed(seed)
+        n = int(samples)
+        src_lens = torch.full((n,), seq_len) if min_len is None else torch.randint(min_len, seq_len + 1, (n,), generator=g)
+        self.target_width = self.target_width_for(seq_len, noise_density, mean_span)
+        sources, targets = [], []
+        for L in src_lens.tolist():
+            text = torch.randint(3, self.TEXT_END, (self._text_len(L),), generator=g)
+            s, t = self._corrupt(text, g)
+            sources.append(torch.cat([torch.tensor([start_id]), s, torch.tensor([self.EOS_ID])]))
+            targets.append(torch.cat([torch.tensor([start_id]), t, torch.tensor([self.EOS_ID])]))
+        self.pad_token_id = self.PAD_ID
+        self.bos_token_id = None
+        self.doc_ids = self.doc_lengths = None
+        slen = [len(x) for x in sources]
+        tlen = [len(y) for y in targets]
+        if pack:
+            rows, free_s, free_t = [], [], []
+            for i in sorted(range(n), key=lambda i: (-slen[i], i)):    # first-fit decreasing by source length
+                r = next((r for r in range(len(rows)) if free_s[r] >= slen[i] and free_t[r] >= tlen[i]), len(rows))
+                if r == len(rows):
+                    rows.append([])
+                    free_s.append(seq_len)
+                    free_t.append(self.target_width)
+                rows[r].append(i)
+                free_s[r] -= slen[i]
+                free_t[r] -= tlen[i]
+            self.doc_ids = rows
+            self.doc_lengths = [[slen[i] for i in docs] for docs in rows]
+            self.bos_token_id = start_id
+        else:
+            rows = [[i] for i in range(n)]
+        self.samples = len(rows)
+        self.X = torch.full((self.samples, seq_len), self.PAD_ID, dtype=torch.long)
+        self.Y = torch.full((self.samples, self.target_width), -100, dtype=torch.long)
+        for r, docs in enumerate(rows):
+            a = b = 0
+            for i in docs:
+                self.X[r, a:a + slen[i]] = sources[i]
+                self.Y[r, b:b + tlen[i]] = targets[i]
+                a, b = a + slen[i], b + tlen[i]
+        self.lengths = (self.X != self.PAD_ID).sum(1)
+
+    @staticmethod
+    def _spans(n: int, density: float, mean_span: float):
+        noise = min(max(int(round(n * density)), 1), n - 1)
+        return noise, max(int(round(noise / mean_span)), 1)
+
+    @classmethod
+    def _lens(cls, n: int, density: float = 0.15, mean_span: float = 3.0):
+        """(source, target) lengths of a document of n text tokens, start and end ids included."""
+        noise, spans = cls._spans(n, density, mean_span)
+        return (n - noise) + spans + 2, noise + spans + 3
+
+    def _text_len(self, src_len: int) -> int:
+        """The longest text whose source fits in src_len tokens."""
+        n = 2
+        while self._lens(n + 1, self.noise_density, self.mean_span)[0] <= src_len:
+            n += 1
+        return n
+
+    @classmethod
+    def target_width_for(cls, seq_len: int, density: float = 0.15, mean_span: float = 3.0) -> int:
+        """Label columns for sources of up to seq_len tokens: the longest target, rounded up to 128."""
+        longest, n = 0, 2
+        while cls._lens(n, density, mean_span)[0] <= seq_len:
+            longest = max(longest, cls._lens(n, density, mean_span)[1])
+            n += 1
+        return (longest + 127) // 128 * 128
+
+    @staticmethod
+    def _segment(items: int, segments: int, g: torch.Generator) -> list:
+        """items split into `segments` non-empty runs at random (T5's random_segmentation)."""
+        cuts = (torch.randperm(items - 1, generator=g)[:segments - 1] + 1).sort().values.tolist()
+        edges = [0] + cuts + [items]
+        return [b - a for a, b in zip(edges[:-1], edges[1:])]
+
+    def _corrupt(self, text: torch.Tensor, g: torch.Generator):
+        """(source body, target body) of one document: kept runs and sentinels; sentinels and noise runs, then the next
+        sentinel."""
+        n = text.numel()
+        noise, spans = self._spans(n, self.noise_density, self.mean_span)
+        kept_runs = self._segment(n - noise, spans, g)
+        noise_runs = self._segment(noise, spans, g)
+        src, tgt, at = [], [], 0
+        for k in range(spans):
+            sentinel = torch.tensor([self.FIRST_SENTINEL - k])
+            src += [text[at:at + kept_runs[k]], sentinel]
+            at += kept_runs[k]
+            tgt += [sentinel, text[at:at + noise_runs[k]]]
+            at += noise_runs[k]
+        tgt.append(torch.tensor([self.FIRST_SENTINEL - spans]))
+        return torch.cat(src), torch.cat(tgt)
+
+    def __len__(self) -> int:
+        return self.samples
+
+    def __getitem__(self, index):
+        return self.X[index], self.Y[index]
+
+    def batch(self, indices: torch.Tensor):
+        return self.X.index_select(0, indices), self.Y.index_select(0, indices)
+
+    def batch_into(self, indices: torch.Tensor, outs) -> None:
+        """Gather straight into caller-owned (pinned) buffers: one pass over the data."""
+        torch.index_select(self.X, 0, indices, out=outs[0])
+        torch.index_select(self.Y, 0, indices, out=outs[1])
+
+
 class SyntheticDenoising(Dataset):
     """Source / target pairs for BART's text-infilling objective (seeded): ``X`` source ids [seq_len], right-padded with
     ``PAD_ID``; ``Y`` labels [seq_len], the target ids, -100 at padding.

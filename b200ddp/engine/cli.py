@@ -315,7 +315,7 @@ def check_contrastive_args(args) -> None:
 
 
 def check_seq2seq_args(args) -> None:
-    """An encoder-decoder (BART) trains on source / target pairs whose sources are always right-padded, so on the GPU its
+    """An encoder-decoder (BART, T5) trains on source / target pairs whose sources are always right-padded, so on the GPU its
     attention always runs on the bf16 document kernels: it needs ``--fp16`` and ``--seq_len`` a multiple of 128 there.
     ``--seq_len`` bounds both sides (the position table's check covers it)."""
     if not model_entry(args.model).seq2seq:

@@ -22,8 +22,9 @@ import torch.distributed as dist
 from tqdm import tqdm
 from tqdm.auto import trange
 
-from ..data import BatchLoader, DevicePrefetcher, FooDataset, SyntheticDenoising, SyntheticImageNet, SyntheticImageText, SyntheticTokens
-from ..models import model_entry
+from ..data import (BatchLoader, DevicePrefetcher, FooDataset, SyntheticDenoising, SyntheticImageNet, SyntheticImageText, SyntheticSpanCorruption,
+                    SyntheticTokens)
+from ..models import T5Config, model_entry
 from ..ops import ClipLoss, CrossEntropyLoss, MSELoss
 from ..optim import FusedAdamW, FusedSGD, get_linear_schedule_with_warmup, weight_decay_groups
 from ..parallel import DataParallel, DistributedDataParallel, ShardedSampler
@@ -58,6 +59,9 @@ def build_dataset(args):
     if entry.kind == "image":
         dense = loss_kind(args) == "mse"
         return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
+    if entry.seq2seq and isinstance(entry.config, T5Config):
+        return SyntheticSpanCorruption(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=entry.config.vocab_size,
+                                       start_id=entry.start_id, min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)))
     if entry.seq2seq:
         return SyntheticDenoising(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=entry.config.vocab_size,
                                   start_id=entry.start_id, min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)))

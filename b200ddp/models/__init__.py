@@ -15,6 +15,7 @@ from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, Mo
 from .vit import VIT_B_16, VIT_B_32, VIT_L_16, ViTConfig, VisionTransformer, vit_b_16, vit_b_32, vit_l_16
 from .clip import CLIP_VIT_B_16, CLIP_VIT_B_32, CLIPConfig, CLIPModel, clip_vit_b_16, clip_vit_b_32
 from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneration, bart_base, bart_large
+from .t5 import T5_BASE, T5_SMALL, T5Config, T5ForConditionalGeneration, t5_base, t5_small
 
 
 @dataclass(frozen=True)
@@ -29,7 +30,7 @@ class ModelEntry:
     max_seq_len: int | None = None     # a training cap on --seq_len below config.max_position
     contrastive: bool = False          # image models trained on image-caption pairs with their own contrastive loss
                                        # (CLIP): forward(images, input_ids), the criterion ops.ClipLoss
-    seq2seq: bool = False              # encoder-decoder trained on source / target pairs (BART): forward(source_ids, labels),
+    seq2seq: bool = False              # encoder-decoder trained on source / target pairs (BART, T5): forward(source_ids, labels),
                                        # kind "causal" (the decoder is a causal LM over the target)
 
     @property
@@ -60,6 +61,10 @@ MODEL_REGISTRY = {
     # id 3 (<unk>), which the synthetic text never holds otherwise
     "bart-base": ModelEntry(bart_base, "causal", BART_BASE, start_id=3, seq2seq=True),
     "bart-large": ModelEntry(bart_large, "causal", BART_LARGE, start_id=3, seq2seq=True),
+    # T5's pad and decoder start id is 0 and </s> is 1, so packed documents start with id 2 (<unk>), which the synthetic
+    # text never holds otherwise
+    "t5-small": ModelEntry(t5_small, "causal", T5_SMALL, start_id=2, seq2seq=True),
+    "t5-base": ModelEntry(t5_base, "causal", T5_BASE, start_id=2, seq2seq=True),
 }
 
 
@@ -75,4 +80,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

@@ -28,6 +28,21 @@ from ..ops import (LayerNorm, Linear, LinearCrossEntropyLoss, causal_attention, 
 POSITION_OFFSET = 2                # transformers' BartLearnedPositionalEmbedding: position p reads row p + 2
 
 
+def shift_documents_right(labels, start_id: int, pad_token_id, bos_token_id, default_fill: int):
+    """(decoder input ids, decoder document bounds, decoder position ids) of an encoder-decoder from labels [B, Sq]
+    (-100 = ignored): each target document shifted right by one with ``start_id`` at its start, -100 as the pad id
+    (``default_fill`` when rows hold no padding).  Torch ops on the device, no host synchronisation."""
+    fill = pad_token_id if pad_token_id is not None else default_fill
+    target = labels.masked_fill(labels == -100, fill)
+    bounds, position_ids = document_bounds(target, bos_token_id, pad_token_id)
+    S = labels.shape[1]
+    pos = torch.arange(S, device=labels.device)
+    start = ((bounds[..., 0] == pos) & (bounds[..., 1] > pos)) | (pos == 0)
+    shifted = torch.cat([torch.full_like(target[:, :1], fill), target[:, :-1]], 1)
+    ids = torch.where(start, torch.full_like(target, start_id), shifted)
+    return ids, bounds, (position_ids if bos_token_id is not None else pos.expand_as(labels))
+
+
 @dataclass
 class BartConfig:
     vocab_size: int = 50265
@@ -118,19 +133,10 @@ class BartModel(nn.Module):
                 nn.init.zeros_(m.bias)
 
     def decoder_inputs(self, labels):
-        """(decoder input ids, decoder document bounds, decoder position ids) from labels [B, Sq] (-100 = ignored):
-        each target document shifted right by one with ``decoder_start_token_id`` at its start, -100 as the pad id.
-        Torch ops on the device, no host synchronisation."""
+        """(decoder input ids, decoder document bounds, decoder position ids) from labels [B, Sq]: ``shift_documents_right``
+        with BART's ids (its own <pad>, 1, as the fill when rows hold no padding)."""
         c = self.config
-        fill = c.pad_token_id if c.pad_token_id is not None else 1   # BART's own <pad> when rows hold no padding
-        target = labels.masked_fill(labels == -100, fill)
-        bounds, position_ids = document_bounds(target, c.bos_token_id, c.pad_token_id)
-        S = labels.shape[1]
-        pos = torch.arange(S, device=labels.device)
-        start = ((bounds[..., 0] == pos) & (bounds[..., 1] > pos)) | (pos == 0)
-        shifted = torch.cat([torch.full_like(target[:, :1], fill), target[:, :-1]], 1)
-        ids = torch.where(start, torch.full_like(target, c.decoder_start_token_id), shifted)
-        return ids, bounds, (position_ids if c.bos_token_id is not None else pos.expand_as(labels))
+        return shift_documents_right(labels, c.decoder_start_token_id, c.pad_token_id, c.bos_token_id, 1)
 
     def forward(self, input_ids, labels):
         c = self.config

@@ -57,6 +57,16 @@ def _tc_ok(M: int, N: int, K: int) -> bool:
     return K % 8 == 0 and N % 8 == 0 and M % 8 == 0
 
 
+_ZERO_BIAS = {}                  # (features, dtype, device) -> zeros, never written
+
+
+def _zero_bias(n: int, dtype, device) -> torch.Tensor:
+    key = (n, dtype, str(device))
+    if key not in _ZERO_BIAS:
+        _ZERO_BIAS[key] = torch.zeros(n, dtype=dtype, device=device)
+    return _ZERO_BIAS[key]
+
+
 class _LinearTC(torch.autograd.Function):
     """bf16 linear on wgmma: fwd y = act(x W^T + b); bwd dgrad/wgrad without transposes (MN-major
     operand descriptors), ReLU/GELU backward applied to dy before the two GEMMs."""
@@ -67,7 +77,7 @@ class _LinearTC(torch.autograd.Function):
         x2 = x.reshape(-1, x.shape[-1])
         if not x2.is_contiguous():
             x2 = x2.contiguous()
-        if bias is None and activation not in (None, *_GELUS):
+        if bias is None and activation not in (None, "relu", *_GELUS):
             raise ValueError("fused activation needs a bias (use bias=True)")
         if activation in _GELUS:
             # keep the pre-activation for the backward (GELU' needs it): two launches, one extra tensor
@@ -75,7 +85,10 @@ class _LinearTC(torch.autograd.Function):
             y = _gelu_fwd(C, pre, activation)
             ctx.save_for_backward(x2, weight, pre)
         else:
-            y = C.gemm_nt(x2, weight, bias, _ACT_TO_EPI[activation] if bias is not None else EPI_NONE, None)
+            epi_bias = bias
+            if bias is None and activation == "relu":            # bias-free ReLU (T5's wi): a zero bias feeds the ReLU epilogue
+                epi_bias = _zero_bias(weight.shape[0], weight.dtype, weight.device)
+            y = C.gemm_nt(x2, weight, epi_bias, _ACT_TO_EPI[activation] if epi_bias is not None else EPI_NONE, None)
             ctx.save_for_backward(x2, weight, y if activation == "relu" else None)
         ctx.activation = activation
         ctx.has_bias = bias is not None
@@ -280,7 +293,7 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
         N, K = weight.shape
         M = x.numel() // K
         if x.dtype == torch.bfloat16 and weight.dtype == torch.bfloat16 and _tc_ok(M, N, K) \
-                and (bias is not None or activation in (None, *_GELUS)) and os.environ.get("B200DDP_DISABLE_TC", "0") != "1":
+                and (bias is not None or activation in (None, "relu", *_GELUS)) and os.environ.get("B200DDP_DISABLE_TC", "0") != "1":
             return _LinearTC.apply(x, weight, bias, activation)
         if x.dtype == torch.float32 and weight.dtype == torch.float32 and N * (K + 1) * 4 <= 48 * 1024 and M * N * 4 <= 48 * 1024 \
                 and activation in (None, "relu"):
@@ -703,6 +716,153 @@ def cross_attention(q: torch.Tensor, kv: torch.Tensor, q_bounds: torch.Tensor, k
     if q.is_cuda:
         _cross_check(q, kv, q_bounds, kv_bounds, heads)
     return _CrossAttention.apply(q, kv, q_bounds, kv_bounds, heads)
+
+
+# ------------------------------------------------------------------------------------------------
+# T5's relative position bias (csrc/attention.cu, kBias): a learned, bucketed bias added to the unscaled scores
+# ------------------------------------------------------------------------------------------------
+RELATIVE_MAX_DISTANCE = 128
+RELATIVE_TABLE_COLS = 2 * RELATIVE_MAX_DISTANCE + 1    # the distances k - i clamped to [-128, 128]
+_RELATIVE_BUCKETS = {}                                  # (bidirectional, num_buckets, device) -> int32 [257]
+
+
+def relative_position_bucket(rel: torch.Tensor, bidirectional: bool, num_buckets: int = 32, max_distance: int = 128) -> torch.Tensor:
+    """T5's bucket of each relative position ``rel = key - query`` (long), with transformers' float32 expression
+    (``T5Attention._relative_position_bucket``), so the bucket edges fall where transformers puts them.  Bidirectional
+    (encoder): half the buckets for positive distances; unidirectional (decoder): only ``rel <= 0`` is told apart."""
+    rel = torch.as_tensor(rel).long()
+    buckets = torch.zeros_like(rel)
+    if bidirectional:
+        num_buckets //= 2
+        buckets = buckets + (rel > 0).long() * num_buckets
+        rel = rel.abs()
+    else:
+        rel = -torch.min(rel, torch.zeros_like(rel))
+    max_exact = num_buckets // 2
+    large = max_exact + (torch.log(rel.float() / max_exact) / math.log(max_distance / max_exact) * (num_buckets - max_exact)).long()
+    large = torch.min(large, torch.full_like(large, num_buckets - 1))
+    return buckets + torch.where(rel < max_exact, rel, large)
+
+
+def _relative_buckets(bidirectional: bool, num_buckets: int, device) -> torch.Tensor:
+    """int32 [257]: the bucket of each clamped distance c - 128, computed on the host once per configuration and device."""
+    key = (bool(bidirectional), int(num_buckets), str(device))
+    if key not in _RELATIVE_BUCKETS:
+        _RELATIVE_BUCKETS[key] = relative_position_buckets(bidirectional, num_buckets).to(device)
+    return _RELATIVE_BUCKETS[key]
+
+
+class _RelativeTable(torch.autograd.Function):
+    """CUDA body: one gather kernel forward; backward one kernel that folds dtable into d weight bucket by bucket in a
+    fixed order (no atomics).  CPU body: indexing, in fp32 (fp64 stays fp64)."""
+
+    @staticmethod
+    def forward(ctx, weight, bidirectional, buckets):
+        idx = _relative_buckets(bidirectional, weight.shape[0], weight.device) if buckets is None else buckets
+        ctx.save_for_backward(weight, idx)
+        if weight.is_cuda:
+            return _C().t5.relative_table_fwd(weight.contiguous(), idx)
+        return weight.to(torch.promote_types(weight.dtype, torch.float32))[idx.long()].t().contiguous()
+
+    @staticmethod
+    def backward(ctx, dtable):
+        weight, idx = ctx.saved_tensors
+        if dtable.is_cuda:
+            return _C().t5.relative_table_bwd(dtable.float().contiguous(), idx, weight.contiguous()), None, None
+        dw = torch.zeros(weight.shape, dtype=dtable.dtype)
+        dw.index_add_(0, idx.long(), dtable.t())
+        return dw.to(weight.dtype), None, None
+
+
+def relative_position_buckets(bidirectional: bool, num_buckets: int = 32) -> torch.Tensor:
+    """int32 [257] on the CPU: the bucket of each clamped distance c - 128 (``relative_position_bucket``).  A module that
+    keeps it as a buffer hands ``relative_position_table`` a device copy made when the module moved, so no forward (and no
+    CUDA-graph capture) copies it to the device."""
+    rel = torch.arange(-RELATIVE_MAX_DISTANCE, RELATIVE_MAX_DISTANCE + 1)
+    return relative_position_bucket(rel, bidirectional, num_buckets, RELATIVE_MAX_DISTANCE).to(torch.int32)
+
+
+def relative_position_table(weight: torch.Tensor, bidirectional: bool, buckets: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """T5's bias per head and clamped distance: weight [num_buckets, heads] (the ``relative_attention_bias`` embedding)
+    -> fp32 [heads, 257], column c holding the bias of distance ``key - query = c - 128`` (exact at any length: every
+    distance beyond +-128 falls in the bucket of +-128).  Differentiable.  A stack builds it once per forward and hands it
+    to all its layers, so autograd sums their fp32 gradients before the one fold into the weight.  ``buckets``:
+    ``relative_position_buckets(bidirectional, num_buckets)`` on weight's device; without it a copy cached per device is
+    used, made on the first call."""
+    if weight.dim() != 2 or not weight.is_floating_point():
+        raise ValueError(f"relative_position_table needs a floating weight [num_buckets, heads], got {weight.dtype} {tuple(weight.shape)}")
+    if buckets is not None and (tuple(buckets.shape) != (RELATIVE_TABLE_COLS,) or buckets.dtype != torch.int32 or buckets.device != weight.device):
+        raise ValueError(f"relative_position_table needs int32 buckets [{RELATIVE_TABLE_COLS}] on weight's device, got "
+                         f"{buckets.dtype} {tuple(buckets.shape)} on {buckets.device}")
+    return _RelativeTable.apply(weight, bidirectional, buckets)
+
+
+def relative_attention_reference(qkv: torch.Tensor, bounds: torch.Tensor, table: torch.Tensor, heads: int, causal: bool) -> torch.Tensor:
+    """softmax(Q K^T + bias) V with T5's unscaled scores, bias[h, i, j] = table[h, clamp(j - i, -128, 128) + 128], under the
+    mask of ``packed_attention`` (causal=False) or ``causal_attention`` (causal=True), as a dense mask in fp32 (fp64 stays
+    fp64); a row that sees no key gives zeros.  qkv [B, S, 3 * hidden], bounds integer [B, S, 2], table [heads, 257];
+    returns [B, S, hidden] in qkv's dtype.  Differentiable in qkv and table."""
+    B, S, W = qkv.shape
+    hidden = W // 3
+    hd = hidden // heads
+    ct = torch.promote_types(qkv.dtype, torch.float32)
+    q, k, v = (t.to(ct).reshape(B, S, heads, hd).transpose(1, 2) for t in qkv.split(hidden, dim=-1))
+    pos = torch.arange(S, device=qkv.device)
+    col = (pos[None, :] - pos[:, None]).clamp(-RELATIVE_MAX_DISTANCE, RELATIVE_MAX_DISTANCE) + RELATIVE_MAX_DISTANCE
+    keep = (_causal_mask if causal else _bounds_mask)(bounds, S, qkv.device)[:, None]
+    scores = q @ k.transpose(-1, -2) + table.to(ct)[:, col]
+    p = torch.softmax(scores.masked_fill(~keep, torch.finfo(ct).min), dim=-1) * keep
+    return (p @ v).transpose(1, 2).reshape(B, S, hidden).to(qkv.dtype)
+
+
+class _RelativeAttention(torch.autograd.Function):
+    """CUDA body: the kBias instantiations of the segment / causal kernels (backward: dqkv, and dtable through per-CTA
+    partials and a fixed-order finish, no atomics).  CPU body: ``relative_attention_reference``."""
+
+    @staticmethod
+    def forward(ctx, qkv, bounds, table, heads, causal):
+        ctx.heads, ctx.causal = heads, causal
+        if qkv.is_cuda:
+            B, S, W = qkv.shape
+            m = bounds.to(device=qkv.device, dtype=torch.int32).contiguous()
+            t = table.float().contiguous()
+            o, lse = _C().t5.relative_attention_fwd(qkv.view(B * S, W), m, t, heads, causal)
+            ctx.save_for_backward(qkv, o, lse, m, t)
+            return o.view(B, S, W // 3)
+        ctx.save_for_backward(qkv, bounds, table)
+        return relative_attention_reference(qkv, bounds, table, heads, causal)
+
+    @staticmethod
+    def backward(ctx, dy):
+        if dy.is_cuda:
+            qkv, o, lse, m, t = ctx.saved_tensors
+            B, S, W = qkv.shape
+            do = dy.reshape(B * S, W // 3).to(torch.bfloat16).contiguous()
+            if do.data_ptr() % 16:                                # the kernels read dO in TMA boxes
+                do = do.clone()
+            dqkv, dtable = _C().t5.relative_attention_bwd(do, qkv.view(B * S, W), o, lse, m, t, ctx.heads, ctx.causal)
+            return dqkv.view(B, S, W), None, dtable, None, None
+        qkv, bounds, table = ctx.saved_tensors
+        with torch.enable_grad():
+            x, tb = qkv.detach().requires_grad_(True), table.detach().requires_grad_(True)
+            dx, dt = torch.autograd.grad(relative_attention_reference(x, bounds, tb, ctx.heads, ctx.causal), (x, tb), dy)
+        return dx, None, dt, None, None
+
+
+def relative_attention(qkv: torch.Tensor, bounds: torch.Tensor, table: torch.Tensor, heads: int, causal: bool) -> torch.Tensor:
+    """T5's self-attention: ``packed_attention`` (causal=False) or ``causal_attention`` (causal=True) over the documents of
+    bounds [B, S, 2], with the scores unscaled and T5's relative bias added, table [heads, 257]
+    (``relative_position_table``).  The distance is ``key - query`` inside a row, which inside a packed document is the
+    in-document distance.  Returns [B, S, hidden], with gradients for qkv and table.  On CUDA: bf16 qkv, head dim 64,
+    S % 128 == 0, contiguous qkv and a [heads, 257] table, else ``ValueError``; no host synchronisation (CUDA-graph
+    safe)."""
+    if qkv.is_cuda:
+        _qkv_check(qkv, heads)
+        _bounds_check(qkv, bounds, "relative attention")
+        if tuple(table.shape) != (heads, RELATIVE_TABLE_COLS) or not table.is_floating_point():
+            raise ValueError(f"relative attention needs a table [heads, {RELATIVE_TABLE_COLS}] = [{heads}, {RELATIVE_TABLE_COLS}], "
+                             f"got {table.dtype} {tuple(table.shape)}")
+    return _RelativeAttention.apply(qkv, bounds, table, heads, causal)
 
 
 def _document_table(bounds: torch.Tensor, slots: int):

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -1018,6 +1018,73 @@ def main():
                 record(f"{name} bwd", timeit(lambda: C.cross.cross_attention_bwd(dout, q, kv, o, lse, qb, kb, H), args.iters),
                        flops=2.5 * fwd_flops, lib_ms=lib, note=f"lib = {lib_name} backward into q and kv")
                 del xq, xkv, y
+    if "t5" in want:
+        # T5's relative position bias at t5-base's attention shape (12 heads, batch 32 x 512), encoder (segment) and
+        # decoder (causal), on full, right-padded (lengths U[S/4, S]) and packed rows (documents U[64, S], first fit).
+        # Three things per case: the bias kernels (forward with the table gather, backward with the dtable finish and the
+        # fold into the embedding), the same kernels without bias (the price of the bias), and SDPA with the float
+        # [1, H, S, S] bias (requiring grad) plus the document mask, which is what transformers' T5 attention amounts to.
+        # FLOPs count the visible pairs only: forward 4 d H pairs, backward 2.5x that.
+        import torch.nn.functional as F
+        H, d, B, S = 12, 64, 32, 512
+        g = torch.Generator(device=dev).manual_seed(0)
+        qkv = torch.randn(B * S, 3 * H * d, device=dev, generator=g).to(torch.bfloat16)
+        dout = torch.randn(B * S, H * d, device=dev, generator=g).to(torch.bfloat16)
+        weight = (torch.randn(32, H, device=dev, generator=g) * 2).to(torch.bfloat16)
+        rng = torch.Generator().manual_seed(1)
+        lens = torch.randint(S // 4, S + 1, (B,), generator=rng)
+        packed = torch.zeros(B, S, 2, dtype=torch.int32)
+        for r in range(B):
+            at = 0
+            while at < S:
+                n = min(int(torch.randint(64, S + 1, (1,), generator=rng)), S - at)
+                packed[r, at:at + n, 0], packed[r, at:at + n, 1] = at, at + n
+                at += n
+        pos = torch.arange(S)
+        layouts = [("full", torch.stack([torch.zeros(B, S, dtype=torch.int32), torch.full((B, S), S, dtype=torch.int32)], -1)),
+                   ("padded", torch.stack([torch.zeros(B, S, dtype=torch.int32), torch.where(pos < lens[:, None], lens[:, None], 0).int()], -1)
+                    * (pos < lens[:, None])[..., None]),
+                   ("packed", packed)]
+        for causal in (False, True):
+            plain = "causal_attention" if causal else "packed_attention"
+            for label, bounds in layouts:
+                bounds = bounds.to(dev).contiguous()
+                vis = Fn._causal_mask(bounds, S, dev) if causal else Fn._bounds_mask(bounds, S, dev)
+                fwd_flops = 4.0 * d * H * float(vis.sum())
+                name = f"t5 {'decoder causal' if causal else 'encoder segment'} {label} B{B} S{S} H{H}"
+
+                def bias_fwd():
+                    table = C.t5.relative_table_fwd(weight, Fn._relative_buckets(not causal, 32, dev))
+                    return C.t5.relative_attention_fwd(qkv, bounds, table, H, causal)
+                table = C.t5.relative_table_fwd(weight, Fn._relative_buckets(not causal, 32, dev))
+                o, lse = C.t5.relative_attention_fwd(qkv, bounds, table, H, causal)
+
+                def bias_bwd():
+                    dqkv, dtable = C.t5.relative_attention_bwd(dout, qkv, o, lse, bounds, table, H, causal)
+                    return C.t5.relative_table_bwd(dtable, Fn._relative_buckets(not causal, 32, dev), weight)
+                po, plse = getattr(C, plain + "_fwd")(qkv, bounds, H)
+                # SDPA: q k^T (scale 1) + bias[h, i, j] + the mask; a row that sees nothing keeps key 0 (not a NaN row)
+                x = qkv.view(B, S, 3 * H * d).detach().clone().requires_grad_(True)
+                qh, kh, vh = (t.reshape(B, S, H, d).transpose(1, 2) for t in x.split(H * d, -1))
+                dense = table[:, (pos[None, :] - pos[:, None]).clamp(-128, 128).to(dev) + 128].to(torch.bfloat16)[None]
+                dense = dense.detach().requires_grad_(True)
+                keep = vis | (~vis.any(-1, keepdim=True) & (torch.arange(S, device=dev) == 0))
+                mask = torch.zeros(B, 1, S, S, device=dev, dtype=torch.bfloat16).masked_fill(~keep[:, None], float("-inf"))
+
+                def sdpa():
+                    return F.scaled_dot_product_attention(qh, kh, vh, attn_mask=dense + mask, scale=1.0).transpose(1, 2).reshape(B, S, H * d)
+                record(f"{name} fwd", timeit(bias_fwd, args.iters), flops=fwd_flops, lib_ms=timeit(lambda: sdpa().detach(), args.iters),
+                       note="lib = SDPA with the float bias + mask")
+                record(f"{name} fwd no bias", timeit(lambda: getattr(C, plain + "_fwd")(qkv, bounds, H), args.iters), flops=fwd_flops,
+                       note=f"{plain}_fwd: the same kernel without the bias")
+                y = sdpa()
+                dy = dout.view(B, S, H * d)
+                record(f"{name} bwd", timeit(bias_bwd, args.iters), flops=2.5 * fwd_flops,
+                       lib_ms=timeit(lambda: torch.autograd.grad(y, (x, dense), dy, retain_graph=True), args.iters),
+                       note="incl. dtable finish and fold; lib = SDPA backward into qkv and the bias")
+                record(f"{name} bwd no bias", timeit(lambda: getattr(C, plain + "_bwd")(dout, qkv, po, plse, bounds, H), args.iters),
+                       flops=2.5 * fwd_flops, note=f"{plain}_bwd: the same kernels without the bias")
+                del x, y, dense, mask
     if "mse" in want:
         n = 64 * 1024 * 1024
         o = torch.randn(n, device=dev, dtype=torch.bfloat16)
