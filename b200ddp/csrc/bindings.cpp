@@ -170,10 +170,21 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip, _C.cross and _C.t5 namespaces of static entry points
+// the types behind the _C.clip, _C.cross, _C.t5 and _C.convnext namespaces of static entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
 struct T5Namespace {};
+struct ConvNextNamespace {};
+
+// An NHWC activation of the depthwise convolution: bf16 [B, H, W, C] contiguous and 16-byte aligned, B, H, W >= 1,
+// 8 <= C <= 1024 with C % 8 == 0 (B is the grid's z extent).  Returns (B, H, W, C).
+std::array<int, 4> dwconv_args(Args& args, const char* name, const at::Tensor& x) {
+  args(name, x, {kBF16}, {kAny, kAny, kAny, kAny}, kContiguous, 16);
+  const int64_t B = x.size(0), H = x.size(1), W = x.size(2), C = x.size(3);
+  if (B < 1 || B > 65535 || H < 1 || W < 1 || C < 8 || C > 1024 || C % 8)
+    args.fail(name, "bf16 [B, H, W, C] with 1 <= B <= 65535, H, W >= 1, 8 <= C <= 1024 and C % 8 == 0", describe(x));
+  return {(int)B, (int)H, (int)W, (int)C};
+}
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
   CommCtx c;
@@ -1744,4 +1755,39 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                               weight.scalar_type() == kBF16, dweight.data_ptr(), cur_stream());
     return dweight;
   }, py::arg("dtable"), py::arg("bucket"), py::arg("weight"));
+
+  // ---- ConvNeXt's depthwise 7x7 convolution, stride 1, padding 3 (convnext.cu), bf16 NHWC --------------------------------
+  // _C.convnext is a namespace of static entry points like _C.t5; its contract rows are in tests/test_convnext_bindings_cpu.py.
+  // x, dy [B, H, W, C]; weight bf16 [C, 49] (the memory of a contiguous or channels_last [C, 1, 7, 7]); bias bf16 [C].
+  py::class_<ConvNextNamespace> convnext(m, "convnext", "ConvNeXt's depthwise 7x7 convolution on NHWC activations (convnext.cu)");
+  convnext.def_static("dwconv_fwd", [](at::Tensor x, at::Tensor weight, at::Tensor bias) {
+    Args args("dwconv_fwd");
+    const auto [B, H, W, C] = dwconv_args(args, "x", x);
+    args("weight", weight, {kBF16}, {C, 49})("bias", bias, {kBF16}, {C});
+    args.device();
+    at::Tensor y = at::empty_like(x);
+    launch_dwconv_fwd(x.data_ptr(), weight.data_ptr(), bias.data_ptr(), B, H, W, C, y.data_ptr(), cur_stream());
+    return y;
+  }, py::arg("x"), py::arg("weight"), py::arg("bias"));
+  convnext.def_static("dwconv_dgrad", [](at::Tensor dy, at::Tensor weight) {
+    Args args("dwconv_dgrad");
+    const auto [B, H, W, C] = dwconv_args(args, "dy", dy);
+    args("weight", weight, {kBF16}, {C, 49});
+    args.device();
+    at::Tensor dx = at::empty_like(dy);
+    launch_dwconv_dgrad(dy.data_ptr(), weight.data_ptr(), B, H, W, C, dx.data_ptr(), cur_stream());
+    return dx;
+  }, py::arg("dy"), py::arg("weight"));
+  // (dweight bf16 [C, 49], dbias bf16 [C])
+  convnext.def_static("dwconv_wgrad", [](at::Tensor dy, at::Tensor x) {
+    Args args("dwconv_wgrad");
+    const auto [B, H, W, C] = dwconv_args(args, "x", x);
+    args("dy", dy, {kBF16}, {B, H, W, C}, kContiguous, 16);
+    args.device();
+    at::Tensor part = at::empty({(int64_t)dwconv_wgrad_slots(B, H, W), 50, C}, x.options().dtype(kF32));
+    at::Tensor dweight = at::empty({C, 49}, x.options());
+    at::Tensor dbias = at::empty({C}, x.options());
+    launch_dwconv_wgrad(dy.data_ptr(), x.data_ptr(), B, H, W, C, part.data_ptr<float>(), dweight.data_ptr(), dbias.data_ptr(), cur_stream());
+    return std::make_tuple(dweight, dbias);
+  }, py::arg("dy"), py::arg("x"));
 }

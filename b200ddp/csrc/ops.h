@@ -259,6 +259,18 @@ void launch_patch_assemble(const void* y, const void* cls, const void* pos, int 
 // dpatch [T, D] = dy at patch rows, 0 elsewhere; dpos [per, D] = fixed-order fp32 sums over the B images; dcls [D] = dpos[0]
 void launch_patch_embed_bwd(const void* dy, int B, int per, int D, int T, void* dpatch, void* dpos, void* dcls, cudaStream_t s);
 
+// ---------------- ConvNeXt depthwise 7x7 convolution, stride 1, padding 3 (convnext.cu), bf16 NHWC ---------------------
+// x, y, dy, dx [B, H, W, C] contiguous and 16-byte aligned, 8 <= C <= 1024, C % 8 == 0; w [C, 49] (a contiguous or
+// channels_last [C, 1, 7, 7]); bias [C] or null.  fp32 sums in a fixed order, one bf16 rounding, no atomics.
+// y = b + sum over the 49 taps of x (zero outside the image) times w
+void launch_dwconv_fwd(const void* x, const void* w, const void* bias, int B, int H, int W, int C, void* y, cudaStream_t s);
+// dx = the forward of dy with the kernel flipped, no bias
+void launch_dwconv_dgrad(const void* dy, const void* w, int B, int H, int W, int C, void* dx, cudaStream_t s);
+// dw bf16 [C, 49] and db bf16 [C] through part fp32 [dwconv_wgrad_slots(B, H, W), 50, C]: one slot per (image, spatial
+// tile), summed in slot order.  dy is read at real pixels only.
+int dwconv_wgrad_slots(int B, int H, int W);
+void launch_dwconv_wgrad(const void* dy, const void* x, int B, int H, int W, int C, float* part, void* dw, void* db, cudaStream_t s);
+
 // ---------------- CLIP contrastive loss (clip.cu) ---------------------------------------------------
 // u bf16 [B, D] = x / ||x|| per row (fp32, one rounding), rnorm fp32 [B] = 1 / ||x||; D % 8 == 0, 16-byte aligned rows
 void launch_l2norm_fwd(const void* x, int B, int D, void* u, float* rnorm, cudaStream_t s);

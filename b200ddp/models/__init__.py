@@ -13,6 +13,7 @@ from .llama import (GRANITE_3_0_1B_A400M, QWEN2_5_1_5B, QWEN3_0_6B, SMOLLM_135M,
 from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, ModernBertModel, ModernBertForMaskedLM, modernbert_base,
                          modernbert_large)
 from .vit import VIT_B_16, VIT_B_32, VIT_L_16, ViTConfig, VisionTransformer, vit_b_16, vit_b_32, vit_l_16
+from .convnext import CONVNEXT_BASE, CONVNEXT_SMALL, CONVNEXT_TINY, ConvNeXt, ConvNeXtConfig, convnext_base, convnext_small, convnext_tiny
 from .clip import CLIP_VIT_B_16, CLIP_VIT_B_32, CLIPConfig, CLIPModel, clip_vit_b_16, clip_vit_b_32
 from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneration, bart_base, bart_large
 from .t5 import T5_BASE, T5_SMALL, T5Config, T5ForConditionalGeneration, t5_base, t5_small
@@ -45,6 +46,9 @@ MODEL_REGISTRY = {
     "vit-b-16": ModelEntry(vit_b_16, "image"),
     "vit-b-32": ModelEntry(vit_b_32, "image"),
     "vit-l-16": ModelEntry(vit_l_16, "image"),
+    "convnext-tiny": ModelEntry(convnext_tiny, "image"),
+    "convnext-small": ModelEntry(convnext_small, "image"),
+    "convnext-base": ModelEntry(convnext_base, "image"),
     "clip-vit-b-32": ModelEntry(clip_vit_b_32, "image", contrastive=True),
     "clip-vit-b-16": ModelEntry(clip_vit_b_16, "image", contrastive=True),
     "bert-base": ModelEntry(bert_base, "encoder", BERT_BASE, start_id=101, fp8=True),                 # [CLS]
@@ -80,4 +84,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

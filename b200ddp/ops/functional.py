@@ -1782,6 +1782,85 @@ def patch_embed(images: torch.Tensor, weight: torch.Tensor, bias: Optional[torch
 
 
 # ------------------------------------------------------------------------------------------------
+# ConvNeXt (csrc/convnext.cu): the depthwise 7x7 convolution on NHWC activations, and the patchify convolutions as gathers
+# ------------------------------------------------------------------------------------------------
+DWCONV_KERNEL = 7
+DWCONV_MAX_CHANNELS = 1024
+
+
+def depthwise_conv2d_reference(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor]) -> torch.Tensor:
+    """``depthwise_conv2d`` through ``F.conv2d(groups=C)`` on the NCHW view of x [B, H, W, C]; returns [B, H, W, C]."""
+    return F.conv2d(x.permute(0, 3, 1, 2), weight, bias, padding=DWCONV_KERNEL // 2, groups=x.shape[-1]).permute(0, 2, 3, 1)
+
+
+def _depthwise_check(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor]) -> None:
+    C = x.shape[-1] if x.dim() == 4 else -1
+    if x.dim() != 4 or tuple(weight.shape) != (C, 1, DWCONV_KERNEL, DWCONV_KERNEL) or bias is None or tuple(bias.shape) != (C,):
+        raise ValueError(f"depthwise_conv2d needs x [B, H, W, C], weight [C, 1, 7, 7] and bias [C], got {tuple(x.shape)}, "
+                         f"{tuple(weight.shape)} and {None if bias is None else tuple(bias.shape)}")
+    if C < 8 or C > DWCONV_MAX_CHANNELS or C % 8 or x.numel() == 0:
+        raise ValueError(f"depthwise_conv2d on CUDA needs 8 <= C <= {DWCONV_MAX_CHANNELS}, C % 8 == 0 and a non-empty x, got "
+                         f"{tuple(x.shape)}")
+    if weight.dtype != torch.bfloat16 or bias.dtype != torch.bfloat16:
+        raise ValueError(f"depthwise_conv2d on CUDA needs bf16 x, weight and bias, got {x.dtype}, {weight.dtype}, {bias.dtype}")
+
+
+def _aligned16(t: torch.Tensor) -> torch.Tensor:
+    t = t.contiguous()
+    return t.clone() if t.data_ptr() % 16 else t                     # the kernels move 16-byte vectors
+
+
+class _DepthwiseConv2d(torch.autograd.Function):
+    """x [B, H, W, C] bf16 -> y (csrc/convnext.cu).  Backward: the data gradient is the forward kernel flipped, and one
+    pass plus an in-order finish gives the weight and bias gradients."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        C = x.shape[-1]
+        w = weight.reshape(C, DWCONV_KERNEL * DWCONV_KERNEL).contiguous()     # free for a contiguous or channels_last weight
+        ctx.save_for_backward(x, w)
+        ctx.weight_shape = weight.shape
+        return _C().convnext.dwconv_fwd(x, w, bias.contiguous())
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, w = ctx.saved_tensors
+        dy = _aligned16(dy)
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = _C().convnext.dwconv_dgrad(dy, w)
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            dw, db = _C().convnext.dwconv_wgrad(dy, x)
+            dw = dw.view(ctx.weight_shape)
+        return dx, dw, db
+
+
+def depthwise_conv2d(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor]) -> torch.Tensor:
+    """ConvNeXt's depthwise convolution (kernel 7, stride 1, padding 3, one filter per channel) on NHWC activations:
+    x [B, H, W, C], weight [C, 1, 7, 7] (contiguous or channels_last), bias [C] -> y [B, H, W, C].
+
+    CUDA with bf16 tensors runs the native kernels: fp32 sums in a fixed order and one bf16 rounding, bitwise repeatable,
+    no host synchronisation; it needs 8 <= C <= 1024 with C % 8 == 0 and a bias, else ``ValueError``.  The weight and bias
+    gradients do not depend on the output gradient anywhere but at real pixels.  Everything else runs
+    ``depthwise_conv2d_reference``."""
+    if not (x.is_cuda and x.dtype == torch.bfloat16):
+        return depthwise_conv2d_reference(x, weight, bias)
+    _depthwise_check(x, weight, bias)
+    return _DepthwiseConv2d.apply(_aligned16(x), weight, bias)
+
+
+def patchify_nhwc(x: torch.Tensor, patch: int) -> torch.Tensor:
+    """The rows of a patch convolution (kernel = stride = ``patch``, no padding) over x [B, H, W, C] (any strides): one
+    row per output pixel in raster order, its p² C inputs in (ky, kx, c) order, [B (H / p) (W / p), p² C].  Times
+    ``weight.permute(0, 2, 3, 1).reshape(D, -1)`` this is the convolution.  A torch permutation copy; its backward is the
+    inverse permutation."""
+    B, H, W, C = x.shape
+    if H % patch or W % patch:
+        raise ValueError(f"patchify_nhwc needs H and W divisible by {patch}, got {tuple(x.shape)}")
+    return x.reshape(B, H // patch, patch, W // patch, patch, C).permute(0, 1, 3, 2, 4, 5).reshape(-1, patch * patch * C)
+
+
+# ------------------------------------------------------------------------------------------------
 # CLIP (csrc/clip.cu): captions as causal documents of one token stream, the contrastive loss over the global batch
 # ------------------------------------------------------------------------------------------------
 def caption_token_bounds(input_ids: torch.Tensor, eos_token_id: int):

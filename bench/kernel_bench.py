@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -1085,6 +1085,37 @@ def main():
                 record(f"{name} bwd no bias", timeit(lambda: getattr(C, plain + "_bwd")(dout, qkv, po, plse, bounds, H), args.iters),
                        flops=2.5 * fwd_flops, note=f"{plain}_bwd: the same kernels without the bias")
                 del x, y, dense, mask
+    if "convnext" in want:
+        # ConvNeXt-T's depthwise 7x7 at batch 64, its four stage shapes: forward, data gradient, and weight + bias gradient
+        # against cuDNN's F.conv2d(groups=C) on channels_last bf16.  Bytes: 4 per element (read one tensor, write one) for
+        # the forward and the data gradient; for the weight gradient 4 per element (dy and x) plus the fp32 partials
+        # written and read once.
+        import torch.nn.functional as F
+        print(f"convnext kernels on {card()}", flush=True)
+        for B, H, W, Cn in ((64, 56, 56, 96), (64, 28, 28, 192), (64, 14, 14, 384), (64, 7, 7, 768)):
+            g = torch.Generator(device="cuda").manual_seed(Cn)
+            x = torch.randn(B, H, W, Cn, device=dev, generator=g).to(torch.bfloat16)
+            dy = torch.randn(B, H, W, Cn, device=dev, generator=g).to(torch.bfloat16)
+            w = (torch.randn(Cn, 1, 7, 7, device=dev, generator=g) / 7).to(torch.bfloat16)
+            b = torch.randn(Cn, device=dev, generator=g).to(torch.bfloat16)
+            w2 = w.reshape(Cn, 49)
+            xl, dyl = x.permute(0, 3, 1, 2), dy.permute(0, 3, 1, 2)          # the same memory as channels_last NCHW
+            n = x.numel()
+            tag = f"[{B},{H},{W},{Cn}]"
+            record(f"dwconv7x7 fwd {tag}", timeit(lambda: C.convnext.dwconv_fwd(x, w2, b), args.iters), bytes_=4 * n,
+                   lib_ms=timeit(lambda: F.conv2d(xl, w, b, padding=3, groups=Cn), args.iters), note="lib = cuDNN channels_last")
+            record(f"dwconv7x7 dgrad {tag}", timeit(lambda: C.convnext.dwconv_dgrad(dy, w2), args.iters), bytes_=4 * n,
+                   lib_ms=timeit(lambda: torch.ops.aten.convolution_backward(dyl, xl, w, [Cn], [1, 1], [3, 3], [1, 1], False, [0, 0], Cn,
+                                                                              [True, False, False]), args.iters),
+                   note="lib = cuDNN channels_last data gradient")
+            slots = B * -(-H // min(H, 16 if min(W, 56) <= 28 else 8)) * -(-W // min(W, 56))
+            record(f"dwconv7x7 wgrad {tag}", timeit(lambda: C.convnext.dwconv_wgrad(dy, x), args.iters),
+                   bytes_=4 * n + 2 * 4 * slots * 50 * Cn,
+                   lib_ms=timeit(lambda: torch.ops.aten.convolution_backward(dyl, xl, w, [Cn], [1, 1], [3, 3], [1, 1], False, [0, 0], Cn,
+                                                                              [False, True, True]), args.iters),
+                   note=f"{slots} partial slots; lib = cuDNN channels_last weight + bias gradient")
+            del x, dy, xl, dyl
+
     if "mse" in want:
         n = 64 * 1024 * 1024
         o = torch.randn(n, device=dev, dtype=torch.bfloat16)
