@@ -170,11 +170,12 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip, _C.cross, _C.t5 and _C.convnext namespaces of static entry points
+// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext and _C.swin namespaces of static entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
 struct T5Namespace {};
 struct ConvNextNamespace {};
+struct SwinNamespace {};
 
 // An NHWC activation of the depthwise convolution: bf16 [B, H, W, C] contiguous and 16-byte aligned, B, H, W >= 1,
 // 8 <= C <= 1024 with C % 8 == 0 (B is the grid's z extent).  Returns (B, H, W, C).
@@ -184,6 +185,25 @@ std::array<int, 4> dwconv_args(Args& args, const char* name, const at::Tensor& x
   if (B < 1 || B > 65535 || H < 1 || W < 1 || C < 8 || C > 1024 || C % 8)
     args.fail(name, "bf16 [B, H, W, C] with 1 <= B <= 65535, H, W >= 1, 8 <= C <= 1024 and C % 8 == 0", describe(x));
   return {(int)B, (int)H, (int)W, (int)C};
+}
+
+// The window-attention geometry: table fp32 [169, heads] with 1 <= heads <= 65535, batch >= 1, height and width positive
+// multiples of 7 and shifts in [0, 7), then qkv bf16 [batch * height * width, 96 heads], contiguous and 16-byte aligned.
+// Returns (rows, heads).
+std::array<int64_t, 2> swin_args(Args& args, const at::Tensor& qkv, const at::Tensor& table, int64_t batch, int64_t height, int64_t width,
+                                 int64_t shift_y, int64_t shift_x) {
+  args("table", table, {kF32}, {169, kAny});
+  const int64_t heads = table.size(1);
+  if (heads < 1 || heads > 65535) args.fail("table", "fp32 [169, heads] with 1 <= heads <= 65535", describe(table));
+  const auto geometry = [&] { return std::to_string(batch) + " x " + std::to_string(height) + " x " + std::to_string(width) + ", shift (" +
+                                     std::to_string(shift_y) + ", " + std::to_string(shift_x) + ")"; };
+  if (batch < 1 || batch > 65535 || height < 7 || width < 7 || height % 7 || width % 7 || height > 65535 || width > 65535 || shift_y < 0 ||
+      shift_y >= 7 || shift_x < 0 || shift_x >= 7)
+    args.fail("geometry", "batch >= 1, height and width positive multiples of 7 and shifts in [0, 7)", geometry());
+  const int64_t rows = batch * height * width;
+  if (rows * 96 * heads >= (1ll << 31)) args.fail("geometry", "at most 2^31 qkv elements", geometry());
+  args("qkv", qkv, {kBF16}, {rows, 96 * heads}, kContiguous, 16);
+  return {rows, heads};
 }
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
@@ -1790,4 +1810,39 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     launch_dwconv_wgrad(dy.data_ptr(), x.data_ptr(), B, H, W, C, part.data_ptr<float>(), dweight.data_ptr(), dbias.data_ptr(), cur_stream());
     return std::make_tuple(dweight, dbias);
   }, py::arg("dy"), py::arg("x"));
+
+  // ---- Swin's shifted-window attention, window 7, head dim 32 (swin.cu), bf16 raster rows ---------------------------------
+  // _C.swin is a namespace of static entry points like _C.convnext; its contract rows are in tests/test_swin_bindings_cpu.py.
+  // qkv [B H W, 3C] (C = 32 heads), table fp32 [169, heads], o and dout [B H W, C], lse fp32 [B H W, heads].
+  py::class_<SwinNamespace> swin(m, "swin", "Swin's shifted-window attention on raster token rows (swin.cu)");
+  // (o bf16 [B H W, C], lse fp32 [B H W, heads])
+  swin.def_static("attention_fwd", [](at::Tensor qkv, at::Tensor table, int64_t batch, int64_t height, int64_t width, int64_t shift_y,
+                                      int64_t shift_x) {
+    Args args("attention_fwd");
+    const auto [rows, heads] = swin_args(args, qkv, table, batch, height, width, shift_y, shift_x);
+    args.device();
+    at::Tensor o = at::empty({rows, 32 * heads}, qkv.options());
+    at::Tensor lse = at::empty({rows, heads}, qkv.options().dtype(kF32));
+    launch_swin_attention_fwd(qkv.data_ptr(), table.data_ptr<float>(), (int)batch, (int)height, (int)width, (int)heads, (int)shift_y,
+                              (int)shift_x, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
+    return std::make_tuple(o, lse);
+  }, py::arg("qkv"), py::arg("table"), py::arg("batch"), py::arg("height"), py::arg("width"), py::arg("shift_y"), py::arg("shift_x"));
+  // (dqkv bf16 [B H W, 3C], dtable fp32 [169, heads])
+  swin.def_static("attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor table, int64_t batch,
+                                      int64_t height, int64_t width, int64_t shift_y, int64_t shift_x) {
+    Args args("attention_bwd");
+    const auto [rows, heads] = swin_args(args, qkv, table, batch, height, width, shift_y, shift_x);
+    args("dout", dout, {kBF16}, {rows, 32 * heads}, kContiguous, 16)("o", o, {kBF16}, {rows, 32 * heads}, kContiguous, 16)
+        ("lse", lse, {kF32}, {rows, heads});
+    args.device();
+    const int windows = swin_windows((int)batch, (int)height, (int)width);
+    at::Tensor dqkv = at::empty_like(qkv);
+    at::Tensor part = at::empty({heads, (int64_t)windows, 169}, qkv.options().dtype(kF32));
+    at::Tensor dtable = at::empty({169, heads}, qkv.options().dtype(kF32));
+    launch_swin_attention_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), table.data_ptr<float>(), (int)batch,
+                              (int)height, (int)width, (int)heads, (int)shift_y, (int)shift_x, dqkv.data_ptr(), part.data_ptr<float>(),
+                              dtable.data_ptr<float>(), cur_stream());
+    return std::make_tuple(dqkv, dtable);
+  }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("table"), py::arg("batch"), py::arg("height"),
+     py::arg("width"), py::arg("shift_y"), py::arg("shift_x"));
 }

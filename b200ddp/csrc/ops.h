@@ -271,6 +271,17 @@ void launch_dwconv_dgrad(const void* dy, const void* w, int B, int H, int W, int
 int dwconv_wgrad_slots(int B, int H, int W);
 void launch_dwconv_wgrad(const void* dy, const void* x, int B, int H, int W, int C, float* part, void* dw, void* db, cudaStream_t s);
 
+// ---------------- Swin shifted-window attention, window 7, head dim 32 (swin.cu), bf16 raster rows ----------------------
+// qkv [B*H*W, 3C] (C = 32 heads, columns q | k | v), 16-byte aligned; table fp32 [169, heads]; H, W multiples of 7,
+// 0 <= sy, sx < 7.  o bf16 [B*H*W, C], lse fp32 [B*H*W, heads].  No atomics, no host synchronisation.
+int swin_windows(int B, int H, int W);
+void launch_swin_attention_fwd(const void* qkv, const float* table, int B, int H, int W, int heads, int sy, int sx, void* o, float* lse,
+                               cudaStream_t s);
+// dqkv bf16 [B*H*W, 3C]; dtable fp32 [169, heads] through part fp32 [heads, swin_windows(B, H, W), 169]: one partial per
+// (head, window), summed in window order
+void launch_swin_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const float* table, int B, int H, int W,
+                               int heads, int sy, int sx, void* dqkv, float* part, float* dtable, cudaStream_t s);
+
 // ---------------- CLIP contrastive loss (clip.cu) ---------------------------------------------------
 // u bf16 [B, D] = x / ||x|| per row (fp32, one rounding), rnorm fp32 [B] = 1 / ||x||; D % 8 == 0, 16-byte aligned rows
 void launch_l2norm_fwd(const void* x, int B, int D, void* u, float* rnorm, cudaStream_t s);

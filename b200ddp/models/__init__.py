@@ -14,6 +14,7 @@ from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, Mo
                          modernbert_large)
 from .vit import VIT_B_16, VIT_B_32, VIT_L_16, ViTConfig, VisionTransformer, vit_b_16, vit_b_32, vit_l_16
 from .convnext import CONVNEXT_BASE, CONVNEXT_SMALL, CONVNEXT_TINY, ConvNeXt, ConvNeXtConfig, convnext_base, convnext_small, convnext_tiny
+from .swin import SWIN_B, SWIN_S, SWIN_T, SwinConfig, SwinTransformer, swin_b, swin_s, swin_t
 from .clip import CLIP_VIT_B_16, CLIP_VIT_B_32, CLIPConfig, CLIPModel, clip_vit_b_16, clip_vit_b_32
 from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneration, bart_base, bart_large
 from .t5 import T5_BASE, T5_SMALL, T5Config, T5ForConditionalGeneration, t5_base, t5_small
@@ -49,6 +50,9 @@ MODEL_REGISTRY = {
     "convnext-tiny": ModelEntry(convnext_tiny, "image"),
     "convnext-small": ModelEntry(convnext_small, "image"),
     "convnext-base": ModelEntry(convnext_base, "image"),
+    "swin-t": ModelEntry(swin_t, "image"),
+    "swin-s": ModelEntry(swin_s, "image"),
+    "swin-b": ModelEntry(swin_b, "image"),
     "clip-vit-b-32": ModelEntry(clip_vit_b_32, "image", contrastive=True),
     "clip-vit-b-16": ModelEntry(clip_vit_b_16, "image", contrastive=True),
     "bert-base": ModelEntry(bert_base, "encoder", BERT_BASE, start_id=101, fp8=True),                 # [CLS]
@@ -84,4 +88,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

@@ -1861,6 +1861,113 @@ def patchify_nhwc(x: torch.Tensor, patch: int) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------------------------
+# Swin Transformer (csrc/swin.cu): shifted-window attention on raster token rows
+# ------------------------------------------------------------------------------------------------
+SWIN_WINDOW = 7
+SWIN_HEAD_DIM = 32
+SWIN_MASK = -100.0                   # torchvision's value between shift regions, not -inf
+
+
+def swin_relative_position_index(device=None) -> torch.Tensor:
+    """int64 [49 * 49]: entry 49 i + j is (yi - yj + 6) 13 + (xi - xj + 6) for the window's tokens i = 7 yi + xi and
+    j = 7 yj + xj, the table row of their relative position (torchvision's ``relative_position_index``)."""
+    t = torch.arange(SWIN_WINDOW * SWIN_WINDOW, device=device)
+    y, x = t // SWIN_WINDOW, t % SWIN_WINDOW
+    return ((y[:, None] - y[None, :] + SWIN_WINDOW - 1) * (2 * SWIN_WINDOW - 1) + (x[:, None] - x[None, :] + SWIN_WINDOW - 1)).flatten()
+
+
+def _shift_pair(shift) -> tuple[int, int]:
+    sy, sx = (shift, shift) if isinstance(shift, int) else tuple(shift)
+    if not (0 <= sy < SWIN_WINDOW and 0 <= sx < SWIN_WINDOW):
+        raise ValueError(f"window_attention needs 0 <= shift < {SWIN_WINDOW}, got {shift}")
+    return int(sy), int(sx)
+
+
+def _shift_regions(n: int, shift: int, device) -> torch.Tensor:
+    """The shift region of each shifted coordinate 0 .. n-1: [0, n-7), [n-7, n-shift), [n-shift, n); one region at shift 0."""
+    c = torch.arange(n, device=device)
+    if shift == 0:
+        return torch.zeros_like(c)
+    return (c >= n - SWIN_WINDOW).long() + (c >= n - shift).long()
+
+
+def window_attention_reference(qkv: torch.Tensor, table: torch.Tensor, batch: int, height: int, width: int, heads: int,
+                               shift) -> torch.Tensor:
+    """``window_attention`` in torch, fp32 for bf16 input: roll the map by -shift, partition it into 7 x 7 windows, dense
+    scores with the relative position bias and the -100 region mask, softmax, and the reverse partition and roll.  Needs
+    height and width multiples of 7; any head dim."""
+    sy, sx = _shift_pair(shift)
+    B, H, W, w = batch, height, width, SWIN_WINDOW
+    if H % w or W % w or qkv.dim() != 2 or qkv.shape[0] != B * H * W or qkv.shape[1] % (3 * heads):
+        raise ValueError(f"window_attention_reference needs qkv [B H W, 3C] with H and W multiples of 7, got {tuple(qkv.shape)} "
+                         f"for {B} x {H} x {W} and {heads} heads")
+    dtype = qkv.dtype if qkv.dtype in (torch.float32, torch.float64) else torch.float32
+    C = qkv.shape[1] // 3
+    d = C // heads
+    x = qkv.to(dtype).view(B, H, W, 3 * C)
+    if sy or sx:
+        x = torch.roll(x, shifts=(-sy, -sx), dims=(1, 2))
+    n = (H // w) * (W // w)
+    x = x.view(B, H // w, w, W // w, w, 3 * C).permute(0, 1, 3, 2, 4, 5).reshape(B * n, w * w, 3, heads, d).permute(2, 0, 3, 1, 4)
+    q, k, v = x[0], x[1], x[2]
+    bias = table.to(dtype)[swin_relative_position_index(table.device)].view(w * w, w * w, heads).permute(2, 0, 1)
+    attn = (q * d ** -0.5) @ k.transpose(-2, -1) + bias
+    if sy or sx:
+        region = _shift_regions(H, sy, qkv.device)[:, None] * 3 + _shift_regions(W, sx, qkv.device)[None, :]
+        region = region.view(H // w, w, W // w, w).permute(0, 2, 1, 3).reshape(n, w * w)
+        mask = torch.where(region[:, :, None] != region[:, None, :], SWIN_MASK, 0.0).to(dtype)
+        attn = (attn.view(B, n, heads, w * w, w * w) + mask[None, :, None]).view(B * n, heads, w * w, w * w)
+    o = (attn.softmax(-1) @ v).transpose(1, 2).reshape(B, H // w, W // w, w, w, C).permute(0, 1, 3, 2, 4, 5).reshape(B, H, W, C)
+    if sy or sx:
+        o = torch.roll(o, shifts=(sy, sx), dims=(1, 2))
+    return o.reshape(B * H * W, C).to(qkv.dtype)
+
+
+class _WindowAttention(torch.autograd.Function):
+    """qkv [B H W, 3C] bf16, table fp32 [169, heads] -> o [B H W, C] (csrc/swin.cu).  Backward: one kernel per window for
+    dqkv and the window's table partials, and an in-order finish for dtable."""
+
+    @staticmethod
+    def forward(ctx, qkv, table, batch, height, width, sy, sx):
+        o, lse = _C().swin.attention_fwd(qkv, table, batch, height, width, sy, sx)
+        ctx.save_for_backward(qkv, table, o, lse)
+        ctx.geometry = (batch, height, width, sy, sx)
+        return o
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, table, o, lse = ctx.saved_tensors
+        dqkv, dtable = _C().swin.attention_bwd(_aligned16(dout), qkv, o, lse, table, *ctx.geometry)
+        return dqkv, dtable, None, None, None, None, None
+
+
+def window_attention(qkv: torch.Tensor, table: torch.Tensor, batch: int, height: int, width: int, heads: int, shift) -> torch.Tensor:
+    """Swin's (shifted) window attention on raster token rows: qkv [B H W, 3C] with rows in (b, y, x) order and columns
+    [q heads | k heads | v heads] (torchvision's reshape order), table [169, heads] -> [B H W, C].  Window 7; ``shift`` is
+    an int or a (y, x) pair in [0, 7).
+
+    The token at (y, x) sits at shifted coordinates y' = (y - sy) mod H, x' = (x - sx) mod W, in window (y' / 7, x' / 7)
+    at local index i = 7 (y' % 7) + x' % 7, and scores its window's tokens j with
+    d^-0.5 q_i . k_j + table[(yi - yj + 6) 13 + (xi - xj + 6), h] - 100 [i and j lie in different shift regions]; the
+    regions are [0, H-7), [H-7, H-sy), [H-sy, H) along y' (one region when sy = 0) and the same along x'.  Each token's
+    output lands on its own row, so no roll, partition or permute is materialised.
+
+    CUDA bf16 input runs the native kernels (head dim 32; H and W multiples of 7; else ``ValueError``): fp32 softmax and
+    sums, bitwise repeatable, no host synchronisation, the table gradient summed in a fixed order and rounded once to the
+    table's dtype.  Everything else runs ``window_attention_reference``."""
+    sy, sx = _shift_pair(shift)
+    if not (qkv.is_cuda and qkv.dtype == torch.bfloat16):
+        return window_attention_reference(qkv, table, batch, height, width, heads, (sy, sx))
+    rows = batch * height * width
+    if qkv.dim() != 2 or qkv.shape[0] != rows or qkv.shape[1] != 3 * SWIN_HEAD_DIM * heads or tuple(table.shape) != (169, heads):
+        raise ValueError(f"window_attention on CUDA needs qkv [B H W, 96 heads] (head dim {SWIN_HEAD_DIM}) and table [169, heads], "
+                         f"got {tuple(qkv.shape)} and {tuple(table.shape)} for {batch} x {height} x {width} and {heads} heads")
+    if height % SWIN_WINDOW or width % SWIN_WINDOW or min(batch, height, width) < 1:
+        raise ValueError(f"window_attention on CUDA needs H and W positive multiples of {SWIN_WINDOW}, got {height} x {width}")
+    return _WindowAttention.apply(_aligned16(qkv), table.float().contiguous(), batch, height, width, sy, sx)
+
+
+# ------------------------------------------------------------------------------------------------
 # CLIP (csrc/clip.cu): captions as causal documents of one token stream, the contrastive loss over the global batch
 # ------------------------------------------------------------------------------------------------
 def caption_token_bounds(input_ids: torch.Tensor, eos_token_id: int):

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,swin,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -1115,6 +1115,82 @@ def main():
                                                                               [False, True, True]), args.iters),
                    note=f"{slots} partial slots; lib = cuDNN channels_last weight + bias gradient")
             del x, dy, xl, dyl
+
+    if "swin" in want:
+        # Swin's shifted-window attention at Swin-T's four stage shapes (batch 64) and Swin-B's first, forward and backward
+        # against torchvision's arithmetic under bf16 (roll, window partition, dense scores with the gathered bias and the
+        # mask, softmax, reverse partition and roll) and against SDPA with the per-window float bias + mask, both around
+        # the same qkv.  Bytes, from shapes: forward reads qkv and writes o and lse; backward reads qkv, o, dO and lse,
+        # writes dqkv, and writes and reads the fp32 table partials.
+        import torch.nn.functional as F
+        from b200ddp.ops import swin_relative_position_index
+        print(f"swin kernels on {card()}", flush=True)
+        index = swin_relative_position_index(dev)
+
+        def partition(t, B, Hs, Ws, sy, sx):                  # [B H W, X] -> [B nW, 49, X] in torchvision's order
+            X = t.shape[-1]
+            t = torch.roll(t.view(B, Hs, Ws, X), shifts=(-sy, -sx), dims=(1, 2)) if sy or sx else t.view(B, Hs, Ws, X)
+            return t.view(B, Hs // 7, 7, Ws // 7, 7, X).permute(0, 1, 3, 2, 4, 5).reshape(-1, 49, X)
+
+        def unpartition(t, B, Hs, Ws, sy, sx):
+            X = t.shape[-1]
+            t = t.view(B, Hs // 7, Ws // 7, 7, 7, X).permute(0, 1, 3, 2, 4, 5).reshape(B, Hs, Ws, X)
+            return (torch.roll(t, shifts=(sy, sx), dims=(1, 2)) if sy or sx else t).reshape(B * Hs * Ws, X)
+
+        def window_mask(Hs, Ws, s):
+            c = torch.arange(Hs, device=dev)
+            ry = (c >= Hs - 7).long() + (c >= Hs - s).long() if s else torch.zeros_like(c)
+            c = torch.arange(Ws, device=dev)
+            rx = (c >= Ws - 7).long() + (c >= Ws - s).long() if s else torch.zeros_like(c)
+            reg = (ry[:, None] * 3 + rx[None, :]).view(Hs // 7, 7, Ws // 7, 7).permute(0, 2, 1, 3).reshape(-1, 49)
+            return torch.where(reg[:, :, None] != reg[:, None, :], -100.0, 0.0).to(torch.bfloat16)
+
+        for name, B, Hs, heads, s in (("swin-t stage 1", 64, 56, 3, 3), ("swin-t stage 2", 64, 28, 6, 3), ("swin-t stage 3", 64, 14, 12, 3),
+                                      ("swin-t stage 4", 64, 7, 24, 0), ("swin-b stage 1", 64, 56, 4, 3)):
+            Cn, nrows = 32 * heads, B * Hs * Hs
+            g = torch.Generator(device="cuda").manual_seed(heads)
+            qkv = torch.randn(nrows, 3 * Cn, device=dev, generator=g).to(torch.bfloat16)
+            table = (torch.randn(169, heads, device=dev, generator=g) * 0.02).to(torch.bfloat16)
+            dout = torch.randn(nrows, Cn, device=dev, generator=g).to(torch.bfloat16)
+            t32 = table.float()
+            o, lse = C.swin.attention_fwd(qkv, t32, B, Hs, Hs, s, s)
+            nw = B * (Hs // 7) ** 2
+            mask = window_mask(Hs, Hs, s) if s else None
+
+            def torchvision_fwd(qkv, table):
+                x = partition(qkv, B, Hs, Hs, s, s).reshape(-1, 49, 3, heads, 32).permute(2, 0, 3, 1, 4)
+                q, k, v = x[0] * 32 ** -0.5, x[1], x[2]
+                attn = q.matmul(k.transpose(-2, -1)) + table[index].view(49, 49, heads).permute(2, 0, 1).unsqueeze(0)
+                if mask is not None:
+                    attn = (attn.view(B, -1, heads, 49, 49) + mask[None, :, None]).view(-1, heads, 49, 49)
+                y = F.softmax(attn, dim=-1).matmul(v).transpose(1, 2).reshape(-1, 49, Cn)
+                return unpartition(y, B, Hs, Hs, s, s)
+
+            def sdpa_fwd(qkv, table):
+                x = partition(qkv, B, Hs, Hs, s, s).reshape(-1, 49, 3, heads, 32).permute(2, 0, 3, 1, 4)
+                bias = table[index].view(49, 49, heads).permute(2, 0, 1).unsqueeze(0)
+                if mask is not None:
+                    bias = (bias.unsqueeze(0) + mask[None, :, None]).reshape(-1, heads, 49, 49)
+                    bias = bias.expand(B, -1, heads, 49, 49).reshape(-1, heads, 49, 49)
+                y = F.scaled_dot_product_attention(x[0], x[1], x[2], attn_mask=bias).transpose(1, 2).reshape(-1, 49, Cn)
+                return unpartition(y, B, Hs, Hs, s, s)
+
+            fwd_bytes = nrows * (3 * Cn * 2 + Cn * 2 + heads * 4)
+            bwd_bytes = nrows * (3 * Cn * 2 + 2 * Cn * 2 + heads * 4 + 3 * Cn * 2) + 2 * heads * nw * 169 * 4
+            tag = f"{name} [{B}, {Hs}x{Hs}, {heads} heads, shift {s}]"
+            lib = {}
+            for lname, fn in (("torchvision", torchvision_fwd), ("sdpa", sdpa_fwd)):
+                qg, tg = qkv.clone().requires_grad_(True), table.clone().requires_grad_(True)
+                lib[lname + " fwd"] = timeit(lambda: fn(qg, tg), args.iters)
+                y = fn(qg, tg)
+                lib[lname + " bwd"] = timeit(lambda: torch.autograd.grad(y, (qg, tg), dout, retain_graph=True), args.iters)
+                del y
+            record(f"window attention fwd {tag}", timeit(lambda: C.swin.attention_fwd(qkv, t32, B, Hs, Hs, s, s), args.iters),
+                   bytes_=fwd_bytes, lib_ms=lib["torchvision fwd"], note=f"lib = torchvision's arithmetic; sdpa {lib['sdpa fwd']:.4f} ms")
+            record(f"window attention bwd {tag}", timeit(lambda: C.swin.attention_bwd(dout, qkv, o, lse, t32, B, Hs, Hs, s, s), args.iters),
+                   bytes_=bwd_bytes, lib_ms=lib["torchvision bwd"],
+                   note=f"incl. the table-gradient finish; lib = torchvision's arithmetic; sdpa {lib['sdpa bwd']:.4f} ms")
+            del qkv, dout, o, lse
 
     if "mse" in want:
         n = 64 * 1024 * 1024
