@@ -170,12 +170,13 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext and _C.swin namespaces of static entry points
+// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin and _C.mamba namespaces of static entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
 struct T5Namespace {};
 struct ConvNextNamespace {};
 struct SwinNamespace {};
+struct MambaNamespace {};
 
 // An NHWC activation of the depthwise convolution: bf16 [B, H, W, C] contiguous and 16-byte aligned, B, H, W >= 1,
 // 8 <= C <= 1024 with C % 8 == 0 (B is the grid's z extent).  Returns (B, H, W, C).
@@ -204,6 +205,29 @@ std::array<int64_t, 2> swin_args(Args& args, const at::Tensor& qkv, const at::Te
   if (rows * 96 * heads >= (1ll << 31)) args.fail("geometry", "at most 2^31 qkv elements", geometry());
   args("qkv", qkv, {kBF16}, {rows, 96 * heads}, kContiguous, 16);
   return {rows, heads};
+}
+
+// Mamba's token rows: bounds int32 [B, S, 2] contiguous and 8-byte aligned (the kernels read int2) with 1 <= B <= 65535, then
+// xz bf16 [B S, 2E] contiguous and 16-byte aligned with E a positive multiple of 8 and B S 2E < 2^31.  Returns (B, S, E).
+std::array<int64_t, 3> mamba_args(Args& args, const at::Tensor& bounds, const at::Tensor& xz) {
+  args("bounds", bounds, {kI32}, {kAny, kAny, 2}, kContiguous, 8);
+  const int64_t B = bounds.size(0), S = bounds.size(1);
+  if (B < 1 || B > 65535 || S < 1) args.fail("bounds", "int32 [B, S, 2] with 1 <= B <= 65535 and S >= 1", describe(bounds));
+  args("xz", xz, {kBF16}, {B * S, kAny}, kContiguous, 16);
+  const int64_t E = xz.size(1) / 2;
+  if (xz.size(1) % 16 || E < 8 || B * S * 2 * E >= (1ll << 31))
+    args.fail("xz", "bf16 [B S, 2E] with E a positive multiple of 8 and fewer than 2^31 elements", describe(xz));
+  return {B, S, E};
+}
+
+// the selective scan's inputs after bounds and xz: u and draw bf16 [T, E], xbc bf16 [T, R + 32] (R >= 0), A_log fp32 [E, 16],
+// D and dt_bias fp32 [E], all contiguous.  Returns R.
+int64_t mamba_scan_args(Args& args, int64_t T, int64_t E, const at::Tensor& u, const at::Tensor& draw, const at::Tensor& xbc,
+                        const at::Tensor& A_log, const at::Tensor& D, const at::Tensor& dt_bias) {
+  args("u", u, {kBF16}, {T, E})("draw", draw, {kBF16}, {T, E})("xbc", xbc, {kBF16}, {T, kAny});
+  if (xbc.size(1) < 32) args.fail("xbc", "bf16 [T, R + 32] with R >= 0 (dt | B | C)", describe(xbc));
+  args("A_log", A_log, {kF32}, {E, 16})("D", D, {kF32}, {E})("dt_bias", dt_bias, {kF32}, {E});
+  return xbc.size(1) - 32;
 }
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
@@ -1845,4 +1869,79 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(dqkv, dtable);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("table"), py::arg("batch"), py::arg("height"),
      py::arg("width"), py::arg("shift_y"), py::arg("shift_x"));
+
+  // ---- Mamba's causal conv1d + SiLU and selective scan (mamba.cu), bf16 token rows ----------------------------------------
+  // _C.mamba is a namespace of static entry points like _C.swin; its contract rows are in tests/test_mamba_bindings_cpu.py.
+  // bounds int32 [B, S, 2], xz bf16 [B S, 2E] = x | z, conv weight fp32 [E, 4] and bias fp32 [E], u / draw / y bf16 [B S, E],
+  // xbc bf16 [B S, R + 32] = dt | B | C, A_log fp32 [E, 16], D / dt_bias fp32 [E].
+  py::class_<MambaNamespace> mamba(m, "mamba", "Mamba's causal conv1d and selective scan on token rows (mamba.cu)");
+  // u bf16 [B S, E]
+  mamba.def_static("conv_fwd", [](at::Tensor xz, at::Tensor weight, at::Tensor bias, at::Tensor bounds) {
+    Args args("conv_fwd");
+    const auto [B, S, E] = mamba_args(args, bounds, xz);
+    args("weight", weight, {kF32}, {E, 4}, kContiguous, 16)("bias", bias, {kF32}, {E});
+    args.device();
+    at::Tensor u = at::empty({B * S, E}, xz.options());
+    launch_mamba_conv_fwd(xz.data_ptr(), weight.data_ptr<float>(), bias.data_ptr<float>(), bounds.data_ptr<int>(), (int)B, (int)S, (int)E,
+                          u.data_ptr(), cur_stream());
+    return u;
+  }, py::arg("xz"), py::arg("weight"), py::arg("bias"), py::arg("bounds"));
+  // (dxz bf16 [B S, 2E] with the x half written: dxz_out when given, whose z half is left as it is; dweight fp32 [E, 4];
+  // dbias fp32 [E])
+  mamba.def_static("conv_bwd", [](at::Tensor du, at::Tensor xz, at::Tensor weight, at::Tensor bias, at::Tensor bounds,
+                                  c10::optional<at::Tensor> dxz_out) {
+    Args args("conv_bwd");
+    const auto [B, S, E] = mamba_args(args, bounds, xz);
+    args("du", du, {kBF16}, {B * S, E}, kContiguous, 16)("weight", weight, {kF32}, {E, 4}, kContiguous, 16)("bias", bias, {kF32}, {E});
+    at::Tensor dxz;
+    args.out(dxz, "dxz_out", dxz_out, {B * S, 2 * E}, xz.options(), 16);
+    args.device();
+    at::Tensor part = at::empty({(int64_t)mamba_conv_blocks((int)B, (int)S), 5, E}, xz.options().dtype(kF32));
+    at::Tensor dweight = at::empty({E, 4}, xz.options().dtype(kF32));
+    at::Tensor dbias = at::empty({E}, xz.options().dtype(kF32));
+    launch_mamba_conv_bwd(du.data_ptr(), xz.data_ptr(), weight.data_ptr<float>(), bias.data_ptr<float>(), bounds.data_ptr<int>(), (int)B,
+                          (int)S, (int)E, dxz.data_ptr(), part.data_ptr<float>(), dweight.data_ptr<float>(), dbias.data_ptr<float>(),
+                          cur_stream());
+    return std::make_tuple(dxz.view({B * S, 2 * E}), dweight, dbias);
+  }, py::arg("du"), py::arg("xz"), py::arg("weight"), py::arg("bias"), py::arg("bounds"), py::arg("dxz_out") = py::none());
+  // (y bf16 [B S, E], hstart fp32 [B, chunks, E, 16], sumd fp32 [B, chunks, E]), chunks = ceil(S / 128)
+  mamba.def_static("scan_fwd", [](at::Tensor u, at::Tensor draw, at::Tensor xbc, at::Tensor xz, at::Tensor A_log, at::Tensor D,
+                                  at::Tensor dt_bias, at::Tensor bounds) {
+    Args args("scan_fwd");
+    const auto [B, S, E] = mamba_args(args, bounds, xz);
+    const int64_t R = mamba_scan_args(args, B * S, E, u, draw, xbc, A_log, D, dt_bias);
+    args.device();
+    const int64_t nc = mamba_chunks((int)S);
+    at::Tensor y = at::empty({B * S, E}, xz.options());
+    at::Tensor hst = at::empty({B, nc, E, 16}, xz.options().dtype(kF32));
+    at::Tensor sumd = at::empty({B, nc, E}, xz.options().dtype(kF32));
+    launch_mamba_scan_fwd(u.data_ptr(), draw.data_ptr(), xbc.data_ptr(), xz.data_ptr(), A_log.data_ptr<float>(), D.data_ptr<float>(),
+                          dt_bias.data_ptr<float>(), bounds.data_ptr<int>(), (int)B, (int)S, (int)E, (int)R, y.data_ptr(), hst.data_ptr<float>(),
+                          sumd.data_ptr<float>(), cur_stream());
+    return std::make_tuple(y, hst, sumd);
+  }, py::arg("u"), py::arg("draw"), py::arg("xbc"), py::arg("xz"), py::arg("A_log"), py::arg("D"), py::arg("dt_bias"), py::arg("bounds"));
+  // (du bf16 [B S, E], ddraw bf16 [B S, E], dxbc bf16 [B S, R + 32] with zero dt columns, dxz bf16 [B S, 2E] with the z half
+  // written and the x half left for conv_bwd, dA_log fp32 [E, 16], dD fp32 [E], ddt_bias fp32 [E])
+  mamba.def_static("scan_bwd", [](at::Tensor dy, at::Tensor u, at::Tensor draw, at::Tensor xbc, at::Tensor xz, at::Tensor A_log, at::Tensor D,
+                                  at::Tensor dt_bias, at::Tensor bounds, at::Tensor hstart, at::Tensor sumd) {
+    Args args("scan_bwd");
+    const auto [B, S, E] = mamba_args(args, bounds, xz);
+    const int64_t R = mamba_scan_args(args, B * S, E, u, draw, xbc, A_log, D, dt_bias);
+    const int64_t nc = mamba_chunks((int)S), groups = mamba_groups((int)E);
+    args("dy", dy, {kBF16}, {B * S, E})("hstart", hstart, {kF32}, {B, nc, E, 16})("sumd", sumd, {kF32}, {B, nc, E});
+    args.device();
+    const auto f32 = xz.options().dtype(kF32);
+    at::Tensor dq = at::empty({B, nc, E, 16}, f32), dbc_part = at::empty({B * S, groups, 32}, f32);
+    at::Tensor dA_part = at::empty({B * nc, E, 16}, f32), dD_part = at::empty({B * nc, E}, f32), dbias_part = at::empty({B * nc, E}, f32);
+    at::Tensor du = at::empty({B * S, E}, xz.options()), ddraw = at::empty({B * S, E}, xz.options());
+    at::Tensor dxbc = at::empty({B * S, R + 32}, xz.options()), dxz = at::empty({B * S, 2 * E}, xz.options());
+    at::Tensor dA_log = at::empty({E, 16}, f32), dD = at::empty({E}, f32), dbias = at::empty({E}, f32);
+    launch_mamba_scan_bwd(dy.data_ptr(), u.data_ptr(), draw.data_ptr(), xbc.data_ptr(), xz.data_ptr(), A_log.data_ptr<float>(),
+                          D.data_ptr<float>(), dt_bias.data_ptr<float>(), bounds.data_ptr<int>(), hstart.data_ptr<float>(), sumd.data_ptr<float>(),
+                          (int)B, (int)S, (int)E, (int)R, dq.data_ptr<float>(), dbc_part.data_ptr<float>(), dA_part.data_ptr<float>(),
+                          dD_part.data_ptr<float>(), dbias_part.data_ptr<float>(), du.data_ptr(), ddraw.data_ptr(), dxbc.data_ptr(), dxz.data_ptr(),
+                          dA_log.data_ptr<float>(), dD.data_ptr<float>(), dbias.data_ptr<float>(), cur_stream());
+    return std::make_tuple(du, ddraw, dxbc, dxz, dA_log, dD, dbias);
+  }, py::arg("dy"), py::arg("u"), py::arg("draw"), py::arg("xbc"), py::arg("xz"), py::arg("A_log"), py::arg("D"), py::arg("dt_bias"),
+     py::arg("bounds"), py::arg("hstart"), py::arg("sumd"));
 }

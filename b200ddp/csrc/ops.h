@@ -282,6 +282,29 @@ void launch_swin_attention_fwd(const void* qkv, const float* table, int B, int H
 void launch_swin_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const float* table, int B, int H, int W,
                                int heads, int sy, int sx, void* dqkv, float* part, float* dtable, cudaStream_t s);
 
+// ---------------- Mamba causal conv1d + SiLU and selective scan (mamba.cu), bf16 token rows -------------------------------
+// T = B S rows; bounds int32 [B, S, 2] (document (start, end) per position, start == end for padding); E % 8 == 0, N = 16,
+// conv width 4.  xz bf16 [T, 2E] = x | z, u / draw / y bf16 [T, E], xbc bf16 [T, R + 32] = dt | B | C; A_log fp32 [E, 16],
+// D / dt_bias fp32 [E]; conv weight fp32 [E, 4], bias fp32 [E].  No atomics, no host synchronisation.
+int mamba_conv_blocks(int B, int S);
+int mamba_chunks(int S);
+int mamba_groups(int E);
+void launch_mamba_conv_fwd(const void* xz, const float* w, const float* bias, const int* bounds, int B, int S, int E, void* u, cudaStream_t s);
+// dx into the x half of dxz [T, 2E]; dw fp32 [E, 4], db fp32 [E] through part fp32 [mamba_conv_blocks(B, S), 5, E]
+void launch_mamba_conv_bwd(const void* du, const void* xz, const float* w, const float* bias, const int* bounds, int B, int S, int E, void* dxz,
+                           float* part, float* dw, float* db, cudaStream_t s);
+// hst fp32 [B, mamba_chunks(S), E, 16] (each chunk's start state, kept for the backward), sumd fp32 [B, chunks, E]
+void launch_mamba_scan_fwd(const void* u, const void* draw, const void* xbc, const void* xz, const float* A_log, const float* D,
+                           const float* dt_bias, const int* bounds, int B, int S, int E, int R, void* y, float* hst, float* sumd,
+                           cudaStream_t s);
+// du, ddraw bf16 [T, E]; dz into the z half of dxz [T, 2E]; dxbc bf16 [T, R + 32] (zero dt columns); dA_log fp32 [E, 16],
+// dD, dbias fp32 [E].  Scratch: dq fp32 like hst, dbc_part fp32 [T, mamba_groups(E), 32], dA_part fp32 [B chunks, E, 16],
+// dD_part and dbias_part fp32 [B chunks, E]
+void launch_mamba_scan_bwd(const void* dy, const void* u, const void* draw, const void* xbc, const void* xz, const float* A_log, const float* D,
+                           const float* dt_bias, const int* bounds, const float* hst, const float* sumd, int B, int S, int E, int R,
+                           float* dq, float* dbc_part, float* dA_part, float* dD_part, float* dbias_part, void* du, void* ddraw, void* dxbc,
+                           void* dxz, float* dA_log, float* dD, float* dbias, cudaStream_t s);
+
 // ---------------- CLIP contrastive loss (clip.cu) ---------------------------------------------------
 // u bf16 [B, D] = x / ||x|| per row (fp32, one rounding), rnorm fp32 [B] = 1 / ||x||; D % 8 == 0, 16-byte aligned rows
 void launch_l2norm_fwd(const void* x, int B, int D, void* u, float* rnorm, cudaStream_t s);

@@ -1968,6 +1968,208 @@ def window_attention(qkv: torch.Tensor, table: torch.Tensor, batch: int, height:
 
 
 # ------------------------------------------------------------------------------------------------
+# Mamba (csrc/mamba.cu): causal depthwise conv1d + SiLU and the selective scan on token rows, reset at document starts
+# ------------------------------------------------------------------------------------------------
+MAMBA_CONV_WIDTH = 4
+MAMBA_STATE = 16
+MAMBA_SOFTPLUS_THRESHOLD = 20.0      # torch's softplus threshold
+
+
+def _ref_dtype(t: torch.Tensor):
+    return torch.float64 if t.dtype == torch.float64 else torch.float32
+
+
+def _mamba_positions(bounds: torch.Tensor, device):
+    """(real [B, S], start [B, S] long, reset [B, S]) from document bounds: a position is real when start < end, and the
+    state resets at a document's first position."""
+    b = bounds.to(device=device, dtype=torch.long)
+    S = b.shape[1]
+    pos = torch.arange(S, device=device)
+    real = b[..., 0] < b[..., 1]
+    start = b[..., 0].clamp(min=0)
+    return real, start, real & ((start >= pos) | (pos == 0))
+
+
+def causal_conv1d_reference(xz: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, bounds: torch.Tensor) -> torch.Tensor:
+    """``causal_conv1d`` in torch, fp32 (fp64 for fp64 input): u[t] = silu(bias + sum_j w[:, j] x[t - 3 + j]) with x the first
+    half of xz [B, S, 2E], taps before the document start reading zero and padding positions giving zero.  Differentiable."""
+    dtype = _ref_dtype(xz)
+    B, S, E2 = xz.shape
+    E = E2 // 2
+    x = xz[..., :E].to(dtype)
+    w = weight.reshape(E, MAMBA_CONV_WIDTH).to(dtype)
+    real, start, _ = _mamba_positions(bounds, xz.device)
+    pos = torch.arange(S, device=xz.device)
+    pre = bias.to(dtype).expand(B, S, E)
+    for j in range(MAMBA_CONV_WIDTH):
+        shift = MAMBA_CONV_WIDTH - 1 - j
+        xs = F.pad(x, (0, 0, shift, 0))[:, :S]
+        keep = (pos - shift >= start) & real
+        pre = pre + w[:, j] * torch.where(keep[..., None], xs, torch.zeros_like(xs))
+    return torch.where(real[..., None], F.silu(pre), torch.zeros_like(pre)).to(xz.dtype)
+
+
+def selective_scan_reference(u: torch.Tensor, delta_raw: torch.Tensor, xbc: torch.Tensor, xz: torch.Tensor, A_log: torch.Tensor,
+                             D: torch.Tensor, dt_bias: torch.Tensor, bounds: torch.Tensor) -> torch.Tensor:
+    """``selective_scan`` in torch, fp32 (fp64 for fp64 input), a loop over the sequence as in transformers'
+    ``MambaMixer.slow_forward`` with the state reset at each document start and zero output at padding.  Differentiable."""
+    dtype = _ref_dtype(u)
+    B, S, E = u.shape
+    N = MAMBA_STATE
+    R = xbc.shape[-1] - 2 * N
+    uu, z = u.to(dtype), xz[..., E:].to(dtype)
+    Bm, Cm = xbc[..., R:R + N].to(dtype), xbc[..., R + N:].to(dtype)
+    delta = F.softplus(delta_raw.to(dtype) + dt_bias.to(dtype), threshold=MAMBA_SOFTPLUS_THRESHOLD)
+    A = -torch.exp(A_log.to(dtype))
+    real, _, reset = _mamba_positions(bounds, u.device)
+    h = torch.zeros(B, E, N, dtype=dtype, device=u.device)
+    ys = []
+    for t in range(S):
+        dA = torch.exp(delta[:, t, :, None] * A)
+        h = torch.where(reset[:, t, None, None], torch.zeros_like(h), dA * h) + delta[:, t, :, None] * Bm[:, t, None, :] * uu[:, t, :, None]
+        h = torch.where(real[:, t, None, None], h, torch.zeros_like(h))
+        ys.append((h * Cm[:, t, None, :]).sum(-1))
+    y = (torch.stack(ys, 1) + uu * D.to(dtype)) * F.silu(z)
+    return torch.where(real[..., None], y, torch.zeros_like(y)).to(u.dtype)
+
+
+class MambaGradLink:
+    """Hands the [T, 2E] gradient buffer of in_proj's output from ``selective_scan``'s backward, which writes its z half,
+    to ``causal_conv1d``'s backward, which writes its x half and returns it whole: no zero fill, no add, no concatenation.
+    Pass one fresh link to both ops of a mixer; the scan's backward always runs first (its input u is the conv's output)."""
+
+    def __init__(self):
+        self.dxz = None
+
+
+def _mamba_check(who: str, xz: torch.Tensor, bounds: torch.Tensor) -> None:
+    if xz.dim() != 3 or tuple(bounds.shape) != (xz.shape[0], xz.shape[1], 2) or bounds.is_floating_point() or bounds.is_complex():
+        raise ValueError(f"{who} needs xz [B, S, 2E] and integer bounds [B, S, 2], got {tuple(xz.shape)} and {bounds.dtype} "
+                         f"{tuple(bounds.shape)}")
+    if xz.shape[-1] % 16 or xz.shape[-1] == 0:
+        raise ValueError(f"{who} needs E = xz.shape[-1] / 2 a positive multiple of 8, got xz {tuple(xz.shape)}")
+
+
+def _mamba_native(who: str, *ts: torch.Tensor) -> bool:
+    """True for CUDA bf16 activations (the native kernels), False for CPU ones or CUDA fp32 / fp64 ones (the reference);
+    any other CUDA dtype, or a mix, raises ``ValueError`` rather than falling back to the reference's loop."""
+    if not any(t.is_cuda for t in ts):
+        return False
+    dtypes = {t.dtype for t in ts}
+    if all(t.is_cuda for t in ts) and dtypes == {torch.bfloat16}:
+        return True
+    if all(t.is_cuda for t in ts) and dtypes <= {torch.float32, torch.float64}:
+        return False
+    raise ValueError(f"{who} on CUDA needs bf16 activations (the native kernels) or fp32 / fp64 ones (the reference), got "
+                     f"{[str(t.dtype) for t in ts]} on {[str(t.device) for t in ts]}")
+
+
+def _rows(t: torch.Tensor) -> torch.Tensor:
+    return _aligned16(t.reshape(-1, t.shape[-1]))
+
+
+class _CausalConv1d(torch.autograd.Function):
+    """xz [B, S, 2E] bf16 -> u [B, S, E] (csrc/mamba.cu).  Backward: dx into the x half of the link's buffer (or a new one
+    with a zero z half), fp32 weight and bias gradients summed in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, xz, weight, bias, bounds, link):
+        B, S, E2 = xz.shape
+        x2, w, b = _rows(xz), weight.reshape(E2 // 2, MAMBA_CONV_WIDTH).float().contiguous(), bias.float().contiguous()
+        bd = _aligned16(bounds.to(torch.int32))                      # the kernels read (start, end) as int2
+        ctx.save_for_backward(x2, w, b, bd)
+        ctx.link, ctx.dtypes, ctx.weight_shape = link, (weight.dtype, bias.dtype), weight.shape
+        return _C().mamba.conv_fwd(x2, w, b, bd).view(B, S, E2 // 2)
+
+    @staticmethod
+    def backward(ctx, du):
+        x2, w, b, bd = ctx.saved_tensors
+        link = ctx.link
+        given = link.dxz if link is not None else None
+        dxz, dw, db = _C().mamba.conv_bwd(_rows(du), x2, w, b, bd, given)
+        if given is None:
+            dxz[:, dxz.shape[1] // 2:].zero_()
+        else:
+            link.dxz = None
+        return (dxz.view(*du.shape[:2], -1), dw.view(ctx.weight_shape).to(ctx.dtypes[0]), db.to(ctx.dtypes[1]), None, None)
+
+
+def causal_conv1d(xz: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, bounds: torch.Tensor,
+                  link: Optional[MambaGradLink] = None) -> torch.Tensor:
+    """Mamba's causal depthwise convolution of width 4 with SiLU over the x half of in_proj's output xz [B, S, 2E]:
+    u[t] = silu(bias + sum_j weight[:, 0, j] x[t - 3 + j]), weight [E, 1, 4], bias [E].  Taps before the document start
+    of ``bounds`` (int32 [B, S, 2], ``document_bounds``) read zero, and padding positions (start == end) give zero.
+
+    CUDA bf16 xz runs the native kernels (E % 8 == 0, else ``ValueError``): fp32 sums with one bf16 rounding, bitwise
+    repeatable, no host synchronisation; its data gradient lands in the x half of the [B, S, 2E] gradient, whose z half
+    ``selective_scan`` fills when both get the same ``link``.  CPU input, and CUDA fp32 or fp64 input, run
+    ``causal_conv1d_reference``; CUDA input of any other dtype raises ``ValueError``."""
+    _mamba_check("causal_conv1d", xz, bounds)
+    E = xz.shape[-1] // 2
+    if tuple(weight.shape) != (E, 1, MAMBA_CONV_WIDTH) or tuple(bias.shape) != (E,):
+        raise ValueError(f"causal_conv1d needs weight [E, 1, 4] and bias [E] for E = {E}, got {tuple(weight.shape)} and {tuple(bias.shape)}")
+    if not _mamba_native("causal_conv1d", xz):
+        return causal_conv1d_reference(xz, weight, bias, bounds)
+    return _CausalConv1d.apply(xz, weight, bias, bounds, link)
+
+
+class _SelectiveScan(torch.autograd.Function):
+    """(u, delta_raw [B, S, E], xbc [B, S, R + 32], xz [B, S, 2E]) bf16 -> y [B, S, E] (csrc/mamba.cu); each chunk's fp32
+    start state is kept for the backward."""
+
+    @staticmethod
+    def forward(ctx, u, delta_raw, xbc, xz, A_log, D, dt_bias, bounds, link):
+        B, S, E = u.shape
+        ins = [_rows(u), _rows(delta_raw), _rows(xbc), _rows(xz), A_log.float().contiguous(), D.float().contiguous(),
+               dt_bias.float().contiguous(), _aligned16(bounds.to(torch.int32))]
+        y, hst, sumd = _C().mamba.scan_fwd(*ins)
+        ctx.save_for_backward(*ins, hst, sumd)
+        ctx.link, ctx.dtypes, ctx.shapes = link, (A_log.dtype, D.dtype, dt_bias.dtype), (u.shape, xbc.shape, xz.shape)
+        return y.view(B, S, E)
+
+    @staticmethod
+    def backward(ctx, dy):
+        du, ddraw, dxbc, dxz, dA_log, dD, dbias = _C().mamba.scan_bwd(_rows(dy), *ctx.saved_tensors)
+        ushape, xbcshape, xzshape = ctx.shapes
+        if ctx.link is not None:
+            ctx.link.dxz, dxz = dxz, None
+        else:
+            dxz[:, :xzshape[-1] // 2].zero_()
+            dxz = dxz.view(xzshape)
+        tA, tD, tb = ctx.dtypes
+        return (du.view(ushape), ddraw.view(ushape), dxbc.view(xbcshape), dxz, dA_log.to(tA), dD.to(tD), dbias.to(tb), None, None)
+
+
+def selective_scan(u: torch.Tensor, delta_raw: torch.Tensor, xbc: torch.Tensor, xz: torch.Tensor, A_log: torch.Tensor, D: torch.Tensor,
+                   dt_bias: torch.Tensor, bounds: torch.Tensor, link: Optional[MambaGradLink] = None) -> torch.Tensor:
+    """Mamba-1's selective scan with the state reset at every document start: per row, channel e and state n,
+    delta = softplus(delta_raw + dt_bias) (threshold 20), A = -exp(A_log),
+    h_t = exp(delta_t A) h_{t-1} + delta_t B_t u_t with h = 0 before each document, y_t = (C_t . h_t + D u_t) silu(z_t).
+    u and delta_raw [B, S, E]; xbc [B, S, R + 32] is x_proj's output dt | B | C (B and C read in place); z is the second
+    half of xz [B, S, 2E]; A_log [E, 16]; D and dt_bias [E]; bounds int32 [B, S, 2] (``document_bounds``).  Padding
+    positions give y = 0 and zero gradients.
+
+    CUDA bf16 activations run the native chunked scan (E % 8 == 0 and N = 16, else ``ValueError``): the state is fp32
+    throughout, gradients are summed in a fixed order (bitwise repeatable), nothing is read back to the host.  The
+    gradient of xz has its z half only; with a ``link`` shared with ``causal_conv1d`` the conv's backward completes and
+    returns it.  CPU activations, and CUDA fp32 or fp64 ones, run ``selective_scan_reference``; CUDA activations of
+    any other dtype, or of mixed dtypes, raise ``ValueError``."""
+    _mamba_check("selective_scan", xz, bounds)
+    B, S, E2 = xz.shape
+    E = E2 // 2
+    if tuple(u.shape) != (B, S, E) or tuple(delta_raw.shape) != (B, S, E) or xbc.dim() != 3 or tuple(xbc.shape[:2]) != (B, S) \
+            or xbc.shape[-1] < 2 * MAMBA_STATE:
+        raise ValueError(f"selective_scan needs u and delta_raw [B, S, E] = [{B}, {S}, {E}] and xbc [B, S, R + 32], got "
+                         f"{tuple(u.shape)}, {tuple(delta_raw.shape)} and {tuple(xbc.shape)}")
+    if tuple(A_log.shape) != (E, MAMBA_STATE) or tuple(D.shape) != (E,) or tuple(dt_bias.shape) != (E,):
+        raise ValueError(f"selective_scan needs A_log [E, 16] and D, dt_bias [E] for E = {E}, got {tuple(A_log.shape)}, "
+                         f"{tuple(D.shape)} and {tuple(dt_bias.shape)}")
+    if not _mamba_native("selective_scan", u, delta_raw, xbc, xz):
+        return selective_scan_reference(u, delta_raw, xbc, xz, A_log, D, dt_bias, bounds)
+    return _SelectiveScan.apply(u, delta_raw, xbc, xz, A_log, D, dt_bias, bounds, link)
+
+
+# ------------------------------------------------------------------------------------------------
 # CLIP (csrc/clip.cu): captions as causal documents of one token stream, the contrastive loss over the global batch
 # ------------------------------------------------------------------------------------------------
 def caption_token_bounds(input_ids: torch.Tensor, eos_token_id: int):

@@ -20,7 +20,7 @@ def to_mixed_bf16(model: nn.Module, keep_norm_fp32: bool = True) -> nn.Module:
                 m.float()
     for m in model.modules():
         for name in getattr(m, "keep_fp32_params", ()):
-            p = getattr(m, name)
+            p = m.get_parameter(name)                 # a dotted name reaches into a child (Mamba's "dt_proj.bias")
             p.data = p.data.float()
     return model
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,swin,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,swin,mamba,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -1216,6 +1216,56 @@ def main():
             print(f"H2D pinned {label:32s} {ms:8.3f} ms {nbytes / ms / 1e6:8.1f} GB/s", flush=True)
             ms = timeit(lambda: host.copy_(devb, non_blocking=True), args.iters, flush=False)
             print(f"D2H pinned {label:32s} {ms:8.3f} ms {nbytes / ms / 1e6:8.1f} GB/s", flush=True)
+
+    if "mamba" in want:
+        # Mamba's causal conv1d + SiLU and selective scan at mamba-130m's and mamba-370m's layer shapes (8 x 2048 rows, E 1536 /
+        # 2048, dt rank 48 / 64) on fixed, right-padded (lengths U[256, 2048]) and packed rows.  Algorithmic bytes, from shapes:
+        # conv forward reads x and writes u; its backward reads du and x, writes dx and the fp32 weight partials.  Scan
+        # forward reads u, delta_raw, z, B and C, writes y and the fp32 chunk start states; its backward reads dy, u,
+        # delta_raw, z, B and C (4 E + 32 columns per row) and the start states, writes du, d delta_raw, dz (3 E) and the
+        # x_proj-output gradient (R + 32), and writes and reads the fp32 chunk carries (one start-state size each way).  The torch reference (fp32 arithmetic, a loop over
+        # the sequence like transformers' slow_forward) is the baseline: the conv forward, and the scan forward timed
+        # over 2 calls.
+        from b200ddp.ops import causal_conv1d, causal_conv1d_reference, document_bounds, selective_scan, selective_scan_reference
+        print(f"mamba kernels on {card()}", flush=True)
+        Bm, Sm = 8, 2048
+        for label, E, R in (("mamba-130m", 1536, 48), ("mamba-370m", 2048, 64)):
+            g = torch.Generator(device="cuda").manual_seed(E)
+            for layout in ("fixed", "padded", "packed"):
+                ids = torch.randint(2, 1000, (Bm, Sm), device=dev, generator=g)
+                if layout != "fixed":
+                    lens = torch.randint(256, Sm + 1, (Bm, 1), device=dev, generator=g)
+                    ids = torch.where(torch.arange(Sm, device=dev) < lens, ids, 0)
+                    if layout == "packed":
+                        ids = torch.where(torch.rand(Bm, Sm, device=dev, generator=g) < 1 / 512, 1, ids) * (ids != 0)
+                bounds = document_bounds(ids, 1 if layout == "packed" else None, None if layout == "fixed" else 0)[0].to(torch.int32)
+                xz = torch.randn(Bm, Sm, 2 * E, device=dev, generator=g).to(torch.bfloat16)
+                w = (torch.randn(E, 1, 4, device=dev, generator=g) * 0.5).to(torch.bfloat16)
+                cb = torch.zeros(E, device=dev, dtype=torch.bfloat16)
+                dr = torch.randn(Bm, Sm, E, device=dev, generator=g).to(torch.bfloat16)
+                xbc = torch.randn(Bm, Sm, R + 32, device=dev, generator=g).to(torch.bfloat16)
+                A_log = torch.log(torch.arange(1, 17.0, device=dev)).repeat(E, 1)
+                D, dtb = torch.ones(E, device=dev), torch.full((E,), -4.0, device=dev)
+                T = Bm * Sm
+                w32, b32, x2 = w.reshape(E, 4).float(), cb.float(), xz.view(T, 2 * E)
+                u2 = C.mamba.conv_fwd(x2, w32, b32, bounds)
+                ms = timeit(lambda: C.mamba.conv_fwd(x2, w32, b32, bounds), args.iters)
+                lib = timeit(lambda: causal_conv1d_reference(xz, w, cb, bounds), args.iters)
+                record(f"{label} conv fwd {layout}", ms, bytes_=T * E * 2 * 2, lib_ms=lib, note="lib: torch reference")
+                du = torch.randn(T, E, device=dev, generator=g).to(torch.bfloat16)
+                ms = timeit(lambda: C.mamba.conv_bwd(du, x2, w32, b32, bounds), args.iters)
+                record(f"{label} conv bwd {layout}", ms, bytes_=T * E * 2 * 3 + 2 * 5 * E * 4 * Bm * Sm // 32)
+                sargs = (u2, dr.view(T, E), xbc.view(T, R + 32), x2, A_log, D, dtb, bounds)
+                y, hst, sumd = C.mamba.scan_fwd(*sargs)
+                state_bytes = hst.numel() * 4
+                ms = timeit(lambda: C.mamba.scan_fwd(*sargs), args.iters)
+                u3 = u2.view(Bm, Sm, E)
+                lib = timeit(lambda: selective_scan_reference(u3, dr, xbc, xz, A_log, D, dtb, bounds), 2, flush=False)
+                record(f"{label} scan fwd {layout}", ms, bytes_=T * (4 * E * 2 + 32 * 2) + state_bytes, lib_ms=lib,
+                       note="lib: torch reference")
+                dy = torch.randn(T, E, device=dev, generator=g).to(torch.bfloat16)
+                ms = timeit(lambda: C.mamba.scan_bwd(dy, *sargs, hst, sumd), args.iters)
+                record(f"{label} scan bwd {layout}", ms, bytes_=T * (7 * E * 2 + (32 + R + 32) * 2) + 3 * state_bytes)
 
     if args.out:
         os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
