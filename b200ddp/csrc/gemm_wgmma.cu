@@ -232,9 +232,11 @@ __device__ __forceinline__ void lm_epilogue_tile(const GemmParams& p, const floa
       float v[32];
       acc_row_ld32(arow, 0, 0, c, r);
       epilogue_math(p, n0 + c, r, v);
+      // A row without a gradient (ignored, no valid row, or past a row-bounded count, whose lse reads 0) writes zeros
+      // without its exponential: a logit above ~88.7 would make it inf, and inf * 0 = NaN.
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
-        float d = __expf(__bfloat162float(__float2bfloat16_rn(v[i])) - lse);
+        float d = coef != 0.f ? __expf(__bfloat162float(__float2bfloat16_rn(v[i])) - lse) : 0.f;
         if (tcol == c + i) d -= 1.f;
         v[i] = d * coef;
       }

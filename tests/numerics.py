@@ -22,7 +22,7 @@ reaches at most 0.037 of the lse bound at C_ACC = 2 and 0.23 at C_ACC = 0.25, an
 has no bf16 rounding to hide behind, so it is what calibrates C_ACC there.  EXP_ULPS = 0 passes as well as 2: no bound
 is filled by the exp2 terms, so EXP_ULPS stays at exp2f's documented maximum.  Its bf16 outputs reach 0.95.
 
-ResNet-50 (the last section).  The convolutions (conv_wgmma.cu, conv_wgrad_wgmma.cu, the stem) are GEMMs on the tensor
+ResNet-50 (its own section below).  The convolutions (conv_wgmma.cu, conv_wgrad_wgmma.cu, the stem) are GEMMs on the tensor
 cores and take the GEMM bound with the same C_ACC, P being the same convolution of the absolute values:
   fprop   K = R S Cin (the stem: 147; its packed layout only adds exact zero products)
   dgrad   K = R S Cout, plus one term for the fp32 addend the epilogue adds before rounding
@@ -46,6 +46,16 @@ On an H100 80GB HBM3 (700 W power limit) test_gpu_conv_elementwise.py and test_g
 at C_ACC = 2: conv fprop 0.992, dgrad 0.993, wgrad 0.994 and stem 0.984 / 0.926 (bf16 outputs, filled by their rounding
 term); epilogue statistics 0.065, fused S1 / S2 0.037; BatchNorm y and dx 0.996, mean 0.11, rstd 0.12 (0.061 with every
 channel at |mean| = 64σ), running statistics 0.38, dgamma / dbeta 0.073; max pool 0.996; MSE dout 0.996, loss 0.033.
+
+Cross-entropy (the last section; its derivation is in lm_loss_reference's docstring).  The references take the kernels'
+own bf16 logits (gemm_nt of the same operands) as exact inputs, so the softmax bounds stay at fp32 level: the error of
+each term exp(x_j - m) is carried by __expf's documented 2 + ⌊1.173 |x|⌋ ulp over the arguments along its path (they
+add up to m - x_j), the rescales and the fp32 sums in the kernels' order; lse takes Σ p_j ρ_j, __logf and the final add.
+The gradients (dh, dw, dbias of the fused head; dlogits of xent_fwd_bwd) take that error times p, the coefficient's
+roundings and the GEMM or column-sum bound.  On an H100 80GB HBM3 (700 W power limit) test_gpu_lm_loss_elementwise.py
+reaches at most, over two runs: lse 0.34, row_loss 0.70, loss 0.11 (fp32); dh 0.93, dw 0.98, dbias 0.79 (bf16, filled
+by their rounding term); xent_fwd_bwd dlogits 0.99 in bf16 and 0.29 in fp32, through autograd with g = 0.7: 0.80 / 0.20;
+loss 0.091.  The grouped expert GEMMs of test_gpu_moe.py take the GEMM bound at C_ACC = 2 and reach 0.99.
 
 Set B200DDP_NUMERICS_LOG to a file path to append "<group> <largest error / bound>" for every check, which is how C_ACC
 is recalibrated after a kernel change.
@@ -601,3 +611,190 @@ def mse_reference(out, target, gscale, blocks, threads=256):
     depth = -(-n // stride) + 8 + 10 + -(-blocks // threads) + 10
     loss = (d * d).sum() / n
     return {"loss": (loss, (depth + 6) * U * loss + FLOOR), "dout": (dout, 6 * U * dout.abs())}
+
+
+# ---- cross-entropy: the fused LM head (kLmLse / kLmDlogits, lm_lse_combine, column_sum) and xent_fwd_bwd ------------------
+# (The bounds of this section are derived in the docstring of lm_loss_reference.)
+EXPF_ULPS = 2.0               # __expf(x): 2 + floor(EXPF_SLOPE |x|) ulp (CUDA C++ Programming Guide, intrinsic functions)
+EXPF_SLOPE = 1.173
+LOGF_ABS = 2.0 ** -21.41      # __logf(x): absolute error 2^-21.41 on [0.5, 2], otherwise 3 ulp
+LOGF_ULPS = 3.0
+FTZ = 2.0 ** -126             # the intrinsics flush subnormal results: an absolute error below the smallest normal
+LM_TILE, LM_CHUNK = 128, 32   # kLmLse: 128-column tiles, four 32-column chunks, one online (max, sum) rescale per chunk
+COMBINE_GROUPS = 8            # lm_lse_combine: thread y merges tiles y, y + 8, ..., then the 8 groups are merged
+XENT_THREADS = 256            # xent_fwd_bwd: one block of 256 per row (block_max / block_sum)
+FINISH_THREADS = 1024         # xent_finish_kernel / count_valid_kernel
+COLSUM_ROWS = 128             # column_sum: an fp32 chain of 128 rows per chunk, then one add per chunk
+XENT_BLOCK = 1 << 22          # fp64 elements of one row block of the cross-entropy references (32 MB)
+
+
+def lm_labelled(t, V, ignore_index=-100):
+    """bool [N]: the row carries a label (not ignore_index, 0 <= t < V), the kernels' rule."""
+    return (t != ignore_index) & (t >= 0) & (t < V)
+
+
+def xent_row_blocks(N, V):
+    rows = max(1, XENT_BLOCK // max(V, 1))
+    return [(r, min(r + rows, N)) for r in range(0, N, rows)]
+
+
+def lm_lse_depths(V):
+    """(__expf calls, other fp32 roundings) on one term's path through kLmLse and lm_lse_combine at vocabulary V."""
+    tiles = _ceil(V, LM_TILE)
+    merges = _ceil(tiles, COMBINE_GROUPS) - 1 + (COMBINE_GROUPS - 1)
+    return 1 + (LM_TILE // LM_CHUNK - 1) + merges, LM_CHUNK + 2 * (LM_TILE // LM_CHUNK) + 2 * merges
+
+
+def xent_depths(cols):
+    """(__expf calls, other fp32 roundings) of one term of xent_fwd_bwd's sum: a strided chain per thread, two warp trees."""
+    return 1, _ceil(cols, XENT_THREADS) + 10
+
+
+def _lse64(X, n_exp, n_ops):
+    """fp64 lse of the rows of X (float64 [r, V], -inf = no column) and its bound: (lse, bound, P = softmax, M = max)."""
+    M = X.amax(1, keepdim=True)
+    gap = (M - X).nan_to_num(posinf=0.0)                      # m - x_j: the arguments of a term's __expf calls add up to it
+    E = torch.exp(X - M)
+    S = E.sum(1, keepdim=True)
+    P = E / S
+    rho = 2 * U * (EXPF_ULPS * n_exp + EXPF_SLOPE * gap) + U * gap + U * n_ops
+    delta = (P * rho).sum(1) + (X.shape[1] + n_exp) * FTZ
+    logS = torch.log(S[:, 0])
+    lse = M[:, 0] + logS
+    bnd = delta / (1 - delta) + LOGF_ABS + 2 * U * LOGF_ULPS * logS.abs() + U * lse.abs() + FLOOR
+    return lse, bnd, P, M[:, 0]
+
+
+def lm_loss_reference(X, t, V, ignore_index=-100, finish=True):
+    """fp64 lse [N], row_loss [N] and loss of the fused forward from the kernel's own bf16 logits X [N, V] (gemm_nt of
+    the same hidden, weight and bias: the epilogue sees exactly the logits the unfused head GEMM stores), with their
+    element-wise bounds: {"lse": (ref, bnd), "row_loss": (ref, bnd), "loss": (ref, bnd)}.
+
+    Judging the softmax from X, not from the fp64 product, keeps the bounds at fp32 level: a dropped or shifted column
+    moves lse by p_j, far more than the bound.  With u = 2⁻²⁴, one fp32 ulp is at most 2u of the value, and m the row max:
+      one term   exp(x_j - m) carries a relative error ρ_j = 2u (2 n_exp + 1.173 (m - x_j)) + u (m - x_j) + u n_ops: each
+                 of its n_exp __expf calls costs 2 + ⌊1.173 |arg|⌋ ulp, and along its path (its chunk, the chunk rescales
+                 s · exp(m - m'), the combine merges a.y · exp(a.x - m)) the arguments add up to m - x_j, which also bounds
+                 their fp32 rounding; n_ops counts the other roundings (the 32-term chunk chain, the rescale products and
+                 adds, two per merge).  lm_lse_depths gives n_exp and n_ops.
+      lse        Σ_j p_j ρ_j (+ FTZ per term and merge for flushed results) through log(1 + δ) ≤ δ / (1 - δ), plus __logf
+                 (2⁻²¹·⁴¹ + 3 ulp) and the add m + log s
+      row_loss   lse - x_t rounded once: the kernel's row_loss equals float32(lse_kernel - X[i, t_i]) bitwise
+      loss       the xent_finish_kernel sum (a strided chain of ⌈N / 1024⌉ then two warp trees) and the division by the
+                 exact count"""
+    X = X.double()
+    N = X.shape[0]
+    n_exp, n_ops = lm_lse_depths(V)
+    lse = torch.zeros(N, dtype=torch.float64, device=X.device)
+    bnd = torch.zeros_like(lse)
+    for r0, r1 in xent_row_blocks(N, V):
+        lse[r0:r1], bnd[r0:r1] = _lse64(X[r0:r1], n_exp, n_ops)[:2]
+    return _row_loss_and_loss(X, lse, bnd, t, V, ignore_index, finish)
+
+
+def _row_loss_and_loss(X, lse, bnd, t, V, ignore_index, finish):
+    lab = lm_labelled(t, V, ignore_index)
+    xt = X.gather(1, torch.where(lab, t, 0)[:, None])[:, 0]
+    rl = torch.where(lab, lse - xt, 0.0)
+    rl_bnd = torch.where(lab, bnd + U * rl.abs(), 0.0) + FLOOR
+    out = {"lse": (lse, bnd), "row_loss": (rl, rl_bnd)}
+    if finish:
+        cnt = int(lab.sum())
+        N = X.shape[0]
+        depth = _ceil(N, FINISH_THREADS) + 10 + 1
+        c = max(cnt, 1)
+        loss = rl.sum() / c if cnt else rl.sum() * 0
+        out["loss"] = (loss, (rl_bnd.sum() + depth * U * rl.abs().sum()) / c + U * loss.abs() + FLOOR)
+    return out
+
+
+def lm_dlogits_reference(X, lse, t, V, coef, ignore_index=-100):
+    """fp64 D = (exp(X - lse) - [j = t]) · coef of the labelled rows (0 elsewhere) at the kernel's own fp32 lse [N], coef
+    = gscale / valid, and the bound of kLmDlogits' fp32 arithmetic before the bf16 rounding: (D, acc) [N, V].  The
+    argument x - lse is rounded once and __expf costs 2 + ⌊1.173 |x - lse|⌋ ulp; the target's - 1, coef = gscale / valid
+    and the product are one rounding each."""
+    X = X.double()
+    L = lse.double()[:, None]
+    lab = lm_labelled(t, V, ignore_index)[:, None]
+    gap = (X - L).abs()
+    P = torch.exp(X - L)
+    onehot = torch.zeros_like(X, dtype=torch.bool)
+    onehot.scatter_(1, torch.where(lab[:, 0], t, 0)[:, None], lab)
+    D = torch.where(lab, (P - onehot.double()) * coef, 0.0)
+    acc = torch.where(lab, abs(coef) * (P * (2 * U * (EXPF_ULPS + EXPF_SLOPE * gap) + U * gap) + FTZ) + 3 * U * D.abs(), 0.0)
+    return D, acc
+
+
+def lm_grad_reference(X, lse, t, h, w, V, coef, slice_width, ignore_index=-100, bound_k=None, c_acc=None):
+    """fp64 dh [N, H], dw [V, H] and dbias [V] of the fused backward at the kernel's own lse, and their bounds before the
+    bf16 rounding: {"dh": (ref, acc), "dw": ..., "dbias": ...}.  With D, δD from lm_dlogits_reference (δD including the
+    bf16 rounding of the stored dlogits):
+      dh     Σ_j δD_ij |W_j| + (C_ACC (vs + 1) + slices) u |D| |W|: per slice of vs columns a tensor-core sum, accumulated
+             in fp32 (one add per slice) into the fp32 buffer that is cast to bf16 once
+      dw     Σ_i δD_ij |h_i| + C_ACC (K + 1) u |D|ᵀ |h|, K = N (or, row-bounded, the count rounded up to 64)
+      dbias  Σ_i δD_ij + (128 + chunks) u Σ_i |D_ij|: column_sum's chain per 128-row chunk, one add per chunk"""
+    c_acc = C_ACC if c_acc is None else c_acc
+    N, H = h.shape
+    vs = min(slice_width, V)
+    slices = _ceil(V, vs)
+    K = N if bound_k is None else bound_k
+    W, Hm = w.double(), h.double()
+    Wa, Ha = W.abs(), Hm.abs()
+    dh = torch.zeros(N, H, dtype=torch.float64, device=h.device)
+    dh_acc = torch.zeros_like(dh)
+    dw, dw_mag, dw_err = (torch.zeros(V, H, dtype=torch.float64, device=h.device) for _ in range(3))
+    db, db_mag, db_err = (torch.zeros(V, dtype=torch.float64, device=h.device) for _ in range(3))
+    for r0, r1 in xent_row_blocks(N, V):
+        D, acc = lm_dlogits_reference(X[r0:r1], lse[r0:r1], t[r0:r1], V, coef, ignore_index)
+        dD = acc + BF16_U * (D.abs() + acc)                      # and the bf16 rounding of the stored dlogits
+        Da = D.abs()
+        dh[r0:r1] = D @ W
+        dh_acc[r0:r1] = dD @ Wa + (c_acc * (vs + 1) + slices) * U * (Da @ Wa)
+        dw += D.t() @ Hm[r0:r1]
+        dw_mag += Da.t() @ Ha[r0:r1]
+        dw_err += dD.t() @ Ha[r0:r1]
+        db += D.sum(0)
+        db_mag += Da.sum(0)
+        db_err += dD.sum(0)
+    chunks = _ceil(max(K, 1), COLSUM_ROWS)
+    return {"dh": (dh, dh_acc), "dw": (dw, dw_err + c_acc * (K + 1) * U * dw_mag),
+            "dbias": (db, db_err + (COLSUM_ROWS + chunks) * U * db_mag)}
+
+
+def xent_reference(x, t, ignore_index=-100, gscale=1.0, g=None):
+    """fp64 references of xent_fwd_bwd (either kernel) on logits x [N, C] (bf16 or fp32, exact in fp64): {"row_loss",
+    "loss": (ref, bnd), "dlogits": (ref, acc) [N, C] before the output rounding}.  Softmax statistics from block_max (exact)
+    and block_sum (xent_depths), dlogits = (exp(x - m) coef - g [j = t]) with coef = (gscale / valid) / s or, in the
+    streaming kernel, (exp(x - m) / s - [j = t]) g: at most four roundings after the exponential.  g (autograd's upstream
+    gradient): the backward multiplies the stored dlogits by g cast to the logits' dtype and rounds again, so acc then
+    holds the first rounding, the rounding of g and the error above times |g|."""
+    X = x.double()
+    N, C = X.shape
+    lab = lm_labelled(t, C, ignore_index)
+    cnt = int(lab.sum())
+    coef = gscale / cnt if cnt else 0.0
+    n_exp, n_ops = xent_depths(C)
+    lse = torch.zeros(N, dtype=torch.float64, device=x.device)
+    bnd = torch.zeros_like(lse)
+    D = torch.zeros_like(X)
+    acc = torch.zeros_like(X)
+    for r0, r1 in xent_row_blocks(N, C):
+        Xb = X[r0:r1]
+        lse[r0:r1], bnd[r0:r1], P, M = _lse64(Xb, n_exp, n_ops)
+        gap = (M[:, None] - Xb)
+        delta = bnd[r0:r1, None]                                 # the sum's relative error is within the lse bound
+        lb = lab[r0:r1, None]
+        onehot = torch.zeros_like(Xb, dtype=torch.bool)
+        onehot.scatter_(1, torch.where(lb[:, 0], t[r0:r1], 0)[:, None], lb)
+        d = torch.where(lb, (P - onehot.double()) * coef, 0.0)
+        e = P * (2 * U * (EXPF_ULPS + EXPF_SLOPE * gap) + U * gap + 2 * delta) + FTZ
+        D[r0:r1] = d
+        acc[r0:r1] = torch.where(lb, abs(coef) * e + 4 * U * (d.abs() + abs(coef) * P), 0.0)
+    out = _row_loss_and_loss(X, lse, bnd + U * lse.abs(), t, C, ignore_index, True)
+    if g is not None:
+        r = rounding(x.dtype)
+        gq = float(torch.tensor(g, dtype=x.dtype))               # g as the backward casts it
+        acc = abs(gq) * (acc + r * (D.abs() + acc)) + abs(gq - g) * D.abs()
+        D = D * g
+    out["dlogits"] = (D, acc)
+    return out

@@ -4,6 +4,7 @@ with new routing, a tiny Granite-shaped model against its CPU body, and an AdamW
 import pytest
 import torch
 
+import numerics as nm
 from b200ddp.ops import functional as Fn
 
 pytestmark = pytest.mark.gpu
@@ -38,19 +39,44 @@ def _skewed_ids(counts, k=1):
     return ids[torch.randperm(len(ids), generator=torch.Generator().manual_seed(0))].view(-1, k).to(DEV)
 
 
-@pytest.mark.parametrize("counts", [[0, 1, 127, 128, 129, 200, 5, 10], [0, 0, 600, 0, 0, 0, 0, 0]])
-@pytest.mark.parametrize("N,K", [(256, 128), (192, 64)])
+EVERY_GROUPED = {"kGrpRows, B K-major", "kGrpRows, B MN-major", "kGrpWgrad"}
+GROUPED_CALLS = [("moe_gemm", False), ("moe_gemm", True), ("moe_gemm_wgrad", None)]   # what every grouped case runs
+
+
+def grouped_kernel(op, dgrad):
+    """Mirror of launch_gemm_grouped (B MN-major exactly for the data gradient) and launch_gemm_grouped_wgrad."""
+    if op == "moe_gemm_wgrad":
+        return "kGrpWgrad"
+    return "kGrpRows, B MN-major" if dgrad else "kGrpRows, B K-major"
+# routing: the skewed counts of the older cases, Granite's (32 experts, top-8 of random router logits), and segments that
+# end exactly on 128-row boundaries
+ROUTINGS = [[0, 1, 127, 128, 129, 200, 5, 10], [0, 0, 600, 0, 0, 0, 0, 0], "granite", [256, 128, 0, 384]]
+
+
+def test_grouped_cases_reach_every_grouped_gemm():
+    assert {grouped_kernel(op, d) for op, d in GROUPED_CALLS} == EVERY_GROUPED
+
+
+@pytest.mark.parametrize("counts", ROUTINGS)
+@pytest.mark.parametrize("N,K", [(256, 128), (192, 64), (64, 64)])
 def test_grouped_gemms_against_per_expert_fp32(counts, N, K):
+    """Each expert segment of the forward, data-gradient and weight-gradient outputs against fp64, element by element:
+    forward and dgrad take the GEMM bound with K from the weight, wgrad with K = the segment's rows."""
     C = _C()
+    if counts == "granite":
+        logits = torch.randn(512, 32, generator=torch.Generator().manual_seed(2))
+        ids = logits.topk(8, -1).indices.to(torch.int32).to(DEV)
+        counts = torch.bincount(ids.reshape(-1).cpu().long(), minlength=32).tolist()
+    else:
+        ids = _skewed_ids(counts)
     E = len(counts)
-    ids = _skewed_ids(counts)
     T = ids.shape[0]
     cnt, offsets, fwd, inv, tiles = C.moe_permute(ids, E)
     assert cnt.tolist() == counts
     g = torch.Generator(device=DEV).manual_seed(1)
     x = torch.randn(T, K, device=DEV, generator=g).to(torch.bfloat16)
     w = (torch.randn(E, N, K, device=DEV, generator=g) * 0.1).to(torch.bfloat16)
-    xp = C.moe_gather(x, fwd, 1)
+    xp = C.moe_gather(x, fwd, ids.shape[1])
     pad = fwd < 0
     assert (xp[pad] == 0).all()
     cap = xp.shape[0]
@@ -84,9 +110,10 @@ def test_grouped_gemms_against_per_expert_fp32(counts, N, K):
         if off[e + 1] == off[e]:
             assert (dw[e] == 0).all()
             continue
-        assert _rel(y[seg], xp[seg].float() @ w[e].float().t()) < 1e-2
-        assert _rel(dx[seg], dy[seg].float() @ w[e].float()) < 1e-2
-        assert _rel(dw[e], dy[seg].float().t() @ xp[seg].float()) < 1e-2
+        where = f"expert {e} rows {off[e]}:{off[e + 1]}"
+        nm.check_gemm(f"{where}: forward [row, n]", y[seg], xp[seg], w[e], group="moe grouped")
+        nm.check_gemm(f"{where}: dgrad [row, k]", dx[seg], dy[seg], w[e].t(), group="moe grouped")
+        nm.check_gemm(f"{where}: wgrad [n, k]", dw[e], dy[seg].t(), xp[seg].t(), group="moe grouped")
         assert (y[seg][pad[seg]] == 0).all() and (dx[seg][pad[seg]] == 0).all()
 
 
