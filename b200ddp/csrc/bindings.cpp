@@ -170,13 +170,14 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin and _C.mamba namespaces of static entry points
+// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin, _C.mamba and _C.mamba2 namespaces of static entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
 struct T5Namespace {};
 struct ConvNextNamespace {};
 struct SwinNamespace {};
 struct MambaNamespace {};
+struct Mamba2Namespace {};
 
 // An NHWC activation of the depthwise convolution: bf16 [B, H, W, C] contiguous and 16-byte aligned, B, H, W >= 1,
 // 8 <= C <= 1024 with C % 8 == 0 (B is the grid's z extent).  Returns (B, H, W, C).
@@ -228,6 +229,40 @@ int64_t mamba_scan_args(Args& args, int64_t T, int64_t E, const at::Tensor& u, c
   if (xbc.size(1) < 32) args.fail("xbc", "bf16 [T, R + 32] with R >= 0 (dt | B | C)", describe(xbc));
   args("A_log", A_log, {kF32}, {E, 16})("D", D, {kF32}, {E})("dt_bias", dt_bias, {kF32}, {E});
   return xbc.size(1) - 32;
+}
+
+// A bf16 row view [rows, cols] read in place through its row pitch (Mamba-2's column windows of in_proj's output): unit
+// column stride, a row stride >= cols that is a multiple of 8 elements, 16-byte aligned.  Returns the pitch.
+int64_t row_view(Args& args, const char* name, const at::Tensor& t, int64_t rows, int64_t cols) {
+  args(name, t, {kBF16}, {rows, cols}, kStrided, 16);
+  if (t.stride(1) != 1 || t.stride(0) < cols || t.stride(0) % 8 || t.size(0) * t.stride(0) >= (1ll << 31))
+    args.fail(name, "a bf16 [" + std::to_string(rows) + ", " + std::to_string(cols) +
+                        "] row view with unit column stride and a row pitch >= the columns, a multiple of 8, under 2^31 elements in all",
+              describe(t) + " with strides (" + std::to_string(t.stride(0)) + ", " + std::to_string(t.stride(1)) + ")");
+  return t.stride(0);
+}
+
+// Mamba-2's bounds int32 [B, S, 2] contiguous and 8-byte aligned with 1 <= B <= 65535, S >= 1.  Returns (B, S).
+std::array<int64_t, 2> mamba2_bounds(Args& args, const at::Tensor& bounds) {
+  args("bounds", bounds, {kI32}, {kAny, kAny, 2}, kContiguous, 8);
+  const int64_t B = bounds.size(0), S = bounds.size(1);
+  if (B < 1 || B > 65535 || S < 1) args.fail("bounds", "int32 [B, S, 2] with 1 <= B <= 65535 and S >= 1", describe(bounds));
+  return {B, S};
+}
+
+// the SSD's inputs: xbc bf16 [B S, 64 H + 256] contiguous, dt a bf16 [B S, H] row view, H a positive multiple of 8 (so E and
+// the dt columns stay 16-byte aligned), A_log / D / dt_bias fp32 [H].  Returns (B, S, H, dt pitch).
+std::array<int64_t, 4> ssd_args(Args& args, const at::Tensor& xbc, const at::Tensor& dt, const at::Tensor& A_log, const at::Tensor& D,
+                                const at::Tensor& dt_bias, const at::Tensor& bounds) {
+  const auto [B, S] = mamba2_bounds(args, bounds);
+  args("xbc", xbc, {kBF16}, {B * S, kAny}, kContiguous, 16);
+  const int64_t H = (xbc.size(1) - 256) / 64;
+  if (xbc.size(1) < 256 + 64 * 8 || (xbc.size(1) - 256) % 512 || B * S * xbc.size(1) >= (1ll << 31))
+    args.fail("xbc", "bf16 [B S, 64 H + 256] (x | B | C, head dim 64, state 128) with H a positive multiple of 8 and fewer than 2^31 elements",
+              describe(xbc));
+  const int64_t dtp = row_view(args, "dt", dt, B * S, H);
+  args("A_log", A_log, {kF32}, {H})("D", D, {kF32}, {H})("dt_bias", dt_bias, {kF32}, {H});
+  return {B, S, H, dtp};
 }
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
@@ -1944,4 +1979,116 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     return std::make_tuple(du, ddraw, dxbc, dxz, dA_log, dD, dbias);
   }, py::arg("dy"), py::arg("u"), py::arg("draw"), py::arg("xbc"), py::arg("xz"), py::arg("A_log"), py::arg("D"), py::arg("dt_bias"),
      py::arg("bounds"), py::arg("hstart"), py::arg("sumd"));
+
+  // ---- Mamba-2's conv, SSD and gated RMSNorm (mamba.cu, mamba2.cu, layernorm.cu), bf16 token rows ----------------------------
+  // _C.mamba2 is a namespace of static entry points like _C.mamba; its contract rows are in tests/test_mamba2_bindings_cpu.py.
+  // Row views (x, dx_out, dt, ddt_out, z, dz_out) are read and written in place through their row pitch (row_view).
+  py::class_<Mamba2Namespace> mamba2(m, "mamba2", "Mamba-2's causal conv1d, chunked SSD scan and gated RMSNorm on token rows");
+  // u bf16 [B S, C] = silu(conv(x) + bias) of the row view x [B S, C], C % 8 == 0; weight fp32 [C, 4], bias fp32 [C]
+  mamba2.def_static("conv_fwd", [](at::Tensor x, at::Tensor weight, at::Tensor bias, at::Tensor bounds) {
+    Args args("conv_fwd");
+    const auto [B, S] = mamba2_bounds(args, bounds);
+    args("x", x, {kBF16}, {B * S, kAny}, kStrided);
+    const int64_t C = x.size(1);
+    if (C < 8 || C % 8) args.fail("x", "a bf16 [B S, C] row view with C a positive multiple of 8", describe(x));
+    const int64_t xp = row_view(args, "x", x, B * S, C);
+    args("weight", weight, {kF32}, {C, 4}, kContiguous, 16)("bias", bias, {kF32}, {C});
+    args.device();
+    at::Tensor u = at::empty({B * S, C}, x.options().memory_format(at::MemoryFormat::Contiguous));
+    launch_mamba2_conv_fwd(x.data_ptr(), xp, weight.data_ptr<float>(), bias.data_ptr<float>(), bounds.data_ptr<int>(), (int)B, (int)S, (int)C,
+                           u.data_ptr(), cur_stream());
+    return u;
+  }, py::arg("x"), py::arg("weight"), py::arg("bias"), py::arg("bounds"));
+  // (dx bf16 [B S, C]: dx_out when given (a row view, written in place and returned), else a new contiguous tensor;
+  // dweight fp32 [C, 4]; dbias fp32 [C])
+  mamba2.def_static("conv_bwd", [](at::Tensor du, at::Tensor x, at::Tensor weight, at::Tensor bias, at::Tensor bounds,
+                                   c10::optional<at::Tensor> dx_out) {
+    Args args("conv_bwd");
+    const auto [B, S] = mamba2_bounds(args, bounds);
+    args("x", x, {kBF16}, {B * S, kAny}, kStrided);
+    const int64_t C = x.size(1);
+    if (C < 8 || C % 8) args.fail("x", "a bf16 [B S, C] row view with C a positive multiple of 8", describe(x));
+    const int64_t xp = row_view(args, "x", x, B * S, C);
+    args("du", du, {kBF16}, {B * S, C}, kContiguous, 16)("weight", weight, {kF32}, {C, 4}, kContiguous, 16)("bias", bias, {kF32}, {C});
+    const int64_t dxp = dx_out.has_value() ? row_view(args, "dx_out", *dx_out, B * S, C) : C;
+    args.device();
+    at::Tensor dx = dx_out.has_value() ? *dx_out : at::empty({B * S, C}, du.options());
+    const auto f32 = du.options().dtype(kF32);
+    at::Tensor part = at::empty({(int64_t)mamba_conv_blocks((int)B, (int)S), 5, C}, f32);
+    at::Tensor dweight = at::empty({C, 4}, f32), dbias = at::empty({C}, f32);
+    launch_mamba2_conv_bwd(du.data_ptr(), x.data_ptr(), xp, weight.data_ptr<float>(), bias.data_ptr<float>(), bounds.data_ptr<int>(), (int)B,
+                           (int)S, (int)C, dx.data_ptr(), dxp, part.data_ptr<float>(), dweight.data_ptr<float>(), dbias.data_ptr<float>(),
+                           cur_stream());
+    return std::make_tuple(dx, dweight, dbias);
+  }, py::arg("du"), py::arg("x"), py::arg("weight"), py::arg("bias"), py::arg("bounds"), py::arg("dx_out") = py::none());
+  // y bf16 [B S, 64 H]; the chunk states are scratch of this call (the backward recomputes them)
+  mamba2.def_static("ssd_fwd", [](at::Tensor xbc, at::Tensor dt, at::Tensor A_log, at::Tensor D, at::Tensor dt_bias, at::Tensor bounds) {
+    Args args("ssd_fwd");
+    const auto [B, S, H, dtp] = ssd_args(args, xbc, dt, A_log, D, dt_bias, bounds);
+    args.device();
+    const int64_t nc = ssd_chunks((int)S);
+    const auto f32 = xbc.options().dtype(kF32);
+    at::Tensor states = at::empty({B, nc, H, 128, 64}, f32), dec = at::empty({B, nc, H}, f32);
+    at::Tensor y = at::empty({B * S, 64 * H}, xbc.options());
+    launch_ssd_fwd(xbc.data_ptr(), dt.data_ptr(), dtp, A_log.data_ptr<float>(), D.data_ptr<float>(), dt_bias.data_ptr<float>(),
+                   bounds.data_ptr<int>(), (int)B, (int)S, (int)H, states.data_ptr<float>(), dec.data_ptr<float>(), y.data_ptr(), cur_stream());
+    return y;
+  }, py::arg("xbc"), py::arg("dt"), py::arg("A_log"), py::arg("D"), py::arg("dt_bias"), py::arg("bounds"));
+  // (dxbc bf16 [B S, 64 H + 256], ddt bf16 [B S, H] (ddt_out when given: a row view, written in place and returned; the
+  // gradient of dt through the softplus), dA_log, dD, ddt_bias fp32 [H])
+  mamba2.def_static("ssd_bwd", [](at::Tensor dy, at::Tensor xbc, at::Tensor dt, at::Tensor A_log, at::Tensor D, at::Tensor dt_bias,
+                                  at::Tensor bounds, c10::optional<at::Tensor> ddt_out) {
+    Args args("ssd_bwd");
+    const auto [B, S, H, dtp] = ssd_args(args, xbc, dt, A_log, D, dt_bias, bounds);
+    args("dy", dy, {kBF16}, {B * S, 64 * H}, kContiguous, 16);
+    const int64_t ddtp = ddt_out.has_value() ? row_view(args, "ddt_out", *ddt_out, B * S, H) : H;
+    args.device();
+    const int64_t nc = ssd_chunks((int)S);
+    const auto f32 = xbc.options().dtype(kF32);
+    at::Tensor states = at::empty({B, nc, H, 128, 64}, f32), gstates = at::empty({B, nc, H, 128, 64}, f32), dec = at::empty({B, nc, H}, f32);
+    at::Tensor dA_part = at::empty({B * nc, H}, f32), dD_part = at::empty({B * nc, H}, f32), dbias_part = at::empty({B * nc, H}, f32);
+    at::Tensor dxbc = at::empty_like(xbc), ddt = ddt_out.has_value() ? *ddt_out : at::empty({B * S, H}, xbc.options());
+    at::Tensor dA_log = at::empty({H}, f32), dD = at::empty({H}, f32), dbias = at::empty({H}, f32);
+    launch_ssd_bwd(dy.data_ptr(), xbc.data_ptr(), dt.data_ptr(), dtp, A_log.data_ptr<float>(), D.data_ptr<float>(), dt_bias.data_ptr<float>(),
+                   bounds.data_ptr<int>(), (int)B, (int)S, (int)H, states.data_ptr<float>(), gstates.data_ptr<float>(), dec.data_ptr<float>(),
+                   dA_part.data_ptr<float>(), dD_part.data_ptr<float>(), dbias_part.data_ptr<float>(), dxbc.data_ptr(), ddt.data_ptr(), ddtp,
+                   dA_log.data_ptr<float>(), dD.data_ptr<float>(), dbias.data_ptr<float>(), cur_stream());
+    return std::make_tuple(dxbc, ddt, dA_log, dD, dbias);
+  }, py::arg("dy"), py::arg("xbc"), py::arg("dt"), py::arg("A_log"), py::arg("D"), py::arg("dt_bias"), py::arg("bounds"),
+     py::arg("ddt_out") = py::none());
+  // (out bf16 [rows, E] = weight * rmsnorm(y * silu(z)), rstd fp32 [rows]); y bf16 [rows, E] contiguous, z a row view, weight
+  // bf16 [E], 1024 < E <= 4096, E % 8 == 0
+  mamba2.def_static("gated_norm_fwd", [](at::Tensor y, at::Tensor z, at::Tensor weight, double eps) {
+    Args args("gated_norm_fwd");
+    args("y", y, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t rows = y.size(0), E = y.size(1);
+    if (rows < 1 || !gated_rmsnorm_supported((int)E) || rows * E >= (1ll << 31))
+      args.fail("y", "bf16 [rows, E] with rows >= 1, E % 8 == 0, 1024 < E <= 4096 and fewer than 2^31 elements", describe(y));
+    const int64_t zp = row_view(args, "z", z, rows, E);
+    args("weight", weight, {kBF16}, {E}, kContiguous, 16);
+    args.device();
+    at::Tensor out = at::empty_like(y), rstd = at::empty({rows}, y.options().dtype(kF32));
+    launch_gated_rmsnorm_fwd(y.data_ptr(), z.data_ptr(), zp, weight.data_ptr(), (int)rows, (int)E, (float)eps, out.data_ptr(),
+                             rstd.data_ptr<float>(), cur_stream());
+    return std::make_tuple(out, rstd);
+  }, py::arg("y"), py::arg("z"), py::arg("weight"), py::arg("eps"));
+  // (dy bf16 [rows, E], dz bf16 [rows, E] (dz_out when given: a row view, written in place and returned), dweight bf16 [E])
+  mamba2.def_static("gated_norm_bwd", [](at::Tensor dout, at::Tensor y, at::Tensor z, at::Tensor weight, at::Tensor rstd,
+                                         c10::optional<at::Tensor> dz_out) {
+    Args args("gated_norm_bwd");
+    args("y", y, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t rows = y.size(0), E = y.size(1);
+    if (rows < 1 || !gated_rmsnorm_supported((int)E) || rows * E >= (1ll << 31))
+      args.fail("y", "bf16 [rows, E] with rows >= 1, E % 8 == 0, 1024 < E <= 4096 and fewer than 2^31 elements", describe(y));
+    args("dout", dout, {kBF16}, {rows, E}, kContiguous, 16);
+    const int64_t zp = row_view(args, "z", z, rows, E);
+    args("weight", weight, {kBF16}, {E}, kContiguous, 16)("rstd", rstd, {kF32}, {rows});
+    const int64_t dzp = dz_out.has_value() ? row_view(args, "dz_out", *dz_out, rows, E) : E;
+    args.device();
+    at::Tensor dy = at::empty_like(y), dz = dz_out.has_value() ? *dz_out : at::empty_like(y), dweight = at::empty_like(weight);
+    at::Tensor wpart = at::empty({(int64_t)gated_rmsnorm_parts((int)rows), E}, y.options().dtype(kF32));
+    launch_gated_rmsnorm_bwd(dout.data_ptr(), y.data_ptr(), z.data_ptr(), zp, weight.data_ptr(), rstd.data_ptr<float>(), (int)rows, (int)E,
+                             dy.data_ptr(), dz.data_ptr(), dzp, wpart.data_ptr<float>(), dweight.data_ptr(), cur_stream());
+    return std::make_tuple(dy, dz, dweight);
+  }, py::arg("dout"), py::arg("y"), py::arg("z"), py::arg("weight"), py::arg("rstd"), py::arg("dz_out") = py::none());
 }

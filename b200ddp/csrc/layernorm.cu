@@ -293,9 +293,13 @@ __device__ __forceinline__ float rms_wide_block_sum(float v, float* red) {
   return r;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const T* __restrict__ x, const T* __restrict__ gamma, int rows,
-                                                                          int cols, float eps, T* __restrict__ y, float* __restrict__ rstd) {
+// kGated (Mamba-2's gated norm, bf16 only): the row is g = x * silu(z), z read through its own row pitch, and the
+// backward also writes dz and per-CTA fp32 partials of dgamma (the CTA's rows, in grid-stride order)
+__device__ __forceinline__ float silu_(float z) { return z / (1.f + expf(-z)); }
+
+template <typename T, bool kGated>
+__device__ __forceinline__ void rmsnorm_wide_fwd_body(const T* __restrict__ x, const T* __restrict__ gamma, int rows, int cols, float eps,
+                                                      T* __restrict__ y, float* __restrict__ rstd, const T* __restrict__ z, size_t zp) {
   __shared__ float red[kRmsWideThreads / 32];
   const int nchunk = cols >> 3;
   float g[kRmsWideChunks][8];
@@ -314,6 +318,12 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const
       const int ch = threadIdx.x + kRmsWideThreads * c;
       if (ch < nchunk) {
         load8<T>(xr + 8 * ch, v[c]);
+        if constexpr (kGated) {
+          float zv[8];
+          load8<T>(z + (size_t)row * zp + 8 * ch, zv);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) v[c][j] *= silu_(zv[j]);
+        }
 #pragma unroll
         for (int j = 0; j < 8; ++j) q += v[c][j] * v[c][j];
       }
@@ -334,18 +344,40 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const
   }
 }
 
-// dx = rs * (dy*gamma - xn * mean(dy*gamma*xn)), xn = x * rs
 template <typename T>
-__global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(const T* __restrict__ dy, const T* __restrict__ x,
-                                                                             const T* __restrict__ gamma, const float* __restrict__ rstd,
-                                                                             int rows, int cols, T* __restrict__ dx) {
+__global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_fwd_kernel(const T* __restrict__ x, const T* __restrict__ gamma, int rows,
+                                                                          int cols, float eps, T* __restrict__ y, float* __restrict__ rstd) {
+  rmsnorm_wide_fwd_body<T, false>(x, gamma, rows, cols, eps, y, rstd, nullptr, 0);
+}
+
+__global__ void __launch_bounds__(kRmsWideThreads) gated_rmsnorm_wide_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ z,
+                                                                                size_t zp, const __nv_bfloat16* __restrict__ gamma, int rows,
+                                                                                int cols, float eps, __nv_bfloat16* __restrict__ y,
+                                                                                float* __restrict__ rstd) {
+  rmsnorm_wide_fwd_body<__nv_bfloat16, true>(x, gamma, rows, cols, eps, y, rstd, z, zp);
+}
+
+// dx = rs * (dy*gamma - xn * mean(dy*gamma*xn)), xn = x * rs
+// kGated: xn = g rs with g = x silu(z); dg as dx above, then dx = dg silu(z), dz = dg x silu'(z), and wpart[blockIdx.x] the
+// CTA's sum of dy * xn
+template <typename T, bool kGated>
+__device__ __forceinline__ void rmsnorm_wide_bwd_body(const T* __restrict__ dy, const T* __restrict__ x, const T* __restrict__ gamma,
+                                                      const float* __restrict__ rstd, int rows, int cols, T* __restrict__ dx,
+                                                      const T* __restrict__ z, size_t zp, T* __restrict__ dz, size_t dzp,
+                                                      float* __restrict__ wpart) {
   __shared__ float red[kRmsWideThreads / 32];
   const int nchunk = cols >> 3;
   float g[kRmsWideChunks][8];
+  float wacc[kGated ? kRmsWideChunks : 1][8];
 #pragma unroll
   for (int c = 0; c < kRmsWideChunks; ++c) {
     const int ch = threadIdx.x + kRmsWideThreads * c;
-    if (ch < nchunk) load8<T>(gamma + 8 * ch, g[c]);
+    if constexpr (kGated) {       // gamma is re-read per row: the gated rows keep dgamma's partials in registers instead
+#pragma unroll
+      for (int j = 0; j < 8; ++j) wacc[c][j] = 0.f;
+    } else if (ch < nchunk) {
+      load8<T>(gamma + 8 * ch, g[c]);
+    }
   }
   const float inv = 1.f / (float)cols;
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
@@ -360,6 +392,16 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(co
       if (ch < nchunk) {
         load8<T>(xr + 8 * ch, xn[c]);
         load8<T>(dyr + 8 * ch, d[c]);
+        if constexpr (kGated) {
+          float zv[8];
+          load8<T>(z + (size_t)row * zp + 8 * ch, zv);
+          load8<T>(gamma + 8 * ch, g[c]);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            xn[c][j] *= silu_(zv[j]);
+            wacc[c][j] = fmaf(d[c][j], xn[c][j] * rs, wacc[c][j]);
+          }
+        }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           xn[c][j] *= rs;
@@ -377,10 +419,54 @@ __global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(co
         float o[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) o[j] = rs * (d[c][j] - xn[c][j] * s2);
+        if constexpr (kGated) {
+          float zv[8], xv[8], oz[8];
+          load8<T>(z + (size_t)row * zp + 8 * ch, zv);
+          load8<T>(xr + 8 * ch, xv);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float sg = 1.f / (1.f + expf(-zv[j]));
+            oz[j] = o[j] * xv[j] * sg * (1.f + zv[j] * (1.f - sg));
+            o[j] *= zv[j] * sg;
+          }
+          store8<T>(dz + (size_t)row * dzp + 8 * ch, oz);
+        }
         store8<T>(dxr + 8 * ch, o);
       }
     }
   }
+  if constexpr (kGated) {
+#pragma unroll
+    for (int c = 0; c < kRmsWideChunks; ++c) {
+      const int ch = threadIdx.x + kRmsWideThreads * c;
+      if (ch < nchunk) store8<float>(wpart + (size_t)blockIdx.x * cols + 8 * ch, wacc[c]);
+    }
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRmsWideThreads) rmsnorm_wide_bwd_dx_kernel(const T* __restrict__ dy, const T* __restrict__ x,
+                                                                             const T* __restrict__ gamma, const float* __restrict__ rstd,
+                                                                             int rows, int cols, T* __restrict__ dx) {
+  rmsnorm_wide_bwd_body<T, false>(dy, x, gamma, rstd, rows, cols, dx, nullptr, 0, nullptr, 0, nullptr);
+}
+
+__global__ void __launch_bounds__(kRmsWideThreads) gated_rmsnorm_wide_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                                                                                const __nv_bfloat16* __restrict__ z, size_t zp,
+                                                                                const __nv_bfloat16* __restrict__ gamma,
+                                                                                const float* __restrict__ rstd, int rows, int cols,
+                                                                                __nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dz,
+                                                                                size_t dzp, float* __restrict__ wpart) {
+  rmsnorm_wide_bwd_body<__nv_bfloat16, true>(dy, x, gamma, rstd, rows, cols, dx, z, zp, dz, dzp, wpart);
+}
+
+// dgamma bf16 [cols] = the per-CTA partials added in CTA order
+__global__ void gated_rmsnorm_dgamma_kernel(const float* __restrict__ wpart, int parts, int cols, __nv_bfloat16* __restrict__ dgamma) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= cols) return;
+  float sum = 0.f;
+  for (int p = 0; p < parts; ++p) sum += wpart[(size_t)p * cols + c];
+  dgamma[c] = __float2bfloat16_rn(sum);
 }
 
 int rmsnorm_wide_blocks(int rows) { return rows < 16 * kNumSMs ? (rows < 1 ? 1 : rows) : 16 * kNumSMs; }
@@ -567,6 +653,33 @@ void launch_rmsnorm_bwd(const void* dy, const void* x, const void* gamma, const 
                                                                                    (float*)dgamma, nullptr);
   }
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+// Mamba-2's gated RMSNorm on the wide kernels: y = gamma * rmsnorm(x * silu(z)), bf16, 1024 < cols <= 4096, cols % 8 == 0;
+// z (and dz) rows at their own pitch (a multiple of 8 elements), all pointers 16-byte aligned
+bool gated_rmsnorm_supported(int cols) { return cols % 8 == 0 && rmsnorm_wide(cols) && cols <= 8 * kRmsWideThreads * kRmsWideChunks; }
+int gated_rmsnorm_parts(int rows) { return rmsnorm_wide_blocks(rows); }
+
+void launch_gated_rmsnorm_fwd(const void* x, const void* z, long long zp, const void* gamma, int rows, int cols, float eps, void* y,
+                              float* rstd, cudaStream_t s) {
+  if (!gated_rmsnorm_supported(cols) || rows < 1)
+    throw std::runtime_error("gated_rmsnorm_fwd: needs rows >= 1, cols % 8 == 0 and 1024 < cols <= 4096 (cols=" + std::to_string(cols) + ")");
+  gated_rmsnorm_wide_fwd_kernel<<<rmsnorm_wide_blocks(rows), kRmsWideThreads, 0, s>>>(
+      (const __nv_bfloat16*)x, (const __nv_bfloat16*)z, (size_t)zp, (const __nv_bfloat16*)gamma, rows, cols, eps, (__nv_bfloat16*)y, rstd);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void launch_gated_rmsnorm_bwd(const void* dy, const void* x, const void* z, long long zp, const void* gamma, const float* rstd, int rows,
+                              int cols, void* dx, void* dz, long long dzp, float* wpart, void* dgamma, cudaStream_t s) {
+  if (!gated_rmsnorm_supported(cols) || rows < 1)
+    throw std::runtime_error("gated_rmsnorm_bwd: needs rows >= 1, cols % 8 == 0 and 1024 < cols <= 4096 (cols=" + std::to_string(cols) + ")");
+  const int parts = gated_rmsnorm_parts(rows);
+  gated_rmsnorm_wide_bwd_kernel<<<parts, kRmsWideThreads, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, (const __nv_bfloat16*)z,
+                                                                 (size_t)zp, (const __nv_bfloat16*)gamma, rstd, rows, cols, (__nv_bfloat16*)dx,
+                                                                 (__nv_bfloat16*)dz, (size_t)dzp, wpart);
+  B200_CUDA_CHECK(cudaGetLastError());
+  gated_rmsnorm_dgamma_kernel<<<(cols + 255) / 256, 256, 0, s>>>(wpart, parts, cols, (__nv_bfloat16*)dgamma);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(2);
 }
 
 }  // namespace b200

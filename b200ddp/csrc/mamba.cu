@@ -43,9 +43,23 @@ __device__ __forceinline__ float sum16(float v) {
 }
 
 // ---------------- causal depthwise conv1d + SiLU ----------------------------------------------------------------------
-__global__ void __launch_bounds__(kConvThreads) mamba_conv_fwd_kernel(const __nv_bfloat16* __restrict__ xz, const float* __restrict__ w,
-                                                                      const float* __restrict__ bias, const int2* __restrict__ bounds,
-                                                                      int T, int S, int E, __nv_bfloat16* __restrict__ u) {
+// The bodies take the input rows through a pitch policy: Mamba-1 reads the x half of xz [T, 2E] (XzRows), Mamba-2 the xBC
+// column window of zxbcdt [T, W] (PitchRows, x already offset to the window).  E is the channel count; u and du are
+// [T, E] contiguous.
+struct XzRows {
+  int E;
+  __device__ __forceinline__ size_t in(size_t r) const { return r * 2 * E; }
+  __device__ __forceinline__ size_t out(size_t r) const { return r * 2 * E; }
+};
+struct PitchRows {
+  size_t in_pitch, out_pitch;
+  __device__ __forceinline__ size_t in(size_t r) const { return r * in_pitch; }
+  __device__ __forceinline__ size_t out(size_t r) const { return r * out_pitch; }
+};
+
+template <class Rows>
+__device__ __forceinline__ void conv_fwd_body(const __nv_bfloat16* __restrict__ xz, const float* __restrict__ w, const float* __restrict__ bias,
+                                              const int2* __restrict__ bounds, int T, int S, int E, Rows rows, __nv_bfloat16* __restrict__ u) {
   const int groups = E / 8;
   const long long idx = (long long)blockIdx.x * kConvThreads + threadIdx.x;
   if (idx >= (long long)T * groups) return;
@@ -70,7 +84,7 @@ __global__ void __launch_bounds__(kConvThreads) mamba_conv_fwd_kernel(const __nv
     const int p = s - (kK - 1) + j;
     if (p < max(bd.x, 0)) continue;
     float xv[8];
-    load8(xz + (size_t)(t - (kK - 1) + j) * 2 * E + e0, xv);
+    load8(xz + rows.in((size_t)(t - (kK - 1) + j)) + e0, xv);
 #pragma unroll
     for (int c = 0; c < 8; ++c) acc[c] = fmaf(wv[c][j], xv[c], acc[c]);
   }
@@ -79,11 +93,23 @@ __global__ void __launch_bounds__(kConvThreads) mamba_conv_fwd_kernel(const __nv
   store8(u + (size_t)t * E + e0, acc);
 }
 
+__global__ void __launch_bounds__(kConvThreads) mamba_conv_fwd_kernel(const __nv_bfloat16* __restrict__ xz, const float* __restrict__ w,
+                                                                      const float* __restrict__ bias, const int2* __restrict__ bounds,
+                                                                      int T, int S, int E, __nv_bfloat16* __restrict__ u) {
+  conv_fwd_body(xz, w, bias, bounds, T, S, E, XzRows{E}, u);
+}
+
+__global__ void __launch_bounds__(kConvThreads) mamba2_conv_fwd_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w,
+                                                                       const float* __restrict__ bias, const int2* __restrict__ bounds,
+                                                                       int T, int S, int E, PitchRows rows, __nv_bfloat16* __restrict__ u) {
+  conv_fwd_body(x, w, bias, bounds, T, S, E, rows, u);
+}
+
 // thread = (row b, block of kConvBlock positions, 8 channels); part fp32 [B * blocks, 5, E] (4 taps, bias)
-__global__ void __launch_bounds__(kConvThreads) mamba_conv_bwd_kernel(const __nv_bfloat16* __restrict__ du, const __nv_bfloat16* __restrict__ xz,
-                                                                      const float* __restrict__ w, const float* __restrict__ bias,
-                                                                      const int2* __restrict__ bounds, int B, int S, int E,
-                                                                      __nv_bfloat16* __restrict__ dxz, float* __restrict__ part) {
+template <class Rows>
+__device__ __forceinline__ void conv_bwd_body(const __nv_bfloat16* __restrict__ du, const __nv_bfloat16* __restrict__ xz,
+                                              const float* __restrict__ w, const float* __restrict__ bias, const int2* __restrict__ bounds,
+                                              int B, int S, int E, Rows rows, __nv_bfloat16* __restrict__ dxz, float* __restrict__ part) {
   const int groups = E / 8, blocks = (S + kConvBlock - 1) / kConvBlock;
   const long long idx = (long long)blockIdx.x * kConvThreads + threadIdx.x;
   if (idx >= (long long)B * blocks * groups) return;
@@ -118,7 +144,7 @@ __global__ void __launch_bounds__(kConvThreads) mamba_conv_bwd_kernel(const __nv
     st[kK - 1] = INT_MAX;
 #pragma unroll
     for (int c = 0; c < 8; ++c) { xr[kK - 1][c] = 0.f; dr[kK - 1][c] = 0.f; }
-    if (s >= 0 && s < S) load8(xz + (row0 + s) * 2 * E + e0, xr[kK - 1]);
+    if (s >= 0 && s < S) load8(xz + rows.in(row0 + s) + e0, xr[kK - 1]);
     if (s >= s0 && s < S) {
       const int2 bd = bounds[row0 + s];
       if (bd.x < bd.y) {
@@ -160,13 +186,27 @@ __global__ void __launch_bounds__(kConvThreads) mamba_conv_bwd_kernel(const __nv
           for (int c = 0; c < 8; ++c) dx[c] = fmaf(wv[c][j], dr[r][c], dx[c]);
         }
       }
-      store8(dxz + (row0 + t) * 2 * E + e0, dx);
+      store8(dxz + rows.out(row0 + t) + e0, dx);
     }
   }
   float* p = part + (size_t)blk * 5 * E + e0;
 #pragma unroll
   for (int j = 0; j < kK; ++j) store8(p + (size_t)j * E, dw[j]);
   store8(p + (size_t)kK * E, db);
+}
+
+__global__ void __launch_bounds__(kConvThreads) mamba_conv_bwd_kernel(const __nv_bfloat16* __restrict__ du, const __nv_bfloat16* __restrict__ xz,
+                                                                      const float* __restrict__ w, const float* __restrict__ bias,
+                                                                      const int2* __restrict__ bounds, int B, int S, int E,
+                                                                      __nv_bfloat16* __restrict__ dxz, float* __restrict__ part) {
+  conv_bwd_body(du, xz, w, bias, bounds, B, S, E, XzRows{E}, dxz, part);
+}
+
+__global__ void __launch_bounds__(kConvThreads) mamba2_conv_bwd_kernel(const __nv_bfloat16* __restrict__ du, const __nv_bfloat16* __restrict__ x,
+                                                                       const float* __restrict__ w, const float* __restrict__ bias,
+                                                                       const int2* __restrict__ bounds, int B, int S, int E, PitchRows rows,
+                                                                       __nv_bfloat16* __restrict__ dx, float* __restrict__ part) {
+  conv_bwd_body(du, x, w, bias, bounds, B, S, E, rows, dx, part);
 }
 
 // dw fp32 [E, 4], db fp32 [E]: the block partials added in block order
@@ -508,6 +548,27 @@ void launch_mamba_conv_bwd(const void* du, const void* xz, const float* w, const
   const int nblk = mamba_conv_blocks(B, S);
   mamba_conv_bwd_kernel<<<ceil_div((long long)nblk * (E / 8), kConvThreads), kConvThreads, 0, s>>>(
       (const __nv_bfloat16*)du, (const __nv_bfloat16*)xz, w, bias, (const int2*)bounds, B, S, E, (__nv_bfloat16*)dxz, part);
+  B200_CUDA_CHECK(cudaGetLastError());
+  mamba_conv_finish_kernel<<<ceil_div(5 * E, kConvThreads), kConvThreads, 0, s>>>(part, nblk, E, dw, db);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(2);
+}
+
+void launch_mamba2_conv_fwd(const void* x, long long x_pitch, const float* w, const float* bias, const int* bounds, int B, int S, int E,
+                            void* u, cudaStream_t s) {
+  check_mamba_shape("mamba2_conv_fwd", B, S, E);
+  const long long n = (long long)B * S * (E / 8);
+  mamba2_conv_fwd_kernel<<<ceil_div(n, kConvThreads), kConvThreads, 0, s>>>((const __nv_bfloat16*)x, w, bias, (const int2*)bounds, B * S, S, E,
+                                                                           PitchRows{(size_t)x_pitch, (size_t)x_pitch}, (__nv_bfloat16*)u);
+  B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(1);
+}
+
+void launch_mamba2_conv_bwd(const void* du, const void* x, long long x_pitch, const float* w, const float* bias, const int* bounds, int B, int S,
+                            int E, void* dx, long long dx_pitch, float* part, float* dw, float* db, cudaStream_t s) {
+  check_mamba_shape("mamba2_conv_bwd", B, S, E);
+  const int nblk = mamba_conv_blocks(B, S);
+  mamba2_conv_bwd_kernel<<<ceil_div((long long)nblk * (E / 8), kConvThreads), kConvThreads, 0, s>>>(
+      (const __nv_bfloat16*)du, (const __nv_bfloat16*)x, w, bias, (const int2*)bounds, B, S, E, PitchRows{(size_t)x_pitch, (size_t)dx_pitch},
+      (__nv_bfloat16*)dx, part);
   B200_CUDA_CHECK(cudaGetLastError());
   mamba_conv_finish_kernel<<<ceil_div(5 * E, kConvThreads), kConvThreads, 0, s>>>(part, nblk, E, dw, db);
   B200_CUDA_CHECK(cudaGetLastError()); B200_COUNT_LAUNCH(2);

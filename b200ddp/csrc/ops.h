@@ -305,6 +305,35 @@ void launch_mamba_scan_bwd(const void* dy, const void* u, const void* draw, cons
                            float* dq, float* dbc_part, float* dA_part, float* dD_part, float* dbias_part, void* du, void* ddraw, void* dxbc,
                            void* dxz, float* dA_log, float* dD, float* dbias, cudaStream_t s);
 
+// ---------------- Mamba-2 (mamba2.cu, mamba.cu, layernorm.cu), bf16 token rows --------------------------------------------
+// T = B S rows, bounds int32 [B, S, 2] as for Mamba-1.  Row views (x, dx, dt, ddt, z, dz) are read and written through their
+// row pitch in elements (a multiple of 8), 16-byte aligned.  No atomics, no host synchronisation.
+// Conv (width 4) + SiLU over E channels of x [T, *] (pitch x_pitch) -> u bf16 [T, E]; the backward writes dx (pitch
+// dx_pitch), dw fp32 [E, 4], db fp32 [E] through part fp32 [mamba_conv_blocks(B, S), 5, E].
+void launch_mamba2_conv_fwd(const void* x, long long x_pitch, const float* w, const float* bias, const int* bounds, int B, int S, int E,
+                            void* u, cudaStream_t s);
+void launch_mamba2_conv_bwd(const void* du, const void* x, long long x_pitch, const float* w, const float* bias, const int* bounds, int B, int S,
+                            int E, void* dx, long long dx_pitch, float* part, float* dw, float* db, cudaStream_t s);
+// SSD, head dim 64, state 128, one group: xbc bf16 [T, 64 H + 256] = x | B | C, dt bf16 [T, *] (pitch dt_pitch, H columns),
+// A_log / D / dt_bias fp32 [H], H % 8 == 0; y bf16 [T, 64 H].  Scratch: states (and gstates) fp32 [B, ssd_chunks(S), H, 128, 64],
+// dec fp32 [B, chunks, H], dA_part / dD_part / dbias_part fp32 [B chunks, H].  The backward writes dxbc bf16 [T, 64 H + 256]
+// and ddt (pitch ddt_pitch, H columns: the gradient of the dt input), dA_log, dD, dbias fp32 [H].
+int ssd_chunks(int S);
+void launch_ssd_fwd(const void* xbc, const void* dt, long long dt_pitch, const float* A_log, const float* D, const float* dt_bias,
+                    const int* bounds, int B, int S, int H, float* states, float* dec, void* y, cudaStream_t s);
+void launch_ssd_bwd(const void* dy, const void* xbc, const void* dt, long long dt_pitch, const float* A_log, const float* D,
+                    const float* dt_bias, const int* bounds, int B, int S, int H, float* states, float* gstates, float* dec,
+                    float* dA_part, float* dD_part, float* dbias_part, void* dxbc, void* ddt, long long ddt_pitch, float* dA_log,
+                    float* dD, float* dbias, cudaStream_t s);
+// Gated RMSNorm y = gamma * rmsnorm(x * silu(z)), bf16 x / y [rows, cols], gamma bf16 [cols], rstd fp32 [rows]; the backward
+// writes dx [rows, cols], dz (pitch dzp) and dgamma through wpart fp32 [gated_rmsnorm_parts(rows), cols]
+bool gated_rmsnorm_supported(int cols);
+int gated_rmsnorm_parts(int rows);
+void launch_gated_rmsnorm_fwd(const void* x, const void* z, long long zp, const void* gamma, int rows, int cols, float eps, void* y,
+                              float* rstd, cudaStream_t s);
+void launch_gated_rmsnorm_bwd(const void* dy, const void* x, const void* z, long long zp, const void* gamma, const float* rstd, int rows,
+                              int cols, void* dx, void* dz, long long dzp, float* wpart, void* dgamma, cudaStream_t s);
+
 // ---------------- CLIP contrastive loss (clip.cu) ---------------------------------------------------
 // u bf16 [B, D] = x / ||x|| per row (fp32, one rounding), rnorm fp32 [B] = 1 / ||x||; D % 8 == 0, 16-byte aligned rows
 void launch_l2norm_fwd(const void* x, int B, int D, void* u, float* rnorm, cudaStream_t s);

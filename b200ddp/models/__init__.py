@@ -19,6 +19,7 @@ from .clip import CLIP_VIT_B_16, CLIP_VIT_B_32, CLIPConfig, CLIPModel, clip_vit_
 from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneration, bart_base, bart_large
 from .t5 import T5_BASE, T5_SMALL, T5Config, T5ForConditionalGeneration, t5_base, t5_small
 from .mamba import MAMBA_130M, MAMBA_370M, MambaConfig, MambaForCausalLM, mamba_130m, mamba_370m
+from .mamba2 import MAMBA2_130M, MAMBA2_370M, Mamba2Config, Mamba2ForCausalLM, mamba2_130m, mamba2_370m
 
 
 @dataclass(frozen=True)
@@ -77,6 +78,8 @@ MODEL_REGISTRY = {
     # Mamba's own start id, <|endoftext|> = 0, is the padding id here, so packed documents start with id 1 instead
     "mamba-130m": ModelEntry(mamba_130m, "causal", MAMBA_130M, start_id=1),
     "mamba-370m": ModelEntry(mamba_370m, "causal", MAMBA_370M, start_id=1),
+    "mamba2-130m": ModelEntry(mamba2_130m, "causal", MAMBA2_130M, start_id=1),
+    "mamba2-370m": ModelEntry(mamba2_370m, "causal", MAMBA2_370M, start_id=1),
 }
 
 
@@ -92,4 +95,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "Mamba2Config", "Mamba2ForCausalLM", "mamba2_130m", "mamba2_370m", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

@@ -2170,6 +2170,291 @@ def selective_scan(u: torch.Tensor, delta_raw: torch.Tensor, xbc: torch.Tensor, 
 
 
 # ------------------------------------------------------------------------------------------------
+# Mamba-2 (csrc/mamba2.cu, the conv in csrc/mamba.cu, the gated norm in csrc/layernorm.cu): the causal conv over the xBC
+# column window of in_proj's output, the chunked SSD scan and the gated RMSNorm on token rows, reset at document starts
+# ------------------------------------------------------------------------------------------------
+MAMBA2_HEAD_DIM = 64
+MAMBA2_STATE = 128
+MAMBA2_CHUNK = 64        # rows per chunk of the SSD (the result does not depend on it in exact arithmetic)
+
+
+class Mamba2GradLink:
+    """Hands one [B, S, W] gradient buffer of in_proj's output zxbcdt between the backwards of a Mamba-2 mixer: the gated
+    norm writes its z columns, ``ssd_scan`` its dt columns, and ``causal_conv1d_window`` its xBC columns and returns it
+    whole: no zero fill, no add, no concatenation.  Build one per mixer call from zxbcdt and pass it to all three ops; the
+    conv's backward runs last (its output feeds the scan, whose output feeds the norm)."""
+
+    def __init__(self, zxbcdt: torch.Tensor):
+        self.shape, self.like = tuple(zxbcdt.shape), zxbcdt
+        self.base = zxbcdt.data_ptr()
+        self.buffer = None
+
+    def window(self, view: torch.Tensor) -> torch.Tensor:
+        """The columns of the gradient buffer under ``view`` (a column window of zxbcdt), allocating the buffer first."""
+        col = (view.data_ptr() - self.base) // view.element_size()
+        if self.buffer is None:
+            self.buffer = torch.empty(self.shape, dtype=self.like.dtype, device=self.like.device)
+            self.like = None
+        return self.buffer[..., col:col + view.shape[-1]]
+
+
+def _row_view(t: torch.Tensor) -> torch.Tensor:
+    """[..., C] -> [T, C] read in place when its rows have unit column stride, a pitch that is a multiple of 8 and a 16-byte
+    aligned start (a column window of a contiguous tensor), else a contiguous copy."""
+    r = t.reshape(-1, t.shape[-1])
+    if r.stride(-1) != 1 or r.stride(0) % 8 or r.stride(0) < r.shape[1] or r.data_ptr() % 16:
+        r = r.contiguous()
+        if r.data_ptr() % 16:
+            r = r.clone()
+    return r
+
+
+def _mamba2_check_rows(who: str, x: torch.Tensor, bounds: torch.Tensor) -> None:
+    if x.dim() != 3 or tuple(bounds.shape) != (x.shape[0], x.shape[1], 2) or bounds.is_floating_point() or bounds.is_complex():
+        raise ValueError(f"{who} needs activations [B, S, *] and integer bounds [B, S, 2], got {tuple(x.shape)} and {bounds.dtype} "
+                         f"{tuple(bounds.shape)}")
+
+
+def causal_conv1d_window_reference(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, bounds: torch.Tensor,
+                                   col: int = 0) -> torch.Tensor:
+    """``causal_conv1d_window`` in torch, fp32 (fp64 for fp64 input): u[t] = silu(bias + sum_j w[:, j] x[t - 3 + j]) over the
+    columns [col, col + C) of x [B, S, W], taps before the document start reading zero and padding positions giving zero.
+    Differentiable."""
+    dtype = _ref_dtype(x)
+    B, S, _ = x.shape
+    C = weight.shape[0]
+    xs0 = x[..., col:col + C].to(dtype)
+    w = weight.reshape(C, MAMBA_CONV_WIDTH).to(dtype)
+    real, start, _ = _mamba_positions(bounds, x.device)
+    pos = torch.arange(S, device=x.device)
+    pre = bias.to(dtype).expand(B, S, C)
+    for j in range(MAMBA_CONV_WIDTH):
+        shift = MAMBA_CONV_WIDTH - 1 - j
+        xs = F.pad(xs0, (0, 0, shift, 0))[:, :S]
+        keep = (pos - shift >= start) & real
+        pre = pre + w[:, j] * torch.where(keep[..., None], xs, torch.zeros_like(xs))
+    return torch.where(real[..., None], F.silu(pre), torch.zeros_like(pre)).to(x.dtype)
+
+
+class _CausalConv1dWindow(torch.autograd.Function):
+    """zxbcdt [B, S, W] bf16 -> u [B, S, C] from the columns [col, col + C) (csrc/mamba.cu).  Backward: dx into those
+    columns of the link's buffer, which it returns whole (or of a new buffer with zeros elsewhere); fp32 weight and bias
+    gradients summed in a fixed order."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, bounds, col, link):
+        B, S, W = x.shape
+        C = weight.shape[0]
+        xw = _row_view(x[..., col:col + C])
+        w, b = weight.reshape(C, MAMBA_CONV_WIDTH).float().contiguous(), bias.float().contiguous()
+        bd = _aligned16(bounds.to(torch.int32))                      # the kernels read (start, end) as int2
+        ctx.save_for_backward(x, xw, w, b, bd)
+        ctx.link, ctx.col, ctx.dtypes, ctx.weight_shape = link, col, (weight.dtype, bias.dtype), weight.shape
+        return _C().mamba2.conv_fwd(xw, w, b, bd).view(B, S, C)
+
+    @staticmethod
+    def backward(ctx, du):
+        x, xw, w, b, bd = ctx.saved_tensors
+        C = w.shape[0]
+        if ctx.link is not None:
+            dx = ctx.link.window(x[..., ctx.col:ctx.col + C])
+            full, ctx.link.buffer = ctx.link.buffer, None
+        else:
+            full = torch.zeros_like(x)
+            dx = full[..., ctx.col:ctx.col + C]
+        _, dw, db = _C().mamba2.conv_bwd(_rows(du), xw, w, b, bd, dx.reshape(-1, C))
+        return full, dw.view(ctx.weight_shape).to(ctx.dtypes[0]), db.to(ctx.dtypes[1]), None, None, None
+
+
+def causal_conv1d_window(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, bounds: torch.Tensor, col: int = 0,
+                         link: Optional[Mamba2GradLink] = None) -> torch.Tensor:
+    """Mamba-2's causal depthwise convolution of width 4 with SiLU over the columns [col, col + C) of x [B, S, W] (in_proj's
+    output, read in place), weight [C, 1, 4], bias [C]: u[t] = silu(bias + sum_j weight[:, 0, j] x[t - 3 + j]) -> [B, S, C].
+    Taps before the document start of ``bounds`` (int32 [B, S, 2], ``document_bounds``) read zero; padding positions give zero.
+
+    CUDA bf16 x runs the native kernels (C and col multiples of 8, else ``ValueError``): fp32 sums with one bf16 rounding,
+    bitwise repeatable, no host synchronisation.  The gradient of x is [B, S, W]: with a ``link`` shared with ``ssd_scan``
+    and ``gated_rms_norm`` it is their common buffer, complete; without one its other columns are zero.  CPU x, and CUDA
+    fp32 or fp64 x, run ``causal_conv1d_window_reference``; CUDA x of any other dtype raises ``ValueError``."""
+    _mamba2_check_rows("causal_conv1d_window", x, bounds)
+    C = weight.shape[0]
+    if tuple(weight.shape) != (C, 1, MAMBA_CONV_WIDTH) or tuple(bias.shape) != (C,) or col < 0 or col + C > x.shape[-1]:
+        raise ValueError(f"causal_conv1d_window needs weight [C, 1, 4], bias [C] and columns [col, col + C) inside x, got "
+                         f"{tuple(weight.shape)}, {tuple(bias.shape)}, col {col} and x {tuple(x.shape)}")
+    if not _mamba_native("causal_conv1d_window", x):
+        return causal_conv1d_window_reference(x, weight, bias, bounds, col)
+    if C % 8 or col % 8 or x.shape[-1] % 8:
+        raise ValueError(f"causal_conv1d_window's kernels need C, col and W multiples of 8, got C {C}, col {col}, W {x.shape[-1]}")
+    return _CausalConv1dWindow.apply(x, weight, bias, bounds, col, link)
+
+
+def _ssd_shapes(who: str, xbc: torch.Tensor, dt: torch.Tensor, A_log, D, dt_bias, bounds, head_dim: int, state_size: int,
+                n_groups: int):
+    _mamba2_check_rows(who, xbc, bounds)
+    if head_dim != MAMBA2_HEAD_DIM or state_size != MAMBA2_STATE or n_groups != 1:
+        raise ValueError(f"{who} takes head dim 64, state 128 and one group, got head dim {head_dim}, state {state_size}, "
+                         f"{n_groups} groups")
+    B, S, _ = xbc.shape
+    H = dt.shape[-1] if dt.dim() == 3 else -1
+    if dt.dim() != 3 or tuple(dt.shape[:2]) != (B, S) or xbc.shape[-1] != H * head_dim + 2 * state_size:
+        raise ValueError(f"{who} needs dt [B, S, H] and xbc [B, S, 64 H + 256] (x | B | C), got {tuple(dt.shape)} and {tuple(xbc.shape)}")
+    if any(tuple(t.shape) != (H,) for t in (A_log, D, dt_bias)):
+        raise ValueError(f"{who} needs A_log, D and dt_bias [H] for H = {H}, got {tuple(A_log.shape)}, {tuple(D.shape)} and "
+                         f"{tuple(dt_bias.shape)}")
+    return B, S, H
+
+
+def ssd_scan_reference(xbc: torch.Tensor, dt: torch.Tensor, A_log: torch.Tensor, D: torch.Tensor, dt_bias: torch.Tensor,
+                       bounds: torch.Tensor, head_dim: int = MAMBA2_HEAD_DIM, state_size: int = MAMBA2_STATE,
+                       n_groups: int = 1) -> torch.Tensor:
+    """``ssd_scan`` in torch, fp32 (fp64 for fp64 input): the chunked SSD of transformers' ``Mamba2Mixer.torch_forward``
+    (intra-chunk C B^T o L, chunk states, their recurrence, state -> output) with the state reset at each document start:
+    L and the chunk states only join rows of one document, and a chunk's incoming state reaches only rows whose document
+    began before the chunk.  Padding positions give y = 0.  Differentiable."""
+    B, S, H = _ssd_shapes("ssd_scan_reference", xbc, dt, A_log, D, dt_bias, bounds, head_dim, state_size, n_groups)
+    dtype = _ref_dtype(xbc)
+    P, N, L = head_dim, state_size, MAMBA2_CHUNK
+    E = H * P
+    dev = xbc.device
+    real, start, _ = _mamba_positions(bounds, dev)
+    pad = (L - S % L) % L
+    nc = (S + pad) // L
+    pos = torch.arange(S + pad, device=dev)
+    real = F.pad(real, (0, pad))
+    start = F.pad(start, (0, pad), value=0)
+    v = dt.to(dtype) + dt_bias.to(dtype)
+    dts = F.softplus(v, threshold=MAMBA_SOFTPLUS_THRESHOLD) * real[:, :S, None]
+    xs = F.pad(xbc.to(dtype), (0, 0, 0, pad))
+    x = xs[..., :E].reshape(B, nc, L, H, P)
+    Bm, Cm = xs[..., E:E + N].reshape(B, nc, L, N), xs[..., E + N:].reshape(B, nc, L, N)
+    dts = F.pad(dts, (0, 0, 0, pad)).reshape(B, nc, L, H)
+    A = -torch.exp(A_log.to(dtype))
+    cum = torch.cumsum(A * dts, dim=2)                                    # [B, nc, L, H]
+    real_c, start_c, pos_c = real.reshape(B, nc, L), start.reshape(B, nc, L), pos.reshape(nc, L)
+    # same document, j <= i, both real
+    tri = torch.tril(torch.ones(L, L, dtype=torch.bool, device=dev))
+    same = (pos_c[None, :, None, :] >= start_c[..., :, None]) & tri & real_c[..., :, None] & real_c[..., None, :]   # [B, nc, i, j]
+    diff = cum[:, :, :, None, :] - cum[:, :, None, :, :]                  # [B, nc, i, j, H]
+    Lm = torch.exp(torch.where(same[..., None], diff, torch.full_like(diff, -math.inf))) * dts[:, :, None, :, :]
+    CB = torch.einsum("bcin,bcjn->bcij", Cm, Bm)
+    y = torch.einsum("bcijh,bcjhp->bcihp", Lm * CB[..., None], x)
+    # each chunk's outgoing state: the rows of its last document
+    last = start_c[..., -1]
+    for_state = real_c & real_c[..., -1:] & (start_c == last[..., None])                 # [B, nc, L]
+    wdecay = torch.exp(torch.where(for_state[..., None], cum[:, :, -1:, :] - cum, torch.full_like(cum, -math.inf))) * dts
+    states = torch.einsum("bcjh,bcjn,bcjhp->bchnp", wdecay, Bm, x)
+    carry = real_c[..., -1] & (last < pos_c[None, :, 0])                                 # [B, nc]
+    dec = torch.where(carry[..., None], torch.exp(cum[:, :, -1, :]), torch.zeros_like(cum[:, :, -1, :]))   # [B, nc, H]
+    h = torch.zeros(B, H, N, P, dtype=dtype, device=dev)
+    hin = []
+    for c in range(nc):
+        hin.append(h)
+        h = dec[:, c, :, None, None] * h + states[:, c]
+    hin = torch.stack(hin, 1)                                                            # [B, nc, H, N, P]
+    off = real_c & (start_c < pos_c[None, :, :1])                                        # [B, nc, L]
+    ecum = torch.exp(torch.where(off[..., None], cum, torch.full_like(cum, -math.inf)))
+    y = y + torch.einsum("bcin,bchnp->bcihp", Cm, hin) * ecum[..., None]
+    y = y + D.to(dtype)[:, None] * x
+    y = y.reshape(B, S + pad, E)[:, :S]
+    return torch.where(real[:, :S, None], y, torch.zeros_like(y)).to(xbc.dtype)
+
+
+class _SsdScan(torch.autograd.Function):
+    """(xbc [B, S, 64 H + 256], dt [B, S, H] view) bf16 -> y [B, S, 64 H] (csrc/mamba2.cu); nothing but the inputs is kept
+    for the backward, which recomputes the chunk states."""
+
+    @staticmethod
+    def forward(ctx, xbc, dt, A_log, D, dt_bias, bounds, link):
+        B, S, _ = xbc.shape
+        ins = [_rows(xbc), _row_view(dt), A_log.float().contiguous(), D.float().contiguous(), dt_bias.float().contiguous(),
+               _aligned16(bounds.to(torch.int32))]
+        y = _C().mamba2.ssd_fwd(*ins)
+        ctx.save_for_backward(dt, *ins)
+        ctx.link, ctx.dtypes, ctx.xshape = link, (A_log.dtype, D.dtype, dt_bias.dtype), xbc.shape
+        return y.view(B, S, -1)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dt, *ins = ctx.saved_tensors
+        given = ctx.link.window(dt) if ctx.link is not None else None
+        dxbc, ddt, dA_log, dD, dbias = _C().mamba2.ssd_bwd(_rows(dy), *ins, None if given is None else given.reshape(-1, dt.shape[-1]))
+        tA, tD, tb = ctx.dtypes
+        return (dxbc.view(ctx.xshape), None if given is not None else ddt.view(dt.shape), dA_log.to(tA), dD.to(tD), dbias.to(tb),
+                None, None)
+
+
+def ssd_scan(xbc: torch.Tensor, dt: torch.Tensor, A_log: torch.Tensor, D: torch.Tensor, dt_bias: torch.Tensor, bounds: torch.Tensor,
+             head_dim: int = MAMBA2_HEAD_DIM, state_size: int = MAMBA2_STATE, n_groups: int = 1,
+             link: Optional[Mamba2GradLink] = None) -> torch.Tensor:
+    """Mamba-2's SSD scan with the state reset at every document start: per row, head h (head dim 64) and state n (128),
+    dt = softplus(dt + dt_bias) (threshold 20), A = -exp(A_log), h_t = exp(dt_t A) h_{t-1} + dt_t B_t x_t^T with h = 0 before
+    each document, y_t = C_t h_t + D x_t.  xbc [B, S, 64 H + 256] is the conv's output x | B | C (one group: B and C shared by
+    all heads); dt [B, S, H] may be a column view of in_proj's output; A_log, D, dt_bias [H]; bounds int32 [B, S, 2]
+    (``document_bounds``).  Padding positions give y = 0 and zero gradients.  Head dims other than 64, states other than
+    128 and more than one group raise ``ValueError``.
+
+    CUDA bf16 activations run the native chunked scan on tensor cores (H a multiple of 8, else ``ValueError``): bf16
+    operands with fp32 sums and fp32 chunk states, gradients summed in a fixed order (bitwise repeatable), nothing read back
+    to the host.  With a ``link`` the gradient of dt goes into the link's buffer instead of being returned.  CPU activations,
+    and CUDA fp32 or fp64 ones, run ``ssd_scan_reference``; CUDA activations of any other dtype, or of mixed dtypes, raise
+    ``ValueError``."""
+    _ssd_shapes("ssd_scan", xbc, dt, A_log, D, dt_bias, bounds, head_dim, state_size, n_groups)
+    if not _mamba_native("ssd_scan", xbc, dt):
+        return ssd_scan_reference(xbc, dt, A_log, D, dt_bias, bounds)
+    if dt.shape[-1] % 8:
+        raise ValueError(f"ssd_scan's kernels need the head count a multiple of 8, got {dt.shape[-1]}")
+    return _SsdScan.apply(xbc, dt, A_log, D, dt_bias, bounds, link)
+
+
+def gated_rms_norm_reference(y: torch.Tensor, z: torch.Tensor, weight: torch.Tensor, eps: float) -> torch.Tensor:
+    """``gated_rms_norm`` in torch as transformers' ``MambaRMSNormGated``: g = y silu(z) in fp32 (fp64 for fp64 input),
+    weight * g * rsqrt(mean(g^2) + eps).  Differentiable."""
+    dtype = _ref_dtype(y)
+    g = y.to(dtype) * F.silu(z.to(dtype))
+    g = g * torch.rsqrt(g.pow(2).mean(-1, keepdim=True) + eps)
+    return (weight.to(dtype) * g).to(y.dtype)
+
+
+class _GatedRmsNorm(torch.autograd.Function):
+    """(y [B, S, E], z [B, S, E] view) bf16 -> weight * rmsnorm(y silu(z)) (csrc/layernorm.cu)."""
+
+    @staticmethod
+    def forward(ctx, y, z, weight, eps, link):
+        y2, z2, w = _rows(y), _row_view(z), weight.to(torch.bfloat16).contiguous()
+        out, rstd = _C().mamba2.gated_norm_fwd(y2, z2, w, eps)
+        ctx.save_for_backward(z, y2, z2, w, rstd)
+        ctx.link, ctx.wdtype = link, weight.dtype
+        return out.view(y.shape)
+
+    @staticmethod
+    def backward(ctx, dout):
+        z, y2, z2, w, rstd = ctx.saved_tensors
+        given = ctx.link.window(z) if ctx.link is not None else None
+        dy, dz, dw = _C().mamba2.gated_norm_bwd(_rows(dout), y2, z2, w, rstd, None if given is None else given.reshape(-1, z.shape[-1]))
+        return dy.view(dout.shape), None if given is not None else dz.view(z.shape), dw.to(ctx.wdtype), None, None
+
+
+def gated_rms_norm(y: torch.Tensor, z: torch.Tensor, weight: torch.Tensor, eps: float,
+                   link: Optional[Mamba2GradLink] = None) -> torch.Tensor:
+    """Mamba-2's gated RMSNorm over the last dim: weight * g / sqrt(mean(g^2) + eps) with g = y silu(z); y [..., E], z [..., E]
+    (it may be a column view of in_proj's output, read in place), weight [E].
+
+    CUDA bf16 y and z run the native wide RMSNorm kernels' gated variant (1024 < E <= 4096, E % 8 == 0, else ``ValueError``):
+    fp32 statistics, one bf16 rounding, dweight summed in a fixed order.  With a ``link`` the gradient of z goes into the
+    link's buffer instead of being returned.  CPU input, and CUDA fp32 or fp64 input, run ``gated_rms_norm_reference``;
+    CUDA input of any other dtype, or of mixed dtypes, raises ``ValueError``."""
+    if y.shape != z.shape or y.dim() < 1 or tuple(weight.shape) != (y.shape[-1],):
+        raise ValueError(f"gated_rms_norm needs y and z of one shape [..., E] and weight [E], got {tuple(y.shape)}, {tuple(z.shape)} "
+                         f"and {tuple(weight.shape)}")
+    if not _mamba_native("gated_rms_norm", y, z):
+        return gated_rms_norm_reference(y, z, weight, eps)
+    E = y.shape[-1]
+    if E % 8 or not 1024 < E <= 4096 or y.numel() == 0:
+        raise ValueError(f"gated_rms_norm's kernels need 1024 < E <= 4096 with E % 8 == 0 and at least one row, got {tuple(y.shape)}")
+    return _GatedRmsNorm.apply(y, z, weight, float(eps), link)
+
+
+# ------------------------------------------------------------------------------------------------
 # CLIP (csrc/clip.cu): captions as causal documents of one token stream, the contrastive loss over the global batch
 # ------------------------------------------------------------------------------------------------
 def caption_token_bounds(input_ids: torch.Tensor, eos_token_id: int):

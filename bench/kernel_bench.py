@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,swin,mamba,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,swin,mamba,mamba2,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -1266,6 +1266,67 @@ def main():
                 dy = torch.randn(T, E, device=dev, generator=g).to(torch.bfloat16)
                 ms = timeit(lambda: C.mamba.scan_bwd(dy, *sargs, hst, sumd), args.iters)
                 record(f"{label} scan bwd {layout}", ms, bytes_=T * (7 * E * 2 + (32 + R + 32) * 2) + 3 * state_bytes)
+
+    if "mamba2" in want:
+        # Mamba-2's conv over in_proj's xBC columns, chunked SSD scan and gated RMSNorm at mamba2-130m's and mamba2-370m's layer
+        # shapes (8 x 2048 rows, 24 / 32 heads of 64, state 128, W = 2E + 256 + H) on fixed, right-padded (lengths U[256, 2048])
+        # and packed rows.  Algorithmic counts, from shapes (ssd_counts): the SSD's matrix products per (chunk, head), each
+        # counted once and over full 64 x 64 tiles, and the bytes each pass must move: bf16 rows read and written once, the
+        # fp32 chunk states [B, chunks, H, 128, 64] written by the state kernel, read and written by the pass, and read by the
+        # output (forward) or gradient (backward) kernel, two such buffers in the backward.
+        from b200ddp.ops import document_bounds
+        print(f"mamba2 kernels on {card()}", flush=True)
+        Bm, Sm, L, N, P = 8, 2048, 64, 128, 64
+
+        def ssd_counts(T, H, nc):
+            E = H * P
+            CD = E + 2 * N
+            state = Bm * nc * H * N * P * 4
+            f_fwd = Bm * nc * (2 * L * L * N + H * 2 * L * P * (L + 2 * N))
+            f_bwd = Bm * nc * (2 * L * L * N + H * (2 * L * N * P * 2 + 2 * L * L * P * 2 + 2 * L * P * N * 5 + 2 * L * L * N * 2))
+            b_fwd = T * (CD + H + E) * 2 + 4 * state
+            b_bwd = T * (E + CD + H + CD + H) * 2 + 8 * state
+            return f_fwd, b_fwd, f_bwd, b_bwd
+
+        for label, H in (("mamba2-130m", 24), ("mamba2-370m", 32)):
+            E = H * P
+            CD, W = E + 2 * N, 2 * E + 2 * N + H
+            g = torch.Generator(device="cuda").manual_seed(E)
+            for layout in ("fixed", "padded", "packed"):
+                ids = torch.randint(2, 1000, (Bm, Sm), device=dev, generator=g)
+                if layout != "fixed":
+                    lens = torch.randint(256, Sm + 1, (Bm, 1), device=dev, generator=g)
+                    ids = torch.where(torch.arange(Sm, device=dev) < lens, ids, 0)
+                    if layout == "packed":
+                        ids = torch.where(torch.rand(Bm, Sm, device=dev, generator=g) < 1 / 512, 1, ids) * (ids != 0)
+                bounds = document_bounds(ids, 1 if layout == "packed" else None, None if layout == "fixed" else 0)[0].to(torch.int32)
+                T = Bm * Sm
+                zx = torch.randn(T, W, device=dev, generator=g).to(torch.bfloat16)
+                w32 = torch.randn(CD, 4, device=dev, generator=g) * 0.5
+                b32 = torch.zeros(CD, device=dev)
+                xw, z, dt = zx[:, E:E + CD], zx[:, :E], zx[:, W - H:]
+                u = C.mamba2.conv_fwd(xw, w32, b32, bounds)
+                ms = timeit(lambda: C.mamba2.conv_fwd(xw, w32, b32, bounds), args.iters)
+                record(f"{label} conv fwd {layout}", ms, bytes_=T * CD * 2 * 2)
+                du = torch.randn(T, CD, device=dev, generator=g).to(torch.bfloat16)
+                dzx = torch.empty_like(zx)
+                ms = timeit(lambda: C.mamba2.conv_bwd(du, xw, w32, b32, bounds, dzx[:, E:E + CD]), args.iters)
+                record(f"{label} conv bwd {layout}", ms, bytes_=T * CD * 2 * 3 + 2 * 5 * CD * 4 * Bm * Sm // 32)
+                A_log = torch.log(torch.arange(1, H + 1.0, device=dev))
+                D, dtb = torch.ones(H, device=dev), torch.full((H,), -4.0, device=dev)
+                f_fwd, b_fwd, f_bwd, b_bwd = ssd_counts(T, H, (Sm + L - 1) // L)
+                ms = timeit(lambda: C.mamba2.ssd_fwd(u, dt, A_log, D, dtb, bounds), args.iters)
+                record(f"{label} ssd fwd {layout}", ms, flops=f_fwd, bytes_=b_fwd)
+                dy = torch.randn(T, E, device=dev, generator=g).to(torch.bfloat16)
+                ms = timeit(lambda: C.mamba2.ssd_bwd(dy, u, dt, A_log, D, dtb, bounds, dzx[:, W - H:]), args.iters)
+                record(f"{label} ssd bwd {layout}", ms, flops=f_bwd, bytes_=b_bwd)
+                y = torch.randn(T, E, device=dev, generator=g).to(torch.bfloat16)
+                nw = torch.ones(E, device=dev, dtype=torch.bfloat16)
+                out, rstd = C.mamba2.gated_norm_fwd(y, z, nw, 1e-5)
+                ms = timeit(lambda: C.mamba2.gated_norm_fwd(y, z, nw, 1e-5), args.iters)
+                record(f"{label} gated norm fwd {layout}", ms, bytes_=T * E * 2 * 3)
+                ms = timeit(lambda: C.mamba2.gated_norm_bwd(dy, y, z, nw, rstd, dzx[:, :E]), args.iters)
+                record(f"{label} gated norm bwd {layout}", ms, bytes_=T * E * 2 * 5)
 
     if args.out:
         os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)

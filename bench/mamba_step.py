@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""mamba-130m training step: ms/step, tokens/s and peak memory of this package, and a row for transformers' slow path.
+"""Mamba training step (mamba-130m by default, or --model mamba-370m, mamba2-130m, mamba2-370m, several in one call):
+ms/step, tokens/s and peak memory of this package, and for mamba-130m a row for transformers' slow path.
 
-  python bench/mamba_step.py [--batch 8] [--seq_len 2048] [--steps 30] [--out mamba_step.json]
+  python bench/mamba_step.py [--model mamba-130m[,mamba2-130m]] [--batch 8] [--seq_len 2048] [--steps 30] [--out mamba_step.json]
 
 Native runs, each a fresh process:
-  python ddp.py --model mamba-130m --fp16 --optimizer adamw --per_gpu_train_batch_size B --seq_len S --max_steps N
+  python ddp.py --model MODEL --fp16 --optimizer adamw --per_gpu_train_batch_size B --seq_len S --max_steps N
   --logging_steps N/2 [--cuda_graph] with fixed rows, --min_seq_len 256, --min_seq_len 256 --pack and --fused_lm_loss
   (bf16 weights, fp32 masters, the native kernels).  ms/step is the mean over the second half of the steps (the trainer's
   own CUDA-event timer); tokens/s counts every row position, padding included.
@@ -62,8 +63,8 @@ def transformers_run(batch, seq_len, steps):
             "peak_mem_gb": torch.cuda.max_memory_allocated(dev) / 2 ** 30, "last_loss": float(loss)}
 
 
-def native_run(batch, seq_len, steps, flags, tmp):
-    argv = [sys.executable, os.path.join(ROOT, "ddp.py"), "--model", "mamba-130m", "--fp16", "--optimizer", "adamw",
+def native_run(batch, seq_len, steps, flags, tmp, model="mamba-130m"):
+    argv = [sys.executable, os.path.join(ROOT, "ddp.py"), "--model", model, "--fp16", "--optimizer", "adamw",
             "--per_gpu_train_batch_size", str(batch), "--seq_len", str(seq_len), "--max_steps", str(steps),
             "--logging_steps", str(steps // 2), "--save_steps", "0", "--no_tensorboard", "--output_dir", os.path.join(tmp, "out"),
             "--lr", "1e-4", *flags]
@@ -83,6 +84,7 @@ def native_run(batch, seq_len, steps, flags, tmp):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", type=str, default="mamba-130m", help="comma-separated: mamba-130m, mamba-370m, mamba2-130m, mamba2-370m")
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--seq_len", type=int, default=2048)
     ap.add_argument("--steps", type=int, default=30)
@@ -96,32 +98,38 @@ def main():
         print(json.dumps(transformers_run(args.hf_batch, args.hf_seq_len, args.hf_steps)), flush=True)
         return
     gpu = card()
-    print(f"mamba-130m {args.batch} x {args.seq_len}, {args.steps} steps, on {gpu}", flush=True)
-    runs = [(f"{mode} {graph}", flags + (["--cuda_graph"] if graph == "graph" else []))
-            for mode, flags in (("fixed", []), ("min_seq_len 256", ["--min_seq_len", "256"]),
-                                ("pack", ["--min_seq_len", "256", "--pack"]), ("fused_lm_loss", ["--fused_lm_loss"]))
-            for graph in ("graph", "eager")]
+    models = args.model.split(",")
+    unknown = set(models) - {"mamba-130m", "mamba-370m", "mamba2-130m", "mamba2-370m"}
+    if unknown:
+        raise SystemExit(f"unknown --model {sorted(unknown)}")
     rows = []
     with tempfile.TemporaryDirectory() as tmp:
-        for name, flags in runs:
-            res = native_run(args.batch, args.seq_len, args.steps, flags, tmp)
-            res.update(run=f"native {name}", batch=args.batch, seq_len=args.seq_len, card=gpu)
+        for model in models:
+            print(f"{model} {args.batch} x {args.seq_len}, {args.steps} steps, on {gpu}", flush=True)
+            runs = [(f"{mode} {graph}", flags + (["--cuda_graph"] if graph == "graph" else []))
+                    for mode, flags in (("fixed", []), ("min_seq_len 256", ["--min_seq_len", "256"]),
+                                        ("pack", ["--min_seq_len", "256", "--pack"]), ("fused_lm_loss", ["--fused_lm_loss"]))
+                    for graph in ("graph", "eager")]
+            for name, flags in runs:
+                res = native_run(args.batch, args.seq_len, args.steps, flags, tmp, model)
+                res.update(run=f"native {model} {name}", batch=args.batch, seq_len=args.seq_len, card=gpu)
+                rows.append(res)
+                print(json.dumps(res), flush=True)
+        if "mamba-130m" in models:
+            res = native_run(args.hf_batch, args.hf_seq_len, args.steps, ["--cuda_graph"], tmp)
+            res.update(run="native fixed graph", batch=args.hf_batch, seq_len=args.hf_seq_len, card=gpu)
             rows.append(res)
             print(json.dumps(res), flush=True)
-        res = native_run(args.hf_batch, args.hf_seq_len, args.steps, ["--cuda_graph"], tmp)
-        res.update(run="native fixed graph", batch=args.hf_batch, seq_len=args.hf_seq_len, card=gpu)
-        rows.append(res)
-        print(json.dumps(res), flush=True)
-        proc = subprocess.run([sys.executable, os.path.abspath(__file__), "--transformers_only", "--hf_batch", str(args.hf_batch),
-                               "--hf_seq_len", str(args.hf_seq_len), "--hf_steps", str(args.hf_steps)], capture_output=True, text=True,
-                              cwd=tmp)
-        if proc.returncode != 0:
-            raise RuntimeError(f"transformers run failed:\n{proc.stdout[-2000:]}{proc.stderr[-4000:]}")
-        res = json.loads(proc.stdout.strip().splitlines()[-1])
-        res.update(run="transformers MambaForCausalLM slow_forward, bf16 autocast, fused AdamW", batch=args.hf_batch,
-                   seq_len=args.hf_seq_len, card=gpu)
-        rows.append(res)
-        print(json.dumps(res), flush=True)
+            proc = subprocess.run([sys.executable, os.path.abspath(__file__), "--transformers_only", "--hf_batch", str(args.hf_batch),
+                                   "--hf_seq_len", str(args.hf_seq_len), "--hf_steps", str(args.hf_steps)], capture_output=True, text=True,
+                                  cwd=tmp)
+            if proc.returncode != 0:
+                raise RuntimeError(f"transformers run failed:\n{proc.stdout[-2000:]}{proc.stderr[-4000:]}")
+            res = json.loads(proc.stdout.strip().splitlines()[-1])
+            res.update(run="transformers MambaForCausalLM slow_forward, bf16 autocast, fused AdamW", batch=args.hf_batch,
+                       seq_len=args.hf_seq_len, card=gpu)
+            rows.append(res)
+            print(json.dumps(res), flush=True)
     if args.out:
         with open(args.out, "w") as f:
             json.dump(rows, f, indent=1)
