@@ -170,7 +170,8 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin, _C.mamba and _C.mamba2 namespaces of static entry points
+// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin, _C.mamba, _C.mamba2 and _C.whisper namespaces of static
+// entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
 struct T5Namespace {};
@@ -178,6 +179,7 @@ struct ConvNextNamespace {};
 struct SwinNamespace {};
 struct MambaNamespace {};
 struct Mamba2Namespace {};
+struct WhisperNamespace {};
 
 // An NHWC activation of the depthwise convolution: bf16 [B, H, W, C] contiguous and 16-byte aligned, B, H, W >= 1,
 // 8 <= C <= 1024 with C % 8 == 0 (B is the grid's z extent).  Returns (B, H, W, C).
@@ -263,6 +265,23 @@ std::array<int64_t, 4> ssd_args(Args& args, const at::Tensor& xbc, const at::Ten
   const int64_t dtp = row_view(args, "dt", dt, B * S, H);
   args("A_log", A_log, {kF32}, {H})("D", D, {kF32}, {H})("dt_bias", dt_bias, {kF32}, {H});
   return {B, S, H, dtp};
+}
+
+// Whisper's stem rows: frames F even and >= 2, rows S >= F / 2, then t bf16 [B * n, cols] contiguous and 16-byte aligned
+// with n = F (h1, dh1) or S (P2, dP2), 1 <= B, cols = d or 3 d with d a positive multiple of 8, and fewer than 2^31
+// elements on either side.  Returns (B, d).
+std::array<int64_t, 2> stem_rows(Args& args, const char* name, const at::Tensor& t, int64_t frames, int64_t rows, bool patches) {
+  if (frames < 2 || frames % 2 || rows < frames / 2 || rows > (1ll << 24))
+    args.fail("frames", "even and >= 2, with rows >= frames / 2", "frames " + std::to_string(frames) + ", rows " + std::to_string(rows));
+  args(name, t, {kBF16}, {kAny, kAny}, kContiguous, 16);
+  const int64_t n = patches ? rows : frames, cols = t.size(1), d = patches ? cols / 3 : cols;
+  const int64_t B = t.size(0) / n;
+  if (t.size(0) < n || t.size(0) % n || d < 8 || d % 8 || (patches && cols % 3) || B * rows * 3 * d >= (1ll << 31) ||
+      B * frames * 3 * d >= (1ll << 31))
+    args.fail(name, std::string("bf16 [B * ") + (patches ? "rows, 3 d]" : "frames, d]") +
+                        " with B >= 1, d a positive multiple of 8 and fewer than 2^31 elements",
+              describe(t));
+  return {B, d};
 }
 
 CommCtx make_ctx(PeerArena& a, size_t pad_off, double timeout_s) {
@@ -2091,4 +2110,56 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                              dy.data_ptr(), dz.data_ptr(), dzp, wpart.data_ptr<float>(), dweight.data_ptr(), cur_stream());
     return std::make_tuple(dy, dz, dweight);
   }, py::arg("dout"), py::arg("y"), py::arg("z"), py::arg("weight"), py::arg("rstd"), py::arg("dz_out") = py::none());
+
+  // ---- Whisper's log-mel front end and stem gathers (whisper.cu) ------------------------------------------------------------
+  // _C.whisper is a namespace of static entry points like _C.mamba2; its contract rows are in tests/test_whisper_bindings_cpu.py.
+  py::class_<WhisperNamespace> whisper(m, "whisper", "Whisper's log-mel front end and convolution-stem gathers (whisper.cu)");
+  // log-mel features [B, 80, 3000] of int16 waveforms [B, 480000] through filters fp32 [201, 80]: bf16 when `bf16`, else fp32;
+  // written into `out` when given (contiguous, that dtype, B * 80 * 3000 elements) and returned
+  whisper.def_static("log_mel", [](at::Tensor wave, at::Tensor filters, bool bf16, c10::optional<at::Tensor> out) {
+    Args args("log_mel");
+    args("wave", wave, {at::kShort}, {kAny, 480000});
+    const int64_t B = wave.size(0);
+    if (B < 1 || B > 65535) args.fail("wave", "int16 [B, 480000] with 1 <= B <= 65535", describe(wave));
+    args("filters", filters, {kF32}, {201, 80});
+    at::Tensor o;
+    args.out(o, "out", out, {B, 80, 3000}, wave.options().dtype(bf16 ? kBF16 : kF32));
+    args.device();
+    const auto f32 = wave.options().dtype(kF32);
+    at::Tensor part = at::empty({B, (int64_t)log_mel_partials()}, f32);
+    at::Tensor logmel = bf16 ? at::empty({B, 80, 3000}, f32) : o;
+    launch_log_mel(wave.data_ptr(), filters.data_ptr<float>(), (int)B, bf16, logmel.data_ptr<float>(), part.data_ptr<float>(), o.data_ptr(),
+                   cur_stream());
+    return o.view({B, 80, 3000});
+  }, py::arg("wave"), py::arg("filters"), py::arg("bf16"), py::arg("out") = py::none());
+  // P1 bf16 [B F, 240] of features bf16 [B, 80, F]
+  whisper.def_static("mel_patches", [](at::Tensor features) {
+    Args args("mel_patches");
+    args("features", features, {kBF16}, {kAny, 80, kAny});
+    const int64_t B = features.size(0), F = features.size(2);
+    if (B < 1 || F < 1 || B * F * 240 >= (1ll << 31))
+      args.fail("features", "bf16 [B, 80, F] with B, F >= 1 and fewer than 2^31 / 3 elements", describe(features));
+    args.device();
+    at::Tensor p1 = at::empty({B * F, 240}, features.options());
+    launch_mel_patches(features.data_ptr(), (int)B, (int)F, p1.data_ptr(), cur_stream());
+    return p1;
+  }, py::arg("features"));
+  // P2 bf16 [B rows, 3 d] of h1 bf16 [B frames, d]
+  whisper.def_static("frame_patches", [](at::Tensor h1, int64_t frames, int64_t rows) {
+    Args args("frame_patches");
+    const auto [B, d] = stem_rows(args, "h1", h1, frames, rows, false);
+    args.device();
+    at::Tensor p2 = at::empty({B * rows, 3 * d}, h1.options());
+    launch_frame_patches(h1.data_ptr(), (int)B, (int)frames, (int)rows, (int)d, p2.data_ptr(), cur_stream());
+    return p2;
+  }, py::arg("h1"), py::arg("frames"), py::arg("rows"));
+  // dh1 bf16 [B frames, d] of dP2 bf16 [B rows, 3 d]
+  whisper.def_static("frame_patches_bwd", [](at::Tensor dp2, int64_t frames, int64_t rows) {
+    Args args("frame_patches_bwd");
+    const auto [B, d] = stem_rows(args, "dp2", dp2, frames, rows, true);
+    args.device();
+    at::Tensor dh1 = at::empty({B * frames, d}, dp2.options());
+    launch_frame_patches_bwd(dp2.data_ptr(), (int)B, (int)frames, (int)rows, (int)d, dh1.data_ptr(), cur_stream());
+    return dh1;
+  }, py::arg("dp2"), py::arg("frames"), py::arg("rows"));
 }

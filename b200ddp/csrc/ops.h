@@ -334,7 +334,18 @@ void launch_gated_rmsnorm_fwd(const void* x, const void* z, long long zp, const 
 void launch_gated_rmsnorm_bwd(const void* dy, const void* x, const void* z, long long zp, const void* gamma, const float* rstd, int rows,
                               int cols, void* dx, void* dz, long long dzp, float* wpart, void* dgamma, cudaStream_t s);
 
-// ---------------- CLIP contrastive loss (clip.cu) ---------------------------------------------------
+// ---------------- Whisper's log-mel front end and stem gathers (whisper.cu) --------------------------------------------
+// Log-mel: wave int16 [B, 480000], filters fp32 [201, 80] -> out [B, 80, 3000] (bf16 when bf16_out, else fp32).  Scratch:
+// logmel fp32 [B, 80, 3000] (may be out itself for fp32 output), part_max fp32 [B, log_mel_partials()].
+int log_mel_partials();
+void launch_log_mel(const void* wave, const float* filters, int B, bool bf16_out, float* logmel, float* part_max, void* out, cudaStream_t s);
+// bf16 features [B, 80, F] -> P1 [B F, 240]; h1 [B F, d] -> P2 [B S, 3 d] (F even, S >= F / 2, d % 8 == 0) and its
+// backward dP2 [B S, 3 d] -> dh1 [B F, d]
+void launch_mel_patches(const void* features, int B, int F, void* p1, cudaStream_t s);
+void launch_frame_patches(const void* h1, int B, int F, int S, int d, void* p2, cudaStream_t s);
+void launch_frame_patches_bwd(const void* dp2, int B, int F, int S, int d, void* dh1, cudaStream_t s);
+
+// ---------------- CLIP contrastive loss (clip.cu)---------------------------------------------------
 // u bf16 [B, D] = x / ||x|| per row (fp32, one rounding), rnorm fp32 [B] = 1 / ||x||; D % 8 == 0, 16-byte aligned rows
 void launch_l2norm_fwd(const void* x, int B, int D, void* u, float* rnorm, cudaStream_t s);
 // dx bf16 [B, D] = rnorm (du - u <u, du>) with u = x rnorm in fp32

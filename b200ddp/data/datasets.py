@@ -4,6 +4,7 @@ holds the same data).  The ImageNet- and token-shaped variants feed the benchmar
 (there is no network for real data)."""
 from __future__ import annotations
 
+import math
 from typing import Tuple
 
 import torch
@@ -92,6 +93,54 @@ class SyntheticImageText(Dataset):
         ids = torch.where(pos == (lens - 1)[:, None], torch.full_like(ids, self.EOT_ID), ids)
         self.Y = torch.where(pos >= lens[:, None], torch.full_like(ids, self.PAD_ID), ids)
         self.caption_lengths = lens
+
+    def __len__(self) -> int:
+        return self.samples
+
+    def __getitem__(self, index):
+        return self.X[index], self.Y[index]
+
+    def batch(self, indices: torch.Tensor):
+        return self.X.index_select(0, indices), self.Y.index_select(0, indices)
+
+    def batch_into(self, indices: torch.Tensor, outs) -> None:
+        """Gather straight into caller-owned (pinned) buffers: one pass over the data."""
+        torch.index_select(self.X, 0, indices, out=outs[0])
+        torch.index_select(self.Y, 0, indices, out=outs[1])
+
+
+class SyntheticSpeech(Dataset):
+    """Waveform / transcript pairs for Whisper (seeded): ``X`` int16 PCM [samples, 480000] (30 seconds at 16 kHz) and ``Y``
+    labels int64 [seq_len].  A transcript holds n tokens from [0, ``EOT_ID``) followed by ``EOT_ID``, then -100; n + 1 is
+    ``seq_len`` or, with ``min_len``, uniform in [min_len, seq_len].  The clip carries one segment per token, a tone whose
+    pitch follows the token plus noise, over the first n / seq_len of the clip, and silence after it.  There is no pad id:
+    the labels' -100 padding gives the transcript lengths.  128 clips take 123 MB."""
+
+    EOT_ID = 50256                 # <|endoftext|>
+    SAMPLES = 480000
+    RATE = 16000
+
+    def __init__(self, samples: int = 128, seq_len: int = 448, min_len: int | None = None, seed: int = 1234):
+        if min_len is not None and not 1 <= min_len <= seq_len:
+            raise ValueError(f"SyntheticSpeech: min_len must lie in [1, seq_len = {seq_len}], got {min_len}")
+        g = torch.Generator().manual_seed(seed)
+        self.samples = int(samples)
+        lens = torch.full((self.samples,), seq_len) if min_len is None else torch.randint(min_len, seq_len + 1, (self.samples,), generator=g)
+        pos = torch.arange(seq_len)[None, :]
+        ids = torch.randint(0, self.EOT_ID, (self.samples, seq_len), generator=g)
+        ids = torch.where(pos == (lens - 1)[:, None], torch.full_like(ids, self.EOT_ID), ids)
+        self.Y = torch.where(pos >= lens[:, None], torch.full_like(ids, -100), ids)
+        self.X = torch.zeros(self.samples, self.SAMPLES, dtype=torch.int16)
+        seg = self.SAMPLES // seq_len
+        for i in range(self.samples):
+            n = int(lens[i]) - 1
+            if n == 0:
+                continue
+            freq = (100.0 + 60.0 * (ids[i, :n] % 64).double()).repeat_interleave(seg)
+            amp = (2000.0 + 6000.0 * torch.rand(n, generator=g, dtype=torch.float64)).repeat_interleave(seg)
+            t = torch.arange(n * seg, dtype=torch.float64) / self.RATE
+            wave = amp * torch.sin(2 * math.pi * freq * t) + 300.0 * torch.randn(n * seg, generator=g, dtype=torch.float64)
+            self.X[i, :n * seg] = wave.round().clamp(-32768, 32767).to(torch.int16)
 
     def __len__(self) -> int:
         return self.samples

@@ -161,6 +161,7 @@ def setup(args):
     check_moe_args(args)
     check_contrastive_args(args)
     check_seq2seq_args(args)
+    check_speech_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -325,6 +326,15 @@ def check_seq2seq_args(args) -> None:
             raise ValueError(f"--model {args.model} on a GPU needs --fp16: its attention kernels read bf16 activations")
         if args.seq_len % 128:
             raise ValueError(f"--model {args.model} on a GPU needs --seq_len to be a multiple of 128 (got {args.seq_len})")
+
+
+def check_speech_args(args) -> None:
+    """A speech model (Whisper) trains on rows that each hold one 30-second clip and its transcript: ``--pack`` does not
+    apply.  ``--seq_len`` is the transcript row length."""
+    if not model_entry(args.model).speech:
+        return
+    if getattr(args, "pack", False):
+        raise ValueError(f"--pack does not apply to --model {args.model}: each row holds one 30-second clip and its transcript")
 
 
 def padding_on(args) -> bool:

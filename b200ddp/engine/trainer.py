@@ -23,7 +23,7 @@ from tqdm import tqdm
 from tqdm.auto import trange
 
 from ..data import (BatchLoader, DevicePrefetcher, FooDataset, SyntheticDenoising, SyntheticImageNet, SyntheticImageText, SyntheticSpanCorruption,
-                    SyntheticTokens)
+                    SyntheticSpeech, SyntheticTokens)
 from ..models import T5Config, model_entry
 from ..ops import ClipLoss, CrossEntropyLoss, MSELoss
 from ..optim import FusedAdamW, FusedSGD, get_linear_schedule_with_warmup, weight_decay_groups
@@ -46,7 +46,7 @@ def _summary_writer():
 
 def build_dataset(args):
     """``args.model``'s synthetic data: the reference's ``FooDataset``, ImageNet-shaped images, image-caption pairs (a whole
-    number of global batches), source / target pairs for an encoder-decoder, or token rows over the model's vocabulary
+    number of global batches), waveform / transcript pairs for a speech model, source / target pairs for an encoder-decoder, or token rows over the model's vocabulary
     whose packed documents start with its registry entry's ``start_id``."""
     entry = model_entry(getattr(args, "model", "foo"))
     n = int(getattr(args, "dataset_size", 100000))
@@ -59,6 +59,8 @@ def build_dataset(args):
     if entry.kind == "image":
         dense = loss_kind(args) == "mse"
         return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
+    if entry.speech:
+        return SyntheticSpeech(samples=min(n, 128), seq_len=int(getattr(args, "seq_len", 448)), min_len=getattr(args, "min_seq_len", None))
     if entry.seq2seq and isinstance(entry.config, T5Config):
         return SyntheticSpanCorruption(samples=min(n, 512), seq_len=int(getattr(args, "seq_len", 512)), vocab=entry.config.vocab_size,
                                        start_id=entry.start_id, min_len=getattr(args, "min_seq_len", None), pack=bool(getattr(args, "pack", False)))
@@ -195,6 +197,8 @@ class Trainer:
         self.paired = entry.contrastive or entry.seq2seq
         if input_transform is None and self.device.type == "cuda" and model_entry(getattr(args, "model", "foo")).kind == "image":
             input_transform = self._make_image_transform()
+        if input_transform is None and entry.speech:
+            input_transform = self._make_speech_transform()
         self.step_fn = TrainStep(model, self.criterion, self.optimizer, self.device,
                                  accumulation=args.gradient_accumulation_steps, use_graph=getattr(args, "cuda_graph", False),
                                  input_transform=input_transform, paired=self.paired,
@@ -277,6 +281,21 @@ class Trainer:
                 return x.to(self.compute_dtype)
             C.normalize_to_channels_last(x, dst, mean, inv_std, 1.0 / 255.0 if x.dtype == torch.uint8 else 1.0)
             return dst
+        return transform
+
+    def _make_speech_transform(self):
+        """int16 waveforms [B, 480000] -> log-mel features [B, 80, 3000] in the compute dtype (``ops.log_mel_spectrogram``:
+        the native kernels on the GPU, written into the CUDA graph's static input once that exists; the reference on the CPU)."""
+        from ..ops import log_mel_spectrogram, whisper_mel_filters
+        filters = whisper_mel_filters().to(self.device, torch.float32)
+
+        def transform(x):
+            if x.dtype != torch.int16:
+                return x
+            dst = self.step_fn.static_inputs()[0]
+            if dst is not None and (tuple(dst.shape) != (x.shape[0], 80, 3000) or dst.dtype != self.compute_dtype):
+                dst = None
+            return log_mel_spectrogram(x, filters, self.compute_dtype, out=dst)
         return transform
 
     def _world(self) -> int:

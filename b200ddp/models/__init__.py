@@ -20,6 +20,8 @@ from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneratio
 from .t5 import T5_BASE, T5_SMALL, T5Config, T5ForConditionalGeneration, t5_base, t5_small
 from .mamba import MAMBA_130M, MAMBA_370M, MambaConfig, MambaForCausalLM, mamba_130m, mamba_370m
 from .mamba2 import MAMBA2_130M, MAMBA2_370M, Mamba2Config, Mamba2ForCausalLM, mamba2_130m, mamba2_370m
+from .whisper import (WHISPER_BASE, WHISPER_SMALL, WHISPER_TINY, WhisperConfig, WhisperForConditionalGeneration, whisper_base, whisper_small,
+                      whisper_tiny)
 
 
 @dataclass(frozen=True)
@@ -36,6 +38,8 @@ class ModelEntry:
                                        # (CLIP): forward(images, input_ids), the criterion ops.ClipLoss
     seq2seq: bool = False              # encoder-decoder trained on source / target pairs (BART, T5): forward(source_ids, labels),
                                        # kind "causal" (the decoder is a causal LM over the target)
+    speech: bool = False               # an encoder-decoder trained on waveform / transcript pairs (Whisper): forward(features,
+                                       # labels) on the log-mel features of int16 clips
 
     @property
     def token_model(self) -> bool:
@@ -80,6 +84,10 @@ MODEL_REGISTRY = {
     "mamba-370m": ModelEntry(mamba_370m, "causal", MAMBA_370M, start_id=1),
     "mamba2-130m": ModelEntry(mamba2_130m, "causal", MAMBA2_130M, start_id=1),
     "mamba2-370m": ModelEntry(mamba2_370m, "causal", MAMBA2_370M, start_id=1),
+    # <|startoftranscript|>; a row holds one clip and its transcript, so the id only starts each decoder input
+    "whisper-tiny": ModelEntry(whisper_tiny, "causal", WHISPER_TINY, start_id=50257, seq2seq=True, speech=True),
+    "whisper-base": ModelEntry(whisper_base, "causal", WHISPER_BASE, start_id=50257, seq2seq=True, speech=True),
+    "whisper-small": ModelEntry(whisper_small, "causal", WHISPER_SMALL, start_id=50257, seq2seq=True, speech=True),
 }
 
 
@@ -95,4 +103,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "Mamba2Config", "Mamba2ForCausalLM", "mamba2_130m", "mamba2_370m", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "Mamba2Config", "Mamba2ForCausalLM", "mamba2_130m", "mamba2_370m", "WhisperConfig", "WhisperForConditionalGeneration", "whisper_tiny", "whisper_base", "whisper_small", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

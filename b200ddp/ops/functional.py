@@ -2579,3 +2579,139 @@ def clip_loss(image_embeds: torch.Tensor, text_embeds: torch.Tensor, logit_scale
     s = logit_scale.exp()
     labels = torch.arange(B, device=image_embeds.device) + rank * B
     return (F.cross_entropy((u_img @ U_txt.t()) * s, labels) + F.cross_entropy((u_txt @ U_img.t()) * s, labels)) / 2.0
+
+
+# ------------------------------------------------------------------------------------------------
+# Whisper's audio side (csrc/whisper.cu): the log-mel front end and the gathers of the two-convolution stem
+# ------------------------------------------------------------------------------------------------
+WHISPER_SAMPLES = 480000         # a 30-second clip at 16 kHz
+WHISPER_N_FFT, WHISPER_HOP = 400, 160
+
+
+def whisper_mel_filters(num_mel_bins: int = 80, n_fft: int = WHISPER_N_FFT, sampling_rate: int = 16000) -> torch.Tensor:
+    """Whisper's mel filterbank, fp64 [n_fft // 2 + 1, num_mel_bins]: triangular filters on the Slaney mel scale between 0 Hz
+    and sampling_rate / 2, each scaled to unit area (Slaney normalisation), as ``WhisperFeatureExtractor.mel_filters``."""
+    f_sp, min_log_hz, min_log_mel, logstep = 200.0 / 3, 1000.0, 15.0, math.log(6.4) / 27.0
+
+    def hz_to_mel(f):
+        return torch.where(f >= min_log_hz, min_log_mel + torch.log(f.clamp(min=min_log_hz) / min_log_hz) / logstep, f / f_sp)
+
+    def mel_to_hz(m):
+        return torch.where(m >= min_log_mel, min_log_hz * torch.exp(logstep * (m - min_log_mel)), f_sp * m)
+
+    edges = torch.tensor([0.0, sampling_rate / 2], dtype=torch.float64)
+    mels = hz_to_mel(edges)
+    freqs = mel_to_hz(torch.linspace(float(mels[0]), float(mels[1]), num_mel_bins + 2, dtype=torch.float64))
+    fft_freqs = torch.linspace(0, sampling_rate // 2, n_fft // 2 + 1, dtype=torch.float64)
+    diff = freqs[1:] - freqs[:-1]
+    slopes = freqs[None, :] - fft_freqs[:, None]
+    down, up = -slopes[:, :-2] / diff[:-1], slopes[:, 2:] / diff[1:]
+    filters = torch.clamp(torch.minimum(down, up), min=0.0)
+    return filters * (2.0 / (freqs[2:] - freqs[:-2]))[None, :]
+
+
+def log_mel_spectrogram_reference(waveform: torch.Tensor, mel_filters: torch.Tensor, dtype=torch.float64) -> torch.Tensor:
+    """Whisper's log-mel features of int16 waveforms [B, N] in ``dtype``: [B, mels, N / 160], as transformers'
+    ``WhisperFeatureExtractor`` (its ``_torch_extract_fbank_features``) computes them from waveform / 32768."""
+    x = waveform.to(dtype) / 32768.0
+    window = torch.hann_window(WHISPER_N_FFT, periodic=True, dtype=dtype, device=x.device)
+    stft = torch.stft(x, WHISPER_N_FFT, WHISPER_HOP, window=window, center=True, pad_mode="reflect", return_complex=True)
+    power = stft[..., :-1].abs() ** 2
+    L = (mel_filters.to(dtype=dtype, device=x.device).T @ power).clamp(min=1e-10).log10()
+    M = L.amax(dim=(1, 2), keepdim=True)
+    return (torch.maximum(L, M - 8.0) + 4.0) / 4.0
+
+
+def log_mel_spectrogram(waveform: torch.Tensor, mel_filters: torch.Tensor, out_dtype=torch.bfloat16,
+                        out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Whisper's log-mel features [B, 80, 3000] in ``out_dtype`` (bf16 or fp32) of 30-second int16 PCM clips
+    ``waveform`` [B, 480000] (shorter clips zero-padded by the caller, as the feature extractor pads them), through
+    ``mel_filters`` [201, 80] (``whisper_mel_filters()``).  Written into ``out`` when given.  Anything else raises
+    ``ValueError``.  On CUDA the native kernels compute it in fp32 in a fixed order without host synchronisation (CUDA-graph
+    safe, bitwise repeatable); on CPU ``log_mel_spectrogram_reference`` in fp32."""
+    if waveform.dtype != torch.int16 or waveform.dim() != 2 or waveform.shape[0] < 1 or waveform.shape[1] != WHISPER_SAMPLES \
+            or not waveform.is_contiguous():
+        raise ValueError(f"log_mel_spectrogram needs contiguous int16 waveforms [B, {WHISPER_SAMPLES}] with B >= 1, got "
+                         f"{waveform.dtype} {tuple(waveform.shape)}{'' if waveform.is_contiguous() else ' strided'}")
+    if tuple(mel_filters.shape) != (WHISPER_N_FFT // 2 + 1, 80) or not mel_filters.is_floating_point():
+        raise ValueError(f"log_mel_spectrogram needs floating mel_filters [201, 80], got {mel_filters.dtype} {tuple(mel_filters.shape)}")
+    if out_dtype not in (torch.bfloat16, torch.float32):
+        raise ValueError(f"log_mel_spectrogram writes bf16 or fp32, got {out_dtype}")
+    B = waveform.shape[0]
+    if out is not None and (out.dtype != out_dtype or tuple(out.shape) != (B, 80, 3000) or not out.is_contiguous()
+                            or out.device != waveform.device):
+        raise ValueError(f"log_mel_spectrogram needs out to be a contiguous {out_dtype} [{B}, 80, 3000] on {waveform.device}, got "
+                         f"{out.dtype} {tuple(out.shape)} on {out.device}")
+    if waveform.is_cuda:
+        filters = mel_filters.to(device=waveform.device, dtype=torch.float32).contiguous()
+        return _C().whisper.log_mel(waveform, filters, out_dtype == torch.bfloat16, out)
+    y = log_mel_spectrogram_reference(waveform, mel_filters, torch.float32).to(out_dtype)
+    return out.copy_(y) if out is not None else y
+
+
+def encoder_rows(frames: int) -> int:
+    """Rows per clip of Whisper's encoder for ``frames`` mel frames: the stride-2 convolution's frames / 2 outputs, rounded
+    up to a multiple of 128 so the attention kernels take them (1536 for 3000 frames: 1500 real rows and 36 padding rows)."""
+    n = frames // 2
+    return (n + ATTENTION_SEQ_MULTIPLE - 1) // ATTENTION_SEQ_MULTIPLE * ATTENTION_SEQ_MULTIPLE
+
+
+def mel_patches_reference(features: torch.Tensor) -> torch.Tensor:
+    """P1 [B F, 3 C] of features [B, C, F]: P1[b F + t, j C + c] = features[b, c, t + j - 1], zero outside [0, F)."""
+    B, C, T = features.shape
+    p = F.pad(features, (1, 1))
+    return torch.stack([p[..., j:j + T] for j in range(3)], 1).permute(0, 3, 1, 2).reshape(B * T, 3 * C)
+
+
+def mel_patches(features: torch.Tensor) -> torch.Tensor:
+    """The im2col rows of Whisper's first convolution (width 3, padding 1) over mel features [B, 80, F]: [B F, 240] with
+    column j 80 + c holding channel c at frame t + j - 1 (``mel_patches_reference``), so that
+    ``linear(P1, conv1.weight.permute(0, 2, 1).reshape(d, 240))`` is the convolution.  Forward only: the features take no
+    gradient.  On CUDA: bf16 features, else ``ValueError``; a native gather."""
+    if features.dim() != 3 or features.shape[1] != 80:
+        raise ValueError(f"mel_patches needs features [B, 80, F], got {tuple(features.shape)}")
+    if features.is_cuda:
+        if features.dtype != torch.bfloat16:
+            raise ValueError(f"mel_patches on CUDA needs bf16 features, got {features.dtype}")
+        return _C().whisper.mel_patches(features.contiguous())
+    return mel_patches_reference(features)
+
+
+def frame_patches_reference(h1: torch.Tensor, frames: int, rows: int) -> torch.Tensor:
+    """P2 [B rows, 3 d] of h1 [B frames, d]: row (b, l) for l < frames / 2 holds h1[b, 2l - 1] | h1[b, 2l] | h1[b, 2l + 1]
+    (h1[b, -1] = 0), rows l >= frames / 2 are zero.  Differentiable."""
+    d = h1.shape[1]
+    B, L = h1.shape[0] // frames, frames // 2
+    hp = F.pad(h1.view(B, frames, d), (0, 0, 1, 1))
+    idx = 2 * torch.arange(L, device=h1.device)
+    p = torch.cat([hp[:, idx + j] for j in range(3)], -1)
+    return F.pad(p, (0, 0, 0, rows - L)).reshape(B * rows, 3 * d)
+
+
+class _FramePatches(torch.autograd.Function):
+    """The stride-2 gather forward; its backward is a col2im gather (each dh1 row sums its at most two taps in order)."""
+
+    @staticmethod
+    def forward(ctx, h1, frames, rows):
+        ctx.geometry = (frames, rows)
+        return _C().whisper.frame_patches(h1, frames, rows)
+
+    @staticmethod
+    def backward(ctx, dp2):
+        frames, rows = ctx.geometry
+        return _C().whisper.frame_patches_bwd(dp2.contiguous(), frames, rows), None, None
+
+
+def frame_patches(h1: torch.Tensor, frames: int, rows: int) -> torch.Tensor:
+    """The im2col rows of Whisper's second convolution (width 3, stride 2, padding 1) over h1 [B frames, d]: [B rows, 3 d]
+    (``frame_patches_reference``), rows >= frames / 2 zero, so that ``linear(P2, conv2.weight.permute(0, 2, 1).reshape(d,
+    3 d))`` gives the encoder's rows.  frames even, rows >= frames / 2.  On CUDA: bf16 h1 with d % 8 == 0, else
+    ``ValueError``; native gathers both ways, the backward summing each h1 row's taps in fp32 with one bf16 rounding."""
+    if h1.dim() != 2 or frames < 2 or frames % 2 or h1.shape[0] % frames or rows < frames // 2:
+        raise ValueError(f"frame_patches needs h1 [B frames, d] with even frames >= 2 and rows >= frames / 2, got "
+                         f"{tuple(h1.shape)}, frames {frames}, rows {rows}")
+    if h1.is_cuda:
+        if h1.dtype != torch.bfloat16 or h1.shape[1] % 8:
+            raise ValueError(f"frame_patches on CUDA needs bf16 h1 with d % 8 == 0, got {h1.dtype} {tuple(h1.shape)}")
+        return _FramePatches.apply(h1.contiguous(), frames, rows)
+    return frame_patches_reference(h1, frames, rows)
