@@ -25,7 +25,7 @@ EXT_NAME = "_C"
 CUDA_SOURCES = ["allreduce.cu", "broadcast.cu", "optim.cu", "loss.cu", "layernorm.cu", "linear_small.cu", "input.cu",
                 "gemm_wgmma.cu", "batchnorm.cu", "pool.cu", "conv_wgmma.cu", "conv_wgrad_wgmma.cu", "conv_stem.cu", "fp8.cu",
                 "attention.cu", "rotary.cu", "moe.cu", "vit.cu", "clip.cu", "cross_attention.cu",
-                "convnext.cu", "swin.cu", "mamba.cu", "mamba2.cu", "whisper.cu"]
+                "convnext.cu", "swin.cu", "mamba.cu", "mamba2.cu", "whisper.cu", "mae.cu"]
 CPP_SOURCES = ["peer_mem.cpp", "reducer.cpp", "tensor_map.cpp", "bindings.cpp"]
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -170,8 +170,8 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin, _C.mamba, _C.mamba2 and _C.whisper namespaces of static
-// entry points
+// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin, _C.mamba, _C.mamba2, _C.whisper and _C.mae namespaces of
+// static entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
 struct T5Namespace {};
@@ -180,6 +180,7 @@ struct SwinNamespace {};
 struct MambaNamespace {};
 struct Mamba2Namespace {};
 struct WhisperNamespace {};
+struct MaeNamespace {};
 
 // An NHWC activation of the depthwise convolution: bf16 [B, H, W, C] contiguous and 16-byte aligned, B, H, W >= 1,
 // 8 <= C <= 1024 with C % 8 == 0 (B is the grid's z extent).  Returns (B, H, W, C).
@@ -208,6 +209,56 @@ std::array<int64_t, 2> swin_args(Args& args, const at::Tensor& qkv, const at::Te
   if (rows * 96 * heads >= (1ll << 31)) args.fail("geometry", "at most 2^31 qkv elements", geometry());
   args("qkv", qkv, {kBF16}, {rows, 96 * heads}, kContiguous, 16);
   return {rows, heads};
+}
+
+// An image batch of the masked autoencoder: bf16 [B, C, H, W], contiguous or channels_last and 16-byte aligned, with
+// 1 <= B <= 65535 and p a multiple of 8 that divides H and W.  Returns (B, C, H, W, N = (H / p)(W / p), channels_last).
+struct MaeImages { int64_t B, C, H, W, N; bool cl; };
+MaeImages mae_images(Args& args, const at::Tensor& images, int64_t patch) {
+  args("images", images, {kBF16}, {kAny, kAny, kAny, kAny}, kStrided, 16);
+  const bool cl = !images.is_contiguous();
+  args.expect(!cl || images.is_contiguous(at::MemoryFormat::ChannelsLast), "images", "contiguous or channels_last", images);
+  const int64_t B = images.size(0), C = images.size(1), H = images.size(2), W = images.size(3);
+  if (B < 1 || B > 65535 || C < 1) args.fail("images", "bf16 [B, C, H, W] with 1 <= B <= 65535 and C >= 1", describe(images));
+  if (patch < 8 || patch % 8 || H % patch || W % patch)
+    args.fail("patch", "a multiple of 8 that divides the image's height and width", std::to_string(patch) + " for " + sizes_str(images.sizes()));
+  if (images.numel() >= (1ll << 31)) args.fail("images", "fewer than 2^31 elements", describe(images));
+  return {B, C, H, W, (H / patch) * (W / patch), cl};
+}
+
+// ids_restore int32 [B, N] (1 <= N <= 1024) and 0 <= keep <= N
+void mae_ids(Args& args, const char* name, const at::Tensor& ids, int64_t B, int64_t N, int64_t keep) {
+  args(name, ids, {kI32}, {B, N});
+  if (N < 1 || N > 1024) args.fail(name, "int32 [B, N] with 1 <= N <= 1024", describe(ids));
+  if (keep < 0 || keep > N) args.fail("keep", "in [0, N] = [0, " + std::to_string(N) + "]", std::to_string(keep));
+}
+
+// The per-image attention's qkv bf16 [T, 96 heads] (head dim 32), contiguous and 16-byte aligned with 1 <= heads <= 65535 and
+// fewer than 2^31 elements, and images of `tokens` rows: batch >= 1, 1 <= tokens <= 256, batch * tokens <= T.  Returns (T, heads).
+std::array<int64_t, 2> mae_attention_args(Args& args, const at::Tensor& qkv, int64_t batch, int64_t tokens) {
+  args("qkv", qkv, {kBF16}, {kAny, kAny}, kContiguous, 16);
+  const int64_t T = qkv.size(0), heads = qkv.size(1) / 96;
+  if (qkv.size(1) % 96 || heads < 1 || heads > 65535 || T * qkv.size(1) >= (1ll << 31))
+    args.fail("qkv", "bf16 [T, 96 heads] (head dim 32) with 1 <= heads <= 65535 and fewer than 2^31 elements", describe(qkv));
+  if (batch < 1 || tokens < 1 || tokens > 256 || batch * tokens > T)
+    args.fail("geometry", "batch >= 1, 1 <= tokens <= 256 and batch * tokens <= T = " + std::to_string(T),
+              std::to_string(batch) + " x " + std::to_string(tokens));
+  return {T, heads};
+}
+
+// The reconstruction loss's pred bf16 [Td, C p^2] (C p^2 <= 768, p from its width and the images' C), its images (as
+// mae_images), ids_restore int32 [B, N], 0 <= keep < N and Td >= B (N + 1).  Returns the images' geometry and p.
+std::pair<MaeImages, int64_t> mae_loss_args(Args& args, const at::Tensor& pred, const at::Tensor& images, const at::Tensor& ids_restore,
+                                            int64_t keep) {
+  args("pred", pred, {kBF16}, {kAny, kAny}, kContiguous, 16);
+  const int64_t C = images.dim() == 4 ? images.size(1) : 1, P = pred.size(1);
+  const int64_t patch = C > 0 && P % C == 0 ? (int64_t)std::lround(std::sqrt((double)(P / C))) : 0;
+  if (P > 768 || patch * patch * C != P) args.fail("pred", "bf16 [T, C p^2] with C p^2 <= 768", describe(pred));
+  const MaeImages im = mae_images(args, images, patch);
+  mae_ids(args, "ids_restore", ids_restore, im.B, im.N, keep);
+  if (keep >= im.N) args.fail("keep", "below N = " + std::to_string(im.N), std::to_string(keep));
+  if (pred.size(0) < im.B * (im.N + 1)) args.fail("pred", "at least B (N + 1) = " + std::to_string(im.B * (im.N + 1)) + " rows", describe(pred));
+  return {im, patch};
 }
 
 // Mamba's token rows: bounds int32 [B, S, 2] contiguous and 8-byte aligned (the kernels read int2) with 1 <= B <= 65535, then
@@ -2162,4 +2213,158 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     launch_frame_patches_bwd(dp2.data_ptr(), (int)B, (int)frames, (int)rows, (int)d, dh1.data_ptr(), cur_stream());
     return dh1;
   }, py::arg("dp2"), py::arg("frames"), py::arg("rows"));
+
+  // ---- Masked-autoencoder pretraining (mae.cu): shuffle, masked patch embedding, unshuffle, attention, loss ---------------
+  // _C.mae is a namespace of static entry points like _C.whisper; its contract rows are in tests/test_vit_mae_bindings_cpu.py.
+  py::class_<MaeNamespace> mae(m, "mae", "Masked-autoencoder shuffle, patch embedding, unshuffle, attention and loss (mae.cu)");
+  // (ids_keep int32 [B, keep], ids_restore int32 [B, N]) of noise fp32 [B, N]
+  mae.def_static("shuffle", [](at::Tensor noise, int64_t keep) {
+    Args args("shuffle");
+    args("noise", noise, {kF32}, {kAny, kAny});
+    const int64_t B = noise.size(0), N = noise.size(1);
+    if (B < 1 || N < 1 || N > 1024) args.fail("noise", "fp32 [B, N] with B >= 1 and 1 <= N <= 1024", describe(noise));
+    if (keep < 0 || keep > N) args.fail("keep", "in [0, N] = [0, " + std::to_string(N) + "]", std::to_string(keep));
+    args.device();
+    at::Tensor ids_keep = at::empty({B, keep}, noise.options().dtype(kI32));
+    at::Tensor ids_restore = at::empty({B, N}, noise.options().dtype(kI32));
+    launch_mae_shuffle(noise.data_ptr<float>(), (int)B, (int)N, (int)keep, ids_keep.data_ptr<int>(), ids_restore.data_ptr<int>(), cur_stream());
+    return std::make_tuple(ids_keep, ids_restore);
+  }, py::arg("noise"), py::arg("keep"));
+  // the kept patches' rows bf16 [tokens, C p p] of images bf16 [B, C, H, W] (NCHW or channels_last); ids_keep int32 [B, keep]
+  mae.def_static("patchify", [](at::Tensor images, at::Tensor ids_keep, int64_t patch, int64_t tokens) {
+    Args args("patchify");
+    const MaeImages im = mae_images(args, images, patch);
+    args("ids_keep", ids_keep, {kI32}, {im.B, kAny});
+    const int64_t keep = ids_keep.size(1);
+    if (keep > im.N) args.fail("ids_keep", "int32 [B, keep] with keep <= patches = " + std::to_string(im.N), describe(ids_keep));
+    if (tokens < im.B * (keep + 1) || tokens * im.C * patch * patch >= (1ll << 31))
+      args.fail("tokens", "at least batch * (keep + 1) = " + std::to_string(im.B * (keep + 1)) + " and below 2^31 patch elements",
+                std::to_string(tokens));
+    args.device();
+    at::Tensor out = at::empty({tokens, im.C * patch * patch}, images.options().memory_format(at::MemoryFormat::Contiguous));
+    launch_mae_patchify(images.data_ptr(), im.cl, ids_keep.data_ptr<int>(), (int)im.B, (int)im.C, (int)im.H, (int)im.W, (int)patch, (int)keep,
+                        (int)tokens, out.data_ptr(), cur_stream());
+    return out;
+  }, py::arg("images"), py::arg("ids_keep"), py::arg("patch"), py::arg("tokens"));
+  // encoder tokens bf16 [T, D] of the GEMM output y [T, D], class_token [D], pos_embedding [N + 1, D], ids_keep int32 [B, keep]
+  mae.def_static("patch_assemble", [](at::Tensor y, at::Tensor class_token, at::Tensor pos_embedding, at::Tensor ids_keep) {
+    Args args("patch_assemble");
+    args("y", y, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t T = y.size(0), D = y.size(1);
+    if (D % 8 || D < 8) args.fail("y", "bf16 [T, D] with D % 8 == 0", describe(y));
+    args("class_token", class_token, {kBF16}, numel(D), kContiguous, 16)("pos_embedding", pos_embedding, {kBF16}, last_dim(D), kContiguous, 16);
+    args("ids_keep", ids_keep, {kI32}, {kAny, kAny});
+    const int64_t B = ids_keep.size(0), keep = ids_keep.size(1), N = pos_embedding.numel() / D - 1;
+    if (B < 1 || keep > N || B * (keep + 1) > T)
+      args.fail("ids_keep", "int32 [B, keep] with B >= 1, keep <= patches = " + std::to_string(N) + " and B (keep + 1) <= T = " +
+                std::to_string(T), describe(ids_keep));
+    args.device();
+    at::Tensor out = at::empty_like(y);
+    launch_mae_patch_assemble(y.data_ptr(), class_token.data_ptr(), pos_embedding.data_ptr(), ids_keep.data_ptr<int>(), (int)B, (int)keep,
+                              (int)D, (int)T, out.data_ptr(), cur_stream());
+    return out;
+  }, py::arg("y"), py::arg("class_token"), py::arg("pos_embedding"), py::arg("ids_keep"));
+  // (dpatch bf16 [T, D], dcls bf16 [D]) of dy bf16 [T, D]
+  mae.def_static("patch_embed_bwd", [](at::Tensor dy, int64_t batch, int64_t tokens_per_image) {
+    Args args("patch_embed_bwd");
+    args("dy", dy, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t T = dy.size(0), D = dy.size(1);
+    if (D % 8 || D < 8) args.fail("dy", "bf16 [T, D] with D % 8 == 0", describe(dy));
+    if (tokens_per_image < 1 || batch < 1 || batch * tokens_per_image > T)
+      args.fail("batch", "batch >= 1 and batch * tokens_per_image <= T = " + std::to_string(T), std::to_string(batch) + " * " +
+                std::to_string(tokens_per_image));
+    args.device();
+    at::Tensor dpatch = at::empty_like(dy);
+    at::Tensor dcls = at::empty({D}, dy.options());
+    launch_mae_patch_embed_bwd(dy.data_ptr(), (int)batch, (int)tokens_per_image, (int)D, (int)T, dpatch.data_ptr(), dcls.data_ptr(), cur_stream());
+    return std::make_tuple(dpatch, dcls);
+  }, py::arg("dy"), py::arg("batch"), py::arg("tokens_per_image"));
+  // the decoder stream bf16 [rows, E] of y bf16 [Te, E], mask_token [E], pos_embedding [N + 1, E], ids_restore int32 [B, N]
+  mae.def_static("unshuffle", [](at::Tensor y, at::Tensor mask_token, at::Tensor pos_embedding, at::Tensor ids_restore, int64_t keep,
+                                 int64_t rows) {
+    Args args("unshuffle");
+    args("y", y, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t Te = y.size(0), E = y.size(1);
+    if (E % 8 || E < 8 || E > 2048) args.fail("y", "bf16 [T, E] with E % 8 == 0 and E <= 2048", describe(y));
+    args("mask_token", mask_token, {kBF16}, numel(E), kContiguous, 16);
+    args("ids_restore", ids_restore, {kI32}, {kAny, kAny});
+    const int64_t B = ids_restore.size(0), N = ids_restore.size(1);
+    mae_ids(args, "ids_restore", ids_restore, B, N, keep);
+    if (B < 1) args.fail("ids_restore", "int32 [B, N] with B >= 1", describe(ids_restore));
+    args("pos_embedding", pos_embedding, {kBF16}, numel((N + 1) * E), kContiguous, 16);
+    if (B * (keep + 1) > Te) args.fail("y", "at least B (keep + 1) = " + std::to_string(B * (keep + 1)) + " rows", describe(y));
+    if (rows < B * (N + 1) || rows * E >= (1ll << 31))
+      args.fail("rows", "at least B (N + 1) = " + std::to_string(B * (N + 1)) + " and below 2^31 elements", std::to_string(rows));
+    args.device();
+    at::Tensor z = at::empty({rows, E}, y.options());
+    launch_mae_unshuffle(y.data_ptr(), mask_token.data_ptr(), pos_embedding.data_ptr(), ids_restore.data_ptr<int>(), (int)B, (int)N, (int)keep,
+                         (int)E, (int)rows, z.data_ptr(), cur_stream());
+    return z;
+  }, py::arg("y"), py::arg("mask_token"), py::arg("pos_embedding"), py::arg("ids_restore"), py::arg("keep"), py::arg("rows"));
+  // (dy bf16 [rows, E], dmask bf16 [E]) of dz bf16 [Td, E], ids_keep int32 [B, keep], ids_restore int32 [B, N]
+  mae.def_static("unshuffle_bwd", [](at::Tensor dz, at::Tensor ids_keep, at::Tensor ids_restore, int64_t rows) {
+    Args args("unshuffle_bwd");
+    args("dz", dz, {kBF16}, {kAny, kAny}, kContiguous, 16);
+    const int64_t Td = dz.size(0), E = dz.size(1);
+    if (E % 8 || E < 8 || E > 2048) args.fail("dz", "bf16 [T, E] with E % 8 == 0 and E <= 2048", describe(dz));
+    args("ids_keep", ids_keep, {kI32}, {kAny, kAny});
+    const int64_t B = ids_keep.size(0), keep = ids_keep.size(1);
+    if (B < 1) args.fail("ids_keep", "int32 [B, keep] with B >= 1", describe(ids_keep));
+    args("ids_restore", ids_restore, {kI32}, {B, kAny});
+    const int64_t N = ids_restore.size(1);
+    mae_ids(args, "ids_restore", ids_restore, B, N, keep);
+    if (B * (N + 1) > Td) args.fail("dz", "at least B (N + 1) = " + std::to_string(B * (N + 1)) + " rows", describe(dz));
+    if (rows < B * (keep + 1) || rows * E >= (1ll << 31))
+      args.fail("rows", "at least B (keep + 1) = " + std::to_string(B * (keep + 1)) + " and below 2^31 elements", std::to_string(rows));
+    args.device();
+    at::Tensor dy = at::empty({rows, E}, dz.options());
+    at::Tensor part = at::empty({(int64_t)mae_mask_partials((int)B), E}, dz.options().dtype(kF32));
+    at::Tensor dmask = at::empty({E}, dz.options());
+    launch_mae_unshuffle_bwd(dz.data_ptr(), ids_keep.data_ptr<int>(), ids_restore.data_ptr<int>(), (int)B, (int)N, (int)keep, (int)E, (int)rows,
+                             dy.data_ptr(), part.data_ptr<float>(), dmask.data_ptr(), cur_stream());
+    return std::make_tuple(dy, dmask);
+  }, py::arg("dz"), py::arg("ids_keep"), py::arg("ids_restore"), py::arg("rows"));
+  // (o bf16 [T, C], lse fp32 [T, heads]) of qkv bf16 [T, 3C], C = 32 heads, images of `tokens` rows (1 <= tokens <= 256)
+  mae.def_static("attention_fwd", [](at::Tensor qkv, int64_t batch, int64_t tokens) {
+    Args args("attention_fwd");
+    const auto [T, heads] = mae_attention_args(args, qkv, batch, tokens);
+    args.device();
+    at::Tensor o = at::empty({T, 32 * heads}, qkv.options());
+    at::Tensor lse = at::empty({T, heads}, qkv.options().dtype(kF32));
+    launch_image_attention_fwd(qkv.data_ptr(), (int)batch, (int)tokens, (int)heads, (int)T, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
+    return std::make_tuple(o, lse);
+  }, py::arg("qkv"), py::arg("batch"), py::arg("tokens"));
+  // dqkv bf16 [T, 3C]
+  mae.def_static("attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, int64_t batch, int64_t tokens) {
+    Args args("attention_bwd");
+    const auto [T, heads] = mae_attention_args(args, qkv, batch, tokens);
+    args("dout", dout, {kBF16}, {T, 32 * heads}, kContiguous, 16)("o", o, {kBF16}, {T, 32 * heads}, kContiguous, 16)("lse", lse, {kF32}, {T, heads});
+    args.device();
+    at::Tensor dqkv = at::empty_like(qkv);
+    launch_image_attention_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), (int)batch, (int)tokens, (int)heads, (int)T,
+                               dqkv.data_ptr(), cur_stream());
+    return dqkv;
+  }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("batch"), py::arg("tokens"));
+  // loss fp32 [] of pred bf16 [Td, C p p] (p from its width), images bf16 [B, C, H, W], ids_restore int32 [B, N], 0 <= keep < N
+  mae.def_static("loss", [](at::Tensor pred, at::Tensor images, at::Tensor ids_restore, int64_t keep, bool norm_pix) {
+    Args args("loss");
+    const auto [im, patch] = mae_loss_args(args, pred, images, ids_restore, keep);
+    args.device();
+    at::Tensor rowloss = at::empty({im.B * im.N}, pred.options().dtype(kF32));
+    at::Tensor loss = at::empty({}, pred.options().dtype(kF32));
+    launch_mae_loss_fwd(pred.data_ptr(), images.data_ptr(), im.cl, ids_restore.data_ptr<int>(), (int)im.B, (int)im.C, (int)im.H, (int)im.W,
+                        (int)patch, (int)keep, norm_pix, rowloss.data_ptr<float>(), loss.data_ptr<float>(), cur_stream());
+    return loss;
+  }, py::arg("pred"), py::arg("images"), py::arg("ids_restore"), py::arg("keep"), py::arg("norm_pix"));
+  // dpred bf16 [Td, C p p] of dloss fp32 (one element, read on the device)
+  mae.def_static("loss_bwd", [](at::Tensor dloss, at::Tensor pred, at::Tensor images, at::Tensor ids_restore, int64_t keep, bool norm_pix) {
+    Args args("loss_bwd");
+    args("dloss", dloss, {kF32}, numel(1));
+    const auto [im, patch] = mae_loss_args(args, pred, images, ids_restore, keep);
+    args.device();
+    at::Tensor dpred = at::empty_like(pred);
+    launch_mae_loss_bwd(dloss.data_ptr<float>(), pred.data_ptr(), images.data_ptr(), im.cl, ids_restore.data_ptr<int>(), (int)im.B, (int)im.C,
+                        (int)im.H, (int)im.W, (int)patch, (int)keep, norm_pix, (int)pred.size(0), dpred.data_ptr(), cur_stream());
+    return dpred;
+  }, py::arg("dloss"), py::arg("pred"), py::arg("images"), py::arg("ids_restore"), py::arg("keep"), py::arg("norm_pix"));
 }

@@ -345,6 +345,39 @@ void launch_mel_patches(const void* features, int B, int F, void* p1, cudaStream
 void launch_frame_patches(const void* h1, int B, int F, int S, int d, void* p2, cudaStream_t s);
 void launch_frame_patches_bwd(const void* dp2, int B, int F, int S, int d, void* dh1, cudaStream_t s);
 
+// ---------------- Masked-autoencoder pretraining (mae.cu): shuffle, masked patch embedding, unshuffle, loss, attention --
+// noise fp32 [B, N] -> ids_keep int32 [B, keep], ids_restore int32 [B, N]: the stable ascending rank of each patch (N <= 1024)
+void launch_mae_shuffle(const float* noise, int B, int N, int keep, int* ids_keep, int* ids_restore, cudaStream_t s);
+// image bf16 (NCHW or channels_last) -> patch matrix [T, C p p] of the kept patches in (c, ky, kx) order, image b's kept
+// patch j at row b (keep + 1) + 1 + j; class and padding rows zero
+void launch_mae_patchify(const void* img, bool channels_last, const int* ids_keep, int B, int C, int H, int W, int p, int keep, int T,
+                         void* out, cudaStream_t s);
+// GEMM output y [T, D] -> tokens: cls + pos[0] at class rows, y + pos[1 + ids_keep] at patch rows, zero padding rows
+void launch_mae_patch_assemble(const void* y, const void* cls, const void* pos, const int* ids_keep, int B, int keep, int D, int T, void* out,
+                               cudaStream_t s);
+// dy [T, D] -> dpatch [T, D] (dy at patch rows, zero elsewhere) and dcls [D] (fixed-order sum over the class rows)
+void launch_mae_patch_embed_bwd(const void* dy, int B, int per, int D, int T, void* dpatch, void* dcls, cudaStream_t s);
+// y [Te, E] -> z [Td, E]: row b (N + 1) the class row of image b, row b (N + 1) + 1 + i its kept patch ids_restore[b, i] or
+// mask_token, plus pos[row in image]; padding rows zero
+void launch_mae_unshuffle(const void* y, const void* mask_token, const void* pos, const int* ids_restore, int B, int N, int keep, int E,
+                          int Td, void* z, cudaStream_t s);
+// dz [Td, E] -> dy [Te, E] (a gather through ids_keep) and dmask [E] through part fp32 [mae_mask_partials(B), E]
+int mae_mask_partials(int B);
+void launch_mae_unshuffle_bwd(const void* dz, const int* ids_keep, const int* ids_restore, int B, int N, int keep, int E, int Te, void* dy,
+                              float* part, void* dmask, cudaStream_t s);
+// Per-image attention at head dim 32: qkv bf16 [T, 3C] (C = 32 heads), image b's rows [b tokens, (b + 1) tokens), tokens <= 256,
+// rows past B tokens padding (zero o, lse and dqkv).  o bf16 [T, C], lse fp32 [T, heads].
+void launch_image_attention_fwd(const void* qkv, int B, int tokens, int heads, int T, void* o, float* lse, cudaStream_t s);
+void launch_image_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, int B, int tokens, int heads, int T,
+                                void* dqkv, cudaStream_t s);
+// Reconstruction loss on the masked patches: pred bf16 [Td, C p p] (rows as the unshuffled stream), the target read from the
+// bf16 image in (ky, kx, c) order, optionally per-patch normalised.  rowloss fp32 [B N] is scratch; loss fp32 [1].  The
+// backward writes dpred bf16 [Td, C p p] = 2 (pred - target) / (C p p B (N - keep)) * dloss[0] on masked rows, zero elsewhere.
+void launch_mae_loss_fwd(const void* pred, const void* img, bool channels_last, const int* ids_restore, int B, int C, int H, int W, int p,
+                         int keep, bool norm_pix, float* rowloss, float* loss, cudaStream_t s);
+void launch_mae_loss_bwd(const float* dloss, const void* pred, const void* img, bool channels_last, const int* ids_restore, int B, int C,
+                         int H, int W, int p, int keep, bool norm_pix, int Td, void* dpred, cudaStream_t s);
+
 // ---------------- CLIP contrastive loss (clip.cu)---------------------------------------------------
 // u bf16 [B, D] = x / ||x|| per row (fp32, one rounding), rnorm fp32 [B] = 1 / ||x||; D % 8 == 0, 16-byte aligned rows
 void launch_l2norm_fwd(const void* x, int B, int D, void* u, float* rnorm, cudaStream_t s);

@@ -23,6 +23,7 @@
 //           partials in window order.
 // No atomics, so two runs give bitwise-equal results; nothing is read back to the host.
 #include "ops.h"
+#include "warp_mma.cuh"
 
 namespace b200 {
 namespace {
@@ -35,28 +36,6 @@ constexpr float kScale = 0.17677669529663687f;   // 32^-0.5
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kMask = -100.f;
 constexpr int kFinishWarps = 32;
-
-__device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint32_t ld32(const __nv_bfloat16* p) { return *reinterpret_cast<const uint32_t*>(p); }
-
-__device__ __forceinline__ uint32_t pack2(float lo, float hi) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
-
-// d (+)= a b, m16n8k16, bf16 x bf16 -> fp32
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// four transposed 8x8 bf16 matrices; lanes 8 i .. 8 i + 7 address the rows of matrix i
-__device__ __forceinline__ void ldsm_x4_t(uint32_t (&r)[4], const __nv_bfloat16* p) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(smem_addr(p)));
-}
 
 // c[16 x 64] = A[m0 .. m0 + 16, 0 .. 32) B[0 .. 64, 0 .. 32)^T, both row-major bf16 in shared memory with pitch kPitch
 __device__ __forceinline__ void mma_abt(float (&c)[8][4], const __nv_bfloat16* A, const __nv_bfloat16* B, int m0, int g, int t) {

@@ -162,6 +162,7 @@ def setup(args):
     check_contrastive_args(args)
     check_seq2seq_args(args)
     check_speech_args(args)
+    check_own_loss_args(args)
     args.train_batch_size = args.per_gpu_train_batch_size * max(1, args.n_gpu)
     set_seed(args.seed, args.n_gpu)
     log.warning("Finish setup.", dict(device=args.device, n_gpu=args.n_gpu, distributed_training=bool(args.local_rank != -1)))
@@ -335,6 +336,21 @@ def check_speech_args(args) -> None:
         return
     if getattr(args, "pack", False):
         raise ValueError(f"--pack does not apply to --model {args.model}: each row holds one 30-second clip and its transcript")
+
+
+def check_own_loss_args(args) -> None:
+    """A model that returns its own loss (MAE pretraining) trains on images alone: ``--loss`` and ``--seq_len`` do not
+    apply, and single-process multi-GPU ``DataParallel`` would return one scalar loss per replica.  (``--fp8``, ``--pack``,
+    ``--min_seq_len``, ``--fused_lm_loss`` and ``--sparse_prediction`` are rejected for every image model already.)"""
+    if not model_entry(args.model).own_loss:
+        return
+    for flag, given in (("--loss", getattr(args, "loss", None) is not None), ("--seq_len", getattr(args, "seq_len_given", False))):
+        if given:
+            raise ValueError(f"{flag} does not apply to --model {args.model}: it trains on images with its own reconstruction loss")
+    if getattr(args, "device", None) is not None and args.device.type == "cuda" and args.local_rank == -1 \
+            and getattr(args, "n_gpu", 1) > 1:
+        raise ValueError(f"--model {args.model} does not run under single-process multi-GPU DataParallel (each replica would "
+                         f"return its own loss); launch one process per GPU (torchrun) or make one GPU visible")
 
 
 def padding_on(args) -> bool:

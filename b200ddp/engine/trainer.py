@@ -91,12 +91,23 @@ class RouterAuxLoss:
         return self.criterion(out, y) + self.coef * self._model[0].router_aux_loss()
 
 
+class OwnLoss:
+    """The criterion of a model whose forward returns its own loss (MAE pretraining): that loss, the labels ignored."""
+
+    def __call__(self, out, y):
+        return out
+
+
 def build_criterion(args, model: Optional[torch.nn.Module] = None):
     """``--loss``'s criterion; with ``--fused_lm_loss`` or ``--sparse_prediction`` the model's own head-plus-cross-entropy
-    (``lm_head_loss``); for a contrastive model (CLIP) its contrastive loss over the global batch (``ClipLoss``).  A model
-    with ``config.router_aux_loss_coef > 0`` (mixture of experts) adds its load-balancing loss (``RouterAuxLoss``)."""
-    if model_entry(getattr(args, "model", "foo")).contrastive:
+    (``lm_head_loss``); for a contrastive model (CLIP) its contrastive loss over the global batch (``ClipLoss``); for a model
+    that returns its own loss (MAE) that loss (``OwnLoss``).  A model with ``config.router_aux_loss_coef > 0`` (mixture of
+    experts) adds its load-balancing loss (``RouterAuxLoss``)."""
+    entry = model_entry(getattr(args, "model", "foo"))
+    if entry.contrastive:
         criterion = ClipLoss()
+    elif entry.own_loss:
+        criterion = OwnLoss()
     elif getattr(args, "fused_lm_loss", False):
         if model is None or not getattr(getattr(model, "config", None), "fused_lm_loss", False):
             raise ValueError("--fused_lm_loss needs a causal LM built with fused_lm_loss=True (it has lm_head_loss)")

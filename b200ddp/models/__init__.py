@@ -20,6 +20,7 @@ from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneratio
 from .t5 import T5_BASE, T5_SMALL, T5Config, T5ForConditionalGeneration, t5_base, t5_small
 from .mamba import MAMBA_130M, MAMBA_370M, MambaConfig, MambaForCausalLM, mamba_130m, mamba_370m
 from .mamba2 import MAMBA2_130M, MAMBA2_370M, Mamba2Config, Mamba2ForCausalLM, mamba2_130m, mamba2_370m
+from .vit_mae import VIT_MAE_BASE, VIT_MAE_LARGE, ViTMAEConfig, ViTMAEForPreTraining, vit_mae_base, vit_mae_large
 from .whisper import (WHISPER_BASE, WHISPER_SMALL, WHISPER_TINY, WhisperConfig, WhisperForConditionalGeneration, whisper_base, whisper_small,
                       whisper_tiny)
 
@@ -40,6 +41,8 @@ class ModelEntry:
                                        # kind "causal" (the decoder is a causal LM over the target)
     speech: bool = False               # an encoder-decoder trained on waveform / transcript pairs (Whisper): forward(features,
                                        # labels) on the log-mel features of int16 clips
+    own_loss: bool = False             # image models whose forward returns their own loss (MAE pretraining): forward(images),
+                                       # the criterion passes it through and the labels are ignored
 
     @property
     def token_model(self) -> bool:
@@ -59,6 +62,8 @@ MODEL_REGISTRY = {
     "swin-t": ModelEntry(swin_t, "image"),
     "swin-s": ModelEntry(swin_s, "image"),
     "swin-b": ModelEntry(swin_b, "image"),
+    "vit-mae-base": ModelEntry(vit_mae_base, "image", own_loss=True),
+    "vit-mae-large": ModelEntry(vit_mae_large, "image", own_loss=True),
     "clip-vit-b-32": ModelEntry(clip_vit_b_32, "image", contrastive=True),
     "clip-vit-b-16": ModelEntry(clip_vit_b_16, "image", contrastive=True),
     "bert-base": ModelEntry(bert_base, "encoder", BERT_BASE, start_id=101, fp8=True),                 # [CLS]
@@ -103,4 +108,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "Mamba2Config", "Mamba2ForCausalLM", "mamba2_130m", "mamba2_370m", "WhisperConfig", "WhisperForConditionalGeneration", "whisper_tiny", "whisper_base", "whisper_small", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ViTMAEConfig", "ViTMAEForPreTraining", "vit_mae_base", "vit_mae_large", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "Mamba2Config", "Mamba2ForCausalLM", "mamba2_130m", "mamba2_370m", "WhisperConfig", "WhisperForConditionalGeneration", "whisper_tiny", "whisper_base", "whisper_small", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

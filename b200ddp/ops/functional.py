@@ -2715,3 +2715,234 @@ def frame_patches(h1: torch.Tensor, frames: int, rows: int) -> torch.Tensor:
             raise ValueError(f"frame_patches on CUDA needs bf16 h1 with d % 8 == 0, got {h1.dtype} {tuple(h1.shape)}")
         return _FramePatches.apply(h1.contiguous(), frames, rows)
     return frame_patches_reference(h1, frames, rows)
+
+
+# ------------------------------------------------------------------------------------------------
+# Masked-autoencoder pretraining (csrc/mae.cu): per-image shuffling, the masked patch embedding, the decoder's unshuffle,
+# per-image attention at head dim 32 and the pixel reconstruction loss, on ``patch_embed``'s token streams
+# ------------------------------------------------------------------------------------------------
+MAE_HEAD_DIM = 32
+MAE_MAX_TOKENS = 256
+MAE_NORM_PIX_EPS = 1e-6
+
+
+def mae_shuffle_reference(noise: torch.Tensor, keep: int):
+    """transformers' ``random_masking`` indices with a stable sort: (ids_keep [B, keep], ids_restore [B, N]), int64.  Patch i
+    of image b has rank ids_restore[b, i] in its image's ascending noise (ties by index) and is kept iff that is below keep."""
+    ids_shuffle = torch.argsort(noise, dim=1, stable=True)
+    return ids_shuffle[:, :keep], torch.argsort(ids_shuffle, dim=1)
+
+
+def mae_shuffle(noise: torch.Tensor, keep: int):
+    """(ids_keep [B, keep], ids_restore [B, N]) of noise [B, N]: the patches ranked by ascending noise, ties in index order,
+    the first `keep` kept.  CUDA: one kernel, int32 results, no host synchronisation (N <= 1024); the ranks of noise without
+    NaNs equal a stable ``argsort``'s.  CPU: ``mae_shuffle_reference``."""
+    if not noise.is_cuda:
+        return mae_shuffle_reference(noise, keep)
+    return _C().mae.shuffle(noise.float().contiguous(), int(keep))
+
+
+def mae_patch_embed_reference(images: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], class_token: torch.Tensor,
+                              pos_embedding: torch.Tensor, ids_keep: torch.Tensor) -> torch.Tensor:
+    """transformers' ViTMAE embeddings (the patch convolution, + pos[1:], the kept patches gathered, the class token + pos[0]
+    in front) as ``mae_patch_embed``'s token stream [image_token_rows(B, keep + 1), D].  Differentiable."""
+    B, keep = ids_keep.shape
+    D, p = weight.shape[0], weight.shape[-1]
+    x = F.conv2d(images, weight, bias, stride=p).flatten(2).transpose(1, 2) + pos_embedding[:, 1:]
+    x = torch.gather(x, 1, ids_keep.long().unsqueeze(-1).expand(-1, -1, D))
+    x = torch.cat([(class_token + pos_embedding[:, :1]).expand(B, -1, -1), x], 1)
+    return F.pad(x.reshape(B * (keep + 1), D), (0, 0, 0, image_token_rows(B, keep + 1) - B * (keep + 1)))
+
+
+class _MaeAssemble(torch.autograd.Function):
+    """GEMM output [T, D] -> encoder tokens (csrc/mae.cu).  Backward: dy at patch rows for the weight-gradient GEMM and
+    d class_token as a fixed-order sum over the images; the frozen position table gets none."""
+
+    @staticmethod
+    def forward(ctx, y, class_token, pos_embedding, ids_keep):
+        ctx.batch, ctx.per, ctx.cls_shape = ids_keep.shape[0], ids_keep.shape[1] + 1, class_token.shape
+        return _C().mae.patch_assemble(y, class_token.contiguous(), pos_embedding.contiguous(), ids_keep)
+
+    @staticmethod
+    def backward(ctx, dy):
+        dpatch, dcls = _C().mae.patch_embed_bwd(_aligned16(dy), ctx.batch, ctx.per)
+        return dpatch, dcls.view(ctx.cls_shape), None, None
+
+
+def mae_patch_embed(images: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], class_token: torch.Tensor,
+                    pos_embedding: torch.Tensor, ids_keep: torch.Tensor) -> torch.Tensor:
+    """The masked autoencoder's encoder input as one token stream: images [B, C, H, W], the patch convolution's weight
+    [D, C, p, p] and bias [D], class_token [1, 1, D], a frozen pos_embedding [1, N + 1, D] and ids_keep [B, keep].  Returns
+    [T, D], T = ``image_token_rows(B, keep + 1)``: image b's class token + pos[0] at row b (keep + 1), then its kept patch
+    ids_keep[b, j] + pos[1 + ids_keep[b, j]] for j = 0 .. keep - 1, zero padding rows; ``image_token_bounds(B, keep + 1)``
+    are its attention bounds.
+
+    On CUDA (the requirements of ``patch_embed``, a pos_embedding that needs no gradient, else ``ValueError``): one kernel
+    writes the kept patches' rows of the patch matrix, the wgmma ``linear`` runs on all T rows and one kernel adds the class
+    token and positions (fp32, one rounding).  On CPU: ``mae_patch_embed_reference``."""
+    if not images.is_cuda:
+        return mae_patch_embed_reference(images, weight, bias, class_token, pos_embedding, ids_keep)
+    _patch_embed_check(images, weight, bias, class_token, pos_embedding)
+    if pos_embedding.requires_grad:
+        raise ValueError("mae_patch_embed treats pos_embedding as a frozen table; pass one with requires_grad=False")
+    B, keep = ids_keep.shape
+    D, p = weight.shape[0], weight.shape[-1]
+    ids_keep = ids_keep.to(torch.int32).contiguous()
+    patches = _C().mae.patchify(images, ids_keep, p, image_token_rows(B, keep + 1))
+    y = linear(patches, weight.reshape(D, -1), bias)
+    return _MaeAssemble.apply(y, class_token, pos_embedding, ids_keep)
+
+
+def mae_unshuffle_reference(y: torch.Tensor, mask_token: torch.Tensor, pos_embedding: torch.Tensor, ids_restore: torch.Tensor,
+                            keep: int) -> torch.Tensor:
+    """transformers' ViTMAE decoder input on token streams: the encoder stream y [Te, E] (B images of keep + 1 rows) ->
+    [image_token_rows(B, N + 1), E] by its ``cat``, ``gather``, ``cat`` and the position add.  Differentiable."""
+    B, N = ids_restore.shape
+    E = y.shape[1]
+    x = y[:B * (keep + 1)].view(B, keep + 1, E)
+    x_ = torch.cat([x[:, 1:], mask_token.view(1, 1, E).expand(B, N - keep, E)], 1)
+    x_ = torch.gather(x_, 1, ids_restore.long().unsqueeze(-1).expand(-1, -1, E))
+    z = torch.cat([x[:, :1], x_], 1) + pos_embedding.view(1, N + 1, E)
+    return F.pad(z.reshape(B * (N + 1), E), (0, 0, 0, image_token_rows(B, N + 1) - B * (N + 1)))
+
+
+class _MaeUnshuffle(torch.autograd.Function):
+    """Encoder stream -> decoder stream (csrc/mae.cu).  Backward: a gather of each encoder row's one decoder row, and
+    d mask_token as a fixed-order fp32 sum over the masked rows."""
+
+    @staticmethod
+    def forward(ctx, y, mask_token, pos_embedding, ids_keep, ids_restore):
+        ctx.save_for_backward(ids_keep, ids_restore)
+        ctx.rows, ctx.mask_shape = y.shape[0], mask_token.shape
+        B, N = ids_restore.shape
+        return _C().mae.unshuffle(y, mask_token.contiguous(), pos_embedding.contiguous(), ids_restore, ids_keep.shape[1],
+                                  image_token_rows(B, N + 1))
+
+    @staticmethod
+    def backward(ctx, dz):
+        ids_keep, ids_restore = ctx.saved_tensors
+        dy, dmask = _C().mae.unshuffle_bwd(_aligned16(dz), ids_keep, ids_restore, ctx.rows)
+        return dy, dmask.view(ctx.mask_shape), None, None, None
+
+
+def mae_unshuffle(y: torch.Tensor, mask_token: torch.Tensor, pos_embedding: torch.Tensor, ids_keep: torch.Tensor,
+                  ids_restore: torch.Tensor) -> torch.Tensor:
+    """The masked autoencoder's decoder input: the encoder stream y [Te, E] (B images of keep + 1 rows, keep =
+    ``ids_keep.shape[1]``), mask_token [1, 1, E], a frozen pos_embedding [1, N + 1, E], ids_keep [B, keep] and ids_restore
+    [B, N] from ``mae_shuffle``.  Returns [image_token_rows(B, N + 1), E]: row b (N + 1) is image b's class row, row
+    b (N + 1) + 1 + i its encoder row of rank ids_restore[b, i] if that is below keep, else mask_token, each plus its
+    position; zero padding rows.
+
+    CUDA (bf16): one kernel, fp32 add and one rounding; backward one gather kernel with per-CTA partials for d mask_token and
+    an in-order finish.  CPU: ``mae_unshuffle_reference``."""
+    if not y.is_cuda:
+        return mae_unshuffle_reference(y, mask_token, pos_embedding, ids_restore, ids_keep.shape[1])
+    if pos_embedding.requires_grad:
+        raise ValueError("mae_unshuffle treats pos_embedding as a frozen table; pass one with requires_grad=False")
+    if y.dtype != torch.bfloat16 or mask_token.dtype != torch.bfloat16 or pos_embedding.dtype != torch.bfloat16:
+        raise ValueError(f"mae_unshuffle on CUDA needs bf16 tensors, got {y.dtype}, {mask_token.dtype}, {pos_embedding.dtype}")
+    return _MaeUnshuffle.apply(_aligned16(y), mask_token, pos_embedding, ids_keep.to(torch.int32).contiguous(),
+                               ids_restore.to(torch.int32).contiguous())
+
+
+def image_attention_reference(qkv: torch.Tensor, batch: int, tokens: int, heads: int) -> torch.Tensor:
+    """``image_attention`` in torch (fp32 for bf16 input): dense softmax attention within each image's `tokens` rows, zero
+    padding rows.  Any head dim."""
+    T, W = qkv.shape
+    dtype = qkv.dtype if qkv.dtype in (torch.float32, torch.float64) else torch.float32
+    x = qkv[:batch * tokens].to(dtype).view(batch, tokens, 3, heads, W // (3 * heads)).permute(2, 0, 3, 1, 4)
+    q, k, v = x[0], x[1], x[2]
+    a = ((q * q.shape[-1] ** -0.5) @ k.transpose(-2, -1)).softmax(-1)
+    o = (a @ v).transpose(1, 2).reshape(batch * tokens, W // 3)
+    return F.pad(o, (0, 0, 0, T - batch * tokens)).to(qkv.dtype)
+
+
+class _ImageAttention(torch.autograd.Function):
+    """qkv [T, 3C] bf16 -> o [T, C] (csrc/mae.cu).  Backward: one kernel per (image, head)."""
+
+    @staticmethod
+    def forward(ctx, qkv, batch, tokens):
+        o, lse = _C().mae.attention_fwd(qkv, batch, tokens)
+        ctx.save_for_backward(qkv, o, lse)
+        ctx.geometry = (batch, tokens)
+        return o
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, o, lse = ctx.saved_tensors
+        return _C().mae.attention_bwd(_aligned16(dout), qkv, o, lse, *ctx.geometry), None, None
+
+
+def image_attention(qkv: torch.Tensor, batch: int, tokens: int, heads: int) -> torch.Tensor:
+    """Per-image self-attention on a token stream: qkv [T, 3C] (columns q heads | k heads | v heads), image b's rows
+    [b tokens, (b + 1) tokens), rows past batch tokens padding.  Returns [T, C]; padding rows are zero and get zero gradient.
+
+    CUDA bf16 input runs the native kernels (head dim 32, tokens <= 256, else ``ValueError``): fp32 online softmax and sums,
+    bitwise repeatable, no host synchronisation.  Everything else runs ``image_attention_reference``."""
+    if not (qkv.is_cuda and qkv.dtype == torch.bfloat16):
+        return image_attention_reference(qkv, batch, tokens, heads)
+    if qkv.dim() != 2 or qkv.shape[1] != 3 * MAE_HEAD_DIM * heads:
+        raise ValueError(f"image_attention on CUDA needs qkv [T, {3 * MAE_HEAD_DIM} heads] (head dim {MAE_HEAD_DIM}), got "
+                         f"{tuple(qkv.shape)} for {heads} heads")
+    if not (1 <= tokens <= MAE_MAX_TOKENS) or batch < 1 or batch * tokens > qkv.shape[0]:
+        raise ValueError(f"image_attention on CUDA needs 1 <= tokens <= {MAE_MAX_TOKENS} and batch * tokens <= T, got {batch} x "
+                         f"{tokens} for T = {qkv.shape[0]}")
+    return _ImageAttention.apply(_aligned16(qkv), batch, tokens)
+
+
+def mae_patchify(images: torch.Tensor, patch: int) -> torch.Tensor:
+    """transformers' ``ViTMAEForPreTraining.patchify``: [B, C, H, W] -> [B, N, p p C] in (ky, kx, c) order."""
+    B, C, H, W = images.shape
+    x = images.reshape(B, C, H // patch, patch, W // patch, patch)
+    return torch.einsum("nchpwq->nhwpqc", x).reshape(B, (H // patch) * (W // patch), patch * patch * C)
+
+
+def mae_loss_reference(pred: torch.Tensor, images: torch.Tensor, ids_restore: torch.Tensor, keep: int, norm_pix: bool) -> torch.Tensor:
+    """transformers' ``forward_loss`` on the decoder stream pred [Td, C p p] (image b's patch i at row b (N + 1) + 1 + i),
+    in pred's dtype (fp32 for bf16)."""
+    B, N = ids_restore.shape
+    dtype = pred.dtype if pred.dtype in (torch.float32, torch.float64) else torch.float32
+    p = int(round(math.sqrt(pred.shape[1] // images.shape[1])))
+    x = pred[:B * (N + 1)].to(dtype).view(B, N + 1, -1)[:, 1:]
+    target = mae_patchify(images.to(dtype), p)
+    if norm_pix:
+        mean = target.mean(dim=-1, keepdim=True)
+        var = target.var(dim=-1, keepdim=True)
+        target = (target - mean) / (var + MAE_NORM_PIX_EPS) ** 0.5
+    mask = (ids_restore >= keep).to(dtype)
+    return (((x - target) ** 2).mean(dim=-1) * mask).sum() / mask.sum()
+
+
+class _MaeLoss(torch.autograd.Function):
+    """pred [Td, C p p] bf16 -> loss fp32 [] (csrc/mae.cu).  Backward: the target recomputed from the image, the incoming
+    gradient read on the device."""
+
+    @staticmethod
+    def forward(ctx, pred, images, ids_restore, keep, norm_pix):
+        ctx.save_for_backward(pred, images, ids_restore)
+        ctx.keep, ctx.norm_pix = keep, norm_pix
+        return _C().mae.loss(pred, images, ids_restore, keep, norm_pix)
+
+    @staticmethod
+    def backward(ctx, dloss):
+        pred, images, ids_restore = ctx.saved_tensors
+        dpred = _C().mae.loss_bwd(dloss.float().reshape(1).contiguous(), pred, images, ids_restore, ctx.keep, ctx.norm_pix)
+        return dpred, None, None, None, None
+
+
+def mae_loss(pred: torch.Tensor, images: torch.Tensor, ids_restore: torch.Tensor, keep: int, norm_pix: bool) -> torch.Tensor:
+    """The masked autoencoder's pixel reconstruction loss: pred [Td, C p p] on the decoder stream (image b's patch i at row
+    b (N + 1) + 1 + i), images [B, C, H, W] and ids_restore [B, N].  The target is image b's patch i in (ky, kx, c) order,
+    with ``norm_pix`` normalised by its mean and unbiased variance (+ 1e-6); the loss is the mean over the B (N - keep) masked
+    patches of the per-patch mean of (pred - target)^2.
+
+    CUDA bf16 runs the native kernels (C p^2 <= 768, p % 8 == 0, contiguous or channels_last images, else ``ValueError``):
+    fixed-order fp32 sums, a backward that writes zeros at class, visible and padding rows and keeps nothing [Td, C p p]-sized
+    in fp32 from the forward.  Everything else runs ``mae_loss_reference``."""
+    if not (pred.is_cuda and pred.dtype == torch.bfloat16):
+        return mae_loss_reference(pred, images, ids_restore, keep, norm_pix)
+    if images.dtype != torch.bfloat16 or not (images.is_contiguous() or images.is_contiguous(memory_format=torch.channels_last)):
+        raise ValueError(f"mae_loss on CUDA needs contiguous or channels_last bf16 images, got {images.dtype}")
+    if images.requires_grad and torch.is_grad_enabled():
+        raise ValueError("mae_loss gives the images no gradient; pass images that do not require one")
+    return _MaeLoss.apply(_aligned16(pred), images, ids_restore.to(torch.int32).contiguous(), int(keep), bool(norm_pix))

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel timings against the measured roofline (MEASURED_PEAKS.json: HBM copy GB/s, cuBLAS bf16 TFLOP/s).
 
-  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,swin,mamba,mamba2,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
+  python bench/kernel_bench.py [--only gemm,fp8,attn,llama,qwen,qwen3,modernbert,vit,clip,cross,t5,convnext,swin,mamba,mamba2,mae,conv,bn,sgd,adamw,ln,xent,lmloss,sparse,moe,mse,input] [--out kernels.json] [--iters 20]
 
 Timing hygiene: >= 3 warm-up launches, CUDA events on the launching stream, a 256 MB write
 between timed launches to flush the 50 MB L2, median of `iters`.  Each entry reports algorithmic bytes / FLOPs,
@@ -1327,6 +1327,98 @@ def main():
                 record(f"{label} gated norm fwd {layout}", ms, bytes_=T * E * 2 * 3)
                 ms = timeit(lambda: C.mamba2.gated_norm_bwd(dy, y, z, nw, rstd, dzx[:, :E]), args.iters)
                 record(f"{label} gated norm bwd {layout}", ms, bytes_=T * E * 2 * 5)
+
+    if "mae" in want:
+        # The masked autoencoder's kernels at ViT-MAE-base's shapes (196 patches, 49 kept, encoder 768 wide, decoder 512 wide
+        # with 16 heads of 32 over 197 rows per image), batch 64 and 256.  image_attention forward and backward against SDPA
+        # on [B, 16, 197, 32] around the same qkv; mae_loss forward and backward against the torch expression under bf16; the
+        # shuffle, the masked patch embedding's gather / assemble and the unshuffle against their torch expressions.  Bytes,
+        # from shapes: what each kernel must read and write once (attention: qkv, o, lse; backward also dO and dqkv).
+        import torch.nn.functional as F
+        from b200ddp.ops import image_token_rows, mae_patchify
+        print(f"mae kernels on {card()}", flush=True)
+        N, keep, D, E, H, P = 196, 49, 768, 512, 16, 768
+        for B in (64, 256):
+            g = torch.Generator(device="cuda").manual_seed(B)
+            S = N + 1
+            Td, Te = image_token_rows(B, S), image_token_rows(B, keep + 1)
+            # image attention
+            qkv = torch.randn(Td, 3 * E, device=dev, generator=g).to(torch.bfloat16)
+            dout = torch.randn(Td, E, device=dev, generator=g).to(torch.bfloat16)
+            o, lse = C.mae.attention_fwd(qkv, B, S)
+
+            def sdpa(qkv):
+                x = qkv[:B * S].view(B, S, 3, H, 32).permute(2, 0, 3, 1, 4)
+                return F.scaled_dot_product_attention(x[0], x[1], x[2]).transpose(1, 2).reshape(B * S, E)
+
+            qg = qkv.clone().requires_grad_(True)
+            lib_f = timeit(lambda: sdpa(qg), args.iters)
+            y = sdpa(qg)
+            lib_b = timeit(lambda: torch.autograd.grad(y, qg, dout[:B * S], retain_graph=True), args.iters)
+            del y
+            rows_ = B * S
+            fwd_bytes = rows_ * (3 * E * 2 + E * 2 + H * 4)
+            bwd_bytes = rows_ * (3 * E * 2 + 2 * E * 2 + H * 4 + 3 * E * 2)
+            attn_flops = 4.0 * 32 * H * B * S * S
+            tag = f"[{B}, {H}, {S}, 32]"
+            record(f"image_attention fwd {tag}", timeit(lambda: C.mae.attention_fwd(qkv, B, S), args.iters), flops=attn_flops,
+                   lib_ms=lib_f, note=f"{fwd_bytes / 1e6:.1f} MB; lib = SDPA")
+            record(f"image_attention bwd {tag}", timeit(lambda: C.mae.attention_bwd(dout, qkv, o, lse, B, S), args.iters),
+                   flops=2.5 * attn_flops, lib_ms=lib_b, note=f"{bwd_bytes / 1e6:.1f} MB; lib = SDPA")
+            del qkv, dout, o, lse, qg
+            # loss
+            images = torch.randn(B, 3, 224, 224, device=dev, generator=g).to(torch.bfloat16)
+            noise = torch.rand(B, N, device=dev, generator=g)
+            ids_keep, ids_restore = C.mae.shuffle(noise, keep)
+            pred = torch.randn(Td, P, device=dev, generator=g).to(torch.bfloat16)
+            dloss = torch.ones(1, device=dev)
+            mask = (ids_restore >= keep).to(torch.bfloat16)
+
+            def torch_loss(pred):
+                t = mae_patchify(images, 16)
+                return ((((pred[:B * S].view(B, S, P)[:, 1:] - t) ** 2).mean(-1) * mask).sum() / mask.sum()).float()
+
+            pg = pred.clone().requires_grad_(True)
+            lib_f = timeit(lambda: torch_loss(pg), args.iters)
+            lt = torch_loss(pg)
+            lib_b = timeit(lambda: torch.autograd.grad(lt, pg, retain_graph=True), args.iters)
+            del lt
+            loss_bytes = B * (N - keep) * P * 2 * 2 + B * N * 4
+            record(f"mae_loss fwd B={B}", timeit(lambda: C.mae.loss(pred, images, ids_restore, keep, False), args.iters),
+                   bytes_=loss_bytes, lib_ms=lib_f, note="lib = torch expression, bf16")
+            record(f"mae_loss bwd B={B}", timeit(lambda: C.mae.loss_bwd(dloss, pred, images, ids_restore, keep, False), args.iters),
+                   bytes_=loss_bytes + Td * P * 2, lib_ms=lib_b, note="lib = torch expression, bf16")
+            del pred, pg
+            # shuffle, masked patch embedding, unshuffle
+            record(f"mae_shuffle B={B}", timeit(lambda: C.mae.shuffle(noise, keep), args.iters), bytes_=B * N * 4 + B * (N + keep) * 4,
+                   lib_ms=timeit(lambda: torch.argsort(torch.argsort(noise, 1), 1), args.iters), note="lib = two torch.argsort")
+            record(f"mae_patchify B={B}", timeit(lambda: C.mae.patchify(images, ids_keep, 16, Te), args.iters),
+                   bytes_=2 * B * keep * P * 2,
+                   lib_ms=timeit(lambda: torch.gather(mae_patchify(images, 16), 1, ids_keep.long()[..., None].expand(-1, -1, P)), args.iters),
+                   note="lib = patchify + gather")
+            yd = torch.randn(Te, D, device=dev, generator=g).to(torch.bfloat16)
+            cls = torch.randn(D, device=dev, generator=g).to(torch.bfloat16)
+            pos = torch.randn(S, D, device=dev, generator=g).to(torch.bfloat16)
+            record(f"mae_patch_assemble B={B}", timeit(lambda: C.mae.patch_assemble(yd, cls, pos, ids_keep), args.iters),
+                   bytes_=2 * Te * D * 2 + B * keep * D * 2,
+                   lib_ms=timeit(lambda: yd[:B * (keep + 1)].view(B, keep + 1, D)[:, 1:] + pos[1:][ids_keep.long()], args.iters),
+                   note="lib = gather + add")
+            ye = torch.randn(Te, E, device=dev, generator=g).to(torch.bfloat16)
+            mtok = torch.randn(E, device=dev, generator=g).to(torch.bfloat16)
+            dpos = torch.randn(S, E, device=dev, generator=g).to(torch.bfloat16)
+            dz = torch.randn(Td, E, device=dev, generator=g).to(torch.bfloat16)
+
+            def torch_unshuffle():
+                x = ye[:B * (keep + 1)].view(B, keep + 1, E)
+                x_ = torch.cat([x[:, 1:], mtok.view(1, 1, E).expand(B, N - keep, E)], 1)
+                x_ = torch.gather(x_, 1, ids_restore.long()[..., None].expand(-1, -1, E))
+                return torch.cat([x[:, :1], x_], 1) + dpos
+
+            record(f"mae_unshuffle B={B}", timeit(lambda: C.mae.unshuffle(ye, mtok, dpos, ids_restore, keep, Td), args.iters),
+                   bytes_=B * keep * E * 2 + Td * E * 2, lib_ms=timeit(torch_unshuffle, args.iters), note="lib = cat, gather, cat, add")
+            record(f"mae_unshuffle bwd B={B}", timeit(lambda: C.mae.unshuffle_bwd(dz, ids_keep, ids_restore, Te), args.iters),
+                   bytes_=B * S * E * 2 + Te * E * 2)
+            del images, yd, ye, dz
 
     if args.out:
         os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
