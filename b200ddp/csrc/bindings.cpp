@@ -170,13 +170,14 @@ class Args {
   c10::cuda::OptionalCUDAGuard guard_;
 };
 
-// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin, _C.mamba, _C.mamba2, _C.whisper and _C.mae namespaces of
-// static entry points
+// the types behind the _C.clip, _C.cross, _C.t5, _C.convnext, _C.swin, _C.swin_v2, _C.mamba, _C.mamba2, _C.whisper and _C.mae
+// namespaces of static entry points
 struct ClipNamespace {};
 struct CrossNamespace {};
 struct T5Namespace {};
 struct ConvNextNamespace {};
 struct SwinNamespace {};
+struct SwinV2Namespace {};
 struct MambaNamespace {};
 struct Mamba2Namespace {};
 struct WhisperNamespace {};
@@ -207,6 +208,27 @@ std::array<int64_t, 2> swin_args(Args& args, const at::Tensor& qkv, const at::Te
     args.fail("geometry", "batch >= 1, height and width positive multiples of 7 and shifts in [0, 7)", geometry());
   const int64_t rows = batch * height * width;
   if (rows * 96 * heads >= (1ll << 31)) args.fail("geometry", "at most 2^31 qkv elements", geometry());
+  args("qkv", qkv, {kBF16}, {rows, 96 * heads}, kContiguous, 16);
+  return {rows, heads};
+}
+
+// Swin V2's window-attention geometry: table fp32 [225, heads] with 1 <= heads <= 65535, scale fp32 [heads], batch >= 1,
+// height and width positive multiples of 8 and shifts in [0, 8), then qkv bf16 [batch * height * width, 96 heads] (head
+// dim 32), contiguous and 16-byte aligned.  Returns (rows, heads).
+std::array<int64_t, 2> swin_v2_args(Args& args, const at::Tensor& qkv, const at::Tensor& table, const at::Tensor& scale, int64_t batch,
+                                    int64_t height, int64_t width, int64_t shift_y, int64_t shift_x) {
+  args("table", table, {kF32}, {225, kAny});
+  const int64_t heads = table.size(1);
+  if (heads < 1 || heads > 65535) args.fail("table", "fp32 [225, heads] with 1 <= heads <= 65535", describe(table));
+  args("scale", scale, {kF32}, {heads});
+  const auto geometry = [&] { return std::to_string(batch) + " x " + std::to_string(height) + " x " + std::to_string(width) + ", shift (" +
+                                     std::to_string(shift_y) + ", " + std::to_string(shift_x) + ")"; };
+  if (batch < 1 || batch > 65535 || height < 8 || width < 8 || height % 8 || width % 8 || height > 65535 || width > 65535 || shift_y < 0 ||
+      shift_y >= 8 || shift_x < 0 || shift_x >= 8)
+    args.fail("geometry", "batch >= 1, height and width positive multiples of 8 and shifts in [0, 8)", geometry());
+  const int64_t rows = batch * height * width;
+  if (rows * 96 * heads >= (1ll << 31)) args.fail("geometry", "at most 2^31 qkv elements", geometry());
+  if (qkv.dim() == 2 && qkv.size(1) != 96 * heads) args.fail("qkv", "bf16 [rows, 96 heads] (head dim 32)", describe(qkv));
   args("qkv", qkv, {kBF16}, {rows, 96 * heads}, kContiguous, 16);
   return {rows, heads};
 }
@@ -1973,6 +1995,43 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                               dtable.data_ptr<float>(), cur_stream());
     return std::make_tuple(dqkv, dtable);
   }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("table"), py::arg("batch"), py::arg("height"),
+     py::arg("width"), py::arg("shift_y"), py::arg("shift_x"));
+
+  // ---- Swin V2's cosine shifted-window attention, window 8, head dim 32 (swin.cu), bf16 raster rows -----------------------
+  // _C.swin_v2 is a namespace of static entry points like _C.swin; its contract rows are in tests/test_swin_v2_bindings_cpu.py.
+  // qkv [B H W, 3C] (C = 32 heads), table fp32 [225, heads] (16 sigmoid of the cpb MLP), scale fp32 [heads] (exp of the
+  // clamped logit_scale), o and dout [B H W, C], lse fp32 [B H W, heads].
+  py::class_<SwinV2Namespace> swin_v2(m, "swin_v2", "Swin V2's cosine shifted-window attention on raster token rows (swin.cu)");
+  // (o bf16 [B H W, C], lse fp32 [B H W, heads])
+  swin_v2.def_static("attention_fwd", [](at::Tensor qkv, at::Tensor table, at::Tensor scale, int64_t batch, int64_t height, int64_t width,
+                                         int64_t shift_y, int64_t shift_x) {
+    Args args("attention_fwd");
+    const auto [rows, heads] = swin_v2_args(args, qkv, table, scale, batch, height, width, shift_y, shift_x);
+    args.device();
+    at::Tensor o = at::empty({rows, 32 * heads}, qkv.options());
+    at::Tensor lse = at::empty({rows, heads}, qkv.options().dtype(kF32));
+    launch_swin_v2_attention_fwd(qkv.data_ptr(), table.data_ptr<float>(), scale.data_ptr<float>(), (int)batch, (int)height, (int)width,
+                                 (int)heads, (int)shift_y, (int)shift_x, o.data_ptr(), lse.data_ptr<float>(), cur_stream());
+    return std::make_tuple(o, lse);
+  }, py::arg("qkv"), py::arg("table"), py::arg("scale"), py::arg("batch"), py::arg("height"), py::arg("width"), py::arg("shift_y"),
+     py::arg("shift_x"));
+  // (dqkv bf16 [B H W, 3C], dtable fp32 [225, heads], dscale fp32 [heads])
+  swin_v2.def_static("attention_bwd", [](at::Tensor dout, at::Tensor qkv, at::Tensor o, at::Tensor lse, at::Tensor table, at::Tensor scale,
+                                         int64_t batch, int64_t height, int64_t width, int64_t shift_y, int64_t shift_x) {
+    Args args("attention_bwd");
+    const auto [rows, heads] = swin_v2_args(args, qkv, table, scale, batch, height, width, shift_y, shift_x);
+    args("dout", dout, {kBF16}, {rows, 32 * heads}, kContiguous, 16)("o", o, {kBF16}, {rows, 32 * heads}, kContiguous, 16)
+        ("lse", lse, {kF32}, {rows, heads});
+    args.device();
+    const int windows = swin_v2_windows((int)batch, (int)height, (int)width);
+    at::Tensor dqkv = at::empty_like(qkv);
+    at::Tensor part = at::empty({heads, (int64_t)windows, 226}, qkv.options().dtype(kF32));
+    at::Tensor grads = at::empty({226, heads}, qkv.options().dtype(kF32));   // the 225 table rows, then d scale
+    launch_swin_v2_attention_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), table.data_ptr<float>(),
+                                 scale.data_ptr<float>(), (int)batch, (int)height, (int)width, (int)heads, (int)shift_y, (int)shift_x,
+                                 dqkv.data_ptr(), part.data_ptr<float>(), grads.data_ptr<float>(), cur_stream());
+    return std::make_tuple(dqkv, grads.narrow(0, 0, 225), grads.select(0, 225));
+  }, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("table"), py::arg("scale"), py::arg("batch"), py::arg("height"),
      py::arg("width"), py::arg("shift_y"), py::arg("shift_x"));
 
   // ---- Mamba's causal conv1d + SiLU and selective scan (mamba.cu), bf16 token rows ----------------------------------------

@@ -281,6 +281,15 @@ void launch_swin_attention_fwd(const void* qkv, const float* table, int B, int H
 // (head, window), summed in window order
 void launch_swin_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const float* table, int B, int H, int W,
                                int heads, int sy, int sx, void* dqkv, float* part, float* dtable, cudaStream_t s);
+// Swin V2's cosine attention, window 8: qkv as above; table fp32 [225, heads] (16 sigmoid of the cpb MLP), scale fp32
+// [heads] (exp of the clamped logit_scale); H, W multiples of 8, 0 <= sy, sx < 8.  o and lse as above.
+int swin_v2_windows(int B, int H, int W);
+void launch_swin_v2_attention_fwd(const void* qkv, const float* table, const float* scale, int B, int H, int W, int heads, int sy, int sx,
+                                  void* o, float* lse, cudaStream_t s);
+// dqkv bf16 [B*H*W, 3C]; dtable fp32 [226, heads], rows 0 .. 224 the table gradient and row 225 d scale, through part fp32
+// [heads, swin_v2_windows(B, H, W), 226]: one partial per (head, window), summed in window order
+void launch_swin_v2_attention_bwd(const void* dout, const void* qkv, const void* o, const float* lse, const float* table, const float* scale,
+                                  int B, int H, int W, int heads, int sy, int sx, void* dqkv, float* part, float* dtable, cudaStream_t s);
 
 // ---------------- Mamba causal conv1d + SiLU and selective scan (mamba.cu), bf16 token rows -------------------------------
 // T = B S rows; bounds int32 [B, S, 2] (document (start, end) per position, start == end for padding); E % 8 == 0, N = 16,

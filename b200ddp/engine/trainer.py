@@ -58,7 +58,7 @@ def build_dataset(args):
                                   batch=int(getattr(args, "train_batch_size", 1)) * world)
     if entry.kind == "image":
         dense = loss_kind(args) == "mse"
-        return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), dense_target=dense)
+        return SyntheticImageNet(samples=min(n, int(getattr(args, "image_samples", 1024))), size=entry.image_size, dense_target=dense)
     if entry.speech:
         return SyntheticSpeech(samples=min(n, 128), seq_len=int(getattr(args, "seq_len", 448)), min_len=getattr(args, "min_seq_len", None))
     if entry.seq2seq and isinstance(entry.config, T5Config):

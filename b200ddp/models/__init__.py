@@ -14,7 +14,8 @@ from .modernbert import (MODERNBERT_BASE, MODERNBERT_LARGE, ModernBertConfig, Mo
                          modernbert_large)
 from .vit import VIT_B_16, VIT_B_32, VIT_L_16, ViTConfig, VisionTransformer, vit_b_16, vit_b_32, vit_l_16
 from .convnext import CONVNEXT_BASE, CONVNEXT_SMALL, CONVNEXT_TINY, ConvNeXt, ConvNeXtConfig, convnext_base, convnext_small, convnext_tiny
-from .swin import SWIN_B, SWIN_S, SWIN_T, SwinConfig, SwinTransformer, swin_b, swin_s, swin_t
+from .swin import (SWIN_B, SWIN_S, SWIN_T, SWIN_V2_B, SWIN_V2_S, SWIN_V2_T, SwinConfig, SwinTransformer, swin_b, swin_s, swin_t, swin_v2_b,
+                   swin_v2_s, swin_v2_t)
 from .clip import CLIP_VIT_B_16, CLIP_VIT_B_32, CLIPConfig, CLIPModel, clip_vit_b_16, clip_vit_b_32
 from .bart import BART_BASE, BART_LARGE, BartConfig, BartForConditionalGeneration, bart_base, bart_large
 from .t5 import T5_BASE, T5_SMALL, T5Config, T5ForConditionalGeneration, t5_base, t5_small
@@ -43,6 +44,7 @@ class ModelEntry:
                                        # labels) on the log-mel features of int16 clips
     own_loss: bool = False             # image models whose forward returns their own loss (MAE pretraining): forward(images),
                                        # the criterion passes it through and the labels are ignored
+    image_size: int = 224              # image models: the side of the square synthetic images they train on
 
     @property
     def token_model(self) -> bool:
@@ -62,6 +64,10 @@ MODEL_REGISTRY = {
     "swin-t": ModelEntry(swin_t, "image"),
     "swin-s": ModelEntry(swin_s, "image"),
     "swin-b": ModelEntry(swin_b, "image"),
+    # Swin V2's 8 x 8 windows tile every stage of a 256 x 256 image (224 leaves stage 2 28 wide)
+    "swin-v2-t": ModelEntry(swin_v2_t, "image", image_size=256),
+    "swin-v2-s": ModelEntry(swin_v2_s, "image", image_size=256),
+    "swin-v2-b": ModelEntry(swin_v2_b, "image", image_size=256),
     "vit-mae-base": ModelEntry(vit_mae_base, "image", own_loss=True),
     "vit-mae-large": ModelEntry(vit_mae_large, "image", own_loss=True),
     "clip-vit-b-32": ModelEntry(clip_vit_b_32, "image", contrastive=True),
@@ -108,4 +114,4 @@ def build_model(name: str, **kwargs):
 
 
 __all__ = ["FooModel", "BranchyFooModel", "ResNet", "resnet50", "resnet152", "BertConfig", "BertModel",
-           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ViTMAEConfig", "ViTMAEForPreTraining", "vit_mae_base", "vit_mae_large", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "Mamba2Config", "Mamba2ForCausalLM", "mamba2_130m", "mamba2_370m", "WhisperConfig", "WhisperForConditionalGeneration", "whisper_tiny", "whisper_base", "whisper_small", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]
+           "BertForMaskedLM", "bert_base", "GPTConfig", "GPTModel", "GPTLMHeadModel", "gpt2", "LlamaConfig", "LlamaModel", "LlamaForCausalLM", "smollm_135m", "qwen2_5_1_5b", "qwen3_0_6b", "granite_3_0_1b_a400m", "ModernBertConfig", "ModernBertModel", "ModernBertForMaskedLM", "modernbert_base", "modernbert_large", "ViTConfig", "VisionTransformer", "vit_b_16", "vit_b_32", "vit_l_16", "ViTMAEConfig", "ViTMAEForPreTraining", "vit_mae_base", "vit_mae_large", "ConvNeXtConfig", "ConvNeXt", "convnext_tiny", "convnext_small", "convnext_base", "SwinConfig", "SwinTransformer", "swin_t", "swin_s", "swin_b", "swin_v2_t", "swin_v2_s", "swin_v2_b", "CLIPConfig", "CLIPModel", "clip_vit_b_32", "clip_vit_b_16", "BartConfig", "BartForConditionalGeneration", "bart_base", "bart_large", "T5Config", "T5ForConditionalGeneration", "t5_small", "t5_base", "MambaConfig", "MambaForCausalLM", "mamba_130m", "mamba_370m", "Mamba2Config", "Mamba2ForCausalLM", "mamba2_130m", "mamba2_370m", "WhisperConfig", "WhisperForConditionalGeneration", "whisper_tiny", "whisper_base", "whisper_small", "ModelEntry", "MODEL_REGISTRY", "model_entry", "build_model"]

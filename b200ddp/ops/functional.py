@@ -1866,40 +1866,49 @@ def patchify_nhwc(x: torch.Tensor, patch: int) -> torch.Tensor:
 SWIN_WINDOW = 7
 SWIN_HEAD_DIM = 32
 SWIN_MASK = -100.0                   # torchvision's value between shift regions, not -inf
+SWIN_V2_WINDOW = 8
 
 
-def swin_relative_position_index(device=None) -> torch.Tensor:
-    """int64 [49 * 49]: entry 49 i + j is (yi - yj + 6) 13 + (xi - xj + 6) for the window's tokens i = 7 yi + xi and
-    j = 7 yj + xj, the table row of their relative position (torchvision's ``relative_position_index``)."""
-    t = torch.arange(SWIN_WINDOW * SWIN_WINDOW, device=device)
-    y, x = t // SWIN_WINDOW, t % SWIN_WINDOW
-    return ((y[:, None] - y[None, :] + SWIN_WINDOW - 1) * (2 * SWIN_WINDOW - 1) + (x[:, None] - x[None, :] + SWIN_WINDOW - 1)).flatten()
+def swin_relative_position_index(device=None, window: int = SWIN_WINDOW) -> torch.Tensor:
+    """int64 [w^4] for window w (7 by default): entry w^2 i + j is (yi - yj + w - 1) (2w - 1) + (xi - xj + w - 1) for the
+    window's tokens i = w yi + xi and j = w yj + xj, the table row of their relative position (torchvision's
+    ``relative_position_index``)."""
+    t = torch.arange(window * window, device=device)
+    y, x = t // window, t % window
+    return ((y[:, None] - y[None, :] + window - 1) * (2 * window - 1) + (x[:, None] - x[None, :] + window - 1)).flatten()
 
 
-def _shift_pair(shift) -> tuple[int, int]:
+def swin_v2_relative_coords_table(window: int = SWIN_V2_WINDOW, device=None) -> torch.Tensor:
+    """fp32 [1, 2w - 1, 2w - 1, 2]: entry (dy + w - 1, dx + w - 1) is f(8 dy / (w - 1)), f(8 dx / (w - 1)) with
+    f(t) = sign(t) log2(|t| + 1) / 3, the input of Swin V2's continuous position bias MLP (torchvision's
+    ``relative_coords_table``)."""
+    r = torch.arange(-(window - 1), window, dtype=torch.float32, device=device)
+    t = torch.stack(torch.meshgrid([r, r], indexing="ij")).permute(1, 2, 0).contiguous().unsqueeze(0)
+    t = t / (window - 1) * 8
+    return torch.sign(t) * torch.log2(torch.abs(t) + 1.0) / 3.0
+
+
+def _shift_pair(shift, window: int = SWIN_WINDOW) -> tuple[int, int]:
     sy, sx = (shift, shift) if isinstance(shift, int) else tuple(shift)
-    if not (0 <= sy < SWIN_WINDOW and 0 <= sx < SWIN_WINDOW):
-        raise ValueError(f"window_attention needs 0 <= shift < {SWIN_WINDOW}, got {shift}")
+    if not (0 <= sy < window and 0 <= sx < window):
+        raise ValueError(f"window_attention needs 0 <= shift < {window}, got {shift}")
     return int(sy), int(sx)
 
 
-def _shift_regions(n: int, shift: int, device) -> torch.Tensor:
-    """The shift region of each shifted coordinate 0 .. n-1: [0, n-7), [n-7, n-shift), [n-shift, n); one region at shift 0."""
+def _shift_regions(n: int, shift: int, device, window: int = SWIN_WINDOW) -> torch.Tensor:
+    """The shift region of each shifted coordinate 0 .. n-1: [0, n-w), [n-w, n-shift), [n-shift, n); one region at shift 0."""
     c = torch.arange(n, device=device)
     if shift == 0:
         return torch.zeros_like(c)
-    return (c >= n - SWIN_WINDOW).long() + (c >= n - shift).long()
+    return (c >= n - window).long() + (c >= n - shift).long()
 
 
-def window_attention_reference(qkv: torch.Tensor, table: torch.Tensor, batch: int, height: int, width: int, heads: int,
-                               shift) -> torch.Tensor:
-    """``window_attention`` in torch, fp32 for bf16 input: roll the map by -shift, partition it into 7 x 7 windows, dense
-    scores with the relative position bias and the -100 region mask, softmax, and the reverse partition and roll.  Needs
-    height and width multiples of 7; any head dim."""
-    sy, sx = _shift_pair(shift)
-    B, H, W, w = batch, height, width, SWIN_WINDOW
+def _window_attention_torch(qkv, table, scale, batch, height, width, heads, shift, window, who):
+    """Both references: V1's scaled dot product when ``scale`` is None, else V2's cosine scores times scale [heads]."""
+    sy, sx = _shift_pair(shift, window)
+    B, H, W, w = batch, height, width, window
     if H % w or W % w or qkv.dim() != 2 or qkv.shape[0] != B * H * W or qkv.shape[1] % (3 * heads):
-        raise ValueError(f"window_attention_reference needs qkv [B H W, 3C] with H and W multiples of 7, got {tuple(qkv.shape)} "
+        raise ValueError(f"{who} needs qkv [B H W, 3C] with H and W multiples of {w}, got {tuple(qkv.shape)} "
                          f"for {B} x {H} x {W} and {heads} heads")
     dtype = qkv.dtype if qkv.dtype in (torch.float32, torch.float64) else torch.float32
     C = qkv.shape[1] // 3
@@ -1910,10 +1919,13 @@ def window_attention_reference(qkv: torch.Tensor, table: torch.Tensor, batch: in
     n = (H // w) * (W // w)
     x = x.view(B, H // w, w, W // w, w, 3 * C).permute(0, 1, 3, 2, 4, 5).reshape(B * n, w * w, 3, heads, d).permute(2, 0, 3, 1, 4)
     q, k, v = x[0], x[1], x[2]
-    bias = table.to(dtype)[swin_relative_position_index(table.device)].view(w * w, w * w, heads).permute(2, 0, 1)
-    attn = (q * d ** -0.5) @ k.transpose(-2, -1) + bias
+    bias = table.to(dtype)[swin_relative_position_index(table.device, w)].view(w * w, w * w, heads).permute(2, 0, 1)
+    if scale is None:
+        attn = (q * d ** -0.5) @ k.transpose(-2, -1) + bias
+    else:
+        attn = (F.normalize(q, dim=-1) @ F.normalize(k, dim=-1).transpose(-2, -1)) * scale.to(dtype).view(heads, 1, 1) + bias
     if sy or sx:
-        region = _shift_regions(H, sy, qkv.device)[:, None] * 3 + _shift_regions(W, sx, qkv.device)[None, :]
+        region = _shift_regions(H, sy, qkv.device, w)[:, None] * 3 + _shift_regions(W, sx, qkv.device, w)[None, :]
         region = region.view(H // w, w, W // w, w).permute(0, 2, 1, 3).reshape(n, w * w)
         mask = torch.where(region[:, :, None] != region[:, None, :], SWIN_MASK, 0.0).to(dtype)
         attn = (attn.view(B, n, heads, w * w, w * w) + mask[None, :, None]).view(B * n, heads, w * w, w * w)
@@ -1921,6 +1933,14 @@ def window_attention_reference(qkv: torch.Tensor, table: torch.Tensor, batch: in
     if sy or sx:
         o = torch.roll(o, shifts=(sy, sx), dims=(1, 2))
     return o.reshape(B * H * W, C).to(qkv.dtype)
+
+
+def window_attention_reference(qkv: torch.Tensor, table: torch.Tensor, batch: int, height: int, width: int, heads: int,
+                               shift) -> torch.Tensor:
+    """``window_attention`` in torch, fp32 for bf16 input: roll the map by -shift, partition it into 7 x 7 windows, dense
+    scores with the relative position bias and the -100 region mask, softmax, and the reverse partition and roll.  Needs
+    height and width multiples of 7; any head dim."""
+    return _window_attention_torch(qkv, table, None, batch, height, width, heads, shift, SWIN_WINDOW, "window_attention_reference")
 
 
 class _WindowAttention(torch.autograd.Function):
@@ -1965,6 +1985,60 @@ def window_attention(qkv: torch.Tensor, table: torch.Tensor, batch: int, height:
     if height % SWIN_WINDOW or width % SWIN_WINDOW or min(batch, height, width) < 1:
         raise ValueError(f"window_attention on CUDA needs H and W positive multiples of {SWIN_WINDOW}, got {height} x {width}")
     return _WindowAttention.apply(_aligned16(qkv), table.float().contiguous(), batch, height, width, sy, sx)
+
+
+def window_attention_v2_reference(qkv: torch.Tensor, table: torch.Tensor, scale: torch.Tensor, batch: int, height: int, width: int,
+                                  heads: int, shift) -> torch.Tensor:
+    """``window_attention_v2`` in torch, fp32 for bf16 input: as ``window_attention_reference`` at window 8, with the
+    scores scale_h cos(q_i, k_j) (``F.normalize``, eps 1e-12) in place of d^-0.5 q_i . k_j.  Needs height and width
+    multiples of 8; any head dim."""
+    return _window_attention_torch(qkv, table, scale, batch, height, width, heads, shift, SWIN_V2_WINDOW, "window_attention_v2_reference")
+
+
+class _WindowAttentionV2(torch.autograd.Function):
+    """qkv [B H W, 3C] bf16, table fp32 [225, heads], scale fp32 [heads] -> o [B H W, C] (csrc/swin.cu).  Backward: one
+    kernel per window for dqkv and the window's table and scale partials, and an in-order finish for dtable and dscale."""
+
+    @staticmethod
+    def forward(ctx, qkv, table, scale, batch, height, width, sy, sx):
+        o, lse = _C().swin_v2.attention_fwd(qkv, table, scale, batch, height, width, sy, sx)
+        ctx.save_for_backward(qkv, table, scale, o, lse)
+        ctx.geometry = (batch, height, width, sy, sx)
+        return o
+
+    @staticmethod
+    def backward(ctx, dout):
+        qkv, table, scale, o, lse = ctx.saved_tensors
+        dqkv, dtable, dscale = _C().swin_v2.attention_bwd(_aligned16(dout), qkv, o, lse, table, scale, *ctx.geometry)
+        return dqkv, dtable, dscale, None, None, None, None, None
+
+
+def window_attention_v2(qkv: torch.Tensor, table: torch.Tensor, scale: torch.Tensor, batch: int, height: int, width: int, heads: int,
+                        shift) -> torch.Tensor:
+    """Swin V2's (shifted) cosine window attention on raster token rows: qkv [B H W, 3C] as in ``window_attention``,
+    table [225, heads] (torchvision's ``16 sigmoid(cpb_mlp(relative_coords_table))``), scale [heads]
+    (``exp(min(logit_scale, log 100))``) -> [B H W, C].  Window 8; ``shift`` is an int or a (y, x) pair in [0, 8).
+
+    Token i scores its window's tokens j with scale_h cos(q_i, k_j) + table[(yi - yj + 7) 15 + (xi - xj + 7), h] - 100
+    [i and j lie in different shift regions], cos the dot product of the rows divided by max(norm, 1e-12); windows and
+    regions are ``window_attention``'s with 8 in place of 7.
+
+    CUDA bf16 input runs the native kernels (head dim 32; H and W multiples of 8; else ``ValueError``): the normalised
+    q and k rounded once to bf16, fp32 softmax and sums, bitwise repeatable, no host synchronisation, the table and scale
+    gradients summed in a fixed order and rounded once to their dtype.  Everything else runs
+    ``window_attention_v2_reference``."""
+    sy, sx = _shift_pair(shift, SWIN_V2_WINDOW)
+    if not (qkv.is_cuda and qkv.dtype == torch.bfloat16):
+        return window_attention_v2_reference(qkv, table, scale, batch, height, width, heads, (sy, sx))
+    rows = batch * height * width
+    if (qkv.dim() != 2 or qkv.shape[0] != rows or qkv.shape[1] != 3 * SWIN_HEAD_DIM * heads or tuple(table.shape) != (225, heads)
+            or tuple(scale.shape) != (heads,)):
+        raise ValueError(f"window_attention_v2 on CUDA needs qkv [B H W, 96 heads] (head dim {SWIN_HEAD_DIM}), table [225, heads] "
+                         f"and scale [heads], got {tuple(qkv.shape)}, {tuple(table.shape)} and {tuple(scale.shape)} for "
+                         f"{batch} x {height} x {width} and {heads} heads")
+    if height % SWIN_V2_WINDOW or width % SWIN_V2_WINDOW or min(batch, height, width) < 1:
+        raise ValueError(f"window_attention_v2 on CUDA needs H and W positive multiples of {SWIN_V2_WINDOW}, got {height} x {width}")
+    return _WindowAttentionV2.apply(_aligned16(qkv), table.float().contiguous(), scale.float().contiguous(), batch, height, width, sy, sx)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -1192,6 +1192,68 @@ def main():
                    note=f"incl. the table-gradient finish; lib = torchvision's arithmetic; sdpa {lib['sdpa bwd']:.4f} ms")
             del qkv, dout, o, lse
 
+        # Swin V2's cosine window attention (window 8) at Swin-V2-T's four stage shapes at 256 x 256 (batch 64) and
+        # Swin-V2-B's first, forward and backward against the attention part of torchvision's shifted_window_attention
+        # with logit_scale under bf16 (roll, window partition, F.normalize of q and k, cosine scores times the scale, the
+        # gathered bias and the mask, softmax, reverse partition and roll), around the same qkv, table and scale.  Bytes as
+        # above, with 226 partial columns per window.
+        index8 = swin_relative_position_index(dev, 8)
+
+        def partition8(t, B, Hs, sy):
+            X = t.shape[-1]
+            t = torch.roll(t.view(B, Hs, Hs, X), shifts=(-sy, -sy), dims=(1, 2)) if sy else t.view(B, Hs, Hs, X)
+            return t.view(B, Hs // 8, 8, Hs // 8, 8, X).permute(0, 1, 3, 2, 4, 5).reshape(-1, 64, X)
+
+        def unpartition8(t, B, Hs, sy):
+            X = t.shape[-1]
+            t = t.view(B, Hs // 8, Hs // 8, 8, 8, X).permute(0, 1, 3, 2, 4, 5).reshape(B, Hs, Hs, X)
+            return (torch.roll(t, shifts=(sy, sy), dims=(1, 2)) if sy else t).reshape(B * Hs * Hs, X)
+
+        def window_mask8(Hs, s):
+            c = torch.arange(Hs, device=dev)
+            r = (c >= Hs - 8).long() + (c >= Hs - s).long()
+            reg = (r[:, None] * 3 + r[None, :]).view(Hs // 8, 8, Hs // 8, 8).permute(0, 2, 1, 3).reshape(-1, 64)
+            return torch.where(reg[:, :, None] != reg[:, None, :], -100.0, 0.0).to(torch.bfloat16)
+
+        for name, B, Hs, heads, s in (("swin-v2-t stage 1", 64, 64, 3, 4), ("swin-v2-t stage 2", 64, 32, 6, 4),
+                                      ("swin-v2-t stage 3", 64, 16, 12, 4), ("swin-v2-t stage 4", 64, 8, 24, 0),
+                                      ("swin-v2-b stage 1", 64, 64, 4, 4)):
+            Cn, nrows = 32 * heads, B * Hs * Hs
+            g = torch.Generator(device="cuda").manual_seed(heads)
+            qkv = torch.randn(nrows, 3 * Cn, device=dev, generator=g).to(torch.bfloat16)
+            t32 = 16 * torch.sigmoid(torch.randn(225, heads, device=dev, generator=g))
+            sc32 = torch.full((heads,), 10.0, device=dev)
+            table, scale = t32.to(torch.bfloat16), sc32.to(torch.bfloat16)
+            dout = torch.randn(nrows, Cn, device=dev, generator=g).to(torch.bfloat16)
+            o, lse = C.swin_v2.attention_fwd(qkv, t32, sc32, B, Hs, Hs, s, s)
+            nw = B * (Hs // 8) ** 2
+            mask = window_mask8(Hs, s) if s else None
+
+            def torchvision_fwd(qkv, table, scale):
+                x = partition8(qkv, B, Hs, s).reshape(-1, 64, 3, heads, 32).permute(2, 0, 3, 1, 4)
+                attn = F.normalize(x[0], dim=-1) @ F.normalize(x[1], dim=-1).transpose(-2, -1)
+                attn = attn * scale.view(heads, 1, 1) + table[index8].view(64, 64, heads).permute(2, 0, 1).unsqueeze(0)
+                if mask is not None:
+                    attn = (attn.view(B, -1, heads, 64, 64) + mask[None, :, None]).view(-1, heads, 64, 64)
+                y = F.softmax(attn, dim=-1).matmul(x[2]).transpose(1, 2).reshape(-1, 64, Cn)
+                return unpartition8(y, B, Hs, s)
+
+            fwd_bytes = nrows * (3 * Cn * 2 + Cn * 2 + heads * 4)
+            bwd_bytes = nrows * (3 * Cn * 2 + 2 * Cn * 2 + heads * 4 + 3 * Cn * 2) + 2 * heads * nw * 226 * 4
+            tag = f"{name} [{B}, {Hs}x{Hs}, {heads} heads, shift {s}]"
+            qg, tg, sg = qkv.clone().requires_grad_(True), table.clone().requires_grad_(True), scale.clone().requires_grad_(True)
+            lib_fwd = timeit(lambda: torchvision_fwd(qg, tg, sg), args.iters)
+            y = torchvision_fwd(qg, tg, sg)
+            lib_bwd = timeit(lambda: torch.autograd.grad(y, (qg, tg, sg), dout, retain_graph=True), args.iters)
+            del y
+            record(f"cosine window attention fwd {tag}", timeit(lambda: C.swin_v2.attention_fwd(qkv, t32, sc32, B, Hs, Hs, s, s), args.iters),
+                   bytes_=fwd_bytes, lib_ms=lib_fwd, note="lib = torchvision's shifted_window_attention arithmetic with logit_scale")
+            record(f"cosine window attention bwd {tag}",
+                   timeit(lambda: C.swin_v2.attention_bwd(dout, qkv, o, lse, t32, sc32, B, Hs, Hs, s, s), args.iters),
+                   bytes_=bwd_bytes, lib_ms=lib_bwd,
+                   note="incl. the table / scale gradient finish; lib = torchvision's arithmetic with logit_scale")
+            del qkv, dout, o, lse, qg, tg, sg
+
     if "mse" in want:
         n = 64 * 1024 * 1024
         o = torch.randn(n, device=dev, dtype=torch.bfloat16)

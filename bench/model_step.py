@@ -64,10 +64,10 @@ def card():
 # ------------------------------------------------------------------------------------------------ baselines
 # Each returns the model on ``dev`` and a closure computing one step's loss on its one device-resident batch.
 
-def _image_loss(model, batch, dev, channels_last):
+def _image_loss(model, batch, dev, channels_last, size=224):
     import torch
     import torch.nn.functional as F
-    x = torch.randn(batch, 3, 224, 224, device=dev)
+    x = torch.randn(batch, 3, size, size, device=dev)
     if channels_last:
         x = x.contiguous(memory_format=torch.channels_last)
     y = torch.randint(0, 1000, (batch,), device=dev)
